@@ -10,9 +10,9 @@ shape, random-init weights; weak scaling (128 samples per GPU per step, the Horo
         --master-port 29500 bench.py --gpus 8 --steps 200 --warmup 20
 
 Arms (`--impl`):
-  ours       (default) mini-Keras + hvd facade; every step = forward/backward out of our tcgen05 kernels + the
+  ours       (default) mini-Keras + hvd facade; every step = forward/backward out of our wgmma kernels + the
              fused reduce-scatter -> Adadelta -> all-gather exchange, replayed from a CUDA graph.
-  reference  the UNMODIFIED reference installed in baseline/_ref: its PyTorch worker
+  reference  the UNMODIFIED reference installed in oracle/_ref: its PyTorch worker
              (tf_yarn.pytorch.tasks.worker._train -> NCCL DistributedDataParallel) on the same model/config,
              see bench/ref_arm.py and bench/shims/README.md.
   standin    what the reference's Horovod path does on an NCCL build, written with stock PyTorch (eager, or
@@ -21,10 +21,14 @@ Arms (`--impl`):
 Other configs (`--config wide_deep | resnet50 | bert`, BASELINE.json configs 3-5) live in bench/*.py and print
 the same JSON schema.
 
-`value` is timed on the device with the input pool (269.7 MB, larger than the 126 MB L2, rotated so no batch
-is re-read from L2) resident in HBM; regions shorter than ~1000 steps are repeated and the median region is
-reported (`repeats`).  `e2e` runs the same number of steps through the public API (`model.fit`) with per-step
-H2D copies from pinned host memory and a per-step D2H read of the loss.
+`value` is timed on the device with the input pool (269.7 MB, larger than the 50 MB L2, rotated so no batch
+is re-read from L2) resident in HBM, over one region of exactly `--steps` steps (`--repeats N` times N regions
+and reports the median region).  `e2e` runs the same number of steps through the public API (`model.fit`) with
+per-step H2D copies from pinned host memory and a per-step D2H read of the loss.
+
+`--dump-outputs DIR` (mnist, ours) writes what the last timed step computed -- its loss and the updated flat
+parameter vector -- as DIR/loss.npy and DIR/params.npy (float32).  Inputs and initial weights are seeded, so two
+builds run with the same arguments can be compared output for output.
 """
 from __future__ import annotations
 
@@ -43,12 +47,16 @@ def main():
     ap.add_argument("--warmup", type=int, default=20)
     ap.add_argument("--impl", default="ours", choices=["ours", "reference", "standin"])
     ap.add_argument("--config", default="mnist", choices=["mnist", "wide_deep", "resnet50", "bert"])
-    ap.add_argument("--repeats", type=int, default=0, help="timed regions (0 = pick from --steps)")
+    ap.add_argument("--repeats", type=int, default=0, help="timed regions of --steps steps each (0 = one)")
     ap.add_argument("--graph", action="store_true", help="standin: capture the step (NCCL included) in a CUDA graph")
     ap.add_argument("--no-exposed", action="store_true", help="ours: skip the LOCAL-mode run behind exposed_comm_ms")
     ap.add_argument("--batch", type=int, default=0, help="per-GPU batch of the secondary configs (0 = default)")
     ap.add_argument("--side-tasks", action="store_true", help="bert: keep the TensorBoard side task alive during the run")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="mnist/ours: write the last timed step's loss and parameters as DIR/*.npy (float32)")
     args = ap.parse_args()
+    if args.dump_outputs and (args.config != "mnist" or args.impl != "ours"):
+        ap.error("--dump-outputs is implemented for --config mnist --impl ours")
     if args.config == "mnist":
         if args.impl == "reference":
             from bench import ref_arm

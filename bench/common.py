@@ -1,6 +1,6 @@
 """Shared measurement harness of bench.py (all arms, all configs).
 
-Timing rules implemented here (B200_PROFILING.md "Timing hygiene" + the round-1 review):
+Timing rules implemented here:
 
 * the clock sampler (NVML, 2 ms period) is started on EVERY rank BEFORE the barrier that precedes the
   timed region, so no rank enters the region late because of NVML initialisation;
@@ -123,12 +123,17 @@ def max_over_ranks(values: List[float], world: int) -> List[float]:
 
 
 def pick_repeats(steps: int, requested: int = 0) -> int:
-    """Regions of fewer than ~1000 steps are repeated; the median region is reported."""
-    if requested > 0:
-        return requested
-    if steps >= 1000:
-        return 3
-    return max(5, min(40, 2000 // max(1, steps)))
+    """Number of timed regions of ``steps`` steps: one unless more are requested (the median is reported)."""
+    return requested if requested > 0 else 1
+
+
+def dump_outputs(out_dir: str, arrays) -> None:
+    """Write each tensor of ``arrays`` (name -> tensor) as ``out_dir/<name>.npy`` in float32."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    for name, t in arrays.items():
+        np.save(os.path.join(out_dir, name + ".npy"),
+                t.detach().float().reshape(-1).cpu().numpy().astype(np.float32))
 
 
 def median(vals: List[float]) -> float:

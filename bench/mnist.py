@@ -7,12 +7,12 @@ import sys
 from bench import common
 
 PER_GPU_BATCH = 128
-POOL_BATCHES = 672          # 672 * 128 * 784 * 4 B = 269.7 MB  > 126 MB L2
+POOL_BATCHES = 672          # 672 * 128 * 784 * 4 B = 269.7 MB  > 50 MB L2
 METRIC = "samples/sec, Keras MNIST-CNN Horovod path (whole job)"
 DATA = ("synthetic (MNIST-shaped, class-conditional so the loss can fall: x = 0.5*template[y] + 0.5*U(0,1)), "
         "random-init weights")
 MODEL = "Keras MNIST-CNN (1,199,882 params), Adadelta(1.0*size), Horovod path"
-L2_NOTE = "inputs rotate through a 269.7 MB pool (> 126 MB L2); no flush"
+L2_NOTE = "inputs rotate through a 269.7 MB pool (> 50 MB L2); no flush"
 
 
 def make_pool(seed: int, nhwc: bool = True):
@@ -117,6 +117,9 @@ def run_ours(args):
         eng.stream.synchronize()
         region_ms = common.timed_regions(world, steps, repeats, run, dev_barrier, eng.stream, sampler)
     clocks = sampler.stop()
+    if args.dump_outputs and rank == 0:
+        eng.stream.synchronize()
+        common.dump_outputs(args.dump_outputs, {"loss": eng._loss, "params": eng.fused.flat_params})
     ms_per_step = common.median(region_ms) / steps
 
     # ---- exposed communication: the same step with the exchange in LOCAL mode (world-1 arena) ----

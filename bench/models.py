@@ -21,15 +21,15 @@ import os
 from bench import common
 
 RESNET_BATCH, BERT_BATCH, BERT_SEQ = 64, 32, 128
-RESNET_POOL = 8            # 8 x 64 x 3 x 224 x 224 x 4 B = 308 MB of inputs (> 126 MB L2), rotated
+RESNET_POOL = 8            # 8 x 64 x 3 x 224 x 224 x 4 B = 308 MB of inputs (> 50 MB L2), rotated
 BERT_POOL = 8
 
 
 def _record(metric, unit, world, args, warm, repeats, ms_per_step, per_gpu_batch, impl, clocks, model, extra=None):
     cfg = {"model": model, "global_batch": world * per_gpu_batch, "per_gpu_batch": per_gpu_batch,
            "seq_len": BERT_SEQ if args.config == "bert" else None, "parallelism": f"dp{world}",
-           "l2": "inputs rotate through a pool larger than the 126 MB L2" if args.config == "resnet50"
-                 else "activations + 220 MB of bf16 weights per step exceed the 126 MB L2"}
+           "l2": "inputs rotate through a pool larger than the 50 MB L2" if args.config == "resnet50"
+                 else "activations + 220 MB of bf16 weights per step exceed the 50 MB L2"}
     cfg.update(extra or {})
     return {"metric": metric, "value": world * per_gpu_batch / (ms_per_step * 1e-3), "unit": unit, "n_gpus": world,
             "steps": args.steps, "warmup": warm, "repeats": repeats, "ms_per_step": ms_per_step,

@@ -1,4 +1,4 @@
-"""`bench.py --impl reference`: the UNMODIFIED reference (baseline/_ref/tf_yarn) on the headline config.
+"""`bench.py --impl reference`: the UNMODIFIED reference (oracle/_ref/tf_yarn) on the headline config.
 
 What runs is the reference's own PyTorch worker, `tf_yarn.pytorch.tasks.worker._train`
 (reference: tf_yarn/pytorch/tasks/worker.py:94-122): it fetches the cloudpickled experiment function from the
@@ -20,11 +20,10 @@ from __future__ import annotations
 import datetime
 import os
 import socket
-import subprocess
 import sys
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-REF_DIR = os.path.join(ROOT, "baseline", "_ref")
+REF_DIR = os.path.join(ROOT, "oracle", "_ref")
 SHIMS = os.path.join(ROOT, "bench", "shims")
 
 
@@ -36,29 +35,10 @@ def _unavailable(why: str) -> int:
 
 
 def _ensure_installed() -> str:
-    """baseline/_ref is git-ignored; (re)install it from /root/reference when it is missing."""
+    """oracle/_ref is built by ``python __graft_entry__.py`` (oracle/build_ref.py) when the reference sources exist."""
     if os.path.isdir(os.path.join(REF_DIR, "tf_yarn")):
         return ""
-    src = "/root/reference"
-    if not os.path.isdir(src):
-        return "baseline/_ref is missing and /root/reference is not mounted on this box"
-    if int(os.environ.get("LOCAL_RANK", 0)) != 0:
-        import time
-        for _ in range(600):
-            if os.path.isfile(os.path.join(REF_DIR, ".installed")):
-                return ""
-            time.sleep(0.5)
-        return "timed out waiting for local rank 0 to install the reference"
-    tmp = "/tmp/tfy_refcopy"
-    subprocess.run(["rm", "-rf", tmp], check=False)
-    subprocess.run(["cp", "-r", src, tmp], check=True)
-    cmd = [sys.executable, "-m", "pip", "install", "--no-index", "--no-build-isolation", "--no-deps",
-           "--find-links", "/opt/wheelhouse", "--target", REF_DIR, tmp]
-    p = subprocess.run(cmd, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)
-    if p.returncode != 0:
-        return "pip install of /root/reference failed: " + p.stdout.strip().splitlines()[-1][:200]
-    open(os.path.join(REF_DIR, ".installed"), "w").close()
-    return ""
+    return "oracle/_ref is not built (the original project's sources were not available to build())"
 
 
 # ------------------------------------------------------------------------------------------------------
@@ -211,7 +191,7 @@ def make_experiment_fn(steps: int, warmup: int, repeats: int, world: int, config
                               "repeats": repeats, "ms_per_step": e2e_ms_per_step, "final_loss": last["loss"]}
                 out["gpu_launches"] = 0
                 out["params_in_sync"] = in_sync
-                out["reference_path"] = "baseline/_ref/tf_yarn/pytorch/tasks/worker.py::_train"
+                out["reference_path"] = "oracle/_ref/tf_yarn/pytorch/tasks/worker.py::_train"
                 common.emit(out)
 
         return PytorchExperiment(

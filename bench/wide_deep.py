@@ -3,14 +3,14 @@
     python bench.py --config wide_deep --gpus 8 [--steps K --warmup W]        (plain python, NOT torchrun:
         the job is launched THROUGH the public API, `run_on_yarn`, which starts its own task processes)
 
-Topology by --gpus (one B200 per cluster task; the BASELINE config is the 8-GPU row):
+Topology by --gpus (one H100 per cluster task; the BASELINE config is the 8-GPU row):
 
     8: 1 chief + 5 workers + 2 ps      4: 1 chief + 2 workers + 1 ps      2: 1 chief + 1 ps      1: chief and ps share GPU 0
 
 ours    : DNNLinearCombinedClassifier (FTRL wide tower, Adagrad deep tower; 26 hashed categorical columns of 100k
           buckets, 13 numeric, embedding dim 64, hidden 1024-512-256, batch 512 per trainer) with the HBM parameter
           server: shards in the ps ranks' HBM, embedding rows gathered / pushed over NVLink by the K5/K6 kernels,
-          Dense weights streamed by TMA into the tcgen05 GEMMs, whole step captured in a CUDA graph.
+          Dense weights streamed by TMA into the wgmma GEMMs, whole step captured in a CUDA graph.
 standin : the same model and topology written with stock PyTorch the way a TF-PS job works on an NCCL build:
           every step a worker receives the dense variables and the embedding rows it needs from the ps ranks
           (NCCL send/recv), runs cuBLAS/`embedding_bag`, sends the gradients back; the ps rank applies them
@@ -212,7 +212,7 @@ def run(args):
                                f"hidden {HIDDEN}, FTRL(wide) + Adagrad(deep)", "topology": f"{n_chief} chief + {n_worker} "
                                f"workers + {n_ps} ps", "global_batch": n_trainers * BATCH, "per_gpu_batch": BATCH,
                       "seq_len": None, "parallelism": f"async-ps {n_trainers} trainers / {n_ps} ps",
-                      "l2": "embedding tables (26 x 100k x 64 fp32 x 3 slots = 2 GB) exceed the 126 MB L2",
+                      "l2": "embedding tables (26 x 100k x 64 fp32 x 3 slots = 2 GB) exceed the 50 MB L2",
                       "cuda_graph": all(r.get("graph") for r in res), "graph_error": res[0].get("graph_error"),
                       "k5_gather_fused_into_first_gemm": all(r.get("fused_first_layer") for r in res),
                       "launched_by": "run_on_yarn"},

@@ -8,7 +8,7 @@ from setuptools import find_packages, setup
 setup(
     name="tf_yarn_b200",
     version="0.2.0",
-    description="B200-native distributed-training launcher with the capabilities of criteo/tf-yarn",
+    description="H100-native distributed-training launcher with the capabilities of criteo/tf-yarn",
     packages=find_packages(include=["tf_yarn_b200", "tf_yarn_b200.*"]),
     package_data={"tf_yarn_b200": ["default.log.conf", "ops/csrc/*", "kv/*.cpp", "examples/*.sh"]},
     python_requires=">=3.10",

@@ -22,7 +22,7 @@ def pytest_configure(config):
             torch.set_num_threads(1)
     except Exception:  # noqa: BLE001
         pass
-    config.addinivalue_line("markers", "gpu: needs a real B200 (run with `pytest -m gpu` under gpurun)")
+    config.addinivalue_line("markers", "gpu: needs a real H100 (run with `pytest -m gpu`)")
     config.addinivalue_line("markers", "slow: multi-process integration test")
 
 

@@ -1,4 +1,4 @@
-"""Multi-GPU numerics + timing check of the comm kernels (run under torchrun on B200).
+"""Multi-GPU numerics + timing check of the comm kernels (run under torchrun on H100).
 
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N --master-addr 127.0.0.1 \
         --master-port 29511 tests/gpu/comm_check.py [--quick]

@@ -1,11 +1,11 @@
-"""Size sweep of the all-reduce kernels (K1/K2/K3) and the fused step (K4, Adam) against NCCL on N B200s.
+"""Size sweep of the all-reduce kernels (K1/K2/K3) and the fused step (K4, Adam) against NCCL on N H100s.
 
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N --master-addr 127.0.0.1 \
         --master-port 29521 tests/gpu/comm_sweep.py [--max-mb 512] [--out gpurun_out/comm_sweep_N<N>.json]
 
 For every size: CUDA-event time of back-to-back launches after warm-up, MAX over ranks; bus bandwidth
 2(N-1)/N * S / t and the fraction of the NVLS floor t_floor = S (1 + 1/N) / 770 GB/s (the measured
-per-direction peer bandwidth of B200_PROFILING.md; 900 GB/s nominal).  Also the cost of the bare
+per-direction NVLink peer bandwidth).  Also the cost of the bare
 cross-GPU barrier kernel for several grid sizes (the latency floor of every kernel here).
 """
 from __future__ import annotations

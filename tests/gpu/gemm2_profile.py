@@ -1,4 +1,4 @@
-"""One launch each of the persistent cta_group::2 GEMM at 8192^3 and 4096^3 (bf16), for `ncu --set full -k regex:tfy_gemm2`.
+"""One launch each of the persistent two-warpgroup GEMM at 8192^3 and 4096^3 (bf16), for `ncu --set full -k regex:tfy_gemm2`.
 
     ncu --set full --clock-control none --import-source on -k regex:tfy_gemm2 -o gpurun_out/prof_gemm2 \
         python tests/gpu/gemm2_profile.py

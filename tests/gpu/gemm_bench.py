@@ -1,9 +1,9 @@
-"""tcgen05 GEMM of this repo vs cuBLAS (torch.matmul) at large shapes, bf16, on one B200.
+"""wgmma GEMM of this repo vs cuBLAS (torch.matmul) at large shapes, bf16, on one H100.
 
     python tests/gpu/gemm_bench.py [--out gpurun_out/gemm_bench.json]
 
 TFLOP/s = 2 M N K / CUDA-event time (median of 5 regions of `iters` launches, L2 flushed by rotating through
-operand copies larger than the 126 MB L2); fractions are of MEASURED_PEAKS.json (bf16_tflops burst / sustained).
+operand copies larger than the 50 MB L2); fractions are of MEASURED_PEAKS.json (bf16_tflops burst / sustained).
 """
 import argparse
 import json

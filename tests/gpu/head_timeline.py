@@ -24,7 +24,7 @@ dw2 = torch.zeros(C, K, dtype=torch.bfloat16, device=dev)
 db2 = torch.zeros(C, dtype=torch.bfloat16, device=dev)
 dh = torch.zeros(B, K, dtype=torch.bfloat16, device=dev)
 db1 = torch.zeros(K, dtype=torch.bfloat16, device=dev)
-scratch = torch.zeros(int(lib.tfy_dense_head_scratch_elems(K, C)), device=dev)
+scratch = torch.zeros(int(lib.tfy_dense_head_scratch_elems(K, C, B)), device=dev)
 counter = torch.zeros(1, dtype=torch.int32, device=dev)
 
 

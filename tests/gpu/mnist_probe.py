@@ -1,4 +1,4 @@
-"""Probe: how fast is the MNIST-CNN step with stock PyTorch pieces on B200?
+"""Probe: how fast is the MNIST-CNN step with stock PyTorch pieces on H100?
 
 Design input for the mini-Keras train step (which ops are worth replacing).
 Times eager vs CUDA-graphed fwd+bwd(+optimizer) in bf16 at batch 128.

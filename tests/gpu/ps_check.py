@@ -1,4 +1,4 @@
-"""B200 check of the HBM parameter-server path (K5 pull incl. remote-weight GEMM, K6 push).
+"""H100 check of the HBM parameter-server path (K5 pull incl. remote-weight GEMM, K6 push).
 
 Run on a box with >= 2 GPUs:   python tests/gpu/ps_check.py [n_workers]
 Topology: 1 chief + n_workers workers + 1 ps (one GPU each) + evaluator on CPU.

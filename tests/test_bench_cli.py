@@ -19,9 +19,9 @@ def test_reference_control_plane_through_the_shims(monkeypatch):
     """The UNMODIFIED reference's control-plane code (event.broadcast / wait, choose_master, _get_experiment,
     TaskSpec) runs against this repo's KV server through bench/shims (what `bench.py --impl reference` relies on)."""
     import pytest
-    ref = os.path.join(ROOT, "baseline", "_ref")
+    ref = os.path.join(ROOT, "oracle", "_ref")
     if not os.path.isdir(os.path.join(ref, "tf_yarn")):
-        pytest.skip("baseline/_ref is not installed")
+        pytest.skip("oracle/_ref is not built: build() installs it when the original project's sources exist")
     code = r"""
 import os, sys
 sys.path[:0] = [os.path.join(%r, "bench", "shims"), %r, %r]

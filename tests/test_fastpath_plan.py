@@ -1,5 +1,5 @@
 """The fast path's layer-pattern grammar (keras/fastpath.py: build_plan), checkable without a GPU: which Sequential
-models are served by the fused tcgen05 kernels, which stages they become, and that anything outside the grammar falls
+models are served by the fused wgmma kernels, which stages they become, and that anything outside the grammar falls
 back to the autograd engine (None) instead of being mis-compiled."""
 import pytest
 import torch
@@ -72,7 +72,7 @@ def test_models_outside_the_grammar_fall_back(layers, loss, metrics):
 
 
 def test_kernel_envelopes_split_k_and_tensor_core_conv(monkeypatch):
-    """Which shapes go to the split-K tcgen05 GEMM and to the tcgen05 convolution kernels (everything else is served by
+    """Which shapes go to the split-K wgmma GEMM and to the wgmma convolution kernels (everything else is served by
     cuBLAS / cuDNN with a one-time warning)."""
     E = fastpath.FastSequentialEngine
     assert E._split_k(128, 128, 9216) == 24            # the MNIST Dense: 144 k-tiles, 6 per CTA

@@ -1,4 +1,4 @@
-"""GPU tests of the B200 train engines (run with `pytest -m gpu` on a B200).
+"""GPU tests of the H100 train engines (run with `pytest -m gpu` on an H100).
 
 Numerics of every hand-written kernel on the single-GPU path are compared with a plain
 PyTorch fp32 reference of the same op.
@@ -188,6 +188,35 @@ def _run_steps(fast: bool, steps: int = 4):
     return m, losses
 
 
+def test_fastpath_training_is_bitwise_reproducible():
+    """Same seed, same batches, dropout on: two fast-path trainings end with bit-identical losses and parameters
+    (every batch reduction of the step -- split-K GEMM, classifier head, weight gradients -- sums in a fixed order)."""
+    from tf_yarn_b200 import keras
+    from tf_yarn_b200.keras.fastpath import FastSequentialEngine
+
+    def train():
+        torch.manual_seed(7)
+        m = _mnist_like(0.25, 0.5)
+        m.compile(loss=keras.losses.SparseCategoricalCrossentropy(from_logits=True),
+                  optimizer=keras.optimizers.Adadelta(1.0), use_fast_path=True)
+        g = torch.Generator().manual_seed(11)
+        x = torch.rand(128 * 12, 28, 28, 1, generator=g)
+        y = torch.randint(0, 10, (128 * 12,), generator=g)
+        hist = m.fit(x, y, batch_size=128, epochs=2, shuffle=False, verbose=0)
+        assert isinstance(m._engine, FastSequentialEngine)
+        torch.cuda.synchronize()
+        return hist.history["loss"], m._engine.fused.flat_params.clone(), [torch.as_tensor(w) for w in m.get_weights()]
+
+    l1, p1, w1 = train()
+    l2, p2, w2 = train()
+    assert l1 == l2, (l1, l2)
+    def bits(t):
+        return t.contiguous().view(torch.int16 if t.element_size() == 2 else torch.int32)
+    assert torch.equal(bits(p1), bits(p2))
+    for a, b in zip(w1, w2):
+        assert torch.equal(bits(a), bits(b))
+
+
 def test_fastpath_matches_autograd_engine():
     """Same init, same batches, dropout off: the fused-kernel plan must track the autograd engine."""
     from tf_yarn_b200.keras.fastpath import FastSequentialEngine
@@ -238,7 +267,7 @@ def test_smoke_entry():
 @pytest.mark.parametrize("shape", [(128, 128, 64), (128, 128, 9216), (256, 384, 512), (100, 72, 200), (1000, 10, 128),
                                    (128, 9216, 128)])
 def test_tcgen05_gemm_matches_fp32_reference(shape):
-    """tcgen05/TMEM/TMA GEMM vs a plain fp32 matmul of the same bf16 inputs (tails, bias, relu)."""
+    """wgmma/TMA GEMM vs a plain fp32 matmul of the same bf16 inputs (tails, bias, relu)."""
     from tf_yarn_b200.ops.gemm import gemm_bf16
     M, N, K = shape
     g = torch.Generator(device="cuda").manual_seed(M * 7 + N * 3 + K)
@@ -297,7 +326,7 @@ def test_fused_dense_head_matches_autograd(B, K, C):
     db2 = torch.zeros(C, dtype=torch.bfloat16, device=dev)
     dh = torch.zeros(B, K, dtype=torch.bfloat16, device=dev)
     db1 = torch.zeros(K, dtype=torch.bfloat16, device=dev)
-    scratch = torch.zeros(int(lib.tfy_dense_head_scratch_elems(K, C)), device=dev)
+    scratch = torch.zeros(int(lib.tfy_dense_head_scratch_elems(K, C, B)), device=dev)
     counter = torch.zeros(1, dtype=torch.int32, device=dev)
     # reference
     hf = h.float().requires_grad_(True)
@@ -333,7 +362,7 @@ def test_fused_dense_head_matches_autograd(B, K, C):
                                             # batch / width beyond one tile: the tiled kernel (K loops, TMA ring)
                                             (512, 1024, 1680, True), (300, 136, 264, True), (512, 256, 1024, False)])
 def test_tcgen05_dense_backward_matches_fp32_reference(B, U, I, want_dx):
-    """dW = dh^T x and dx = dh W out of ONE tcgen05 kernel (MN-major operand views of the same tiles, TMA-store
+    """dW = dh^T x and dx = dh W out of ONE wgmma kernel (MN-major operand views of the same tiles, TMA-store
     epilogue) vs fp32 matmuls of the same bf16 inputs; ragged extents exercise the TMA zero-fill / clipping."""
     from tf_yarn_b200.keras import fastpath  # noqa: F401  (declares the kernel)
     from tf_yarn_b200.ops import native
@@ -417,7 +446,7 @@ def test_fused_splitk_epilogue_matches_two_launch_path(monkeypatch):
 
 @pytest.mark.parametrize("shape", [(256, 256, 64), (512, 768, 512), (1000, 520, 264), (4096, 1024, 128), (130, 304, 72)])
 def test_tcgen05_2cta_gemm_matches_fp32_reference(shape):
-    """Persistent cta_group::2 GEMM (256x256 tiles of a CTA pair, double-buffered TMEM, TMA-store epilogue) vs fp32."""
+    """Persistent two-warpgroup wgmma GEMM (128x256 tiles, register epilogue) vs fp32."""
     from tf_yarn_b200.ops.gemm import gemm_bf16
     M, N, K = shape
     g = torch.Generator(device="cuda").manual_seed(M + 3 * N + 7 * K)
@@ -436,7 +465,7 @@ def test_tcgen05_2cta_gemm_matches_fp32_reference(shape):
 
 @pytest.mark.parametrize("B,N,T,n_num", [(200, 264, 3, 13), (512, 1024, 26, 13), (64, 8, 1, 0)])
 def test_ps_gather_gemm_matches_fp32_reference(B, N, T, n_num):
-    """K5: embedding-row gather (A-operand producer) + remote-weight tcgen05 GEMM + bias in one kernel vs the unfused
+    """K5: embedding-row gather (A-operand producer) + remote-weight wgmma GEMM + bias in one kernel vs the unfused
     fp32 computation (same bf16 rounding of activations and weights); the gathered activations it keeps for the
     backward must equal the gathered rows."""
     from tf_yarn_b200.estimator import ps_hbm  # noqa: F401  (declares the kernel)

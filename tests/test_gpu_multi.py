@@ -1,4 +1,4 @@
-"""Multi-GPU tests (run with `pytest -m gpu` on a box with >= 2 B200s; skipped otherwise).
+"""Multi-GPU tests (run with `pytest -m gpu` on a box with >= 2 H100s; skipped otherwise).
 
 The stand-alone checks under tests/gpu/ are launched with torch.distributed.run, one process per GPU:
 every collective / fused-step kernel against an fp32 PyTorch reference and against NCCL, the parameter-server

@@ -159,6 +159,6 @@ def test_every_kernel_launched_with_programmatic_dependent_launch_waits_for_its_
         waits = [body.find(w) for w in ("tfy_pdl_sync()", "tfy_pdl_wait()") if w in body]
         assert waits, f"{kernel} ({os.path.basename(path)}) is launched with PDL but never waits for its dependency"
         prologue = body[:min(waits)]
-        # the prologue may set up shared memory, barriers, TMEM and prefetch tensor maps / this kernel's own state
+        # the prologue may set up shared memory, barriers and prefetch tensor maps / this kernel's own state
         for forbidden in ("tfy_ld16(", "__ldg(", "__ldcg(", "atomicAdd(", "tfy_st16(", "red_add", "cp.async.bulk.tensor"):
             assert forbidden not in prologue, (kernel, forbidden)

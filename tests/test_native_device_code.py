@@ -1,7 +1,7 @@
 """The update formulas of the fused K4 kernel (ops/csrc/tfy_fused_step.cuh: tfy_step_consts + tfy_opt_update_rt), built
 for the host and checked against torch.optim on the CPU -- through the framework's own chain: mini-Keras optimizer
 -> OptimizerSpec (hyper-parameter packing) -> TfyOptHyper (device struct) -> per-element update.  The GPU tests cover
-SGD / Adadelta / Adam / Adagrad in LOCAL mode on a B200; this also covers FTRL, AdamW, Nesterov momentum, weight decay
+SGD / Adadelta / Adam / Adagrad in LOCAL mode on a H100; this also covers FTRL, AdamW, Nesterov momentum, weight decay
 and the 1/world gradient scaling, on every box."""
 import ctypes
 import os

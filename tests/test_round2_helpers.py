@@ -62,17 +62,18 @@ def test_checkpoint_without_a_step_is_rejected_loudly():
 def test_bench_region_arithmetic():
     sys.path.insert(0, ROOT)
     from bench import common
-    assert common.pick_repeats(20) == 40 and common.pick_repeats(200) == 10 and common.pick_repeats(500) == 5
-    assert common.pick_repeats(1000) == 3 and common.pick_repeats(20, requested=7) == 7
+    # one timed region of exactly --steps steps unless more regions are requested
+    assert common.pick_repeats(20) == 1 and common.pick_repeats(200) == 1 and common.pick_repeats(1000) == 1
+    assert common.pick_repeats(20, requested=7) == 7
     assert common.median([3.0, 1.0, 2.0]) == 2.0 and common.median([4.0, 1.0, 2.0, 3.0]) == 2.5
 
 
 def test_results_table_reads_the_committed_bench_lines():
-    out = subprocess.run([sys.executable, os.path.join(ROOT, "tools", "results_table.py")], capture_output=True, text=True,
-                         cwd=ROOT)
+    out = subprocess.run([sys.executable, os.path.join(ROOT, "tools", "results_table.py"),
+                          os.path.join(ROOT, "tests", "golden", "bench_lines")], capture_output=True, text=True, cwd=ROOT)
     assert out.returncode == 0, out.stderr
     assert "| 8 |" in out.stdout and "Scaling efficiency" in out.stdout and "### wide_deep" in out.stdout
-    d = json.load(open(os.path.join(ROOT, "profiles", "r2", "bench_mnist_ours_N8_r2v.json")))
+    d = json.load(open(os.path.join(ROOT, "tests", "golden", "bench_lines", "bench_mnist_ours_N8_t.json")))
     for key in ("metric", "value", "unit", "n_gpus", "steps", "warmup", "ms_per_step", "higher_is_better", "scaling",
                 "vs_baseline", "dtype", "data", "config", "clocks", "e2e", "gpu_launches"):
         assert key in d, key

@@ -2,7 +2,7 @@
 
 Runs the real C++ code path (connect / SCM_RIGHTS / accept ordering) with several
 processes and no GPU: every rank sends to all peers BEFORE accepting, which must not
-deadlock (a first version waited for an ack and hung on the B200 box).
+deadlock (a first version waited for an ack and hung on the H100 box).
 """
 import multiprocessing as mp
 import os

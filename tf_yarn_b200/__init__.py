@@ -1,4 +1,4 @@
-"""tf_yarn_b200: a B200-native distributed-training launcher with the capabilities of criteo/tf-yarn.
+"""tf_yarn_b200: a H100-native distributed-training launcher with the capabilities of criteo/tf-yarn.
 
 Public surface (reference: tf_yarn/__init__.py:1-8)::
 

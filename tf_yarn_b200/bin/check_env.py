@@ -51,8 +51,8 @@ def check_gpus() -> bool:
         prop = torch.cuda.get_device_properties(i)
         logger.info("GPU %d: %s sm_%d%d %.0f GB %d SMs", i, prop.name, prop.major, prop.minor,
                     prop.total_memory / 2 ** 30, prop.multi_processor_count)
-        if (prop.major, prop.minor) != (10, 0):
-            logger.warning("GPU %d is not sm_100 (B200): the kernels are compiled for sm_100a only", i)
+        if (prop.major, prop.minor) != (9, 0):
+            logger.warning("GPU %d is not sm_90 (H100): the kernels are compiled for sm_90a only", i)
             ok = False
     for i in range(n):
         for j in range(n):

@@ -3,7 +3,7 @@
 The reference (tf_yarn/bin/check_hadoop_env.py:26-172) verifies the Hadoop variables, does a round trip
 of a small file through HDFS with TensorFlow's filesystem layer, launches a one-container application that
 re-reads the file and posts ``result`` to the KV store, and writes everything to ``check_hadoop_env.log``
-in the working directory.  There is neither Hadoop nor YARN on a B200 box: this module keeps the command,
+in the working directory.  There is neither Hadoop nor YARN on a H100 box: this module keeps the command,
 the hidden ``--file`` container mode, the ``result`` key and the log file, and runs the single-box
 equivalents (toolchain, native kernels, GPUs + peer access, KV store, file round trip through
 :mod:`tf_yarn_b200.utils.fs`, one-task application through the local launcher) implemented in
@@ -113,7 +113,7 @@ def main(argv=None) -> int:
             if check_ok:
                 check_ok = launch_remote_check(path)
                 logger.info("remote_check: %s", check_ok)
-    logger.info("B200 box setup: %s", "OK" if check_ok else "KO")
+    logger.info("H100 box setup: %s", "OK" if check_ok else "KO")
     return 0 if check_ok else 1
 
 

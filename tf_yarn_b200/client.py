@@ -4,7 +4,7 @@
 tf_yarn/client.py:299-469) so user scripts switch over by changing an import;
 ``run_on_b200`` is an alias.  What changes is the substrate: instead of a
 skein/YARN application, :mod:`tf_yarn_b200.launcher.local` starts one process per
-task instance on this 8xB200 box, pins GPU-labelled instances to B200s and
+task instance on this 8xH100 box, pins GPU-labelled instances to H100s and
 hosts the KV rendezvous store.  YARN-only arguments (``queue``, ``acls``,
 ``file_systems``, ``pyenv_zip_path``, ``cuda_runtime_hdfs_path``) are accepted
 and ignored with a debug log.
@@ -103,7 +103,7 @@ def _setup_to_use_cuda_archive(env: Dict[str, str], pre_script_hook: str, cuda_r
     """The reference ships a CUDA runtime tarball from HDFS (client.py:154-167); the box already has
     CUDA 12.9, so this only validates the arguments the same way and leaves the hook untouched."""
     if "LD_LIBRARY_PATH" not in env:
-        logger.warning("No LD_LIBRARY_PATH found in env. The cuda archive option is ignored on a B200 box.")
+        logger.warning("No LD_LIBRARY_PATH found in env. The cuda archive option is ignored on a H100 box.")
         return pre_script_hook
     logger.info("cuda_runtime_hdfs_path=%s ignored: the box's CUDA toolkit is used", cuda_runtime_hdfs_path)
     return pre_script_hook
@@ -204,7 +204,7 @@ def run_on_yarn(
         cuda_runtime_hdfs_path: Optional[str] = None,
         poll_every_secs: float = DEFAULT_POLL_EVERY_SECS,
 ) -> Optional[metrics.Metrics]:
-    """Run an experiment on the local 8xB200 box.
+    """Run an experiment on the local 8xH100 box.
 
     Parameters keep the reference's meaning (reference: tf_yarn/client.py:317-417):
 

@@ -30,7 +30,7 @@ class TaskParameters(NamedTuple):
     master_port: int
     n_workers_per_executor: int = 1
     local_rank: int = 0
-    device: Optional[int] = None   # B200 index assigned by the launcher (None on CPU)
+    device: Optional[int] = None   # H100 index assigned by the launcher (None on CPU)
 
 
 def _gpu_for(local_rank: int) -> Optional[int]:

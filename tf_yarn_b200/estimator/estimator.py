@@ -12,7 +12,7 @@ Three training data planes, chosen from the process's role:
 * local / single process  -- plain optimizer step;
 * all-reduce (``optimizer`` wrapped by ``hvd.DistributedOptimizer``) -- gradients
   averaged across ranks by ONE all-reduce kernel over the fusion buffer (NVLS / P2P kernels of
-  ``ops/csrc/tfy_comm.cu`` on B200, gloo on CPU), then the optimizer step (the fully fused
+  ``ops/csrc/tfy_comm.cu`` on H100, gloo on CPU), then the optimizer step (the fully fused
   reduce-scatter -> optimizer -> all-gather kernel serves the Keras engines and the DDP wrapper);
 * parameter server (``TF_CONFIG`` lists ``ps`` tasks) -- parameters live on the ps
   ranks; workers pull before and push after every step, asynchronously
@@ -389,7 +389,7 @@ class Estimator:
         return loss.detach()
 
     def _ps_step_cuda(self, features, labels) -> torch.Tensor:
-        """B200 parameter-server step.  After three eager steps the whole pull/forward/backward/push sequence is
+        """H100 parameter-server step.  After three eager steps the whole pull/forward/backward/push sequence is
         captured in a CUDA graph and replayed on static input buffers: the data plane is a handful of
         microsecond-scale peer-memory kernels, so an eager step is bound by Python / launch overhead (the
         round-1 review measured it host-bound).  TFY_PS_GRAPH=0 keeps it eager."""

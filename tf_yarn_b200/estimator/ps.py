@@ -13,7 +13,7 @@ read (pull) and update (push) the shard memory directly:
 
 * CPU box (plumbing / CI):  the shard is a POSIX shared-memory file mapped by
   every worker (``ShmShard``).
-* B200:  the shard lives in the ps rank's HBM inside the symmetric arena;
+* H100:  the shard lives in the ps rank's HBM inside the symmetric arena;
   workers reach it over NVLink with the K5 (pull) / K6 (push) kernels
   (``HbmShard``, :mod:`tf_yarn_b200.parallel.ps_kernels`).
 

@@ -1,4 +1,4 @@
-"""B200 data plane of the asynchronous parameter server: shards in the ps ranks' HBM.
+"""H100 data plane of the asynchronous parameter server: shards in the ps ranks' HBM.
 
 Every task of the training cluster (chief, workers AND ps) joins one symmetric arena
 (:mod:`tf_yarn_b200.parallel.symm`, rendezvous through the launcher's KV store).  A ps rank's
@@ -7,7 +7,7 @@ shard is a region of ITS arena; chief/workers reach it through the peer mapping 
 * dense pull   : ``tfy_ps_pull`` -- peer fp32 master -> local replica, ONE launch for the variables that need a
   local copy (biases, small vectors); Dense weights and embedding rows are never copied;
 * GEMM pull    : the weight matrix of a Dense layer stays on the ps rank: its row-padded bf16 shadow is streamed
-  by TMA into the tcgen05 GEMM that consumes it (forward ``tfy_gemm_bf16``, backward ``tfy_dense_bwd``: dW and
+  by TMA into the wgmma GEMM that consumes it (forward ``tfy_gemm_bf16``, backward ``tfy_dense_bwd``: dW and
   dx in one kernel against the same remote shadow);
 * sparse pull  : ``tfy_ps_embedding_bag`` / ``tfy_ps_multi_bag`` (all tables of a tower in one launch); for the
   first deep layer the gather IS the A-operand producer of the GEMM (K5, ``tfy_ps_gather_gemm``);
@@ -354,7 +354,7 @@ def _make_linear_forward(conn: HbmConnection, idx: int, mod: nn.Linear):
             dyb = dy.to(torch.bfloat16).contiguous()
             dw = torch.empty((N, Kp), dtype=torch.bfloat16, device=dy.device)
             dx = torch.empty((B, Kp), dtype=torch.bfloat16, device=dy.device) if ctx.needs_input_grad[0] else None
-            # dW = dy^T x and dx = dy W in one tcgen05 kernel; W is the ps rank's bf16 shadow, read over NVLink
+            # dW = dy^T x and dx = dy W in one wgmma kernel; W is the ps rank's bf16 shadow, read over NVLink
             native.check(conn.lib.tfy_dense_bwd(dyb.data_ptr(), xb.data_ptr(), shadow, dw.data_ptr(),
                                                 dx.data_ptr() if dx is not None else None, B, N, Kp,
                                                 torch.cuda.current_stream().cuda_stream), "tfy_dense_bwd")
@@ -475,7 +475,7 @@ def _try_fuse_first_layer(conn: HbmConnection, network: nn.Module) -> bool:
     Pattern (the canned wide-and-deep / DNN networks): ``network.dense_features`` concatenates embedding columns
     of dimension 64 with one id per example followed by numeric columns (<= 64 values in total), and
     ``network.hidden[0]`` is a Linear served by the remote-weight GEMM.  The gather of the rows from the ps ranks'
-    HBM becomes the A-operand producer of that GEMM; the backward (dW, dx) is one tcgen05 kernel against the same
+    HBM becomes the A-operand producer of that GEMM; the backward (dW, dx) is one wgmma kernel against the same
     remote shadow, and the row gradients are pushed straight out of its dx.  TFY_PS_FUSE_FIRST=0 disables it."""
     from tf_yarn_b200.estimator import feature_column as fc
     if os.environ.get("TFY_PS_FUSE_FIRST", "1") == "0":
@@ -630,7 +630,7 @@ def connect_worker(network: nn.Module, opt_desc, cluster, is_chief: bool, global
 
 
 def serve(cluster, poll_secs: float = 0.2) -> None:
-    """``ps`` task on B200: join the arena, reserve the shard region, publish the header, idle."""
+    """``ps`` task on H100: join the arena, reserve the shard region, publish the header, idle."""
     import time
     client = _task_commons.TaskClient.from_current()
     kv = client.kv

@@ -1,7 +1,7 @@
 """The BASELINE.json configurations as runnable examples (not in the reference tree: they exercise its three
 training paths -- Horovod all-reduce, parameter server, torch DDP -- at realistic sizes).
 
-Every example runs at full size on a B200 box and at toy size on a CPU-only box (``EXAMPLE_SMALL=1`` forces the toy
+Every example runs at full size on a H100 box and at toy size on a CPU-only box (``EXAMPLE_SMALL=1`` forces the toy
 size); all data is synthetic (no network).
 """
 import os

@@ -1,4 +1,4 @@
-"""BASELINE config 5: Keras BERT-base pre-training on the Horovod all-reduce path, bf16, one trainer per B200,
+"""BASELINE config 5: Keras BERT-base pre-training on the Horovod all-reduce path, bf16, one trainer per H100,
 with the evaluator and TensorBoard side tasks.
 
     python -m tf_yarn_b200.examples.baseline.bert_allreduce

@@ -1,10 +1,10 @@
-"""BASELINE config 2: Keras MNIST-CNN on the Horovod all-reduce path, one trainer per B200.
+"""BASELINE config 2: Keras MNIST-CNN on the Horovod all-reduce path, one trainer per H100.
 
     python -m tf_yarn_b200.examples.baseline.mnist_cnn_allreduce
 
 The model is the canonical Horovod ``keras_mnist`` network the reference's README compiles with
 ``Adadelta(1.0 * HVD_SIZE)`` (reference: README.md:104-113, examples/native_keras_with_gloo_example.py:65-90).
-On B200 the whole step is ten kernels of this repo captured in a CUDA graph; the gradient exchange is the fused
+On H100 the whole step is ten kernels of this repo captured in a CUDA graph; the gradient exchange is the fused
 reduce-scatter -> Adadelta -> all-gather kernel over NVSwitch.
 """
 import logging

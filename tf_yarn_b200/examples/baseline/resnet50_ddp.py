@@ -1,10 +1,10 @@
-"""BASELINE config 4: PytorchExperiment ResNet-50 under DistributedDataParallel, one worker per B200.
+"""BASELINE config 4: PytorchExperiment ResNet-50 under DistributedDataParallel, one worker per H100.
 
     python -m tf_yarn_b200.examples.baseline.resnet50_ddp
 
 The user code is what the reference expects (reference: tf_yarn/pytorch/experiment.py:6-56,
 examples/pytorch/pytorch_example.py:39-108): ``main_fn(model, loader, device, rank, tb_writer)`` receives the model
-already wrapped.  On B200 the wrapper is this repo's (bucketed NVLS reduction launched by a native reducer while
+already wrapped.  On H100 the wrapper is this repo's (bucketed NVLS reduction launched by a native reducer while
 backward runs); ``model.fuse_optimizer("sgd", ...)`` additionally moves the optimizer into that exchange.
 """
 import logging

@@ -1,10 +1,10 @@
 """BASELINE config 3: Estimator wide & deep on the asynchronous parameter-server path
-(1 chief + 5 workers + 2 ps on eight B200s; 1 chief + 1 worker + 1 ps on smaller boxes).
+(1 chief + 5 workers + 2 ps on eight H100s; 1 chief + 1 worker + 1 ps on smaller boxes).
 
     python -m tf_yarn_b200.examples.baseline.wide_deep_ps
 
 Same task program as the reference's default (reference: tf_yarn/tensorflow/tasks/_independent_workers_task.py:17-43,
-examples/keras_example.py:94-107).  On B200 the ps ranks only own HBM: workers gather embedding rows inside the first
+examples/keras_example.py:94-107).  On H100 the ps ranks only own HBM: workers gather embedding rows inside the first
 GEMM, stream the Dense weights over NVLink and push gradients with the FTRL / Adagrad update fused.
 """
 import logging

@@ -1,7 +1,7 @@
 """Keras model -> Estimator, trained with the asynchronous parameter-server strategy.
 
 1 chief + 4 workers + 2 ps + evaluator, as in the reference (reference:
-tf_yarn/examples/keras_example.py:55-107).  On a B200 box give the trainers / ps tasks
+tf_yarn/examples/keras_example.py:55-107).  On a H100 box give the trainers / ps tasks
 ``label=NodeLabel.GPU``: the shards then live in the ps ranks' HBM and are pulled / pushed over
 NVLink (K5 / K6 kernels); on a CPU box they live in shared memory.
 """

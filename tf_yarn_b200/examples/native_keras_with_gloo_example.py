@@ -2,7 +2,7 @@
 
 (reference: tf_yarn/examples/native_keras_with_gloo_example.py:41-111)
 
-Every trainer is one process on one B200; gradients are averaged by the fused
+Every trainer is one process on one H100; gradients are averaged by the fused
 reduce-scatter -> Adadelta -> all-gather kernel over NVLink (gloo only on CPU-only boxes).
 The evaluator picks up the chief's ``ModelCheckpoint`` files.
 """

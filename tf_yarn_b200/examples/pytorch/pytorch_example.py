@@ -2,7 +2,7 @@
 
 (reference: tf_yarn/examples/pytorch/pytorch_example.py:19-108)
 
-``main_fn`` receives the model wrapped for data-parallel training: on B200 that wrapper reduces the
+``main_fn`` receives the model wrapped for data-parallel training: on H100 that wrapper reduces the
 gradient buckets with the NVLS all-reduce kernels while backward is still running.
 CIFAR-10 is not downloadable on an air-gapped box: a synthetic dataset of the same shape is used.
 """

@@ -6,7 +6,7 @@ for ex in id_estimator_example linear_classifier_example keras_example native_ke
   echo "=== $ex"
   EXAMPLE_EPOCHS=1 python -m tf_yarn_b200.examples.$ex
 done
-# the BASELINE.json configurations (full size on B200, toy size on a CPU-only box or with EXAMPLE_SMALL=1)
+# the BASELINE.json configurations (full size on H100, toy size on a CPU-only box or with EXAMPLE_SMALL=1)
 for ex in baseline.mnist_cnn_allreduce baseline.wide_deep_ps baseline.resnet50_ddp baseline.bert_allreduce; do
   echo "=== $ex"
   EXAMPLE_EPOCHS=1 python -m tf_yarn_b200.examples.$ex

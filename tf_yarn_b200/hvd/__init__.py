@@ -1,4 +1,4 @@
-"""Horovod-shaped facade over the B200 comm runtime.
+"""Horovod-shaped facade over the H100 comm runtime.
 
 User code written for the reference's all-reduce path keeps working::
 
@@ -122,7 +122,7 @@ def ensure_cpu_group() -> None:
 
 
 def _communicator():
-    """The NVLink communicator of this rank (B200 only)."""
+    """The NVLink communicator of this rank (H100 only)."""
     from tf_yarn_b200.parallel import runtime
     from tf_yarn_b200.parallel.symm import default_rendezvous
     os.environ.setdefault("TFY_RANK", str(_state["rank"]))
@@ -264,7 +264,7 @@ class _KerasDistributedOptimizer:
 def DistributedOptimizer(optimizer, named_parameters=None, **_ignored):
     """Wrap an optimizer so that gradients are averaged over all ranks before the update.
 
-    * mini-Keras optimizer descriptor -> marker for ``compile`` (fused K4 kernel on B200);
+    * mini-Keras optimizer descriptor -> marker for ``compile`` (fused K4 kernel on H100);
     * a factory (callable returning a descriptor, as Estimators take) -> wrapped factory;
     * ``torch.optim.Optimizer`` -> same object whose ``step()`` first all-reduces the gradients.
     """

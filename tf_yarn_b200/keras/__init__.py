@@ -1,7 +1,7 @@
 """mini-Keras: a torch/CUDA-backed subset of the Keras API (TensorFlow is not required).
 
 The reference drives ``tf.keras`` models (``KerasExperiment``); this package
-accepts the same user-code patterns and runs them on the B200 train engine
+accepts the same user-code patterns and runs them on the H100 train engine
 (:mod:`tf_yarn_b200.keras.engine`).
 """
 from tf_yarn_b200.keras import callbacks, layers, losses, metrics, optimizers  # noqa: F401

@@ -1,6 +1,6 @@
 """Train-step engines behind ``Model.fit``.
 
-``GraphTrainEngine`` (B200) — the flagship path of the Horovod-style Keras
+``GraphTrainEngine`` (H100) — the flagship path of the Horovod-style Keras
 configuration:
 
 * parameters live in ONE flat bf16 buffer in the symmetric arena, gradients in

@@ -1,16 +1,16 @@
-"""Fast path of the B200 train engine: explicit forward/backward out of fused kernels.
+"""Fast path of the H100 train engine: explicit forward/backward out of fused kernels.
 
 For ``Sequential`` models made of Conv2D(3x3, valid, stride 1) / MaxPooling2D(2x2) /
 Dropout / Flatten / Dense layers with relu|linear activations and a sparse-categorical
 cross-entropy (from logits) head -- the MNIST-CNN of the headline benchmark, the wine MLP --
 the step does not go through autograd at all:
 
-* convolutions are tcgen05 implicit GEMMs (:mod:`ops/csrc/tfy_conv.cu`): conv2 forward with
+* convolutions are wgmma implicit GEMMs (:mod:`ops/csrc/tfy_conv.cu`): conv2 forward with
   bias + ReLU + 2x2 max-pool + dropout in the epilogue, conv2 data / weight gradients whose dz
   operand is rebuilt in shared memory from the pooled gradient (un-pool + dropout + ReLU gate
   fused, db included), the first layer's forward and weight/bias gradient with im2col built in
   shared memory;
-* the long-K Dense forward is the split-K tcgen05 GEMM (:mod:`ops/csrc/tfy_gemm.cu`);
+* the long-K Dense forward is the split-K wgmma GEMM (:mod:`ops/csrc/tfy_gemm.cu`);
 * the classifier head runs forward AND backward in one kernel (:mod:`ops/csrc/tfy_nn.cu`);
 * weight gradients are written straight into the flat gradient buffer consumed by the fused
   reduce-scatter / optimizer / all-gather kernel (no ``grad += g`` accumulation launches).
@@ -39,7 +39,7 @@ native.declare("tfy_conv3x3_c1_fwd", [_vp, _i, _vp, _vp, _vp, _i, _i, _i, _i, _v
 native.declare("tfy_conv3x3_c1_fwd_tc", [_vp, _i, _vp, _vp, _vp, _i, _i, _i, _vp])
 native.declare("tfy_conv3x3_c1_wgrad", [_vp, _i, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _vp])
 native.declare("tfy_bias_act_drop_fwd", [_vp, _vp, _vp, _vp, _sz, _i, _i, _f, _u32, _vp, _vp])
-native.declare("tfy_bias_act_drop_fwd_f32", [_vp, _vp, _vp, _vp, _sz, _i, _i, _f, _u32, _vp, _vp])
+native.declare("tfy_bias_act_drop_fwd_f32", [_vp, _vp, _vp, _vp, _sz, _i, _i, _f, _u32, _vp, _i, _vp])
 native.declare("tfy_act_drop_bwd_bias", [_vp, _vp, _vp, _vp, _f, _sz, _i, _vp, _vp, _vp, _vp])
 native.declare("tfy_bias_relu_pool_drop_fwd", [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _f, _u32, _vp, _vp])
 native.declare("tfy_pool_drop_relu_bwd", [_vp, _vp, _vp, _f, _i, _i, _i, _i, _vp, _vp, _vp, _vp])
@@ -56,7 +56,7 @@ native.declare("tfy_conv3x3_c32_wgrad_spare_ctas", [_i, _i, _i])
 native.declare("tfy_dense_bwd", [_vp, _vp, _vp, _vp, _vp, _i, _i, _i, _vp])
 native.declare("tfy_gemm_bf16_splitk_fused", [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _f, _u32, _vp, _i,
                                               _vp])
-native.declare("tfy_dense_head_scratch_elems", [_i, _i], restype=ctypes.c_size_t)
+native.declare("tfy_dense_head_scratch_elems", [_i, _i, _i], restype=ctypes.c_size_t)
 native.declare("tfy_dense_head_fused", [_vp, _vp, _vp, _vp, _vp, _f, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i,
                                         _i, _vp])
 
@@ -175,18 +175,15 @@ class FastSequentialEngine(GraphTrainEngine):
         # convolution weight-gradient kernel starts (every layer AFTER that convolution: for the MNIST-CNN the two
         # Dense layers, 98 % of the bytes) can be reduce-scattered / updated / all-gathered by COMMUNICATION CTAs
         # inside that kernel (ops/csrc/tfy_fused_step.cuh: tfy_overlap_role) on the 4 SMs its patch grid leaves
-        # idle, the trailing fused-step launch handling the rest.  Numerically equivalent (GPU test), but measured
-        # on 1 and 2 B200s it does not pay for this model (profiles/r2/overlap_role_r2.md): four SMs move ~8k of the
-        # 75k (N=2) / 19k (N=8) groups per rank inside the 17 us kernel, while the cost of the trailing launch is
-        # the LATENCY chain signal -> in-switch reduce -> store/ack -> signal (12.5 us for 320 parameters, 19.7 us
-        # for all 1.2 M at N=2), which a smaller range does not shorten.  Round 1's variant (a separate kernel on a
-        # side stream) lost for a different reason: no co-residency guarantee + graph fork/join cost.
+        # idle, the trailing fused-step launch handling the rest.  Numerically equivalent (GPU test); off by default
+        # because the cost of the trailing launch is the LATENCY chain signal -> in-switch reduce -> store/ack ->
+        # signal, which a smaller range does not shorten.
         self._overlap = os.environ.get("TFY_OVERLAP", "0") == "1"
         self._ov_used = False
         self._ov_gmid = 0
         self._warned = set()
         self._conv_sync = torch.zeros(1024, dtype=torch.int32, device=dev)     # grid barrier of the wgrad kernel
-        self._c1_acc = torch.zeros(16 * 320, dtype=torch.float32, device=dev)    # first-layer dW/db accumulator
+        self._c1_acc = torch.zeros(160 * 320, dtype=torch.float32, device=dev)   # first-layer dW/db per-CTA partials
         self._c1_cnt = torch.zeros(1, dtype=torch.int32, device=dev)
 
     # ------------------------------------------------------------------ helpers
@@ -204,7 +201,7 @@ class FastSequentialEngine(GraphTrainEngine):
 
     @staticmethod
     def _split_k(M: int, N: int, K: int) -> int:
-        """Split factor of the tcgen05 GEMM for skinny-output / long-K dense layers (1 = use cuBLAS)."""
+        """Split factor of the wgmma GEMM for skinny-output / long-K dense layers (1 = use cuBLAS)."""
         tiles = ((M + 127) // 128) * ((N + 127) // 128)
         k_tiles = (K + 63) // 64
         if K % 8 or tiles > 8 or k_tiles < 32:
@@ -214,7 +211,7 @@ class FastSequentialEngine(GraphTrainEngine):
 
     @staticmethod
     def _tc_conv(st, B: int) -> bool:
-        """True when the stage is served by the tcgen05 implicit-GEMM kernels of ops/csrc/tfy_conv.cu."""
+        """True when the stage is served by the wgmma implicit-GEMM kernels of ops/csrc/tfy_conv.cu."""
         if os.environ.get("TFY_NO_TC_CONV") == "1":       # A/B switch: cuDNN + separate pool kernel instead
             return False
         ly = st.layer
@@ -269,9 +266,9 @@ class FastSequentialEngine(GraphTrainEngine):
         self._loss_in_host[slot] = True
         return self._loss_host[slot].data_ptr()
 
-    def _splitk_acc(self, key, M: int, N: int) -> torch.Tensor:
-        if key not in self._acc32:
-            self._acc32[key] = torch.zeros((M, N), dtype=torch.float32, device=self.device)
+    def _splitk_acc(self, key, slabs: int, M: int, N: int) -> torch.Tensor:
+        if key not in self._acc32 or tuple(self._acc32[key].shape) != (slabs, M, N):
+            self._acc32[key] = torch.zeros((slabs, M, N), dtype=torch.float32, device=self.device)
         return self._acc32[key]
 
     def pop_metrics(self):
@@ -309,7 +306,7 @@ class FastSequentialEngine(GraphTrainEngine):
                 OH, OW = H - 2, W - 2
                 fused_pre = False
                 if self._tc_conv(st, B):
-                    # tcgen05 implicit GEMM; bias + ReLU + 2x2 max-pool + dropout in the epilogue
+                    # wgmma implicit GEMM; bias + ReLU + 2x2 max-pool + dropout in the epilogue
                     xin = cur if (cur.dtype == bf16 and cur.is_contiguous()) else cur.to(bf16).contiguous()
                     p = torch.empty((B, OH // 2, OW // 2, O), dtype=bf16, device=cur.device)
                     code = torch.empty((B, OH // 2, OW // 2, O), dtype=torch.uint8, device=cur.device)
@@ -340,7 +337,7 @@ class FastSequentialEngine(GraphTrainEngine):
                     z = None
                 if z is None:
                     self._warn_once(f"conv_fwd:{li}", f"Conv2D layer {li} ({Cin} -> {O} channels, {H}x{W}, batch {B}) is "
-                                    "outside the tcgen05 convolution kernels' envelope (C_in 32 / C_out 64 with ReLU + 2x2 "
+                                    "outside the wgmma convolution kernels' envelope (C_in 32 / C_out 64 with ReLU + 2x2 "
                                     "pool, or C_in 1): forward and backward use cuDNN")
                     xin = cur.to(bf16) if cur.dtype != bf16 else cur
                     zc = F.conv2d(xin.permute(0, 3, 1, 2), w)       # NCHW logical over NHWC bytes
@@ -385,18 +382,18 @@ class FastSequentialEngine(GraphTrainEngine):
                 split = self._split_k(B, ly.units, K)
                 if split > 1:
                     # skinny GEMM with a long K (e.g. 128 x 128 x 9216): split K over ~48 CTAs of the
-                    # tcgen05 kernel; partial sums meet in an fp32 accumulator that the epilogue clears
-                    acc = self._splitk_acc(li, B, ly.units)
+                    # wgmma kernel; each K-slice stores its fp32 partial in its own slab and the epilogue sums the
+                    # slabs in slice order
+                    acc = self._splitk_acc(li, int(lib.tfy_gemm_bf16_splitk_slabs(K, split)), B, ly.units)
                     z = torch.empty((B, ly.units), dtype=bf16, device=cur.device)
                     tiles = ((B + 127) // 128) * ((ly.units + 127) // 128)
                     co_resident = tiles * split <= torch.cuda.get_device_properties(cur.device).multi_processor_count
                     if co_resident and os.environ.get("TFY_SPLITK_FUSE") == "1":
                         # ONE launch (opt-in): the K-slice CTAs of a tile meet on a counter, then each applies bias +
-                        # ReLU + dropout to 1/split of the tile, writes the bf16 activations and the gate mask and
-                        # clears the accumulator.  (The slices spin on each other: the grid must be co-resident.)
-                        # Measured on B200 (profiles/r2/README.md): 84.9 us/step against 83.0 us for the two-launch
-                        # path below -- the fence + counter + spin costs more than the 3 us second kernel of the same
-                        # CUDA graph it removes, so two launches stay the default.
+                        # ReLU + dropout to 1/split of the tile (summing the slabs in slice order) and writes the bf16
+                        # activations and the gate mask.  (The slices spin on each other: the grid must be co-resident.)
+                        # Off by default: the fence + counter + spin can cost more than the short second kernel of
+                        # the same CUDA graph it removes.
                         key = ("splitk_cnt", li)
                         if key not in self._acc32:
                             self._acc32[key] = torch.zeros(2 * tiles, dtype=torch.int32, device=cur.device)
@@ -412,10 +409,10 @@ class FastSequentialEngine(GraphTrainEngine):
                         self._chk(lib.tfy_bias_act_drop_fwd_f32(acc.data_ptr(), b.data_ptr(), z.data_ptr(),
                                                                 mask.data_ptr() if mask is not None else None, B,
                                                                 ly.units, int(st.relu), float(st.drop), seed, self._hp,
-                                                                s), "bias_act_drop_fwd_f32")
+                                                                acc.shape[0], s), "bias_act_drop_fwd_f32")
                 else:
                     self._warn_once(f"dense_fwd:{li}", f"Dense layer {li} ({K} -> {ly.units}, batch {B}) is outside the "
-                                    "split-K tcgen05 GEMM's envelope (long K, at most 8 output tiles): forward uses cuBLAS")
+                                    "split-K wgmma GEMM's envelope (long K, at most 8 output tiles): forward uses cuBLAS")
                     z = torch.mm(xin, w.t())
                     self._chk(lib.tfy_bias_act_drop_fwd(z.data_ptr(), b.data_ptr(), z.data_ptr(),
                                                         mask.data_ptr() if mask is not None else None, B, ly.units,
@@ -437,9 +434,9 @@ class FastSequentialEngine(GraphTrainEngine):
                     pmask = saved[li - 1][1]
                     pscale = 1.0 / (1.0 - prev.drop) if prev.drop > 0 else 1.0
                     _, pb = self._wb(prev.layer)
-                    if "head_scratch" not in self._acc32:
-                        self._acc32["head_scratch"] = torch.zeros(
-                            int(lib.tfy_dense_head_scratch_elems(K, C)), dtype=torch.float32, device=cur.device)
+                    need = int(lib.tfy_dense_head_scratch_elems(K, C, B))      # one slab per 16 rows of the batch
+                    if "head_scratch" not in self._acc32 or self._acc32["head_scratch"].numel() < need:
+                        self._acc32["head_scratch"] = torch.zeros(need, dtype=torch.float32, device=cur.device)
                         self._acc32["head_counter"] = torch.zeros(1, dtype=torch.int32, device=cur.device)
                     dh = torch.empty((B, K), dtype=bf16, device=cur.device)
                     self._chk(lib.tfy_dense_head_fused(
@@ -494,7 +491,7 @@ class FastSequentialEngine(GraphTrainEngine):
                 if (ly.units % 8 == 0 and I % 8 == 0 and grad.is_contiguous()
                         and xin.is_contiguous() and w.is_contiguous() and w.grad.is_contiguous()
                         and os.environ.get("TFY_NO_TC_DENSE_BWD") != "1"):
-                    # dW = dh^T x (straight into the flat gradient buffer) and dx = dh W in ONE tcgen05 kernel
+                    # dW = dh^T x (straight into the flat gradient buffer) and dx = dh W in ONE wgmma kernel
                     dx = torch.empty((B, I), dtype=bf16, device=grad.device) if not first else None
                     self._chk(lib.tfy_dense_bwd(grad.data_ptr(), xin.data_ptr(), w.data_ptr(), w.grad.data_ptr(),
                                                 dx.data_ptr() if dx is not None else None, B, ly.units, I, s),
@@ -502,7 +499,7 @@ class FastSequentialEngine(GraphTrainEngine):
                     grad = dx
                 else:
                     self._warn_once(f"dense_bwd:{li}", f"Dense layer {li} ({I} -> {ly.units}, batch {B}) is outside "
-                                    "the tcgen05 dense-backward kernel's envelope: cuBLAS computes dW / dx")
+                                    "the wgmma dense-backward kernel's envelope: cuBLAS computes dW / dx")
                     torch.mm(grad.t(), xin, out=w.grad)
                     grad = torch.mm(grad, w) if not first else None
             elif st.kind == "flatten":

@@ -7,7 +7,7 @@ README.md:104-109) plus the blocks of the MNIST-CNN and BERT-base configs.
 Layout: like Keras, image tensors are NHWC at the API (``input_shape=(28, 28,
 1)``).  Internally a 4-D activation is a torch tensor with NCHW *logical*
 shape in ``channels_last`` memory format -- the NHWC bytes untouched -- which
-is the layout cuDNN's bf16 tensor-core kernels want on B200.
+is the layout cuDNN's bf16 tensor-core kernels want on H100.
 """
 from __future__ import annotations
 

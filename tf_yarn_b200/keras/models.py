@@ -576,7 +576,7 @@ class Model:
             v.copy_(w.to(v.dtype))
 
     def _fp32_state(self) -> Dict[str, torch.Tensor]:
-        """Full-precision state dict (fp32 master weights when training on B200 in bf16)."""
+        """Full-precision state dict (fp32 master weights when training on H100 in bf16)."""
         self.build()
         state = {k: v.detach().float().cpu().clone() for k, v in self.net.state_dict().items()}
         if isinstance(self._engine, GraphTrainEngine) and not self._sharded_across_ranks():
@@ -597,7 +597,7 @@ class Model:
         COLLECTIVE (every rank would have to call it), while checkpoints are written by one rank alone -- the
         all-reduce task strips ``ModelCheckpoint`` from every rank but the chief, as the reference does
         (tf_yarn/tensorflow/tasks/gloo_allred_task.py:79-84) -- so single-rank readers use the replicated compute
-        parameters instead (bf16-rounded on B200) and leave the optimizer state out."""
+        parameters instead (bf16-rounded on H100) and leave the optimizer state out."""
         comm = getattr(self._engine, "comm", None)
         return comm is not None and getattr(comm, "world", 1) > 1
 

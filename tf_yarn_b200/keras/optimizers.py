@@ -1,6 +1,6 @@
 """Keras-style optimizer descriptors.
 
-A descriptor only carries hyper-parameters.  On B200 the train engine maps it to
+A descriptor only carries hyper-parameters.  On H100 the train engine maps it to
 the fused K4 kernel (``OptimizerSpec``); on CPU it is instantiated as the
 equivalent ``torch.optim`` optimizer (same update formulas, see
 tests/test_optimizer_math.py).

@@ -3,12 +3,12 @@
 The reference submits a ``skein.ApplicationSpec`` (one ``Service`` per task
 type) to a Java ApplicationMaster that starts one YARN container per task
 instance and hosts the KV store (reference: tf_yarn/client.py:179-269).  On one
-8xB200 box the same contract is met by:
+8xH100 box the same contract is met by:
 
 * one OS process (own session / process group) per task instance, started with
   the task's command line, environment and a private working directory;
 * GPU placement: every ``NodeLabel.GPU`` instance is pinned to
-  ``nb_proc_per_worker`` B200s, handed out round-robin (``TFY_GPU_IDS``);
+  ``nb_proc_per_worker`` H100s, handed out round-robin (``TFY_GPU_IDS``);
 * the KV rendezvous server hosted in the launcher process (``tf_yarn_b200.kv``);
 * per-task log files (the "container logs");
 * an application report with YARN-like ``state`` / ``final_status`` derived from

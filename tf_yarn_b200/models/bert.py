@@ -98,6 +98,6 @@ def synthetic_batch(batch: int, seq_len: int = 128, vocab: int = 30522, seed: in
 
 
 def keras_bert_base(**kwargs):
-    """BERT-base as a mini-Keras model (trains through the B200 graph engine + fused K4 Adam step)."""
+    """BERT-base as a mini-Keras model (trains through the H100 graph engine + fused K4 Adam step)."""
     from tf_yarn_b200 import keras
     return keras.Model.from_torch(BertForPreTraining(**kwargs), name="bert_base")

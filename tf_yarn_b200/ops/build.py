@@ -1,11 +1,11 @@
-"""In-tree native build for tf_yarn_b200 (sm_100a only).
+"""In-tree native build for tf_yarn_b200 (sm_90a only: NVIDIA H100).
 
-Two shared objects are produced next to the sources (they are git-ignored but
-travel to the GPU box with the repo snapshot):
+Two shared objects are produced next to the sources (they are git-ignored and
+rebuilt by ``build_all`` whenever a source or a flag changes):
 
 * ``tf_yarn_b200/ops/lib/libtfy_b200.so`` -- every CUDA kernel + the VMM /
   multicast symmetric-memory runtime (nvcc, ``-gencode
-  arch=compute_100a,code=sm_100a -lineinfo``).
+  arch=compute_90a,code=sm_90a -lineinfo``).
 * ``tf_yarn_b200/kv/libtfy_kv.so`` -- the C++ key-value rendezvous server
   (g++, no CUDA), the stand-in for the skein ApplicationMaster KV store.
 
@@ -33,7 +33,7 @@ KV_DIR = os.path.join(os.path.dirname(HERE), "kv")
 KV_LIB = os.path.join(KV_DIR, "libtfy_kv.so")
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-lineinfo", "-O3", "-std=c++17",
     "--expt-relaxed-constexpr",
     "-Xcompiler", "-fPIC",
@@ -100,7 +100,7 @@ def _compile_one(src: str, verbose: bool) -> str:
     cmd = [_nvcc()] + NVCC_FLAGS + ["-I", CSRC, "-c", src, "-o", tmp_obj]
     if src.endswith(".cpp"):
         cmd = [_nvcc(), "-O2", "-std=c++17", "-Xcompiler", "-fPIC", "-x", "cu",
-               "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo",
+               "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo",
                "-I", CSRC, "-c", src, "-o", tmp_obj]
     res = subprocess.run(cmd, capture_output=True, text=True)
     log = os.path.join(OBJDIR, base + ".log")
@@ -120,7 +120,7 @@ def _compile_one(src: str, verbose: bool) -> str:
 
 
 def build_cuda(verbose: bool = False) -> str:
-    """Compile every ``.cu``/``.cpp`` under ``ops/csrc`` for sm_100a and link them."""
+    """Compile every ``.cu``/``.cpp`` under ``ops/csrc`` for sm_90a and link them."""
     srcs = cuda_sources()
     with _build_lock(os.path.join(LIBDIR, ".build.lock")):
         with concurrent.futures.ThreadPoolExecutor(max_workers=min(8, len(srcs))) as ex:
@@ -158,26 +158,6 @@ def build_kv(verbose: bool = False) -> str:
     return KV_LIB
 
 
-def build_probe(verbose: bool = False) -> str:
-    """Stand-alone tcgen05 operand-fetch probe (tests/gpu/umma_probe.cu -> tests/gpu/umma_probe), run through
-    gpurun: it measures the cycles per MMA of every operand layout and which shared-memory chunks a swizzled
-    descriptor reads.  Returns '' when the source is not there (installed package)."""
-    root = os.path.dirname(os.path.dirname(HERE))
-    src = os.path.join(root, "tests", "gpu", "umma_probe.cu")
-    out = os.path.join(root, "tests", "gpu", "umma_probe")
-    if not os.path.exists(src):
-        return ""
-    if os.path.exists(out) and os.path.getmtime(out) >= os.path.getmtime(src):
-        return out
-    cmd = [_nvcc(), "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O2", "-std=c++17", "-o", out, src]
-    res = subprocess.run(cmd, capture_output=True, text=True)
-    if res.returncode != 0:
-        raise RuntimeError(f"nvcc failed for umma_probe.cu:\n{res.stdout}\n{res.stderr}")
-    if verbose:
-        sys.stderr.write(f"[tf_yarn_b200.build] built {out}\n")
-    return out
-
-
 def build_all(verbose: bool = True, require_cuda: bool = True) -> None:
     """Build everything.  ``require_cuda=False`` (CPU CI): without nvcc only the host-side KV server is built."""
     build_kv(verbose)
@@ -186,7 +166,6 @@ def build_all(verbose: bool = True, require_cuda: bool = True) -> None:
             sys.stderr.write("[tf_yarn_b200.build] nvcc not found: CUDA libraries skipped\n")
         return
     build_cuda(verbose)
-    build_probe(verbose)
 
 
 def sass_dump(out_dir: str) -> None:

@@ -1,4 +1,4 @@
-// Communication kernels over NVLink 5 / NVSwitch peer memory (sm_100a).
+// Communication kernels over NVLink / NVSwitch peer memory (sm_90a).
 //
 //   K1  one-shot all-reduce     every rank reads every peer's buffer (latency-optimal, small)
 //   K2  two-shot all-reduce     P2P reduce-scatter + P2P all-gather in ONE kernel
@@ -256,7 +256,7 @@ int tfy_allreduce(const TfyCommCtx* c, int dtype, int algo, uint64_t off, size_t
     if (block <= 0) block = 512;
     const size_t work = algo == TFY_ALGO_ONESHOT ? n_packs : n_packs / c->world;
     // small messages: one pack per thread (a single NVLink round trip); large ones: 2 CTAs per SM x 4 packs in flight
-    if (grid <= 0) grid = tfy_pick_grid(work, block, 148 * 2);
+    if (grid <= 0) grid = tfy_pick_grid(work, block, TFY_NUM_SMS * 2);
     if (grid > TFY_MAX_BLOCKS) grid = TFY_MAX_BLOCKS;
 #define TFY_AR(T, A) tfy_allreduce_kernel<T, A, 4><<<grid, block, 0, s>>>(*c, off, n_packs, scale, (uint4*)out)
     if (dtype == TFY_BF16) {
@@ -277,7 +277,7 @@ int tfy_broadcast(const TfyCommCtx* c, uint64_t off, size_t nbytes, int root, in
     if (nbytes % 16) return -2;
     const size_t n_packs = nbytes / 16;
     if (block <= 0) block = 512;
-    if (grid <= 0) grid = tfy_pick_grid(n_packs, block * 2, 148);
+    if (grid <= 0) grid = tfy_pick_grid(n_packs, block * 2, TFY_NUM_SMS);
     if (grid > TFY_MAX_BLOCKS) grid = TFY_MAX_BLOCKS;
     if (use_nvls && c->mc_base)
         tfy_broadcast_kernel<TFY_MODE_NVLS><<<grid, block, 0, s>>>(*c, off, n_packs, root);
@@ -290,7 +290,7 @@ int tfy_allgather(const TfyCommCtx* c, uint64_t off, size_t shard_bytes, int gri
     if (shard_bytes % 16) return -2;
     const size_t shard_packs = shard_bytes / 16;
     if (block <= 0) block = 512;
-    if (grid <= 0) grid = tfy_pick_grid(shard_packs, block * 2, 148);
+    if (grid <= 0) grid = tfy_pick_grid(shard_packs, block * 2, TFY_NUM_SMS);
     if (grid > TFY_MAX_BLOCKS) grid = TFY_MAX_BLOCKS;
     tfy_allgather_kernel<<<grid, block, 0, s>>>(*c, off, shard_packs);
     return (int)cudaGetLastError();
@@ -307,7 +307,7 @@ static int tfy_fused_step_groups(const TfyCommCtx* c, int grad_dtype, int param_
     // single GPU: nothing to synchronise with, so oversubscribe the SMs for memory-level parallelism;
     // multi GPU: the cross-GPU barriers are grid-level (one signal per rank pair), 2 groups in flight per thread
     if (grid <= 0) grid = tfy_pick_grid(span_groups + 1, block * (mode == TFY_MODE_LOCAL ? 1 : 2),
-                                        mode == TFY_MODE_LOCAL ? 148 * 6 : 148 * 2);
+                                        mode == TFY_MODE_LOCAL ? TFY_NUM_SMS * 6 : TFY_NUM_SMS * 2);
     if (grid > TFY_MAX_BLOCKS) grid = TFY_MAX_BLOCKS;
 #define TFY_FS4(GT, PT, O, M, U)                                                                                 \
     tfy_launch_pdl_if(tfy_pdl_enabled() || tfy_pdl_k4_enabled(), (tfy_fused_step_kernel<GT, PT, O, M, U>), dim3(grid), dim3(block), 0, s, *c, grad_off, param_off, \

@@ -1,7 +1,7 @@
-// Shared device helpers for the tf_yarn_b200 sm_100a kernels.
+// Shared device helpers for the tf_yarn_b200 sm_90a kernels.
 //
-// Everything in ops/csrc is written for ONE target: Blackwell B200
-// (-gencode arch=compute_100a,code=sm_100a).  There is no fallback path for
+// Everything in ops/csrc is written for ONE target: Hopper H100
+// (-gencode arch=compute_90a,code=sm_90a).  There is no fallback path for
 // other architectures.
 #pragma once
 #include <cuda_runtime.h>
@@ -10,6 +10,7 @@
 #include <stdlib.h>
 #include <string.h>
 
+#define TFY_NUM_SMS 132               // H100 SXM: sizes the grid caps of the streaming kernels
 #define TFY_MAX_RANKS 16
 #define TFY_MAX_BLOCKS 1024            // barrier slots (one per CTA index)
 #define TFY_FLAGS_BYTES (TFY_MAX_BLOCKS * TFY_MAX_RANKS * 4)
@@ -83,10 +84,9 @@ __device__ __forceinline__ void tfy_block_barrier(const TfyCommCtx& c) {
 }
 
 // ---------------------------------------------------------------------------
-// Grid-level cross-GPU barriers (K2/K3/K4).  Measured on 2xB200 (gpurun_out/r2g_comm_sweep_N2.json, launches
-// captured in a CUDA graph): a kernel that only runs tfy_block_barrier costs 3.8 us with 1 CTA but 6.5 / 7.2 us
-// with 16 / 148 CTAs -- every CTA pays its own system-scope release and its own NVLink hop -- and the fused step
-// ran two of them.  What the collectives need is weaker:
+// Grid-level cross-GPU barriers (K2/K3/K4).  A kernel that only runs tfy_block_barrier pays, in every CTA, its
+// own system-scope release and its own NVLink hop, so its cost grows with the grid, and the fused step ran two
+// of them.  What the collectives need is weaker:
 //   entry: "every rank has STARTED this kernel" (its inputs are complete by stream order).  ONE signal per rank
 //          pair, sent by CTA 0; every CTA polls the LOCAL pad.
 //   exit : "every rank's stores have landed".  Each CTA fences its own stores and arrives on a local counter;
@@ -292,11 +292,8 @@ struct TfyPack<float> {
 // serialisation attribute and starts with tfy_pdl_sync(): it lets ITS dependents start launching at once
 // (all our grids are a single wave, so early dependents never take a slot a primary CTA still needs) and
 // then waits for the grids it depends on to complete and flush.  Under stream capture these become
-// programmatic edges of the CUDA graph: launch latency and each kernel's prologue (barrier init, TMEM
-// allocation, tensor-map prefetch) overlap the tail of the previous kernel.  Opt-in (TFY_PDL=1).  On round 1's
-// kernel set it was a wash (103.3 vs 101.5 us per step, profiles/bench_ours_N1_pdl_r1m.json); on the final
-// round-2 step it measures 78.2 vs 84.0 us on one GPU (profiles/r2/README.md), but the GPU test-suite and the
-// multi-GPU runs have not been repeated with it yet, so the default is still off.
+// programmatic edges of the CUDA graph: launch latency and each kernel's prologue (barrier init, tensor-map
+// prefetch) overlap the tail of the previous kernel.  Opt-in (TFY_PDL=1); the default is off.
 // ---------------------------------------------------------------------------------------------
 #ifdef __CUDACC__
 __device__ __forceinline__ void tfy_pdl_sync() {

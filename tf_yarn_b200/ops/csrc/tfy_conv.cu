@@ -1,13 +1,13 @@
-// tcgen05 implicit-GEMM 3x3 convolution kernels (C_in = 32 -> C_out = 64, stride 1, VALID) for sm_100a:
+// Hopper (wgmma) implicit-GEMM 3x3 convolution kernels (C_in = 32 -> C_out = 64, stride 1, VALID) for sm_90a:
 // the second convolution of the MNIST-CNN, forward (fused with bias + ReLU + 2x2 max-pool + dropout),
 // data gradient (fused with the ReLU gate of the previous layer) and weight gradient.
 //
 // Shared-memory operand format (all three kernels).  A work item is an 8 x 8 pixel patch of an image
 // PAIR; TMA stores the (haloed) patch as
 //        [h][image n][w][all channels of the pixel]         one pixel = one 64- or 128-byte row,
-// with the 64B / 128B hardware swizzle.  tests/gpu/umma_probe.cu established that the UMMA operand fetch
-// XORs the 16-byte chunk index with ABSOLUTE shared-memory address bits (base_offset = 0), whatever the
-// descriptor's start address and stride between 8-row groups are.  So a filter tap (kh, kw) is just a
+// with the 64B / 128B hardware swizzle.  The wgmma operand fetch XORs the 16-byte chunk index with ABSOLUTE
+// shared-memory address bits (base_offset = 0), as TMA does when it writes the tile, whatever the descriptor's
+// start address and stride between 8-row groups are.  So a filter tap (kh, kw) is just a
 // different START ADDRESS into the same halo patch (+kh rows, +kw pixels) and the stride between 8-pixel
 // groups is the 10-pixel halo row: the halo is loaded ONCE per patch by ONE TMA and the nine im2col views
 // never materialise, neither in HBM nor in shared memory.  The pixel dimension is GEMM-M for fprop / dgrad
@@ -21,19 +21,16 @@
 // and, read with the MN-major flag, the transposed operand dgrad needs -- no transpose kernel.
 //
 // All three are persistent (one CTA per SM walking the patch list) and warp-specialised: one TMA thread,
-// one MMA thread (elect.sync, so descriptors stay in uniform registers and UTCHMMAs issue back to back),
-// epilogue warps overlapped with the next patch through a double-buffered TMEM accumulator.
+// one MMA warpgroup (wgmma M64 on each 64-row half of the tile, accumulators in registers), epilogue warps
+// overlapped with the next patch through a double-buffered fp32 accumulator tile in shared memory.
 //
-// History, kept because the numbers drove the design (profiles/conv_check_*.json, umma_probe_*.jsonl):
-//   v1  5-D TMA boxes with a 16-byte inner dimension into an un-swizzled layout: one L2 request per
-//       16-byte row at ~3 cycles/row/SM -> 25-33 us per kernel.
-//   v2  cp.async gathers for the same layout: LDGSTS.128 sustains ~14 B/cycle/SM and the first operands
-//       land 5.6 us after launch -> 13-20 us per kernel.
-//   v3  (this file) whole-pixel rows (64/128 B) + swizzle: 200 TMA rows per patch instead of 800-1600.
+// Operand layout: whole-pixel rows (64/128 B) + swizzle, so a patch is 200 TMA rows instead of the
+// 800-1600 16-byte rows of an un-swizzled [pixel][16 B] layout.
 #include <cuda.h>
 
 #include "tfy_common.cuh"
 #include "tfy_fused_step.cuh"
+#include "tfy_wgmma.cuh"
 
 namespace {
 
@@ -50,17 +47,20 @@ constexpr int Z_PATCH_B = 8 * 2 * 8 * Z_PIX_B;         // 16384
 constexpr int W_TAP_B = COUT * A_PIX_B;                // 4096 : [64 o][32 c]
 constexpr int W_BYTES = TAPS * W_TAP_B;                // 36864
 
-constexpr int FP_STAGES = 3, FP_EPI_WARPS = 16, FP_THREADS = (FP_EPI_WARPS + 2) * 32;     // 576
-constexpr size_t FP_SMEM = (size_t)FP_STAGES * A_HALO_PAD + W_BYTES + 1024 + 256;
-constexpr int DG_STAGES = 3, DG_EPI_WARPS = 4, DG_THREADS = (DG_EPI_WARPS + 2 + 4) * 32;  // 320: +4 un-pool producer warps
-constexpr size_t DG_SMEM = (size_t)DG_STAGES * Z_HALO_B + W_BYTES + 1024 + 256;
+// double-buffered fp32 accumulator tiles [2][128 rows][N + 4] (the pad keeps row-per-thread reads conflict-free)
+constexpr int FP_ACC_LD = COUT + 4, DG_ACC_LD = CIN + 4;
+constexpr int FP_STAGES = 3, FP_EPI_WARPS = 16, FP_THREADS = (FP_EPI_WARPS + 4 + 1) * 32;   // 672
+constexpr size_t FP_SMEM = (size_t)FP_STAGES * A_HALO_PAD + W_BYTES + 2 * 128 * FP_ACC_LD * 4 + 1024 + 256;
+constexpr int DG_STAGES = 3, DG_EPI_WARPS = 4, DG_THREADS = (DG_EPI_WARPS + 4 + 1 + 4) * 32;  // 416: +4 un-pool producer warps
+constexpr size_t DG_SMEM = (size_t)DG_STAGES * Z_HALO_B + W_BYTES + 2 * 128 * DG_ACC_LD * 4 + 1024 + 256;
 constexpr int WG_STAGES = 4, WG_STAGE_B = Z_PATCH_B + A_HALO_PAD;                         // 29696
-constexpr int WG_WORK_WARPS = 16, WG_THREADS = (WG_WORK_WARPS + 2) * 32;                   // 576
+constexpr int WG_WORK_WARPS = 16, WG_THREADS = (WG_WORK_WARPS + 4 + 1) * 32;               // 672
 constexpr int WG_OUT = COUT * TAPS * CIN;                                                 // 18432
 constexpr int WG_PART = WG_OUT + COUT;                 // per-CTA partial: dW tile + db (un-pool variant)
-constexpr size_t WG_SMEM = (size_t)WG_STAGES * WG_STAGE_B + 1024 + 512 + WG_WORK_WARPS * COUT * 4;
+constexpr int WG_ACC_B = TAPS * 16 * 128 * 4;          // 9 taps x 64 x 32 fp32 in fragment order [tap][16][128 threads]
+constexpr size_t WG_SMEM = (size_t)WG_STAGES * WG_STAGE_B + 1024 + 512 + WG_WORK_WARPS * COUT * 4 + WG_ACC_B;
 
-constexpr uint32_t SW128 = 2, SW64 = 4;                // UMMA descriptor layout types
+constexpr uint32_t SW128 = TFY_WG_SW128, SW64 = TFY_WG_SW64;
 
 __device__ __forceinline__ uint32_t c_smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 __device__ __forceinline__ void c_mbar_init(uint64_t* bar, uint32_t count) {
@@ -101,60 +101,13 @@ __device__ __forceinline__ void c_tma_3d(const CUtensorMap* map, uint64_t* bar, 
 __device__ __forceinline__ void c_prefetch_map(const CUtensorMap* map) {
     asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(map)) : "memory");
 }
-// Swizzled UMMA shared-memory descriptor (base_offset 0: the swizzle phase comes from the absolute address).
+// Swizzled wgmma shared-memory descriptor (base_offset 0: the swizzle phase comes from the absolute address).
 // sbo = byte distance between consecutive groups of 8 rows (K-major: 8 M/N rows; MN-major: 8 K rows).
 __device__ __forceinline__ uint64_t c_desc(uint32_t smem_addr, uint32_t sbo, uint32_t layout) {
-    uint64_t d = 0;
-    d |= (uint64_t)((smem_addr & 0x3FFFF) >> 4);
-    d |= (uint64_t)(sbo >> 4) << 32;
-    d |= (uint64_t)1 << 46;              // descriptor version (sm_100)
-    d |= (uint64_t)layout << 61;
-    return d;
+    return tfy_wg_desc(smem_addr, 16, sbo, layout);
 }
-// kind::f16 instruction descriptor: D = f32, A = B = bf16
-__device__ __forceinline__ uint32_t c_idesc(uint32_t m, uint32_t n, uint32_t a_mn_major, uint32_t b_mn_major) {
-    return (1u << 4) | (1u << 7) | (1u << 10) | (a_mn_major << 15) | (b_mn_major << 16) | ((n >> 3) << 17) |
-           ((m >> 4) << 24);
-}
-__device__ __forceinline__ void c_umma(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t acc) {
-    asm volatile(
-        "{\n\t"
-        ".reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t"
-        "}" ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(acc)
-        : "memory");
-}
-__device__ __forceinline__ void c_commit(uint64_t* bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(c_smem_u32(bar))
-                 : "memory");
-}
-__device__ __forceinline__ void c_tmem_ld16(uint32_t taddr, uint32_t* r) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-          "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-        : "r"(taddr)
-        : "memory");
-}
-__device__ __forceinline__ void c_tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-template <int COLS>
-__device__ __forceinline__ void c_tmem_alloc(uint32_t* slot) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(c_smem_u32(slot)),
-                 "r"((uint32_t)COLS)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-template <int COLS>
-__device__ __forceinline__ void c_tmem_free(uint32_t base) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(base), "r"((uint32_t)COLS) : "memory");
-}
-__device__ __forceinline__ void c_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void c_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-// One lane of a CONVERGED warp.  Unlike `lane == 0`, the compiler knows the guarded region runs on exactly
-// one thread and keeps descriptor arithmetic + tcgen05.mma operands in uniform registers; with `lane == 0`
-// every UTCHMMA was wrapped in an ELECT / R2UR / BRA.U.ANY loop (~48 cycles per MMA, measured with
-// tests/gpu/umma_probe.cu).
+// One lane of a CONVERGED warp: the compiler knows the guarded region runs on exactly one thread and keeps
+// the TMA operands in uniform registers.
 __device__ __forceinline__ bool c_elect_one() {
     uint32_t pred;
     asm volatile("{\n\t.reg .pred P;\n\telect.sync _|P, 0xffffffff;\n\tselp.b32 %0, 1, 0, P;\n\t}" : "=r"(pred));
@@ -234,7 +187,7 @@ __device__ __forceinline__ void c_unpool_emit(uint8_t* tile, const CUnpoolIn& in
 // ------------------------------------------------------------------------------------------------
 // forward: pooled = dropout(maxpool2x2(relu(conv(a, W) + bias))), code byte per pooled element
 // (bits 0-1 = argmax position dy*2+dx inside the 2x2 window, bit 2 = gradient flows).
-// warps 0..15 epilogue (TMEM quadrant = warp & 3, 16-column slice = warp >> 2), warp 16 MMA, warp 17 TMA
+// warps 0..15 epilogue (row quadrant = warp & 3, 16-column slice = warp >> 2), warps 16..19 MMA, warp 20 TMA
 // ------------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(FP_THREADS, 1)
 tfy_conv3x3_fprop_pool_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_w,
@@ -245,32 +198,28 @@ tfy_conv3x3_fprop_pool_kernel(const __grid_constant__ CUtensorMap map_a, const _
     C_TIMELINE_BEGIN();
     uint8_t* stages = c_align1024(smem_raw);                      // [3][10 h][2 n][10 w][64 B], 64B swizzle
     uint8_t* w_tile = stages + (size_t)FP_STAGES * A_HALO_PAD;    // [9][64 o][64 B], 64B swizzle
-    uint64_t* full = reinterpret_cast<uint64_t*>(w_tile + W_BYTES);
+    float* acc_s = reinterpret_cast<float*>(w_tile + W_BYTES);    // [2][128][FP_ACC_LD]
+    uint64_t* full = reinterpret_cast<uint64_t*>(acc_s + 2 * 128 * FP_ACC_LD);
     uint64_t* empty = full + FP_STAGES;
     uint64_t* tfull = empty + FP_STAGES;
     uint64_t* tempty = tfull + 2;
     uint64_t* wfull = tempty + 2;
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(wfull + 1);
 
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int warp = __shfl_sync(0xffffffffu, (int)threadIdx.x >> 5, 0), lane = threadIdx.x & 31;   // warp-uniform role index
     if (threadIdx.x == 0) {
         c_prefetch_map(&map_a);
         c_prefetch_map(&map_w);
-        for (int s = 0; s < FP_STAGES; ++s) { c_mbar_init(&full[s], 1); c_mbar_init(&empty[s], 1); }
-        for (int b = 0; b < 2; ++b) { c_mbar_init(&tfull[b], 1); c_mbar_init(&tempty[b], FP_EPI_WARPS * 32); }
+        for (int s = 0; s < FP_STAGES; ++s) { c_mbar_init(&full[s], 1); c_mbar_init(&empty[s], 4); }
+        for (int b = 0; b < 2; ++b) { c_mbar_init(&tfull[b], 128); c_mbar_init(&tempty[b], FP_EPI_WARPS * 32); }
         c_mbar_init(wfull, 1);
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
-    if (warp == FP_EPI_WARPS) c_tmem_alloc<128>(tmem_slot);
-    c_fence_before();
     __syncthreads();
-    c_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
     tfy_pdl_sync();                      // upstream grids complete; our dependents may start launching
     if (threadIdx.x == 0) C_MARK(1);
     const int my_patches = ((int)blockIdx.x < n_patches) ? (n_patches - 1 - (int)blockIdx.x) / (int)gridDim.x + 1 : 0;
 
-    if (warp == FP_EPI_WARPS + 1) {
+    if (warp == FP_EPI_WARPS + 4) {
         // ---------------- TMA producer
         if (c_elect_one()) {
             c_mbar_expect_tx(wfull, W_BYTES);
@@ -284,39 +233,44 @@ tfy_conv3x3_fprop_pool_kernel(const __grid_constant__ CUtensorMap map_a, const _
                 if (i == 0) C_MARK(2);
             }
         }
-    } else if (warp == FP_EPI_WARPS) {
-        // ---------------- MMA issuer
-        if (c_elect_one()) {
-            const uint32_t idesc = c_idesc(128, COUT, 0, 0);
-            const uint32_t w0 = c_smem_u32(w_tile);
-            c_mbar_wait(wfull, 0);
-            for (int i = 0; i < my_patches; ++i) {
-                const int s = i % FP_STAGES, b = i & 1;
-                c_mbar_wait(&full[s], (i / FP_STAGES) & 1);
-                if (i == 0) C_MARK(4);
-                if (i >= 2) c_mbar_wait(&tempty[b], ((i >> 1) - 1) & 1);
-                c_fence_after();
-                const uint32_t a0 = c_smem_u32(stages + (size_t)s * A_HALO_PAD);
+    } else if (warp >= FP_EPI_WARPS) {
+        // ---------------- MMA warpgroup: both 64-pixel halves of the patch (8 (h, n) rows of the halo apart)
+        const uint32_t w0 = c_smem_u32(w_tile);
+        c_mbar_wait(wfull, 0);
+        for (int i = 0; i < my_patches; ++i) {
+            const int s = i % FP_STAGES, b = i & 1;
+            c_mbar_wait(&full[s], (i / FP_STAGES) & 1);
+            if (i == 0 && threadIdx.x == FP_EPI_WARPS * 32) C_MARK(4);
+            const uint32_t a0 = c_smem_u32(stages + (size_t)s * A_HALO_PAD);
+            float acc[2][COUT / 2];
+            tfy_wg_fence();
 #pragma unroll 1
-                for (int t = 0; t < TAPS; ++t) {
-                    const int kh = t / 3, kw = t - kh * 3;
+            for (int t = 0; t < TAPS; ++t) {
+                const int kh = t / 3, kw = t - kh * 3;
 #pragma unroll
-                    for (int ks = 0; ks < CIN / 16; ++ks) {
+                for (int ks = 0; ks < CIN / 16; ++ks) {
+                    // B rows = output channels (64 B apart), 8-row groups 512 B apart
+                    const uint64_t bdesc = c_desc(w0 + t * W_TAP_B + ks * 32, 8 * A_PIX_B, SW64);
+#pragma unroll
+                    for (int h = 0; h < 2; ++h) {
                         // A rows = pixels: 8 consecutive w (64 B apart), next group = next (h, n) row of the halo
-                        const uint64_t adesc = c_desc(a0 + kh * 2 * A_ROW_B + kw * A_PIX_B + ks * 32, A_ROW_B, SW64);
-                        // B rows = output channels (64 B apart), 8-row groups 512 B apart
-                        const uint64_t bdesc = c_desc(w0 + t * W_TAP_B + ks * 32, 8 * A_PIX_B, SW64);
-                        c_umma(tmem_base + (uint32_t)(b * COUT), adesc, bdesc, idesc, (t > 0 || ks > 0) ? 1u : 0u);
+                        const uint64_t adesc =
+                            c_desc(a0 + (kh + 4 * h) * 2 * A_ROW_B + kw * A_PIX_B + ks * 32, A_ROW_B, SW64);
+                        tfy_wgmma_m64n64<0, 0>(acc[h], adesc, bdesc, (t > 0 || ks > 0) ? 1u : 0u);
                     }
                 }
-                c_commit(&empty[s]);
-                c_commit(&tfull[b]);
-                if (i == 0) C_MARK(5);
-                if (i == my_patches - 1) C_MARK(11);
             }
+            tfy_wg_commit();
+            tfy_wg_wait<0>();
+            if (lane == 0) c_mbar_arrive(&empty[s]);
+            if (i >= 2) c_mbar_wait(&tempty[b], ((i >> 1) - 1) & 1);
+            tfy_wg_store_rows<COUT>(acc_s + b * 128 * FP_ACC_LD, FP_ACC_LD, acc[0], 0);
+            tfy_wg_store_rows<COUT>(acc_s + b * 128 * FP_ACC_LD, FP_ACC_LD, acc[1], 64);
+            c_mbar_arrive(&tfull[b]);
+            if (threadIdx.x == FP_EPI_WARPS * 32) { if (i == 0) C_MARK(5); if (i == my_patches - 1) C_MARK(11); }
         }
     } else {
-        // ---------------- epilogue: accumulator row r = (h, n, w) = (r/16, (r/8)&1, r%8) lives in TMEM lane r
+        // ---------------- epilogue: accumulator row r = (h, n, w) = (r/16, (r/8)&1, r%8) is row r of the staged tile
         const int quad = warp & 3, cq = warp >> 2;
         const int r = quad * 32 + lane;
         const int h = r >> 4, n = (r >> 3) & 1, w = r & 7;
@@ -339,12 +293,11 @@ tfy_conv3x3_fprop_pool_kernel(const __grid_constant__ CUtensorMap map_a, const _
                 (uint32_t)((((it.bz * 2 + n) * PH + ((it.ty * 8 + h) >> 1)) * PW + ((it.tx * 8 + w) >> 1)) * COUT + col);
             c_mbar_wait(&tfull[b], (i >> 1) & 1);
             if (threadIdx.x == 0) { if (i == 0) C_MARK(6); if (i == my_patches - 1) C_MARK(8); }
-            c_fence_after();
             uint32_t acc[16];
-            c_tmem_ld16(tmem_base + ((uint32_t)(quad * 32) << 16) + (uint32_t)(b * COUT + cq * 16), acc);
-            c_tmem_ld_wait();
-            c_fence_before();
-            c_mbar_arrive(&tempty[b]);                             // the MMA warp may overwrite this buffer now
+            const float* src = acc_s + (size_t)(b * 128 + r) * FP_ACC_LD + cq * 16;
+#pragma unroll
+            for (int j = 0; j < 16; j += 4) *reinterpret_cast<uint4*>(acc + j) = *reinterpret_cast<const uint4*>(src + j);
+            c_mbar_arrive(&tempty[b]);                             // the MMA warps may overwrite this buffer now
             // tag every value with its window position in the 2 low mantissa bits, then reduce-scatter the
             // max over the window (lane ^ 1: other column, lane ^ 16: other row)
             float v[16];
@@ -385,18 +338,16 @@ tfy_conv3x3_fprop_pool_kernel(const __grid_constant__ CUtensorMap map_a, const _
             if (threadIdx.x == 0) { if (i == 0) C_MARK(7); if (i == my_patches - 1) C_MARK(9); }
         }
     }
-    c_fence_before();
     __syncthreads();
-    if (warp == FP_EPI_WARPS) c_tmem_free<128>(tmem_base);
     if (threadIdx.x == 0) C_MARK(10);
 }
 
 // ------------------------------------------------------------------------------------------------
 // data gradient: dx[b, y, x, c] = sum_{kh,kw,o} dz[b, y-kh, x-kw, o] W[o, kh, kw, c], optionally gated by
 // the previous layer's ReLU (gate = that layer's output: dx is zeroed where gate <= 0).
-// dz: [B, H-2, W-2, 64]; dx: [B, H, W, 32].  warps 0..3 epilogue, warp 4 MMA, warp 5 TMA (zero-fills the halo)
+// dz: [B, H-2, W-2, 64]; dx: [B, H, W, 32].  warps 0..3 epilogue, warps 4..7 MMA, warp 8 TMA (zero-fills the halo)
 // ------------------------------------------------------------------------------------------------
-// UNPOOL: the A operand is not loaded from a materialised dz but rebuilt by warps 6..9 from the pooled gradient
+// UNPOOL: the A operand is not loaded from a materialised dz but rebuilt by warps 9..12 from the pooled gradient
 // dp [B, (H-2)/2, (W-2)/2, 64] and the forward kernel's code bytes (c_unpool_task).
 template <bool UNPOOL>
 __global__ void __launch_bounds__(DG_THREADS, 1)
@@ -408,32 +359,28 @@ tfy_conv3x3_dgrad_kernel(const __grid_constant__ CUtensorMap map_dz, const __gri
     C_TIMELINE_BEGIN();
     uint8_t* stages = c_align1024(smem_raw);                      // [3][10 h][2 n][10 w][128 B], 128B swizzle
     uint8_t* w_tile = stages + (size_t)DG_STAGES * Z_HALO_B;      // [9][64 o][64 B], 64B swizzle
-    uint64_t* full = reinterpret_cast<uint64_t*>(w_tile + W_BYTES);
+    float* acc_s = reinterpret_cast<float*>(w_tile + W_BYTES);    // [2][128][DG_ACC_LD]
+    uint64_t* full = reinterpret_cast<uint64_t*>(acc_s + 2 * 128 * DG_ACC_LD);
     uint64_t* empty = full + DG_STAGES;
     uint64_t* tfull = empty + DG_STAGES;
     uint64_t* tempty = tfull + 2;
     uint64_t* wfull = tempty + 2;
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(wfull + 1);
 
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int warp = __shfl_sync(0xffffffffu, (int)threadIdx.x >> 5, 0), lane = threadIdx.x & 31;   // warp-uniform role index
     if (threadIdx.x == 0) {
         if (!UNPOOL) c_prefetch_map(&map_dz);
         c_prefetch_map(&map_w);
-        for (int s = 0; s < DG_STAGES; ++s) { c_mbar_init(&full[s], UNPOOL ? 128 : 1); c_mbar_init(&empty[s], 1); }
-        for (int b = 0; b < 2; ++b) { c_mbar_init(&tfull[b], 1); c_mbar_init(&tempty[b], DG_EPI_WARPS * 32); }
+        for (int s = 0; s < DG_STAGES; ++s) { c_mbar_init(&full[s], UNPOOL ? 128 : 1); c_mbar_init(&empty[s], 4); }
+        for (int b = 0; b < 2; ++b) { c_mbar_init(&tfull[b], 128); c_mbar_init(&tempty[b], DG_EPI_WARPS * 32); }
         c_mbar_init(wfull, 1);
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
-    if (warp == DG_EPI_WARPS) c_tmem_alloc<64>(tmem_slot);
-    c_fence_before();
     __syncthreads();
-    c_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
     tfy_pdl_sync();                      // upstream grids complete; our dependents may start launching
     if (threadIdx.x == 0) C_MARK(1);
     const int my_patches = ((int)blockIdx.x < n_patches) ? (n_patches - 1 - (int)blockIdx.x) / (int)gridDim.x + 1 : 0;
 
-    if (warp == DG_EPI_WARPS + 1) {
+    if (warp == DG_EPI_WARPS + 4) {
         if (c_elect_one()) {
             c_mbar_expect_tx(wfull, W_BYTES);
             c_tma_3d(&map_w, wfull, w_tile, 0, 0, 0);
@@ -447,42 +394,47 @@ tfy_conv3x3_dgrad_kernel(const __grid_constant__ CUtensorMap map_dz, const __gri
                 if (i == 0) C_MARK(2);
             }
         }
-    } else if (warp == DG_EPI_WARPS) {
-        if (c_elect_one()) {
-            const uint32_t idesc = c_idesc(128, CIN, 0, 1);                    // B is MN-major: N = c contiguous
-            const uint32_t w0 = c_smem_u32(w_tile);
-            c_mbar_wait(wfull, 0);
-            for (int i = 0; i < my_patches; ++i) {
-                const int s = i % DG_STAGES, b = i & 1;
-                c_mbar_wait(&full[s], (i / DG_STAGES) & 1);
-                if (UNPOOL) asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-                if (i == 0) C_MARK(4);
-                if (i >= 2) c_mbar_wait(&tempty[b], ((i >> 1) - 1) & 1);
-                c_fence_after();
-                const uint32_t a0 = c_smem_u32(stages + (size_t)s * Z_HALO_B);
+    } else if (warp >= DG_EPI_WARPS && warp < DG_EPI_WARPS + 4) {
+        // ---------------- MMA warpgroup: both 64-pixel halves of the patch (4 h rows of the halo apart)
+        const uint32_t w0 = c_smem_u32(w_tile);
+        c_mbar_wait(wfull, 0);
+        for (int i = 0; i < my_patches; ++i) {
+            const int s = i % DG_STAGES, b = i & 1;
+            c_mbar_wait(&full[s], (i / DG_STAGES) & 1);
+            if (UNPOOL) asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+            if (i == 0 && threadIdx.x == DG_EPI_WARPS * 32) C_MARK(4);
+            const uint32_t a0 = c_smem_u32(stages + (size_t)s * Z_HALO_B);
+            float acc[2][CIN / 2];
+            tfy_wg_fence();
 #pragma unroll 1
-                for (int t = 0; t < TAPS; ++t) {
-                    const int kh = t / 3, kw = t - kh * 3;
+            for (int t = 0; t < TAPS; ++t) {
+                const int kh = t / 3, kw = t - kh * 3;
 #pragma unroll
-                    for (int ks = 0; ks < COUT / 16; ++ks) {
+                for (int ks = 0; ks < COUT / 16; ++ks) {
+                    // W tap [o][32 c]: K = o (rows of 64 B, 8-row groups 512 B apart), N = c inside the row (MN-major)
+                    const uint64_t bdesc = c_desc(w0 + t * W_TAP_B + ks * 16 * A_PIX_B, 8 * A_PIX_B, SW64);
+#pragma unroll
+                    for (int h = 0; h < 2; ++h) {
                         // dz[y-kh, x-kw] sits (2-kh, 2-kw) into the halo patch; rows = pixels of 128 B
-                        const uint64_t adesc =
-                            c_desc(a0 + (2 - kh) * 2 * Z_ROW_B + (2 - kw) * Z_PIX_B + ks * 32, Z_ROW_B, SW128);
-                        // W tap [o][32 c]: K = o (rows of 64 B, 8-row groups 512 B apart), N = c inside the row
-                        const uint64_t bdesc = c_desc(w0 + t * W_TAP_B + ks * 16 * A_PIX_B, 8 * A_PIX_B, SW64);
-                        c_umma(tmem_base + (uint32_t)(b * CIN), adesc, bdesc, idesc, (t > 0 || ks > 0) ? 1u : 0u);
+                        const uint64_t adesc = c_desc(a0 + (2 - kh + 4 * h) * 2 * Z_ROW_B + (2 - kw) * Z_PIX_B + ks * 32,
+                                                      Z_ROW_B, SW128);
+                        tfy_wgmma_m64n32<0, 1>(acc[h], adesc, bdesc, (t > 0 || ks > 0) ? 1u : 0u);
                     }
                 }
-                c_commit(&empty[s]);
-                c_commit(&tfull[b]);
-                if (i == 0) C_MARK(5);
-                if (i == my_patches - 1) C_MARK(11);
             }
+            tfy_wg_commit();
+            tfy_wg_wait<0>();
+            if (lane == 0) c_mbar_arrive(&empty[s]);
+            if (i >= 2) c_mbar_wait(&tempty[b], ((i >> 1) - 1) & 1);
+            tfy_wg_store_rows<CIN>(acc_s + b * 128 * DG_ACC_LD, DG_ACC_LD, acc[0], 0);
+            tfy_wg_store_rows<CIN>(acc_s + b * 128 * DG_ACC_LD, DG_ACC_LD, acc[1], 64);
+            c_mbar_arrive(&tfull[b]);
+            if (threadIdx.x == DG_EPI_WARPS * 32) { if (i == 0) C_MARK(5); if (i == my_patches - 1) C_MARK(11); }
         }
-    } else if (warp > DG_EPI_WARPS + 1) {
+    } else if (warp > DG_EPI_WARPS + 4) {
         // ---------------- un-pool producers (UNPOOL only): 5 x 5 pooled pixels x 2 images x 8 channel groups
         if (UNPOOL) {
-            const int ptid = threadIdx.x - (DG_EPI_WARPS + 2) * 32;           // 0..127
+            const int ptid = threadIdx.x - (DG_EPI_WARPS + 5) * 32;           // 0..127
             const int PH = (H - 2) / 2, PWp = (W - 2) / 2;
             CPatchIter it(tiles_x, tiles_y);
             for (int i = 0; i < my_patches; ++i, it.next()) {
@@ -531,13 +483,10 @@ tfy_conv3x3_dgrad_kernel(const __grid_constant__ CUtensorMap map_dz, const __gri
             }
             c_mbar_wait(&tfull[b], (i >> 1) & 1);
             if (threadIdx.x == 0) { if (i == 0) C_MARK(6); if (i == my_patches - 1) C_MARK(8); }
-            c_fence_after();
             uint32_t acc[2][16];
-            const uint32_t taddr = tmem_base + ((uint32_t)(quad * 32) << 16) + (uint32_t)(b * CIN);
-            c_tmem_ld16(taddr, acc[0]);
-            c_tmem_ld16(taddr + 16, acc[1]);
-            c_tmem_ld_wait();
-            c_fence_before();
+            const float* src = acc_s + (size_t)(b * 128 + r) * DG_ACC_LD;
+#pragma unroll
+            for (int j = 0; j < 32; j += 4) *reinterpret_cast<uint4*>(&acc[j >> 4][j & 15]) = *reinterpret_cast<const uint4*>(src + j);
             c_mbar_arrive(&tempty[b]);
             if (valid) {
                 float v[32];
@@ -557,19 +506,18 @@ tfy_conv3x3_dgrad_kernel(const __grid_constant__ CUtensorMap map_dz, const __gri
             }
         }
     }
-    c_fence_before();
     __syncthreads();
-    if (warp == DG_EPI_WARPS) c_tmem_free<64>(tmem_base);
     if (threadIdx.x == 0) C_MARK(10);
 }
 
 // ------------------------------------------------------------------------------------------------
 // weight gradient: dW[o, t, c] = sum_{b,y,x} dz[b, y, x, o] a[b, y+kh, x+kw, c].  The pixel patches are the
-// GEMM K dimension: every CTA accumulates nine 64x32 tiles in TMEM (one per tap: 288 of the 512 columns)
-// over its share of the patches, stages the fp32 partial tile in shared memory and bulk-copies it to
-// `partials[blockIdx.x]` (L2 resident); after a grid-wide arrive/release it reduces a slice of the 18432
-// outputs over all partials in a fixed order (deterministic, no atomics) and writes bf16 dW.
-// warps 0..15 epilogue + final reduction, warp 16 MMA, warp 17 TMA.
+// GEMM K dimension: every CTA accumulates nine 64x32 tiles (one per tap) over its share of the patches -- each
+// group of staged patches is one wgmma chain per tap in registers, added into fp32 tiles in shared memory --
+// and writes the fp32 partial tile to `partials[blockIdx.x]` (L2 resident); after a grid-wide arrive/release it
+// reduces a slice of the 18432 outputs over all partials in a fixed order (deterministic, no atomics) and writes
+// bf16 dW.
+// warps 0..15 un-pool producers (UNPOOL) + final reduction, warps 16..19 MMA + partial tile, warp 20 TMA.
 // sync: 1024 uint32, zero-initialised once (generation + two levels of arrival counters, see below).
 // ------------------------------------------------------------------------------------------------
 // UNPOOL: dz tiles are rebuilt by warps 0..3 from the pooled gradient dp and the forward kernel's code bytes
@@ -597,29 +545,23 @@ tfy_conv3x3_wgrad_kernel(const __grid_constant__ CUtensorMap map_dz, const __gri
     uint8_t* stages = c_align1024(smem_raw);        // [4] { dz [8 h][2 n][8 w][128 B] sw128 ; a [10 h][2 n][10 w][64 B] sw64 }
     uint64_t* full = reinterpret_cast<uint64_t*>(stages + (size_t)WG_STAGES * WG_STAGE_B);
     uint64_t* empty = full + WG_STAGES;
-    uint64_t* tap_full = empty + WG_STAGES;                         // [9]: accumulator of tap t is final
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tap_full + TAPS);
-    float* s_db = reinterpret_cast<float*>(tmem_slot + 4);          // [16 warps][64] bias-gradient partials (UNPOOL)
+    float* s_db = reinterpret_cast<float*>(empty + WG_STAGES);      // [16 warps][64] bias-gradient partials (UNPOOL)
+    float* acc_s = s_db + WG_WORK_WARPS * COUT;                      // [9 taps][16][128 threads] fp32
 
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int warp = __shfl_sync(0xffffffffu, (int)threadIdx.x >> 5, 0), lane = threadIdx.x & 31;   // warp-uniform role index
     if (threadIdx.x == 0) {
         if (!UNPOOL) c_prefetch_map(&map_dz);
         c_prefetch_map(&map_a);
-        for (int s = 0; s < WG_STAGES; ++s) { c_mbar_init(&full[s], UNPOOL ? 257 : 1); c_mbar_init(&empty[s], 1); }
-        for (int t = 0; t < TAPS; ++t) c_mbar_init(&tap_full[t], 1);
+        for (int s = 0; s < WG_STAGES; ++s) { c_mbar_init(&full[s], UNPOOL ? 257 : 1); c_mbar_init(&empty[s], 4); }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
-    if (warp == WG_WORK_WARPS) c_tmem_alloc<512>(tmem_slot);
-    c_fence_before();
     __syncthreads();
-    c_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
     tfy_pdl_sync();                      // upstream grids complete; our dependents may start launching
     if (threadIdx.x == 0) C_MARK(1);
     const uint32_t gen0 = threadIdx.x == 0 ? *reinterpret_cast<volatile uint32_t*>(sync) : 0u;
     const int my_patches = ((int)blockIdx.x < n_patches) ? (n_patches - 1 - (int)blockIdx.x) / n_cmp + 1 : 0;
 
-    if (warp == WG_WORK_WARPS + 1) {
+    if (warp == WG_WORK_WARPS + 4) {
         if (c_elect_one()) {
             CPatchIter it(tiles_x, tiles_y, n_cmp);
             for (int i = 0; i < my_patches; ++i, it.next()) {
@@ -632,40 +574,59 @@ tfy_conv3x3_wgrad_kernel(const __grid_constant__ CUtensorMap map_dz, const __gri
                 if (i == 0) C_MARK(2);
             }
         }
-    } else if (warp == WG_WORK_WARPS) {
-        if (c_elect_one()) {
-            // Patches are taken WG_STAGES at a time and the taps form the OUTER loop: the accumulator of tap t
-            // is final after the last group's pass over t, so its store overlaps the MMAs of taps t+1..8.
-            const uint32_t idesc = c_idesc(64, CIN, 1, 1);
-            const int n_groups = (my_patches + WG_STAGES - 1) / WG_STAGES;
-            for (int g = 0; g < n_groups; ++g) {
-                const int cnt = min(WG_STAGES, my_patches - g * WG_STAGES);
-                for (int q = 0; q < cnt; ++q) c_mbar_wait(&full[q], g & 1);
-                if (UNPOOL) asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-                if (g == 0) C_MARK(4);
-                c_fence_after();
-                const uint32_t st0 = c_smem_u32(stages);
+    } else if (warp >= WG_WORK_WARPS) {
+        // Patches are taken WG_STAGES at a time; per group and tap, one wgmma chain over the group's pixels in
+        // registers, then added into the tap's fp32 tile (fragment order: thread t owns words [tap][i][t]).
+        const int tid = (int)threadIdx.x - WG_WORK_WARPS * 32;
+        float* mine = acc_s + tid;
+        for (int i = 0; i < TAPS * 16; ++i) mine[i * 128] = 0.f;
+        const int n_groups = (my_patches + WG_STAGES - 1) / WG_STAGES;
+        for (int g = 0; g < n_groups; ++g) {
+            const int cnt = min(WG_STAGES, my_patches - g * WG_STAGES);
+            for (int q = 0; q < cnt; ++q) c_mbar_wait(&full[q], g & 1);
+            if (UNPOOL) asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+            if (g == 0 && tid == 0) C_MARK(4);
+            const uint32_t st0 = c_smem_u32(stages);
 #pragma unroll 1
-                for (int t = 0; t < TAPS; ++t) {
-                    const int kh = t / 3, kw = t - kh * 3;
+            for (int t = 0; t < TAPS; ++t) {
+                const int kh = t / 3, kw = t - kh * 3;
+                float d[16];
+                tfy_wg_fence();
 #pragma unroll 1
-                    for (int q = 0; q < cnt; ++q) {
-                        const uint32_t dz0 = st0 + q * WG_STAGE_B, a0 = dz0 + Z_PATCH_B;
+                for (int q = 0; q < cnt; ++q) {
+                    const uint32_t dz0 = st0 + q * WG_STAGE_B, a0 = dz0 + Z_PATCH_B;
 #pragma unroll
-                        for (int j = 0; j < 8; ++j) {      // 16 pixels (one h row of both images) per MMA
-                            // A = dz^T: M = 64 o inside the 128 B pixel row; K = pixels, 8-pixel groups 1024 B apart
-                            const uint64_t adesc = c_desc(dz0 + j * 2 * 8 * Z_PIX_B, 8 * Z_PIX_B, SW128);
-                            // B = a (tap shifted): N = 32 c inside the 64 B pixel row; K = pixels, groups = (h, n) rows
-                            const uint64_t bdesc = c_desc(a0 + (j + kh) * 2 * A_ROW_B + kw * A_PIX_B, A_ROW_B, SW64);
-                            c_umma(tmem_base + (uint32_t)(t * CIN), adesc, bdesc, idesc, (g > 0 || q > 0 || j > 0) ? 1u : 0u);
-                        }
+                    for (int j = 0; j < 8; ++j) {      // 16 pixels (one h row of both images) per MMA
+                        // A = dz^T: M = 64 o inside the 128 B pixel row; K = pixels, 8-pixel groups 1024 B apart
+                        const uint64_t adesc = c_desc(dz0 + j * 2 * 8 * Z_PIX_B, 8 * Z_PIX_B, SW128);
+                        // B = a (tap shifted): N = 32 c inside the 64 B pixel row; K = pixels, groups = (h, n) rows
+                        const uint64_t bdesc = c_desc(a0 + (j + kh) * 2 * A_ROW_B + kw * A_PIX_B, A_ROW_B, SW64);
+                        tfy_wgmma_m64n32<1, 1>(d, adesc, bdesc, (q > 0 || j > 0) ? 1u : 0u);
                     }
-                    if (g == n_groups - 1) c_commit(&tap_full[t]);
                 }
-                for (int q = 0; q < cnt; ++q) c_commit(&empty[q]);     // stages reusable once these MMAs retire
+                tfy_wg_commit();
+                tfy_wg_wait<0>();
+#pragma unroll
+                for (int i = 0; i < 16; ++i) mine[(t * 16 + i) * 128] += d[i];
             }
-            C_MARK(5);
+            if (lane == 0)
+                for (int q = 0; q < cnt; ++q) c_mbar_arrive(&empty[q]);     // stages reusable
         }
+        if (tid == 0) C_MARK(5);
+        // partial tile rows o = (o, tap) rows of 128 B: value i of this thread is o = 16 w + lane / 4 + 8 ((i / 2) % 2),
+        // c = 8 (i / 4) + 2 (lane % 4) + i % 2
+        float* part = partials + (size_t)blockIdx.x * WG_PART;
+        const int w = tid >> 5;
+#pragma unroll 1
+        for (int t = 0; t < TAPS; ++t) {
+#pragma unroll
+            for (int i = 0; i < 16; i += 2) {
+                const int o = 16 * w + (lane >> 2) + 8 * ((i >> 1) & 1), c = 8 * (i >> 2) + 2 * (lane & 3);
+                __stcg(reinterpret_cast<float2*>(part + (size_t)o * (TAPS * CIN) + t * CIN + c),
+                       make_float2(mine[(t * 16 + i) * 128], mine[(t * 16 + i + 1) * 128]));
+            }
+        }
+        __threadfence();
     } else if (my_patches > 0) {
         if (UNPOOL) {
             // ---------------- un-pool producers (all 16 worker warps): a patch needs 4 x 4 pooled pixels x 2 images
@@ -720,29 +681,6 @@ tfy_conv3x3_wgrad_kernel(const __grid_constant__ CUtensorMap map_dz, const __gri
                 for (int k = 0; k < 8; ++k) s_db[warp * COUT + g * 8 + k] = colacc[k];
             }
         }
-        // M = 64 accumulator: row o lives in TMEM lane (o % 16) + 32 * (o / 16): lanes 0..15 of each quadrant.
-        // warp = (quadrant, tap group): 16 lanes write the 128-byte (o, tap) rows of the fp32 partial tile.
-        const int quad = warp & 3, tg = warp >> 2;                       // taps tg, tg+4, tg+8
-        float* mine = partials + (size_t)blockIdx.x * WG_PART + (size_t)(quad * 16 + (lane & 15)) * (TAPS * CIN);
-#pragma unroll 1
-        for (int t = tg; t < TAPS; t += 4) {
-            c_mbar_wait(&tap_full[t], 0);
-            if (threadIdx.x == 0 && t == 0) C_MARK(6);
-            c_fence_after();
-            uint32_t acc[2][16];
-            const uint32_t taddr = tmem_base + ((uint32_t)(quad * 32) << 16) + (uint32_t)(t * CIN);
-            c_tmem_ld16(taddr, acc[0]);
-            c_tmem_ld16(taddr + 16, acc[1]);
-            c_tmem_ld_wait();
-            if (lane < 16) {
-#pragma unroll
-                for (int j = 0; j < 32; j += 4)
-                    __stcg(reinterpret_cast<float4*>(mine + t * CIN + j),
-                           make_float4(__uint_as_float(acc[j >> 4][j & 15]), __uint_as_float(acc[j >> 4][(j & 15) + 1]),
-                                       __uint_as_float(acc[j >> 4][(j & 15) + 2]),
-                                       __uint_as_float(acc[j >> 4][(j & 15) + 3])));
-            }
-        }
         if (UNPOOL) {
             asm volatile("bar.sync 1, %0;" ::"r"(WG_WORK_WARPS * 32) : "memory");     // all producers added their db
             if (threadIdx.x < COUT) {
@@ -754,9 +692,7 @@ tfy_conv3x3_wgrad_kernel(const __grid_constant__ CUtensorMap map_dz, const __gri
         }
         __threadfence();
     }
-    c_fence_before();
     __syncthreads();
-    if (warp == WG_WORK_WARPS) c_tmem_free<512>(tmem_base);
     if (threadIdx.x == 0) C_MARK(7);
 
     // Grid-wide arrive / release (all CTAs are co-resident: grid <= #SMs, one CTA per SM).  Same-sector atomics
@@ -843,15 +779,15 @@ tfy_conv3x3_wgrad_kernel(const __grid_constant__ CUtensorMap map_dz, const __gri
 //   D[n, o] = sum_pix X~[pix, n] dz[pix, o],   X~[pix, 0..8] = x[pix + tap], X~[pix, 9] = 1 (bias), rest 0
 // M = 64 (n, padded), N = 32 (o), K = pixels.  dz rows (64 B) arrive by TMA exactly as they sit in memory
 // (MN-major B, 64B swizzle); the im2col operand X~ (128-byte rows, 128B swizzle, MN-major A) is built in
-// shared memory by 128 threads from the tiny single-channel input.  Replaces the CUDA-core wgrad kernel
-// (28.8 us) and the separate bias-gradient column sum (8.2 us) of the first layer.
-// warps 0..3 build X~ (warp 0 also runs the epilogue), warp 4 MMA, warp 5 TMA.
-// acc: 16 replicas of 320 floats [n][o] (same-sector atomics serialise, so CTAs spread over replicas), zero on
-// entry, left zero; counter: one uint32, zero on entry, left zero.
+// shared memory by 128 threads from the tiny single-channel input.  Replaces the CUDA-core wgrad kernel and the
+// separate bias-gradient column sum of the first layer.
+// warps 0..3 build X~, warps 4..7 MMA (warp 4, which holds rows 0..15 of D, also runs the epilogue), warp 8 TMA.
+// acc: one partial [10 n][32 o] of 320 floats per CTA (plain stores, no float atomics); the last CTA to finish sums
+// them in CTA order, so dW / db are the same bit for bit on every run.  counter: one uint32, zero on entry, left zero.
 // ------------------------------------------------------------------------------------------------
-constexpr int C1_O = 32, C1_STAGES = 4, C1_PIX = 128, C1_REPLICAS = 16;
+constexpr int C1_O = 32, C1_STAGES = 4, C1_PIX = 128, C1_MAX_CTAS = 160;
 constexpr int C1_A_B = C1_PIX * 128, C1_B_B = C1_PIX * 64, C1_STAGE_B = C1_A_B + C1_B_B;   // 16 KB + 8 KB
-constexpr int C1_THREADS = 192;
+constexpr int C1_THREADS = 288;
 constexpr size_t C1_SMEM = (size_t)C1_STAGES * C1_STAGE_B + 1024 + 256;
 
 template <typename XT>
@@ -866,38 +802,31 @@ tfy_conv3x3_c1_wgrad_tc_kernel(const __grid_constant__ CUtensorMap map_dz, const
     uint64_t* full_a = reinterpret_cast<uint64_t*>(stages + (size_t)C1_STAGES * C1_STAGE_B);
     uint64_t* full_b = full_a + C1_STAGES;
     uint64_t* empty = full_b + C1_STAGES;
-    uint64_t* tmem_full = empty + C1_STAGES;
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tmem_full + 1);
     __shared__ uint32_t s_last;
 
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int warp = __shfl_sync(0xffffffffu, (int)threadIdx.x >> 5, 0), lane = threadIdx.x & 31;   // warp-uniform role index
     if (threadIdx.x == 0) {
         c_prefetch_map(&map_dz);
         for (int s = 0; s < C1_STAGES; ++s) {
             c_mbar_init(&full_a[s], 128);
             c_mbar_init(&full_b[s], 1);
-            c_mbar_init(&empty[s], 1);
+            c_mbar_init(&empty[s], 4);
         }
-        c_mbar_init(tmem_full, 1);
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
-    if (warp == 4) c_tmem_alloc<32>(tmem_slot);
     // the padding columns of X~ (n >= 16) stay zero for the whole kernel
     for (int i = threadIdx.x; i < C1_STAGES * C1_A_B / 16; i += C1_THREADS) {
         const int s = i / (C1_A_B / 16), r = i - s * (C1_A_B / 16);
         *reinterpret_cast<uint4*>(stages + (size_t)s * C1_STAGE_B + (size_t)r * 16) = make_uint4(0, 0, 0, 0);
     }
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-    c_fence_before();
     __syncthreads();
-    c_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
     tfy_pdl_sync();                      // upstream grids complete; our dependents may start launching
     if (threadIdx.x == 0) C_MARK(1);
     const int my_chunks = ((int)blockIdx.x < n_chunks) ? (n_chunks - 1 - (int)blockIdx.x) / (int)gridDim.x + 1 : 0;
     const int OH = H - 2, OW = W - 2;
 
-    if (warp == 5) {
+    if (warp == 8) {
         if (c_elect_one()) {
             for (int i = 0; i < my_chunks; ++i) {
                 const int s = i % C1_STAGES;
@@ -911,27 +840,39 @@ tfy_conv3x3_c1_wgrad_tc_kernel(const __grid_constant__ CUtensorMap map_dz, const
                     : "memory");
             }
         }
-    } else if (warp == 4) {
-        if (c_elect_one()) {
-            const uint32_t idesc = c_idesc(64, C1_O, 1, 1);
-            for (int i = 0; i < my_chunks; ++i) {
-                const int s = i % C1_STAGES;
-                c_mbar_wait(&full_a[s], (i / C1_STAGES) & 1);
-                c_mbar_wait(&full_b[s], (i / C1_STAGES) & 1);
-                if (i == 0) C_MARK(4);
-                c_fence_after();
-                const uint32_t a0 = c_smem_u32(stages + (size_t)s * C1_STAGE_B), b0 = a0 + C1_A_B;
+    } else if (warp >= 4) {
+        float d[16];
+        tfy_wg_zero<C1_O>(d);
+        for (int i = 0; i < my_chunks; ++i) {
+            const int s = i % C1_STAGES;
+            c_mbar_wait(&full_a[s], (i / C1_STAGES) & 1);
+            c_mbar_wait(&full_b[s], (i / C1_STAGES) & 1);
+            if (i == 0 && threadIdx.x == 128) C_MARK(4);
+            const uint32_t a0 = c_smem_u32(stages + (size_t)s * C1_STAGE_B), b0 = a0 + C1_A_B;
+            tfy_wg_fence();
 #pragma unroll
-                for (int j = 0; j < C1_PIX / 16; ++j) {
-                    // A = X~^T: M = 64 n inside the 128 B pixel row; B = dz: N = 32 o inside the 64 B pixel row
-                    const uint64_t adesc = c_desc(a0 + j * 16 * 128, 8 * 128, SW128);
-                    const uint64_t bdesc = c_desc(b0 + j * 16 * 64, 8 * 64, SW64);
-                    c_umma(tmem_base, adesc, bdesc, idesc, (i > 0 || j > 0) ? 1u : 0u);
-                }
-                c_commit(&empty[s]);
+            for (int j = 0; j < C1_PIX / 16; ++j) {
+                // A = X~^T: M = 64 n inside the 128 B pixel row; B = dz: N = 32 o inside the 64 B pixel row
+                const uint64_t adesc = c_desc(a0 + j * 16 * 128, 8 * 128, SW128);
+                const uint64_t bdesc = c_desc(b0 + j * 16 * 64, 8 * 64, SW64);
+                tfy_wgmma_m64n32<1, 1>(d, adesc, bdesc, 1u);
             }
-            c_commit(tmem_full);
-            C_MARK(5);
+            tfy_wg_commit();
+            tfy_wg_wait<0>();
+            if (lane == 0) c_mbar_arrive(&empty[s]);
+        }
+        if (threadIdx.x == 128) C_MARK(5);
+        if (warp == 4) {
+            // D rows 0..8 = taps, row 9 = bias; value i of this thread: row lane / 4 + 8 ((i / 2) % 2),
+            // column 8 (i / 4) + 2 (lane % 4) + i % 2
+            float* part = acc + (size_t)blockIdx.x * (10 * C1_O);
+#pragma unroll
+            for (int i = 0; i < 16; ++i) {
+                const int n = (lane >> 2) + 8 * ((i >> 1) & 1), o = 8 * (i >> 2) + 2 * (lane & 3) + (i & 1);
+                if (n < 10) __stcg(part + n * C1_O + o, d[i]);
+            }
+            __threadfence();
+            if (lane == 0) C_MARK(7);
         }
     } else {
         // ---------------- im2col builders: one pixel per thread per chunk; the next chunk's inputs are gathered
@@ -969,31 +910,9 @@ tfy_conv3x3_c1_wgrad_tc_kernel(const __grid_constant__ CUtensorMap map_dz, const
             c_mbar_arrive(&full_a[s]);
             if (threadIdx.x == 0) { if (i == 0) C_MARK(2); if (i == my_chunks - 1) C_MARK(3); }
         }
-        if (warp == 0 && my_chunks > 0) {
-            // D row n lives in TMEM lane n (n < 16 -> quadrant 0); lanes 0..8 = taps, lane 9 = bias
-            c_mbar_wait(tmem_full, 0);
-            if (threadIdx.x == 0) C_MARK(6);
-            c_fence_after();
-            uint32_t d[2][16];
-            c_tmem_ld16(tmem_base, d[0]);
-            c_tmem_ld16(tmem_base + 16, d[1]);
-            c_tmem_ld_wait();
-            if (lane < 10) {
-#pragma unroll
-                for (int o = 0; o < C1_O; ++o)
-                    asm volatile("red.global.add.f32 [%0], %1;" ::"l"(acc + (blockIdx.x % C1_REPLICAS) * (10 * C1_O) +
-                                                                        lane * C1_O + o),
-                                 "f"(__uint_as_float(d[o >> 4][o & 15]))
-                                 : "memory");
-            }
-            __threadfence();
-            if (threadIdx.x == 0) C_MARK(7);
-        }
     }
-    c_fence_before();
     __syncthreads();
-    if (warp == 4) c_tmem_free<32>(tmem_base);
-    // the last CTA to finish converts the sums and clears the accumulator for the next step
+    // the last CTA to finish sums the per-CTA partials in CTA order and converts them
     if (threadIdx.x == 0) {
         __threadfence();
         s_last = (atomicAdd(counter, 1u) == gridDim.x - 1) ? 1u : 0u;
@@ -1002,16 +921,34 @@ tfy_conv3x3_c1_wgrad_tc_kernel(const __grid_constant__ CUtensorMap map_dz, const
     if (threadIdx.x == 0) C_MARK(8);
     if (s_last) {
         __threadfence();
-        for (int i = threadIdx.x; i < 10 * C1_O; i += C1_THREADS) {
-            const int n = i / C1_O, o = i - n * C1_O;
-            float val = 0.f;
-#pragma unroll
-            for (int rep = 0; rep < C1_REPLICAS; ++rep) {
-                val += __ldcg(acc + rep * (10 * C1_O) + i);
-                __stcg(acc + rep * (10 * C1_O) + i, 0.f);
+        // PARTS thread groups each sum every PARTS-th partial (float4 columns), then the groups are added in order
+        constexpr int F4 = 10 * C1_O / 4, PARTS = C1_THREADS / F4;
+        __shared__ float4 s_part[PARTS * F4];
+        const int f = (int)threadIdx.x % F4, part = (int)threadIdx.x / F4;
+        if (part < PARTS) {
+            float4 a = make_float4(0.f, 0.f, 0.f, 0.f);
+            const float4* src = reinterpret_cast<const float4*>(acc);
+#pragma unroll 8
+            for (int g = part; g < (int)gridDim.x; g += PARTS) {
+                const float4 v = __ldcg(src + (size_t)g * F4 + f);
+                a.x += v.x; a.y += v.y; a.z += v.z; a.w += v.w;
             }
-            if (n < 9) dw[o * 9 + n] = __float2bfloat16(val);
-            else dbias[o] = __float2bfloat16(val);
+            s_part[part * F4 + f] = a;
+        }
+        __syncthreads();
+        if ((int)threadIdx.x < F4) {
+            float4 a = s_part[f];
+            for (int q = 1; q < PARTS; ++q) {
+                const float4 v = s_part[q * F4 + f];
+                a.x += v.x; a.y += v.y; a.z += v.z; a.w += v.w;
+            }
+            const float vals[4] = {a.x, a.y, a.z, a.w};
+#pragma unroll
+            for (int e = 0; e < 4; ++e) {
+                const int i = f * 4 + e, n = i / C1_O, o = i - n * C1_O;
+                if (n < 9) dw[o * 9 + n] = __float2bfloat16(vals[e]);
+                else dbias[o] = __float2bfloat16(vals[e]);
+            }
         }
         if (threadIdx.x == 0) *counter = 0u;
     }
@@ -1021,24 +958,19 @@ tfy_conv3x3_c1_wgrad_tc_kernel(const __grid_constant__ CUtensorMap map_dz, const
 // ------------------------------------------------------------------------------------------------
 // First-layer forward (C_in = 1, 32 filters) on the tensor core:
 //   y[pix, o] = relu( sum_k X~[pix, k] W~[o, k] ),  X~[pix, 0..8] = x[pix + tap], X~[pix, 9] = 1,  W~[o, 9] = bias[o]
-// One M128 N32 K16 tcgen05.mma per 128 pixels; both operands are built in shared memory in the un-swizzled
-// K-major core-matrix layout ([k half][row][16 B]: lbo = distance between the halves, sbo = 128).  The CUDA-core
-// version spent its time on 288 shared-memory weight loads + FMAs per pixel; here a thread gathers 9 inputs,
-// stores 2 x 16 B, and later packs 32 accumulator columns.
-// warps 0..3 build X~, warps 4..7 epilogue (TMEM quadrant = warp & 3), warp 8 MMA.
+// Two wgmma M64 N32 K16 per 128 pixels; both operands are built in shared memory in the un-swizzled K-major
+// core-matrix layout ([k half][row][16 B]: lbo = distance between the halves, sbo = 128).  The CUDA-core
+// version spends its time on 288 shared-memory weight loads + FMAs per pixel; here a thread gathers 9 inputs and
+// stores 2 x 16 B, and the MMA warpgroup writes ReLU'd bf16 pairs straight from its accumulator registers.
+// warps 0..3 build X~, warps 4..7 MMA + epilogue.
 // ------------------------------------------------------------------------------------------------
 constexpr int F1_STAGES = 4, F1_PIX = 128, F1_A_B = 2 * F1_PIX * 16;      // 4 KB per stage
 constexpr int F1_W_B = 2 * C1_O * 16;                                     // 1 KB
-constexpr int F1_THREADS = 9 * 32;
+constexpr int F1_THREADS = 8 * 32;
 constexpr size_t F1_SMEM = (size_t)F1_STAGES * F1_A_B + F1_W_B + 128 + 256;
 
 __device__ __forceinline__ uint64_t c_desc_nosw(uint32_t smem_addr, uint32_t lbo, uint32_t sbo) {
-    uint64_t d = 0;
-    d |= (uint64_t)((smem_addr & 0x3FFFF) >> 4);
-    d |= (uint64_t)(lbo >> 4) << 16;
-    d |= (uint64_t)(sbo >> 4) << 32;
-    d |= (uint64_t)1 << 46;
-    return d;
+    return tfy_wg_desc(smem_addr, lbo, sbo, TFY_WG_NOSWIZZLE);
 }
 
 template <typename XT>
@@ -1051,17 +983,12 @@ tfy_conv3x3_c1_fwd_tc_kernel(const XT* __restrict__ x, const __nv_bfloat16* __re
     uint8_t* w_tile = stages + (size_t)F1_STAGES * F1_A_B;          // [2 k halves][32 o][16 B]
     uint64_t* full = reinterpret_cast<uint64_t*>(w_tile + F1_W_B);
     uint64_t* empty = full + F1_STAGES;
-    uint64_t* tfull = empty + F1_STAGES;
-    uint64_t* tempty = tfull + 2;
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tempty + 2);
 
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int warp = __shfl_sync(0xffffffffu, (int)threadIdx.x >> 5, 0), lane = threadIdx.x & 31;   // warp-uniform role index
     if (threadIdx.x == 0) {
-        for (int s = 0; s < F1_STAGES; ++s) { c_mbar_init(&full[s], 128); c_mbar_init(&empty[s], 1); }
-        for (int b = 0; b < 2; ++b) { c_mbar_init(&tfull[b], 1); c_mbar_init(&tempty[b], 128); }
+        for (int s = 0; s < F1_STAGES; ++s) { c_mbar_init(&full[s], 128); c_mbar_init(&empty[s], 4); }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
-    if (warp == 8) c_tmem_alloc<64>(tmem_slot);
     tfy_pdl_sync();                      // (the weights below are produced by the previous step's optimizer kernel)
     if (threadIdx.x < C1_O) {
         // W~ row o: taps 0..7 | tap 8, bias, 0 x 6
@@ -1075,30 +1002,41 @@ tfy_conv3x3_c1_fwd_tc_kernel(const XT* __restrict__ x, const __nv_bfloat16* __re
         *reinterpret_cast<uint4*>(w_tile + C1_O * 16 + o * 16) = TfyPack<__nv_bfloat16>::pack(k1);
     }
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-    c_fence_before();
     __syncthreads();
-    c_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
     const int my_chunks = ((int)blockIdx.x < n_chunks) ? (n_chunks - 1 - (int)blockIdx.x) / (int)gridDim.x + 1 : 0;
     const int OH = H - 2, OW = W - 2;
 
-    if (warp == 8) {
-        if (c_elect_one()) {
-            const uint32_t idesc = c_idesc(128, C1_O, 0, 0);
-            const uint64_t bdesc = c_desc_nosw(c_smem_u32(w_tile), C1_O * 16, 128);
-            for (int i = 0; i < my_chunks; ++i) {
-                const int s = i % F1_STAGES, b = i & 1;
-                c_mbar_wait(&full[s], (i / F1_STAGES) & 1);
-                asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-                if (i >= 2) c_mbar_wait(&tempty[b], ((i >> 1) - 1) & 1);
-                c_fence_after();
-                const uint64_t adesc = c_desc_nosw(c_smem_u32(stages + (size_t)s * F1_A_B), F1_PIX * 16, 128);
-                c_umma(tmem_base + (uint32_t)(b * C1_O), adesc, bdesc, idesc, 0u);
-                c_commit(&empty[s]);
-                c_commit(&tfull[b]);
+    if (warp >= 4) {
+        const uint64_t bdesc = c_desc_nosw(c_smem_u32(w_tile), C1_O * 16, 128);
+        const int w = warp & 3;
+        for (int i = 0; i < my_chunks; ++i) {
+            const int s = i % F1_STAGES;
+            const int chunk = (int)blockIdx.x + i * (int)gridDim.x;
+            c_mbar_wait(&full[s], (i / F1_STAGES) & 1);
+            asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+            float acc[2][C1_O / 2];
+            tfy_wg_fence();
+#pragma unroll
+            for (int h = 0; h < 2; ++h)       // pixels [64 h, 64 h + 64): 8 core-matrix rows of 128 B further
+                tfy_wgmma_m64n32<0, 0>(acc[h], c_desc_nosw(c_smem_u32(stages + (size_t)s * F1_A_B + h * 64 * 16),
+                                                           F1_PIX * 16, 128), bdesc, 0u);
+            tfy_wg_commit();
+            tfy_wg_wait<0>();
+            if (lane == 0) c_mbar_arrive(&empty[s]);
+            // value i of this thread: pixel row 64 h + 16 w + lane / 4 + 8 ((i / 2) % 2), channel 8 (i / 4) + 2 (lane % 4)
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+#pragma unroll
+                for (int i2 = 0; i2 < C1_O / 2; i2 += 2) {
+                    const int p = chunk * F1_PIX + 64 * h + 16 * w + (lane >> 2) + 8 * ((i2 >> 1) & 1);
+                    const int o = 8 * (i2 >> 2) + 2 * (lane & 3);
+                    if (p < n_pix)
+                        *reinterpret_cast<__nv_bfloat162*>(y + (size_t)p * C1_O + o) =
+                            __floats2bfloat162_rn(fmaxf(acc[h][i2], 0.f), fmaxf(acc[h][i2 + 1], 0.f));
+                }
             }
         }
-    } else if (warp < 4) {
+    } else {
         // ---------------- im2col builders: one pixel per thread per chunk; the next chunk's inputs are loaded
         // before this chunk's stage is waited for
         const int r = threadIdx.x;
@@ -1132,36 +1070,7 @@ tfy_conv3x3_c1_fwd_tc_kernel(const XT* __restrict__ x, const __nv_bfloat16* __re
             asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
             c_mbar_arrive(&full[s]);
         }
-    } else {
-        // ---------------- epilogue: accumulator row = pixel of the chunk; ReLU, bf16, 64 contiguous bytes
-        const int quad = warp & 3;
-        const int r = quad * 32 + lane;
-        for (int i = 0; i < my_chunks; ++i) {
-            const int b = i & 1;
-            const int chunk = (int)blockIdx.x + i * (int)gridDim.x;
-            c_mbar_wait(&tfull[b], (i >> 1) & 1);
-            c_fence_after();
-            uint32_t acc[2][16];
-            const uint32_t taddr = tmem_base + ((uint32_t)(quad * 32) << 16) + (uint32_t)(b * C1_O);
-            c_tmem_ld16(taddr, acc[0]);
-            c_tmem_ld16(taddr + 16, acc[1]);
-            c_tmem_ld_wait();
-            c_fence_before();
-            c_mbar_arrive(&tempty[b]);
-            const int p = chunk * F1_PIX + r;
-            if (p < n_pix) {
-                float o[32];
-#pragma unroll
-                for (int j = 0; j < 32; ++j) o[j] = fmaxf(__uint_as_float(acc[j >> 4][j & 15]), 0.f);
-                __nv_bfloat16* yp = y + (size_t)p * C1_O;
-#pragma unroll
-                for (int j = 0; j < 32; j += 8) tfy_st16(yp + j, TfyPack<__nv_bfloat16>::pack(o + j));
-            }
-        }
     }
-    c_fence_before();
-    __syncthreads();
-    if (warp == 8) c_tmem_free<64>(tmem_base);
 }
 
 namespace {
@@ -1301,9 +1210,9 @@ int tfy_conv3x3_c32_dgrad_unpool(const void* dp, const void* code, float scale, 
 
 // also writes db [64] = sum over batch and positions of the gated pooled gradient.
 // ov (optional): a fused gradient-exchange/optimizer step to run on SPARE SMs next to the weight gradient
-// (tfy_overlap_role).  ov->n_cta is clamped to the SMs the compute grid leaves free (576 patches -> 144 compute
-// CTAs on a 148-SM B200 -> 4 communication CTAs); tfy_conv3x3_c32_wgrad_spare_ctas() tells the caller how many
-// that is so that it can size the overlapped range.
+// (tfy_overlap_role).  ov->n_cta is clamped to the SMs the compute grid leaves free (576 patches -> 116 compute
+// CTAs of 5 patches on a 132-SM H100 -> up to 16 communication CTAs); tfy_conv3x3_c32_wgrad_spare_ctas() tells
+// the caller how many that is so that it can size the overlapped range.
 int tfy_conv3x3_c32_wgrad_unpool_ov(const void* a, const void* dp, const void* code, float scale, float* partials,
                                     void* dw, void* db, uint32_t* sync, int B, int H, int W, const TfyOverlapStep* ov,
                                     cudaStream_t s) {
@@ -1359,11 +1268,11 @@ int tfy_conv3x3_c1_fwd_tc(const void* x, int x_is_f32, const void* w, const void
 }
 
 // First-layer (C_in = 1, 32 filters) weight + bias gradient.  x: [B, H, W, 1] fp32 or bf16, dz: [B, H-2, W-2, 32] bf16
-// (already gated by the layer's ReLU), dw: [32, 3, 3, 1] bf16, dbias: [32] bf16.  acc: 16 x 320 floats and counter:
-// one uint32, both zero on entry (and left zero).
+// (already gated by the layer's ReLU), dw: [32, 3, 3, 1] bf16, dbias: [32] bf16.  acc: 160 x 320 floats of scratch
+// (one partial per CTA) and counter: one uint32, zero on entry (and left zero).
 int tfy_conv3x3_c1_wgrad_tc(const void* x, int x_is_f32, const void* dz, float* acc, uint32_t* counter, void* dw,
                             void* dbias, int B, int H, int W, cudaStream_t s) {
-    if (!c_init()) return -4;
+    if (!c_init() || c_sms > C1_MAX_CTAS) return -4;
     static bool attr = false;
     if (!attr) {
         if (cudaFuncSetAttribute(tfy_conv3x3_c1_wgrad_tc_kernel<float>, cudaFuncAttributeMaxDynamicSharedMemorySize,

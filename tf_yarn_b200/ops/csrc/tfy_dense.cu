@@ -1,4 +1,4 @@
-// Dense-layer backward on tcgen05 (sm_100a): BOTH products of a Linear layer's backward in one kernel.
+// Dense-layer backward on the Hopper tensor core (sm_90a): BOTH products of a Linear layer's backward in one kernel.
 //
 //   dW[u, i] = sum_b dh[b, u] * x[b, i]        (M = units, N = in-features, K = batch)
 //   dx[b, i] = sum_u dh[b, u] * W[u, i]        (M = batch, N = in-features, K = units)
@@ -6,33 +6,39 @@
 // for the skinny-batch / wide-input layers of the mini-Keras fast path (the MNIST-CNN's 9216 -> 128 layer:
 // batch <= 128, units <= 128, in-features = 9216).  The two GEMMs share the dh operand, have the same
 // output width and a tiny K, so ONE CTA per 64-column slice of the in-features does both: dh (32 KB) and the
-// slice's x and W tiles (16 KB each) arrive by TMA, sixteen tcgen05.mma (M128 N64 K16) fill two TMEM accumulators,
-// and the epilogue warps convert them to bf16 in shared memory and hand them to TMA stores (dW straight into
-// the flat gradient buffer the fused optimizer/collective step consumes).  No operand is transposed in memory:
-// the SAME shared-memory bytes of dh serve as the K-major A operand of dx and, through a second descriptor with
-// the MN-major flag, as the transposed A operand of dW; x and W tiles are MN-major B operands as they sit in
-// memory (in-features contiguous).  This replaces two cuBLAS GEMM launches of the round-1 step
+// slice's x and W tiles (16 KB each) arrive by TMA, one warpgroup per product issues wgmma M64 N64 K16 on both
+// 64-row halves of its 128-row accumulator, and converts it to bf16 in shared memory for a TMA store (dW straight
+// into the flat gradient buffer the fused optimizer/collective step consumes).  No operand is transposed in
+// memory: the SAME shared-memory bytes of dh serve as the K-major A operand of dx and, through the transpose flag
+// of the wgmma, as the MN-major A operand of dW; x and W tiles are MN-major B operands as they sit in memory
+// (in-features contiguous).  This replaces two cuBLAS GEMM launches of the round-1 step
 // (reference path being replaced: the Dense backward of the Keras/Horovod worker, tf_yarn/tensorflow/tasks/
 // gloo_allred_task.py:54 running TensorFlow's MatMul gradients).
 //
-// warp 0: TMA loads   warp 1: TMEM allocation + MMA issue   warps 2-5: dW epilogue   warps 6-9: dx epilogue
+// warps 0-3: dW wgmma + epilogue   warps 4-7: dx wgmma + epilogue   warp 8: TMA loads
 #include <cuda.h>
 
 #include "tfy_common.cuh"
+#include "tfy_wgmma.cuh"
 
 namespace {
 
 constexpr int DB_M = 128;             // MMA M: units (dW) / batch (dx), zero-filled by TMA beyond the real extent
 constexpr int DB_N = 64;              // in-features per CTA = one 128-byte swizzle atom of bf16
 constexpr int DB_K = 128;             // batch (dW) / units (dx)
-constexpr int DB_THREADS = 320;
+constexpr int DB_THREADS = 288;
 constexpr int DH_BYTES = DB_M * 128 * 2;          // two 64-column boxes of 128 rows x 128 B
 constexpr int TILE_BYTES = 128 * 128;             // 128 rows x 64 bf16
-constexpr size_t DB_SMEM = 1024 + DH_BYTES + 2 * TILE_BYTES /*x, w*/ + 2 * TILE_BYTES /*staging*/ + 256;
+constexpr int ACC_LD = DB_N + 4;                  // fp32 row pitch of a staged accumulator
+constexpr int ACC_BYTES = DB_M * ACC_LD * 4;
+constexpr size_t DB_SMEM = 1024 + DH_BYTES + 2 * TILE_BYTES /*x, w*/ + 2 * TILE_BYTES /*staging*/ + 2 * ACC_BYTES + 256;
 
 __device__ __forceinline__ uint32_t d_smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 __device__ __forceinline__ void d_mbar_init(uint64_t* bar, uint32_t count) {
     asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(d_smem_u32(bar)), "r"(count) : "memory");
+}
+__device__ __forceinline__ void d_mbar_arrive(uint64_t* bar) {
+    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(d_smem_u32(bar)) : "memory");
 }
 __device__ __forceinline__ void d_mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
     asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(d_smem_u32(bar)), "r"(bytes) : "memory");
@@ -64,43 +70,52 @@ __device__ __forceinline__ bool d_elect_one() {
     asm volatile("{\n\t.reg .pred P;\n\telect.sync _|P, 0xffffffff;\n\tselp.b32 %0, 1, 0, P;\n\t}" : "=r"(pred));
     return pred != 0;
 }
-// Swizzled (128 B) UMMA shared-memory descriptor.
-//   K-major : rows = M/N index (128 B each = 64 K-elements), sbo = 8 rows.  lbo unused (one atom along K per MMA).
-//   MN-major: rows = K index (128 B each = 64 MN-elements), sbo = 8 K-rows, lbo = distance between consecutive
-//             64-element atoms along MN (needed when M = 128 spans two atoms).
-__device__ __forceinline__ uint64_t d_desc(uint32_t smem_addr, uint32_t lbo, uint32_t sbo) {
-    uint64_t d = 0;
-    d |= (uint64_t)((smem_addr & 0x3FFFF) >> 4);
-    d |= (uint64_t)((lbo >> 4) & 0x3FFF) << 16;
-    d |= (uint64_t)((sbo >> 4) & 0x3FFF) << 32;
-    d |= (uint64_t)1 << 46;              // descriptor version (sm_100)
-    d |= (uint64_t)2 << 61;              // SWIZZLE_128B
-    return d;
+// 128-byte swizzled operand views, sbo = 8 rows of 128 B.  K-major: rows = M/N index (64 K-elements each).
+// MN-major: rows = K index (64 M/N-elements each); one M64 / N64 operand is exactly one atom, so lbo is unused.
+__device__ __forceinline__ uint64_t d_desc(uint32_t smem_addr) { return tfy_wg_desc(smem_addr, 16, 1024, TFY_WG_SW128); }
+
+// dW = dh^T . x (A = dh MN-major: M = units, 64-unit halves TILE_BYTES apart; K = batch rows, 16 rows = 2048 B per
+// MMA; B = x / W tile MN-major: N = 64 in-features in one atom)   -- TA = 1
+// dx = dh . W   (A = dh K-major: M = batch rows, 64-row halves 8 KB apart; K = units: 4 x 32 B inside each 64-unit
+// atom; B = W tile MN-major, K = unit rows, 2048 B per MMA)      -- TA = 0
+template <int TA>
+__device__ __forceinline__ void d_mma_chunk(float (&acc)[2][DB_N / 2], uint32_t dh0, uint32_t t0, bool first) {
+#pragma unroll
+    for (int k = 0; k < DB_K / 16; ++k) {
+        const uint64_t bdesc = d_desc(t0 + k * 2048);
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+            const uint32_t a = TA ? dh0 + h * TILE_BYTES + k * 2048 : dh0 + (k >> 2) * TILE_BYTES + (k & 3) * 32 + h * 8192;
+            tfy_wgmma_m64n64<TA, 1>(acc[h], d_desc(a), bdesc, (first && k == 0) ? 0u : 1u);
+        }
+    }
 }
-__device__ __forceinline__ uint32_t d_idesc(uint32_t m, uint32_t n, uint32_t a_mn_major, uint32_t b_mn_major) {
-    return (1u << 4) | (1u << 7) | (1u << 10) | (a_mn_major << 15) | (b_mn_major << 16) | ((n >> 3) << 17) |
-           ((m >> 4) << 24);
-}
-__device__ __forceinline__ void d_umma(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t acc) {
-    asm volatile(
-        "{\n\t"
-        ".reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t"
-        "}" ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(acc)
-        : "memory");
-}
-__device__ __forceinline__ void d_commit(uint64_t* bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(d_smem_u32(bar))
-                 : "memory");
-}
-__device__ __forceinline__ void d_tmem_ld16(uint32_t taddr, uint32_t* r) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-          "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-        : "r"(taddr)
-        : "memory");
+
+// Warpgroup epilogue: accumulator -> fp32 rows (acc_s) -> bf16, 128-byte-swizzled [128 rows][128 B] tile (stage)
+// -> one TMA store.  `bar` is the named barrier of the warpgroup.
+__device__ __forceinline__ void d_epilogue(float (&acc)[2][DB_N / 2], float* acc_s, uint8_t* stage, int bar,
+                                           const CUtensorMap* map, int c0, int c1) {
+    tfy_wg_store_rows<DB_N>(acc_s, ACC_LD, acc[0], 0);
+    tfy_wg_store_rows<DB_N>(acc_s, ACC_LD, acc[1], 64);
+    asm volatile("bar.sync %0, 128;" ::"r"(bar) : "memory");
+    const int row = threadIdx.x & 127;
+    const float* src = acc_s + row * ACC_LD;
+    uint8_t* dst = stage + row * 128;
+#pragma unroll
+    for (int ch = 0; ch < 8; ++ch) {                  // 8 chunks of 16 B (8 bf16) per 128-byte row
+        float v[8];
+        *reinterpret_cast<float4*>(v) = *reinterpret_cast<const float4*>(src + ch * 8);
+        *reinterpret_cast<float4*>(v + 4) = *reinterpret_cast<const float4*>(src + ch * 8 + 4);
+        // 128-byte swizzle of the TMA store map: 16-byte chunk index XOR (row mod 8)
+        *reinterpret_cast<uint4*>(dst + ((ch ^ (row & 7)) << 4)) = TfyPack<__nv_bfloat16>::pack(v);
+    }
+    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");     // generic-proxy writes -> async proxy
+    asm volatile("bar.sync %0, 128;" ::"r"(bar) : "memory");
+    if (row < 32 && d_elect_one()) {
+        d_tma_store_2d(map, stage, c0, c1);
+        asm volatile("cp.async.bulk.commit_group;" ::: "memory");
+        asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");  // smem must outlive the read
+    }
 }
 
 }  // namespace
@@ -115,11 +130,10 @@ tfy_dense_bwd_kernel(const __grid_constant__ CUtensorMap map_dh, const __grid_co
     uint8_t* s_x = s_dh + DH_BYTES;                  // [128 rows (batch)][128 B (64 in-features)]     sw128
     uint8_t* s_w = s_x + TILE_BYTES;                 // [128 rows (units)][128 B (64 in-features)]     sw128
     uint8_t* s_out = s_w + TILE_BYTES;               // [2][128 rows][128 B] staging for the TMA stores, sw128
-    uint64_t* full = reinterpret_cast<uint64_t*>(s_out + 2 * TILE_BYTES);
-    uint64_t* acc_full = full + 1;                   // [2]
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(acc_full + 2);
+    float* s_acc = reinterpret_cast<float*>(s_out + 2 * TILE_BYTES);    // [2][128][ACC_LD] fp32
+    uint64_t* full = reinterpret_cast<uint64_t*>(reinterpret_cast<uint8_t*>(s_acc) + 2 * ACC_BYTES);
 
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int warp = __shfl_sync(0xffffffffu, (int)threadIdx.x >> 5, 0);   // warp-uniform role index
     const int n0 = blockIdx.x * DB_N;
     if (threadIdx.x == 0) {
         asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&map_dh)) : "memory");
@@ -128,23 +142,12 @@ tfy_dense_bwd_kernel(const __grid_constant__ CUtensorMap map_dh, const __grid_co
         asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&map_dw)) : "memory");
         asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&map_dx)) : "memory");
         d_mbar_init(full, 1);
-        d_mbar_init(&acc_full[0], 1);
-        d_mbar_init(&acc_full[1], 1);
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
-    if (warp == 1) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(d_smem_u32(tmem_slot)),
-                     "r"(128)
-                     : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
     __syncthreads();
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    const uint32_t tmem_base = *tmem_slot;
     tfy_pdl_sync();
 
-    if (warp == 0) {
+    if (warp == 8) {
         if (d_elect_one()) {
             d_mbar_expect_tx(full, DH_BYTES + TILE_BYTES + (want_dx ? TILE_BYTES : 0));
             d_tma_load_2d(&map_dh, full, s_dh, 0, 0);
@@ -152,75 +155,20 @@ tfy_dense_bwd_kernel(const __grid_constant__ CUtensorMap map_dh, const __grid_co
             d_tma_load_2d(&map_x, full, s_x, n0, 0);
             if (want_dx) d_tma_load_2d(&map_w, full, s_w, n0, 0);
         }
-    } else if (warp == 1) {
-        if (d_elect_one()) {
-            d_mbar_wait(full, 0);
-            asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-            const uint32_t dh0 = d_smem_u32(s_dh), x0 = d_smem_u32(s_x), w0 = d_smem_u32(s_w);
-            // dW = dh^T . x : A = dh read MN-major (M = units: two 64-unit atoms TILE_BYTES apart; K = batch rows,
-            // 16 rows = 2048 B per MMA), B = x tile MN-major (N = 64 in-features in one atom)
-            {
-                const uint32_t idesc = d_idesc(DB_M, DB_N, 1, 1);
-#pragma unroll
-                for (int k = 0; k < DB_K / 16; ++k) {
-                    const uint64_t adesc = d_desc(dh0 + k * 2048, TILE_BYTES, 1024);
-                    const uint64_t bdesc = d_desc(x0 + k * 2048, 0, 1024);
-                    d_umma(tmem_base, adesc, bdesc, idesc, k > 0 ? 1u : 0u);
-                }
-                d_commit(&acc_full[0]);
-            }
-            // dx = dh . W : A = dh K-major (M = batch rows; K = units: 4 x 32 B inside each 64-unit atom),
-            // B = W tile MN-major (K = unit rows, 2048 B per MMA)
-            if (want_dx) {
-                const uint32_t idesc = d_idesc(DB_M, DB_N, 0, 1);
-#pragma unroll
-                for (int k = 0; k < DB_K / 16; ++k) {
-                    const uint64_t adesc = d_desc(dh0 + (k >> 2) * TILE_BYTES + (k & 3) * 32, 0, 1024);
-                    const uint64_t bdesc = d_desc(w0 + k * 2048, 0, 1024);
-                    d_umma(tmem_base + DB_N, adesc, bdesc, idesc, k > 0 ? 1u : 0u);
-                }
-                d_commit(&acc_full[1]);
-            }
-        }
-    } else {
-        // epilogue: which = 0 -> dW (warps 2-5), 1 -> dx (warps 6-9); a warp may only read its TMEM lane quadrant
-        const int which = (warp - 2) >> 2, quad = warp & 3;
-        if (which == 0 || want_dx) {
-            d_mbar_wait(&acc_full[which], 0);
-            asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-            const int row = quad * 32 + lane;
-            uint8_t* stage = s_out + which * TILE_BYTES + row * 128;
-            uint32_t r[4][16];
-            const uint32_t taddr = tmem_base + ((uint32_t)(quad * 32) << 16) + (uint32_t)(which * DB_N);
-#pragma unroll
-            for (int q = 0; q < 4; ++q) d_tmem_ld16(taddr + q * 16, r[q]);
-            asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-            for (int ch = 0; ch < 8; ++ch) {                  // 8 chunks of 16 B (8 bf16) per 128-byte row
-                const uint32_t* src = &r[ch >> 1][(ch & 1) * 8];
-                uint4 v;
-                v.x = tfy_pack_bf16x2(__uint_as_float(src[0]), __uint_as_float(src[1]));
-                v.y = tfy_pack_bf16x2(__uint_as_float(src[2]), __uint_as_float(src[3]));
-                v.z = tfy_pack_bf16x2(__uint_as_float(src[4]), __uint_as_float(src[5]));
-                v.w = tfy_pack_bf16x2(__uint_as_float(src[6]), __uint_as_float(src[7]));
-                // 128-byte swizzle of the TMA store map: 16-byte chunk index XOR (row mod 8)
-                *reinterpret_cast<uint4*>(stage + ((ch ^ (row & 7)) << 4)) = v;
-            }
-            asm volatile("fence.proxy.async.shared::cta;" ::: "memory");     // generic-proxy writes -> async proxy
-            if (which == 0) asm volatile("bar.sync 1, 128;" ::: "memory");   // the four warps of this accumulator
-            else asm volatile("bar.sync 2, 128;" ::: "memory");
-            if (quad == 2 && d_elect_one()) {
-                d_tma_store_2d(which == 0 ? &map_dw : &map_dx, s_out + which * TILE_BYTES, n0, 0);
-                asm volatile("cp.async.bulk.commit_group;" ::: "memory");
-                asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");  // smem must outlive the read
-            }
-        }
+        return;
     }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    __syncthreads();
-    if (warp == 1) {
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(128) : "memory");
-    }
+    const int which = warp >> 2;                     // 0 -> dW (warps 0-3), 1 -> dx (warps 4-7)
+    if (which == 1 && !want_dx) return;
+    d_mbar_wait(full, 0);
+    const uint32_t dh0 = d_smem_u32(s_dh);
+    float acc[2][DB_N / 2];
+    tfy_wg_fence();
+    if (which == 0) d_mma_chunk<1>(acc, dh0, d_smem_u32(s_x), true);
+    else d_mma_chunk<0>(acc, dh0, d_smem_u32(s_w), true);
+    tfy_wg_commit();
+    tfy_wg_wait<0>();
+    d_epilogue(acc, s_acc + which * (ACC_BYTES / 4), s_out + which * TILE_BYTES, 1 + which,
+               which == 0 ? &map_dw : &map_dx, n0, 0);
 }
 
 // ---------------------------------------------------------------------------------------------------------
@@ -228,11 +176,11 @@ tfy_dense_bwd_kernel(const __grid_constant__ CUtensorMap map_dh, const __grid_co
 // a job is either a 128-unit tile of dW -- K loop over the batch in chunks of 128 rows -- or a 128-row tile of
 // dx -- K loop over the units in chunks of 128.  Same operand views and epilogue as the single-shot kernel, with
 // a 3-stage TMA ring (48 KB per stage: the two 64-column boxes of the dh chunk + the x or W tile).
-// warp 0: TMA producer   warp 1: TMEM + MMA issue   warps 2-5: epilogue
+// warps 0-3: wgmma + epilogue   warp 4: TMA producer
 // ---------------------------------------------------------------------------------------------------------
 namespace {
-constexpr int DT_STAGES = 3, DT_STAGE_BYTES = DH_BYTES + TILE_BYTES, DT_THREADS = 192;
-constexpr size_t DT_SMEM = 1024 + (size_t)DT_STAGES * DT_STAGE_BYTES + TILE_BYTES + 256;
+constexpr int DT_STAGES = 3, DT_STAGE_BYTES = DH_BYTES + TILE_BYTES, DT_THREADS = 160;
+constexpr size_t DT_SMEM = 1024 + (size_t)DT_STAGES * DT_STAGE_BYTES + TILE_BYTES + ACC_BYTES + 256;
 }  // namespace
 
 __global__ void __launch_bounds__(DT_THREADS, 1)
@@ -243,12 +191,11 @@ tfy_dense_bwd_tiled_kernel(const __grid_constant__ CUtensorMap map_dh, const __g
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
     uint8_t* ring = smem;                                            // [3] { dh box0, dh box1, tile }
     uint8_t* s_out = ring + (size_t)DT_STAGES * DT_STAGE_BYTES;      // staging for the TMA store
-    uint64_t* full = reinterpret_cast<uint64_t*>(s_out + TILE_BYTES);
+    float* s_acc = reinterpret_cast<float*>(s_out + TILE_BYTES);     // [128][ACC_LD] fp32
+    uint64_t* full = reinterpret_cast<uint64_t*>(reinterpret_cast<uint8_t*>(s_acc) + ACC_BYTES);
     uint64_t* empty = full + DT_STAGES;
-    uint64_t* acc_full = empty + DT_STAGES;
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(acc_full + 1);
 
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int warp = __shfl_sync(0xffffffffu, (int)threadIdx.x >> 5, 0), lane = threadIdx.x & 31;   // warp-uniform role index
     const int n0 = blockIdx.x * DB_N;
     const int job = blockIdx.y;
     const bool is_dw = job < n_u_tiles;
@@ -258,23 +205,13 @@ tfy_dense_bwd_tiled_kernel(const __grid_constant__ CUtensorMap map_dh, const __g
     if (threadIdx.x == 0) {
         asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&map_dh)) : "memory");
         asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(is_dw ? &map_x : &map_w)) : "memory");
-        for (int st = 0; st < DT_STAGES; ++st) { d_mbar_init(&full[st], 1); d_mbar_init(&empty[st], 1); }
-        d_mbar_init(acc_full, 1);
+        for (int st = 0; st < DT_STAGES; ++st) { d_mbar_init(&full[st], 1); d_mbar_init(&empty[st], 4); }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
-    if (warp == 1) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(d_smem_u32(tmem_slot)),
-                     "r"(64)
-                     : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
     __syncthreads();
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    const uint32_t tmem_base = *tmem_slot;
     tfy_pdl_sync();
 
-    if (warp == 0) {
+    if (warp == 4) {
         if (d_elect_one()) {
             for (int i = 0; i < n_chunks; ++i) {
                 const int st = i % DT_STAGES;
@@ -293,59 +230,23 @@ tfy_dense_bwd_tiled_kernel(const __grid_constant__ CUtensorMap map_dh, const __g
                 }
             }
         }
-    } else if (warp == 1) {
-        if (d_elect_one()) {
-            const uint32_t idesc = d_idesc(DB_M, DB_N, is_dw ? 1 : 0, 1);
-            for (int i = 0; i < n_chunks; ++i) {
-                const int st = i % DT_STAGES;
-                d_mbar_wait(&full[st], (i / DT_STAGES) & 1);
-                asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-                const uint32_t dh0 = d_smem_u32(ring + (size_t)st * DT_STAGE_BYTES), t0 = dh0 + DH_BYTES;
-#pragma unroll
-                for (int k = 0; k < DB_K / 16; ++k) {
-                    const uint64_t adesc = is_dw ? d_desc(dh0 + k * 2048, TILE_BYTES, 1024)
-                                                 : d_desc(dh0 + (k >> 2) * TILE_BYTES + (k & 3) * 32, 0, 1024);
-                    const uint64_t bdesc = d_desc(t0 + k * 2048, 0, 1024);
-                    d_umma(tmem_base, adesc, bdesc, idesc, (i > 0 || k > 0) ? 1u : 0u);
-                }
-                d_commit(&empty[st]);
-            }
-            d_commit(acc_full);
-        }
-    } else {
-        const int quad = warp & 3;
-        d_mbar_wait(acc_full, 0);
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        const int row = quad * 32 + lane;
-        uint8_t* stage = s_out + row * 128;
-        uint32_t r[4][16];
-        const uint32_t taddr = tmem_base + ((uint32_t)(quad * 32) << 16);
-#pragma unroll
-        for (int q = 0; q < 4; ++q) d_tmem_ld16(taddr + q * 16, r[q]);
-        asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-        for (int ch = 0; ch < 8; ++ch) {
-            const uint32_t* src = &r[ch >> 1][(ch & 1) * 8];
-            uint4 v;
-            v.x = tfy_pack_bf16x2(__uint_as_float(src[0]), __uint_as_float(src[1]));
-            v.y = tfy_pack_bf16x2(__uint_as_float(src[2]), __uint_as_float(src[3]));
-            v.z = tfy_pack_bf16x2(__uint_as_float(src[4]), __uint_as_float(src[5]));
-            v.w = tfy_pack_bf16x2(__uint_as_float(src[6]), __uint_as_float(src[7]));
-            *reinterpret_cast<uint4*>(stage + ((ch ^ (row & 7)) << 4)) = v;
-        }
-        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-        asm volatile("bar.sync 1, 128;" ::: "memory");
-        if (quad == 2 && d_elect_one()) {
-            d_tma_store_2d(is_dw ? &map_dw : &map_dx, s_out, n0, m0);
-            asm volatile("cp.async.bulk.commit_group;" ::: "memory");
-            asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
-        }
+        return;
     }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    __syncthreads();
-    if (warp == 1) {
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(64) : "memory");
+    float acc[2][DB_N / 2];
+    tfy_wg_zero<DB_N>(acc[0]);
+    tfy_wg_zero<DB_N>(acc[1]);
+    for (int i = 0; i < n_chunks; ++i) {
+        const int st = i % DT_STAGES;
+        d_mbar_wait(&full[st], (i / DT_STAGES) & 1);
+        tfy_wg_fence();
+        const uint32_t dh0 = d_smem_u32(ring + (size_t)st * DT_STAGE_BYTES), t0 = dh0 + DH_BYTES;
+        if (is_dw) d_mma_chunk<1>(acc, dh0, t0, false);
+        else d_mma_chunk<0>(acc, dh0, t0, false);
+        tfy_wg_commit();
+        tfy_wg_wait<0>();
+        if (lane == 0) d_mbar_arrive(&empty[st]);
     }
+    d_epilogue(acc, s_acc, s_out, 1, is_dw ? &map_dw : &map_dx, n0, m0);
 }
 
 namespace {

@@ -1,4 +1,4 @@
-// tcgen05 GEMM for sm_100a:  C[M,N] = act(A[M,K] . B[N,K]^T + bias[N])   (bf16 in, fp32 accumulate)
+// Hopper GEMM for sm_90a:  C[M,N] = act(A[M,K] . B[N,K]^T + bias[N])   (bf16 in, fp32 accumulate)
 //
 // This is the compute half of K5, the parameter-server PULL fused with the consuming GEMM:
 // B (the layer's weight matrix) is addressed through a TMA tensor map whose base pointer may be a
@@ -8,30 +8,34 @@
 // TF gRPC RecvTensor of every variable before the first consumer op, tf_yarn/tensorflow/cluster.py:
 // 60-66).  With a local B it is also the dense-layer GEMM of the mini-Keras fast path.
 //
-// Structure (one 128x128 output tile per CTA, 192 threads):
-//   warp 0   : TMA producer  -- cp.async.bulk.tensor.2d of a 128x64 A box and a 128x64 B box per
+// Structure (one 128x128 output tile per CTA, 160 threads):
+//   warps 0-3: one warpgroup -- wgmma M64 N128 K16 (kind f32.bf16.bf16) on both 64-row halves of the tile,
+//              accumulators in registers; then the epilogue: the fp32 tile goes through shared memory so that
+//              each thread owns one row, bias + activation, bf16 stores; or fp32 red.add for split-K
+//   warp 4   : TMA producer  -- cp.async.bulk.tensor.2d of a 128x64 A box and a 128x64 B box per
 //              stage (128-byte swizzle), completion on an mbarrier (complete_tx)
-//   warp 1   : TMEM allocation + MMA issuer -- one elected lane issues 4 x tcgen05.mma
-//              (M128 N128 K16, kind::f16) per stage, tcgen05.commit releases the stage
-//   warps 2-5: epilogue -- tcgen05.ld the fp32 accumulator out of TMEM (each warp owns the 32 TMEM
-//              lanes of its quadrant), bias + activation, bf16 stores; or fp32 red.add for split-K
 // Pipeline: STAGES-deep ring of {A,B} tiles guarded by full/empty mbarriers.
 #include <cuda.h>
 
 #include "tfy_common.cuh"
+#include "tfy_wgmma.cuh"
 
 namespace {
 
-constexpr int BM = 128, BN = 128, BK = 64, UMMA_K = 16, STAGES = 6;
+constexpr int BM = 128, BN = 128, BK = 64, UMMA_K = 16, STAGES = 4;
 constexpr int A_BYTES = BM * BK * 2, B_BYTES = BN * BK * 2, STAGE_BYTES = A_BYTES + B_BYTES;
-constexpr int GEMM_THREADS = 192;
-constexpr uint32_t TMEM_COLS = 128;   // fp32 accumulator: 128 lanes x 128 columns
-constexpr size_t SMEM_BYTES = (size_t)STAGES * STAGE_BYTES + 1024 /*align slack*/ + 256 /*barriers*/;
+constexpr int GEMM_THREADS = 160;
+constexpr int ACC_LD = BN + 4;        // fp32 row pitch of the staged accumulator (conflict-free row reads)
+constexpr size_t SMEM_BYTES = (size_t)STAGES * STAGE_BYTES + (size_t)BM * ACC_LD * 4 + 1024 /*align slack*/ +
+                              256 /*barriers*/;
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 
 __device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
     asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count) : "memory");
+}
+__device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
+    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
 }
 __device__ __forceinline__ void mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
     asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
@@ -53,15 +57,8 @@ __device__ __forceinline__ void tma_load_2d(const CUtensorMap* map, uint64_t* ba
         ::"r"(smem_u32(dst)), "l"(reinterpret_cast<uint64_t>(map)), "r"(smem_u32(bar)), "r"(c0), "r"(c1)
         : "memory");
 }
-__device__ __forceinline__ void tc_commit(uint64_t* bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-                 : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
 
-// One lane of a converged warp: the compiler keeps descriptors in uniform registers and emits back-to-back
-// UTCHMMA / UTMALDG (with `lane == 0` each one was wrapped in an ELECT / R2UR / BRA.U.ANY loop, ~48 cycles).
+// One lane of a converged warp: the compiler keeps the TMA operands in uniform registers.
 __device__ __forceinline__ bool tc_elect_one() {
     uint32_t pred;
     asm volatile("{\n\t.reg .pred P;\n\telect.sync _|P, 0xffffffff;\n\tselp.b32 %0, 1, 0, P;\n\t}" : "=r"(pred));
@@ -70,47 +67,18 @@ __device__ __forceinline__ bool tc_elect_one() {
 
 // K-major, 128-byte swizzled operand tile: rows of 64 bf16 (128 B); 8-row core groups 1024 B apart.
 __device__ __forceinline__ uint64_t make_kmajor_sw128_desc(uint32_t smem_addr) {
-    uint64_t d = 0;
-    d |= (uint64_t)((smem_addr & 0x3FFFF) >> 4);        // start address        bits [0,14)
-    d |= (uint64_t)0 << 16;                              // leading byte offset  bits [16,30): unused (1 atom on K)
-    d |= (uint64_t)(1024 >> 4) << 32;                    // stride byte offset   bits [32,46): 8 rows x 128 B
-    d |= (uint64_t)1 << 46;                              // descriptor version 1 (sm_100)
-    d |= (uint64_t)2 << 61;                              // layout: SWIZZLE_128B
-    return d;
-}
-
-// kind::f16 instruction descriptor: D=f32, A=B=bf16, both K-major, M=128, N=128
-__device__ __forceinline__ uint32_t make_idesc_bf16_m128(uint32_t n) {
-    return (1u << 4) | (1u << 7) | (1u << 10) | ((n >> 3) << 17) | ((128u >> 4) << 24);
-}
-
-__device__ __forceinline__ void umma_bf16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                          uint32_t accumulate) {
-    asm volatile(
-        "{\n\t"
-        ".reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t"
-        "}" ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t* r) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-          "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-        : "r"(taddr)
-        : "memory");
-    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+    return tfy_wg_desc(smem_addr, 16, 1024, TFY_WG_SW128);
 }
 
 }  // namespace
 
-// Fused split-K epilogue (out_mode 2): what runs after the partial sums of ALL K-slices of a tile have been added.
-// The CTA whose arrival completes the tile reads the fp32 accumulator back (L2), clears it for the next step,
-// applies bias + ReLU + dropout and writes the bf16 activations and the gradient-gate mask -- the work of the
-// separate tfy_bias_act_drop_fwd_f32 launch of round 1 (same element indexing, same random numbers).
+// Split-K partial sums are never added with atomics: K-slice z stores its fp32 partial tile into slab z of the
+// workspace (slab stride M * ldc) and the slabs are summed in slice order afterwards, so the result is the same
+// bit for bit on every run.
+// Fused split-K epilogue (out_mode 2): what runs after the partial sums of ALL K-slices of a tile are stored.
+// The K-slice CTAs of the tile share the work: each sums a part of the tile over the slabs, applies bias + ReLU +
+// dropout and writes the bf16 activations and the gradient-gate mask -- the work of the separate
+// tfy_bias_act_drop_fwd_f32 launch (same element indexing, same random numbers).
 struct TfySplitKEpilogue {
     uint32_t* counters;      // two per output tile (arrive, finish), zero on entry, left zero
     __nv_bfloat16* y;        // [M, N] bf16 activations (row pitch ldy)
@@ -121,8 +89,8 @@ struct TfySplitKEpilogue {
     int ldy;
 };
 
-// out_mode 0: C (bf16) = act(acc + bias)      out_mode 1: C32 (fp32) += acc   (split-K partial sums)
-// out_mode 2: as 1, then the last-arriving CTA of every tile runs the fused epilogue above
+// out_mode 0: C (bf16) = act(acc + bias)      out_mode 1: slab blockIdx.z of C32 (fp32) = acc   (split-K partials)
+// out_mode 2: as 1, then the K-slice CTAs of every tile run the fused epilogue above
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
 tfy_gemm_bf16_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b,
                      __nv_bfloat16* __restrict__ C, float* __restrict__ C32, const __nv_bfloat16* __restrict__ bias,
@@ -130,10 +98,9 @@ tfy_gemm_bf16_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_con
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
     uint8_t* tiles = smem;
-    uint64_t* full = reinterpret_cast<uint64_t*>(smem + (size_t)STAGES * STAGE_BYTES);
+    float* acc_s = reinterpret_cast<float*>(smem + (size_t)STAGES * STAGE_BYTES);     // [BM][ACC_LD]
+    uint64_t* full = reinterpret_cast<uint64_t*>(acc_s + (size_t)BM * ACC_LD);
     uint64_t* empty = full + STAGES;
-    uint64_t* tmem_full = empty + STAGES;
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tmem_full + 1);
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int m0 = blockIdx.x * BM, n0 = blockIdx.y * BN;
@@ -143,29 +110,19 @@ tfy_gemm_bf16_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_con
     if (kt1 > total_k_tiles) kt1 = total_k_tiles;
     const int n_kt = kt1 - kt0;
 
-    if (warp == 0 && lane == 0) {
+    if (threadIdx.x == 0) {
         asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&map_a)) : "memory");
         asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&map_b)) : "memory");
         for (int s = 0; s < STAGES; ++s) {
             mbar_init(&full[s], 1);
-            mbar_init(&empty[s], 1);
+            mbar_init(&empty[s], 4);           // one arrival per MMA warp
         }
-        mbar_init(tmem_full, 1);
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
-    if (warp == 1) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)),
-                     "r"(TMEM_COLS)
-                     : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
     tfy_pdl_sync();                      // upstream grids complete; our dependents may start launching
 
-    if (warp == 0) {
+    if (warp == 4) {
         if (tc_elect_one()) {
             for (int i = 0; i < n_kt; ++i) {
                 const int s = i % STAGES;
@@ -179,56 +136,59 @@ tfy_gemm_bf16_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_con
                 tma_load_2d(&map_b, &full[s], b_dst, k0, n0);
             }
         }
-    } else if (warp == 1) {
-        if (tc_elect_one()) {
-            const uint32_t idesc = make_idesc_bf16_m128(BN);
-            for (int i = 0; i < n_kt; ++i) {
-                const int s = i % STAGES;
-                const uint32_t ph = (i / STAGES) & 1;
-                mbar_wait(&full[s], ph);
-                tc_fence_after();
-                const uint32_t a_addr = smem_u32(tiles + (size_t)s * STAGE_BYTES);
-                const uint64_t adesc = make_kmajor_sw128_desc(a_addr);
-                const uint64_t bdesc = make_kmajor_sw128_desc(a_addr + A_BYTES);
+        return;
+    }
+    {
+        // ---- MMA: the warpgroup accumulates both 64-row halves; a stage is released once the wgmmas of the
+        // NEXT stage are issued and the older group has retired (one group in flight behind the TMA ring)
+        float acc[2][BN / 2];
+        tfy_wg_zero<BN>(acc[0]);
+        tfy_wg_zero<BN>(acc[1]);
+        for (int i = 0; i < n_kt; ++i) {
+            const int s = i % STAGES;
+            mbar_wait(&full[s], (i / STAGES) & 1);
+            tfy_wg_fence();
+            const uint32_t a_addr = smem_u32(tiles + (size_t)s * STAGE_BYTES);
+            const uint64_t bdesc = make_kmajor_sw128_desc(a_addr + A_BYTES);
 #pragma unroll
-                for (int k = 0; k < BK / UMMA_K; ++k) {
-                    // advance 16 bf16 = 32 B along K inside the 128 B swizzle atom: +2 in 16-byte units
-                    umma_bf16(tmem_base, adesc + (uint64_t)(2 * k), bdesc + (uint64_t)(2 * k), idesc,
-                              (i > 0 || k > 0) ? 1u : 0u);
-                }
-                tc_commit(&empty[s]);          // frees the smem stage when these MMAs have read it
+            for (int k = 0; k < BK / UMMA_K; ++k) {
+                // advance 16 bf16 = 32 B along K inside the 128 B swizzle atom: +2 in 16-byte units
+#pragma unroll
+                for (int h = 0; h < 2; ++h)
+                    tfy_wgmma_m64n128<0, 0>(acc[h], make_kmajor_sw128_desc(a_addr + h * 64 * 128) + (uint64_t)(2 * k),
+                                            bdesc + (uint64_t)(2 * k), 1u);
             }
-            tc_commit(tmem_full);              // accumulator complete
+            tfy_wg_commit();
+            tfy_wg_wait<1>();
+            if (i > 0 && lane == 0) mbar_arrive(&empty[(i - 1) % STAGES]);
         }
-    } else {
-        // epilogue: this warp may only touch the TMEM lanes of its quadrant
+        tfy_wg_wait<0>();
+        tfy_wg_store_rows<BN>(acc_s, ACC_LD, acc[0], 0);
+        tfy_wg_store_rows<BN>(acc_s, ACC_LD, acc[1], 64);
+        asm volatile("bar.sync 1, 128;" ::: "memory");
+    }
+    {
+        // epilogue: warp q owns rows [32 q, 32 q + 32) of the tile, one row per thread
         const int quad = warp & 3;
-        mbar_wait(tmem_full, 0);
-        tc_fence_after();
         const int row = m0 + quad * 32 + lane;
         const bool row_ok = row < M;
+        const float* acc_row = acc_s + (size_t)(quad * 32 + lane) * ACC_LD;
 #pragma unroll 1
         for (int c = 0; c < BN; c += 16) {
-            uint32_t r[16];
-            tmem_ld16(tmem_base + ((uint32_t)(quad * 32) << 16) + (uint32_t)c, r);
             const int n = n0 + c;
             if (!row_ok || n >= N || n_kt <= 0) continue;
             float v[16];
 #pragma unroll
-            for (int j = 0; j < 16; ++j) v[j] = __uint_as_float(r[j]);
+            for (int j = 0; j < 16; j += 4) *reinterpret_cast<float4*>(v + j) = *reinterpret_cast<const float4*>(acc_row + c + j);
             if (out_mode >= 1) {
-                float* dst = C32 + (size_t)row * ldc + n;
+                float* dst = C32 + (size_t)blockIdx.z * M * ldc + (size_t)row * ldc + n;
                 if (n + 16 <= N && (ldc & 3) == 0 && (n & 3) == 0) {
-                    // 4 x red.v4.f32 instead of 16 scalar REDs
 #pragma unroll
-                    for (int j = 0; j < 16; j += 4)
-                        asm volatile("red.global.add.v4.f32 [%0], {%1,%2,%3,%4};" ::"l"(dst + j), "f"(v[j]),
-                                     "f"(v[j + 1]), "f"(v[j + 2]), "f"(v[j + 3])
-                                     : "memory");
+                    for (int j = 0; j < 16; j += 4) __stcg(reinterpret_cast<float4*>(dst + j), *reinterpret_cast<float4*>(v + j));
                 } else {
 #pragma unroll
                     for (int j = 0; j < 16; ++j)
-                        if (n + j < N) atomicAdd(dst + j, v[j]);
+                        if (n + j < N) __stcg(dst + j, v[j]);
                 }
             } else {
                 if (bias) {
@@ -252,15 +212,15 @@ tfy_gemm_bf16_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_con
             }
         }
     }
-    if (out_mode == 2 && warp >= 2) {
+    if (out_mode == 2) {
         // ---- fused split-K epilogue, spread over ALL K-slice CTAs of the tile ----
-        // Every CTA arrives on the tile's counter after its red.adds, waits until all gridDim.z slices have arrived
+        // Every CTA arrives on the tile's counter after its slab stores, waits until all gridDim.z slices have arrived
         // (they are co-resident: the host only selects this mode when the whole grid fits the SMs) and then finishes
         // 1/gridDim.z of the tile: one 8-element group per thread, i.e. ONE L2 round trip.  (A first version let the
         // last-arriving CTA finish the whole 128x128 tile alone: 16 dependent L2 round trips per thread, +9 us.)
         uint32_t* cnt = ep.counters + 2 * (blockIdx.y * gridDim.x + blockIdx.x);
-        asm volatile("bar.sync 1, 128;" ::: "memory");                 // this CTA's red.adds are all issued
-        if (threadIdx.x == 64) {
+        asm volatile("bar.sync 1, 128;" ::: "memory");                 // this CTA's slab stores are all issued
+        if (threadIdx.x == 0) {
             __threadfence();
             atomicAdd(cnt, 1u);
             while (*reinterpret_cast<volatile uint32_t*>(cnt) < gridDim.z) {
@@ -271,7 +231,7 @@ tfy_gemm_bf16_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_con
         {
             const uint32_t step = ep.hp ? (uint32_t)ep.hp->step : 0u;
             const float keep_scale = ep.drop_rate > 0.f ? 1.f / (1.f - ep.drop_rate) : 1.f;
-            const int t = threadIdx.x - 64;                            // 0..127
+            const int t = threadIdx.x;                                 // 0..127
             const int G = N / 8;                                       // 8-element groups per row (N % 8 == 0)
             constexpr int tile_g = BN / 8, tile_groups = BM * tile_g;
             const int per = (tile_groups + (int)gridDim.z - 1) / (int)gridDim.z;
@@ -280,11 +240,14 @@ tfy_gemm_bf16_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_con
                 const int r = i / tile_g, gq = i % tile_g;
                 const int row = m0 + r, n = n0 + gq * 8;
                 if (row >= M || n >= N) continue;
-                float4* zp = reinterpret_cast<float4*>(C32 + (size_t)row * ldc + n);
-                const float4 a = __ldcg(zp), b = __ldcg(zp + 1);
-                zp[0] = make_float4(0.f, 0.f, 0.f, 0.f);
-                zp[1] = make_float4(0.f, 0.f, 0.f, 0.f);
-                float v[8] = {a.x, a.y, a.z, a.w, b.x, b.y, b.z, b.w};
+                float v[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
+#pragma unroll 4
+                for (int z = 0; z < (int)gridDim.z; ++z) {             // slice order: the same sum on every run
+                    const float4* zp = reinterpret_cast<const float4*>(C32 + (size_t)z * M * ldc + (size_t)row * ldc + n);
+                    const float4 a = __ldcg(zp), b = __ldcg(zp + 1);
+                    v[0] += a.x; v[1] += a.y; v[2] += a.z; v[3] += a.w;
+                    v[4] += b.x; v[5] += b.y; v[6] += b.z; v[7] += b.w;
+                }
                 if (bias) {
                     float bv[8];
                     TfyPack<__nv_bfloat16>::unpack(tfy_ld16(bias + n), bv);
@@ -310,18 +273,13 @@ tfy_gemm_bf16_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_con
             }
         }
         asm volatile("bar.sync 1, 128;" ::: "memory");
-        if (threadIdx.x == 64) {                                       // the CTA that finishes last re-arms both counters
+        if (threadIdx.x == 0) {                                       // the CTA that finishes last re-arms both counters
             __threadfence();
             if (atomicAdd(cnt + 1, 1u) == gridDim.z - 1) {
                 cnt[0] = 0u;
                 cnt[1] = 0u;
             }
         }
-    }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 1) {
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(TMEM_COLS) : "memory");
     }
 }
 
@@ -361,10 +319,47 @@ bool make_map(CUtensorMap* map, const void* ptr, uint64_t rows, uint64_t K, uint
 
 }  // namespace
 
+__global__ void __launch_bounds__(256) tfy_splitk_sum_f32_kernel(const float* __restrict__ slabs, float* __restrict__ out,
+                                                                int splits, size_t slab, size_t n4) {
+    tfy_pdl_sync();
+    for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n4; i += (size_t)gridDim.x * blockDim.x) {
+        float4 a = __ldcg(reinterpret_cast<const float4*>(slabs) + i);
+#pragma unroll 8
+        for (int z = 1; z < splits; ++z) {
+            const float4 b = __ldcg(reinterpret_cast<const float4*>(slabs + (size_t)z * slab) + i);
+            a.x += b.x; a.y += b.y; a.z += b.z; a.w += b.w;
+        }
+        reinterpret_cast<float4*>(out)[i] = a;
+    }
+}
+
 extern "C" {
 
+// Number of K-slices (= workspace slabs) tfy_gemm_bf16 / tfy_gemm_bf16_splitk_fused run for a requested split_k.
+int tfy_gemm_bf16_splitk_slabs(int K, int split_k) {
+    const int k_tiles = (K + BK - 1) / BK;
+    if (split_k < 1) split_k = 1;
+    if (split_k > k_tiles) split_k = k_tiles;
+    if (split_k < 1) return 1;
+    const int per = (k_tiles + split_k - 1) / split_k;
+    return (k_tiles + per - 1) / per;
+}
+
+// out[i] = sum over z in order of slabs[z * slab + i], i < n (n % 4 == 0, 16-byte aligned): the split-K reduction.
+int tfy_splitk_sum_f32(const float* slabs, float* out, int splits, size_t slab, size_t n, cudaStream_t s) {
+    if (splits < 1 || (n & 3) || (slab & 3) || (((uintptr_t)slabs | (uintptr_t)out) & 15)) return -2;
+    const size_t n4 = n / 4;
+    int grid = (int)((n4 + 255) / 256);
+    if (grid > TFY_NUM_SMS * 4) grid = TFY_NUM_SMS * 4;
+    if (grid < 1) grid = 1;
+    tfy_launch_pdl(tfy_splitk_sum_f32_kernel, dim3(grid), dim3(256), 0, s, slabs, out, splits, slab, n4);
+    return (int)cudaGetLastError();
+}
+
 // C[M,N] (bf16, ld ldc) = act(A[M,K] (ld lda) . B[N,K]^T (ld ldb) + bias[N]);  B may be a peer (NVLink) pointer.
-// split_k > 1: partial products are accumulated with fp32 atomics into C32[M,N] (ld ldc, must be zeroed).
+// split_k > 1 (or C == nullptr): C32 is a workspace of tfy_gemm_bf16_splitk_slabs(K, split_k) x M x ldc floats; slab z
+// (C32 + z * M * ldc) receives the partial product of K-slice z, to be summed in slab order (tfy_splitk_sum_f32,
+// tfy_bias_act_drop_fwd_f32).
 // Requirements: K % 8 == 0, lda % 8 == 0, ldb % 8 == 0, 16-byte aligned base pointers.
 int tfy_gemm_bf16(const void* A, const void* B, void* C, float* C32, const void* bias, int M, int N, int K, int lda,
                   int ldb, int ldc, int relu, int split_k, cudaStream_t s) {
@@ -394,7 +389,7 @@ int tfy_gemm_bf16(const void* A, const void* B, void* C, float* C32, const void*
 }
 
 // Split-K GEMM with the fused epilogue: y[M,N] (bf16) = dropout(act(A . B^T + bias)), mask[M,N] (optional bytes).
-// acc32 [M,N] fp32 (row pitch N) is scratch that must be zero on entry and is left zero; counters: two uint32 per
+// acc32: fp32 scratch of tfy_gemm_bf16_splitk_slabs(K, split_k) x M x N floats (slabs of row pitch N); counters: two uint32 per
 // 128x128 output tile, zero on entry, left zero.  N % 8 == 0.  The K-slice CTAs of a tile meet on a counter, so the
 // whole grid must be co-resident: returns -8 when tiles x split_k exceeds the SM count (use the two-launch path).
 int tfy_gemm_bf16_splitk_fused(const void* A, const void* B, float* acc32, uint32_t* counters, const void* bias, void* y,

@@ -1,39 +1,34 @@
-// Persistent 2-CTA tcgen05 GEMM for sm_100a:  C[M,N] = act(A[M,K] . B[N,K]^T + bias[N])   (bf16 in, fp32 accumulate)
+// Persistent Hopper GEMM for sm_90a:  C[M,N] = act(A[M,K] . B[N,K]^T + bias[N])   (bf16 in, fp32 accumulate)
 //
-// The large-shape companion of tfy_gemm.cu (one 128x128 tile per CTA, which tops out far below the tensor-core
-// peak: a single SM issues M=128 MMAs and every CTA re-reads both operands).  Here two SMs of a TPC form a CTA
-// pair (cluster 2x1x1) and issue ONE `tcgen05.mma.cta_group::2` of M=256 x N=256 x K=16 per step:
-//   * each CTA stages only ITS half of the operands -- 128 rows of A and 128 of the 256 B rows -- so shared-memory
-//     traffic per FLOP is half that of two independent CTAs, and the pair's 256x256 tile re-uses every operand
-//     byte 256 times;
-//   * the kernel is persistent (one pair per TPC, static round-robin over output tiles) with a 5-stage TMA ring
-//     shared by all tiles and a DOUBLE-BUFFERED accumulator (2 x 256 TMEM columns): the epilogue of tile i
-//     overlaps the main loop of tile i+1;
-//   * epilogue: tcgen05.ld -> bias / ReLU -> bf16 -> swizzled staging tile -> TMA store.
-// Roles per CTA: warp 0 TMA producer (both CTAs; `cp.async.bulk.tensor...cta_group::2` completes on the LEADER's
-// barrier), warp 1 MMA issuer (leader CTA only; tcgen05.commit multicast frees the stage in both CTAs), warp 2 TMEM
-// allocation, warps 4-7 epilogue (each CTA drains its own 128 accumulator lanes; arrivals on the leader's
-// tmem_empty barrier travel through distributed shared memory).
+// The large-shape companion of tfy_gemm.cu (one 128x128 tile per CTA, which re-reads both operands for every
+// tile and runs one warpgroup).  Here one CTA per SM walks the output tiles of 128 x 256 (static round-robin):
+//   * two consumer warpgroups, each issuing wgmma M64 N256 K16 on its 64-row half of the tile, share every
+//     B byte staged in shared memory (256 x 64 per stage) -- twice the operand re-use of the 128x128 kernel;
+//   * a 4-stage TMA ring (48 KB per stage) shared by all tiles of the CTA, so the loads of the next tile start
+//     while the current one is drained;
+//   * epilogue straight from the accumulator registers: bias / ReLU -> bf16 pairs -> global.
+// Roles: warps 0-3 and 4-7 the two consumer warpgroups, warp 8 the TMA producer.
 // The B operand may be a peer (NVLink) address, as in tfy_gemm.cu.
 #include <cuda.h>
 
 #include "tfy_common.cuh"
+#include "tfy_wgmma.cuh"
 
 namespace {
 
-constexpr int G2_BM = 256, G2_BN = 256, G2_BK = 64;      // tile of the CTA pair
-constexpr int G2_HALF_M = 128, G2_HALF_N = 128;          // rows of A / B staged per CTA
-constexpr int G2_STAGES = 5;
-constexpr int G2_A_BYTES = G2_HALF_M * G2_BK * 2, G2_B_BYTES = G2_HALF_N * G2_BK * 2;
-constexpr int G2_STAGE_BYTES = G2_A_BYTES + G2_B_BYTES;                // 32 KB per CTA per stage
-constexpr int G2_OUT_BYTES = 128 * 128;                                // staging: 128 rows x 64 bf16
-constexpr int G2_THREADS = 256;
-constexpr size_t G2_SMEM = 1024 + (size_t)G2_STAGES * G2_STAGE_BYTES + 2 * G2_OUT_BYTES + 512;
-constexpr uint32_t G2_PEER_MASK = 0xFEFFFFFFu;           // clears the CTA-rank bit of a shared::cluster address
+constexpr int G2_BM = 128, G2_BN = 256, G2_BK = 64;      // output tile of a CTA
+constexpr int G2_STAGES = 4;
+constexpr int G2_A_BYTES = G2_BM * G2_BK * 2, G2_B_BYTES = G2_BN * G2_BK * 2;
+constexpr int G2_STAGE_BYTES = G2_A_BYTES + G2_B_BYTES;                // 48 KB per stage
+constexpr int G2_THREADS = 288;
+constexpr size_t G2_SMEM = 1024 + (size_t)G2_STAGES * G2_STAGE_BYTES + 512;
 
 __device__ __forceinline__ uint32_t g2_smem(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 __device__ __forceinline__ void g2_mbar_init(uint64_t* bar, uint32_t count) {
     asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(g2_smem(bar)), "r"(count) : "memory");
+}
+__device__ __forceinline__ void g2_mbar_arrive(uint64_t* bar) {
+    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(g2_smem(bar)) : "memory");
 }
 __device__ __forceinline__ void g2_mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
     asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(g2_smem(bar)), "r"(bytes) : "memory");
@@ -49,23 +44,11 @@ __device__ __forceinline__ void g2_mbar_wait(uint64_t* bar, uint32_t parity) {
         "G2DONE:\n\t"
         "}" ::"r"(g2_smem(bar)), "r"(parity) : "memory");
 }
-// arrive on the barrier at the same offset in CTA `rank` of the cluster
-__device__ __forceinline__ void g2_mbar_arrive_cluster(uint64_t* bar, uint32_t rank) {
-    uint32_t remote;
-    asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(remote) : "r"(g2_smem(bar)), "r"(rank));
-    asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(remote) : "memory");
-}
-__device__ __forceinline__ void g2_tma_load_2sm(const CUtensorMap* map, uint64_t* bar, void* dst, int c0, int c1) {
-    // executed by both CTAs: the transaction bytes land on CTA 0's barrier (peer bit cleared)
+__device__ __forceinline__ void g2_tma_load(const CUtensorMap* map, uint64_t* bar, void* dst, int c0, int c1) {
     asm volatile(
-        "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
-        ::"r"(g2_smem(dst)), "l"(reinterpret_cast<uint64_t>(map)), "r"(g2_smem(bar) & G2_PEER_MASK), "r"(c0), "r"(c1)
+        "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
+        ::"r"(g2_smem(dst)), "l"(reinterpret_cast<uint64_t>(map)), "r"(g2_smem(bar)), "r"(c0), "r"(c1)
         : "memory");
-}
-__device__ __forceinline__ void g2_tma_store(const CUtensorMap* map, const void* src, int c0, int c1) {
-    asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];"
-                 ::"l"(reinterpret_cast<uint64_t>(map)), "r"(g2_smem(src)), "r"(c0), "r"(c1)
-                 : "memory");
 }
 __device__ __forceinline__ bool g2_elect() {
     uint32_t pred;
@@ -73,61 +56,22 @@ __device__ __forceinline__ bool g2_elect() {
     return pred != 0;
 }
 __device__ __forceinline__ uint64_t g2_desc(uint32_t smem_addr) {     // K-major, SWIZZLE_128B, 8-row groups 1024 B apart
-    uint64_t d = 0;
-    d |= (uint64_t)((smem_addr & 0x3FFFF) >> 4);
-    d |= (uint64_t)(1024 >> 4) << 32;
-    d |= (uint64_t)1 << 46;
-    d |= (uint64_t)2 << 61;
-    return d;
-}
-__device__ __forceinline__ void g2_umma(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t acc) {
-    asm volatile(
-        "{\n\t"
-        ".reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t"
-        "}" ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(acc)
-        : "memory");
-}
-__device__ __forceinline__ void g2_commit_mc(uint64_t* bar) {       // arrive on `bar` in BOTH CTAs when the MMAs retire
-    asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;"
-                 ::"r"(g2_smem(bar)), "h"((uint16_t)3)
-                 : "memory");
-}
-__device__ __forceinline__ void g2_tmem_ld16(uint32_t taddr, uint32_t* r) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-          "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-        : "r"(taddr)
-        : "memory");
-}
-__device__ __forceinline__ void g2_cluster_sync() {
-    asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
-    asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
+    return tfy_wg_desc(smem_addr, 16, 1024, TFY_WG_SW128);
 }
 
 }  // namespace
 
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(G2_THREADS, 1)
+__global__ void __launch_bounds__(G2_THREADS, 1)
 tfy_gemm2_bf16_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b,
-                      const __grid_constant__ CUtensorMap map_c, const __nv_bfloat16* __restrict__ bias, int M, int N,
-                      int K, int relu) {
+                      __nv_bfloat16* __restrict__ C, const __nv_bfloat16* __restrict__ bias, int M, int N, int K,
+                      int ldc, int relu) {
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
     uint8_t* ring = smem;
-    uint8_t* s_out = ring + (size_t)G2_STAGES * G2_STAGE_BYTES;          // [2][128 rows][128 B]
-    uint64_t* full = reinterpret_cast<uint64_t*>(s_out + 2 * G2_OUT_BYTES);
+    uint64_t* full = reinterpret_cast<uint64_t*>(ring + (size_t)G2_STAGES * G2_STAGE_BYTES);
     uint64_t* empty = full + G2_STAGES;
-    uint64_t* tmem_full = empty + G2_STAGES;       // [2]
-    uint64_t* tmem_empty = tmem_full + 2;          // [2] (used in the leader)
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tmem_empty + 2);
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    uint32_t cta_rank;
-    asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(cta_rank));
-    const bool leader = cta_rank == 0;
-    const int pair = blockIdx.x >> 1, n_pairs = gridDim.x >> 1;
     const int tiles_m = (M + G2_BM - 1) / G2_BM, tiles_n = (N + G2_BN - 1) / G2_BN;
     const int n_tiles = tiles_m * tiles_n;
     const int k_blocks = (K + G2_BK - 1) / G2_BK;
@@ -135,131 +79,72 @@ tfy_gemm2_bf16_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_co
     if (threadIdx.x == 0) {
         asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&map_a)) : "memory");
         asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&map_b)) : "memory");
-        asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&map_c)) : "memory");
         for (int s = 0; s < G2_STAGES; ++s) {
-            g2_mbar_init(&full[s], 1);         // leader's producer arms it; both CTAs' TMA bytes complete it
-            g2_mbar_init(&empty[s], 1);        // one multicast tcgen05.commit
-        }
-        for (int a = 0; a < 2; ++a) {
-            g2_mbar_init(&tmem_full[a], 1);    // one multicast tcgen05.commit
-            g2_mbar_init(&tmem_empty[a], 8);   // 4 epilogue warps x 2 CTAs
+            g2_mbar_init(&full[s], 1);         // the producer's expect_tx + the TMA bytes
+            g2_mbar_init(&empty[s], 8);        // one arrival per consumer warp
         }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
-    if (warp == 2) {
-        asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(g2_smem(tmem_slot)),
-                     "r"(512)
-                     : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-    }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    g2_cluster_sync();                          // barriers + TMEM of both CTAs are ready
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    const uint32_t tmem_base = *tmem_slot;
+    __syncthreads();
     tfy_pdl_sync();
 
-    if (warp == 0) {
-        // ===== TMA producer (both CTAs): my 128 rows of A, my 128 of the tile's 256 B rows =====
+    if (warp == 8) {
+        // ===== TMA producer: 128 rows of A and 256 rows of B (two 128-row boxes) per stage =====
         if (g2_elect()) {
             uint32_t it = 0;
-            for (int t = pair; t < n_tiles; t += n_pairs) {
-                const int tm = t % tiles_m, tn = t / tiles_m;
-                const int m0 = tm * G2_BM + (int)cta_rank * G2_HALF_M, n0 = tn * G2_BN + (int)cta_rank * G2_HALF_N;
+            for (int t = blockIdx.x; t < n_tiles; t += gridDim.x) {
+                const int m0 = (t % tiles_m) * G2_BM, n0 = (t / tiles_m) * G2_BN;
                 for (int kb = 0; kb < k_blocks; ++kb, ++it) {
                     const int s = it % G2_STAGES;
                     if (it >= G2_STAGES) g2_mbar_wait(&empty[s], ((it / G2_STAGES) - 1) & 1);
                     uint8_t* a_dst = ring + (size_t)s * G2_STAGE_BYTES;
-                    if (leader) g2_mbar_expect_tx(&full[s], 2 * G2_STAGE_BYTES);
-                    g2_tma_load_2sm(&map_a, &full[s], a_dst, kb * G2_BK, m0);
-                    g2_tma_load_2sm(&map_b, &full[s], a_dst + G2_A_BYTES, kb * G2_BK, n0);
+                    g2_mbar_expect_tx(&full[s], G2_STAGE_BYTES);
+                    g2_tma_load(&map_a, &full[s], a_dst, kb * G2_BK, m0);
+                    g2_tma_load(&map_b, &full[s], a_dst + G2_A_BYTES, kb * G2_BK, n0);
+                    g2_tma_load(&map_b, &full[s], a_dst + G2_A_BYTES + G2_B_BYTES / 2, kb * G2_BK, n0 + 128);
                 }
             }
         }
-    } else if (warp == 1) {
-        // ===== MMA issuer (leader only): M256 N256 K16 x 4 per stage, accumulator double-buffered in TMEM =====
-        if (leader && g2_elect()) {
-            const uint32_t idesc = (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(G2_BN >> 3) << 17) |
-                                   ((uint32_t)(G2_BM >> 4) << 24);
-            uint32_t it = 0, tile_i = 0;
-            for (int t = pair; t < n_tiles; t += n_pairs, ++tile_i) {
-                const uint32_t acc = tile_i & 1;
-                if (tile_i >= 2) g2_mbar_wait(&tmem_empty[acc], ((tile_i >> 1) - 1) & 1);
-                asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-                for (int kb = 0; kb < k_blocks; ++kb, ++it) {
-                    const int s = it % G2_STAGES;
-                    g2_mbar_wait(&full[s], (it / G2_STAGES) & 1);
-                    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-                    const uint32_t a_addr = g2_smem(ring + (size_t)s * G2_STAGE_BYTES);
-                    const uint64_t adesc = g2_desc(a_addr), bdesc = g2_desc(a_addr + G2_A_BYTES);
-#pragma unroll
-                    for (int k = 0; k < G2_BK / 16; ++k)
-                        g2_umma(tmem_base + acc * G2_BN, adesc + (uint64_t)(2 * k), bdesc + (uint64_t)(2 * k), idesc,
-                                (kb > 0 || k > 0) ? 1u : 0u);
-                    g2_commit_mc(&empty[s]);                 // both CTAs may refill this stage
-                }
-                g2_commit_mc(&tmem_full[acc]);               // both CTAs' epilogues may drain the accumulator
-            }
-        }
-    } else if (warp >= 4) {
-        // ===== epilogue (both CTAs): my 128 accumulator lanes, 4 chunks of 64 columns =====
-        const int quad = warp & 3;
-        const int row = quad * 32 + lane;
-        uint32_t tile_i = 0, chunk_i = 0;
-        for (int t = pair; t < n_tiles; t += n_pairs, ++tile_i) {
-            const int tm = t % tiles_m, tn = t / tiles_m;
-            const int m0 = tm * G2_BM + (int)cta_rank * G2_HALF_M, n0 = tn * G2_BN;
-            const uint32_t acc = tile_i & 1;
-            g2_mbar_wait(&tmem_full[acc], (tile_i >> 1) & 1);
-            asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-            for (int ch = 0; ch < G2_BN / 64; ++ch, ++chunk_i) {
-                uint32_t r[4][16];
-                const uint32_t taddr = tmem_base + ((uint32_t)(quad * 32) << 16) + acc * G2_BN + ch * 64;
-#pragma unroll
-                for (int q = 0; q < 4; ++q) g2_tmem_ld16(taddr + q * 16, r[q]);
-                asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-                if (ch == G2_BN / 64 - 1) {
-                    // the whole accumulator is in registers: hand the TMEM buffer back to the MMA issuer
-                    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-                    __syncwarp();
-                    if (lane == 0) g2_mbar_arrive_cluster(&tmem_empty[acc], 0);
-                }
-                uint8_t* stage = s_out + (chunk_i & 1) * G2_OUT_BYTES;
-                // the TMA store that last read this staging buffer (two chunks ago) must be done reading
-                if (quad == 0 && lane == 0) asm volatile("cp.async.bulk.wait_group.read 1;" ::: "memory");
-                asm volatile("bar.sync 1, 128;" ::: "memory");
-                const int nbase = n0 + ch * 64;
-#pragma unroll
-                for (int c8 = 0; c8 < 8; ++c8) {
-                    float v[8];
-#pragma unroll
-                    for (int j = 0; j < 8; ++j) v[j] = __uint_as_float(r[c8 >> 1][(c8 & 1) * 8 + j]);
-                    if (bias) {
-#pragma unroll
-                        for (int j = 0; j < 8; ++j) {
-                            const int n = nbase + c8 * 8 + j;
-                            if (n < N) v[j] += __bfloat162float(bias[n]);
-                        }
-                    }
-                    if (relu) {
-#pragma unroll
-                        for (int j = 0; j < 8; ++j) v[j] = fmaxf(v[j], 0.f);
-                    }
-                    *reinterpret_cast<uint4*>(stage + row * 128 + ((c8 ^ (row & 7)) << 4)) = TfyPack<__nv_bfloat16>::pack(v);
-                }
-                asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-                asm volatile("bar.sync 1, 128;" ::: "memory");
-                if (quad == 0 && lane == 0) {
-                    g2_tma_store(&map_c, stage, nbase, m0);
-                    asm volatile("cp.async.bulk.commit_group;" ::: "memory");
-                }
-            }
-        }
-        if (quad == 0 && lane == 0) asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
+        return;
     }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    g2_cluster_sync();                          // nobody frees TMEM / exits while the peer may still signal it
-    if (warp == 2) {
-        asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(512) : "memory");
+    // ===== consumers: warpgroup h owns rows [64 h, 64 h + 64) of every tile =====
+    const int h = warp >> 2, w = warp & 3;
+    uint32_t it = 0;
+    for (int t = blockIdx.x; t < n_tiles; t += gridDim.x) {
+        const int m0 = (t % tiles_m) * G2_BM, n0 = (t / tiles_m) * G2_BN;
+        float acc[G2_BN / 2];
+        tfy_wg_zero<G2_BN>(acc);
+        for (int kb = 0; kb < k_blocks; ++kb, ++it) {
+            const int s = it % G2_STAGES;
+            g2_mbar_wait(&full[s], (it / G2_STAGES) & 1);
+            tfy_wg_fence();
+            const uint32_t a_addr = g2_smem(ring + (size_t)s * G2_STAGE_BYTES);
+            const uint64_t adesc = g2_desc(a_addr + h * 64 * 128), bdesc = g2_desc(a_addr + G2_A_BYTES);
+#pragma unroll
+            for (int k = 0; k < G2_BK / 16; ++k)
+                tfy_wgmma_m64n256<0, 0>(acc, adesc + (uint64_t)(2 * k), bdesc + (uint64_t)(2 * k), 1u);
+            tfy_wg_commit();
+            tfy_wg_wait<1>();                            // the previous stage's wgmmas have retired
+            if (kb > 0 && lane == 0) g2_mbar_arrive(&empty[(it - 1) % G2_STAGES]);
+        }
+        tfy_wg_wait<0>();
+        if (k_blocks > 0 && lane == 0) g2_mbar_arrive(&empty[(it - 1) % G2_STAGES]);
+        // fragment layout: value i of this thread is row 16 w + lane / 4 + 8 ((i / 2) % 2), column 8 (i / 4) + 2 (lane % 4)
+        const int r0 = m0 + h * 64 + 16 * w + (lane >> 2);
+#pragma unroll
+        for (int i = 0; i < G2_BN / 2; i += 2) {
+            const int row = r0 + 8 * ((i >> 1) & 1), n = n0 + 8 * (i >> 2) + 2 * (lane & 3);
+            if (row >= M || n >= N) continue;
+            float v0 = acc[i], v1 = acc[i + 1];
+            if (bias) {
+                v0 += __bfloat162float(bias[n]);
+                if (n + 1 < N) v1 += __bfloat162float(bias[n + 1]);
+            }
+            if (relu) { v0 = fmaxf(v0, 0.f); v1 = fmaxf(v1, 0.f); }
+            __nv_bfloat16* dst = C + (size_t)row * ldc + n;
+            if (n + 1 < N) *reinterpret_cast<__nv_bfloat162*>(dst) = __floats2bfloat162_rn(v0, v1);
+            else dst[0] = __float2bfloat16(v0);
+        }
     }
 }
 
@@ -306,16 +191,15 @@ int tfy_gemm2_bf16(const void* A, const void* B, void* C, const void* bias, int 
             return -5;
         int dev = 0;
         cudaGetDevice(&dev);
-        if (cudaDeviceGetAttribute(&g2_sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || g2_sms < 2) return -5;
+        if (cudaDeviceGetAttribute(&g2_sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || g2_sms < 1) return -5;
         g2_attr_set = true;
     }
-    CUtensorMap ma, mb, mc;
-    if (!g2_map(&ma, A, M, K, lda) || !g2_map(&mb, B, N, K, ldb) || !g2_map(&mc, C, M, N, ldc)) return -6;
+    CUtensorMap ma, mb;
+    if (!g2_map(&ma, A, M, K, lda) || !g2_map(&mb, B, N, K, ldb)) return -6;
     const int n_tiles = ((M + G2_BM - 1) / G2_BM) * ((N + G2_BN - 1) / G2_BN);
-    int pairs = g2_sms / 2;
-    if (pairs > n_tiles) pairs = n_tiles;
-    tfy_launch_pdl((tfy_gemm2_bf16_kernel), dim3(2 * pairs), dim3(G2_THREADS), G2_SMEM, s, ma, mb, mc,
-                   (const __nv_bfloat16*)bias, M, N, K, relu);
+    const int grid = n_tiles < g2_sms ? n_tiles : g2_sms;
+    tfy_launch_pdl((tfy_gemm2_bf16_kernel), dim3(grid), dim3(G2_THREADS), G2_SMEM, s, ma, mb, (__nv_bfloat16*)C,
+                   (const __nv_bfloat16*)bias, M, N, K, ldc, relu);
     return (int)cudaGetLastError();
 }
 

@@ -1,4 +1,4 @@
-// Fused layer kernels of the mini-Keras fast path (sm_100a, bf16 activations, NHWC).
+// Fused layer kernels of the mini-Keras fast path (sm_90a, bf16 activations, NHWC).
 //
 // The stock-PyTorch rendition of the MNIST-CNN step launches 53 kernels, most of
 // them tiny elementwise / reduction kernels around the cuDNN/cuBLAS calls (bias
@@ -190,13 +190,13 @@ tfy_conv3x3_c1_wgrad_kernel(const XT* __restrict__ x, const __nv_bfloat16* __res
 // y = dropout(act(z + bias[c])) over a [rows, C] bf16 matrix (C % 8 == 0); y may alias z.
 // mask (optional, 1 byte per element): 1 = gradient flows (act'(.) != 0 and kept).
 // ---------------------------------------------------------------------------------------------
-// ZT = __nv_bfloat16: z is a bf16 matrix.  ZT = float: z is the fp32 split-K accumulator of the tcgen05
-// GEMM; it is consumed AND cleared here so the next step's partial sums start from zero.
+// ZT = __nv_bfloat16: z is a bf16 matrix.  ZT = float: z holds the `splits` fp32 partial-product slabs
+// ([splits][rows][C]) of the split-K GEMM; they are summed here in slab order (the same result on every run).
 template <typename ZT>
 __global__ void __launch_bounds__(256)
 tfy_bias_act_drop_fwd_kernel(ZT* z, const __nv_bfloat16* __restrict__ bias, __nv_bfloat16* y,
                              uint8_t* __restrict__ mask, size_t rows, int C, int relu, float drop_rate, uint32_t seed,
-                             const TfyOptHyper* __restrict__ hp) {
+                             const TfyOptHyper* __restrict__ hp, int splits) {
     tfy_pdl_sync();
     const int G = C / 8;
     const size_t total = rows * G;
@@ -207,11 +207,14 @@ tfy_bias_act_drop_fwd_kernel(ZT* z, const __nv_bfloat16* __restrict__ bias, __nv
         const int g = idx % G;
         float v[8], bv[8];
         if (sizeof(ZT) == 4) {
-            float4* zp = reinterpret_cast<float4*>(z) + idx * 2;
-            const float4 a = zp[0], b = zp[1];
-            v[0] = a.x; v[1] = a.y; v[2] = a.z; v[3] = a.w; v[4] = b.x; v[5] = b.y; v[6] = b.z; v[7] = b.w;
-            zp[0] = make_float4(0.f, 0.f, 0.f, 0.f);
-            zp[1] = make_float4(0.f, 0.f, 0.f, 0.f);
+#pragma unroll
+            for (int k = 0; k < 8; ++k) v[k] = 0.f;
+#pragma unroll 8
+            for (int sl = 0; sl < splits; ++sl) {              // unrolled: eight slabs' loads in flight at once
+                const float4* zp = reinterpret_cast<const float4*>(z) + (size_t)sl * total * 2 + idx * 2;
+                const float4 a = __ldcg(zp), b = __ldcg(zp + 1);
+                v[0] += a.x; v[1] += a.y; v[2] += a.z; v[3] += a.w; v[4] += b.x; v[5] += b.y; v[6] += b.z; v[7] += b.w;
+            }
         } else {
             TfyPack<__nv_bfloat16>::unpack(tfy_ld16(reinterpret_cast<const __nv_bfloat16*>(z) + idx * 8), v);
         }
@@ -475,11 +478,12 @@ tfy_softmax_xent_kernel(const __nv_bfloat16* __restrict__ logits, const __nv_bfl
 //                                                                          ReLU / dropout gate + bias gradient)
 // Replaces a cuBLAS GEMM, the softmax/CE kernel, two more cuBLAS GEMMs and the gate/bias-gradient kernel
 // (3.9 + 6.6 + 4.6 + 4.1 + 6.9 us of launches for 128 x 128 x 10).  Intermediates stay in fp32.
-// One CTA per 16 rows; the batch reductions (dW2, db2, db1, loss) meet in an fp32 scratch buffer and the
-// last CTA to finish converts and clears it.
+// One CTA per 16 rows; every CTA stores its part of the batch reductions (dW2, db2, db1, loss) in its own slab of
+// an fp32 scratch buffer and the last CTA to finish sums the slabs in CTA order (no float atomics: the result is
+// the same bit for bit on every run), converts and clears them.
 // h: [B, K] bf16, W2: [C, K] bf16, b2: [C] bf16, labels: [B] int64, mask1: [B, K] uint8 (bit 0 = gradient
 // flows) or null.  K in {128, 256, 512}, C <= 16.
-// scratch: [C*K | 16 | K | 2] floats, zero on entry and on exit; counter: one uint32, same.
+// scratch: one slab [C*K | 16 | K | 4] floats per CTA, zero on entry and on exit; counter: one uint32, same.
 // ---------------------------------------------------------------------------------------------
 // debug: per-CTA event timeline of the head kernel (16 slots of SM-clock deltas per CTA), see tfy_nn_set_timeline
 __device__ long long* n_timeline = nullptr;
@@ -488,7 +492,7 @@ __device__ long long* n_timeline = nullptr;
         if (n_tl && threadIdx.x == 0) n_tl[(size_t)blockIdx.x * 16 + (k)] = clock64() - n_t0; \
     } while (0)
 
-constexpr int HEAD_THREADS = 256, HEAD_CMAX = 16, HEAD_ROWS = 16;
+constexpr int HEAD_THREADS = 256, HEAD_CMAX = 16, HEAD_ROWS = 16, HEAD_WARPS = HEAD_THREADS / 32;
 
 template <int K>
 __global__ void __launch_bounds__(HEAD_THREADS)
@@ -512,14 +516,15 @@ tfy_dense_head_fused_kernel(const __nv_bfloat16* __restrict__ h, const __nv_bflo
     float* s_w = reinterpret_cast<float*>(head_smem + (size_t)HEAD_ROWS * KP * 2);    // [16][K], rows >= C are zero
     float* s_dl = s_w + (size_t)HEAD_CMAX * K;                                                // [16][HEAD_CMAX]
     float* s_b = s_dl + HEAD_ROWS * HEAD_CMAX;                                        // [HEAD_CMAX]
-    float* s_red = s_b + HEAD_CMAX;                                                   // loss, correct
-    float* s_col = s_red + 4;                                                         // [max(K, 256)], 16-byte aligned
+    float* s_red = s_b + HEAD_CMAX;                                                   // [warp][loss, correct]
+    float* s_col = s_red + 2 * HEAD_WARPS;                                            // [max(K, 256)], 16-byte aligned
     __shared__ uint32_t s_last;
     const int tid = threadIdx.x;
     const int row0 = blockIdx.x * HEAD_ROWS;
     const int rows = min(HEAD_ROWS, B - row0);
-    float* g_dw = scratch;
-    float* g_db2 = scratch + (size_t)C * K;
+    const size_t slab = (size_t)C * K + HEAD_CMAX + K + 4;          // this CTA's partial sums
+    float* g_dw = scratch + blockIdx.x * slab;
+    float* g_db2 = g_dw + (size_t)C * K;
     float* g_db1 = g_db2 + HEAD_CMAX;
     float* g_red = g_db1 + K;
 
@@ -545,7 +550,6 @@ tfy_dense_head_fused_kernel(const __nv_bfloat16* __restrict__ h, const __nv_bflo
         }
     }
     if (tid < HEAD_CMAX) s_b[tid] = (tid < C && b2) ? bf16_to_f(b2[tid]) : 0.f;
-    if (tid < 2) s_red[tid] = 0.f;
     for (int i = tid; i < HEAD_ROWS * HEAD_CMAX; i += HEAD_THREADS) s_dl[i] = 0.f;
     __syncthreads();
 
@@ -615,8 +619,8 @@ tfy_dense_head_fused_kernel(const __nv_bfloat16* __restrict__ h, const __nv_bflo
                 my_correct += __shfl_xor_sync(0xffffffffu, my_correct, off);
             }
             if ((tid & 31) == 0) {
-                atomicAdd(&s_red[0], my_loss);
-                atomicAdd(&s_red[1], my_correct);
+                s_red[2 * (tid >> 5)] = my_loss;
+                s_red[2 * (tid >> 5) + 1] = my_correct;
             }
         }
     }
@@ -624,8 +628,10 @@ tfy_dense_head_fused_kernel(const __nv_bfloat16* __restrict__ h, const __nv_bflo
     for (int i = tid; i < K; i += HEAD_THREADS) s_col[i] = 0.f;     // s_logit scratch -> column sums
     __syncthreads();
     if (tid == 0) {
-        atomicAdd(g_red, s_red[0]);
-        atomicAdd(g_red + 1, s_red[1]);
+        float l = 0.f, c = 0.f;
+        for (int w = 0; w < HEAD_WARPS; ++w) { l += s_red[2 * w]; c += s_red[2 * w + 1]; }
+        __stcg(g_red, l);
+        __stcg(g_red + 1, c);
     }
 
     N_MARK(2);
@@ -647,7 +653,7 @@ tfy_dense_head_fused_kernel(const __nv_bfloat16* __restrict__ h, const __nv_bflo
                 float a = 0.f;
 #pragma unroll
                 for (int r = 0; r < HEAD_ROWS; ++r) a = fmaf(s_dl[r * HEAD_CMAX + c], hc[r], a);
-                if (c < C) atomicAdd(g_dw + (size_t)c * K + k, a);
+                if (c < C) __stcg(g_dw + (size_t)c * K + k, a);
             }
         }
     }
@@ -655,7 +661,7 @@ tfy_dense_head_fused_kernel(const __nv_bfloat16* __restrict__ h, const __nv_bflo
         float a = 0.f;
 #pragma unroll
         for (int r = 0; r < HEAD_ROWS; ++r) a += s_dl[r * HEAD_CMAX + tid];
-        atomicAdd(g_db2 + tid, a);
+        __stcg(g_db2 + tid, a);
     }
 
     N_MARK(3);
@@ -695,11 +701,11 @@ tfy_dense_head_fused_kernel(const __nv_bfloat16* __restrict__ h, const __nv_bflo
                     col += v;
                 }
             }
-            if (db1) atomicAdd(&s_col[k], col);
+            if (db1) atomicAdd(&s_col[k], col);     // at most two addends per column: order-independent
         }
         if (db1) {
             __syncthreads();
-            for (int k = tid; k < K; k += HEAD_THREADS) atomicAdd(g_db1 + k, s_col[k]);
+            for (int k = tid; k < K; k += HEAD_THREADS) __stcg(g_db1 + k, s_col[k]);
         }
     }
 
@@ -713,13 +719,24 @@ tfy_dense_head_fused_kernel(const __nv_bfloat16* __restrict__ h, const __nv_bflo
     N_MARK(6);
     if (s_last) {
         __threadfence();
+        const int G = (int)gridDim.x;
         {
             constexpr int FV = HEAD_CMAX * K / 4 / HEAD_THREADS;    // float4 packs per thread (upper bound)
             float4 fv[FV];
 #pragma unroll
-            for (int q = 0; q < FV; ++q) {
-                const int i = tid + q * HEAD_THREADS;
-                fv[q] = i < C * K / 4 ? __ldcg(reinterpret_cast<const float4*>(g_dw) + i) : make_float4(0, 0, 0, 0);
+            for (int q = 0; q < FV; ++q) fv[q] = make_float4(0.f, 0.f, 0.f, 0.f);
+#pragma unroll 8
+            for (int g = 0; g < G; ++g) {                           // CTA order; unrolled: loads in flight together
+                float4* src = reinterpret_cast<float4*>(scratch + (size_t)g * slab);
+#pragma unroll
+                for (int q = 0; q < FV; ++q) {
+                    const int i = tid + q * HEAD_THREADS;
+                    if (i < C * K / 4) {
+                        const float4 v = __ldcg(src + i);
+                        fv[q].x += v.x; fv[q].y += v.y; fv[q].z += v.z; fv[q].w += v.w;
+                        __stcg(src + i, make_float4(0.f, 0.f, 0.f, 0.f));
+                    }
+                }
             }
 #pragma unroll
             for (int q = 0; q < FV; ++q) {
@@ -730,25 +747,41 @@ tfy_dense_head_fused_kernel(const __nv_bfloat16* __restrict__ h, const __nv_bflo
                     packed.x = *reinterpret_cast<uint32_t*>(&lo);
                     packed.y = *reinterpret_cast<uint32_t*>(&hi);
                     *reinterpret_cast<uint2*>(dw2 + (size_t)i * 4) = packed;
-                    __stcg(reinterpret_cast<float4*>(g_dw) + i, make_float4(0.f, 0.f, 0.f, 0.f));
                 }
             }
         }
+        const size_t o_db2 = (size_t)C * K, o_db1 = o_db2 + HEAD_CMAX, o_red = o_db1 + K;
         if (tid < HEAD_CMAX) {
-            if (tid < C && db2) db2[tid] = __float2bfloat16(__ldcg(g_db2 + tid));
-            __stcg(g_db2 + tid, 0.f);
+            float a = 0.f;
+#pragma unroll 8
+            for (int g = 0; g < G; ++g) {
+                a += __ldcg(scratch + g * slab + o_db2 + tid);
+                __stcg(scratch + g * slab + o_db2 + tid, 0.f);
+            }
+            if (tid < C && db2) db2[tid] = __float2bfloat16(a);
         }
         for (int k = tid; k < K; k += HEAD_THREADS) {
-            if (db1) db1[k] = __float2bfloat16(__ldcg(g_db1 + k));
-            __stcg(g_db1 + k, 0.f);
+            float a = 0.f;
+#pragma unroll 8
+            for (int g = 0; g < G; ++g) {
+                a += __ldcg(scratch + g * slab + o_db1 + k);
+                __stcg(scratch + g * slab + o_db1 + k, 0.f);
+            }
+            if (db1) db1[k] = __float2bfloat16(a);
         }
         if (tid == 0) {
-            const float mean_loss = __ldcg(g_red) * invB;
+            float l = 0.f, c = 0.f;
+#pragma unroll 8
+            for (int g = 0; g < G; ++g) {
+                l += __ldcg(scratch + g * slab + o_red);
+                c += __ldcg(scratch + g * slab + o_red + 1);
+                __stcg(scratch + g * slab + o_red, 0.f);
+                __stcg(scratch + g * slab + o_red + 1, 0.f);
+            }
+            const float mean_loss = l * invB;
             *loss = mean_loss;
             if (loss_host) *loss_host = mean_loss;      // pinned host scalar (UVA): no D2H copy node per step
-            if (stats) { stats[0] += __ldcg(g_red + 1); stats[1] += (float)B; }
-            __stcg(g_red, 0.f);
-            __stcg(g_red + 1, 0.f);
+            if (stats) { stats[0] += c; stats[1] += (float)B; }
             *counter = 0u;
         }
     }
@@ -774,7 +807,7 @@ int tfy_conv3x3_c1_fwd(const void* x, int x_is_f32, const void* w, const void* b
                        int O, cudaStream_t s) {
     if (O % 8) return -2;
     const size_t total = (size_t)B * (H - 2) * (W - 2);
-    const int grid = tfy_grid_for(total, 256, 148 * 8);
+    const int grid = tfy_grid_for(total, 256, TFY_NUM_SMS * 8);
     const size_t smem = (size_t)(10 * O) * sizeof(float);
     if (x_is_f32)
         tfy_launch_pdl((tfy_conv3x3_c1_fwd_kernel<float>), dim3(grid), dim3(256), smem, s, (const float*)x, (const __nv_bfloat16*)w,
@@ -802,21 +835,22 @@ int tfy_conv3x3_c1_wgrad(const void* x, int x_is_f32, const void* dz, float* par
 int tfy_bias_act_drop_fwd(const void* z, const void* bias, void* y, void* mask, size_t rows, int C, int relu,
                           float drop_rate, uint32_t seed, const TfyOptHyper* hp, cudaStream_t s) {
     if (C % 8) return -2;
-    const int grid = tfy_grid_for(rows * (C / 8), 256, 148 * 8);
+    const int grid = tfy_grid_for(rows * (C / 8), 256, TFY_NUM_SMS * 8);
     tfy_launch_pdl((tfy_bias_act_drop_fwd_kernel<__nv_bfloat16>), dim3(grid), dim3(256), 0, s, (__nv_bfloat16*)z, (const __nv_bfloat16*)bias,
                                                                      (__nv_bfloat16*)y, (uint8_t*)mask, rows, C, relu,
-                                                                     drop_rate, seed, hp);
+                                                                     drop_rate, seed, hp, 1);
     return (int)cudaGetLastError();
 }
 
-// same, reading (and clearing) the fp32 split-K accumulator z32 [rows, C]
+// same, summing the `splits` fp32 split-K slabs z32 [splits][rows][C] of tfy_gemm_bf16 in slab order
 int tfy_bias_act_drop_fwd_f32(void* z32, const void* bias, void* y, void* mask, size_t rows, int C, int relu,
-                              float drop_rate, uint32_t seed, const TfyOptHyper* hp, cudaStream_t s) {
-    if (C % 8) return -2;
-    const int grid = tfy_grid_for(rows * (C / 8), 256, 148 * 8);
-    tfy_launch_pdl((tfy_bias_act_drop_fwd_kernel<float>), dim3(grid), dim3(256), 0, s, (float*)z32, (const __nv_bfloat16*)bias,
+                              float drop_rate, uint32_t seed, const TfyOptHyper* hp, int splits, cudaStream_t s) {
+    if (C % 8 || splits < 1) return -2;
+    // one warp per block: every thread reads `splits` slabs, so the reads are spread over as many SMs as possible
+    const int grid = tfy_grid_for(rows * (C / 8), 32, TFY_NUM_SMS * 16);
+    tfy_launch_pdl((tfy_bias_act_drop_fwd_kernel<float>), dim3(grid), dim3(32), 0, s, (float*)z32, (const __nv_bfloat16*)bias,
                                                              (__nv_bfloat16*)y, (uint8_t*)mask, rows, C, relu,
-                                                             drop_rate, seed, hp);
+                                                             drop_rate, seed, hp, splits);
     return (int)cudaGetLastError();
 }
 
@@ -836,7 +870,7 @@ int tfy_bias_relu_pool_drop_fwd(const void* z, const void* bias, void* p, void* 
                                 float drop_rate, uint32_t seed, const TfyOptHyper* hp, cudaStream_t s) {
     if (C % 8 || H % 2 || W % 2) return -2;
     const size_t total = (size_t)B * (H / 2) * (W / 2) * (C / 8);
-    const int grid = tfy_grid_for(total, 256, 148 * 8);
+    const int grid = tfy_grid_for(total, 256, TFY_NUM_SMS * 8);
     tfy_bias_relu_pool_drop_fwd_kernel<<<grid, 256, 0, s>>>((const __nv_bfloat16*)z, (const __nv_bfloat16*)bias,
                                                             (__nv_bfloat16*)p, (uint8_t*)code, B, H, W, C, drop_rate,
                                                             seed, hp);
@@ -873,9 +907,11 @@ int tfy_memcpy_async(void* dst, const void* src, size_t bytes, cudaStream_t s) {
 int tfy_nn_set_timeline(long long* buf) { return (int)cudaMemcpyToSymbol(n_timeline, &buf, sizeof(buf)); }
 
 // fused classifier head (forward + backward); returns -2 when the shape is outside the kernel's envelope.
-// scratch: tfy_dense_head_scratch_elems(K, C) floats and counter: one uint32, zero on entry (left zero).
+// scratch: tfy_dense_head_scratch_elems(K, C, B) floats and counter: one uint32, zero on entry (left zero).
 // loss_host: optional second destination of the loss, e.g. a pinned host scalar (device-accessible under UVA).
-size_t tfy_dense_head_scratch_elems(int K, int C) { return (size_t)C * K + HEAD_CMAX + K + 2; }
+size_t tfy_dense_head_scratch_elems(int K, int C, int B) {
+    return (size_t)((B + HEAD_ROWS - 1) / HEAD_ROWS) * ((size_t)C * K + HEAD_CMAX + K + 4);
+}
 
 int tfy_dense_head_fused(const void* h, const void* w2, const void* b2, const void* labels, const void* mask1,
                          float scale1, float* loss, float* loss_host, float* stats, void* dw2, void* db2, void* dh,
@@ -883,7 +919,7 @@ int tfy_dense_head_fused(const void* h, const void* w2, const void* b2, const vo
                          float* scratch, uint32_t* counter, int B, int K, int C, cudaStream_t s) {
     if (!(K == 128 || K == 256 || K == 512) || C < 1 || C > HEAD_CMAX || B < 1) return -2;
     const size_t smem = (size_t)HEAD_ROWS * (K + 8) * 2 +
-                        ((size_t)HEAD_CMAX * K + HEAD_ROWS * HEAD_CMAX + HEAD_CMAX + 4 + (K > 256 ? K : 256)) * 4;
+                        ((size_t)HEAD_CMAX * K + HEAD_ROWS * HEAD_CMAX + HEAD_CMAX + 2 * HEAD_WARPS + (K > 256 ? K : 256)) * 4;
     const int grid = (B + HEAD_ROWS - 1) / HEAD_ROWS;
 #define TFY_HEAD(KK)                                                                                                   \
     do {                                                                                                               \

@@ -1,4 +1,4 @@
-// Parameter-server data plane over NVLink peer memory (sm_100a): K5 pull / K6 push.
+// Parameter-server data plane over NVLink peer memory (sm_90a): K5 pull / K6 push.
 //
 // A ps rank owns shards in ITS HBM (inside the symmetric arena); chief/worker ranks map them and
 // run these kernels against the peer addresses -- there is no server thread on the data path
@@ -8,7 +8,7 @@
 //   pull   dense : peer fp32 master -> local replica (fp32 or bf16), 16-byte peer loads
 //          sparse: gather the rows of a batch from a peer embedding table, fused with the bag
 //                  reduction (sum / mean) that consumes them
-//          GEMM  : weights stay remote and are streamed by TMA into the tcgen05 GEMM (tfy_gemm.cu)
+//          GEMM  : weights stay remote and are streamed by TMA into the wgmma GEMM (tfy_gemm.cu)
 //   push   dense : every worker applies its gradient to the peer master with red/atom -- asynchronous,
 //                  lock free (TF's use_locking=False semantics), optimizer fused, chosen PER VARIABLE (wide-and-deep
 //                  trains its linear tower with FTRL and its deep tower with Adagrad):
@@ -424,7 +424,7 @@ int tfy_ps_pull(const TfyPsSeg* segs, int nseg, size_t max_n, int local_is_bf16,
     if (nseg <= 0) return 0;
     size_t gx = (max_n / 4 + 255) / 256;
     if (gx < 1) gx = 1;
-    if (gx > 148 * 4) gx = 148 * 4;
+    if (gx > TFY_NUM_SMS * 4) gx = TFY_NUM_SMS * 4;
     dim3 grid((unsigned)gx, nseg);
     if (local_is_bf16) tfy_ps_pull_kernel<__nv_bfloat16><<<grid, 256, 0, s>>>(segs);
     else tfy_ps_pull_kernel<float><<<grid, 256, 0, s>>>(segs);
@@ -437,7 +437,7 @@ int tfy_ps_push(const TfyPsSeg* segs, int nseg, size_t max_n, int grad_is_bf16, 
     if (nseg <= 0) return 0;
     size_t gx = (max_n / 4 + 255) / 256;
     if (gx < 1) gx = 1;
-    if (gx > 148 * 4) gx = 148 * 4;
+    if (gx > TFY_NUM_SMS * 4) gx = TFY_NUM_SMS * 4;
     dim3 grid((unsigned)gx, nseg);
     if (grad_is_bf16) tfy_ps_push_kernel<__nv_bfloat16><<<grid, 256, 0, s>>>(segs, grad_scale, adam_scale);
     else tfy_ps_push_kernel<float><<<grid, 256, 0, s>>>(segs, grad_scale, adam_scale);
@@ -448,7 +448,7 @@ int tfy_ps_refresh_shadow(const TfyPsSeg* segs, int nseg, size_t max_n, cudaStre
     if (nseg <= 0) return 0;
     size_t gx = (max_n / 4 + 255) / 256;
     if (gx < 1) gx = 1;
-    if (gx > 148 * 4) gx = 148 * 4;
+    if (gx > TFY_NUM_SMS * 4) gx = TFY_NUM_SMS * 4;
     dim3 grid((unsigned)gx, nseg);
     tfy_ps_refresh_shadow_kernel<<<grid, 256, 0, s>>>(segs);
     return (int)cudaGetLastError();
@@ -459,7 +459,7 @@ int tfy_ps_embedding_bag(const void* table, const void* ids, void* out, int out_
     if (D % 4) {
         size_t g1 = ((size_t)B * D + 255) / 256;
         if (g1 < 1) g1 = 1;
-        if (g1 > 148 * 8) g1 = 148 * 8;
+        if (g1 > TFY_NUM_SMS * 8) g1 = TFY_NUM_SMS * 8;
         if (out_is_bf16)
             tfy_ps_embedding_bag_scalar_kernel<__nv_bfloat16><<<(unsigned)g1, 256, 0, s>>>(
                 (const float*)table, (const long long*)ids, (__nv_bfloat16*)out, B, L, D, V, mean);
@@ -470,7 +470,7 @@ int tfy_ps_embedding_bag(const void* table, const void* ids, void* out, int out_
     }
     size_t gx = ((size_t)B * (D / 4) + 255) / 256;
     if (gx < 1) gx = 1;
-    if (gx > 148 * 8) gx = 148 * 8;
+    if (gx > TFY_NUM_SMS * 8) gx = TFY_NUM_SMS * 8;
     if (out_is_bf16)
         tfy_ps_embedding_bag_kernel<__nv_bfloat16><<<(unsigned)gx, 256, 0, s>>>(
             (const float*)table, (const long long*)ids, (__nv_bfloat16*)out, B, L, D, V, mean);
@@ -491,13 +491,13 @@ int tfy_ps_push_rows(void* table, void* s1_table, void* s2_table, const void* id
     if ((opt == TFY_OPT_ADAM || opt == TFY_OPT_FTRL) && !s2_table) return -4;
     size_t gx = ((size_t)B * L * (D / 4) + 255) / 256;
     if (gx < 1) gx = 1;
-    if (gx > 148 * 8) gx = 148 * 8;
+    if (gx > TFY_NUM_SMS * 8) gx = TFY_NUM_SMS * 8;
     TfyPsHyper h;
     h.opt = opt; h.lr = lr; h.eps = eps; h.wd = 0.f; h.p1 = p1; h.p2 = p2; h.p3 = p3; h.grad_scale = grad_scale;
     if (D % 4) {
         size_t g1 = ((size_t)B * L * D + 255) / 256;
         if (g1 < 1) g1 = 1;
-        if (g1 > 148 * 8) g1 = 148 * 8;
+        if (g1 > TFY_NUM_SMS * 8) g1 = TFY_NUM_SMS * 8;
         if (grad_is_bf16)
             tfy_ps_push_rows_scalar_kernel<__nv_bfloat16><<<(unsigned)g1, 256, 0, s>>>(
                 (float*)table, (float*)s1_table, (float*)s2_table, (const long long*)ids, (const __nv_bfloat16*)dout, B,
@@ -523,7 +523,7 @@ int tfy_ps_multi_bag(const uint64_t* tables, const void* ids, void* out, int out
                      long long V, cudaStream_t s) {
     if (B < 1 || T < 1 || D < 1) return -2;
     size_t gx = ((size_t)B * D + 255) / 256;
-    if (gx > 148 * 8) gx = 148 * 8;
+    if (gx > TFY_NUM_SMS * 8) gx = TFY_NUM_SMS * 8;
     if (out_is_bf16)
         tfy_ps_multi_bag_kernel<__nv_bfloat16><<<(unsigned)gx, 256, 0, s>>>(tables, (const long long*)ids,
                                                                            (__nv_bfloat16*)out, B, T, D, V);
@@ -546,7 +546,7 @@ int tfy_ps_multi_push_rows(const uint64_t* tables, const uint64_t* s1s, const ui
     const bool vec = (D % 4 == 0) && (dout_ld % 4 == 0) && (col_stride % 4 == 0);
     size_t gx = ((size_t)T * B * (vec ? D / 4 : D) + 255) / 256;
     if (gx < 1) gx = 1;
-    if (gx > 148 * 8) gx = 148 * 8;
+    if (gx > TFY_NUM_SMS * 8) gx = TFY_NUM_SMS * 8;
 #define TFY_MPR(GT, VV)                                                                                              \
     tfy_ps_multi_push_rows_kernel<GT, VV><<<(unsigned)gx, 256, 0, s>>>(tables, s1s, s2s, (const long long*)ids,       \
                                                                        (const GT*)dout, B, T, D, V, h, adam_scale,    \

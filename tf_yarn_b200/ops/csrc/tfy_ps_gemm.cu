@@ -1,4 +1,4 @@
-// K5, the parameter-server PULL fused with the GEMM that consumes it (sm_100a).
+// K5, the parameter-server PULL fused with the GEMM that consumes it (sm_90a).
 //
 // First deep layer of a wide-and-deep model on the parameter-server path:
 //     y[b, :] = concat_t( table_t[ids[t, b], :] ) ++ numeric[b, :]   .   W^T  + bias
@@ -11,24 +11,30 @@
 //     of the GEMM;
 //   * B operand: the layer's weights stay on THEIR ps rank; TMA streams the bf16 shadow (row pitch padded to 8
 //     elements) tile by tile into shared memory;
-//   * tcgen05.mma M128 N256 K16 accumulates in TMEM; the epilogue adds the bias and stores bf16.
+//   * a warpgroup runs wgmma M64 N64 K16 on the eight 64 x 64 pieces of the 128 x 256 tile; each piece's
+//     chunk product is added into an fp32 accumulator kept in shared memory (in fragment order, so every thread
+//     reads and writes only its own words -- the whole tile would not fit the warpgroup's registers next to the
+//     producers'); the epilogue adds the bias and stores bf16.
 // The gathered activations are also written out once (bf16, [B, Kp]) because the backward needs them
 // (dW = dy^T x, tfy_dense_bwd).  K chunk c < T is table c (embedding dim 64); chunk T holds the numeric features.
-// warp 0: TMA (B tiles)   warp 1: TMEM + MMA issue   warps 2-17: A-tile producers (4 threads per row, 3 chunks in
-// flight each: a gather is a dependent id -> row round trip to (remote) HBM per chunk, so the K loop is only as
-// fast as the number of rows in flight)   warps 2-5 then run the epilogue
+// warps 0-15: A-tile producers (4 threads per row, 3 chunks in flight each: a gather is a dependent id -> row round
+// trip to (remote) HBM per chunk, so the K loop is only as fast as the number of rows in flight)
+// warps 16-19: wgmma + epilogue   warp 20: TMA (B tiles)
 #include <cuda.h>
 
 #include "tfy_common.cuh"
+#include "tfy_wgmma.cuh"
 
 namespace {
 
-constexpr int PG_BM = 128, PG_BN = 256, PG_BK = 64, PG_STAGES = 4;
+constexpr int PG_BM = 128, PG_BN = 256, PG_BK = 64, PG_STAGES = 2;
 constexpr int PG_A_BYTES = PG_BM * PG_BK * 2, PG_B_BYTES = PG_BN * PG_BK * 2, PG_STAGE_BYTES = PG_A_BYTES + PG_B_BYTES;
 constexpr int PG_PROD_WARPS = 16, PG_PROD_THREADS = PG_PROD_WARPS * 32;   // 4 threads per A-tile row
 constexpr int PG_DEPTH = 3;                                                  // gathered chunks in flight per thread
-constexpr int PG_THREADS = (2 + PG_PROD_WARPS) * 32;                         // 576
-constexpr size_t PG_SMEM = 1024 + (size_t)PG_STAGES * PG_STAGE_BYTES + 512;
+constexpr int PG_MMA_WARP = PG_PROD_WARPS, PG_TMA_WARP = PG_PROD_WARPS + 4;
+constexpr int PG_THREADS = (PG_PROD_WARPS + 5) * 32;                         // 672
+constexpr int PG_ACC_BYTES = PG_BM * PG_BN * 4;                              // [8 pieces][32 values][128 threads]
+constexpr size_t PG_SMEM = 1024 + (size_t)PG_STAGES * PG_STAGE_BYTES + PG_ACC_BYTES + 512;
 
 __device__ __forceinline__ uint32_t pg_smem(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 __device__ __forceinline__ void pg_mbar_init(uint64_t* bar, uint32_t count) {
@@ -63,33 +69,7 @@ __device__ __forceinline__ bool pg_elect() {
     return pred != 0;
 }
 __device__ __forceinline__ uint64_t pg_desc(uint32_t smem_addr) {      // K-major, SWIZZLE_128B
-    uint64_t d = 0;
-    d |= (uint64_t)((smem_addr & 0x3FFFF) >> 4);
-    d |= (uint64_t)(1024 >> 4) << 32;
-    d |= (uint64_t)1 << 46;
-    d |= (uint64_t)2 << 61;
-    return d;
-}
-__device__ __forceinline__ void pg_umma(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t acc) {
-    asm volatile(
-        "{\n\t"
-        ".reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t"
-        "}" ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(acc)
-        : "memory");
-}
-__device__ __forceinline__ void pg_commit(uint64_t* bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(pg_smem(bar))
-                 : "memory");
-}
-__device__ __forceinline__ void pg_tmem_ld16(uint32_t taddr, uint32_t* r) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-          "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-        : "r"(taddr)
-        : "memory");
+    return tfy_wg_desc(smem_addr, 16, 1024, TFY_WG_SW128);
 }
 __device__ __forceinline__ float4 pg_ld_peer(const float* p) {
     float4 v;
@@ -113,11 +93,10 @@ tfy_ps_gather_gemm_kernel(const __grid_constant__ CUtensorMap map_w, const uint6
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
     uint8_t* ring = smem;
-    uint64_t* full_a = reinterpret_cast<uint64_t*>(ring + (size_t)PG_STAGES * PG_STAGE_BYTES);
+    float* acc_s = reinterpret_cast<float*>(ring + (size_t)PG_STAGES * PG_STAGE_BYTES);
+    uint64_t* full_a = reinterpret_cast<uint64_t*>(reinterpret_cast<uint8_t*>(acc_s) + PG_ACC_BYTES);
     uint64_t* full_b = full_a + PG_STAGES;
     uint64_t* empty = full_b + PG_STAGES;
-    uint64_t* acc_full = empty + PG_STAGES;
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(acc_full + 1);
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int b0 = blockIdx.x * PG_BM, n0 = blockIdx.y * PG_BN;
@@ -127,24 +106,14 @@ tfy_ps_gather_gemm_kernel(const __grid_constant__ CUtensorMap map_w, const uint6
         for (int s = 0; s < PG_STAGES; ++s) {
             pg_mbar_init(&full_a[s], PG_PROD_THREADS);
             pg_mbar_init(&full_b[s], 1);
-            pg_mbar_init(&empty[s], 1);
+            pg_mbar_init(&empty[s], 4);        // one arrival per MMA warp
         }
-        pg_mbar_init(acc_full, 1);
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
-    if (warp == 1) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(pg_smem(tmem_slot)),
-                     "r"(256)
-                     : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
     __syncthreads();
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    const uint32_t tmem_base = *tmem_slot;
     tfy_pdl_sync();
 
-    if (warp == 0) {
+    if (warp == PG_TMA_WARP) {
         // ===== weights: the ps rank's bf16 shadow, two 128-row boxes per 64-column chunk =====
         if (pg_elect()) {
             for (int c = 0; c < n_chunks; ++c) {
@@ -156,28 +125,56 @@ tfy_ps_gather_gemm_kernel(const __grid_constant__ CUtensorMap map_w, const uint6
                 pg_tma_load(&map_w, &full_b[s], b_dst + PG_B_BYTES / 2, c * PG_BK, n0 + 128);
             }
         }
-    } else if (warp == 1) {
-        if (pg_elect()) {
-            const uint32_t idesc = (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(PG_BN >> 3) << 17) |
-                                   ((uint32_t)(PG_BM >> 4) << 24);
-            for (int c = 0; c < n_chunks; ++c) {
-                const int s = c % PG_STAGES;
-                const uint32_t ph = (c / PG_STAGES) & 1;
-                pg_mbar_wait(&full_a[s], ph);
-                pg_mbar_wait(&full_b[s], ph);
-                asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-                const uint32_t a_addr = pg_smem(ring + (size_t)s * PG_STAGE_BYTES);
-                const uint64_t adesc = pg_desc(a_addr), bdesc = pg_desc(a_addr + PG_A_BYTES);
+    } else if (warp >= PG_MMA_WARP) {
+        // ===== wgmma: piece q = (64-row half q / 4, 64-column quarter q % 4); accumulator word (q, i) of thread t at
+        // acc_s[(q * 32 + i) * 128 + t] =====
+        const int t = (int)threadIdx.x - PG_MMA_WARP * 32;
+        float* mine = acc_s + t;
+        for (int i = 0; i < 8 * 32; ++i) mine[i * 128] = 0.f;
+        for (int c = 0; c < n_chunks; ++c) {
+            const int s = c % PG_STAGES;
+            const uint32_t ph = (c / PG_STAGES) & 1;
+            pg_mbar_wait(&full_a[s], ph);
+            pg_mbar_wait(&full_b[s], ph);
+            const uint32_t a_addr = pg_smem(ring + (size_t)s * PG_STAGE_BYTES), b_addr = a_addr + PG_A_BYTES;
+#pragma unroll 1
+            for (int q = 0; q < 8; ++q) {
+                float d[32];
+                const uint64_t adesc = pg_desc(a_addr + (q >> 2) * 64 * 128);
+                const uint64_t bdesc = pg_desc(b_addr + (q & 3) * 64 * 128);
+                tfy_wg_fence();
 #pragma unroll
                 for (int k = 0; k < PG_BK / 16; ++k)
-                    pg_umma(tmem_base, adesc + (uint64_t)(2 * k), bdesc + (uint64_t)(2 * k), idesc, (c > 0 || k > 0) ? 1u : 0u);
-                pg_commit(&empty[s]);
+                    tfy_wgmma_m64n64<0, 0>(d, adesc + (uint64_t)(2 * k), bdesc + (uint64_t)(2 * k), k > 0 ? 1u : 0u);
+                tfy_wg_commit();
+                tfy_wg_wait<0>();
+                float* acc_q = mine + q * 32 * 128;
+#pragma unroll
+                for (int i = 0; i < 32; ++i) acc_q[i * 128] += d[i];
             }
-            pg_commit(acc_full);
+            if (lane == 0) pg_mbar_arrive(&empty[s]);
+        }
+        // ===== epilogue: bias, bf16 pairs (fragment layout: row 16 w + l / 4 (+8), column 8 j + 2 (l % 4)) =====
+        const int w = t >> 5;
+#pragma unroll 1
+        for (int q = 0; q < 8; ++q) {
+            const float* acc_q = mine + q * 32 * 128;
+#pragma unroll 4
+            for (int i = 0; i < 32; i += 2) {
+                const int ob = b0 + (q >> 2) * 64 + 16 * w + (lane >> 2) + 8 * ((i >> 1) & 1);
+                const int n = n0 + (q & 3) * 64 + 8 * (i >> 2) + 2 * (lane & 3);
+                if (ob >= B || n >= N) continue;                 // N % 8 == 0: n < N covers n + 1
+                float v0 = acc_q[i * 128], v1 = acc_q[(i + 1) * 128];
+                if (bias) {
+                    v0 += __bfloat162float(bias[n]);
+                    v1 += __bfloat162float(bias[n + 1]);
+                }
+                *reinterpret_cast<__nv_bfloat162*>(y + (size_t)ob * N + n) = __floats2bfloat162_rn(v0, v1);
+            }
         }
     } else {
         // ===== A-tile producers: 4 threads per sample; thread (r, p) owns columns [16 p, 16 p + 16) of every chunk =====
-        const int pt = (int)threadIdx.x - 64;
+        const int pt = (int)threadIdx.x;
         const int r = pt >> 2, p = pt & 3;
         const int b = b0 + r;
         const bool live = b < B;
@@ -233,37 +230,6 @@ tfy_ps_gather_gemm_kernel(const __grid_constant__ CUtensorMap map_w, const uint6
                 }
             }
         }
-        if (warp >= 6) goto pg_done;                     // warps 2-5 go on to the epilogue
-        // ===== epilogue: bias, bf16, row-contiguous 16-byte stores =====
-        const int quad = warp & 3;
-        const int row = quad * 32 + lane;                 // TMEM lane == accumulator row of this thread
-        const int ob = b0 + row;
-        pg_mbar_wait(acc_full, 0);
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-#pragma unroll 1
-        for (int cc = 0; cc < PG_BN; cc += 16) {
-            uint32_t acc[16];
-            pg_tmem_ld16(tmem_base + ((uint32_t)(quad * 32) << 16) + (uint32_t)cc, acc);
-            asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-            const int n = n0 + cc;
-            if (ob >= B || n >= N) continue;
-            float v[16];
-#pragma unroll
-            for (int j = 0; j < 16; ++j) v[j] = __uint_as_float(acc[j]) + ((bias && n + j < N) ? __bfloat162float(bias[n + j]) : 0.f);
-            __nv_bfloat16* dst = y + (size_t)ob * N + n;
-            if (n + 16 <= N) {
-                tfy_st16(dst, TfyPack<__nv_bfloat16>::pack(v));
-                tfy_st16(dst + 8, TfyPack<__nv_bfloat16>::pack(v + 8));
-            } else {
-                for (int j = 0; j < 16 && n + j < N; ++j) dst[j] = __float2bfloat16(v[j]);
-            }
-        }
-    }
-pg_done:
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    __syncthreads();
-    if (warp == 1) {
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(256) : "memory");
     }
 }
 

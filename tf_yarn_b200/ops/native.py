@@ -1,4 +1,4 @@
-"""ctypes bindings of ``libtfy_b200.so`` (the sm_100a kernel library).
+"""ctypes bindings of ``libtfy_b200.so`` (the sm_90a kernel library).
 
 The library is built in-tree by :mod:`tf_yarn_b200.ops.build`.  On a machine
 with a GPU a missing/unloadable library is a hard error: the kernels ARE the

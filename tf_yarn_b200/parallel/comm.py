@@ -1,4 +1,4 @@
-"""Collectives over the symmetric arena (hand-written sm_100a kernels, no NCCL).
+"""Collectives over the symmetric arena (hand-written sm_90a kernels, no NCCL).
 
 ``Communicator`` is the data plane behind the Horovod-like facade
 (:mod:`tf_yarn_b200.hvd`), the DDP-like wrapper
@@ -22,7 +22,7 @@ _DT = {torch.bfloat16: native.BF16, torch.float32: native.F32}
 
 # below this many bytes the latency-optimal one-shot kernel wins (one barrier
 # pair + every rank reads everything); above it the 2-phase kernels move 1/N of
-# the data per rank.  Tuned on 8xB200, see profiles/.
+# the data per rank.
 ONESHOT_MAX_BYTES = 128 * 1024
 
 

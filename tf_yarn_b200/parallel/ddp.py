@@ -394,7 +394,7 @@ class _FusedOptimizer:
 
 
 def wrap_model(model: nn.Module, device, ddp_kwargs: Optional[dict] = None, comm: Optional[Communicator] = None):
-    """Data-parallel wrapper appropriate for the process: ours on B200, torch DDP on CPU/gloo."""
+    """Data-parallel wrapper appropriate for the process: ours on H100, torch DDP on CPU/gloo."""
     import torch.distributed as dist
     ddp_kwargs = dict(ddp_kwargs or {})
     on_gpu = isinstance(device, int) or torch.device(device).type == "cuda"

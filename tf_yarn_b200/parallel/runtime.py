@@ -14,7 +14,7 @@ def get_communicator(rdv=None, device: Optional[int] = None):
 
     Sizes: ``TFY_ARENA_MB`` (default 2048) of symmetric HBM for flat parameter /
     gradient buffers, ``TFY_FUSION_MB`` (default 64) for the Horovod-style fusion
-    buffer.  B200 has 180 GB of HBM3e; the defaults fit BERT-base fp32 grads
+    buffer.  H100 has 80 GB of HBM3; the defaults fit BERT-base fp32 grads
     (440 MB) with room to spare.
     """
     global _comm

@@ -116,7 +116,7 @@ class SymmArena:
     def __init__(self, size_bytes: int, device: Optional[int] = None, rdv: Optional[Rendezvous] = None,
                  timeout_s: float = 120.0):
         if not torch.cuda.is_available():
-            raise RuntimeError("SymmArena needs a CUDA device (B200)")
+            raise RuntimeError("SymmArena needs a CUDA device (H100)")
         self.lib = native.load()
         self.rdv = rdv if rdv is not None else default_rendezvous()
         self.rank, self.world = self.rdv.rank, self.rdv.world

@@ -6,7 +6,7 @@ the KV store, ``init_process_group``, wrap the model for data-parallel
 training, build the rank's dataloader, call the user's ``main_fn(model,
 trainloader, device, rank, tb_writer)``, collect the TensorBoard event files.
 
-B200 specifics:
+H100 specifics:
 
 * one process per GPU; the GPU index comes from the launcher's placement
   (``TFY_GPU_IDS``), not from ``local_index % n_gpus``;
@@ -98,7 +98,7 @@ def _assigned_gpus() -> List[int]:
 
 
 def _get_device(worker_id: int) -> Optional[int]:
-    """B200 index for local process ``worker_id``; None means CPU."""
+    """H100 index for local process ``worker_id``; None means CPU."""
     if not torch.cuda.is_available():
         return None
     ids = _assigned_gpus()

@@ -3,7 +3,7 @@
 Every cluster task publishes ``<task>/init = "host:port"`` and waits for all the others
 (the INIT barrier); the aggregated addresses become ``TF_CONFIG``, from which the Estimator
 facade derives its role.  There is no gRPC server to start: the ps data plane is direct
-memory access (shared memory on CPU, peer HBM over NVLink on B200), so ``start_tf_server``
+memory access (shared memory on CPU, peer HBM over NVLink on H100), so ``start_tf_server``
 only records the role.
 """
 from __future__ import annotations

@@ -3,8 +3,8 @@
 API parity with the reference (reference: tf_yarn/topologies.py:7-160) --
 ``TaskSpec``, ``NodeLabel``, ``ContainerKey``, ``ContainerTask``,
 ``single_server_topology``, ``ps_strategy_topology`` -- re-targeted at ONE
-8xB200 NVSwitch box: a ``NodeLabel.GPU`` task instance is pinned to
-``nb_proc_per_worker`` B200s by the local launcher instead of being a YARN
+8xH100 NVSwitch box: a ``NodeLabel.GPU`` task instance is pinned to
+``nb_proc_per_worker`` H100s by the local launcher instead of being a YARN
 container on a ``gpu``-labelled node.
 """
 from __future__ import annotations
@@ -54,7 +54,7 @@ def parse_memory(value: Union[int, str]) -> int:
 
 
 class NodeLabel(Enum):
-    """Where a task instance runs: host CPU only, or pinned to B200 GPU(s)."""
+    """Where a task instance runs: host CPU only, or pinned to H100 GPU(s)."""
     CPU = ""
     GPU = "gpu"
 
@@ -183,7 +183,7 @@ def ps_strategy_topology(nb_workers: int = 2, nb_ps: int = 1, memory: Union[int,
 def allreduce_topology(nb_workers: int = 8, memory: Union[int, str] = MAX_MEMORY_CONTAINER,
                        vcores: int = MAX_VCORES_CONTAINER, label: NodeLabel = NodeLabel.GPU,
                        with_evaluator: bool = True, with_tensorboard: bool = False) -> Dict[str, TaskSpec]:
-    """chief + (nb_workers - 1) workers, one B200 each: the synchronous all-reduce layout
+    """chief + (nb_workers - 1) workers, one H100 each: the synchronous all-reduce layout
     (the reference builds this by hand in native_keras_with_gloo_example.py:98-104)."""
     if nb_workers < 1:
         raise ValueError("nb_workers must be >= 1")

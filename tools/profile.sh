@@ -6,7 +6,7 @@ OUT=gpurun_out
 mkdir -p $OUT
 ncu --profile-from-start off --metrics gpu__time_duration.sum --clock-control none --cache-control none --csv \
     --log-file $OUT/launches.csv python tests/gpu/profile_step.py
-# every tcgen05 kernel of the step + the fused optimizer/collective kernel, one capture each
+# every wgmma kernel of the step + the fused optimizer/collective kernel, one capture each
 PROFILE_STEPS=1 ncu --set full --clock-control none --import-source on --profile-from-start off \
     -k regex:"tfy_conv3x3|tfy_dense|tfy_gemm|tfy_fused_step" -f -o $OUT/prof_step_kernels \
     python tests/gpu/profile_step.py

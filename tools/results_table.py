@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""Collect the bench JSON lines under profiles/r2/ into markdown tables (README "Results").
+"""Collect bench JSON lines (one file per run, as printed by bench.py) into markdown tables (README "Results").
 
-    python tools/results_table.py            # prints the tables
+    python tools/results_table.py DIR        # prints the tables of DIR/bench_*.json
 Files are named bench_<config>_<impl>_N<n>_<tag>.json (one JSON object each, as printed by bench.py).
 """
 import glob
@@ -13,9 +13,9 @@ import sys
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
-def load():
+def load(results_dir):
     rows = {}
-    for f in sorted(glob.glob(os.path.join(ROOT, "profiles", "r2", "bench_*.json"))):
+    for f in sorted(glob.glob(os.path.join(results_dir, "bench_*.json"))):
         m = re.match(r"bench_(.+?)_N(\d+)_(\w+)\.json", os.path.basename(f))
         if not m:
             continue
@@ -57,7 +57,9 @@ def table(rows, config, arms, unit):
 
 
 def main():
-    rows = load()
+    if len(sys.argv) != 2:
+        sys.exit("usage: results_table.py DIR")
+    rows = load(sys.argv[1])
     print("### Headline: Keras MNIST-CNN, Horovod path (samples/s)\n")
     print(table(rows, "mnist", ["ours", "standin_graph", "reference"], "samples/s"))
     base = rows.get(("mnist_ours", 1))

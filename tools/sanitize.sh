@@ -1,5 +1,5 @@
 #!/usr/bin/env bash
-# Race / memory checking of the single-GPU kernels (run on a B200 through gpurun):
+# Race / memory checking of the single-GPU kernels (run on an H100):
 #   gpurun --timeout 1500 -- tools/sanitize.sh          (SAN_TIMEOUT=<s> bounds each run; rc=124 = cut off, not an error)
 # Writes gpurun_out/sanitizer_<tool>_<suite>.log plus a one-line-per-run summary (sanitizer_summary.txt) and
 # FAILS (exit 1) when a tool reports an error.  The reference has no sanitizer usage at all (SURVEY.md §5.2).
@@ -22,7 +22,7 @@ run() {  # tool suite command...
   echo "$tool $suite rc=$rc :: ${verdict:-no summary line}" | tee -a "$SUMMARY"
   if [ $rc -ne 0 ] && [ $rc -ne 124 ]; then status=1; fi
 }
-K="nn_kernels or fused_step_local or tcgen05 or dense_head or dense_backward"
+K="nn_kernels or fused_step_local or wgmma or dense_head or dense_backward"
 run memcheck  engine python -m pytest tests/test_gpu_engine.py -m gpu -q -x -k "$K"
 run racecheck engine python -m pytest tests/test_gpu_engine.py -m gpu -q -x -k "$K"
 run memcheck  conv   python tests/gpu/conv_check.py 2

@@ -2,7 +2,6 @@
 # Validation of programmatic dependent launch for every kernel (TFY_PDL=1) before making it the default:
 #   gpurun --timeout 900 -- tools/validate_pdl.sh 1 TAG          # one GPU: GPU test-suite + A/B bench
 #   gpurun --gpus N --timeout 900 -- tools/validate_pdl.sh N TAG # N GPUs: comm / DDP checks + A/B bench (params_in_sync)
-# Round 2 measured 78.2 vs 84.0 us/step on one GPU (profiles/r2/README.md) but had no GPU time left for this.
 set -uo pipefail
 N=${1:-1}; TAG=${2:-pdl}; OUT=gpurun_out; mkdir -p $OUT
 R="python -m torch.distributed.run --nnodes=1 --nproc-per-node $N --master-addr 127.0.0.1"
