@@ -28,6 +28,9 @@ from typing import Callable, Dict, List, Optional, Sequence, Tuple
 import torch
 import torch.nn as nn
 
+from tf_yarn_b200.keras import losses as loss_mod
+from tf_yarn_b200.keras import weighting
+
 logger = logging.getLogger(__name__)
 
 
@@ -43,13 +46,21 @@ class EagerTrainEngine:
     """Reference-semantics engine for CPU (and the fp32 numerics oracle for the graph engine)."""
 
     def __init__(self, net: nn.Module, loss_fn: Callable, optimizer, metric_fns: Sequence[Tuple[str, Callable]],
-                 device: torch.device, distributed: bool = False):
+                 device: torch.device, distributed: bool = False,
+                 weighted_metric_fns: Sequence[Tuple[str, Callable]] = ()):
         self.net, self.loss_fn, self.metric_fns = net, loss_fn, list(metric_fns)
+        self.weighted_metric_fns = list(weighted_metric_fns)
         self.device = device
         self.distributed = distributed
         self.opt_desc = optimizer
         self.opt = optimizer.to_torch([p for p in net.parameters() if p.requires_grad])
         self.kernel_launches = 0
+        self._cw = None                     # class-weight table [C] on the device (None: no class_weight)
+        self._wacc = [[0.0, 0.0] for _ in self.weighted_metric_fns]     # epoch sums (sum w*m, sum w)
+
+    def set_class_weight(self, table: Optional[torch.Tensor]) -> None:
+        """Class-weight table of the following steps (None: off)."""
+        self._cw = table.to(self.device, torch.float32).reshape(-1) if table is not None else None
 
     # -- distributed helpers (gloo) -------------------------------------------
     def _world(self) -> int:
@@ -62,13 +73,18 @@ class EagerTrainEngine:
             for t in list(self.net.parameters()) + list(self.net.buffers()):
                 dist.broadcast(t.data, src=root)
 
-    def train_step(self, x, y) -> Dict[str, torch.Tensor]:
+    def train_step(self, x, y, w=None) -> Dict[str, torch.Tensor]:
         import torch.distributed as dist
         self.net.train()
         x, y = _to_device_batch(x, self.device), _to_device_batch(y, self.device)
         self.opt.zero_grad(set_to_none=False)
         out = self.net(x)
-        loss = self.loss_fn(y, out)
+        sw = None
+        if w is None and self._cw is None:
+            loss = self.loss_fn(y, out)
+        else:
+            sw = weighting.sample_weights(y, w.to(self.device) if w is not None else None, self._cw)
+            loss = weighting.weighted_loss(loss_mod.per_sample(self.loss_fn), y, out, sw)
         loss.backward()
         world = self._world()
         if world > 1:
@@ -86,7 +102,17 @@ class EagerTrainEngine:
             for name, fn in self.metric_fns:
                 num, den = fn(y, out)
                 logs[name] = num / den
+            for acc, (_, fn) in zip(self._wacc, self.weighted_metric_fns):
+                num, den = fn(y, out, sample_weight=sw)
+                acc[0] += float(num)
+                acc[1] += float(den)
         return logs
+
+    def pop_metrics(self) -> Dict[str, float]:
+        """The weighted metrics of the steps since the last call, ``sum(w*m) / sum(w)`` over all of them."""
+        out = {name: (num / den if den else 0.0) for (name, _), (num, den) in zip(self.weighted_metric_fns, self._wacc)}
+        self._wacc = [[0.0, 0.0] for _ in self.weighted_metric_fns]
+        return out
 
     def set_learning_rate(self, lr: float) -> None:
         for g in self.opt.param_groups:
@@ -116,10 +142,12 @@ class GraphTrainEngine:
 
     def __init__(self, net: nn.Module, loss_fn: Callable, optimizer, metric_fns: Sequence[Tuple[str, Callable]],
                  device: torch.device, distributed: bool, example_x, example_y,
-                 compute_dtype: torch.dtype = torch.bfloat16, use_graph: bool = True, comm=None):
+                 compute_dtype: torch.dtype = torch.bfloat16, use_graph: bool = True, comm=None,
+                 weighted_metric_fns: Sequence[Tuple[str, Callable]] = ()):
         from tf_yarn_b200.parallel import runtime
         from tf_yarn_b200.parallel.comm import FusedShardedOptimizer
         self.net, self.loss_fn, self.metric_fns = net, loss_fn, list(metric_fns)
+        self.weighted_metric_fns = list(weighted_metric_fns)
         self.device = device
         self.compute_dtype = compute_dtype
         self.use_graph = use_graph
@@ -157,11 +185,36 @@ class GraphTrainEngine:
         self._slot = 0
         self._slot_free = [None, None]  # event: the step that read staging[slot] has copied it out
         self._loss = torch.zeros((), dtype=torch.float32, device=device)
-        self._metric_acc = torch.zeros(max(1, len(self.metric_fns)), 2, dtype=torch.float32, device=device)
+        # rows: the metrics, then the weighted metrics (sum w*m, sum w)
+        self._metric_acc = torch.zeros(max(1, len(self.metric_fns) + len(self.weighted_metric_fns)), 2,
+                                       dtype=torch.float32, device=device)
         self._example = (example_x, example_y)
         self.kernel_launches = 0
         self._launches_per_step = 1          # the fused K4 kernel
         self._captured = False
+        # Keras sample weighting.  The weighting mode -- (class_weight, sample_weight) -- is part of the captured
+        # graphs: a step in another mode captures them again.  The class-weight table is an engine-owned device
+        # buffer read by the graphs, so a new table of the same size is copied in place without a recapture;
+        # sample weights get a [B] buffer per staging slot.
+        self._cw: Optional[torch.Tensor] = None
+        self._cw_on = False
+        self._wmode = (False, False)
+        self._staging_w = [None, None]
+
+    def set_class_weight(self, table: Optional[torch.Tensor]) -> None:
+        """Class-weight table ``[C]`` of the following steps (None: off)."""
+        if table is None:
+            self._cw_on = False
+            return
+        table = table.to(torch.float32).reshape(-1)
+        if self._cw is None or self._cw.numel() != table.numel():
+            if self._wmode[0]:
+                self._captured = False       # the graphs read the old buffer
+            self._cw = torch.empty(table.numel(), dtype=torch.float32, device=self.device)
+        with torch.cuda.stream(self.stream):  # ordered after the steps already queued, before the next ones
+            self._cw.copy_(table)
+        self.stream.synchronize()
+        self._cw_on = True
 
     # ------------------------------------------------------------------ variables
     def broadcast_variables(self, root: int = 0) -> None:
@@ -186,12 +239,17 @@ class GraphTrainEngine:
         pass  # module parameters ARE the flat buffer
 
     # ------------------------------------------------------------------ step body
-    def _forward_backward(self, x, y) -> None:
+    def _forward_backward(self, x, y, w=None) -> None:
         xin = x
         if torch.is_tensor(xin) and torch.is_floating_point(xin):
             xin = xin.to(self.compute_dtype)
         out = self.net(xin)
-        loss = self.loss_fn(y, out)
+        sw = None
+        if self._wmode == (False, False):
+            loss = self.loss_fn(y, out)
+        else:
+            sw = weighting.sample_weights(y, w, self._cw if self._wmode[0] else None)
+            loss = weighting.weighted_loss(loss_mod.per_sample(self.loss_fn), y, out, sw)
         loss.backward()
         self._loss.copy_(loss.detach())
         if self.metric_fns:
@@ -200,15 +258,25 @@ class GraphTrainEngine:
                     num, den = fn(y, out)
                     self._metric_acc[i, 0] += num
                     self._metric_acc[i, 1] += den
+        if self.weighted_metric_fns:
+            with torch.no_grad():
+                for i, (_, fn) in enumerate(self.weighted_metric_fns, start=len(self.metric_fns)):
+                    num, den = fn(y, out, sample_weight=sw)
+                    self._metric_acc[i, 0] += num
+                    self._metric_acc[i, 1] += den
         self.fused.step()
 
-    def _capture(self, x, y) -> None:
+    def _capture(self, x, y, w=None) -> None:
         self.net.train()
         # two input slots, and one captured graph per slot reading it in place: the copy stream fills slot
         # (i+1) % 2 while graph[i % 2] runs, and no staging -> static copy sits in front of every step
         self._staging = [(_clone_struct(x), _clone_struct(y)) for _ in range(2)]
         self._static_x, self._static_y = self._staging[0]
-        self._loss_host = [torch.zeros((), dtype=torch.float32).pin_memory() for _ in range(2)]
+        self._wmode = (self._cw_on, w is not None)
+        self._staging_w = [w.reshape(-1).float().clone() if w is not None else None for _ in range(2)]
+        if getattr(self, "_loss_host", None) is None:
+            # (a recapture keeps them: the loss of the step queued before it is still to be read)
+            self._loss_host = [torch.zeros((), dtype=torch.float32).pin_memory() for _ in range(2)]
         self._loss_in_host = [False, False]
         self._capture_slot = None
         self._ready_ev = [torch.cuda.Event() for _ in range(2)]
@@ -223,7 +291,7 @@ class GraphTrainEngine:
         self.stream.wait_stream(torch.cuda.current_stream())
         with torch.cuda.stream(self.stream):
             for _ in range(3):
-                self._forward_backward(self._static_x, self._static_y)
+                self._forward_backward(self._static_x, self._static_y, self._staging_w[0])
         self.stream.synchronize()
         self.graphs = [None, None]
         if self.use_graph:
@@ -237,11 +305,12 @@ class GraphTrainEngine:
                 for slot in range(2):
                     g = torch.cuda.CUDAGraph()
                     sx, sy = self._staging[slot]
+                    sw = self._staging_w[slot]
                     # the graphs never run concurrently (same stream), so they share one memory pool
                     pool = self.graphs[0].pool() if slot else None
                     self._capture_slot = slot
                     with torch.cuda.graph(g, stream=self.stream, pool=pool):
-                        self._forward_backward(sx, sy)
+                        self._forward_backward(sx, sy, sw)
                         if not self._loss_in_host[slot]:      # (the fast path's head kernel writes it itself)
                             self._loss_host[slot].copy_(self._loss, non_blocking=True)     # D2H node of the graph
                     self._capture_slot = None
@@ -262,35 +331,45 @@ class GraphTrainEngine:
         self._captured = True
 
     # ------------------------------------------------------------------ public
-    def ensure_captured(self, x, y) -> None:
+    def ensure_captured(self, x, y, w=None) -> None:
+        if self._captured and self._wmode != (self._cw_on, w is not None):
+            self._captured = False          # another weighting mode: capture the step graphs again
         if not self._captured:
-            self._capture(_to_device_batch(x, self.device, False), _to_device_batch(y, self.device, False))
+            self._capture(_to_device_batch(x, self.device, False), _to_device_batch(y, self.device, False),
+                          w.to(self.device) if w is not None else None)
 
-    def stage_inputs(self, x, y):
-        """Asynchronous copy (H2D from pinned memory, or D2D) of the next batch into a staging slot.
+    def stage_inputs(self, x, y, w=None):
+        """Asynchronous copy (H2D from pinned memory, or D2D) of the next batch -- and of its sample weights
+        ``w`` [B], if any -- into a staging slot.
 
         Runs on the copy stream, so it overlaps the step that is currently executing.  Returns a
         ticket for :meth:`launch_step`.
         """
-        self.ensure_captured(x, y)
+        self.ensure_captured(x, y, w)
         slot = self._slot
         self._slot ^= 1
         sx, sy = self._staging[slot]
+        sw = self._staging_w[slot]
         cs = self.copy_stream
         free = self._slot_free[slot]
         if free is not None:
             cs.wait_event(free)
         if (self._fast_copy and torch.is_tensor(x) and torch.is_tensor(y) and x.dtype == sx.dtype
                 and y.dtype == sy.dtype and x.is_contiguous() and y.is_contiguous()
-                and x.numel() == sx.numel() and y.numel() == sy.numel()):
-            # hot path: two cudaMemcpyAsync calls through ctypes, no stream context manager
+                and x.numel() == sx.numel() and y.numel() == sy.numel()
+                and (w is None or (w.dtype == sw.dtype and w.is_contiguous() and w.numel() == sw.numel()))):
+            # hot path: two cudaMemcpyAsync calls through ctypes, no stream context manager (three with weights)
             lib, sp = self._lib, cs.cuda_stream
             lib.tfy_memcpy_async(sx.data_ptr(), x.data_ptr(), x.numel() * x.element_size(), sp)
             lib.tfy_memcpy_async(sy.data_ptr(), y.data_ptr(), y.numel() * y.element_size(), sp)
+            if w is not None:
+                lib.tfy_memcpy_async(sw.data_ptr(), w.data_ptr(), w.numel() * w.element_size(), sp)
         else:
             with torch.cuda.stream(cs):
                 _copy_struct(sx, x)
                 _copy_struct(sy, y)
+                if w is not None:
+                    sw.copy_(w.reshape(-1), non_blocking=True)
         ev = self._ready_ev[slot]
         ev.record(cs)
         return slot, ev
@@ -318,7 +397,7 @@ class GraphTrainEngine:
             self.graphs[slot].replay()
         else:
             sx, sy = self._staging[slot]
-            self._forward_backward(sx, sy)
+            self._forward_backward(sx, sy, self._staging_w[slot])
             self._loss_host[slot].copy_(self._loss, non_blocking=True)
 
     def loss_host(self, slot: int) -> torch.Tensor:
@@ -329,9 +408,9 @@ class GraphTrainEngine:
         with torch.cuda.stream(self.stream):
             pinned_slot.copy_(self._loss, non_blocking=True)
 
-    def train_step(self, x, y) -> Dict[str, torch.Tensor]:
+    def train_step(self, x, y, w=None) -> Dict[str, torch.Tensor]:
         """Synchronous convenience wrapper (tests, smoke): one step, returns device scalars."""
-        ticket = self.stage_inputs(x, y)
+        ticket = self.stage_inputs(x, y) if w is None else self.stage_inputs(x, y, w)
         self.launch_step(ticket)
         self.stream.synchronize()
         return {"loss": self._loss.clone()}
@@ -340,7 +419,10 @@ class GraphTrainEngine:
         self.stream.synchronize()
         acc = self._metric_acc.cpu()
         self._metric_acc.zero_()
-        return {name: float(acc[i, 0] / acc[i, 1].clamp_min(1)) for i, (name, _) in enumerate(self.metric_fns)}
+        out = {name: float(acc[i, 0] / acc[i, 1].clamp_min(1)) for i, (name, _) in enumerate(self.metric_fns)}
+        for i, (name, _) in enumerate(self.weighted_metric_fns, start=len(self.metric_fns)):
+            out[name] = float(acc[i, 0] / acc[i, 1]) if float(acc[i, 1]) != 0.0 else 0.0
+        return out
 
     def set_learning_rate(self, lr: float) -> None:
         with torch.cuda.stream(self.stream):

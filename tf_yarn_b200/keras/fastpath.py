@@ -44,6 +44,7 @@ native.declare("tfy_act_drop_bwd_bias", [_vp, _vp, _vp, _vp, _f, _sz, _i, _vp, _
 native.declare("tfy_bias_relu_pool_drop_fwd", [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _f, _u32, _vp, _vp])
 native.declare("tfy_pool_drop_relu_bwd", [_vp, _vp, _vp, _f, _i, _i, _i, _i, _vp, _vp, _vp, _vp])
 native.declare("tfy_softmax_xent", [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _vp])
+native.declare("tfy_softmax_xent_weighted", [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _vp])
 native.declare("tfy_conv3x3_c32_pool_fwd", [_vp, _vp, _vp, _vp, _vp, _i, _i, _i, _f, _u32, _vp, _vp])
 native.declare("tfy_conv3x3_c32_dgrad", [_vp, _vp, _vp, _vp, _i, _i, _i, _vp])
 native.declare("tfy_conv3x3_c32_wgrad", [_vp, _vp, _vp, _vp, _vp, _i, _i, _i, _vp])
@@ -59,6 +60,8 @@ native.declare("tfy_gemm_bf16_splitk_fused", [_vp, _vp, _vp, _vp, _vp, _vp, _vp,
 native.declare("tfy_dense_head_scratch_elems", [_i, _i, _i], restype=ctypes.c_size_t)
 native.declare("tfy_dense_head_fused", [_vp, _vp, _vp, _vp, _vp, _f, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i,
                                         _i, _vp])
+native.declare("tfy_dense_head_fused_weighted", [_vp, _vp, _vp, _vp, _vp, _f, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp,
+                                                 _vp, _i, _i, _i, _vp, _vp, _vp])
 
 PARTIAL_BLOCKS = 592
 
@@ -86,6 +89,10 @@ def build_plan(model) -> Optional[List[_Stage]]:
     for m in model._metrics_spec:
         if m not in ("accuracy", "acc", "sparse_categorical_accuracy"):
             return None
+    # the head kernel counts the (weighted) hits: one weighted accuracy at most
+    weighted = getattr(model, "_weighted_metrics_spec", [])
+    if len(weighted) > 1 or any(m not in ("accuracy", "acc", "sparse_categorical_accuracy") for m in weighted):
+        return None
     layers = [ly for ly in model.layers if not isinstance(ly, L.InputLayer)]
     plan: List[_Stage] = []
     i, n = 0, len(layers)
@@ -166,7 +173,7 @@ class FastSequentialEngine(GraphTrainEngine):
                 width = max(width, st.layer.units)
         self._partial = torch.zeros(PARTIAL_BLOCKS * width, dtype=torch.float32, device=dev)
         self._counter = torch.zeros(1, dtype=torch.int32, device=dev)
-        self._stats = torch.zeros(2, dtype=torch.float32, device=dev)
+        self._stats = torch.zeros(4, dtype=torch.float32, device=dev)     # hits, rows (, sum w*hit, sum w: weighted)
         self._seed = int(torch.initial_seed() & 0x7fffffff)
         self._hp = self.fused.hyper.data_ptr()
         self._k = 0
@@ -275,19 +282,33 @@ class FastSequentialEngine(GraphTrainEngine):
         self.stream.synchronize()
         st = self._stats.cpu()
         self._stats.zero_()
-        if not self.metric_fns:
-            return {}
-        return {self.metric_fns[0][0]: float(st[0] / st[1].clamp_min(1))}
+        out = {}
+        if self.metric_fns:
+            out[self.metric_fns[0][0]] = float(st[0] / st[1].clamp_min(1))
+        if self.weighted_metric_fns:
+            if self._wmode == (False, False):        # every weight is 1
+                out[self.weighted_metric_fns[0][0]] = float(st[0] / st[1].clamp_min(1))
+            else:
+                out[self.weighted_metric_fns[0][0]] = float(st[2] / st[3]) if float(st[3]) != 0.0 else 0.0
+        return out
 
-    def _capture(self, x, y) -> None:
-        super()._capture(x, y)
+    def _stats_ptr(self):
+        return self._stats.data_ptr() if (self.metric_fns or self.weighted_metric_fns) else None
+
+    def _weight_ptrs(self, sw):
+        """(sample weights, class-weight table, stream) arguments of the weighted head kernels."""
+        return (sw.data_ptr() if sw is not None else None, self._cw.data_ptr() if self._wmode[0] else None,
+                self._s())
+
+    def _capture(self, x, y, w=None) -> None:
+        super()._capture(x, y, w)
         with torch.cuda.stream(self.stream):
             self._stats.zero_()          # warm-up steps must not count in the epoch metrics
         self.stream.synchronize()
 
     # ------------------------------------------------------------------ the step
     @torch.no_grad()
-    def _forward_backward(self, x, y) -> None:
+    def _forward_backward(self, x, y, sw=None) -> None:
         lib, s = self.lib, self._s()
         self._k = 0
         B = x.shape[0]
@@ -439,13 +460,22 @@ class FastSequentialEngine(GraphTrainEngine):
                         self._acc32["head_scratch"] = torch.zeros(need, dtype=torch.float32, device=cur.device)
                         self._acc32["head_counter"] = torch.zeros(1, dtype=torch.int32, device=cur.device)
                     dh = torch.empty((B, K), dtype=bf16, device=cur.device)
-                    self._chk(lib.tfy_dense_head_fused(
-                        xin.data_ptr(), w.data_ptr(), b.data_ptr(), y.data_ptr(),
-                        pmask.data_ptr() if pmask is not None else None, pscale, self._loss.data_ptr(),
-                        self._host_loss_ptr(), self._stats.data_ptr() if self.metric_fns else None,
-                        w.grad.data_ptr(), b.grad.data_ptr(),
-                        dh.data_ptr(), pb.grad.data_ptr(), self._acc32["head_scratch"].data_ptr(),
-                        self._acc32["head_counter"].data_ptr(), B, K, C, s), "dense_head_fused")
+                    if self._wmode == (False, False):
+                        self._chk(lib.tfy_dense_head_fused(
+                            xin.data_ptr(), w.data_ptr(), b.data_ptr(), y.data_ptr(),
+                            pmask.data_ptr() if pmask is not None else None, pscale, self._loss.data_ptr(),
+                                self._host_loss_ptr(), self._stats_ptr(), w.grad.data_ptr(), b.grad.data_ptr(),
+                            dh.data_ptr(), pb.grad.data_ptr(), self._acc32["head_scratch"].data_ptr(),
+                            self._acc32["head_counter"].data_ptr(), B, K, C, s), "dense_head_fused")
+                    else:
+                        # Keras sample / class weights: each row's dlogits scaled by its weight inside the kernel
+                        self._chk(lib.tfy_dense_head_fused_weighted(
+                            xin.data_ptr(), w.data_ptr(), b.data_ptr(), y.data_ptr(),
+                            pmask.data_ptr() if pmask is not None else None, pscale, self._loss.data_ptr(),
+                            self._host_loss_ptr(), self._stats_ptr(), w.grad.data_ptr(), b.grad.data_ptr(),
+                            dh.data_ptr(), pb.grad.data_ptr(), self._acc32["head_scratch"].data_ptr(),
+                            self._acc32["head_counter"].data_ptr(), B, K, C, *self._weight_ptrs(sw)),
+                            "dense_head_fused_weighted")
                     saved.append(("fused", dh))
                     continue
                 self._warn_once(f"head:{li}", f"classifier head {li} ({xin.shape[1]} -> {ly.units}, batch {B}) is outside "
@@ -454,10 +484,16 @@ class FastSequentialEngine(GraphTrainEngine):
                 logits = torch.mm(xin, w.t())
                 C = ly.units
                 dlogits = torch.empty((B, C), dtype=bf16, device=cur.device)
-                self._chk(lib.tfy_softmax_xent(logits.data_ptr(), b.data_ptr(), y.data_ptr(), self._loss.data_ptr(),
-                                               dlogits.data_ptr(), b.grad.data_ptr(),
-                                               self._stats.data_ptr() if self.metric_fns else None, B, C, s),
-                          "softmax_xent")
+                if self._wmode == (False, False):
+                    self._chk(lib.tfy_softmax_xent(logits.data_ptr(), b.data_ptr(), y.data_ptr(), self._loss.data_ptr(),
+                                                   dlogits.data_ptr(), b.grad.data_ptr(), self._stats_ptr(), B, C, s),
+                              "softmax_xent")
+                else:
+                    sw_ptr, cw_ptr, _ = self._weight_ptrs(sw)
+                    self._chk(lib.tfy_softmax_xent_weighted(logits.data_ptr(), b.data_ptr(), y.data_ptr(), sw_ptr,
+                                                            cw_ptr, self._loss.data_ptr(), dlogits.data_ptr(),
+                                                            b.grad.data_ptr(), self._stats_ptr(), B, C, s),
+                              "softmax_xent_weighted")
                 saved.append((xin, dlogits))
         # -------- backward
         grad = None

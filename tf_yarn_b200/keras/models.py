@@ -78,13 +78,17 @@ _NO_WATCHDOG = _NoWatchdog()
 
 
 class _ArrayBatches:
-    """Batches out of in-memory arrays; pinned host memory when feeding a GPU."""
+    """Batches out of in-memory arrays; pinned host memory when feeding a GPU.  With sample weights ``w`` the
+    batches are ``(x, y, w)`` triples (``w`` fp32 ``[B]``), gathered with the same permutation as x and y."""
 
-    def __init__(self, x, y, batch_size: int, shuffle: bool, pin: bool, drop_remainder: bool):
+    def __init__(self, x, y, batch_size: int, shuffle: bool, pin: bool, drop_remainder: bool, w=None):
         self.x, self.y = _as_tensor(x), (_as_tensor(y) if y is not None else None)
+        self.w = _as_tensor(w).reshape(-1).float().contiguous() if w is not None else None
         if self.x.dtype == torch.float64:
             self.x = self.x.float()
         self.n = self.x.shape[0]
+        if self.w is not None and self.w.shape[0] != self.n:
+            raise ValueError(f"sample_weight has {self.w.shape[0]} entries for {self.n} samples")
         self.bs = batch_size
         self.shuffle = shuffle
         self.drop = drop_remainder
@@ -93,13 +97,18 @@ class _ArrayBatches:
             self.x = self.x.pin_memory() if not self.x.is_pinned() else self.x
             if self.y is not None:
                 self.y = self.y.pin_memory() if not self.y.is_pinned() else self.y
+            if self.w is not None:
+                self.w = self.w.pin_memory() if not self.w.is_pinned() else self.w
             self._stage = None
             self._slot = 0
 
     def __len__(self) -> int:
         return self.n // self.bs if self.drop else -(-self.n // self.bs)
 
-    def __iter__(self) -> Iterator[Tuple[torch.Tensor, Optional[torch.Tensor]]]:
+    def __iter__(self) -> Iterator[Tuple[torch.Tensor, ...]]:
+        if self.w is not None:
+            yield from self._iter_weighted()
+            return
         if not self.shuffle:
             for i in range(len(self)):
                 s = slice(i * self.bs, min(self.n, (i + 1) * self.bs))
@@ -123,11 +132,46 @@ class _ArrayBatches:
             else:
                 yield self.x[idx], (self.y[idx] if self.y is not None else None)
 
+    def _iter_weighted(self) -> Iterator[Tuple[torch.Tensor, ...]]:
+        y = self.y
+        if not self.shuffle:
+            for i in range(len(self)):
+                s = slice(i * self.bs, min(self.n, (i + 1) * self.bs))
+                yield self.x[s], (y[s] if y is not None else None), self.w[s]
+            return
+        perm = torch.randperm(self.n)
+        if self.pin and self._stage is None:
+            self._stage = [(torch.empty((self.bs,) + tuple(self.x.shape[1:]), dtype=self.x.dtype).pin_memory(),
+                            torch.empty((self.bs,) + tuple(y.shape[1:]), dtype=y.dtype).pin_memory()
+                            if y is not None else None,
+                            torch.empty((self.bs,), dtype=torch.float32).pin_memory()) for _ in range(4)]
+        for i in range(len(self)):
+            idx = perm[i * self.bs:(i + 1) * self.bs]
+            if self.pin and idx.numel() == self.bs:
+                sx, sy, sw = self._stage[self._slot]
+                self._slot = (self._slot + 1) % len(self._stage)
+                torch.index_select(self.x, 0, idx, out=sx)
+                if y is not None:
+                    torch.index_select(y, 0, idx, out=sy)
+                torch.index_select(self.w, 0, idx, out=sw)
+                yield sx, sy, sw
+            else:
+                yield self.x[idx], (y[idx] if y is not None else None), self.w[idx]
+
 
 def _split_batch(item):
+    """``(x, y)`` or ``(x, y, sample_weight)`` -> ``(x, y, sample_weight or None)``."""
     if isinstance(item, (tuple, list)) and len(item) >= 2:
-        return item[0], item[1]
-    return item, None
+        return item[0], item[1], (item[2] if len(item) >= 3 else None)
+    return item, None, None
+
+
+def _as_weights(w) -> Optional[torch.Tensor]:
+    return None if w is None else _as_tensor(w).reshape(-1).float()
+
+
+def _is_array(x) -> bool:
+    return hasattr(x, "shape") and not hasattr(x, "__next__")
 
 
 class Model:
@@ -143,6 +187,9 @@ class Model:
         self.loss = None
         self._loss_fn: Optional[Callable] = None
         self._metrics_spec: List[Any] = []
+        self._weighted_metrics_spec: List[str] = []
+        self._fit_class_weight: Optional[dict] = None
+        self._class_weight_pending = False      # fit() got a new class_weight (or none) for the engine
         self._engine = None
         self._device: Optional[torch.device] = None
         self.compute_dtype = torch.bfloat16
@@ -208,13 +255,20 @@ class Model:
     # ------------------------------------------------------------------ compile
     def compile(self, optimizer="sgd", loss=None, metrics: Optional[Sequence[Any]] = None,
                 compute_dtype: Optional[torch.dtype] = None, use_cuda_graph: bool = True,
-                use_fast_path: bool = True, **_ignored) -> None:
+                use_fast_path: bool = True, weighted_metrics: Optional[Sequence[str]] = None, **_ignored) -> None:
+        """``metrics`` are unweighted; ``weighted_metrics`` (built-in metric names) are ``sum(w*m) / sum(w)`` over the
+        sample weights of ``fit`` / ``evaluate`` (``class_weight`` included)."""
         if _ignored:
             logger.warning("Model.compile: unsupported arguments ignored: %s", sorted(_ignored))
+        for m in weighted_metrics or []:
+            if not isinstance(m, str):
+                raise ValueError(f"weighted_metrics accepts built-in metric names only, got {m!r}")
+            metric_mod.resolve(m, loss_mod.name_of(loss), 2)          # unknown names fail here
         self.optimizer = opt_mod.get(optimizer)
         self.loss = loss
         self._loss_fn = loss_mod.get(loss) if loss is not None else None
         self._metrics_spec = list(metrics or [])
+        self._weighted_metrics_spec = list(weighted_metrics or [])
         if compute_dtype is not None:
             self.compute_dtype = compute_dtype
         self.use_cuda_graph = use_cuda_graph
@@ -225,6 +279,34 @@ class Model:
         out_dim = self.layers[-1].output_shape_[-1] if self.layers[-1].output_shape_ else 1
         return [metric_mod.resolve(m, loss_mod.name_of(self.loss), out_dim) for m in self._metrics_spec]
 
+    def _weighted_metric_fns(self) -> List[Tuple[str, Callable]]:
+        """Resolved ``weighted_metrics``; one that is also in ``metrics`` is logged as ``weighted_<name>``."""
+        out_dim = self.layers[-1].output_shape_[-1] if self.layers[-1].output_shape_ else 1
+        plain = {name for name, _ in self._metric_fns()}
+        out = []
+        for m in self._weighted_metrics_spec:
+            name, fn = metric_mod.resolve(m, loss_mod.name_of(self.loss), out_dim)
+            out.append((f"weighted_{name}" if name in plain else name, fn))
+        return out
+
+    def _class_weight_table(self, class_weight: Optional[dict]) -> Optional[torch.Tensor]:
+        """``class_weight`` dict -> fp32 table ``[num_classes]``.  Keys must be class indices; classes the dict
+        leaves out weigh 1.0 (with a warning)."""
+        if class_weight is None:
+            return None
+        shape = self.layers[-1].output_shape_
+        n = max(int(shape[-1]), 2) if shape else None
+        for k in class_weight:
+            if isinstance(k, bool) or not isinstance(k, (int, np.integer)) or k < 0 or (n is not None and k >= n):
+                raise ValueError(f"class_weight key {k!r} is not a class index in [0, {n if n is not None else 'C'})")
+        n = n if n is not None else (max(int(k) for k in class_weight) + 1 if class_weight else 1)
+        table = torch.ones(n, dtype=torch.float32)
+        for k, v in class_weight.items():
+            table[int(k)] = float(v)
+        missing = [c for c in range(n) if c not in {int(k) for k in class_weight}]
+        if missing:
+            logger.warning("class_weight has no entry for classes %s: they weigh 1.0", missing)
+        return table
     def _ensure_engine(self, x0, y0) -> None:
         if self._engine is not None:
             return
@@ -243,17 +325,18 @@ class Model:
             if plan is not None:
                 self._engine = fastpath.FastSequentialEngine(
                     self, plan, self.net, self._loss_fn, self.optimizer, self._metric_fns(), self._device,
-                    distributed, x0, y0, self.compute_dtype, self.use_cuda_graph)
+                    distributed, x0, y0, self.compute_dtype, self.use_cuda_graph,
+                    weighted_metric_fns=self._weighted_metric_fns())
             else:
                 self._engine = GraphTrainEngine(self.net, self._loss_fn, self.optimizer, self._metric_fns(),
                                                 self._device, distributed, x0, y0, self.compute_dtype,
-                                                self.use_cuda_graph)
+                                                self.use_cuda_graph, weighted_metric_fns=self._weighted_metric_fns())
         else:
             if distributed:
                 from tf_yarn_b200 import hvd
                 hvd.ensure_cpu_group()
             self._engine = EagerTrainEngine(self.net, self._loss_fn, self.optimizer, self._metric_fns(),
-                                            self._device, distributed)
+                                            self._device, distributed, weighted_metric_fns=self._weighted_metric_fns())
         self._restore_engine_state()
         if self._pending_broadcast_root is not None:
             self._engine.broadcast_variables(self._pending_broadcast_root)
@@ -288,16 +371,22 @@ class Model:
     def fit(self, x=None, y=None, batch_size: Optional[int] = None, epochs: int = 1, verbose: int = 1,
             callbacks: Optional[List[cb_mod.Callback]] = None, validation_data=None, shuffle: bool = True,
             steps_per_epoch: Optional[int] = None, initial_epoch: int = 0, validation_steps: Optional[int] = None,
-            validation_split: float = 0.0, **_ignored):
+            validation_split: float = 0.0, sample_weight=None, class_weight: Optional[dict] = None, **_ignored):
         """Train.  ``x`` may be an array/tensor (with ``y`` and ``batch_size``) or an iterable of
-        ``(features, labels)`` batches such as :class:`tf_yarn_b200.data.Dataset`.  ``validation_split`` holds out
-        the LAST fraction of array inputs (before shuffling), as Keras does."""
+        ``(features, labels)`` or ``(features, labels, sample_weight)`` batches such as
+        :class:`tf_yarn_b200.data.Dataset`.  ``validation_split`` holds out the LAST fraction of array inputs
+        (before shuffling), as Keras does.  ``sample_weight`` (one weight per sample of an array ``x``) and
+        ``class_weight`` (``{class index: weight}``) weigh the loss as ``sum(w*l) / B`` and the weighted metrics."""
         if _ignored:
             logger.warning("Model.fit: unsupported arguments ignored: %s", sorted(_ignored))
         if callable(x) and not torch.is_tensor(x):
             x = x()
         if callable(y):
             y = y()
+        if sample_weight is not None and not _is_array(x):
+            raise ValueError("sample_weight needs array inputs x; a dataset yields (x, y, sample_weight) batches instead")
+        if class_weight is not None and not isinstance(class_weight, dict):
+            raise ValueError("class_weight must be a dict {class index: weight}")
         if validation_split and validation_data is None:
             if not (hasattr(x, "shape") and not hasattr(x, "__next__")) or y is None:
                 raise ValueError("validation_split needs array inputs x and y")
@@ -306,9 +395,15 @@ class Model:
             cut = int(len(x) * (1.0 - validation_split))
             validation_data = (x[cut:], y[cut:])
             x, y = x[:cut], y[:cut]
+            if sample_weight is not None:
+                validation_data += (sample_weight[cut:],)
+                sample_weight = sample_weight[:cut]
+        self._fit_class_weight = class_weight
+        self._class_weight_pending = True
         if hasattr(x, "shape") and not hasattr(x, "__next__"):
             on_gpu = (self._device or default_device()).type == "cuda"
-            batches = _ArrayBatches(x, y, batch_size or 32, shuffle, pin=on_gpu, drop_remainder=on_gpu)
+            batches = _ArrayBatches(x, y, batch_size or 32, shuffle, pin=on_gpu, drop_remainder=on_gpu,
+                                    w=sample_weight)
             make_iter = lambda: iter(batches)   # noqa: E731
             if steps_per_epoch is None:
                 steps_per_epoch = len(batches)
@@ -347,11 +442,12 @@ class Model:
             epoch_it = it if infinite else make_iter()
             logs = self._run_epoch(epoch_it, steps_per_epoch, cbs)
             if validation_data is not None:
-                val = self.evaluate(validation_data[0] if isinstance(validation_data, (tuple, list))
-                                    else validation_data,
-                                    validation_data[1] if isinstance(validation_data, (tuple, list)) else None,
+                pair = isinstance(validation_data, (tuple, list))
+                val = self.evaluate(validation_data[0] if pair else validation_data,
+                                    validation_data[1] if pair else None,
                                     batch_size=batch_size or 32, steps=validation_steps, verbose=0,
-                                    return_dict=True)
+                                    return_dict=True,
+                                    sample_weight=validation_data[2] if pair and len(validation_data) > 2 else None)
                 logs.update({f"val_{k}": v for k, v in val.items()})
             if verbose:
                 msg = " - ".join(f"{k}: {v:.4f}" for k, v in logs.items())
@@ -366,9 +462,12 @@ class Model:
             first = next(it, None)
             if first is None:
                 return {}
-            x0, y0 = _split_batch(first)
+            x0, y0, _ = _split_batch(first)
             self._ensure_engine(_as_struct(x0), _as_struct(y0))
         eng = self._engine
+        if self._class_weight_pending:
+            eng.set_class_weight(self._class_weight_table(self._fit_class_weight))
+            self._class_weight_pending = False
         if eng.pipelined:
             return self._run_epoch_pipelined(it, steps, cbs, first)
         loss_sum, n = 0.0, 0
@@ -380,10 +479,13 @@ class Model:
             first = None
             if item is None:
                 break
-            xb, yb = _split_batch(item)
+            xb, yb, wb = _split_batch(item)
             if cbs.has_batch_hooks:
                 cbs.call("on_train_batch_begin", step, None)
-            logs = eng.train_step(_as_struct(xb), _as_struct(yb))
+            if wb is None:
+                logs = eng.train_step(_as_struct(xb), _as_struct(yb))
+            else:
+                logs = eng.train_step(_as_struct(xb), _as_struct(yb), _as_weights(wb))
             wd.beat()
             loss_sum += float(logs["loss"])
             for k, v in logs.items():
@@ -395,6 +497,8 @@ class Model:
             step += 1
         out = {"loss": loss_sum / max(n, 1)}
         out.update({k: v / max(n, 1) for k, v in metric_sums.items()})
+        if getattr(eng, "weighted_metric_fns", None):
+            out.update(eng.pop_metrics())
         return out
 
     def _run_epoch_pipelined(self, it, steps, cbs, first) -> Dict[str, float]:
@@ -413,8 +517,10 @@ class Model:
             first = None
             if item is None:
                 return None
-            xb, yb = _split_batch(item)
-            return _as_struct(xb), _as_struct(yb)
+            xb, yb, wb = _split_batch(item)
+            if wb is None:
+                return _as_struct(xb), _as_struct(yb)
+            return _as_struct(xb), _as_struct(yb), _as_weights(wb)
 
         nxt = fetch()
         if nxt is None:
@@ -456,14 +562,18 @@ class Model:
         return out
 
     # ------------------------------------------------------------------ inference
-    def _infer_batches(self, x, y, batch_size, steps):
+    def _infer_batches(self, x, y, batch_size, steps, sample_weight=None):
         if callable(x) and not torch.is_tensor(x):
             x = x()
-        if (y is None and isinstance(x, (tuple, list)) and len(x) == 2 and all(hasattr(t, "shape") for t in x)
-                and len(x[0]) == len(x[1])):
-            x, y = x                      # ``validation_data_fn=lambda: (x_val, y_val)``: a pair of arrays, not batches
+        if (y is None and isinstance(x, (tuple, list)) and len(x) in (2, 3) and all(hasattr(t, "shape") for t in x)
+                and all(len(t) == len(x[0]) for t in x)):
+            # ``validation_data_fn=lambda: (x_val, y_val[, w_val])``: arrays, not batches
+            x, y, sample_weight = x[0], x[1], (x[2] if len(x) == 3 else sample_weight)
         if hasattr(x, "shape") and not hasattr(x, "__next__"):
-            return iter(_ArrayBatches(x, y, batch_size or 32, False, pin=False, drop_remainder=False)), steps
+            return iter(_ArrayBatches(x, y, batch_size or 32, False, pin=False, drop_remainder=False,
+                                      w=sample_weight)), steps
+        if sample_weight is not None:
+            raise ValueError("sample_weight needs array inputs x; a dataset yields (x, y, sample_weight) batches instead")
         return iter(x), steps
 
     def _prep_infer(self, xb):
@@ -479,13 +589,18 @@ class Model:
         return xb
 
     def evaluate(self, x=None, y=None, batch_size: Optional[int] = None, steps: Optional[int] = None,
-                 verbose: int = 0, return_dict: bool = False, **_ignored):
-        """Mean loss and metrics over ``x``; returns ``[loss, *metrics]`` (or a dict)."""
-        it, steps = self._infer_batches(x, y, batch_size, steps)
+                 verbose: int = 0, return_dict: bool = False, sample_weight=None, **_ignored):
+        """Mean loss and metrics over ``x``; returns ``[loss, *metrics, *weighted metrics]`` (or a dict).  With sample
+        weights (``sample_weight``, or ``(x, y, w)`` batches) the loss is ``sum(w*l) / N`` over the N samples and the
+        weighted metrics ``sum(w*m) / sum(w)``; ``metrics`` stay unweighted."""
+        it, steps = self._infer_batches(x, y, batch_size, steps, sample_weight)
         fns = self._metric_fns() if self.built and self.loss is not None else []
+        wfns = self._weighted_metric_fns() if self.built and self.loss is not None else []
         loss_sum, count = 0.0, 0
         m_num = [0.0] * len(fns)
         m_den = [0.0] * len(fns)
+        w_num = [0.0] * len(wfns)
+        w_den = [0.0] * len(wfns)
         self.net.eval() if self.net is not None else None
         n = 0
         wd = getattr(self, "_watchdog", None)
@@ -493,28 +608,40 @@ class Model:
             for item in it:
                 if steps is not None and n >= steps:
                     break
-                xb, yb = _split_batch(item)
+                xb, yb, wb = _split_batch(item)
                 xb = self._prep_infer(_as_struct(xb))
                 self.net.eval()
                 if not fns and self.loss is not None:
                     fns = self._metric_fns()
                     m_num, m_den = [0.0] * len(fns), [0.0] * len(fns)
+                    wfns = self._weighted_metric_fns()
+                    w_num, w_den = [0.0] * len(wfns), [0.0] * len(wfns)
                 yb = _move(_as_struct(yb), self._device)
+                wb = _move(_as_weights(wb), self._device)
                 out = self.net(xb)
                 if wd is not None:
                     wd.beat()
                 bs = _batch_size_of(out)
                 if self._loss_fn is not None:
-                    loss_sum += float(self._loss_fn(yb, out)) * bs
+                    if wb is None:
+                        loss_sum += float(self._loss_fn(yb, out)) * bs
+                    else:
+                        loss_sum += float((loss_mod.per_sample(self._loss_fn)(yb, out) * wb).sum())
                 count += bs
                 for i, (_, fn) in enumerate(fns):
                     a, b = fn(yb, out)
                     m_num[i] += float(a)
                     m_den[i] += float(b)
+                for i, (_, fn) in enumerate(wfns):
+                    a, b = fn(yb, out, sample_weight=wb)
+                    w_num[i] += float(a)
+                    w_den[i] += float(b)
                 n += 1
         res = {"loss": loss_sum / max(count, 1)}
         for i, (name, _) in enumerate(fns):
             res[name] = m_num[i] / max(m_den[i], 1.0)
+        for i, (name, _) in enumerate(wfns):
+            res[name] = w_num[i] / w_den[i] if w_den[i] else 0.0
         if return_dict:
             return res
         vals = list(res.values())
@@ -528,7 +655,7 @@ class Model:
             for item in it:
                 if steps is not None and n >= steps:
                     break
-                xb, _ = _split_batch(item) if isinstance(item, (tuple, list)) else (item, None)
+                xb = _split_batch(item)[0] if isinstance(item, (tuple, list)) else item
                 xb = self._prep_infer(_as_struct(xb))
                 self.net.eval()
                 outs.append(self.net(xb).float().cpu())
@@ -613,7 +740,8 @@ class Model:
             "weights": self._fp32_state(),
             "compile": {"loss": loss_mod.serialize(self.loss),
                         "optimizer": self.optimizer.get_config() if self.optimizer is not None else None,
-                        "metrics": [m for m in self._metrics_spec if isinstance(m, str)]},
+                        "metrics": [m for m in self._metrics_spec if isinstance(m, str)],
+                        "weighted_metrics": list(self._weighted_metrics_spec)},
             "optimizer_state": (self._engine.state_dict() if (include_optimizer and self._engine is not None
                                                               and not self._sharded_across_ranks()) else None),
         }
@@ -661,7 +789,7 @@ def load_model(filepath: str, compile: bool = True) -> Model:
     comp = payload.get("compile") or {}
     if compile and comp.get("loss") and comp.get("optimizer"):
         model.compile(optimizer=opt_mod.from_config(comp["optimizer"]), loss=loss_mod.deserialize(comp["loss"]),
-                      metrics=comp.get("metrics") or [])
+                      metrics=comp.get("metrics") or [], weighted_metrics=comp.get("weighted_metrics") or [])
         model._pending_engine_state = payload.get("optimizer_state")
     return model
 

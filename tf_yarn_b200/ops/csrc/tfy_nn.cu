@@ -469,6 +469,92 @@ tfy_softmax_xent_kernel(const __nv_bfloat16* __restrict__ logits, const __nv_bfl
         for (int c = threadIdx.x; c < C; c += blockDim.x) dbias[c] = __float2bfloat16(s_db[c]);
 }
 
+// Weighted form of the head above (Keras sample_weight / class_weight): row r weighs
+// w_r = sample_w[r] * class_w[label_r] (a null pointer, or a label outside [0, C), counts as 1).
+// loss = sum_r w_r l_r / B, dlogits = w_r (softmax - onehot) / B, dbias = column sums of dlogits,
+// stats[0..3] += [hits, B, sum w*hit, sum w].  Every block-level sum is taken in a fixed order (warp shuffles,
+// then warps in index order; dbias from one partial row per warp), so the result is the same bit for bit on every run.
+__global__ void __launch_bounds__(1024)
+tfy_softmax_xent_weighted_kernel(const __nv_bfloat16* __restrict__ logits, const __nv_bfloat16* __restrict__ bias,
+                                 const long long* __restrict__ labels, const float* __restrict__ sample_w,
+                                 const float* __restrict__ class_w, float* __restrict__ loss,
+                                 __nv_bfloat16* __restrict__ dlogits, __nv_bfloat16* __restrict__ dbias,
+                                 float* __restrict__ stats, int B, int C) {
+    tfy_pdl_sync();
+    extern __shared__ float sm[];  // [C] bias | [warps][C] dbias partials | [warps][4] loss, hits, w*hits, w
+    const int warps = blockDim.x >> 5, warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    float* s_bias = sm;
+    float* s_db = sm + C;
+    float* s_red = s_db + (size_t)warps * C;
+    for (int c = threadIdx.x; c < C; c += blockDim.x) s_bias[c] = bias ? bf16_to_f(bias[c]) : 0.f;
+    for (int i = threadIdx.x; i < warps * C; i += blockDim.x) s_db[i] = 0.f;
+    __syncthreads();
+    const float invB = 1.f / (float)B;
+    float acc[4] = {0.f, 0.f, 0.f, 0.f};        // loss, hits, w*hits, w
+    const int rounds = (B + blockDim.x - 1) / blockDim.x;      // same trip count on every warp: shuffles converge
+    for (int it = 0; it < rounds; ++it) {
+        const int r = it * blockDim.x + threadIdx.x;
+        const bool ok = r < B;
+        const __nv_bfloat16* row = logits + (size_t)(ok ? r : 0) * C;
+        const int lab = ok ? (int)labels[r] : -1;
+        float wr = 0.f;
+        if (ok) {
+            wr = sample_w ? sample_w[r] : 1.f;
+            if (class_w && lab >= 0 && lab < C) wr *= class_w[lab];
+        }
+        float mx = -3.0e38f;
+        int amax = 0;
+        for (int c = 0; c < C; ++c) {
+            const float v = bf16_to_f(row[c]) + s_bias[c];
+            if (v > mx) { mx = v; amax = c; }
+        }
+        float se = 0.f;
+        for (int c = 0; c < C; ++c) se += __expf(bf16_to_f(row[c]) + s_bias[c] - mx);
+        const float lse = mx + __logf(se);
+        const float inv_se = 1.f / se;
+        for (int c = 0; c < C; ++c) {
+            const float v = bf16_to_f(row[c]) + s_bias[c];
+            float d = (__expf(v - mx) * inv_se - (c == lab ? 1.f : 0.f)) * invB * wr;
+            if (!ok) d = 0.f;
+            if (ok) {
+                if (c == lab) acc[0] += wr * (lse - v);
+                dlogits[(size_t)r * C + c] = __float2bfloat16(d);
+            }
+            if (dbias) {
+                float t = d;
+#pragma unroll
+                for (int off = 16; off > 0; off >>= 1) t += __shfl_xor_sync(0xffffffffu, t, off);
+                if (lane == 0) s_db[(size_t)warp * C + c] += t;        // one writer per (warp, class)
+            }
+        }
+        if (ok && amax == lab) { acc[1] += 1.f; acc[2] += wr; }
+        acc[3] += wr;
+    }
+#pragma unroll
+    for (int off = 16; off > 0; off >>= 1) {
+#pragma unroll
+        for (int k = 0; k < 4; ++k) acc[k] += __shfl_xor_sync(0xffffffffu, acc[k], off);
+    }
+    if (lane == 0) {
+#pragma unroll
+        for (int k = 0; k < 4; ++k) s_red[warp * 4 + k] = acc[k];
+    }
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        float t[4] = {0.f, 0.f, 0.f, 0.f};
+        for (int w = 0; w < warps; ++w)
+            for (int k = 0; k < 4; ++k) t[k] += s_red[w * 4 + k];
+        *loss = t[0] * invB;
+        if (stats) { stats[0] += t[1]; stats[1] += (float)B; stats[2] += t[2]; stats[3] += t[3]; }
+    }
+    if (dbias)
+        for (int c = threadIdx.x; c < C; c += blockDim.x) {
+            float a = 0.f;
+            for (int w = 0; w < warps; ++w) a += s_db[(size_t)w * C + c];
+            dbias[c] = __float2bfloat16(a);
+        }
+}
+
 
 // ---------------------------------------------------------------------------------------------
 // Classifier head, forward AND backward, in one launch (the whole problem is ~0.5 MFLOP):
@@ -484,6 +570,10 @@ tfy_softmax_xent_kernel(const __nv_bfloat16* __restrict__ logits, const __nv_bfl
 // h: [B, K] bf16, W2: [C, K] bf16, b2: [C] bf16, labels: [B] int64, mask1: [B, K] uint8 (bit 0 = gradient
 // flows) or null.  K in {128, 256, 512}, C <= 16.
 // scratch: one slab [C*K | 16 | K | 4] floats per CTA, zero on entry and on exit; counter: one uint32, same.
+// WEIGHTED (Keras sample_weight / class_weight): row r weighs w_r = sample_w[r] * class_w[label_r] (a null table, or a
+// label outside [0, C), counts as 1).  Its dlogits row is scaled by w_r, so dW2, db2, dh and db1 follow; the loss is
+// sum_r w_r l_r / B, and stats holds 4 floats [hits, B, sum w*hit, sum w].  The two extra sums use the spare floats
+// of each CTA's reduction slab and are summed in CTA order like the others.
 // ---------------------------------------------------------------------------------------------
 // debug: per-CTA event timeline of the head kernel (16 slots of SM-clock deltas per CTA), see tfy_nn_set_timeline
 __device__ long long* n_timeline = nullptr;
@@ -494,7 +584,7 @@ __device__ long long* n_timeline = nullptr;
 
 constexpr int HEAD_THREADS = 256, HEAD_CMAX = 16, HEAD_ROWS = 16, HEAD_WARPS = HEAD_THREADS / 32;
 
-template <int K>
+template <int K, bool WEIGHTED>
 __global__ void __launch_bounds__(HEAD_THREADS)
 tfy_dense_head_fused_kernel(const __nv_bfloat16* __restrict__ h, const __nv_bfloat16* __restrict__ w2,
                             const __nv_bfloat16* __restrict__ b2, const long long* __restrict__ labels,
@@ -503,7 +593,9 @@ tfy_dense_head_fused_kernel(const __nv_bfloat16* __restrict__ h, const __nv_bflo
                             __nv_bfloat16* __restrict__ dw2,
                             __nv_bfloat16* __restrict__ db2, __nv_bfloat16* __restrict__ dh,
                             __nv_bfloat16* __restrict__ db1, float* __restrict__ scratch,
-                            uint32_t* __restrict__ counter, int B, int C) {
+                            uint32_t* __restrict__ counter, int B, int C,
+                            const float* __restrict__ sample_w, const float* __restrict__ class_w) {
+    // (the weights come last: the parameter offsets of the unweighted instantiations do not move)
     // K is a template parameter: every loop that waits on global memory has a constant trip count and is
     // fully unrolled, so its loads are issued back to back (the first version had ~18 serialised L2 round
     // trips in five-iteration loops: 15 us for 0.5 MFLOP).
@@ -512,12 +604,13 @@ tfy_dense_head_fused_kernel(const __nv_bfloat16* __restrict__ h, const __nv_bflo
     const long long n_t0 = clock64();
     extern __shared__ __align__(16) uint8_t head_smem[];
     constexpr int KP = K + 8;                                       // padded row (bank spread)
+    constexpr int NRED = WEIGHTED ? 4 : 2;                          // per-warp sums: loss, correct (, w*correct, w)
     __nv_bfloat16* s_h = reinterpret_cast<__nv_bfloat16*>(head_smem);                 // [16][KP]
     float* s_w = reinterpret_cast<float*>(head_smem + (size_t)HEAD_ROWS * KP * 2);    // [16][K], rows >= C are zero
     float* s_dl = s_w + (size_t)HEAD_CMAX * K;                                                // [16][HEAD_CMAX]
     float* s_b = s_dl + HEAD_ROWS * HEAD_CMAX;                                        // [HEAD_CMAX]
-    float* s_red = s_b + HEAD_CMAX;                                                   // [warp][loss, correct]
-    float* s_col = s_red + 2 * HEAD_WARPS;                                            // [max(K, 256)], 16-byte aligned
+    float* s_red = s_b + HEAD_CMAX;                                                   // [warp][NRED]
+    float* s_col = s_red + NRED * HEAD_WARPS;                                         // [max(K, 256)], 16-byte aligned
     __shared__ uint32_t s_last;
     const int tid = threadIdx.x;
     const int row0 = blockIdx.x * HEAD_ROWS;
@@ -563,6 +656,13 @@ tfy_dense_head_fused_kernel(const __nv_bfloat16* __restrict__ h, const __nv_bflo
         const int r = tid >> 4, part = tid & 15;
         constexpr int kq = K / 16;
         const int lab = r < rows ? (int)labels[row0 + r] : -1;     // issued early: used after the GEMV
+        float wr = 0.f;                                             // this row's weight (WEIGHTED only)
+        if constexpr (WEIGHTED) {
+            if (r < rows) {
+                wr = sample_w ? sample_w[row0 + r] : 1.f;
+                if (class_w && lab >= 0 && lab < C) wr *= class_w[lab];
+            }
+        }
         const __nv_bfloat16* hr = s_h + (size_t)r * KP + part * kq;
         float* s_logit = s_col;                                     // [16][16] scratch (s_col is used later)
 #pragma unroll 1
@@ -610,17 +710,35 @@ tfy_dense_head_fused_kernel(const __nv_bfloat16* __restrict__ h, const __nv_bflo
 #pragma unroll
             for (int off = 1; off < 16; off <<= 1) se += __shfl_xor_sync(0xffffffffu, se, off);
             const bool hit = live && c == lab;
-            if (live) s_dl[r * HEAD_CMAX + c] = (e / se - (hit ? 1.f : 0.f)) * invB;
+            if constexpr (WEIGHTED) {
+                if (live) s_dl[r * HEAD_CMAX + c] = (e / se - (hit ? 1.f : 0.f)) * invB * wr;
+            } else {
+                if (live) s_dl[r * HEAD_CMAX + c] = (e / se - (hit ? 1.f : 0.f)) * invB;
+            }
             float my_loss = hit ? (mx + __logf(se)) - v : 0.f;
             float my_correct = (hit && amax == lab) ? 1.f : 0.f;
+            float my_wcorrect = 0.f, my_w = 0.f;
+            if constexpr (WEIGHTED) {
+                my_loss *= wr;
+                my_wcorrect = my_correct * wr;
+                my_w = (c == 0 && r < rows) ? wr : 0.f;             // once per row
+            }
 #pragma unroll
             for (int off = 16; off > 0; off >>= 1) {
                 my_loss += __shfl_xor_sync(0xffffffffu, my_loss, off);
                 my_correct += __shfl_xor_sync(0xffffffffu, my_correct, off);
+                if constexpr (WEIGHTED) {
+                    my_wcorrect += __shfl_xor_sync(0xffffffffu, my_wcorrect, off);
+                    my_w += __shfl_xor_sync(0xffffffffu, my_w, off);
+                }
             }
             if ((tid & 31) == 0) {
-                s_red[2 * (tid >> 5)] = my_loss;
-                s_red[2 * (tid >> 5) + 1] = my_correct;
+                s_red[NRED * (tid >> 5)] = my_loss;
+                s_red[NRED * (tid >> 5) + 1] = my_correct;
+                if constexpr (WEIGHTED) {
+                    s_red[NRED * (tid >> 5) + 2] = my_wcorrect;
+                    s_red[NRED * (tid >> 5) + 3] = my_w;
+                }
             }
         }
     }
@@ -629,9 +747,15 @@ tfy_dense_head_fused_kernel(const __nv_bfloat16* __restrict__ h, const __nv_bflo
     __syncthreads();
     if (tid == 0) {
         float l = 0.f, c = 0.f;
-        for (int w = 0; w < HEAD_WARPS; ++w) { l += s_red[2 * w]; c += s_red[2 * w + 1]; }
+        for (int w = 0; w < HEAD_WARPS; ++w) { l += s_red[NRED * w]; c += s_red[NRED * w + 1]; }
         __stcg(g_red, l);
         __stcg(g_red + 1, c);
+        if constexpr (WEIGHTED) {
+            float wc = 0.f, ws = 0.f;
+            for (int w = 0; w < HEAD_WARPS; ++w) { wc += s_red[NRED * w + 2]; ws += s_red[NRED * w + 3]; }
+            __stcg(g_red + 2, wc);
+            __stcg(g_red + 3, ws);
+        }
     }
 
     N_MARK(2);
@@ -782,6 +906,17 @@ tfy_dense_head_fused_kernel(const __nv_bfloat16* __restrict__ h, const __nv_bflo
             *loss = mean_loss;
             if (loss_host) *loss_host = mean_loss;      // pinned host scalar (UVA): no D2H copy node per step
             if (stats) { stats[0] += c; stats[1] += (float)B; }
+            if constexpr (WEIGHTED) {
+                float wc = 0.f, ws = 0.f;
+#pragma unroll 8
+                for (int g = 0; g < G; ++g) {
+                    wc += __ldcg(scratch + g * slab + o_red + 2);
+                    ws += __ldcg(scratch + g * slab + o_red + 3);
+                    __stcg(scratch + g * slab + o_red + 2, 0.f);
+                    __stcg(scratch + g * slab + o_red + 3, 0.f);
+                }
+                if (stats) { stats[2] += wc; stats[3] += ws; }
+            }
             *counter = 0u;
         }
     }
@@ -898,6 +1033,24 @@ int tfy_softmax_xent(const void* logits, const void* bias, const void* labels, f
     return (int)cudaGetLastError();
 }
 
+// weighted variant: sample_w [B] and class_w [C] fp32 (either may be null), stats null or 4 floats
+// [hits, B, sum w*hit, sum w]; returns -2 when C is too wide for one partial row of dbias per warp
+int tfy_softmax_xent_weighted(const void* logits, const void* bias, const void* labels, const float* sample_w,
+                              const float* class_w, float* loss, void* dlogits, void* dbias, float* stats, int B, int C,
+                              cudaStream_t s) {
+    if (B < 1 || C < 1) return -2;
+    const int max_warps = (int)((48 * 1024 / sizeof(float) - (size_t)C) / ((size_t)C + 4));
+    if (max_warps < 1) return -2;
+    int warps = (B + 31) / 32;
+    if (warps > 32) warps = 32;
+    if (warps > max_warps) warps = max_warps;
+    const size_t smem = ((size_t)C + (size_t)warps * (C + 4)) * sizeof(float);
+    tfy_launch_pdl((tfy_softmax_xent_weighted_kernel), dim3(1), dim3(warps * 32), smem, s,
+                   (const __nv_bfloat16*)logits, (const __nv_bfloat16*)bias, (const long long*)labels, sample_w,
+                   class_w, loss, (__nv_bfloat16*)dlogits, (__nv_bfloat16*)dbias, stats, B, C);
+    return (int)cudaGetLastError();
+}
+
 // thin cudaMemcpyAsync wrapper: the input pipeline issues its per-step copies through ctypes (about 1 us per call
 // instead of ~10 us for Tensor.copy_ under a stream context manager)
 int tfy_memcpy_async(void* dst, const void* src, size_t bytes, cudaStream_t s) {
@@ -913,34 +1066,59 @@ size_t tfy_dense_head_scratch_elems(int K, int C, int B) {
     return (size_t)((B + HEAD_ROWS - 1) / HEAD_ROWS) * ((size_t)C * K + HEAD_CMAX + K + 4);
 }
 
-int tfy_dense_head_fused(const void* h, const void* w2, const void* b2, const void* labels, const void* mask1,
-                         float scale1, float* loss, float* loss_host, float* stats, void* dw2, void* db2, void* dh,
-                         void* db1,
-                         float* scratch, uint32_t* counter, int B, int K, int C, cudaStream_t s) {
+}  // extern "C"
+
+template <bool WEIGHTED>
+static int tfy_dense_head_launch(const void* h, const void* w2, const void* b2, const void* labels, const void* mask1,
+                                 float scale1, float* loss, float* loss_host, float* stats, void* dw2, void* db2,
+                                 void* dh, void* db1, float* scratch, uint32_t* counter, int B, int K, int C,
+                                 const float* sample_w, const float* class_w, cudaStream_t s) {
     if (!(K == 128 || K == 256 || K == 512) || C < 1 || C > HEAD_CMAX || B < 1) return -2;
+    constexpr int NRED = WEIGHTED ? 4 : 2;
     const size_t smem = (size_t)HEAD_ROWS * (K + 8) * 2 +
-                        ((size_t)HEAD_CMAX * K + HEAD_ROWS * HEAD_CMAX + HEAD_CMAX + 2 * HEAD_WARPS + (K > 256 ? K : 256)) * 4;
+                        ((size_t)HEAD_CMAX * K + HEAD_ROWS * HEAD_CMAX + HEAD_CMAX + NRED * HEAD_WARPS + (K > 256 ? K : 256)) * 4;
     const int grid = (B + HEAD_ROWS - 1) / HEAD_ROWS;
 #define TFY_HEAD(KK)                                                                                                   \
     do {                                                                                                               \
         static bool configured = false;                                                                                \
         if (smem > 48 * 1024 && !configured) {                                                                         \
-            if (cudaFuncSetAttribute(tfy_dense_head_fused_kernel<KK>, cudaFuncAttributeMaxDynamicSharedMemorySize,     \
-                                     96 * 1024) != cudaSuccess)                                                        \
+            if (cudaFuncSetAttribute(tfy_dense_head_fused_kernel<KK, WEIGHTED>,                                        \
+                                     cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024) != cudaSuccess)           \
                 return -5;                                                                                             \
             configured = true;                                                                                         \
         }                                                                                                              \
-        tfy_launch_pdl((tfy_dense_head_fused_kernel<KK>), dim3(grid), dim3(HEAD_THREADS), smem, s,                     \
+        tfy_launch_pdl((tfy_dense_head_fused_kernel<KK, WEIGHTED>), dim3(grid), dim3(HEAD_THREADS), smem, s,           \
                        (const __nv_bfloat16*)h, (const __nv_bfloat16*)w2, (const __nv_bfloat16*)b2,                    \
                        (const long long*)labels, (const uint8_t*)mask1, scale1, loss, loss_host, stats,              \
                        (__nv_bfloat16*)dw2,                                                                            \
-                       (__nv_bfloat16*)db2, (__nv_bfloat16*)dh, (__nv_bfloat16*)db1, scratch, counter, B, C);          \
+                       (__nv_bfloat16*)db2, (__nv_bfloat16*)dh, (__nv_bfloat16*)db1, scratch, counter, B, C,           \
+                       sample_w, class_w);                                                                             \
     } while (0)
     if (K == 128) TFY_HEAD(128);
     else if (K == 256) TFY_HEAD(256);
     else TFY_HEAD(512);
 #undef TFY_HEAD
     return (int)cudaGetLastError();
+}
+
+extern "C" {
+
+int tfy_dense_head_fused(const void* h, const void* w2, const void* b2, const void* labels, const void* mask1,
+                         float scale1, float* loss, float* loss_host, float* stats, void* dw2, void* db2, void* dh,
+                         void* db1,
+                         float* scratch, uint32_t* counter, int B, int K, int C, cudaStream_t s) {
+    return tfy_dense_head_launch<false>(h, w2, b2, labels, mask1, scale1, loss, loss_host, stats, dw2, db2, dh, db1,
+                                        scratch, counter, B, K, C, nullptr, nullptr, s);
+}
+
+// weighted variant: sample_w [B] and class_w [C] fp32 (either may be null), stats null or 4 floats
+// [hits, B, sum w*hit, sum w]; same envelope, scratch size and return codes as tfy_dense_head_fused
+int tfy_dense_head_fused_weighted(const void* h, const void* w2, const void* b2, const void* labels, const void* mask1,
+                                  float scale1, float* loss, float* loss_host, float* stats, void* dw2, void* db2,
+                                  void* dh, void* db1, float* scratch, uint32_t* counter, int B, int K, int C,
+                                  const float* sample_w, const float* class_w, cudaStream_t s) {
+    return tfy_dense_head_launch<true>(h, w2, b2, labels, mask1, scale1, loss, loss_host, stats, dw2, db2, dh, db1,
+                                       scratch, counter, B, K, C, sample_w, class_w, s);
 }
 
 }  // extern "C"
