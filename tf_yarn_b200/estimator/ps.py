@@ -46,6 +46,14 @@ KV_READY = "ps/ready"
 _SLOTS = {"sgd": 0, "adagrad": 1, "adadelta": 2, "adam": 2, "adamw": 2, "ftrl": 2}
 
 
+def _var_slots(kind: str, hyper: Dict[str, float]) -> int:
+    """Slots of one variable.  RMSprop's depend on its hyper-parameters: mean square, then the momentum buffer
+    (p2 = momentum > 0), then the mean gradient (flags bit 0 = centered)."""
+    if kind == "rmsprop":
+        return 1 + (hyper["p2"] > 0) + (int(hyper["flags"]) & 1)
+    return _SLOTS[kind]
+
+
 def _job_tag() -> str:
     return f"{os.environ.get('TFY_APP_ID', 'local')}_{_task_commons.n_try()}"
 
@@ -65,7 +73,7 @@ class Layout:
         self.hyper = hyper
         self.kinds = list(kinds) if kinds else [opt_kind] * len(variables)
         self.hypers = list(hypers) if hypers else [hyper] * len(variables)
-        self.var_slots = [_SLOTS[k] for k in self.kinds]
+        self.var_slots = [_var_slots(k, h) for k, h in zip(self.kinds, self.hypers)]
         self.slots = max(self.var_slots + [0])
         self.owner: List[int] = []
         self.offset: List[int] = []
@@ -191,6 +199,21 @@ class WorkerConnection:
                     n.copy_(n_new)
                     neww = -(z - torch.sign(z) * p1) / ((eps + n_new.sqrt()) / lr + 2 * p2)
                     w.copy_(torch.where(z.abs() <= p1, torch.zeros_like(neww), neww))
+                elif kind == "rmsprop":        # p1 = rho, p2 = momentum, flags bit 0 = centered (OptimizerSpec.rmsprop)
+                    v = self._region(i, 1)
+                    v.mul_(p1).addcmul_(g, g, value=1 - p1)
+                    denom = v
+                    if int(h["flags"]) & 1:
+                        mg = self._region(i, 3 if p2 > 0 else 2)
+                        mg.mul_(p1).add_(g, alpha=1 - p1)
+                        denom = v - mg * mg
+                    inc = lr * g * (denom + eps).rsqrt()
+                    if p2 > 0:
+                        m = self._region(i, 2)
+                        m.mul_(p2).add_(inc)
+                        w.sub_(m)
+                    else:
+                        w.sub_(inc)
                 elif kind == "adadelta":
                     sq, dx = self._region(i, 1), self._region(i, 2)
                     sq.mul_(p1).addcmul_(g, g, value=1 - p1)

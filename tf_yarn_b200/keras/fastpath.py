@@ -243,6 +243,8 @@ class FastSequentialEngine(GraphTrainEngine):
         if not self._overlap or self._ov_used or fused.zero_grads or fused.param_dtype != torch.bfloat16 \
                 or fused.grad_dtype != torch.bfloat16:
             return None
+        if fused.spec.kind == "rmsprop":             # no overlap role for RMSprop: the trailing step updates everything
+            return None
         n_cta = int(self.lib.tfy_conv3x3_c32_wgrad_spare_ctas(B, H, W))
         later = [st for st in self.plan[li + 1:] if st.kind in ("conv", "dense", "head")]
         if n_cta <= 0 or not later:

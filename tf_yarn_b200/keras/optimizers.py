@@ -164,7 +164,77 @@ class TorchFtrl(torch.optim.Optimizer):
                 p.copy_(torch.where(z.abs() <= l1, torch.zeros_like(w), w))
 
 
-_BY_NAME = {"sgd": SGD, "adadelta": Adadelta, "adam": Adam, "adamw": AdamW, "adagrad": Adagrad, "ftrl": Ftrl}
+class RMSprop(Optimizer):
+    """RMSprop as ``tf.keras.optimizers.RMSprop`` (Keras 2.11+ and Keras 3) defines it, per element::
+
+        v  = rho * v + (1 - rho) * g^2
+        mg = rho * mg + (1 - rho) * g               (centered only)
+        inc = lr * g / sqrt(v [- mg^2] + epsilon)
+        m  = momentum * m + inc;  p -= m            (momentum > 0; otherwise p -= inc)
+
+    Unlike ``torch.optim.RMSprop``, epsilon sits inside the square root and the learning rate inside the momentum
+    buffer, so a learning-rate change only scales later increments.  ``weight_decay`` is coupled, as for SGD,
+    Adadelta and Adagrad here: ``g += weight_decay * p`` before the update."""
+    kind = "rmsprop"
+
+    def __init__(self, learning_rate: float = 0.001, rho: float = 0.9, momentum: float = 0.0, epsilon: float = 1e-7,
+                 centered: bool = False, weight_decay: float = 0.0, lr: float = None):
+        if momentum < 0:
+            raise ValueError(f"RMSprop momentum must be >= 0, got {momentum}")
+        super().__init__(lr if lr is not None else learning_rate, rho=rho, momentum=momentum, epsilon=epsilon,
+                         centered=centered, weight_decay=weight_decay)
+        self.rho, self.momentum, self.epsilon = rho, momentum, epsilon
+        self.centered, self.weight_decay = bool(centered), weight_decay
+
+    def to_spec(self):
+        return OptimizerSpec.rmsprop(self.learning_rate, self.rho, self.momentum, self.epsilon, self.centered,
+                                     self.weight_decay)
+
+    def to_torch(self, params):
+        return TorchRMSprop(params, lr=self.learning_rate, rho=self.rho, momentum=self.momentum, eps=self.epsilon,
+                            centered=self.centered, weight_decay=self.weight_decay)
+
+
+class TorchRMSprop(torch.optim.Optimizer):
+    """torch.optim rendition of the Keras RMSprop (same formulas as the fused kernel; see :class:`RMSprop`)."""
+
+    def __init__(self, params, lr=1e-3, rho=0.9, momentum=0.0, eps=1e-7, centered=False, weight_decay=0.0):
+        super().__init__(params, dict(lr=lr, rho=rho, momentum=momentum, eps=eps, centered=centered,
+                                      weight_decay=weight_decay))
+
+    @torch.no_grad()
+    def step(self, closure=None):
+        for grp in self.param_groups:
+            lr, rho, mom, eps, wd = grp["lr"], grp["rho"], grp["momentum"], grp["eps"], grp["weight_decay"]
+            for p in grp["params"]:
+                if p.grad is None:
+                    continue
+                st = self.state[p]
+                if not st:
+                    st["v"] = torch.zeros_like(p)
+                    if mom > 0:
+                        st["m"] = torch.zeros_like(p)
+                    if grp["centered"]:
+                        st["mg"] = torch.zeros_like(p)
+                g = p.grad + wd * p if wd else p.grad
+                v = st["v"]
+                v.mul_(rho).addcmul_(g, g, value=1 - rho)
+                denom = v
+                if grp["centered"]:
+                    mg = st["mg"]
+                    mg.mul_(rho).add_(g, alpha=1 - rho)
+                    denom = v - mg * mg
+                inc = lr * g * (denom + eps).rsqrt()
+                if mom > 0:
+                    m = st["m"]
+                    m.mul_(mom).add_(inc)
+                    p.sub_(m)
+                else:
+                    p.sub_(inc)
+
+
+_BY_NAME = {"sgd": SGD, "adadelta": Adadelta, "adam": Adam, "adamw": AdamW, "adagrad": Adagrad, "ftrl": Ftrl,
+            "rmsprop": RMSprop}
 
 
 def get(identifier) -> Optimizer:

@@ -151,7 +151,8 @@ __global__ void tfy_barrier_kernel(TfyCommCtx c) { tfy_block_barrier(c); }
 // ---------------------------------------------------------------------------
 // GT: gradient dtype in the symmetric grad buffer, PT: dtype of the replicated
 // compute parameters.  master/s1/s2: local fp32 arrays of shard_n elements
-// (rank r owns elements [r*shard_n, (r+1)*shard_n) of the flat buffers).
+// (rank r owns elements [r*shard_n, (r+1)*shard_n) of the flat buffers); RMSprop's s2 holds up to two states
+// back to back (tfy_rmsprop_states).
 // [g_lo, g_hi): shard-relative groups of 8 elements this launch handles (the whole shard for the classic single
 // launch).  Splitting a step into ranges lets the engine run the update of gradients that are final early (the
 // big Dense kernel) inside the convolution-backward kernel (tfy_overlap_role) while this launch only handles the
@@ -175,8 +176,10 @@ tfy_fused_step_kernel(TfyCommCtx c, uint64_t grad_off, uint64_t param_off, size_
     // launch, on the preceding backward kernel): its loads are issued BEFORE the dependency wait, the cross-GPU
     // barrier and the (2-3 us) in-switch reduction, so their latency hides behind all three.  (TFY_PDL_K4=1
     // assumes a different kernel separates two fused-step launches on the stream -- true for every train step.)
-    TfyStepRegs<U> r;
-    tfy_step_load_state<OPT, U>(r, OPT, master, s1, s2, tid, nthreads, g_hi);
+    TfyStepRegs<U, OPT == TFY_OPT_RMSPROP> r;
+    float* s3 = nullptr;
+    if constexpr (OPT == TFY_OPT_RMSPROP) tfy_rmsprop_states(hp, shard_n, s2, s3);
+    tfy_step_load_state<OPT, U>(r, OPT, master, s1, s2, tid, nthreads, g_hi, s3);
     tfy_pdl_wait();                                     // the gradients of THIS rank are complete
     const TfyStepConsts k = tfy_step_consts(hp, c.world, OPT);
     const int step = hp->step;
@@ -186,8 +189,9 @@ tfy_fused_step_kernel(TfyCommCtx c, uint64_t grad_off, uint64_t param_off, size_
 
     for (size_t g8 = tid; g8 < g_hi; g8 += nthreads * U) {
         tfy_step_batch<GT, PT, OPT, MODE, U>(c, OPT, MODE, k, r, grad_off, param_off, shard_start, master, s1, s2, g8,
-                                             nthreads, g_hi);
-        if (g8 + nthreads * U < g_hi) tfy_step_load_state<OPT, U>(r, OPT, master, s1, s2, g8 + nthreads * U, nthreads, g_hi);
+                                             nthreads, g_hi, s3);
+        if (g8 + nthreads * U < g_hi)
+            tfy_step_load_state<OPT, U>(r, OPT, master, s1, s2, g8 + nthreads * U, nthreads, g_hi, s3);
     }
 
     // updated params visible on every rank before the grid completes; with zero_grads every CTA waits, because it
@@ -324,6 +328,7 @@ static int tfy_fused_step_groups(const TfyCommCtx* c, int grad_dtype, int param_
         else if (opt == TFY_OPT_ADADELTA) TFY_FS3(GT, PT, TFY_OPT_ADADELTA); \
         else if (opt == TFY_OPT_ADAM) TFY_FS3(GT, PT, TFY_OPT_ADAM); \
         else if (opt == TFY_OPT_FTRL) TFY_FS3(GT, PT, TFY_OPT_FTRL); \
+        else if (opt == TFY_OPT_RMSPROP) TFY_FS3(GT, PT, TFY_OPT_RMSPROP); \
         else TFY_FS3(GT, PT, TFY_OPT_ADAGRAD);                     \
     } while (0)
     if (grad_dtype == TFY_BF16 && param_dtype == TFY_BF16) TFY_FS2(__nv_bfloat16, __nv_bfloat16);

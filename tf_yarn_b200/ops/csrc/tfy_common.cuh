@@ -31,20 +31,21 @@ struct TfyCommCtx {
 // and the step counter advancing without being re-captured.
 struct TfyOptHyper {
     float lr;
-    float p1;            // Adadelta: rho   | Adam: beta1 | SGD: momentum | Adagrad: initial acc (unused in kernel)
-    float p2;            // Adam: beta2     | SGD: dampening
+    float p1;            // Adadelta: rho   | Adam: beta1 | SGD: momentum | Adagrad: initial acc (unused in kernel) | RMSprop: rho
+    float p2;            // Adam: beta2     | SGD: dampening | RMSprop: momentum
     float eps;
     float weight_decay;
     float grad_scale;    // multiplied into the (already averaged) gradient, e.g. 1/loss_scale
     int32_t step;        // completed optimizer steps
-    int32_t flags;       // bit0: nesterov (SGD) / decoupled weight decay (Adam)
+    int32_t flags;       // bit0: nesterov (SGD) / decoupled weight decay (Adam) / centered (RMSprop)
     uint32_t done;       // CTA completion counter used to advance `step` exactly once per launch
     uint32_t pad;
 };
 
 enum TfyDtype { TFY_BF16 = 0, TFY_F32 = 1 };
 enum TfyAlgo { TFY_ALGO_ONESHOT = 0, TFY_ALGO_TWOSHOT = 1, TFY_ALGO_NVLS = 2 };
-enum TfyOpt { TFY_OPT_SGD = 0, TFY_OPT_ADADELTA = 1, TFY_OPT_ADAM = 2, TFY_OPT_ADAGRAD = 3, TFY_OPT_FTRL = 4 };
+enum TfyOpt { TFY_OPT_SGD = 0, TFY_OPT_ADADELTA = 1, TFY_OPT_ADAM = 2, TFY_OPT_ADAGRAD = 3, TFY_OPT_FTRL = 4,
+               TFY_OPT_RMSPROP = 5 };
 enum TfyMode { TFY_MODE_LOCAL = 0, TFY_MODE_P2P = 1, TFY_MODE_NVLS = 2 };
 
 // ---------------------------------------------------------------------------

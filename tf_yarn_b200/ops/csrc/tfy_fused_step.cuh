@@ -129,6 +129,44 @@ __device__ __forceinline__ void tfy_opt_update_rt(int opt_rt, float& p, float g,
     }
 }
 
+// Three-state form: RMSprop (tf.keras): s1 = v (mean square), s2 = momentum buffer, s3 = mean gradient (centered);
+// p1 = rho, p2 = momentum, flags bit 0 = centered.  As in Keras, epsilon sits inside the square root and lr inside
+// the momentum buffer.  Every other optimizer ignores s3.
+template <int OPT_T>
+__device__ __forceinline__ void tfy_opt_update_rt(int opt_rt, float& p, float g, float& s1, float& s2, float& s3,
+                                                  const float lr, const float p1, const float p2, const float eps,
+                                                  const float wd, const int flags, const float lr_bc1,
+                                                  const float bc2_rsqrt, const bool first_step) {
+    const int opt = OPT_T >= 0 ? OPT_T : opt_rt;
+    if (opt == TFY_OPT_RMSPROP) {
+        g += wd * p;
+        s1 = p1 * s1 + (1.f - p1) * g * g;
+        float denom = s1;
+        if (flags & 1) {
+            s3 = p1 * s3 + (1.f - p1) * g;
+            denom -= s3 * s3;
+        }
+        const float inc = lr * g * tfy_rsqrt_approx(denom + eps);
+        if (p2 > 0.f) {
+            s2 = p2 * s2 + inc;
+            p -= s2;
+        } else {
+            p -= inc;
+        }
+    } else {
+        tfy_opt_update_rt<OPT_T>(opt_rt, p, g, s1, s2, lr, p1, p2, eps, wd, flags, lr_bc1, bc2_rsqrt, first_step);
+    }
+}
+
+// RMSprop's optional states share the s2 buffer back to back, each shard_n long, momentum first.  On return s2 is
+// the momentum buffer and s3 the mean-gradient buffer, each nullptr when that state is off.
+__device__ __forceinline__ void tfy_rmsprop_states(const TfyOptHyper* hp, size_t shard_n, float* __restrict__& s2,
+                                                   float*& s3) {
+    const bool momentum = hp->p2 > 0.f, centered = (hp->flags & 1) != 0;
+    s3 = centered ? (momentum ? s2 + shard_n : s2) : nullptr;
+    if (!momentum) s2 = nullptr;
+}
+
 struct TfyStepConsts {
     float lr, p1, p2, eps, wd, gscale, lr_bc1, bc2_rsqrt;
     int flags;
@@ -151,17 +189,25 @@ __device__ __forceinline__ TfyStepConsts tfy_step_consts(const TfyOptHyper* hp, 
     return k;
 }
 
-// State of U groups held in registers between the (early) state loads and the update.
-template <int U>
+// State of U groups held in registers between the (early) state loads and the update; THREE adds the third state
+// of RMSprop (s3, see tfy_rmsprop_states).
+template <int U, bool THREE = false>
 struct TfyStepRegs {
     float4 m[U][2], x[U][2], y[U][2];
 };
+template <int U>
+struct TfyStepRegs<U, true> {
+    float4 m[U][2], x[U][2], y[U][2], z[U][2];
+};
 
-template <int OPT_T, int U>
-__device__ __forceinline__ void tfy_step_load_state(TfyStepRegs<U>& r, int opt_rt, const float* master, const float* s1,
-                                                    const float* s2, size_t g_first, size_t stride, size_t g_hi) {
+// RMSprop's s2 / s3 may be nullptr (state off): nothing is loaded or stored for them
+template <int OPT_T, int U, bool THREE>
+__device__ __forceinline__ void tfy_step_load_state(TfyStepRegs<U, THREE>& r, int opt_rt, const float* master,
+                                                    const float* s1, const float* s2, size_t g_first, size_t stride,
+                                                    size_t g_hi, const float* s3 = nullptr) {
     const int opt = OPT_T >= 0 ? OPT_T : opt_rt;
-    const bool two = (opt == TFY_OPT_ADADELTA || opt == TFY_OPT_ADAM || opt == TFY_OPT_FTRL);
+    const bool two = (opt == TFY_OPT_ADADELTA || opt == TFY_OPT_ADAM || opt == TFY_OPT_FTRL) ||
+                     (opt == TFY_OPT_RMSPROP && s2 != nullptr);
 #pragma unroll
     for (int u = 0; u < U; ++u) {
         const size_t g8 = g_first + (size_t)u * stride;
@@ -174,22 +220,29 @@ __device__ __forceinline__ void tfy_step_load_state(TfyStepRegs<U>& r, int opt_r
                 const float4* tp = reinterpret_cast<const float4*>(s2 + g8 * 8);
                 r.y[u][0] = tp[0]; r.y[u][1] = tp[1];
             }
+            if constexpr (THREE) {
+                if (s3 != nullptr) {
+                    const float4* zp = reinterpret_cast<const float4*>(s3 + g8 * 8);
+                    r.z[u][0] = zp[0]; r.z[u][1] = zp[1];
+                }
+            }
         }
     }
 }
 
 // Groups g_first + u*stride (u < U), all < g_hi handled; state must have been loaded into `r`.
-template <typename GT, typename PT, int OPT_T, int MODE_T, int U>
+template <typename GT, typename PT, int OPT_T, int MODE_T, int U, bool THREE>
 __device__ __forceinline__ void tfy_step_batch(const TfyCommCtx& c, int opt_rt, int mode_rt, const TfyStepConsts& k,
-                                               TfyStepRegs<U>& r, uint64_t grad_off, uint64_t param_off,
+                                               TfyStepRegs<U, THREE>& r, uint64_t grad_off, uint64_t param_off,
                                                size_t shard_start, float* master, float* s1, float* s2,
-                                               size_t g_first, size_t stride, size_t g_hi) {
+                                               size_t g_first, size_t stride, size_t g_hi, float* s3 = nullptr) {
     using GP = TfyPack<GT>;
     using PP = TfyPack<PT>;
     constexpr int NG = 8 / GP::N;  // 16-byte packs per 8 gradient elements
     constexpr int NP = 8 / PP::N;
     const int opt = OPT_T >= 0 ? OPT_T : opt_rt;
-    const bool two = (opt == TFY_OPT_ADADELTA || opt == TFY_OPT_ADAM || opt == TFY_OPT_FTRL);
+    const bool two = (opt == TFY_OPT_ADADELTA || opt == TFY_OPT_ADAM || opt == TFY_OPT_FTRL) ||
+                     (opt == TFY_OPT_RMSPROP && s2 != nullptr);
     float g[U][8];
 #pragma unroll
     for (int u = 0; u < U; ++u) {
@@ -218,10 +271,30 @@ __device__ __forceinline__ void tfy_step_batch(const TfyCommCtx& c, int opt_rt, 
 #pragma unroll
             for (int q = 0; q < 8; ++q) b[q] = 0.f;
         }
+        if constexpr (THREE) {
+            float z[8];
+            if (s3 != nullptr) {
+                z[0] = r.z[u][0].x; z[1] = r.z[u][0].y; z[2] = r.z[u][0].z; z[3] = r.z[u][0].w;
+                z[4] = r.z[u][1].x; z[5] = r.z[u][1].y; z[6] = r.z[u][1].z; z[7] = r.z[u][1].w;
+            } else {
 #pragma unroll
-        for (int q = 0; q < 8; ++q)
-            tfy_opt_update_rt<OPT_T>(opt_rt, p[q], g[u][q] * k.gscale, a[q], b[q], k.lr, k.p1, k.p2, k.eps, k.wd,
-                                     k.flags, k.lr_bc1, k.bc2_rsqrt, k.first_step);
+                for (int q = 0; q < 8; ++q) z[q] = 0.f;
+            }
+#pragma unroll
+            for (int q = 0; q < 8; ++q)
+                tfy_opt_update_rt<OPT_T>(opt_rt, p[q], g[u][q] * k.gscale, a[q], b[q], z[q], k.lr, k.p1, k.p2, k.eps,
+                                         k.wd, k.flags, k.lr_bc1, k.bc2_rsqrt, k.first_step);
+            if (s3 != nullptr) {
+                float4* zp = reinterpret_cast<float4*>(s3 + g8 * 8);
+                zp[0] = make_float4(z[0], z[1], z[2], z[3]);
+                zp[1] = make_float4(z[4], z[5], z[6], z[7]);
+            }
+        } else {
+#pragma unroll
+            for (int q = 0; q < 8; ++q)
+                tfy_opt_update_rt<OPT_T>(opt_rt, p[q], g[u][q] * k.gscale, a[q], b[q], k.lr, k.p1, k.p2, k.eps, k.wd,
+                                         k.flags, k.lr_bc1, k.bc2_rsqrt, k.first_step);
+        }
         float4* mp = reinterpret_cast<float4*>(master + g8 * 8);
         mp[0] = make_float4(p[0], p[1], p[2], p[3]);
         mp[1] = make_float4(p[4], p[5], p[6], p[7]);
@@ -246,6 +319,8 @@ __device__ __forceinline__ void tfy_step_batch(const TfyCommCtx& c, int opt_rt, 
 // while the compute CTAs run the convolution weight gradient.  Co-residency with the compute CTAs is guaranteed
 // by construction (one CTA per SM, grid <= #SMs), which a second kernel on a side stream cannot promise.
 // bf16 gradients and parameters; optimizer and transport are runtime values (the role is latency-bound).
+// RMSprop has no role instantiation (its third state is not part of TfyOverlapStep): the host never builds a
+// descriptor for it (FusedShardedOptimizer.overlap_step raises) and the trailing launch updates every group.
 // Cross-GPU protocol: ONE barrier (slots `slot0 + i`) before the reduction; the all-gathered parameters are
 // published by the exit barrier of the trailing tfy_fused_step launch of the same step (stream order).
 // ---------------------------------------------------------------------------------------------------------

@@ -19,7 +19,7 @@ FLAGS_BYTES = MAX_BLOCKS * MAX_RANKS * 4
 
 BF16, F32 = 0, 1
 ALGO_ONESHOT, ALGO_TWOSHOT, ALGO_NVLS = 0, 1, 2
-OPT_SGD, OPT_ADADELTA, OPT_ADAM, OPT_ADAGRAD, OPT_FTRL = 0, 1, 2, 3, 4
+OPT_SGD, OPT_ADADELTA, OPT_ADAM, OPT_ADAGRAD, OPT_FTRL, OPT_RMSPROP = 0, 1, 2, 3, 4, 5
 MODE_LOCAL, MODE_P2P, MODE_NVLS = 0, 1, 2
 
 

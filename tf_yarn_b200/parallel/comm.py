@@ -310,7 +310,7 @@ class FusedShardedOptimizer:
         self.flat_grads.zero_()
         self.master = torch.zeros(self.shard_n, dtype=torch.float32, device=dev)
         self.s1 = torch.full((self.shard_n,), spec.init_s1, dtype=torch.float32, device=dev)
-        self.s2 = torch.zeros(self.shard_n if spec.n_states > 1 else 8, dtype=torch.float32, device=dev)
+        self.s2 = torch.zeros(spec.s2_numel(self.shard_n), dtype=torch.float32, device=dev)
         self._hyper_host = native.OptHyper(spec.lr, spec.p1, spec.p2, spec.eps, spec.weight_decay, 1.0, 0,
                                            spec.flags, 0, 0)
         self.hyper = torch.zeros(ctypes.sizeof(native.OptHyper), dtype=torch.uint8, device=dev)
@@ -411,6 +411,9 @@ class FusedShardedOptimizer:
         ``step(shard_groups=(0, g0))`` of the same training step publishes the result (its exit barrier)."""
         if self.grad_dtype != torch.bfloat16 or self.param_dtype != torch.bfloat16:
             raise ValueError("overlap_step needs bf16 gradients and parameters")
+        if self.spec.kind == "rmsprop":
+            raise ValueError("overlap_step does not run RMSprop: its states do not fit the descriptor; "
+                             "update every group with step()")
         c = self.comm
         ov = native.OverlapStep()
         ov.c = c.arena.ctx
@@ -422,14 +425,17 @@ class FusedShardedOptimizer:
         return ov
 
     # -- checkpoint support ----------------------------------------------------
+    def _states(self):
+        """(name, shard) of every fp32 array the step updates; the states after ``s1`` are consecutive
+        ``shard_n``-long parts of the ``s2`` buffer."""
+        out = [("master", self.master), ("s1", self.s1)]
+        for i in range(1, self.spec.n_states):
+            out.append((f"s{i + 1}", self.s2[(i - 1) * self.shard_n:i * self.shard_n]))
+        return out
+
     def gather_state(self) -> dict:
         """Materialise full (unsharded) fp32 master / state tensors on every rank."""
-        c = self.comm
-        out = {}
-        for name, t in (("master", self.master), ("s1", self.s1), ("s2", self.s2)):
-            if name == "s2" and self.spec.n_states < 2:
-                continue
-            out[name] = self._gather_full(t)
+        out = {name: self._gather_full(t) for name, t in self._states()}
         out["step"] = self.step_count
         return out
 
@@ -448,10 +454,9 @@ class FusedShardedOptimizer:
     def load_state(self, state: dict) -> None:
         r = self.comm.rank if self.comm.world > 1 else 0
         sl = slice(r * self.shard_n, (r + 1) * self.shard_n)
-        self.master.copy_(state["master"][sl])
-        self.s1.copy_(state["s1"][sl])
-        if "s2" in state and self.spec.n_states > 1:
-            self.s2.copy_(state["s2"][sl])
+        for name, t in self._states():
+            if name in ("master", "s1") or name in state:
+                t.copy_(state[name][sl])
         self.flat_params.copy_(state["master"].to(self.flat_params.device).to(self.param_dtype))
         self.set_step_count(int(state.get("step", 0)))
 

@@ -162,17 +162,21 @@ class DistributedDataParallel(nn.Module):
     def fuse_optimizer(self, kind: str = "sgd", **hyper):
         """Move the optimizer INTO the gradient exchange: every bucket runs the fused reduce-scatter -> update
         -> all-gather kernel (K4: ``multimem.ld_reduce`` of the owned 1/world shard, SGD-momentum / Adam / Adagrad /
-        Adadelta on fp32 master + sharded state, ``multimem.st`` of the new parameters) on the communication stream
-        as soon as its gradients are complete, so the whole optimizer step overlaps backward.  Parameters are
+        Adadelta / RMSprop on fp32 master + sharded state, ``multimem.st`` of the new parameters) on the communication
+        stream as soon as its gradients are complete, so the whole optimizer step overlaps backward.  Parameters are
         re-pointed at flat symmetric buffers.  Returns an optimizer-shaped object (``step`` / ``zero_grad`` are
         no-ops: by the time backward returns, the update is queued behind it).  Gradient clipping between
-        ``backward()`` and ``step()`` is not available in this mode."""
+        ``backward()`` and ``step()`` is not available in this mode.
+
+        ``hyper`` are the keyword arguments of the matching ``OptimizerSpec`` constructor, e.g.
+        ``fuse_optimizer("rmsprop", lr=1e-3, rho=0.9, momentum=0.9, eps=1e-7, centered=True)`` for the Keras
+        RMSprop (epsilon inside the square root, lr inside the momentum buffer)."""
         if not self._reducer:
             raise RuntimeError("fuse_optimizer needs the native reducer (CUDA)")
         if self._fused is not None:
             return self._fused
         kinds = {"sgd": OptimizerSpec.sgd, "adam": OptimizerSpec.adam, "adagrad": OptimizerSpec.adagrad,
-                 "adadelta": OptimizerSpec.adadelta}
+                 "adadelta": OptimizerSpec.adadelta, "rmsprop": OptimizerSpec.rmsprop}
         if kind not in kinds:
             raise ValueError(f"unknown fused optimizer {kind!r}")
         spec = kinds[kind](**hyper)
@@ -192,7 +196,7 @@ class DistributedDataParallel(nn.Module):
             r = comm.rank if world > 1 else 0
             b.master = b.pflat[r * b.shard_n:(r + 1) * b.shard_n].float().clone()
             b.s1 = torch.full((b.shard_n,), spec.init_s1, dtype=torch.float32, device=dev)
-            b.s2 = torch.zeros(b.shard_n if spec.n_states > 1 else 8, dtype=torch.float32, device=dev)
+            b.s2 = torch.zeros(spec.s2_numel(b.shard_n), dtype=torch.float32, device=dev)
             host = native.OptHyper(spec.lr, spec.p1, spec.p2, spec.eps, spec.weight_decay, 1.0, 0, spec.flags, 0, 0)
             b.hyper = torch.frombuffer(bytearray(bytes(host)), dtype=torch.uint8).to(dev)
             native.check(comm.lib.tfy_reducer_set_fused(

@@ -1,14 +1,14 @@
 """Fused-optimizer hyper-parameter description (no CUDA dependency)."""
 from __future__ import annotations
 
-OPT_SGD, OPT_ADADELTA, OPT_ADAM, OPT_ADAGRAD, OPT_FTRL = 0, 1, 2, 3, 4
+OPT_SGD, OPT_ADADELTA, OPT_ADAM, OPT_ADAGRAD, OPT_FTRL, OPT_RMSPROP = 0, 1, 2, 3, 4, 5
 
 
 class OptimizerSpec:
     """Hyper-parameters of a fused optimizer (device-independent description)."""
 
     KINDS = {"sgd": OPT_SGD, "adadelta": OPT_ADADELTA, "adam": OPT_ADAM,
-             "adamw": OPT_ADAM, "adagrad": OPT_ADAGRAD, "ftrl": OPT_FTRL}
+             "adamw": OPT_ADAM, "adagrad": OPT_ADAGRAD, "ftrl": OPT_FTRL, "rmsprop": OPT_RMSPROP}
 
     def __init__(self, kind: str, lr: float, p1: float = 0.0, p2: float = 0.0, eps: float = 1e-7,
                  weight_decay: float = 0.0, flags: int = 0, init_s1: float = 0.0):
@@ -26,7 +26,14 @@ class OptimizerSpec:
 
     @property
     def n_states(self) -> int:
+        if self.kind == "rmsprop":
+            return 1 + (self.p2 > 0) + (self.flags & 1)
         return 2 if self.kind in ("adadelta", "adam", "adamw", "ftrl") else 1
+
+    def s2_numel(self, shard_n: int) -> int:
+        """Length of the fp32 ``s2`` buffer of a shard of ``shard_n`` elements: every state after the first, back to
+        back (at least 8 elements, so the kernel always gets a valid pointer)."""
+        return max(8, shard_n * (self.n_states - 1))
 
     @staticmethod
     def sgd(lr, momentum=0.0, dampening=0.0, nesterov=False, weight_decay=0.0):
@@ -49,3 +56,12 @@ class OptimizerSpec:
         """FTRL-proximal with learning_rate_power = -0.5 (TF's FtrlOptimizer default): s1 = accumulator n
         (initial_accumulator_value), s2 = linear z; p1 = l1, p2 = l2, eps carries beta."""
         return OptimizerSpec("ftrl", lr, l1, l2, beta, weight_decay, init_s1=initial_accumulator_value)
+
+    @staticmethod
+    def rmsprop(lr=1e-3, rho=0.9, momentum=0.0, eps=1e-7, centered=False, weight_decay=0.0):
+        """RMSprop as tf.keras defines it (epsilon inside the square root, lr inside the momentum buffer): s1 = mean
+        square; s2 = momentum buffer (momentum > 0) then mean gradient (centered), each shard long; p1 = rho,
+        p2 = momentum, flags bit 0 = centered."""
+        if momentum < 0:
+            raise ValueError(f"RMSprop momentum must be >= 0, got {momentum}")
+        return OptimizerSpec("rmsprop", lr, rho, momentum, eps, weight_decay, 1 if centered else 0)
