@@ -134,7 +134,7 @@ def _hbm_connection(network, opt="adagrad", n_ps=2):
     conn._classify(network)
     conn.dense_idx = [i for i in range(len(conn.names)) if i not in conn.sparse]
     conn.pull_idx = [i for i in conn.dense_idx if i not in conn.gemm]
-    conn.adam_scale = torch.ones(1)
+    conn.adam_scale = torch.ones(2)
     conn._acct = {"pull_bytes": 0, "push_bytes": 0, "launches_per_step": 0}
     return conn
 

@@ -42,11 +42,12 @@ native.declare("tfy_ps_push", [_vp, _i, _sz, _i, _f, _vp, _vp])
 native.declare("tfy_ps_refresh_shadow", [_vp, _i, _sz, _vp])
 native.declare("tfy_dense_bwd", [_vp, _vp, _vp, _vp, _vp, _i, _i, _i, _vp])
 native.declare("tfy_ps_embedding_bag", [_vp, _vp, _vp, _i, _i, _i, _i, _ll, _i, _vp])
+native.declare("tfy_ps_push_rows_scratch_bytes", [_ll], _sz)
 native.declare("tfy_ps_push_rows", [_vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _ll, _i, _i, _f, _f, _f, _f, _f, _f, _vp,
-                                    _i, _vp])
+                                    _i, _vp, _sz, _vp])
 native.declare("tfy_ps_multi_bag", [_vp, _vp, _vp, _i, _i, _i, _i, _ll, _vp])
 native.declare("tfy_ps_multi_push_rows", [_vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _ll, _i, _f, _f, _f, _f, _f, _f, _vp, _i,
-                                          _i, _vp])
+                                          _i, _vp, _sz, _vp])
 native.declare("tfy_ps_gather_gemm", [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _ll, _vp])
 
 OPT_CODES = {"sgd": native.OPT_SGD, "adagrad": native.OPT_ADAGRAD, "adam": native.OPT_ADAM,
@@ -60,6 +61,20 @@ class PsSeg(ctypes.Structure):
                 ("opt", ctypes.c_int32), ("lr", ctypes.c_float), ("eps", ctypes.c_float), ("wd", ctypes.c_float),
                 ("p1", ctypes.c_float), ("p2", ctypes.c_float), ("p3", ctypes.c_float), ("pad", ctypes.c_int32),
                 ("cols", ctypes.c_uint32), ("shadow_ld", ctypes.c_uint32)]
+
+
+def push_rows_launches(per_table: int) -> int:
+    """Kernel launches of one sparse push of `per_table` ids per table: a per-table block sort (up to 2048 ids per
+    table, tfy_ps.cu kPsBlockSortMax) or the key kernel and CUB's device radix sort (histogram, scan and one kernel
+    per 8-bit pass, counted here as one launch), then the short-run and long-run apply kernels."""
+    return 3 if per_table <= 2048 else 4
+
+
+def push_rows_scratch(lib, n: int, device) -> torch.Tensor:
+    """Device scratch of a sparse push of n ids (tfy_ps_push_rows / tfy_ps_multi_push_rows fold duplicates in it).
+    Allocated per push from the caching allocator, so a captured CUDA graph keeps its own."""
+    nbytes = int(lib.tfy_ps_push_rows_scratch_bytes(n)) if n > 0 else 0
+    return torch.empty(max(nbytes, 1), dtype=torch.uint8, device=device)
 
 
 def cluster_ranks(cluster) -> Dict[str, int]:
@@ -122,11 +137,11 @@ class HbmConnection:
         self._max_n = max([self._n4(i) for i in self.dense_idx] + [4])
         self.pull_stream = torch.cuda.Stream(device=dev)
         self._pull_done: Optional[torch.cuda.Event] = None
-        # Adam bias correction sqrt(1-b2^t)/(1-b1^t): a device scalar the push kernels read, refreshed from the
-        # global step before every push (so a captured CUDA graph sees it advance)
+        # Adam bias correction {1/(1-b1^t), 1/sqrt(1-b2^t)}: device scalars the push kernels read, refreshed from the
+        # global step before every push (so a captured CUDA graph sees them advance)
         self._adam = [i for i, k in enumerate(layout.kinds) if k == "adam"]
-        self.adam_scale = torch.ones(1, dtype=torch.float32, device=dev)
-        self._adam_host = torch.ones(1, dtype=torch.float32).pin_memory() if self._adam else None
+        self.adam_scale = torch.ones(2, dtype=torch.float32, device=dev)
+        self._adam_host = torch.ones(2, dtype=torch.float32).pin_memory() if self._adam else None
         # NVLink traffic / kernel launches of one step, counted on the host while a step runs eagerly (the
         # captured graph replays exactly the same launches)
         self._acct = {"pull_bytes": 0, "push_bytes": 0, "launches_per_step": 0}
@@ -260,7 +275,8 @@ class HbmConnection:
             return
         h = self.layout.hypers[self._adam[0]]
         t = max(self.global_step(), 0) + 1
-        self._adam_host[0] = (1.0 - h["p2"] ** t) ** 0.5 / (1.0 - h["p1"] ** t)
+        self._adam_host[0] = 1.0 / (1.0 - h["p1"] ** t)
+        self._adam_host[1] = 1.0 / (1.0 - h["p2"] ** t) ** 0.5
         self.adam_scale.copy_(self._adam_host, non_blocking=True)
 
     def refresh_shadows(self) -> None:
@@ -312,11 +328,13 @@ def _make_bag_forward(conn: HbmConnection, idx: int, mod: nn.EmbeddingBag):
             s1 = conn.master_ptr(idx, 1) if lay.var_slots[idx] >= 1 else None
             s2 = conn.master_ptr(idx, 2) if lay.var_slots[idx] >= 2 else None
             p3 = float(h["eps"]) if lay.kinds[idx] == "ftrl" else 0.0
+            scratch = push_rows_scratch(lib, B * L, dout.device)
             native.check(lib.tfy_ps_push_rows(conn.master_ptr(idx), s1, s2, ids.data_ptr(), dout.data_ptr(), 0, B, L, D,
                                               V, mean, conn.var_opt[idx], float(h["lr"]), float(h["eps"]),
                                               float(h["p1"]), float(h["p2"]), p3, 1.0, conn.adam_scale.data_ptr(), 0,
+                                              scratch.data_ptr(), scratch.numel(),
                                               torch.cuda.current_stream().cuda_stream), "tfy_ps_push_rows")
-            conn.account(push=B * L * D * 4 * (1 + lay.var_slots[idx]))
+            conn.account(push=B * L * D * 4 * (1 + lay.var_slots[idx]), launches=push_rows_launches(B * L))
             return None, None
 
     anchor = torch.zeros((), device=conn.device, requires_grad=True)
@@ -400,13 +418,14 @@ class _TableGroup:
     def push(self, ids: torch.Tensor, dout: torch.Tensor, D: int, dout_ld: int, col_stride: int) -> None:
         conn, h = self.conn, self.h
         B, T = ids.shape[1], len(self.idx)
+        scratch = push_rows_scratch(conn.lib, T * B, dout.device)
         native.check(conn.lib.tfy_ps_multi_push_rows(
             self.tables.data_ptr(), self.s1.data_ptr() if self.s1 is not None else None,
             self.s2.data_ptr() if self.s2 is not None else None, ids.data_ptr(), dout.data_ptr(),
             1 if dout.dtype == torch.bfloat16 else 0, B, T, D, self.V, self.opt, float(h["lr"]), float(h["eps"]),
             float(h["p1"]), float(h["p2"]), self.p3, 1.0, conn.adam_scale.data_ptr(), dout_ld, col_stride,
-            torch.cuda.current_stream().cuda_stream), "tfy_ps_multi_push_rows")
-        conn.account(push=T * B * D * 4 * (1 + self.slots))
+            scratch.data_ptr(), scratch.numel(), torch.cuda.current_stream().cuda_stream), "tfy_ps_multi_push_rows")
+        conn.account(push=T * B * D * 4 * (1 + self.slots), launches=push_rows_launches(B))
 
 
 def _try_fuse_wide_tower(conn: HbmConnection, network: nn.Module) -> bool:
@@ -552,11 +571,12 @@ def _try_fuse_first_layer(conn: HbmConnection, network: nn.Module) -> bool:
                 s1 = conn.master_ptr(ti, 1) if lay.var_slots[ti] >= 1 else None
                 s2 = conn.master_ptr(ti, 2) if lay.var_slots[ti] >= 2 else None
                 p3 = float(h["eps"]) if lay.kinds[ti] == "ftrl" else 0.0
+                scratch = push_rows_scratch(lib, B, dev)
                 native.check(lib.tfy_ps_push_rows(
                     conn.master_ptr(ti), s1, s2, ids[t].data_ptr(), dx.data_ptr() + 2 * 64 * t, 1, B, 1, 64, V, 0,
                     conn.var_opt[ti], float(h["lr"]), float(h["eps"]), float(h["p1"]), float(h["p2"]), p3, 1.0,
-                    conn.adam_scale.data_ptr(), Kp, s), "tfy_ps_push_rows")
-                conn.account(push=B * 64 * 4 * (1 + lay.var_slots[ti]))
+                    conn.adam_scale.data_ptr(), Kp, scratch.data_ptr(), scratch.numel(), s), "tfy_ps_push_rows")
+                conn.account(push=B * 64 * 4 * (1 + lay.var_slots[ti]), launches=push_rows_launches(B))
             return None, None, dw[:, :K].to(weight.dtype), dy.float().sum(0).to(weight.dtype)
 
     class _Deferred:

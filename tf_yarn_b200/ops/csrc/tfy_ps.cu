@@ -16,10 +16,20 @@
 //                    Adagrad  acc += g^2 ; w += -lr*g/(sqrt(acc)+eps)            (atom.v4.f32 returns old acc)
 //                    FTRL     n += g^2 ; z += g - (sqrt(n')-sqrt(n))/lr * w ;    (two atom.v4.f32)
 //                             w  = |z|<=l1 ? 0 : -(z - sgn(z) l1) / ((beta+sqrt(n'))/lr + 2 l2)
-//                    Adam     m = b1 m + (1-b1) g ; v = b2 v + (1-b2) g^2 ;      (hogwild read-modify-write of m, v)
-//                             w += -lr_t m/(sqrt(v)+eps)                         (red.v4.f32)
+//                    Adam     m = b1 m + (1-b1) g ; v = b2 v + (1-b2) g^2 ;      (read-modify-write of m, v)
+//                             w += -lr/(1-b1^t) m/(sqrt(v)/sqrt(1-b2^t)+eps)     (red.v4.f32; torch's formula, as
+//                                                                                 K4 and the CPU plane)
 //                  and refreshes the bf16 shadow copy that the GEMM pull reads
-//          sparse: the same per touched embedding row (duplicate ids handled by the atomics)
+//          sparse: the same per touched embedding row.  The ids of one push are folded first: every distinct
+//                  (table, row) receives the SUM of its gradients (x 1/L for a mean bag) and its optimizer runs ONCE,
+//                  like TF's SparseApply* on IndexedSlices with repeated indices summed.  The fold is a stable radix
+//                  sort of the (table, id) keys into caller-provided scratch, then the apply kernels, which reduce
+//                  every run in a fixed order (a thread per short run, a warp per long one): a push is deterministic
+//                  and needs no host synchronisation (capturable).  Rows outside the batch are not touched, Adam's
+//                  m and v included (lazy Adam).  Out-of-range ids (< 0 or >= V) are skipped.
+#include <cub/block/block_radix_sort.cuh>
+#include <cub/device/device_radix_sort.cuh>
+
 #include "tfy_common.cuh"
 
 struct TfyPsSeg {
@@ -144,10 +154,11 @@ __device__ __forceinline__ float ftrl_w(float z, float n_new, float lr, float l1
 }
 
 // One 4-element pack of an asynchronous update against the peer master: gv already scaled (and decayed).
-// Returns the new weights when they are known (needed for the bf16 shadow), via `neww`; `has_new` tells whether
-// the caller must refresh the shadow from them (true whenever a shadow exists).
+// Returns the new weights when they are known (needed for the bf16 shadow), via `neww`; `want_new` tells whether
+// the caller must refresh the shadow from them (true whenever a shadow exists).  Adam: lr already carries
+// 1/(1-b1^t), vs = 1/sqrt(1-b2^t).
 __device__ __forceinline__ void ps_apply4(int opt, float* w, float* s1, float* s2, float4 gv, float lr, float eps,
-                                          float p1, float p2, float p3, bool want_new, float4& neww) {
+                                          float p1, float p2, float p3, float vs, bool want_new, float4& neww) {
     if (opt == TFY_OPT_FTRL) {
         const float4 g2 = make_float4(gv.x * gv.x, gv.y * gv.y, gv.z * gv.z, gv.w * gv.w);
         const float4 n_old = atom_add_f32x4(s1, g2);
@@ -180,8 +191,8 @@ __device__ __forceinline__ void ps_apply4(int opt, float* w, float* s1, float* s
                         p2 * v.z + (1.f - p2) * gv.z * gv.z, p2 * v.w + (1.f - p2) * gv.w * gv.w);
         st_peer_f32x4(s1, m);
         st_peer_f32x4(s2, v);
-        delta = make_float4(-lr * m.x / (sqrtf(v.x) + eps), -lr * m.y / (sqrtf(v.y) + eps),
-                            -lr * m.z / (sqrtf(v.z) + eps), -lr * m.w / (sqrtf(v.w) + eps));
+        delta = make_float4(-lr * m.x / (sqrtf(v.x) * vs + eps), -lr * m.y / (sqrtf(v.y) * vs + eps),
+                            -lr * m.z / (sqrtf(v.z) * vs + eps), -lr * m.w / (sqrtf(v.w) * vs + eps));
     } else {
         delta = f4_mul(gv, -lr);
     }
@@ -194,7 +205,7 @@ __device__ __forceinline__ void ps_apply4(int opt, float* w, float* s1, float* s
 }
 
 __device__ __forceinline__ float ps_apply1(int opt, float* w, float* s1, float* s2, float g, float lr, float eps, float p1,
-                                           float p2, float p3) {
+                                           float p2, float p3, float vs) {
     if (opt == TFY_OPT_FTRL) {
         const float n_old = atomicAdd(s1, g * g), n_new = n_old + g * g;
         const float dz = g - (sqrtf(n_new) - sqrtf(n_old)) / lr * *w;
@@ -210,18 +221,26 @@ __device__ __forceinline__ float ps_apply1(int opt, float* w, float* s1, float* 
     } else if (opt == TFY_OPT_ADAM) {
         const float m = p1 * *s1 + (1.f - p1) * g, v = p2 * *s2 + (1.f - p2) * g * g;
         *s1 = m; *s2 = v;
-        delta = -lr * m / (sqrtf(v) + eps);
+        delta = -lr * m / (sqrtf(v) * vs + eps);
     } else {
         delta = -lr * g;
     }
     return atomicAdd(w, delta) + delta;
 }
 
+// Adam's bias correction: adam_scale = {1/(1-b1^t), 1/sqrt(1-b2^t)} in device memory (so that a captured CUDA graph
+// sees it advance); nullptr = no correction.  Returns the learning rate to use and sets `vs`.
+__device__ __forceinline__ float ps_adam_lr(int opt, float lr, const float* adam_scale, float& vs) {
+    vs = 1.f;
+    if (opt != TFY_OPT_ADAM || !adam_scale) return lr;
+    vs = adam_scale[1];
+    return lr * adam_scale[0];
+}
+
 }  // namespace
 
 // The optimizer is a per-segment (= per-variable) runtime value (uniform per blockIdx.y).  grad_scale multiplies the
-// local gradient first; adam_scale[0] = sqrt(1-b2^t)/(1-b1^t) lives in device memory so that a captured CUDA graph
-// sees the bias correction advance.
+// local gradient first.
 template <typename GT>
 __global__ void __launch_bounds__(256)
 tfy_ps_push_kernel(const TfyPsSeg* __restrict__ segs, float grad_scale, const float* __restrict__ adam_scale) {
@@ -233,7 +252,8 @@ tfy_ps_push_kernel(const TfyPsSeg* __restrict__ segs, float grad_scale, const fl
     const GT* g = reinterpret_cast<const GT*>(sg.local);
     const int opt = sg.opt;
     const float wd = sg.wd, eps = sg.eps, p1 = sg.p1, p2 = sg.p2, p3 = sg.p3;
-    const float lr = (opt == TFY_OPT_ADAM && adam_scale) ? sg.lr * adam_scale[0] : sg.lr;
+    float vs;
+    const float lr = ps_adam_lr(opt, sg.lr, adam_scale, vs);
     const size_t n4 = sg.n / 4;
     for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n4; i += (size_t)gridDim.x * blockDim.x) {
         float4 gv = f4_mul(ld_local4<GT>(g + i * 4), grad_scale);
@@ -242,14 +262,14 @@ tfy_ps_push_kernel(const TfyPsSeg* __restrict__ segs, float grad_scale, const fl
             gv.x += wd * wv.x; gv.y += wd * wv.y; gv.z += wd * wv.z; gv.w += wd * wv.w;
         }
         float4 neww;
-        ps_apply4(opt, w + i * 4, s1 + i * 4, s2 + i * 4, gv, lr, eps, p1, p2, p3, shadow != nullptr, neww);
+        ps_apply4(opt, w + i * 4, s1 + i * 4, s2 + i * 4, gv, lr, eps, p1, p2, p3, vs, shadow != nullptr, neww);
         if (shadow) st_shadow4(shadow, i * 4, neww, sg.cols, sg.shadow_ld);
     }
     if (blockIdx.x == 0) {   // scalar tail (n % 4 elements)
         for (size_t i = n4 * 4 + threadIdx.x; i < sg.n; i += blockDim.x) {
             float gv = (float)g[i] * grad_scale;
             if (wd != 0.f) gv += wd * w[i];
-            const float nw = ps_apply1(opt, w + i, s1 + i, s2 + i, gv, lr, eps, p1, p2, p3);
+            const float nw = ps_apply1(opt, w + i, s1 + i, s2 + i, gv, lr, eps, p1, p2, p3, vs);
             if (shadow) shadow[shadow_index(i, sg.cols, sg.shadow_ld)] = __float2bfloat16(nw);
         }
     }
@@ -301,49 +321,291 @@ tfy_ps_embedding_bag_scalar_kernel(const float* __restrict__ table, const long l
 }
 
 // ------------------------------------------------------------------------------------ sparse push
-// For every (b, j): row = ids[b, j]; g = dout[b, :] * (mean ? 1/L : 1) applied to the peer row.
-template <typename GT>
+// Both sparse pushes are one gradient scatter.  tfy_ps_push_rows is one table with L ids per example;
+// tfy_ps_multi_push_rows is T tables with one id per example each.  Occurrence o in [0, T*B*L) is id ids[o] of table
+// t = o / (B*L); its gradient is row b = (o % (B*L)) / L of dout, columns [t*col_stride, t*col_stride + D).
+struct TfyPsRows {
+    const uint64_t* tables;  // device arrays of T peer pointers (tfy_ps_multi_push_rows) ...
+    const uint64_t* s1s;
+    const uint64_t* s2s;
+    float* w0;               // ... or, when they are nullptr, the single table of tfy_ps_push_rows
+    float* s10;
+    float* s20;
+    const long long* ids;
+    const void* dout;
+    int B, L, T, D;
+    long long V;
+    int dout_ld, col_stride;
+    float scale;             // grad_scale (x 1/L for a mean bag), applied to the folded sum
+};
+
+namespace {
+__device__ __forceinline__ float* rows_base(const uint64_t* arr, float* one, int t) {
+    return arr ? reinterpret_cast<float*>(arr[t]) : one;
+}
+template <typename GT, int VEC>
+__device__ __forceinline__ float4 ld_grad(const GT* p) {
+    if constexpr (VEC == 4) return ld_local4<GT>(p);
+    else return make_float4((float)p[0], 0.f, 0.f, 0.f);
+}
+}  // namespace
+
+// keys[o] = t * V + id, or T * V (sorts last, never applied) for an out-of-range id; occ[o] = o
 __global__ void __launch_bounds__(256)
-tfy_ps_push_rows_kernel(float* __restrict__ table, float* __restrict__ s1_table, float* __restrict__ s2_table,
-                        const long long* __restrict__ ids, const GT* __restrict__ dout, int B, int L, int D, long long V,
-                        int mean, TfyPsHyper h, const float* __restrict__ adam_scale, int dout_ld) {
-    const int D4 = D / 4;
-    const size_t total = (size_t)B * L * D4;
-    const float scale = (mean ? 1.f / (float)L : 1.f) * h.grad_scale;
-    const float lr = (h.opt == TFY_OPT_ADAM && adam_scale) ? h.lr * adam_scale[0] : h.lr;
-    for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
-        const int d = (i % D4) * 4;
-        const size_t bj = i / D4;
-        const int b = bj / L;
-        const long long id = ids[bj];
-        if (id < 0 || id >= V) continue;
-        const float4 gv = f4_mul(ld_local4<GT>(dout + (size_t)b * dout_ld + d), scale);
-        const size_t o = (size_t)id * D + d;
+tfy_ps_row_keys_kernel(const long long* __restrict__ ids, int n, int per_table, long long V,
+                       unsigned long long* __restrict__ keys, int* __restrict__ occ) {
+    const unsigned long long sentinel = (unsigned long long)(n / per_table) * (unsigned long long)V;
+    for (int o = blockIdx.x * blockDim.x + threadIdx.x; o < n; o += gridDim.x * blockDim.x) {
+        const long long id = ids[o];
+        keys[o] = (id < 0 || id >= V) ? sentinel : (unsigned long long)(o / per_table) * (unsigned long long)V + id;
+        occ[o] = o;
+    }
+}
+
+// The same keys for a push whose per-table segments (B*L occurrences each) fit one block: block t stably sorts
+// segment t in shared memory.  The segments are in table order, so the concatenation is sorted by (table, id) too,
+// except that a segment's out-of-range ids (the sentinel) sit at its end instead of the array's: the apply kernels
+// skip sentinels wherever they are.  One launch instead of a key kernel plus a multi-pass device sort.
+constexpr int kPsSortThreads = 256, kPsSortItems = 8, kPsBlockSortMax = kPsSortThreads * kPsSortItems;
+
+__global__ void __launch_bounds__(kPsSortThreads)
+tfy_ps_segment_sort_kernel(const long long* __restrict__ ids, int per_table, long long V, int local_bits,
+                           unsigned long long* __restrict__ keys, int* __restrict__ occ) {
+    using Sort = cub::BlockRadixSort<unsigned int, kPsSortThreads, kPsSortItems, int>;
+    __shared__ typename Sort::TempStorage tmp;
+    const int t = blockIdx.x;
+    const size_t base = (size_t)t * per_table;
+    const unsigned long long sentinel = (unsigned long long)gridDim.x * (unsigned long long)V;
+    unsigned int k[kPsSortItems];
+    int v[kPsSortItems];
+#pragma unroll
+    for (int j = 0; j < kPsSortItems; ++j) {
+        const int r = threadIdx.x * kPsSortItems + j;               // blocked arrangement: r keeps the original order
+        if (r < per_table) {
+            const long long id = ids[base + r];
+            k[j] = (id < 0 || id >= V) ? (unsigned int)V : (unsigned int)id;
+        } else {
+            k[j] = 0xffffffffu;                                      // padding: after every real key
+        }
+        v[j] = (int)base + r;
+    }
+    Sort(tmp).Sort(k, v, 0, local_bits);
+#pragma unroll
+    for (int j = 0; j < kPsSortItems; ++j) {
+        const int r = threadIdx.x * kPsSortItems + j;
+        if (r < per_table) {
+            keys[base + r] = k[j] == (unsigned int)V ? sentinel : (unsigned long long)t * (unsigned long long)V + k[j];
+            occ[base + r] = v[j];
+        }
+    }
+}
+
+// keys / occ: the occurrences stably sorted by key, so each run of equal keys is one (table, row) with its
+// occurrences in their original order.  Two kernels apply the runs; each sums a run in a fixed order and runs the
+// optimizer once per element, so the result does not depend on scheduling:
+//   short runs (<= kPsShortRun occurrences, nearly every row of a hashed batch): one thread per (run, column group),
+//     all in parallel, summing the run sequentially;
+//   long runs (hot rows, up to the whole batch): a warp per run, its lanes (CL across the row's column groups x OL
+//     along the run) summing strided partial sums that a butterfly reduction combines.
+constexpr int kPsShortRun = 32;
+
+namespace {
+// peer row of `key` (= t * V + id) in table t, with its slots (nullptr when the optimizer has none)
+struct RowRef {
+    float* w;
+    float* s1;
+    float* s2;
+    int t;
+};
+__device__ __forceinline__ RowRef row_of(const TfyPsRows& r, unsigned long long key) {
+    RowRef x;
+    x.t = (int)(key / (unsigned long long)r.V);
+    const size_t row = (size_t)(key % (unsigned long long)r.V) * r.D;
+    x.w = rows_base(r.tables, r.w0, x.t) + row;
+    x.s1 = rows_base(r.s1s, r.s10, x.t);
+    x.s2 = rows_base(r.s2s, r.s20, x.t);
+    if (x.s1) x.s1 += row;
+    if (x.s2) x.s2 += row;
+    return x;
+}
+template <int VEC>
+__device__ __forceinline__ void apply_sum(const TfyPsHyper& h, const RowRef& x, size_t d, float4 acc, float scale,
+                                          float lr, float vs) {
+    if constexpr (VEC == 4) {
         float4 unused;
-        ps_apply4(h.opt, table + o, s1_table + o, s2_table + o, gv, lr, h.eps, h.p1, h.p2, h.p3, false, unused);
+        ps_apply4(h.opt, x.w + d, x.s1 ? x.s1 + d : nullptr, x.s2 ? x.s2 + d : nullptr, f4_mul(acc, scale), lr, h.eps,
+                  h.p1, h.p2, h.p3, vs, false, unused);
+    } else {
+        ps_apply1(h.opt, x.w + d, x.s1 ? x.s1 + d : nullptr, x.s2 ? x.s2 + d : nullptr, acc.x * scale, lr, h.eps, h.p1,
+                  h.p2, h.p3, vs);
     }
 }
+}  // namespace
 
-template <typename GT>
+template <typename GT, int VEC>
 __global__ void __launch_bounds__(256)
-tfy_ps_push_rows_scalar_kernel(float* __restrict__ table, float* __restrict__ s1_table, float* __restrict__ s2_table,
-                               const long long* __restrict__ ids, const GT* __restrict__ dout, int B, int L, int D,
-                               long long V, int mean, TfyPsHyper h, const float* __restrict__ adam_scale, int dout_ld) {
-    const size_t total = (size_t)B * L * D;
-    const float scale = (mean ? 1.f / (float)L : 1.f) * h.grad_scale;
-    const float lr = (h.opt == TFY_OPT_ADAM && adam_scale) ? h.lr * adam_scale[0] : h.lr;
+tfy_ps_apply_short_rows_kernel(TfyPsRows r, TfyPsHyper h, const float* __restrict__ adam_scale,
+                               const unsigned long long* __restrict__ keys, const int* __restrict__ occ, int n) {
+    const int DV = r.D / VEC, BL = r.B * r.L;
+    const unsigned long long sentinel = (unsigned long long)r.T * (unsigned long long)r.V;
+    float vs;
+    const float lr = ps_adam_lr(h.opt, h.lr, adam_scale, vs);
+    const GT* dout = reinterpret_cast<const GT*>(r.dout);
+    const size_t total = (size_t)n * DV;
     for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
-        const int d = i % D;
-        const size_t bj = i / D;
-        const int b = bj / L;
-        const long long id = ids[bj];
-        if (id < 0 || id >= V) continue;
-        const size_t o = (size_t)id * D + d;
-        ps_apply1(h.opt, table + o, s1_table + o, s2_table + o, (float)dout[(size_t)b * dout_ld + d] * scale, lr, h.eps, h.p1,
-                  h.p2, h.p3);
+        const int p = (int)(i / DV), c = (int)(i % DV);
+        const unsigned long long key = keys[p];
+        if (key == sentinel || (p > 0 && keys[p - 1] == key)) continue;          // not the start of a run
+        int e = p + 1;
+        while (e < n && e - p <= kPsShortRun && keys[e] == key) ++e;
+        if (e - p > kPsShortRun) continue;                                        // a long run: the warp kernel's
+        const RowRef x = row_of(r, key);
+        const GT* g = dout + (size_t)x.t * r.col_stride + c * VEC;
+        float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
+        for (int q = p; q < e; ++q) {
+            const float4 gv = ld_grad<GT, VEC>(g + (size_t)((occ[q] % BL) / r.L) * r.dout_ld);
+            acc.x += gv.x; acc.y += gv.y; acc.z += gv.z; acc.w += gv.w;
+        }
+        apply_sum<VEC>(h, x, (size_t)c * VEC, acc, r.scale, lr, vs);
     }
 }
 
+template <typename GT, int VEC>
+__global__ void __launch_bounds__(256)
+tfy_ps_apply_long_rows_kernel(TfyPsRows r, TfyPsHyper h, const float* __restrict__ adam_scale,
+                              const unsigned long long* __restrict__ keys, const int* __restrict__ occ, int n,
+                              int cl_log2) {
+    const int lane = threadIdx.x & 31;
+    const int CL = 1 << cl_log2, OL = 32 >> cl_log2;
+    const int cl = lane & (CL - 1), ol = lane >> cl_log2;
+    const int DV = r.D / VEC, BL = r.B * r.L;
+    const unsigned long long sentinel = (unsigned long long)r.T * (unsigned long long)r.V;
+    float vs;
+    const float lr = ps_adam_lr(h.opt, h.lr, adam_scale, vs);
+    const GT* dout = reinterpret_cast<const GT*>(r.dout);
+    const long long nwarp = (long long)gridDim.x * (blockDim.x >> 5);
+    for (long long base = ((long long)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5)) * 32; base < n;
+         base += nwarp * 32) {
+        const int p = (int)base + lane;
+        const unsigned long long k = p < n ? keys[p] : sentinel;
+        // the starts of runs longer than kPsShortRun (keys are sorted: the run reaches p + kPsShortRun)
+        unsigned starts = __ballot_sync(0xffffffffu, k != sentinel && (p == 0 || keys[p - 1] != k) &&
+                                                         p + kPsShortRun < n && keys[p + kPsShortRun] == k);
+        while (starts) {
+            const int src = __ffs(starts) - 1;
+            starts &= starts - 1;
+            const int p0 = (int)base + src;
+            const unsigned long long key = __shfl_sync(0xffffffffu, k, src);
+            int e = p0 + kPsShortRun + 1;      // the run ends at the first different key
+            for (;;) {
+                const int q = e + lane;
+                const unsigned same = __ballot_sync(0xffffffffu, q < n && keys[q] == key);
+                if (same != 0xffffffffu) {
+                    e += __ffs(~same) - 1;
+                    break;
+                }
+                e += 32;
+            }
+            const RowRef x = row_of(r, key);
+            const GT* g = dout + (size_t)x.t * r.col_stride;
+            for (int c0 = 0; c0 < DV; c0 += CL) {
+                const int c = c0 + cl;
+                float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
+                if (c < DV)
+                    for (int q = p0 + ol; q < e; q += OL) {
+                        const int b = (occ[q] % BL) / r.L;
+                        const float4 gv = ld_grad<GT, VEC>(g + (size_t)b * r.dout_ld + c * VEC);
+                        acc.x += gv.x; acc.y += gv.y; acc.z += gv.z; acc.w += gv.w;
+                    }
+                for (int off = 16; off >= CL; off >>= 1) {
+                    acc.x += __shfl_xor_sync(0xffffffffu, acc.x, off);
+                    if constexpr (VEC == 4) {
+                        acc.y += __shfl_xor_sync(0xffffffffu, acc.y, off);
+                        acc.z += __shfl_xor_sync(0xffffffffu, acc.z, off);
+                        acc.w += __shfl_xor_sync(0xffffffffu, acc.w, off);
+                    }
+                }
+                if (ol == 0 && c < DV) apply_sum<VEC>(h, x, (size_t)c * VEC, acc, r.scale, lr, vs);
+            }
+        }
+    }
+}
+
+namespace {
+
+constexpr long long kPsRowsMaxOcc = 1LL << 30;
+
+size_t align256(size_t b) { return (b + 255) & ~(size_t)255; }
+
+// bytes of CUB's radix-sort temporary storage for n (key, occurrence) pairs over bits [0, end_bit)
+size_t rows_sort_temp_bytes(int n, int end_bit) {
+    size_t bytes = 0;
+    cub::DoubleBuffer<unsigned long long> kb(nullptr, nullptr);
+    cub::DoubleBuffer<int> vb(nullptr, nullptr);
+    if (cub::DeviceRadixSort::SortPairs(nullptr, bytes, kb, vb, n, 0, end_bit) != cudaSuccess) return 0;
+    return bytes;
+}
+
+size_t rows_scratch_fixed(int n) { return 2 * align256((size_t)n * 8) + 2 * align256((size_t)n * 4); }
+
+// Fold + apply of one sparse push: key build, stable radix sort, apply of the short and of the long runs.
+int ps_push_rows_launch(const TfyPsRows& r, const TfyPsHyper& h, const float* adam_scale, int grad_is_bf16,
+                        void* scratch, size_t scratch_bytes, cudaStream_t s) {
+    const long long n_ll = (long long)r.T * r.B * r.L;
+    if (n_ll == 0) return 0;
+    if (n_ll < 0 || n_ll > kPsRowsMaxOcc || r.D < 1 || r.V < 1) return -2;
+    const int n = (int)n_ll;
+    const unsigned long long sentinel = (unsigned long long)r.T * (unsigned long long)r.V;
+    const int end_bit = 64 - __builtin_clzll(sentinel);            // enough bits for every key, the sentinel included
+    const size_t temp_bytes = rows_sort_temp_bytes(n, end_bit);
+    if (!scratch || temp_bytes == 0 || rows_scratch_fixed(n) + temp_bytes > scratch_bytes) return -5;
+    char* p = static_cast<char*>(scratch);
+    unsigned long long* k0 = reinterpret_cast<unsigned long long*>(p);
+    unsigned long long* k1 = reinterpret_cast<unsigned long long*>(p + align256((size_t)n * 8));
+    int* v0 = reinterpret_cast<int*>(p + 2 * align256((size_t)n * 8));
+    int* v1 = reinterpret_cast<int*>(p + 2 * align256((size_t)n * 8) + align256((size_t)n * 4));
+    void* temp = p + rows_scratch_fixed(n);
+
+    cub::DoubleBuffer<unsigned long long> kb(k0, k1);
+    cub::DoubleBuffer<int> vb(v0, v1);
+    const int per_table = r.B * r.L;
+    if (per_table <= kPsBlockSortMax && r.V < 0x7fffffffLL) {
+        const int local_bits = 64 - __builtin_clzll((unsigned long long)r.V);     // ids and the local sentinel V
+        tfy_ps_segment_sort_kernel<<<r.T, kPsSortThreads, 0, s>>>(r.ids, per_table, r.V, local_bits, k0, v0);
+    } else {
+        size_t gk = ((size_t)n + 255) / 256;
+        if (gk > TFY_NUM_SMS * 8) gk = TFY_NUM_SMS * 8;
+        tfy_ps_row_keys_kernel<<<(unsigned)gk, 256, 0, s>>>(r.ids, n, per_table, r.V, k0, v0);
+        size_t tb = temp_bytes;
+        cudaError_t err = cub::DeviceRadixSort::SortPairs(temp, tb, kb, vb, n, 0, end_bit, s);
+        if (err != cudaSuccess) return (int)err;
+    }
+
+    // 16-byte gradient loads only when every row of every table slice starts on a 4-element boundary
+    const size_t gsize = grad_is_bf16 ? 2 : 4;
+    const bool vec = (r.D % 4 == 0) && (r.dout_ld % 4 == 0) && (r.col_stride % 4 == 0) &&
+                     (reinterpret_cast<uintptr_t>(r.dout) % (4 * gsize) == 0);
+    const int dv = vec ? r.D / 4 : r.D;
+    int cl_log2 = 0;
+    while (cl_log2 < 5 && (2 << cl_log2) <= dv) ++cl_log2;          // column lanes: largest power of 2 <= min(dv, 32)
+    size_t gs = ((size_t)n * dv + 255) / 256;                           // one thread per (position, column group)
+    if (gs > TFY_NUM_SMS * 8) gs = TFY_NUM_SMS * 8;
+    size_t gl = ((size_t)n + 255) / 256;                                // one warp per 32 sorted positions
+    if (gl > TFY_NUM_SMS * 8) gl = TFY_NUM_SMS * 8;
+#define TFY_APPLY_ROWS(GT, VV)                                                                                         \
+    do {                                                                                                               \
+        tfy_ps_apply_short_rows_kernel<GT, VV><<<(unsigned)gs, 256, 0, s>>>(r, h, adam_scale, kb.Current(),           \
+                                                                             vb.Current(), n);                         \
+        tfy_ps_apply_long_rows_kernel<GT, VV><<<(unsigned)gl, 256, 0, s>>>(r, h, adam_scale, kb.Current(),            \
+                                                                            vb.Current(), n, cl_log2);                 \
+    } while (0)
+    if (grad_is_bf16) { if (vec) TFY_APPLY_ROWS(__nv_bfloat16, 4); else TFY_APPLY_ROWS(__nv_bfloat16, 1); }
+    else { if (vec) TFY_APPLY_ROWS(float, 4); else TFY_APPLY_ROWS(float, 1); }
+#undef TFY_APPLY_ROWS
+    return (int)cudaGetLastError();
+}
+
+}  // namespace
 // ------------------------------------------------------------------------------- multi-table sparse ops
 // A wide-and-deep step touches one row in each of T tables per example (26 hashed categorical columns, twice: the
 // wide tower's [V, 1] tables and the deep tower's [V, 64] tables).  One launch per table made the step launch-bound
@@ -375,35 +637,6 @@ tfy_ps_multi_bag_kernel(const uint64_t* __restrict__ tables, const long long* __
     }
 }
 
-template <typename GT, int VEC>
-__global__ void __launch_bounds__(256)
-tfy_ps_multi_push_rows_kernel(const uint64_t* __restrict__ tables, const uint64_t* __restrict__ s1s,
-                              const uint64_t* __restrict__ s2s, const long long* __restrict__ ids,
-                              const GT* __restrict__ dout, int B, int T, int D, long long V, TfyPsHyper h,
-                              const float* __restrict__ adam_scale, int dout_ld, int col_stride) {
-    const int DV = D / VEC;
-    const size_t total = (size_t)T * B * DV;
-    const float lr = (h.opt == TFY_OPT_ADAM && adam_scale) ? h.lr * adam_scale[0] : h.lr;
-    for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
-        const int d = (i % DV) * VEC;
-        const size_t tb = i / DV;
-        const int b = tb % B, t = tb / B;
-        const long long id = ids[tb];
-        if (id < 0 || id >= V) continue;
-        const size_t o = (size_t)id * D + d;
-        float* w = reinterpret_cast<float*>(tables[t]) + o;
-        float* s1 = s1s ? reinterpret_cast<float*>(s1s[t]) + o : nullptr;
-        float* s2 = s2s ? reinterpret_cast<float*>(s2s[t]) + o : nullptr;
-        const GT* g = dout + (size_t)b * dout_ld + (size_t)t * col_stride + d;
-        if (VEC == 4) {
-            float4 unused;
-            ps_apply4(h.opt, w, s1, s2, f4_mul(ld_local4<GT>(g), h.grad_scale), lr, h.eps, h.p1, h.p2, h.p3, false, unused);
-        } else {
-            ps_apply1(h.opt, w, s1, s2, (float)g[0] * h.grad_scale, lr, h.eps, h.p1, h.p2, h.p3);
-        }
-    }
-}
-
 // fp32 -> bf16 shadow refresh of a whole segment (run by the chief after initialisation / restore)
 __global__ void __launch_bounds__(256) tfy_ps_refresh_shadow_kernel(const TfyPsSeg* __restrict__ segs) {
     const TfyPsSeg sg = segs[blockIdx.y];
@@ -431,7 +664,7 @@ int tfy_ps_pull(const TfyPsSeg* segs, int nseg, size_t max_n, int local_is_bf16,
     return (int)cudaGetLastError();
 }
 
-// adam_scale: device pointer to sqrt(1-b2^t)/(1-b1^t) (may be nullptr when no segment uses Adam)
+// adam_scale: device pointer to {1/(1-b1^t), 1/sqrt(1-b2^t)} (may be nullptr when no segment uses Adam)
 int tfy_ps_push(const TfyPsSeg* segs, int nseg, size_t max_n, int grad_is_bf16, float grad_scale,
                 const float* adam_scale, cudaStream_t s) {
     if (nseg <= 0) return 0;
@@ -480,43 +713,31 @@ int tfy_ps_embedding_bag(const void* table, const void* ids, void* out, int out_
     return (int)cudaGetLastError();
 }
 
+// Scratch (device bytes) that a sparse push of n = B*L (tfy_ps_push_rows) or T*B (tfy_ps_multi_push_rows) ids needs:
+// the keys and occurrence indices of the fold, double-buffered, and the radix sort's temporary storage.
+size_t tfy_ps_push_rows_scratch_bytes(long long n) {
+    if (n <= 0 || n > kPsRowsMaxOcc) return 0;
+    return rows_scratch_fixed((int)n) + rows_sort_temp_bytes((int)n, 64);
+}
+
 int tfy_ps_push_rows(void* table, void* s1_table, void* s2_table, const void* ids, const void* dout, int grad_is_bf16,
                      int B, int L, int D, long long V, int mean, int opt, float lr, float eps, float p1, float p2, float p3,
-                     float grad_scale, const float* adam_scale, int dout_ld, cudaStream_t s) {
+                     float grad_scale, const float* adam_scale, int dout_ld, void* scratch, size_t scratch_bytes,
+                     cudaStream_t s) {
     // dout_ld: row pitch (elements) of dout; 0 = D (contiguous [B, D]).  A larger pitch lets the caller push a
     // column slice of a wider gradient matrix (the fused first layer's dx) without copying it out.
     if (dout_ld <= 0) dout_ld = D;
     if (opt != TFY_OPT_SGD && opt != TFY_OPT_ADAGRAD && opt != TFY_OPT_ADAM && opt != TFY_OPT_FTRL) return -3;
     if (opt != TFY_OPT_SGD && !s1_table) return -4;
     if ((opt == TFY_OPT_ADAM || opt == TFY_OPT_FTRL) && !s2_table) return -4;
-    size_t gx = ((size_t)B * L * (D / 4) + 255) / 256;
-    if (gx < 1) gx = 1;
-    if (gx > TFY_NUM_SMS * 8) gx = TFY_NUM_SMS * 8;
     TfyPsHyper h;
     h.opt = opt; h.lr = lr; h.eps = eps; h.wd = 0.f; h.p1 = p1; h.p2 = p2; h.p3 = p3; h.grad_scale = grad_scale;
-    if (D % 4) {
-        size_t g1 = ((size_t)B * L * D + 255) / 256;
-        if (g1 < 1) g1 = 1;
-        if (g1 > TFY_NUM_SMS * 8) g1 = TFY_NUM_SMS * 8;
-        if (grad_is_bf16)
-            tfy_ps_push_rows_scalar_kernel<__nv_bfloat16><<<(unsigned)g1, 256, 0, s>>>(
-                (float*)table, (float*)s1_table, (float*)s2_table, (const long long*)ids, (const __nv_bfloat16*)dout, B,
-                L, D, V, mean, h, adam_scale, dout_ld);
-        else
-            tfy_ps_push_rows_scalar_kernel<float><<<(unsigned)g1, 256, 0, s>>>(
-                (float*)table, (float*)s1_table, (float*)s2_table, (const long long*)ids, (const float*)dout, B, L, D, V,
-                mean, h, adam_scale, dout_ld);
-        return (int)cudaGetLastError();
-    }
-    if (grad_is_bf16)
-        tfy_ps_push_rows_kernel<__nv_bfloat16><<<(unsigned)gx, 256, 0, s>>>(
-            (float*)table, (float*)s1_table, (float*)s2_table, (const long long*)ids, (const __nv_bfloat16*)dout, B, L, D,
-            V, mean, h, adam_scale, dout_ld);
-    else
-        tfy_ps_push_rows_kernel<float><<<(unsigned)gx, 256, 0, s>>>((float*)table, (float*)s1_table, (float*)s2_table,
-                                                                    (const long long*)ids, (const float*)dout, B, L, D,
-                                                                    V, mean, h, adam_scale, dout_ld);
-    return (int)cudaGetLastError();
+    TfyPsRows r = {};
+    r.w0 = (float*)table; r.s10 = (float*)s1_table; r.s20 = (float*)s2_table;
+    r.ids = (const long long*)ids; r.dout = dout;
+    r.B = B; r.L = L; r.T = 1; r.D = D; r.V = V; r.dout_ld = dout_ld; r.col_stride = 0;
+    r.scale = (mean ? 1.f / (float)L : 1.f) * grad_scale;
+    return ps_push_rows_launch(r, h, adam_scale, grad_is_bf16, scratch, scratch_bytes, s);
 }
 
 int tfy_ps_multi_bag(const uint64_t* tables, const void* ids, void* out, int out_is_bf16, int B, int T, int D,
@@ -536,25 +757,19 @@ int tfy_ps_multi_bag(const uint64_t* tables, const void* ids, void* out, int out
 int tfy_ps_multi_push_rows(const uint64_t* tables, const uint64_t* s1s, const uint64_t* s2s, const void* ids,
                            const void* dout, int grad_is_bf16, int B, int T, int D, long long V, int opt, float lr,
                            float eps, float p1, float p2, float p3, float grad_scale, const float* adam_scale,
-                           int dout_ld, int col_stride, cudaStream_t s) {
+                           int dout_ld, int col_stride, void* scratch, size_t scratch_bytes, cudaStream_t s) {
     if (opt != TFY_OPT_SGD && opt != TFY_OPT_ADAGRAD && opt != TFY_OPT_ADAM && opt != TFY_OPT_FTRL) return -3;
     if (opt != TFY_OPT_SGD && !s1s) return -4;
     if ((opt == TFY_OPT_ADAM || opt == TFY_OPT_FTRL) && !s2s) return -4;
     if (dout_ld <= 0) dout_ld = D;
     TfyPsHyper h;
     h.opt = opt; h.lr = lr; h.eps = eps; h.wd = 0.f; h.p1 = p1; h.p2 = p2; h.p3 = p3; h.grad_scale = grad_scale;
-    const bool vec = (D % 4 == 0) && (dout_ld % 4 == 0) && (col_stride % 4 == 0);
-    size_t gx = ((size_t)T * B * (vec ? D / 4 : D) + 255) / 256;
-    if (gx < 1) gx = 1;
-    if (gx > TFY_NUM_SMS * 8) gx = TFY_NUM_SMS * 8;
-#define TFY_MPR(GT, VV)                                                                                              \
-    tfy_ps_multi_push_rows_kernel<GT, VV><<<(unsigned)gx, 256, 0, s>>>(tables, s1s, s2s, (const long long*)ids,       \
-                                                                       (const GT*)dout, B, T, D, V, h, adam_scale,    \
-                                                                       dout_ld, col_stride)
-    if (grad_is_bf16) { if (vec) TFY_MPR(__nv_bfloat16, 4); else TFY_MPR(__nv_bfloat16, 1); }
-    else { if (vec) TFY_MPR(float, 4); else TFY_MPR(float, 1); }
-#undef TFY_MPR
-    return (int)cudaGetLastError();
+    TfyPsRows r = {};
+    r.tables = tables; r.s1s = s1s; r.s2s = s2s;
+    r.ids = (const long long*)ids; r.dout = dout;
+    r.B = B; r.L = 1; r.T = T; r.D = D; r.V = V; r.dout_ld = dout_ld; r.col_stride = col_stride;
+    r.scale = grad_scale;
+    return ps_push_rows_launch(r, h, adam_scale, grad_is_bf16, scratch, scratch_bytes, s);
 }
 
 }  // extern "C"
