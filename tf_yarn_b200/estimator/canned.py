@@ -65,9 +65,9 @@ class _WideDeepNet(nn.Module):
     """logits = linear(wide columns) + dnn(dense(deep columns))."""
 
     def __init__(self, linear_columns, dnn_columns, hidden_units: Sequence[int], n_out: int,
-                 activation=F.relu, dropout: Optional[float] = None):
+                 activation=F.relu, dropout: Optional[float] = None, sparse_combiner: str = "sum"):
         super().__init__()
-        self.linear = fc.LinearModel(linear_columns, n_out) if linear_columns else None
+        self.linear = fc.LinearModel(linear_columns, n_out, sparse_combiner) if linear_columns else None
         self.dense_features = fc.DenseFeatures(dnn_columns) if dnn_columns else None
         self.activation = activation
         self.dropout = dropout
@@ -115,7 +115,7 @@ def _tf_default(opt, tower: str, n_columns: int, combined: bool):
 
 
 def _canned_model_fn(linear_columns, dnn_columns, hidden_units, n_classes, optimizer, dropout=None,
-                     linear_optimizer=None):
+                     linear_optimizer=None, sparse_combiner="sum"):
     n_out = 1 if n_classes == 2 else n_classes
     combined = bool(linear_columns) and bool(dnn_columns)
     if dnn_columns:
@@ -125,7 +125,8 @@ def _canned_model_fn(linear_columns, dnn_columns, hidden_units, n_classes, optim
         optimizer = _tf_default(optimizer, "linear", len(linear_columns), False)
 
     def model_fn(features, labels, mode, params=None, config=None):
-        net = _WideDeepNet(linear_columns, dnn_columns, hidden_units, n_out, dropout=dropout)
+        net = _WideDeepNet(linear_columns, dnn_columns, hidden_units, n_out, dropout=dropout,
+                           sparse_combiner=sparse_combiner)
         # the wide tower's parameters live under "linear."; everything else belongs to the deep tower
         per_tower = {"linear.": linear_optimizer} if (linear_optimizer is not None and linear_columns) else None
         return EstimatorSpec(mode=mode, network=net, loss=_classification_loss(n_classes), optimizer=optimizer,
@@ -136,9 +137,11 @@ def _canned_model_fn(linear_columns, dnn_columns, hidden_units, n_classes, optim
 
 class LinearClassifier(Estimator):
     def __init__(self, feature_columns, model_dir: Optional[str] = None, n_classes: int = 2, optimizer: Any = "ftrl",
-                 config: Optional[RunConfig] = None, **_ignored):
+                 config: Optional[RunConfig] = None, sparse_combiner: str = "sum", **_ignored):
         # FTRL is TF's default for linear models (tf.estimator.LinearClassifier)
-        super().__init__(_canned_model_fn(list(feature_columns), [], [], n_classes, optimizer), model_dir, config)
+        fc._check_combiner(sparse_combiner)
+        super().__init__(_canned_model_fn(list(feature_columns), [], [], n_classes, optimizer,
+                                          sparse_combiner=sparse_combiner), model_dir, config)
 
 
 class DNNClassifier(Estimator):
@@ -155,10 +158,11 @@ class DNNLinearCombinedClassifier(Estimator):
     def __init__(self, model_dir: Optional[str] = None, linear_feature_columns=None, linear_optimizer: Any = "ftrl",
                  dnn_feature_columns=None, dnn_optimizer: Any = "adagrad", dnn_hidden_units: Sequence[int] = (),
                  dnn_dropout: Optional[float] = None, n_classes: int = 2, config: Optional[RunConfig] = None,
-                 **_ignored):
+                 linear_sparse_combiner: str = "sum", **_ignored):
+        fc._check_combiner(linear_sparse_combiner)
         super().__init__(_canned_model_fn(list(linear_feature_columns or []), list(dnn_feature_columns or []),
                                           list(dnn_hidden_units), n_classes, dnn_optimizer, dnn_dropout,
-                                          linear_optimizer=linear_optimizer),
+                                          linear_optimizer=linear_optimizer, sparse_combiner=linear_sparse_combiner),
                          model_dir, config)
 
 

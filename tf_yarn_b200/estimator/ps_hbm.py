@@ -28,6 +28,7 @@ from typing import Dict, List, Optional
 
 import torch
 import torch.nn as nn
+import torch.nn.functional as F
 
 from tf_yarn_b200 import _task_commons
 from tf_yarn_b200.estimator import ps as ps_cpu
@@ -49,9 +50,14 @@ native.declare("tfy_ps_multi_bag", [_vp, _vp, _vp, _i, _i, _i, _i, _ll, _vp])
 native.declare("tfy_ps_multi_push_rows", [_vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _ll, _i, _f, _f, _f, _f, _f, _f, _vp, _i,
                                           _i, _vp, _sz, _vp])
 native.declare("tfy_ps_gather_gemm", [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _ll, _vp])
+native.declare("tfy_ps_multi_bag_weighted", [_vp, _vp, _vp, _i, _i, _i, _i, _i, _ll, _vp, _i, _i, _i, _vp, _i, _vp,
+                                             _vp])
+native.declare("tfy_ps_multi_push_rows_weighted", [_vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _ll, _i, _f, _f, _f, _f, _f,
+                                                   _f, _vp, _i, _i, _i, _vp, _vp, _i, _vp, _sz, _vp])
 
 OPT_CODES = {"sgd": native.OPT_SGD, "adagrad": native.OPT_ADAGRAD, "adam": native.OPT_ADAM,
              "ftrl": native.OPT_FTRL}
+COMBINER_CODES = {"sum": 0, "mean": 1, "sqrtn": 2}      # tfy_ps_multi_bag_weighted / tfy_ps_multi_push_rows_weighted
 
 
 class PsSeg(ctypes.Structure):
@@ -75,6 +81,23 @@ def push_rows_scratch(lib, n: int, device) -> torch.Tensor:
     Allocated per push from the caching allocator, so a captured CUDA graph keeps its own."""
     nbytes = int(lib.tfy_ps_push_rows_scratch_bytes(n)) if n > 0 else 0
     return torch.empty(max(nbytes, 1), dtype=torch.uint8, device=device)
+
+
+def _ptr(t: Optional[torch.Tensor]) -> Optional[int]:
+    return t.data_ptr() if t is not None else None
+
+
+def weighted_bag(lib, tables: torch.Tensor, ids: torch.Tensor, weights: Optional[torch.Tensor], combiner: int, D: int,
+                 V: int, out: torch.Tensor, out_ld: int, col_stride: int, f: torch.Tensor,
+                 numeric: Optional[torch.Tensor] = None) -> None:
+    """tfy_ps_multi_bag_weighted: ids int64 [T, B, L] (-1 = missing), weights fp32 [T, B, L] or None, f fp32 [T, B]
+    receives 1/den for the push."""
+    T, B, L = ids.shape
+    n_num = numeric.shape[1] if numeric is not None else 0
+    native.check(lib.tfy_ps_multi_bag_weighted(tables.data_ptr(), ids.data_ptr(), _ptr(weights), combiner, B, L, T, D,
+                                               V, out.data_ptr(), int(out.dtype == torch.bfloat16), out_ld, col_stride,
+                                               _ptr(numeric), n_num, f.data_ptr(),
+                                               torch.cuda.current_stream().cuda_stream), "tfy_ps_multi_bag_weighted")
 
 
 def cluster_ranks(cluster) -> Dict[str, int]:
@@ -337,10 +360,56 @@ def _make_bag_forward(conn: HbmConnection, idx: int, mod: nn.EmbeddingBag):
             conn.account(push=B * L * D * 4 * (1 + lay.var_slots[idx]), launches=push_rows_launches(B * L))
             return None, None
 
+    # multi-hot, weighted or sqrtn input: the weighted bag and push with T = 1
+    combiner = getattr(mod, "combiner", mod.mode)
+    code = COMBINER_CODES[combiner]
+    group = _TableGroup.single(conn, idx, V)
+    tables = group.tables
+
+    class _WBag(torch.autograd.Function):
+        @staticmethod
+        def forward(ctx, ids, weights, anchor):
+            B, L = ids.shape
+            out = torch.empty((B, D), dtype=torch.float32, device=ids.device)
+            f = torch.empty((1, B), dtype=torch.float32, device=ids.device)
+            weighted_bag(lib, tables, ids[None], weights[None] if weights is not None else None, code, D, V, out, D, 0,
+                         f)
+            conn.account(pull=B * L * D * 4)
+            ctx.ids, ctx.weights, ctx.f = ids, weights, f
+            return out
+
+        @staticmethod
+        def backward(ctx, dout):
+            ids = ctx.ids
+            w = ctx.weights[None] if ctx.weights is not None else None
+            group.push_weighted(ids[None], w, ctx.f, code, dout.contiguous().float(), D, D, 0)
+            return None, None, None
+
     anchor = torch.zeros((), device=conn.device, requires_grad=True)
 
-    def forward(ids, offsets=None, per_sample_weights=None):
-        return _Bag.apply(ids, anchor)
+    def run(ids, weights):
+        ids = ids.contiguous().long()
+        if ids.dim() == 1:
+            ids = ids[:, None]
+        if weights is None and ids.shape[1] == 1 and combiner in ("sum", "mean"):
+            return _Bag.apply(ids, anchor)          # one id per example: the one-table kernels
+        if weights is not None:
+            weights = weights.contiguous().float().reshape(ids.shape[0], -1)
+            if weights.shape != ids.shape:
+                raise ValueError(f"weights {tuple(weights.shape)} do not match ids {tuple(ids.shape)}")
+        return _WBag.apply(ids, weights, anchor)
+
+    from tf_yarn_b200.estimator import feature_column as fc
+    if isinstance(mod, fc.CombinedBag):
+        def forward(ids, weights=None):
+            return run(ids, weights)
+    else:
+        def forward(ids, offsets=None, per_sample_weights=None):
+            if offsets is not None:
+                raise NotImplementedError("the HBM parameter server serves [B, L] id batches; offsets are not supported")
+            if per_sample_weights is not None and mod.mode != "sum":
+                raise ValueError("per_sample_weights needs mode='sum' (as for torch.nn.EmbeddingBag)")
+            return run(ids, per_sample_weights)
     return forward
 
 
@@ -407,13 +476,71 @@ class _TableGroup:
         self.p3 = float(h["eps"]) if lay.kinds[first] == "ftrl" else 0.0
         self.slots = ns
 
+    @classmethod
+    def single(cls, conn: HbmConnection, idx: int, V: int) -> "_TableGroup":
+        """The one table of an unfused bag (push_weighted only)."""
+        from tf_yarn_b200.estimator import feature_column as fc
+        return cls(conn, [idx], [fc.CategoricalColumn("", V)])
+
+    @property
+    def weighted(self) -> bool:
+        from tf_yarn_b200.estimator import feature_column as fc
+        return any(isinstance(c, fc.WeightedCategoricalColumn) for c in self.cols)
+
+    def one_hot(self, features) -> bool:
+        """True when the batch has one id per example in every column ([B] or [B, 1]) and no column is weighted: the
+        one-id kernels (K5, tfy_ps_multi_bag) serve it.  Decided from shapes, without a device synchronisation."""
+        return not self.weighted and all(features[c.key].reshape(features[c.key].shape[0], -1).shape[1] == 1
+                                         for c in self.cols)
+
     def ids_of(self, features) -> torch.Tensor:
-        """int64 [T, B] bucket ids of the batch: ONE hash over the stacked columns (26 separate 3-kernel hashes
-        were 40 % of the step's device time in the first profile)."""
+        """int64 [T, B] bucket ids of the batch (-1 = missing): ONE hash over the stacked columns (26 separate
+        3-kernel hashes were 40 % of the step's device time in the first profile)."""
         raw = torch.stack([features[c.key].reshape(-1) for c in self.cols]).long()
-        if self.cols[0].hashed:
-            raw = (raw * 2654435761) % (2 ** 32)
-        return (raw % self.V).contiguous()
+        return self._bucket(raw)
+
+    def _bucket(self, raw: torch.Tensor) -> torch.Tensor:
+        """feature_column._ids of the stacked columns (the CPU plane's mapping, -1 = missing): one call when the
+        columns share V and hashing, else column by column."""
+        from tf_yarn_b200.estimator import feature_column as fc
+        if self.same_v:
+            return fc._ids(self.cols[0], raw).contiguous()
+        return torch.stack([fc._ids(c, r) for c, r in zip(self.cols, raw)]).contiguous()
+
+    def multi_of(self, features):
+        """int64 [T, B, L] bucket ids (-1 = missing), every column padded on the device to the group's largest L with
+        -1, and the
+        fp32 [T, B, L] weights (1 for an unweighted column) or None when no column is weighted."""
+        from tf_yarn_b200.estimator import feature_column as fc
+        raws = [features[c.key] for c in self.cols]
+        raws = [r.reshape(r.shape[0], -1).long() for r in raws]
+        L = max(r.shape[1] for r in raws)
+        ids = self._bucket(torch.stack([F.pad(r, (0, L - r.shape[1]), value=-1) for r in raws]))
+        if not self.weighted:
+            return ids, None
+        ws = []
+        for c, r in zip(self.cols, raws):
+            if isinstance(c, fc.WeightedCategoricalColumn):
+                w = fc._weights(c, features, r.shape).float()
+            else:
+                w = torch.ones(r.shape, dtype=torch.float32, device=r.device)
+            ws.append(F.pad(w, (0, L - w.shape[1])))
+        return ids, torch.stack(ws).contiguous()
+
+    def push_weighted(self, ids: torch.Tensor, weights: Optional[torch.Tensor], f: torch.Tensor, combiner: int,
+                      dout: torch.Tensor, D: int, dout_ld: int, col_stride: int) -> None:
+        """tfy_ps_multi_push_rows_weighted of a weighted bag's backward: ids / weights [T, B, L], f [T, B]."""
+        conn, h = self.conn, self.h
+        T, B, L = ids.shape
+        scratch = push_rows_scratch(conn.lib, T * B * L, dout.device)
+        native.check(conn.lib.tfy_ps_multi_push_rows_weighted(
+            self.tables.data_ptr(), _ptr(self.s1), _ptr(self.s2), ids.data_ptr(), dout.data_ptr(),
+            1 if dout.dtype == torch.bfloat16 else 0, B, T, D, self.V, self.opt, float(h["lr"]), float(h["eps"]),
+            float(h["p1"]), float(h["p2"]), self.p3, 1.0, conn.adam_scale.data_ptr(), dout_ld, col_stride, L,
+            _ptr(weights), f.data_ptr(), combiner, scratch.data_ptr(), scratch.numel(),
+            torch.cuda.current_stream().cuda_stream), "tfy_ps_multi_push_rows_weighted")
+        # one launch more than an unweighted push: the per-occurrence factors w * f
+        conn.account(push=T * B * L * D * 4 * (1 + self.slots), launches=push_rows_launches(B * L) + 1)
 
     def push(self, ids: torch.Tensor, dout: torch.Tensor, D: int, dout_ld: int, col_stride: int) -> None:
         conn, h = self.conn, self.h
@@ -441,11 +568,11 @@ def _try_fuse_wide_tower(conn: HbmConnection, network: nn.Module) -> bool:
     by_param = {id(p): i for i, p in enumerate(conn.params)}
     cat_cols, tables_idx = [], []
     for c in lin.columns:
-        cc = c.categorical_column if isinstance(c, (fc.EmbeddingColumn, fc.IndicatorColumn)) else c
-        if isinstance(cc, fc.CategoricalColumn):
+        cc = fc._categorical(c)
+        if cc is not None:
             emb = lin.tables[cc.key]
             ti = by_param.get(id(emb.weight))
-            if ti is None or ti not in conn.sparse or emb.mode != "sum":
+            if ti is None or ti not in conn.sparse or not isinstance(emb, fc.CombinedBag):
                 return False
             cat_cols.append(cc)
             tables_idx.append(ti)
@@ -454,6 +581,8 @@ def _try_fuse_wide_tower(conn: HbmConnection, network: nn.Module) -> bool:
         return False
     units = lin.units
     dev = conn.device
+    combiner = lin.sparse_combiner
+    code = COMBINER_CODES[combiner]
 
     class _MultiBag(torch.autograd.Function):
         @staticmethod
@@ -472,11 +601,32 @@ def _try_fuse_wide_tower(conn: HbmConnection, network: nn.Module) -> bool:
             group.push(ctx.ids, dout.contiguous().float(), units, units, 0)     # every table gets the same gradient
             return None, None
 
+    class _WMultiBag(torch.autograd.Function):
+        """Multi-hot, weighted or non-sum wide tower: every column combined by the sparse combiner, then summed."""
+
+        @staticmethod
+        def forward(ctx, ids, weights, anchor):
+            T, B, L = ids.shape
+            out = torch.empty((B, units), dtype=torch.float32, device=dev)
+            f = torch.empty((T, B), dtype=torch.float32, device=dev)
+            weighted_bag(conn.lib, group.tables, ids, weights, code, units, group.V, out, units, 0, f)
+            conn.account(pull=T * B * L * units * 4)
+            ctx.ids, ctx.weights, ctx.f = ids, weights, f
+            return out
+
+        @staticmethod
+        def backward(ctx, dout):
+            group.push_weighted(ctx.ids, ctx.weights, ctx.f, code, dout.contiguous().float(), units, units, 0)
+            return None, None, None
+
     anchor = torch.zeros((), device=dev, requires_grad=True)
     num_cols = [c for c in lin.columns if isinstance(c, fc.NumericColumn)]
 
     def forward(features):
-        out = _MultiBag.apply(group.ids_of(features), anchor)
+        if combiner == "sum" and group.one_hot(features):
+            out = _MultiBag.apply(group.ids_of(features), anchor)
+        else:
+            out = _WMultiBag.apply(*group.multi_of(features), anchor)
         if lin.numeric is not None and num_cols:
             nums = [features[c.key].reshape(features[c.key].shape[0], -1).float() for c in num_cols]
             x = nums[0] if len(nums) == 1 else torch.cat(nums, dim=1)
@@ -497,6 +647,7 @@ def _try_fuse_first_layer(conn: HbmConnection, network: nn.Module) -> bool:
     HBM becomes the A-operand producer of that GEMM; the backward (dW, dx) is one wgmma kernel against the same
     remote shadow, and the row gradients are pushed straight out of its dx.  TFY_PS_FUSE_FIRST=0 disables it."""
     from tf_yarn_b200.estimator import feature_column as fc
+    from tf_yarn_b200.ops.gemm import gemm_bf16
     if os.environ.get("TFY_PS_FUSE_FIRST", "1") == "0":
         return False
     df, hidden = getattr(network, "dense_features", None), getattr(network, "hidden", None)
@@ -523,7 +674,7 @@ def _try_fuse_first_layer(conn: HbmConnection, network: nn.Module) -> bool:
     for c in emb_cols:
         emb = df.embeddings[c.categorical_column.key]
         ti = by_param.get(id(emb.weight))
-        if ti is None or ti not in conn.sparse or emb.mode not in ("sum", "mean"):
+        if ti is None or ti not in conn.sparse or not isinstance(emb, fc.CombinedBag):
             return False
         tables_idx.append(ti)
     V = emb_cols[0].categorical_column.num_buckets
@@ -535,6 +686,25 @@ def _try_fuse_first_layer(conn: HbmConnection, network: nn.Module) -> bool:
     group = _TableGroup(conn, tables_idx, [c.categorical_column for c in emb_cols])
     table_ptrs = group.tables
     lib, lay = conn.lib, conn.layout
+    # the bag takes one combiner per launch: a group whose columns differ is gathered table by table.  The push takes
+    # the per-table 1/den in f, so one push serves any mix (its combiner argument only says that f is given).
+    codes = [COMBINER_CODES[c.combiner] for c in emb_cols]
+    one_code = len(set(codes)) == 1
+    push_code = COMBINER_CODES["mean"]
+    # tables of mixed optimizers push one by one: {w, s1, s2} pointers of each, for a T = 1 weighted push
+    singles = None if group.uniform else [_TableGroup.single(conn, ti, V) for ti in tables_idx]
+
+    def first_backward(xbuf, dy, weight, push):
+        """dW and dx in one wgmma kernel against the remote shadow, then push(dx) of the embedding rows."""
+        B = xbuf.shape[0]
+        dyb = dy.to(torch.bfloat16).contiguous()
+        dw = torch.empty((N, Kp), dtype=torch.bfloat16, device=dev)
+        dx = torch.empty((B, Kp), dtype=torch.bfloat16, device=dev)
+        native.check(lib.tfy_dense_bwd(dyb.data_ptr(), xbuf.data_ptr(), shadow, dw.data_ptr(), dx.data_ptr(), B, N,
+                                       Kp, torch.cuda.current_stream().cuda_stream), "tfy_dense_bwd")
+        conn.account(pull=N * Kp * 2)
+        push(dx)
+        return dw[:, :K].to(weight.dtype), dy.float().sum(0).to(weight.dtype)
 
     class _FusedFirst(torch.autograd.Function):
         @staticmethod
@@ -556,53 +726,91 @@ def _try_fuse_first_layer(conn: HbmConnection, network: nn.Module) -> bool:
             xbuf, ids, weight = ctx.saved_tensors
             B = xbuf.shape[0]
             s = torch.cuda.current_stream().cuda_stream
-            dyb = dy.to(torch.bfloat16).contiguous()
-            dw = torch.empty((N, Kp), dtype=torch.bfloat16, device=dev)
-            dx = torch.empty((B, Kp), dtype=torch.bfloat16, device=dev)
-            native.check(lib.tfy_dense_bwd(dyb.data_ptr(), xbuf.data_ptr(), shadow, dw.data_ptr(), dx.data_ptr(), B, N,
-                                           Kp, s), "tfy_dense_bwd")
+
+            def push(dx):
+                if group.uniform:
+                    # table t takes columns [64 t, 64 t + 64) of dx: ONE launch for all tables, straight out of dx
+                    group.push(ids, dx, 64, Kp, 64)
+                    return
+                for t, ti in enumerate(tables_idx):          # (mixed optimizers) table by table
+                    h = lay.hypers[ti]
+                    s1 = conn.master_ptr(ti, 1) if lay.var_slots[ti] >= 1 else None
+                    s2 = conn.master_ptr(ti, 2) if lay.var_slots[ti] >= 2 else None
+                    p3 = float(h["eps"]) if lay.kinds[ti] == "ftrl" else 0.0
+                    scratch = push_rows_scratch(lib, B, dev)
+                    native.check(lib.tfy_ps_push_rows(
+                        conn.master_ptr(ti), s1, s2, ids[t].data_ptr(), dx.data_ptr() + 2 * 64 * t, 1, B, 1, 64, V, 0,
+                        conn.var_opt[ti], float(h["lr"]), float(h["eps"]), float(h["p1"]), float(h["p2"]), p3, 1.0,
+                        conn.adam_scale.data_ptr(), Kp, scratch.data_ptr(), scratch.numel(), s), "tfy_ps_push_rows")
+                    conn.account(push=B * 64 * 4 * (1 + lay.var_slots[ti]), launches=push_rows_launches(B))
+            dw, db = first_backward(xbuf, dy, weight, push)
+            return None, None, dw, db
+
+    class _BagFirst(torch.autograd.Function):
+        """Multi-hot or weighted batches: the weighted bag writes the activation buffer K5 would (embeddings, then
+        the numeric columns), then the remote-weight GEMM; the backward is K5's, with the weighted push."""
+
+        @staticmethod
+        def forward(ctx, ids, weights, numeric, weight, bias):
+            _, B, L = ids.shape
+            xbuf = torch.zeros((B, Kp), dtype=torch.bfloat16, device=dev)
+            f = torch.empty((T, B), dtype=torch.float32, device=dev)
+            if one_code:
+                weighted_bag(lib, table_ptrs, ids, weights, codes[0], 64, V, xbuf, Kp, 64, f, numeric)
+            else:                                           # table t into columns [64 t, 64 t + 64); numeric last
+                for t in range(T):
+                    weighted_bag(lib, table_ptrs[t:t + 1], ids[t:t + 1],
+                                 weights[t:t + 1] if weights is not None else None, codes[t], 64, V, xbuf[:, 64 * t:],
+                                 Kp, 64, f[t:t + 1], numeric if t == T - 1 else None)
+            y = gemm_bf16(xbuf, None, bias=bias.to(torch.bfloat16), b_ptr=shadow, b_rows=N, b_ld=Kp, impl="1cta")
+            conn.account(pull=T * B * L * 64 * 4, launches=1 if one_code else T)
             conn.account(pull=N * Kp * 2)
-            if group.uniform:
-                # table t takes columns [64 t, 64 t + 64) of dx: ONE launch for all tables, straight out of dx
-                group.push(ids, dx, 64, Kp, 64)
-                return None, None, dw[:, :K].to(weight.dtype), dy.float().sum(0).to(weight.dtype)
-            for t, ti in enumerate(tables_idx):          # (mixed optimizers) table by table
-                h = lay.hypers[ti]
-                s1 = conn.master_ptr(ti, 1) if lay.var_slots[ti] >= 1 else None
-                s2 = conn.master_ptr(ti, 2) if lay.var_slots[ti] >= 2 else None
-                p3 = float(h["eps"]) if lay.kinds[ti] == "ftrl" else 0.0
-                scratch = push_rows_scratch(lib, B, dev)
-                native.check(lib.tfy_ps_push_rows(
-                    conn.master_ptr(ti), s1, s2, ids[t].data_ptr(), dx.data_ptr() + 2 * 64 * t, 1, B, 1, 64, V, 0,
-                    conn.var_opt[ti], float(h["lr"]), float(h["eps"]), float(h["p1"]), float(h["p2"]), p3, 1.0,
-                    conn.adam_scale.data_ptr(), Kp, scratch.data_ptr(), scratch.numel(), s), "tfy_ps_push_rows")
-                conn.account(push=B * 64 * 4 * (1 + lay.var_slots[ti]), launches=push_rows_launches(B))
-            return None, None, dw[:, :K].to(weight.dtype), dy.float().sum(0).to(weight.dtype)
+            ctx.save_for_backward(xbuf, ids, weight)
+            ctx.weights, ctx.f = weights, f
+            return y.to(weight.dtype)
+
+        @staticmethod
+        def backward(ctx, dy):
+            xbuf, ids, weight = ctx.saved_tensors
+            w, f = ctx.weights, ctx.f
+
+            def push(dx):
+                if group.uniform:
+                    group.push_weighted(ids, w, f, push_code, dx, 64, Kp, 64)
+                    return
+                for t, one in enumerate(singles):           # (mixed optimizers) table by table
+                    one.push_weighted(ids[t:t + 1], w[t:t + 1] if w is not None else None, f[t:t + 1], push_code,
+                                      dx[:, 64 * t:], 64, Kp, 0)
+            dw, db = first_backward(xbuf, dy, weight, push)
+            return None, None, None, dw, db
 
     class _Deferred:
-        """What the patched DenseFeatures returns: the raw inputs of the fused first layer."""
+        """What the patched DenseFeatures returns: the raw inputs of the fused first layer (weights is None and ids
+        [T, B] for K5; ids [T, B, L] for the weighted bag)."""
 
-        def __init__(self, ids, numeric):
-            self.ids, self.numeric = ids, numeric
+        def __init__(self, ids, weights, numeric, one_hot):
+            self.ids, self.weights, self.numeric, self.one_hot = ids, weights, numeric, one_hot
 
         def to(self, *a, **k):
             return self
 
     def df_forward(features):
-        if group.same_v:
-            ids = group.ids_of(features)
+        one_hot = group.one_hot(features)
+        if one_hot:
+            ids, weights = group.ids_of(features), None
         else:
-            ids = torch.stack([fc._ids(c.categorical_column, features[c.categorical_column.key]).reshape(-1)
-                               for c in emb_cols]).contiguous()
+            ids, weights = group.multi_of(features)
         numeric = None
         if num_cols:
             parts = [features[c.key].reshape(features[c.key].shape[0], -1).float() for c in num_cols]
             numeric = (parts[0] if len(parts) == 1 else torch.cat(parts, dim=1)).contiguous()
-        return _Deferred(ids, numeric)
+        return _Deferred(ids, weights, numeric, one_hot)
 
     def lin_forward(x):
         if isinstance(x, _Deferred):
-            return _FusedFirst.apply(x.ids, x.numeric, lin.weight, lin.bias)
+            if x.one_hot:
+                return _FusedFirst.apply(x.ids, x.numeric, lin.weight, lin.bias)
+            return _BagFirst.apply(x.ids, x.weights, x.numeric, lin.weight, lin.bias)
         return _make_linear_forward(conn, widx, lin)(x)
 
     df.forward = df_forward

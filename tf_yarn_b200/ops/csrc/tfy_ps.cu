@@ -27,6 +27,14 @@
 //                  every run in a fixed order (a thread per short run, a warp per long one): a push is deterministic
 //                  and needs no host synchronisation (capturable).  Rows outside the batch are not touched, Adam's
 //                  m and v included (lazy Adam).  Out-of-range ids (< 0 or >= V) are skipped.
+//   multi-hot / weighted (TF's embedding_column combiners), T tables x L ids per example, weight w (1 if none):
+//          an occurrence is present iff 0 <= id < V and w != 0.  S = sum_present w row, out = S / den with
+//          den = 1 (sum), sum_present w (mean), sqrt(sum_present w^2) (sqrtn), and 0 where den == 0.
+//          tfy_ps_multi_bag_weighted writes out (a column slice per table, or all tables summed) and f = 1/den;
+//          tfy_ps_multi_push_rows_weighted is the fold above with a compile-time weighted flag: zero weights get
+//          the sentinel key, one more kernel writes every occurrence's factor w f into the sort's free buffer, and
+//          the apply kernels add w f g in the sorted order.  The unweighted instantiations are unchanged; K5 and the
+//          one-id kernels keep serving one-hot unweighted batches.
 #include <cub/block/block_radix_sort.cuh>
 #include <cub/device/device_radix_sort.cuh>
 
@@ -350,14 +358,19 @@ __device__ __forceinline__ float4 ld_grad(const GT* p) {
 }
 }  // namespace
 
-// keys[o] = t * V + id, or T * V (sorts last, never applied) for an out-of-range id; occ[o] = o
+// Weighted pushes (W = true) take two more arrays, nullptr meaning "all ones": wts [T, B, L], the weight of every
+// occurrence, and fs [T, B], the bag's per-example factor 1/den.  A zero-weight occurrence is absent: it gets the
+// sentinel key like an out-of-range id, so it touches no row.  The unweighted instantiations ignore both.
+// keys[o] = t * V + id, or T * V (sorts last, never applied) for an absent occurrence; occ[o] = o
+template <bool W>
 __global__ void __launch_bounds__(256)
 tfy_ps_row_keys_kernel(const long long* __restrict__ ids, int n, int per_table, long long V,
-                       unsigned long long* __restrict__ keys, int* __restrict__ occ) {
+                       unsigned long long* __restrict__ keys, int* __restrict__ occ, const float* __restrict__ wts) {
     const unsigned long long sentinel = (unsigned long long)(n / per_table) * (unsigned long long)V;
     for (int o = blockIdx.x * blockDim.x + threadIdx.x; o < n; o += gridDim.x * blockDim.x) {
         const long long id = ids[o];
-        keys[o] = (id < 0 || id >= V) ? sentinel : (unsigned long long)(o / per_table) * (unsigned long long)V + id;
+        keys[o] = (id < 0 || id >= V || (W && wts && wts[o] == 0.f))
+                      ? sentinel : (unsigned long long)(o / per_table) * (unsigned long long)V + id;
         occ[o] = o;
     }
 }
@@ -368,9 +381,10 @@ tfy_ps_row_keys_kernel(const long long* __restrict__ ids, int n, int per_table, 
 // skip sentinels wherever they are.  One launch instead of a key kernel plus a multi-pass device sort.
 constexpr int kPsSortThreads = 256, kPsSortItems = 8, kPsBlockSortMax = kPsSortThreads * kPsSortItems;
 
+template <bool W>
 __global__ void __launch_bounds__(kPsSortThreads)
 tfy_ps_segment_sort_kernel(const long long* __restrict__ ids, int per_table, long long V, int local_bits,
-                           unsigned long long* __restrict__ keys, int* __restrict__ occ) {
+                           unsigned long long* __restrict__ keys, int* __restrict__ occ, const float* __restrict__ wts) {
     using Sort = cub::BlockRadixSort<unsigned int, kPsSortThreads, kPsSortItems, int>;
     __shared__ typename Sort::TempStorage tmp;
     const int t = blockIdx.x;
@@ -383,7 +397,7 @@ tfy_ps_segment_sort_kernel(const long long* __restrict__ ids, int per_table, lon
         const int r = threadIdx.x * kPsSortItems + j;               // blocked arrangement: r keeps the original order
         if (r < per_table) {
             const long long id = ids[base + r];
-            k[j] = (id < 0 || id >= V) ? (unsigned int)V : (unsigned int)id;
+            k[j] = (id < 0 || id >= V || (W && wts && wts[base + r] == 0.f)) ? (unsigned int)V : (unsigned int)id;
         } else {
             k[j] = 0xffffffffu;                                      // padding: after every real key
         }
@@ -428,6 +442,17 @@ __device__ __forceinline__ RowRef row_of(const TfyPsRows& r, unsigned long long 
     if (x.s2) x.s2 += row;
     return x;
 }
+// gradient of occurrence o as the fold adds it: g, or cs[o] * g for a weighted push (cs = w_o * f[t, b], written by
+// tfy_ps_occ_factors_kernel: one array read through a kernel parameter keeps the scalar apply paths spill-free)
+template <bool W>
+__device__ __forceinline__ void acc_occ(float4& acc, float4 gv, const float* cs, int o) {
+    if constexpr (W) {
+        const float c = cs[o];
+        acc.x += c * gv.x; acc.y += c * gv.y; acc.z += c * gv.z; acc.w += c * gv.w;
+    } else {
+        acc.x += gv.x; acc.y += gv.y; acc.z += gv.z; acc.w += gv.w;
+    }
+}
 template <int VEC>
 __device__ __forceinline__ void apply_sum(const TfyPsHyper& h, const RowRef& x, size_t d, float4 acc, float scale,
                                           float lr, float vs) {
@@ -442,10 +467,11 @@ __device__ __forceinline__ void apply_sum(const TfyPsHyper& h, const RowRef& x, 
 }
 }  // namespace
 
-template <typename GT, int VEC>
+template <typename GT, int VEC, bool W>
 __global__ void __launch_bounds__(256)
 tfy_ps_apply_short_rows_kernel(TfyPsRows r, TfyPsHyper h, const float* __restrict__ adam_scale,
-                               const unsigned long long* __restrict__ keys, const int* __restrict__ occ, int n) {
+                               const unsigned long long* __restrict__ keys, const int* __restrict__ occ, int n,
+                               const float* __restrict__ cs) {
     const int DV = r.D / VEC, BL = r.B * r.L;
     const unsigned long long sentinel = (unsigned long long)r.T * (unsigned long long)r.V;
     float vs;
@@ -463,18 +489,18 @@ tfy_ps_apply_short_rows_kernel(TfyPsRows r, TfyPsHyper h, const float* __restric
         const GT* g = dout + (size_t)x.t * r.col_stride + c * VEC;
         float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
         for (int q = p; q < e; ++q) {
-            const float4 gv = ld_grad<GT, VEC>(g + (size_t)((occ[q] % BL) / r.L) * r.dout_ld);
-            acc.x += gv.x; acc.y += gv.y; acc.z += gv.z; acc.w += gv.w;
+            const int o = occ[q], b = (o % BL) / r.L;
+            acc_occ<W>(acc, ld_grad<GT, VEC>(g + (size_t)b * r.dout_ld), cs, o);
         }
         apply_sum<VEC>(h, x, (size_t)c * VEC, acc, r.scale, lr, vs);
     }
 }
 
-template <typename GT, int VEC>
+template <typename GT, int VEC, bool W>
 __global__ void __launch_bounds__(256)
 tfy_ps_apply_long_rows_kernel(TfyPsRows r, TfyPsHyper h, const float* __restrict__ adam_scale,
                               const unsigned long long* __restrict__ keys, const int* __restrict__ occ, int n,
-                              int cl_log2) {
+                              int cl_log2, const float* __restrict__ cs) {
     const int lane = threadIdx.x & 31;
     const int CL = 1 << cl_log2, OL = 32 >> cl_log2;
     const int cl = lane & (CL - 1), ol = lane >> cl_log2;
@@ -513,9 +539,8 @@ tfy_ps_apply_long_rows_kernel(TfyPsRows r, TfyPsHyper h, const float* __restrict
                 float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
                 if (c < DV)
                     for (int q = p0 + ol; q < e; q += OL) {
-                        const int b = (occ[q] % BL) / r.L;
-                        const float4 gv = ld_grad<GT, VEC>(g + (size_t)b * r.dout_ld + c * VEC);
-                        acc.x += gv.x; acc.y += gv.y; acc.z += gv.z; acc.w += gv.w;
+                        const int o = occ[q], b = (o % BL) / r.L;
+                        acc_occ<W>(acc, ld_grad<GT, VEC>(g + (size_t)b * r.dout_ld + c * VEC), cs, o);
                     }
                 for (int off = 16; off >= CL; off >>= 1) {
                     acc.x += __shfl_xor_sync(0xffffffffu, acc.x, off);
@@ -529,6 +554,15 @@ tfy_ps_apply_long_rows_kernel(TfyPsRows r, TfyPsHyper h, const float* __restrict
             }
         }
     }
+}
+
+// cs[o] = w_o * f[t, b] of every occurrence o (nullptr arrays count as ones), in the original order
+__global__ void __launch_bounds__(256)
+tfy_ps_occ_factors_kernel(const float* __restrict__ wts, const float* __restrict__ fs, int n, int B, int L,
+                          float* __restrict__ cs) {
+    const int BL = B * L;
+    for (int o = blockIdx.x * blockDim.x + threadIdx.x; o < n; o += gridDim.x * blockDim.x)
+        cs[o] = (wts ? wts[o] : 1.f) * (fs ? fs[(o / BL) * B + (o % BL) / L] : 1.f);
 }
 
 namespace {
@@ -549,8 +583,10 @@ size_t rows_sort_temp_bytes(int n, int end_bit) {
 size_t rows_scratch_fixed(int n) { return 2 * align256((size_t)n * 8) + 2 * align256((size_t)n * 4); }
 
 // Fold + apply of one sparse push: key build, stable radix sort, apply of the short and of the long runs.
+// weighted: take the W = true kernels, with occurrence weights wts and per-example factors fs (either may be nullptr).
 int ps_push_rows_launch(const TfyPsRows& r, const TfyPsHyper& h, const float* adam_scale, int grad_is_bf16,
-                        void* scratch, size_t scratch_bytes, cudaStream_t s) {
+                        void* scratch, size_t scratch_bytes, cudaStream_t s, bool weighted = false,
+                        const float* wts = nullptr, const float* fs = nullptr) {
     const long long n_ll = (long long)r.T * r.B * r.L;
     if (n_ll == 0) return 0;
     if (n_ll < 0 || n_ll > kPsRowsMaxOcc || r.D < 1 || r.V < 1) return -2;
@@ -571,16 +607,32 @@ int ps_push_rows_launch(const TfyPsRows& r, const TfyPsHyper& h, const float* ad
     const int per_table = r.B * r.L;
     if (per_table <= kPsBlockSortMax && r.V < 0x7fffffffLL) {
         const int local_bits = 64 - __builtin_clzll((unsigned long long)r.V);     // ids and the local sentinel V
-        tfy_ps_segment_sort_kernel<<<r.T, kPsSortThreads, 0, s>>>(r.ids, per_table, r.V, local_bits, k0, v0);
+        if (weighted)
+            tfy_ps_segment_sort_kernel<true><<<r.T, kPsSortThreads, 0, s>>>(r.ids, per_table, r.V, local_bits, k0, v0,
+                                                                             wts);
+        else
+            tfy_ps_segment_sort_kernel<false><<<r.T, kPsSortThreads, 0, s>>>(r.ids, per_table, r.V, local_bits, k0, v0,
+                                                                              nullptr);
     } else {
         size_t gk = ((size_t)n + 255) / 256;
         if (gk > TFY_NUM_SMS * 8) gk = TFY_NUM_SMS * 8;
-        tfy_ps_row_keys_kernel<<<(unsigned)gk, 256, 0, s>>>(r.ids, n, per_table, r.V, k0, v0);
+        if (weighted)
+            tfy_ps_row_keys_kernel<true><<<(unsigned)gk, 256, 0, s>>>(r.ids, n, per_table, r.V, k0, v0, wts);
+        else
+            tfy_ps_row_keys_kernel<false><<<(unsigned)gk, 256, 0, s>>>(r.ids, n, per_table, r.V, k0, v0, nullptr);
         size_t tb = temp_bytes;
         cudaError_t err = cub::DeviceRadixSort::SortPairs(temp, tb, kb, vb, n, 0, end_bit, s);
         if (err != cudaSuccess) return (int)err;
     }
 
+    // weighted: the per-occurrence factors go to the sort's alternate key buffer, free once the keys are sorted
+    float* cs = nullptr;
+    if (weighted) {
+        cs = reinterpret_cast<float*>(kb.Current() == k0 ? k1 : k0);
+        size_t gf = ((size_t)n + 255) / 256;
+        if (gf > TFY_NUM_SMS * 8) gf = TFY_NUM_SMS * 8;
+        tfy_ps_occ_factors_kernel<<<(unsigned)gf, 256, 0, s>>>(wts, fs, n, r.B, r.L, cs);
+    }
     // 16-byte gradient loads only when every row of every table slice starts on a 4-element boundary
     const size_t gsize = grad_is_bf16 ? 2 : 4;
     const bool vec = (r.D % 4 == 0) && (r.dout_ld % 4 == 0) && (r.col_stride % 4 == 0) &&
@@ -592,15 +644,20 @@ int ps_push_rows_launch(const TfyPsRows& r, const TfyPsHyper& h, const float* ad
     if (gs > TFY_NUM_SMS * 8) gs = TFY_NUM_SMS * 8;
     size_t gl = ((size_t)n + 255) / 256;                                // one warp per 32 sorted positions
     if (gl > TFY_NUM_SMS * 8) gl = TFY_NUM_SMS * 8;
-#define TFY_APPLY_ROWS(GT, VV)                                                                                         \
+#define TFY_APPLY_ROWS(GT, VV, WW)                                                                                     \
     do {                                                                                                               \
-        tfy_ps_apply_short_rows_kernel<GT, VV><<<(unsigned)gs, 256, 0, s>>>(r, h, adam_scale, kb.Current(),           \
-                                                                             vb.Current(), n);                         \
-        tfy_ps_apply_long_rows_kernel<GT, VV><<<(unsigned)gl, 256, 0, s>>>(r, h, adam_scale, kb.Current(),            \
-                                                                            vb.Current(), n, cl_log2);                 \
+        tfy_ps_apply_short_rows_kernel<GT, VV, WW><<<(unsigned)gs, 256, 0, s>>>(r, h, adam_scale, kb.Current(),       \
+                                                                                 vb.Current(), n, cs);                 \
+        tfy_ps_apply_long_rows_kernel<GT, VV, WW><<<(unsigned)gl, 256, 0, s>>>(r, h, adam_scale, kb.Current(),        \
+                                                                                vb.Current(), n, cl_log2, cs);         \
     } while (0)
-    if (grad_is_bf16) { if (vec) TFY_APPLY_ROWS(__nv_bfloat16, 4); else TFY_APPLY_ROWS(__nv_bfloat16, 1); }
-    else { if (vec) TFY_APPLY_ROWS(float, 4); else TFY_APPLY_ROWS(float, 1); }
+#define TFY_APPLY_ROWS_W(GT, VV)                                                                                       \
+    do {                                                                                                               \
+        if (weighted) TFY_APPLY_ROWS(GT, VV, true); else TFY_APPLY_ROWS(GT, VV, false);                               \
+    } while (0)
+    if (grad_is_bf16) { if (vec) TFY_APPLY_ROWS_W(__nv_bfloat16, 4); else TFY_APPLY_ROWS_W(__nv_bfloat16, 1); }
+    else { if (vec) TFY_APPLY_ROWS_W(float, 4); else TFY_APPLY_ROWS_W(float, 1); }
+#undef TFY_APPLY_ROWS_W
 #undef TFY_APPLY_ROWS
     return (int)cudaGetLastError();
 }
@@ -635,6 +692,71 @@ tfy_ps_multi_bag_kernel(const uint64_t* __restrict__ tables, const long long* __
         }
         out[i] = (OT)acc;
     }
+}
+
+// Weighted multi-hot bag (TF's embedding_column combiners, see the header): T tables x L ids per example.
+//   out[b, t * col_stride + d] (col_stride > 0)  or  out[b, d] = sum_t (col_stride 0), of S_t[b, d] / den_t[b],
+//   S = sum_present w table[i], den = 1 (sum), sum_present w (mean), sqrt(sum_present w^2) (sqrtn), 0 where den == 0.
+// One thread per (b, column slice, VEC columns); each recomputes den from its L weights (L is small), so no second
+// pass.  Sums run over t, then j.  fs[t, b] = 1/den (0 where den == 0) for the push; numeric [B, n_num] is copied
+// to columns [T*D, T*D + n_num) as K5 does.  Other columns of out are not written (the caller's pad zeros stay).
+namespace {
+template <int VEC>
+__device__ __forceinline__ float4 ld_row(const float* p) {
+    if constexpr (VEC == 4) {
+        return ld_peer_f32x4(p);
+    } else {
+        float v;
+        asm volatile("ld.global.relaxed.sys.L1::no_allocate.f32 %0, [%1];" : "=f"(v) : "l"(p) : "memory");
+        return make_float4(v, 0.f, 0.f, 0.f);
+    }
+}
+template <typename OT, int VEC>
+__device__ __forceinline__ void st_out(OT* p, float4 v) {
+    if constexpr (VEC == 4) st_local4<OT>(p, v);
+    else *p = (OT)v.x;
+}
+}  // namespace
+
+template <typename OT, int VEC>
+__global__ void __launch_bounds__(256)
+tfy_ps_multi_bag_weighted_kernel(const uint64_t* __restrict__ tables, const long long* __restrict__ ids,
+                                 const float* __restrict__ wts, int combiner, int B, int L, int T, int D, long long V,
+                                 OT* __restrict__ out, int out_ld, int col_stride, const float* __restrict__ numeric,
+                                 int n_num, float* __restrict__ fs) {
+    const int DV = D / VEC, TT = col_stride ? T : 1;
+    const size_t total = (size_t)B * TT * DV;
+    const size_t stride = (size_t)gridDim.x * blockDim.x;
+    for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += stride) {
+        const int b = (int)(i / ((size_t)TT * DV)), r = (int)(i % ((size_t)TT * DV));
+        const int tq = r / DV, c = r % DV;
+        const int t0 = col_stride ? tq : 0, t1 = col_stride ? tq + 1 : T;
+        float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
+        for (int t = t0; t < t1; ++t) {
+            const size_t o0 = ((size_t)t * B + b) * L;
+            const float* table = reinterpret_cast<const float*>(tables[t]) + (size_t)c * VEC;
+            float4 s = make_float4(0.f, 0.f, 0.f, 0.f);
+            float den = 0.f;
+            for (int j = 0; j < L; ++j) {
+                const long long id = ids[o0 + j];
+                const float w = wts ? wts[o0 + j] : 1.f;
+                if (id < 0 || id >= V || w == 0.f) continue;
+                const float4 v = ld_row<VEC>(table + (size_t)id * D);
+                s.x += w * v.x; s.y += w * v.y; s.z += w * v.z; s.w += w * v.w;
+                den += combiner == 2 ? w * w : w;
+            }
+            if (combiner == 0) den = 1.f;
+            else if (combiner == 2) den = sqrtf(den);
+            if (den != 0.f) {
+                acc.x += s.x / den; acc.y += s.y / den; acc.z += s.z / den; acc.w += s.w / den;
+            }
+            if (fs && c == 0) fs[(size_t)t * B + b] = den != 0.f ? 1.f / den : 0.f;
+        }
+        st_out<OT, VEC>(out + (size_t)b * out_ld + (size_t)tq * col_stride + (size_t)c * VEC, acc);
+    }
+    const size_t nn = (size_t)B * n_num;
+    for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < nn; i += stride)
+        out[(i / n_num) * out_ld + (size_t)T * D + i % n_num] = (OT)numeric[i];
 }
 
 // fp32 -> bf16 shadow refresh of a whole segment (run by the chief after initialisation / restore)
@@ -770,6 +892,60 @@ int tfy_ps_multi_push_rows(const uint64_t* tables, const uint64_t* s1s, const ui
     r.B = B; r.L = 1; r.T = T; r.D = D; r.V = V; r.dout_ld = dout_ld; r.col_stride = col_stride;
     r.scale = grad_scale;
     return ps_push_rows_launch(r, h, adam_scale, grad_is_bf16, scratch, scratch_bytes, s);
+}
+
+// ids int64 [T, B, L]; weights fp32 [T, B, L] or nullptr (all 1); combiner 0 sum, 1 mean, 2 sqrtn.  out (fp32 or
+// bf16, row pitch out_ld): table t in columns [t * col_stride, t * col_stride + D), or, col_stride 0, all tables
+// summed into [0, D).  numeric fp32 [B, n_num] (n_num <= 64, col_stride == D) goes to columns [T*D, T*D + n_num).
+// f fp32 [T, B] receives 1/den (0 where den == 0), or nullptr.
+int tfy_ps_multi_bag_weighted(const uint64_t* tables, const void* ids, const float* weights, int combiner, int B,
+                              int L, int T, int D, long long V, void* out, int out_is_bf16, int out_ld, int col_stride,
+                              const float* numeric, int n_num, float* f, cudaStream_t s) {
+    if (B < 1 || L < 1 || T < 1 || D < 1 || V < 1 || combiner < 0 || combiner > 2) return -2;
+    if (col_stride != 0 && col_stride < D) return -2;
+    if (n_num < 0 || n_num > 64 || (n_num > 0 && (col_stride != D || !numeric))) return -2;
+    if (out_ld < (col_stride ? (T - 1) * col_stride + D : D) + n_num) return -2;
+    const size_t osize = out_is_bf16 ? 2 : 4;
+    const bool vec = (D % 4 == 0) && (out_ld % 4 == 0) && (col_stride % 4 == 0) &&
+                     (reinterpret_cast<uintptr_t>(out) % (4 * osize) == 0);
+    const size_t total = (size_t)B * (col_stride ? T : 1) * (vec ? D / 4 : D);
+    size_t gx = (total > (size_t)B * n_num ? total : (size_t)B * n_num) + 255;
+    gx /= 256;
+    if (gx > TFY_NUM_SMS * 8) gx = TFY_NUM_SMS * 8;
+    const long long* idp = (const long long*)ids;
+#define TFY_BAG_W(OT, VV)                                                                                              \
+    tfy_ps_multi_bag_weighted_kernel<OT, VV><<<(unsigned)gx, 256, 0, s>>>(tables, idp, weights, combiner, B, L, T, D, \
+                                                                          V, (OT*)out, out_ld, col_stride, numeric,   \
+                                                                          n_num, f)
+    if (out_is_bf16) { if (vec) TFY_BAG_W(__nv_bfloat16, 4); else TFY_BAG_W(__nv_bfloat16, 1); }
+    else { if (vec) TFY_BAG_W(float, 4); else TFY_BAG_W(float, 1); }
+#undef TFY_BAG_W
+    return (int)cudaGetLastError();
+}
+
+// The sparse push of a weighted bag: the arguments of tfy_ps_multi_push_rows, plus L ids per example, the
+// occurrence weights (or nullptr) and the bag's f = 1/den (or nullptr = 1, only for combiner 0 = sum).  Occurrence
+// (t, b, j) adds weights[t, b, j] * f[t, b] * dout[b, t * col_stride + d] to its row's folded gradient.
+int tfy_ps_multi_push_rows_weighted(const uint64_t* tables, const uint64_t* s1s, const uint64_t* s2s, const void* ids,
+                                    const void* dout, int grad_is_bf16, int B, int T, int D, long long V, int opt,
+                                    float lr, float eps, float p1, float p2, float p3, float grad_scale,
+                                    const float* adam_scale, int dout_ld, int col_stride, int L, const float* weights,
+                                    const float* f, int combiner, void* scratch, size_t scratch_bytes,
+                                    cudaStream_t s) {
+    if (L < 1 || B < 0 || T < 0 || combiner < 0 || combiner > 2) return -2;
+    if (opt != TFY_OPT_SGD && opt != TFY_OPT_ADAGRAD && opt != TFY_OPT_ADAM && opt != TFY_OPT_FTRL) return -3;
+    if (opt != TFY_OPT_SGD && !s1s) return -4;
+    if ((opt == TFY_OPT_ADAM || opt == TFY_OPT_FTRL) && !s2s) return -4;
+    if (!f && combiner != 0) return -4;
+    if (dout_ld <= 0) dout_ld = D;
+    TfyPsHyper h;
+    h.opt = opt; h.lr = lr; h.eps = eps; h.wd = 0.f; h.p1 = p1; h.p2 = p2; h.p3 = p3; h.grad_scale = grad_scale;
+    TfyPsRows r = {};
+    r.tables = tables; r.s1s = s1s; r.s2s = s2s;
+    r.ids = (const long long*)ids; r.dout = dout;
+    r.B = B; r.L = L; r.T = T; r.D = D; r.V = V; r.dout_ld = dout_ld; r.col_stride = col_stride;
+    r.scale = grad_scale;
+    return ps_push_rows_launch(r, h, adam_scale, grad_is_bf16, scratch, scratch_bytes, s, true, weights, f);
 }
 
 }  // extern "C"
