@@ -49,7 +49,8 @@ constexpr int W_BYTES = TAPS * W_TAP_B;                // 36864
 
 // double-buffered fp32 accumulator tiles [2][128 rows][N + 4] (the pad keeps row-per-thread reads conflict-free)
 constexpr int FP_ACC_LD = COUT + 4, DG_ACC_LD = CIN + 4;
-constexpr int FP_STAGES = 3, FP_EPI_WARPS = 16, FP_THREADS = (FP_EPI_WARPS + 4 + 1) * 32;   // 672
+// 416 threads: the launch bound leaves the MMA warpgroup room for both halves' accumulators (2 x 32 fp32) in flight
+constexpr int FP_STAGES = 3, FP_EPI_WARPS = 8, FP_THREADS = (FP_EPI_WARPS + 4 + 1) * 32;    // 416
 constexpr size_t FP_SMEM = (size_t)FP_STAGES * A_HALO_PAD + W_BYTES + 2 * 128 * FP_ACC_LD * 4 + 1024 + 256;
 constexpr int DG_STAGES = 3, DG_EPI_WARPS = 4, DG_THREADS = (DG_EPI_WARPS + 4 + 1 + 4) * 32;  // 416: +4 un-pool producer warps
 constexpr size_t DG_SMEM = (size_t)DG_STAGES * Z_HALO_B + W_BYTES + 2 * 128 * DG_ACC_LD * 4 + 1024 + 256;
@@ -187,7 +188,8 @@ __device__ __forceinline__ void c_unpool_emit(uint8_t* tile, const CUnpoolIn& in
 // ------------------------------------------------------------------------------------------------
 // forward: pooled = dropout(maxpool2x2(relu(conv(a, W) + bias))), code byte per pooled element
 // (bits 0-1 = argmax position dy*2+dx inside the 2x2 window, bit 2 = gradient flows).
-// warps 0..15 epilogue (row quadrant = warp & 3, 16-column slice = warp >> 2), warps 16..19 MMA, warp 20 TMA
+// warps 0..7 epilogue (row quadrant = warp & 3, 16-column slices warp >> 2 and (warp >> 2) + 2), warps 8..11 MMA,
+// warp 12 TMA
 // ------------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(FP_THREADS, 1)
 tfy_conv3x3_fprop_pool_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_w,
@@ -234,44 +236,49 @@ tfy_conv3x3_fprop_pool_kernel(const __grid_constant__ CUtensorMap map_a, const _
             }
         }
     } else if (warp >= FP_EPI_WARPS) {
-        // ---------------- MMA warpgroup: both 64-pixel halves of the patch (8 (h, n) rows of the halo apart)
+        // ---------------- MMA warpgroup: the two 64-pixel halves of the patch (8 (h, n) rows of the halo apart) are
+        // two chains, each its own commit group; half 0's accumulators are stored while the tensor core runs half 1.
+        // Each chain is fully unrolled and keeps the (tap, k-step) order, so no wgmma waits on another one's
+        // registers and the result is the same bit for bit as one interleaved chain.
         const uint32_t w0 = c_smem_u32(w_tile);
-        c_mbar_wait(wfull, 0);
-        for (int i = 0; i < my_patches; ++i) {
-            const int s = i % FP_STAGES, b = i & 1;
-            c_mbar_wait(&full[s], (i / FP_STAGES) & 1);
-            if (i == 0 && threadIdx.x == FP_EPI_WARPS * 32) C_MARK(4);
-            const uint32_t a0 = c_smem_u32(stages + (size_t)s * A_HALO_PAD);
-            float acc[2][COUT / 2];
+        float acc[2][COUT / 2];
+        auto issue = [&](float (&d)[COUT / 2], uint32_t a0) {
             tfy_wg_fence();
-#pragma unroll 1
+#pragma unroll
             for (int t = 0; t < TAPS; ++t) {
                 const int kh = t / 3, kw = t - kh * 3;
 #pragma unroll
                 for (int ks = 0; ks < CIN / 16; ++ks) {
                     // B rows = output channels (64 B apart), 8-row groups 512 B apart
                     const uint64_t bdesc = c_desc(w0 + t * W_TAP_B + ks * 32, 8 * A_PIX_B, SW64);
-#pragma unroll
-                    for (int h = 0; h < 2; ++h) {
-                        // A rows = pixels: 8 consecutive w (64 B apart), next group = next (h, n) row of the halo
-                        const uint64_t adesc =
-                            c_desc(a0 + (kh + 4 * h) * 2 * A_ROW_B + kw * A_PIX_B + ks * 32, A_ROW_B, SW64);
-                        tfy_wgmma_m64n64<0, 0>(acc[h], adesc, bdesc, (t > 0 || ks > 0) ? 1u : 0u);
-                    }
+                    // A rows = pixels: 8 consecutive w (64 B apart), next group = next (h, n) row of the halo
+                    const uint64_t adesc = c_desc(a0 + kh * 2 * A_ROW_B + kw * A_PIX_B + ks * 32, A_ROW_B, SW64);
+                    tfy_wgmma_m64n64<0, 0>(d, adesc, bdesc, (t > 0 || ks > 0) ? 1u : 0u);
                 }
             }
             tfy_wg_commit();
+        };
+        c_mbar_wait(wfull, 0);
+        for (int i = 0; i < my_patches; ++i) {
+            const int s = i % FP_STAGES, b = i & 1;
+            float* tile = acc_s + b * 128 * FP_ACC_LD;
+            c_mbar_wait(&full[s], (i / FP_STAGES) & 1);
+            if (i == 0 && threadIdx.x == FP_EPI_WARPS * 32) C_MARK(4);
+            const uint32_t a0 = c_smem_u32(stages + (size_t)s * A_HALO_PAD);
+            issue(acc[0], a0);
+            issue(acc[1], a0 + 4 * 2 * A_ROW_B);
+            if (i >= 2) c_mbar_wait(&tempty[b], ((i >> 1) - 1) & 1);
+            tfy_wg_wait<1>();                                     // half 0 is complete
+            tfy_wg_store_rows<COUT>(tile, FP_ACC_LD, acc[0], 0);
             tfy_wg_wait<0>();
             if (lane == 0) c_mbar_arrive(&empty[s]);
-            if (i >= 2) c_mbar_wait(&tempty[b], ((i >> 1) - 1) & 1);
-            tfy_wg_store_rows<COUT>(acc_s + b * 128 * FP_ACC_LD, FP_ACC_LD, acc[0], 0);
-            tfy_wg_store_rows<COUT>(acc_s + b * 128 * FP_ACC_LD, FP_ACC_LD, acc[1], 64);
+            tfy_wg_store_rows<COUT>(tile, FP_ACC_LD, acc[1], 64);
             c_mbar_arrive(&tfull[b]);
             if (threadIdx.x == FP_EPI_WARPS * 32) { if (i == 0) C_MARK(5); if (i == my_patches - 1) C_MARK(11); }
         }
     } else {
         // ---------------- epilogue: accumulator row r = (h, n, w) = (r/16, (r/8)&1, r%8) is row r of the staged tile
-        const int quad = warp & 3, cq = warp >> 2;
+        const int quad = warp & 3, cq0 = warp >> 2;                // column slices cq0 and cq0 + 2
         const int r = quad * 32 + lane;
         const int h = r >> 4, n = (r >> 3) & 1, w = r & 7;
         const int dx = lane & 1, dy = (lane >> 4) & 1;            // position inside the 2x2 pooling window
@@ -282,60 +289,74 @@ tfy_conv3x3_fprop_pool_kernel(const __grid_constant__ CUtensorMap map_a, const _
         const uint32_t thr = drop_rate > 0.f ? (uint32_t)(drop_rate * 256.f + 0.5f) : 0u;
         const float keep_scale = 256.f / (256.f - (float)thr);
         const uint32_t salt = seed ^ c_hash32(step * 0x9E3779B9U + 0x85ebca6bU);
-        // after the two exchanges below lane (dy, dx) owns columns [8 dx + 4 dy, +4) of the warp's 16
-        const int col = cq * 16 + dx * 8 + dy * 4;
-        const uint2 braw = *reinterpret_cast<const uint2*>(bias + col);
-        const float bv[4] = {tfy_bf16lo(braw.x), tfy_bf16hi(braw.x), tfy_bf16lo(braw.y), tfy_bf16hi(braw.y)};
+        // after the two exchanges below lane (dy, dx) owns columns [8 dx + 4 dy, +4) of each of the warp's slices
+        float bv[2][4];
+#pragma unroll
+        for (int k = 0; k < 2; ++k) {
+            const uint2 braw = *reinterpret_cast<const uint2*>(bias + (cq0 + 2 * k) * 16 + dx * 8 + dy * 4);
+            bv[k][0] = tfy_bf16lo(braw.x); bv[k][1] = tfy_bf16hi(braw.x);
+            bv[k][2] = tfy_bf16lo(braw.y); bv[k][3] = tfy_bf16hi(braw.y);
+        }
         CPatchIter it(tiles_x, tiles_y);
         for (int i = 0; i < my_patches; ++i, it.next()) {
             const int b = i & 1;
-            const uint32_t prow =
-                (uint32_t)((((it.bz * 2 + n) * PH + ((it.ty * 8 + h) >> 1)) * PW + ((it.tx * 8 + w) >> 1)) * COUT + col);
             c_mbar_wait(&tfull[b], (i >> 1) & 1);
             if (threadIdx.x == 0) { if (i == 0) C_MARK(6); if (i == my_patches - 1) C_MARK(8); }
-            uint32_t acc[16];
-            const float* src = acc_s + (size_t)(b * 128 + r) * FP_ACC_LD + cq * 16;
+            uint32_t accs[2][16];
 #pragma unroll
-            for (int j = 0; j < 16; j += 4) *reinterpret_cast<uint4*>(acc + j) = *reinterpret_cast<const uint4*>(src + j);
+            for (int k = 0; k < 2; ++k) {
+                const float* src = acc_s + (size_t)(b * 128 + r) * FP_ACC_LD + (cq0 + 2 * k) * 16;
+#pragma unroll
+                for (int j = 0; j < 16; j += 4)
+                    *reinterpret_cast<uint4*>(accs[k] + j) = *reinterpret_cast<const uint4*>(src + j);
+            }
             c_mbar_arrive(&tempty[b]);                             // the MMA warps may overwrite this buffer now
-            // tag every value with its window position in the 2 low mantissa bits, then reduce-scatter the
-            // max over the window (lane ^ 1: other column, lane ^ 16: other row)
-            float v[16];
 #pragma unroll
-            for (int j = 0; j < 16; ++j) v[j] = __uint_as_float((acc[j] & ~3u) | tag);
-            float m8[8];
+            for (int k = 0; k < 2; ++k) {
+                const int col = (cq0 + 2 * k) * 16 + dx * 8 + dy * 4;
+                const uint32_t prow = (uint32_t)((((it.bz * 2 + n) * PH + ((it.ty * 8 + h) >> 1)) * PW +
+                                                  ((it.tx * 8 + w) >> 1)) * COUT + col);
+                const uint32_t* acc = accs[k];
+                // tag every value with its window position in the 2 low mantissa bits, then reduce-scatter the
+                // max over the window (lane ^ 1: other column, lane ^ 16: other row)
+                float v[16];
 #pragma unroll
-            for (int j = 0; j < 8; ++j) {
-                const float send = dx ? v[j] : v[8 + j];
-                const float keep = dx ? v[8 + j] : v[j];
-                m8[j] = fmaxf(keep, __shfl_xor_sync(0xffffffffu, send, 1));
+                for (int j = 0; j < 16; ++j) v[j] = __uint_as_float((acc[j] & ~3u) | tag);
+                float m8[8];
+#pragma unroll
+                for (int j = 0; j < 8; ++j) {
+                    const float send = dx ? v[j] : v[8 + j];
+                    const float keep = dx ? v[8 + j] : v[j];
+                    m8[j] = fmaxf(keep, __shfl_xor_sync(0xffffffffu, send, 1));
+                }
+                float m4[4];
+#pragma unroll
+                for (int j = 0; j < 4; ++j) {
+                    const float send = dy ? m8[j] : m8[4 + j];
+                    const float keep = dy ? m8[4 + j] : m8[j];
+                    m4[j] = fmaxf(keep, __shfl_xor_sync(0xffffffffu, send, 16));
+                }
+                const uint32_t rnd =
+                    thr ? c_hash32(salt ^ c_hash32((prow >> 2) * 0xC2B2AE35U + 0x27d4eb2fU)) : 0xffffffffu;
+                float o[4];
+                uint32_t codes = 0;
+#pragma unroll
+                for (int j = 0; j < 4; ++j) {
+                    const uint32_t pos = __float_as_uint(m4[j]) & 3u;
+                    float x = m4[j] + bv[k][j];
+                    const bool on = x > 0.f && ((rnd >> (8 * j)) & 0xffu) >= thr;
+                    x = on ? x * keep_scale : 0.f;
+                    o[j] = x;
+                    codes |= (pos | (on ? 4u : 0u)) << (8 * j);
+                }
+                __nv_bfloat162 lo = __floats2bfloat162_rn(o[0], o[1]), hi = __floats2bfloat162_rn(o[2], o[3]);
+                uint2 packed;
+                packed.x = *reinterpret_cast<uint32_t*>(&lo);
+                packed.y = *reinterpret_cast<uint32_t*>(&hi);
+                *reinterpret_cast<uint2*>(pooled + prow) = packed;
+                *reinterpret_cast<uint32_t*>(code + prow) = codes;
+                if (threadIdx.x == 0) { if (i == 0) C_MARK(7); if (i == my_patches - 1) C_MARK(9); }
             }
-            float m4[4];
-#pragma unroll
-            for (int j = 0; j < 4; ++j) {
-                const float send = dy ? m8[j] : m8[4 + j];
-                const float keep = dy ? m8[4 + j] : m8[j];
-                m4[j] = fmaxf(keep, __shfl_xor_sync(0xffffffffu, send, 16));
-            }
-            const uint32_t rnd = thr ? c_hash32(salt ^ c_hash32((prow >> 2) * 0xC2B2AE35U + 0x27d4eb2fU)) : 0xffffffffu;
-            float o[4];
-            uint32_t codes = 0;
-#pragma unroll
-            for (int j = 0; j < 4; ++j) {
-                const uint32_t pos = __float_as_uint(m4[j]) & 3u;
-                float x = m4[j] + bv[j];
-                const bool on = x > 0.f && ((rnd >> (8 * j)) & 0xffu) >= thr;
-                x = on ? x * keep_scale : 0.f;
-                o[j] = x;
-                codes |= (pos | (on ? 4u : 0u)) << (8 * j);
-            }
-            __nv_bfloat162 lo = __floats2bfloat162_rn(o[0], o[1]), hi = __floats2bfloat162_rn(o[2], o[3]);
-            uint2 packed;
-            packed.x = *reinterpret_cast<uint32_t*>(&lo);
-            packed.y = *reinterpret_cast<uint32_t*>(&hi);
-            *reinterpret_cast<uint2*>(pooled + prow) = packed;
-            *reinterpret_cast<uint32_t*>(code + prow) = codes;
-            if (threadIdx.x == 0) { if (i == 0) C_MARK(7); if (i == my_patches - 1) C_MARK(9); }
         }
     }
     __syncthreads();
