@@ -19,6 +19,7 @@ from tf_yarn_b200.estimator import feature_column as fc
 from tf_yarn_b200.estimator.config import RunConfig
 from tf_yarn_b200.estimator.estimator import Estimator
 from tf_yarn_b200.estimator.spec import EstimatorSpec
+from tf_yarn_b200.keras import metrics as kmetrics
 from tf_yarn_b200.keras import optimizers as kopt
 
 
@@ -44,7 +45,49 @@ def _classification_metrics(n_classes: int) -> Dict[str, Callable]:
     def average_loss(labels, logits):
         n = labels.reshape(-1).shape[0]
         return _classification_loss(n_classes)(labels, logits) * n, float(n)
-    return {"accuracy": accuracy, "average_loss": average_loss}
+    ops: Dict[str, Any] = {"accuracy": accuracy, "average_loss": average_loss}
+    if n_classes == 2:
+        # the rest of TF's binary head: tensorflow_estimator head/binary_class_head.py
+        def label_mean(labels, logits):
+            y = labels.float().reshape(-1)
+            return y.sum(), float(y.numel())
+
+        def prediction_mean(labels, logits):
+            p = torch.sigmoid(logits.float().reshape(-1))
+            return p.sum(), float(p.numel())
+
+        ops.update({"auc": kmetrics.AUC(from_logits=True, name="auc"),
+                    "auc_precision_recall": kmetrics.AUC(curve="PR", from_logits=True, name="auc_precision_recall"),
+                    "precision": kmetrics.Precision(from_logits=True), "recall": kmetrics.Recall(from_logits=True),
+                    "label/mean": label_mean, "prediction/mean": prediction_mean,
+                    "accuracy_baseline": _AccuracyBaseline()})
+    return ops
+
+
+class _AccuracyBaseline(kmetrics.Metric):
+    """``max(m, 1 - m)`` for the label mean ``m``: the accuracy of always predicting the majority class."""
+
+    def __init__(self, name: str = "accuracy_baseline"):
+        super().__init__(name)
+        self._sum: Optional[torch.Tensor] = None         # float64 [2]: sum of the labels, their count
+
+    def update_state(self, y_true, y_pred, sample_weight=None) -> None:
+        y = y_true.detach().reshape(-1).double()
+        if self._sum is None:
+            self._sum = torch.zeros(2, dtype=torch.float64, device=y.device)
+        self._sum[0] += y.sum()
+        self._sum[1] += y.numel()
+
+    def result(self) -> float:
+        if self._sum is None:
+            return 0.0
+        s, n = self._sum.tolist()
+        m = s / n if n else 0.0
+        return max(m, 1.0 - m)
+
+    def reset_state(self) -> None:
+        if self._sum is not None:
+            self._sum.zero_()
 
 
 def _classification_predictions(n_classes: int) -> Callable:

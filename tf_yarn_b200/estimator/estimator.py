@@ -36,6 +36,7 @@ from tf_yarn_b200.estimator.config import RunConfig
 from tf_yarn_b200.estimator.hooks import (GLOBAL_STEP, SessionRunArgs, SessionRunContext, SessionRunValues)
 from tf_yarn_b200.estimator.spec import EstimatorSpec, GraphKeys, ModeKeys
 from tf_yarn_b200.keras import optimizers as kopt
+from tf_yarn_b200.keras.metrics import Metric
 
 logger = logging.getLogger(__name__)
 
@@ -491,6 +492,10 @@ class Estimator:
                 h.after_create_session()
         ctx = SessionRunContext(self, gs)
         metric_fns = dict(spec.eval_metric_ops or {})
+        # values are (numerator, denominator) callables or stateful keras.metrics.Metric objects (AUC, ...), as in TF2
+        stateful = {k for k, fn in metric_fns.items() if isinstance(fn, Metric)}
+        for k in stateful:
+            metric_fns[k].reset_state()
         num = {k: 0.0 for k in metric_fns}
         den = {k: 0.0 for k in metric_fns}
         loss_sum, n_batches = 0.0, 0
@@ -507,6 +512,9 @@ class Estimator:
                 if spec.loss is not None:
                     loss_sum += float(spec.loss(labels, outputs))
                 for k, fn in metric_fns.items():
+                    if k in stateful:
+                        fn.update_state(labels, outputs)        # device-side state: no host read per batch
+                        continue
                     a, b = fn(labels, outputs)
                     num[k] += float(a)
                     den[k] += float(b)
@@ -522,8 +530,8 @@ class Estimator:
             except TypeError:
                 h.end()
         results: Dict[str, Any] = {"loss": loss_sum / max(n_batches, 1)}
-        for k in metric_fns:
-            results[k] = num[k] / max(den[k], 1.0)
+        for k, fn in metric_fns.items():
+            results[k] = fn.result() if k in stateful else num[k] / max(den[k], 1.0)
         results[GraphKeys.GLOBAL_STEP] = gs
         eval_dir = os.path.join(self._model_dir, "eval" if not name else f"eval_{name}")
         w = summary_lib.writer(eval_dir)

@@ -27,7 +27,9 @@ class EstimatorSpec(NamedTuple):
     optimizers      optional ``{parameter-name prefix: optimizer}``: a different optimizer per part of the
                     network (longest matching prefix wins, ``optimizer`` is the default) -- TF's wide-and-deep
                     trains the linear tower with FTRL and the deep tower with Adagrad.
-    eval_metric_ops ``{name: callable(labels, outputs) -> (numerator, denominator)}`` streaming metrics.
+    eval_metric_ops ``{name: callable(labels, outputs) -> (numerator, denominator)}`` streaming metrics, or
+                    ``{name: keras.metrics.Metric}`` (``reset_state`` / ``update_state(labels, outputs)`` /
+                    ``result``, as TF2 Estimators take them).
     predictions     callable ``outputs -> dict`` (PREDICT), default identity.
     train_op / export_outputs are accepted for signature parity and ignored.
     """

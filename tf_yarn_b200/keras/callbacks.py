@@ -13,6 +13,13 @@ from typing import Any, Callable, Dict, List, Optional
 logger = logging.getLogger(__name__)
 
 
+def _auto_mode(monitor: str) -> str:
+    """``mode="auto"``: larger is better for accuracies and for the AUC / precision / recall metrics."""
+    if "acc" in monitor or monitor.endswith(("auc", "precision", "recall")):
+        return "max"
+    return "min"
+
+
 class Callback:
     def __init__(self):
         self.model = None
@@ -71,7 +78,7 @@ class ModelCheckpoint(Callback):
         self.period, self.verbose = period, verbose
         self._since = 0
         if mode == "auto":
-            mode = "max" if "acc" in monitor else "min"
+            mode = _auto_mode(monitor)
         self._better = (lambda a, b: a > b) if mode == "max" else (lambda a, b: a < b)
         self.best: Optional[float] = None
 
@@ -137,7 +144,7 @@ class EarlyStopping(Callback):
         super().__init__()
         self.monitor, self.min_delta, self.patience = monitor, min_delta, patience
         if mode == "auto":
-            mode = "max" if "acc" in monitor else "min"
+            mode = _auto_mode(monitor)
         self._sign = 1.0 if mode == "max" else -1.0
         self.best: Optional[float] = None
         self.wait = 0

@@ -30,6 +30,7 @@ import torch.nn as nn
 
 from tf_yarn_b200.keras import losses as loss_mod
 from tf_yarn_b200.keras import weighting
+from tf_yarn_b200.keras.metrics import Metric
 
 logger = logging.getLogger(__name__)
 
@@ -100,18 +101,33 @@ class EagerTrainEngine:
         logs = {"loss": loss.detach()}
         with torch.no_grad():
             for name, fn in self.metric_fns:
+                if isinstance(fn, Metric):
+                    fn.update_state(y, out)
+                    continue
                 num, den = fn(y, out)
                 logs[name] = num / den
             for acc, (_, fn) in zip(self._wacc, self.weighted_metric_fns):
+                if isinstance(fn, Metric):
+                    fn.update_state(y, out, sample_weight=sw)
+                    continue
                 num, den = fn(y, out, sample_weight=sw)
                 acc[0] += float(num)
                 acc[1] += float(den)
         return logs
 
+    @property
+    def stateful_metrics(self) -> List[Metric]:
+        return [fn for _, fn in self.metric_fns + self.weighted_metric_fns if isinstance(fn, Metric)]
+
     def pop_metrics(self) -> Dict[str, float]:
-        """The weighted metrics of the steps since the last call, ``sum(w*m) / sum(w)`` over all of them."""
-        out = {name: (num / den if den else 0.0) for (name, _), (num, den) in zip(self.weighted_metric_fns, self._wacc)}
+        """The weighted metrics of the steps since the last call, ``sum(w*m) / sum(w)`` over all of them, and the
+        results of the stateful metrics (AUC, ...), which are then reset."""
+        out = {name: fn.result() for name, fn in self.metric_fns if isinstance(fn, Metric)}
+        for (name, fn), (num, den) in zip(self.weighted_metric_fns, self._wacc):
+            out[name] = fn.result() if isinstance(fn, Metric) else (num / den if den else 0.0)
         self._wacc = [[0.0, 0.0] for _ in self.weighted_metric_fns]
+        for m in self.stateful_metrics:
+            m.reset_state()
         return out
 
     def set_learning_rate(self, lr: float) -> None:
@@ -255,12 +271,18 @@ class GraphTrainEngine:
         if self.metric_fns:
             with torch.no_grad():
                 for i, (_, fn) in enumerate(self.metric_fns):
+                    if isinstance(fn, Metric):          # stateful: one histogram kernel launch, state on the device
+                        fn.update_state(y, out)
+                        continue
                     num, den = fn(y, out)
                     self._metric_acc[i, 0] += num
                     self._metric_acc[i, 1] += den
         if self.weighted_metric_fns:
             with torch.no_grad():
                 for i, (_, fn) in enumerate(self.weighted_metric_fns, start=len(self.metric_fns)):
+                    if isinstance(fn, Metric):
+                        fn.update_state(y, out, sample_weight=sw)
+                        continue
                     num, den = fn(y, out, sample_weight=sw)
                     self._metric_acc[i, 0] += num
                     self._metric_acc[i, 1] += den
@@ -288,6 +310,8 @@ class GraphTrainEngine:
         fused = self.fused
         snap = (fused.master.clone(), fused.s1.clone(), fused.s2.clone(), fused.flat_params.clone(),
                 fused.hyper.clone(), self._metric_acc.clone())
+        # stateful metrics allocate their device state on their first update (a warm-up step): empty until then
+        metric_snap = [[t.clone() for t in m.state_tensors()] for m in self.stateful_metrics]
         self.stream.wait_stream(torch.cuda.current_stream())
         with torch.cuda.stream(self.stream):
             for _ in range(3):
@@ -324,6 +348,12 @@ class GraphTrainEngine:
             fused.master.copy_(snap[0]); fused.s1.copy_(snap[1]); fused.s2.copy_(snap[2])
             fused.flat_params.copy_(snap[3]); fused.hyper.copy_(snap[4]); self._metric_acc.copy_(snap[5])
             fused.flat_grads.zero_()
+            for m, saved in zip(self.stateful_metrics, metric_snap):
+                if saved:
+                    for t, v in zip(m.state_tensors(), saved):
+                        t.copy_(v)
+                else:
+                    m.reset_state()
         self.stream.synchronize()
         if self.distributed:
             self.comm.barrier()
@@ -415,13 +445,25 @@ class GraphTrainEngine:
         self.stream.synchronize()
         return {"loss": self._loss.clone()}
 
+    @property
+    def stateful_metrics(self) -> List[Metric]:
+        return [fn for _, fn in self.metric_fns + self.weighted_metric_fns if isinstance(fn, Metric)]
+
     def pop_metrics(self) -> Dict[str, float]:
         self.stream.synchronize()
         acc = self._metric_acc.cpu()
         self._metric_acc.zero_()
-        out = {name: float(acc[i, 0] / acc[i, 1].clamp_min(1)) for i, (name, _) in enumerate(self.metric_fns)}
-        for i, (name, _) in enumerate(self.weighted_metric_fns, start=len(self.metric_fns)):
-            out[name] = float(acc[i, 0] / acc[i, 1]) if float(acc[i, 1]) != 0.0 else 0.0
+        out = {}
+        for i, (name, fn) in enumerate(self.metric_fns):
+            out[name] = fn.result() if isinstance(fn, Metric) else float(acc[i, 0] / acc[i, 1].clamp_min(1))
+        for i, (name, fn) in enumerate(self.weighted_metric_fns, start=len(self.metric_fns)):
+            if isinstance(fn, Metric):
+                out[name] = fn.result()
+            else:
+                out[name] = float(acc[i, 0] / acc[i, 1]) if float(acc[i, 1]) != 0.0 else 0.0
+        with torch.cuda.stream(self.stream):            # ordered before the next epoch's steps
+            for m in self.stateful_metrics:
+                m.reset_state()
         return out
 
     def set_learning_rate(self, lr: float) -> None:

@@ -257,13 +257,21 @@ class Model:
                 compute_dtype: Optional[torch.dtype] = None, use_cuda_graph: bool = True,
                 use_fast_path: bool = True, weighted_metrics: Optional[Sequence[str]] = None, **_ignored) -> None:
         """``metrics`` are unweighted; ``weighted_metrics`` (built-in metric names) are ``sum(w*m) / sum(w)`` over the
-        sample weights of ``fit`` / ``evaluate`` (``class_weight`` included)."""
+        sample weights of ``fit`` / ``evaluate`` (``class_weight`` included).  Both accept the stateful metrics
+        ``"AUC"``, ``"Precision"`` and ``"Recall"``; ``metrics`` also takes such objects (``keras.metrics.AUC(...)``),
+        whose names must be unique."""
         if _ignored:
             logger.warning("Model.compile: unsupported arguments ignored: %s", sorted(_ignored))
         for m in weighted_metrics or []:
             if not isinstance(m, str):
                 raise ValueError(f"weighted_metrics accepts built-in metric names only, got {m!r}")
             metric_mod.resolve(m, loss_mod.name_of(loss), 2)          # unknown names fail here
+        for spec in (metrics or [], weighted_metrics or []):
+            resolved = [metric_mod.resolve(m, loss_mod.name_of(loss), 2) for m in spec]
+            names = [name for name, _ in resolved]
+            for name, fn in resolved:
+                if isinstance(fn, metric_mod.Metric) and names.count(name) > 1:
+                    raise ValueError(f"metric name {name!r} is used twice: give the metrics distinct names")
         self.optimizer = opt_mod.get(optimizer)
         self.loss = loss
         self._loss_fn = loss_mod.get(loss) if loss is not None else None
@@ -450,7 +458,7 @@ class Model:
                                     sample_weight=validation_data[2] if pair and len(validation_data) > 2 else None)
                 logs.update({f"val_{k}": v for k, v in val.items()})
             if verbose:
-                msg = " - ".join(f"{k}: {v:.4f}" for k, v in logs.items())
+                msg = " - ".join(f"{k}: {_fmt(v)}" for k, v in logs.items())
                 logger.info("Epoch %d/%d - %.1fs - %s", epoch + 1, epochs, time.time() - t0, msg)
             cbs.call("on_epoch_end", epoch, logs)
         cbs.call("on_train_end", None)
@@ -497,7 +505,7 @@ class Model:
             step += 1
         out = {"loss": loss_sum / max(n, 1)}
         out.update({k: v / max(n, 1) for k, v in metric_sums.items()})
-        if getattr(eng, "weighted_metric_fns", None):
+        if getattr(eng, "weighted_metric_fns", None) or getattr(eng, "stateful_metrics", None):
             out.update(eng.pop_metrics())
         return out
 
@@ -611,7 +619,7 @@ class Model:
                 xb, yb, wb = _split_batch(item)
                 xb = self._prep_infer(_as_struct(xb))
                 self.net.eval()
-                if not fns and self.loss is not None:
+                if not fns and not wfns and self.loss is not None:
                     fns = self._metric_fns()
                     m_num, m_den = [0.0] * len(fns), [0.0] * len(fns)
                     wfns = self._weighted_metric_fns()
@@ -629,19 +637,28 @@ class Model:
                         loss_sum += float((loss_mod.per_sample(self._loss_fn)(yb, out) * wb).sum())
                 count += bs
                 for i, (_, fn) in enumerate(fns):
+                    if isinstance(fn, metric_mod.Metric):      # streaming state on the device, read once at the end
+                        fn.update_state(yb, out)
+                        continue
                     a, b = fn(yb, out)
                     m_num[i] += float(a)
                     m_den[i] += float(b)
                 for i, (_, fn) in enumerate(wfns):
+                    if isinstance(fn, metric_mod.Metric):
+                        fn.update_state(yb, out, sample_weight=wb)
+                        continue
                     a, b = fn(yb, out, sample_weight=wb)
                     w_num[i] += float(a)
                     w_den[i] += float(b)
                 n += 1
         res = {"loss": loss_sum / max(count, 1)}
-        for i, (name, _) in enumerate(fns):
-            res[name] = m_num[i] / max(m_den[i], 1.0)
-        for i, (name, _) in enumerate(wfns):
-            res[name] = w_num[i] / w_den[i] if w_den[i] else 0.0
+        for i, (name, fn) in enumerate(fns):
+            res[name] = fn.result() if isinstance(fn, metric_mod.Metric) else m_num[i] / max(m_den[i], 1.0)
+        for i, (name, fn) in enumerate(wfns):
+            if isinstance(fn, metric_mod.Metric):
+                res[name] = fn.result()
+            else:
+                res[name] = w_num[i] / w_den[i] if w_den[i] else 0.0
         if return_dict:
             return res
         vals = list(res.values())
@@ -740,7 +757,8 @@ class Model:
             "weights": self._fp32_state(),
             "compile": {"loss": loss_mod.serialize(self.loss),
                         "optimizer": self.optimizer.get_config() if self.optimizer is not None else None,
-                        "metrics": [m for m in self._metrics_spec if isinstance(m, str)],
+                        "metrics": [spec for spec in map(metric_mod.serialize, self._metrics_spec)
+                                    if spec is not None],
                         "weighted_metrics": list(self._weighted_metrics_spec)},
             "optimizer_state": (self._engine.state_dict() if (include_optimizer and self._engine is not None
                                                               and not self._sharded_across_ranks()) else None),
@@ -789,9 +807,15 @@ def load_model(filepath: str, compile: bool = True) -> Model:
     comp = payload.get("compile") or {}
     if compile and comp.get("loss") and comp.get("optimizer"):
         model.compile(optimizer=opt_mod.from_config(comp["optimizer"]), loss=loss_mod.deserialize(comp["loss"]),
-                      metrics=comp.get("metrics") or [], weighted_metrics=comp.get("weighted_metrics") or [])
+                      metrics=[m for m in map(metric_mod.deserialize, comp.get("metrics") or []) if m is not None],
+                      weighted_metrics=comp.get("weighted_metrics") or [])
         model._pending_engine_state = payload.get("optimizer_state")
     return model
+
+
+def _fmt(v) -> str:
+    """A log value: a float, or the list of values of a metric with several thresholds."""
+    return "[" + ", ".join(f"{x:.4f}" for x in v) + "]" if isinstance(v, (list, tuple)) else f"{v:.4f}"
 
 
 def _batch_size_of(out) -> int:
