@@ -160,5 +160,7 @@ def test_every_kernel_launched_with_programmatic_dependent_launch_waits_for_its_
         assert waits, f"{kernel} ({os.path.basename(path)}) is launched with PDL but never waits for its dependency"
         prologue = body[:min(waits)]
         # the prologue may set up shared memory, barriers and prefetch tensor maps / this kernel's own state
-        for forbidden in ("tfy_ld16(", "__ldg(", "__ldcg(", "atomicAdd(", "tfy_st16(", "red_add", "cp.async.bulk.tensor"):
+        # (tfy_tma_*: the TMA load / store helpers of tfy_tma.cuh)
+        for forbidden in ("tfy_ld16(", "__ldg(", "__ldcg(", "atomicAdd(", "tfy_st16(", "red_add", "cp.async.bulk.tensor",
+                          "tfy_tma_"):
             assert forbidden not in prologue, (kernel, forbidden)

@@ -184,6 +184,15 @@ __device__ __forceinline__ uint4 tfy_ld16_stream(const void* p) {
                  : "memory");
     return v;
 }
+// the same load as fp32 lanes: rows of a parameter server's master tables, possibly on a peer GPU
+__device__ __forceinline__ float4 tfy_ld_peer_f32x4(const void* p) {
+    float4 v;
+    asm volatile("ld.global.relaxed.sys.L1::no_allocate.v4.f32 {%0,%1,%2,%3}, [%4];"
+                 : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w)
+                 : "l"(p)
+                 : "memory");
+    return v;
+}
 __device__ __forceinline__ void tfy_st16(void* p, uint4 v) {
     asm volatile("st.global.v4.u32 [%0], {%1,%2,%3,%4};" ::"l"(p), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w)
                  : "memory");

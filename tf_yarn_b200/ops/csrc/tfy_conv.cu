@@ -26,10 +26,9 @@
 //
 // Operand layout: whole-pixel rows (64/128 B) + swizzle, so a patch is 200 TMA rows instead of the
 // 800-1600 16-byte rows of an un-swizzled [pixel][16 B] layout.
-#include <cuda.h>
-
 #include "tfy_common.cuh"
 #include "tfy_fused_step.cuh"
+#include "tfy_tma.cuh"
 #include "tfy_wgmma.cuh"
 
 namespace {
@@ -63,62 +62,6 @@ constexpr size_t WG_SMEM = (size_t)WG_STAGES * WG_STAGE_B + 1024 + 512 + WG_WORK
 
 constexpr uint32_t SW128 = TFY_WG_SW128, SW64 = TFY_WG_SW64;
 
-__device__ __forceinline__ uint32_t c_smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ void c_mbar_init(uint64_t* bar, uint32_t count) {
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(c_smem_u32(bar)), "r"(count) : "memory");
-}
-__device__ __forceinline__ void c_mbar_arrive(uint64_t* bar) {
-    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(c_smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void c_mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
-    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(c_smem_u32(bar)), "r"(bytes)
-                 : "memory");
-}
-__device__ __forceinline__ void c_mbar_wait(uint64_t* bar, uint32_t parity) {
-    asm volatile(
-        "{\n\t"
-        ".reg .pred P1;\n\t"
-        "CWAIT_LOOP:\n\t"
-        "mbarrier.try_wait.parity.shared::cta.b64 P1, [%0], %1;\n\t"
-        "@P1 bra CDONE;\n\t"
-        "bra CWAIT_LOOP;\n\t"
-        "CDONE:\n\t"
-        "}" ::"r"(c_smem_u32(bar)), "r"(parity) : "memory");
-}
-__device__ __forceinline__ void c_tma_4d(const CUtensorMap* map, uint64_t* bar, void* dst, int c0, int c1, int c2,
-                                         int c3) {
-    asm volatile(
-        "cp.async.bulk.tensor.4d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], "
-        "[%2];" ::"r"(c_smem_u32(dst)), "l"(reinterpret_cast<uint64_t>(map)), "r"(c_smem_u32(bar)), "r"(c0), "r"(c1),
-        "r"(c2), "r"(c3)
-        : "memory");
-}
-__device__ __forceinline__ void c_tma_3d(const CUtensorMap* map, uint64_t* bar, void* dst, int c0, int c1, int c2) {
-    asm volatile(
-        "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];"
-        ::"r"(c_smem_u32(dst)), "l"(reinterpret_cast<uint64_t>(map)), "r"(c_smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2)
-        : "memory");
-}
-__device__ __forceinline__ void c_prefetch_map(const CUtensorMap* map) {
-    asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(map)) : "memory");
-}
-// Swizzled wgmma shared-memory descriptor (base_offset 0: the swizzle phase comes from the absolute address).
-// sbo = byte distance between consecutive groups of 8 rows (K-major: 8 M/N rows; MN-major: 8 K rows).
-__device__ __forceinline__ uint64_t c_desc(uint32_t smem_addr, uint32_t sbo, uint32_t layout) {
-    return tfy_wg_desc(smem_addr, 16, sbo, layout);
-}
-// One lane of a CONVERGED warp: the compiler knows the guarded region runs on exactly one thread and keeps
-// the TMA operands in uniform registers.
-__device__ __forceinline__ bool c_elect_one() {
-    uint32_t pred;
-    asm volatile("{\n\t.reg .pred P;\n\telect.sync _|P, 0xffffffff;\n\tselp.b32 %0, 1, 0, P;\n\t}" : "=r"(pred));
-    return pred != 0;
-}
-
-__device__ __forceinline__ uint32_t c_hash32(uint32_t x) {
-    x ^= x >> 16; x *= 0x7feb352dU; x ^= x >> 15; x *= 0x846ca68bU; x ^= x >> 16;
-    return x;
-}
 // Optional per-CTA event timeline (tests/gpu/conv_check.py): 16 slots of SM-clock deltas per CTA.
 __device__ long long* c_timeline = nullptr;
 #define C_MARK(k)                                                                  \
@@ -133,10 +76,6 @@ __device__ long long* c_timeline = nullptr;
         asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(ns)); \
         c_tl[(size_t)blockIdx.x * 16] = (long long)ns;          \
     }
-
-__device__ __forceinline__ uint8_t* c_align1024(uint8_t* p) {
-    return reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(p) + 1023) & ~(uintptr_t)1023);
-}
 
 #include "tfy_conv_index.cuh"
 
@@ -198,7 +137,7 @@ tfy_conv3x3_fprop_pool_kernel(const __grid_constant__ CUtensorMap map_a, const _
                               float drop_rate, uint32_t seed, const TfyOptHyper* __restrict__ hp) {
     extern __shared__ uint8_t smem_raw[];
     C_TIMELINE_BEGIN();
-    uint8_t* stages = c_align1024(smem_raw);                      // [3][10 h][2 n][10 w][64 B], 64B swizzle
+    uint8_t* stages = tfy_align1024(smem_raw);                      // [3][10 h][2 n][10 w][64 B], 64B swizzle
     uint8_t* w_tile = stages + (size_t)FP_STAGES * A_HALO_PAD;    // [9][64 o][64 B], 64B swizzle
     float* acc_s = reinterpret_cast<float*>(w_tile + W_BYTES);    // [2][128][FP_ACC_LD]
     uint64_t* full = reinterpret_cast<uint64_t*>(acc_s + 2 * 128 * FP_ACC_LD);
@@ -209,11 +148,11 @@ tfy_conv3x3_fprop_pool_kernel(const __grid_constant__ CUtensorMap map_a, const _
 
     const int warp = __shfl_sync(0xffffffffu, (int)threadIdx.x >> 5, 0), lane = threadIdx.x & 31;   // warp-uniform role index
     if (threadIdx.x == 0) {
-        c_prefetch_map(&map_a);
-        c_prefetch_map(&map_w);
-        for (int s = 0; s < FP_STAGES; ++s) { c_mbar_init(&full[s], 1); c_mbar_init(&empty[s], 4); }
-        for (int b = 0; b < 2; ++b) { c_mbar_init(&tfull[b], 128); c_mbar_init(&tempty[b], FP_EPI_WARPS * 32); }
-        c_mbar_init(wfull, 1);
+        tfy_prefetch_tensormap(&map_a);
+        tfy_prefetch_tensormap(&map_w);
+        for (int s = 0; s < FP_STAGES; ++s) { tfy_mbar_init(&full[s], 1); tfy_mbar_init(&empty[s], 4); }
+        for (int b = 0; b < 2; ++b) { tfy_mbar_init(&tfull[b], 128); tfy_mbar_init(&tempty[b], FP_EPI_WARPS * 32); }
+        tfy_mbar_init(wfull, 1);
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
     __syncthreads();
@@ -223,15 +162,15 @@ tfy_conv3x3_fprop_pool_kernel(const __grid_constant__ CUtensorMap map_a, const _
 
     if (warp == FP_EPI_WARPS + 4) {
         // ---------------- TMA producer
-        if (c_elect_one()) {
-            c_mbar_expect_tx(wfull, W_BYTES);
-            c_tma_3d(&map_w, wfull, w_tile, 0, 0, 0);
+        if (tfy_elect_one()) {
+            tfy_mbar_expect_tx(wfull, W_BYTES);
+            tfy_tma_load_3d(&map_w, wfull, w_tile, 0, 0, 0);
             CPatchIter it(tiles_x, tiles_y);
             for (int i = 0; i < my_patches; ++i, it.next()) {
                 const int s = i % FP_STAGES;
-                if (i >= FP_STAGES) c_mbar_wait(&empty[s], ((i / FP_STAGES) - 1) & 1);
-                c_mbar_expect_tx(&full[s], A_HALO_B);
-                c_tma_4d(&map_a, &full[s], stages + (size_t)s * A_HALO_PAD, 0, it.tx * 8, it.bz * 2, it.ty * 8);
+                if (i >= FP_STAGES) tfy_mbar_wait(&empty[s], ((i / FP_STAGES) - 1) & 1);
+                tfy_mbar_expect_tx(&full[s], A_HALO_B);
+                tfy_tma_load_4d(&map_a, &full[s], stages + (size_t)s * A_HALO_PAD, 0, it.tx * 8, it.bz * 2, it.ty * 8);
                 if (i == 0) C_MARK(2);
             }
         }
@@ -240,7 +179,7 @@ tfy_conv3x3_fprop_pool_kernel(const __grid_constant__ CUtensorMap map_a, const _
         // two chains, each its own commit group; half 0's accumulators are stored while the tensor core runs half 1.
         // Each chain is fully unrolled and keeps the (tap, k-step) order, so no wgmma waits on another one's
         // registers and the result is the same bit for bit as one interleaved chain.
-        const uint32_t w0 = c_smem_u32(w_tile);
+        const uint32_t w0 = tfy_smem_u32(w_tile);
         float acc[2][COUT / 2];
         auto issue = [&](float (&d)[COUT / 2], uint32_t a0) {
             tfy_wg_fence();
@@ -250,30 +189,31 @@ tfy_conv3x3_fprop_pool_kernel(const __grid_constant__ CUtensorMap map_a, const _
 #pragma unroll
                 for (int ks = 0; ks < CIN / 16; ++ks) {
                     // B rows = output channels (64 B apart), 8-row groups 512 B apart
-                    const uint64_t bdesc = c_desc(w0 + t * W_TAP_B + ks * 32, 8 * A_PIX_B, SW64);
+                    const uint64_t bdesc = tfy_wg_desc(w0 + t * W_TAP_B + ks * 32, 16, 8 * A_PIX_B, SW64);
                     // A rows = pixels: 8 consecutive w (64 B apart), next group = next (h, n) row of the halo
-                    const uint64_t adesc = c_desc(a0 + kh * 2 * A_ROW_B + kw * A_PIX_B + ks * 32, A_ROW_B, SW64);
+                    const uint64_t adesc =
+                        tfy_wg_desc(a0 + kh * 2 * A_ROW_B + kw * A_PIX_B + ks * 32, 16, A_ROW_B, SW64);
                     tfy_wgmma_m64n64<0, 0>(d, adesc, bdesc, (t > 0 || ks > 0) ? 1u : 0u);
                 }
             }
             tfy_wg_commit();
         };
-        c_mbar_wait(wfull, 0);
+        tfy_mbar_wait(wfull, 0);
         for (int i = 0; i < my_patches; ++i) {
             const int s = i % FP_STAGES, b = i & 1;
             float* tile = acc_s + b * 128 * FP_ACC_LD;
-            c_mbar_wait(&full[s], (i / FP_STAGES) & 1);
+            tfy_mbar_wait(&full[s], (i / FP_STAGES) & 1);
             if (i == 0 && threadIdx.x == FP_EPI_WARPS * 32) C_MARK(4);
-            const uint32_t a0 = c_smem_u32(stages + (size_t)s * A_HALO_PAD);
+            const uint32_t a0 = tfy_smem_u32(stages + (size_t)s * A_HALO_PAD);
             issue(acc[0], a0);
             issue(acc[1], a0 + 4 * 2 * A_ROW_B);
-            if (i >= 2) c_mbar_wait(&tempty[b], ((i >> 1) - 1) & 1);
+            if (i >= 2) tfy_mbar_wait(&tempty[b], ((i >> 1) - 1) & 1);
             tfy_wg_wait<1>();                                     // half 0 is complete
             tfy_wg_store_rows<COUT>(tile, FP_ACC_LD, acc[0], 0);
             tfy_wg_wait<0>();
-            if (lane == 0) c_mbar_arrive(&empty[s]);
+            if (lane == 0) tfy_mbar_arrive(&empty[s]);
             tfy_wg_store_rows<COUT>(tile, FP_ACC_LD, acc[1], 64);
-            c_mbar_arrive(&tfull[b]);
+            tfy_mbar_arrive(&tfull[b]);
             if (threadIdx.x == FP_EPI_WARPS * 32) { if (i == 0) C_MARK(5); if (i == my_patches - 1) C_MARK(11); }
         }
     } else {
@@ -288,7 +228,7 @@ tfy_conv3x3_fprop_pool_kernel(const __grid_constant__ CUtensorMap map_a, const _
         // dropout decisions come 4 to a hash (one byte each): the rate is quantised to 1/256
         const uint32_t thr = drop_rate > 0.f ? (uint32_t)(drop_rate * 256.f + 0.5f) : 0u;
         const float keep_scale = 256.f / (256.f - (float)thr);
-        const uint32_t salt = seed ^ c_hash32(step * 0x9E3779B9U + 0x85ebca6bU);
+        const uint32_t salt = seed ^ tfy_hash32(step * 0x9E3779B9U + 0x85ebca6bU);
         // after the two exchanges below lane (dy, dx) owns columns [8 dx + 4 dy, +4) of each of the warp's slices
         float bv[2][4];
 #pragma unroll
@@ -300,7 +240,7 @@ tfy_conv3x3_fprop_pool_kernel(const __grid_constant__ CUtensorMap map_a, const _
         CPatchIter it(tiles_x, tiles_y);
         for (int i = 0; i < my_patches; ++i, it.next()) {
             const int b = i & 1;
-            c_mbar_wait(&tfull[b], (i >> 1) & 1);
+            tfy_mbar_wait(&tfull[b], (i >> 1) & 1);
             if (threadIdx.x == 0) { if (i == 0) C_MARK(6); if (i == my_patches - 1) C_MARK(8); }
             uint32_t accs[2][16];
 #pragma unroll
@@ -310,7 +250,7 @@ tfy_conv3x3_fprop_pool_kernel(const __grid_constant__ CUtensorMap map_a, const _
                 for (int j = 0; j < 16; j += 4)
                     *reinterpret_cast<uint4*>(accs[k] + j) = *reinterpret_cast<const uint4*>(src + j);
             }
-            c_mbar_arrive(&tempty[b]);                             // the MMA warps may overwrite this buffer now
+            tfy_mbar_arrive(&tempty[b]);                             // the MMA warps may overwrite this buffer now
 #pragma unroll
             for (int k = 0; k < 2; ++k) {
                 const int col = (cq0 + 2 * k) * 16 + dx * 8 + dy * 4;
@@ -337,7 +277,7 @@ tfy_conv3x3_fprop_pool_kernel(const __grid_constant__ CUtensorMap map_a, const _
                     m4[j] = fmaxf(keep, __shfl_xor_sync(0xffffffffu, send, 16));
                 }
                 const uint32_t rnd =
-                    thr ? c_hash32(salt ^ c_hash32((prow >> 2) * 0xC2B2AE35U + 0x27d4eb2fU)) : 0xffffffffu;
+                    thr ? tfy_hash32(salt ^ tfy_hash32((prow >> 2) * 0xC2B2AE35U + 0x27d4eb2fU)) : 0xffffffffu;
                 float o[4];
                 uint32_t codes = 0;
 #pragma unroll
@@ -378,7 +318,7 @@ tfy_conv3x3_dgrad_kernel(const __grid_constant__ CUtensorMap map_dz, const __gri
                          const uint8_t* __restrict__ code, float scale) {
     extern __shared__ uint8_t smem_raw[];
     C_TIMELINE_BEGIN();
-    uint8_t* stages = c_align1024(smem_raw);                      // [3][10 h][2 n][10 w][128 B], 128B swizzle
+    uint8_t* stages = tfy_align1024(smem_raw);                      // [3][10 h][2 n][10 w][128 B], 128B swizzle
     uint8_t* w_tile = stages + (size_t)DG_STAGES * Z_HALO_B;      // [9][64 o][64 B], 64B swizzle
     float* acc_s = reinterpret_cast<float*>(w_tile + W_BYTES);    // [2][128][DG_ACC_LD]
     uint64_t* full = reinterpret_cast<uint64_t*>(acc_s + 2 * 128 * DG_ACC_LD);
@@ -389,11 +329,11 @@ tfy_conv3x3_dgrad_kernel(const __grid_constant__ CUtensorMap map_dz, const __gri
 
     const int warp = __shfl_sync(0xffffffffu, (int)threadIdx.x >> 5, 0), lane = threadIdx.x & 31;   // warp-uniform role index
     if (threadIdx.x == 0) {
-        if (!UNPOOL) c_prefetch_map(&map_dz);
-        c_prefetch_map(&map_w);
-        for (int s = 0; s < DG_STAGES; ++s) { c_mbar_init(&full[s], UNPOOL ? 128 : 1); c_mbar_init(&empty[s], 4); }
-        for (int b = 0; b < 2; ++b) { c_mbar_init(&tfull[b], 128); c_mbar_init(&tempty[b], DG_EPI_WARPS * 32); }
-        c_mbar_init(wfull, 1);
+        if (!UNPOOL) tfy_prefetch_tensormap(&map_dz);
+        tfy_prefetch_tensormap(&map_w);
+        for (int s = 0; s < DG_STAGES; ++s) { tfy_mbar_init(&full[s], UNPOOL ? 128 : 1); tfy_mbar_init(&empty[s], 4); }
+        for (int b = 0; b < 2; ++b) { tfy_mbar_init(&tfull[b], 128); tfy_mbar_init(&tempty[b], DG_EPI_WARPS * 32); }
+        tfy_mbar_init(wfull, 1);
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
     __syncthreads();
@@ -402,29 +342,30 @@ tfy_conv3x3_dgrad_kernel(const __grid_constant__ CUtensorMap map_dz, const __gri
     const int my_patches = ((int)blockIdx.x < n_patches) ? (n_patches - 1 - (int)blockIdx.x) / (int)gridDim.x + 1 : 0;
 
     if (warp == DG_EPI_WARPS + 4) {
-        if (c_elect_one()) {
-            c_mbar_expect_tx(wfull, W_BYTES);
-            c_tma_3d(&map_w, wfull, w_tile, 0, 0, 0);
+        if (tfy_elect_one()) {
+            tfy_mbar_expect_tx(wfull, W_BYTES);
+            tfy_tma_load_3d(&map_w, wfull, w_tile, 0, 0, 0);
             CPatchIter it(tiles_x, tiles_y);
             for (int i = 0; !UNPOOL && i < my_patches; ++i, it.next()) {
                 const int s = i % DG_STAGES;
-                if (i >= DG_STAGES) c_mbar_wait(&empty[s], ((i / DG_STAGES) - 1) & 1);
-                c_mbar_expect_tx(&full[s], Z_HALO_B);
+                if (i >= DG_STAGES) tfy_mbar_wait(&empty[s], ((i / DG_STAGES) - 1) & 1);
+                tfy_mbar_expect_tx(&full[s], Z_HALO_B);
                 // halo origin (y0-2, x0-2) of the dz image: pixels outside it are zero-filled by TMA
-                c_tma_4d(&map_dz, &full[s], stages + (size_t)s * Z_HALO_B, 0, it.tx * 8 - 2, it.bz * 2, it.ty * 8 - 2);
+                tfy_tma_load_4d(&map_dz, &full[s], stages + (size_t)s * Z_HALO_B, 0, it.tx * 8 - 2, it.bz * 2,
+                                it.ty * 8 - 2);
                 if (i == 0) C_MARK(2);
             }
         }
     } else if (warp >= DG_EPI_WARPS && warp < DG_EPI_WARPS + 4) {
         // ---------------- MMA warpgroup: both 64-pixel halves of the patch (4 h rows of the halo apart)
-        const uint32_t w0 = c_smem_u32(w_tile);
-        c_mbar_wait(wfull, 0);
+        const uint32_t w0 = tfy_smem_u32(w_tile);
+        tfy_mbar_wait(wfull, 0);
         for (int i = 0; i < my_patches; ++i) {
             const int s = i % DG_STAGES, b = i & 1;
-            c_mbar_wait(&full[s], (i / DG_STAGES) & 1);
-            if (UNPOOL) asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+            tfy_mbar_wait(&full[s], (i / DG_STAGES) & 1);
+            if (UNPOOL) tfy_fence_proxy_async();
             if (i == 0 && threadIdx.x == DG_EPI_WARPS * 32) C_MARK(4);
-            const uint32_t a0 = c_smem_u32(stages + (size_t)s * Z_HALO_B);
+            const uint32_t a0 = tfy_smem_u32(stages + (size_t)s * Z_HALO_B);
             float acc[2][CIN / 2];
             tfy_wg_fence();
 #pragma unroll 1
@@ -433,23 +374,23 @@ tfy_conv3x3_dgrad_kernel(const __grid_constant__ CUtensorMap map_dz, const __gri
 #pragma unroll
                 for (int ks = 0; ks < COUT / 16; ++ks) {
                     // W tap [o][32 c]: K = o (rows of 64 B, 8-row groups 512 B apart), N = c inside the row (MN-major)
-                    const uint64_t bdesc = c_desc(w0 + t * W_TAP_B + ks * 16 * A_PIX_B, 8 * A_PIX_B, SW64);
+                    const uint64_t bdesc = tfy_wg_desc(w0 + t * W_TAP_B + ks * 16 * A_PIX_B, 16, 8 * A_PIX_B, SW64);
 #pragma unroll
                     for (int h = 0; h < 2; ++h) {
                         // dz[y-kh, x-kw] sits (2-kh, 2-kw) into the halo patch; rows = pixels of 128 B
-                        const uint64_t adesc = c_desc(a0 + (2 - kh + 4 * h) * 2 * Z_ROW_B + (2 - kw) * Z_PIX_B + ks * 32,
-                                                      Z_ROW_B, SW128);
+                        const uint64_t adesc = tfy_wg_desc(
+                            a0 + (2 - kh + 4 * h) * 2 * Z_ROW_B + (2 - kw) * Z_PIX_B + ks * 32, 16, Z_ROW_B, SW128);
                         tfy_wgmma_m64n32<0, 1>(acc[h], adesc, bdesc, (t > 0 || ks > 0) ? 1u : 0u);
                     }
                 }
             }
             tfy_wg_commit();
             tfy_wg_wait<0>();
-            if (lane == 0) c_mbar_arrive(&empty[s]);
-            if (i >= 2) c_mbar_wait(&tempty[b], ((i >> 1) - 1) & 1);
+            if (lane == 0) tfy_mbar_arrive(&empty[s]);
+            if (i >= 2) tfy_mbar_wait(&tempty[b], ((i >> 1) - 1) & 1);
             tfy_wg_store_rows<CIN>(acc_s + b * 128 * DG_ACC_LD, DG_ACC_LD, acc[0], 0);
             tfy_wg_store_rows<CIN>(acc_s + b * 128 * DG_ACC_LD, DG_ACC_LD, acc[1], 64);
-            c_mbar_arrive(&tfull[b]);
+            tfy_mbar_arrive(&tfull[b]);
             if (threadIdx.x == DG_EPI_WARPS * 32) { if (i == 0) C_MARK(5); if (i == my_patches - 1) C_MARK(11); }
         }
     } else if (warp > DG_EPI_WARPS + 4) {
@@ -460,7 +401,7 @@ tfy_conv3x3_dgrad_kernel(const __grid_constant__ CUtensorMap map_dz, const __gri
             CPatchIter it(tiles_x, tiles_y);
             for (int i = 0; i < my_patches; ++i, it.next()) {
                 const int s = i % DG_STAGES;
-                if (i >= DG_STAGES) c_mbar_wait(&empty[s], ((i / DG_STAGES) - 1) & 1);
+                if (i >= DG_STAGES) tfy_mbar_wait(&empty[s], ((i / DG_STAGES) - 1) & 1);
                 uint8_t* tile = stages + (size_t)s * Z_HALO_B;
                 // 400 tasks per patch, 4 slots per thread: all loads are issued before the first is consumed
                 // (one L2 round trip per patch instead of four)
@@ -483,8 +424,8 @@ tfy_conv3x3_dgrad_kernel(const __grid_constant__ CUtensorMap map_dz, const __gri
                     float gated[8];
                     if (t < 400) c_unpool_emit(tile, in[u], scale, t & 7, row0[u], 2 * HALO, gated);
                 }
-                asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-                c_mbar_arrive(&full[s]);
+                tfy_fence_proxy_async();
+                tfy_mbar_arrive(&full[s]);
             }
         }
     } else {
@@ -502,13 +443,13 @@ tfy_conv3x3_dgrad_kernel(const __grid_constant__ CUtensorMap map_dz, const __gri
                 g0 = tfy_ld16(gate + off); g1 = tfy_ld16(gate + off + 8);
                 g2 = tfy_ld16(gate + off + 16); g3 = tfy_ld16(gate + off + 24);
             }
-            c_mbar_wait(&tfull[b], (i >> 1) & 1);
+            tfy_mbar_wait(&tfull[b], (i >> 1) & 1);
             if (threadIdx.x == 0) { if (i == 0) C_MARK(6); if (i == my_patches - 1) C_MARK(8); }
             uint32_t acc[2][16];
             const float* src = acc_s + (size_t)(b * 128 + r) * DG_ACC_LD;
 #pragma unroll
             for (int j = 0; j < 32; j += 4) *reinterpret_cast<uint4*>(&acc[j >> 4][j & 15]) = *reinterpret_cast<const uint4*>(src + j);
-            c_mbar_arrive(&tempty[b]);
+            tfy_mbar_arrive(&tempty[b]);
             if (valid) {
                 float v[32];
 #pragma unroll
@@ -558,12 +499,12 @@ tfy_conv3x3_wgrad_kernel(const __grid_constant__ CUtensorMap map_dz, const __gri
     if ((int)blockIdx.x >= n_cmp) {
         extern __shared__ uint8_t smem_role[];
         tfy_pdl_sync();
-        tfy_overlap_role<WG_THREADS>(ov, (int)blockIdx.x - n_cmp, c_align1024(smem_role));
+        tfy_overlap_role<WG_THREADS>(ov, (int)blockIdx.x - n_cmp, tfy_align1024(smem_role));
         return;
     }
     extern __shared__ uint8_t smem_raw[];
     C_TIMELINE_BEGIN();
-    uint8_t* stages = c_align1024(smem_raw);        // [4] { dz [8 h][2 n][8 w][128 B] sw128 ; a [10 h][2 n][10 w][64 B] sw64 }
+    uint8_t* stages = tfy_align1024(smem_raw);    // [4] { dz [8 h][2 n][8 w][128 B] sw128 ; a [10 h][2 n][10 w][64 B] sw64 }
     uint64_t* full = reinterpret_cast<uint64_t*>(stages + (size_t)WG_STAGES * WG_STAGE_B);
     uint64_t* empty = full + WG_STAGES;
     float* s_db = reinterpret_cast<float*>(empty + WG_STAGES);      // [16 warps][64] bias-gradient partials (UNPOOL)
@@ -571,9 +512,9 @@ tfy_conv3x3_wgrad_kernel(const __grid_constant__ CUtensorMap map_dz, const __gri
 
     const int warp = __shfl_sync(0xffffffffu, (int)threadIdx.x >> 5, 0), lane = threadIdx.x & 31;   // warp-uniform role index
     if (threadIdx.x == 0) {
-        if (!UNPOOL) c_prefetch_map(&map_dz);
-        c_prefetch_map(&map_a);
-        for (int s = 0; s < WG_STAGES; ++s) { c_mbar_init(&full[s], UNPOOL ? 257 : 1); c_mbar_init(&empty[s], 4); }
+        if (!UNPOOL) tfy_prefetch_tensormap(&map_dz);
+        tfy_prefetch_tensormap(&map_a);
+        for (int s = 0; s < WG_STAGES; ++s) { tfy_mbar_init(&full[s], UNPOOL ? 257 : 1); tfy_mbar_init(&empty[s], 4); }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
     __syncthreads();
@@ -583,15 +524,15 @@ tfy_conv3x3_wgrad_kernel(const __grid_constant__ CUtensorMap map_dz, const __gri
     const int my_patches = ((int)blockIdx.x < n_patches) ? (n_patches - 1 - (int)blockIdx.x) / n_cmp + 1 : 0;
 
     if (warp == WG_WORK_WARPS + 4) {
-        if (c_elect_one()) {
+        if (tfy_elect_one()) {
             CPatchIter it(tiles_x, tiles_y, n_cmp);
             for (int i = 0; i < my_patches; ++i, it.next()) {
                 const int s = i % WG_STAGES;
-                if (i >= WG_STAGES) c_mbar_wait(&empty[s], ((i / WG_STAGES) - 1) & 1);
+                if (i >= WG_STAGES) tfy_mbar_wait(&empty[s], ((i / WG_STAGES) - 1) & 1);
                 uint8_t* st = stages + (size_t)s * WG_STAGE_B;
-                c_mbar_expect_tx(&full[s], (UNPOOL ? 0 : Z_PATCH_B) + A_HALO_B);
-                if (!UNPOOL) c_tma_4d(&map_dz, &full[s], st, 0, it.tx * 8, it.bz * 2, it.ty * 8);
-                c_tma_4d(&map_a, &full[s], st + Z_PATCH_B, 0, it.tx * 8, it.bz * 2, it.ty * 8);
+                tfy_mbar_expect_tx(&full[s], (UNPOOL ? 0 : Z_PATCH_B) + A_HALO_B);
+                if (!UNPOOL) tfy_tma_load_4d(&map_dz, &full[s], st, 0, it.tx * 8, it.bz * 2, it.ty * 8);
+                tfy_tma_load_4d(&map_a, &full[s], st + Z_PATCH_B, 0, it.tx * 8, it.bz * 2, it.ty * 8);
                 if (i == 0) C_MARK(2);
             }
         }
@@ -604,10 +545,10 @@ tfy_conv3x3_wgrad_kernel(const __grid_constant__ CUtensorMap map_dz, const __gri
         const int n_groups = (my_patches + WG_STAGES - 1) / WG_STAGES;
         for (int g = 0; g < n_groups; ++g) {
             const int cnt = min(WG_STAGES, my_patches - g * WG_STAGES);
-            for (int q = 0; q < cnt; ++q) c_mbar_wait(&full[q], g & 1);
-            if (UNPOOL) asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+            for (int q = 0; q < cnt; ++q) tfy_mbar_wait(&full[q], g & 1);
+            if (UNPOOL) tfy_fence_proxy_async();
             if (g == 0 && tid == 0) C_MARK(4);
-            const uint32_t st0 = c_smem_u32(stages);
+            const uint32_t st0 = tfy_smem_u32(stages);
 #pragma unroll 1
             for (int t = 0; t < TAPS; ++t) {
                 const int kh = t / 3, kw = t - kh * 3;
@@ -619,9 +560,10 @@ tfy_conv3x3_wgrad_kernel(const __grid_constant__ CUtensorMap map_dz, const __gri
 #pragma unroll
                     for (int j = 0; j < 8; ++j) {      // 16 pixels (one h row of both images) per MMA
                         // A = dz^T: M = 64 o inside the 128 B pixel row; K = pixels, 8-pixel groups 1024 B apart
-                        const uint64_t adesc = c_desc(dz0 + j * 2 * 8 * Z_PIX_B, 8 * Z_PIX_B, SW128);
+                        const uint64_t adesc = tfy_wg_desc(dz0 + j * 2 * 8 * Z_PIX_B, 16, 8 * Z_PIX_B, SW128);
                         // B = a (tap shifted): N = 32 c inside the 64 B pixel row; K = pixels, groups = (h, n) rows
-                        const uint64_t bdesc = c_desc(a0 + (j + kh) * 2 * A_ROW_B + kw * A_PIX_B, A_ROW_B, SW64);
+                        const uint64_t bdesc =
+                            tfy_wg_desc(a0 + (j + kh) * 2 * A_ROW_B + kw * A_PIX_B, 16, A_ROW_B, SW64);
                         tfy_wgmma_m64n32<1, 1>(d, adesc, bdesc, (q > 0 || j > 0) ? 1u : 0u);
                     }
                 }
@@ -631,7 +573,7 @@ tfy_conv3x3_wgrad_kernel(const __grid_constant__ CUtensorMap map_dz, const __gri
                 for (int i = 0; i < 16; ++i) mine[(t * 16 + i) * 128] += d[i];
             }
             if (lane == 0)
-                for (int q = 0; q < cnt; ++q) c_mbar_arrive(&empty[q]);     // stages reusable
+                for (int q = 0; q < cnt; ++q) tfy_mbar_arrive(&empty[q]);     // stages reusable
         }
         if (tid == 0) C_MARK(5);
         // partial tile rows o = (o, tap) rows of 128 B: value i of this thread is o = 16 w + lane / 4 + 8 ((i / 2) % 2),
@@ -672,21 +614,21 @@ tfy_conv3x3_wgrad_kernel(const __grid_constant__ CUtensorMap map_dz, const __gri
                 float gated[8];
                 {
                     const int s = i % WG_STAGES;
-                    if (i >= WG_STAGES) c_mbar_wait(&empty[s], ((i / WG_STAGES) - 1) & 1);
+                    if (i >= WG_STAGES) tfy_mbar_wait(&empty[s], ((i / WG_STAGES) - 1) & 1);
                     c_unpool_emit(stages + (size_t)s * WG_STAGE_B, in0, scale, g, row0, 16, gated);
 #pragma unroll
                     for (int k = 0; k < 8; ++k) colacc[k] += gated[k];
-                    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-                    c_mbar_arrive(&full[s]);
+                    tfy_fence_proxy_async();
+                    tfy_mbar_arrive(&full[s]);
                 }
                 if (two) {
                     const int i2 = i + 2, s = i2 % WG_STAGES;
-                    if (i2 >= WG_STAGES) c_mbar_wait(&empty[s], ((i2 / WG_STAGES) - 1) & 1);
+                    if (i2 >= WG_STAGES) tfy_mbar_wait(&empty[s], ((i2 / WG_STAGES) - 1) & 1);
                     c_unpool_emit(stages + (size_t)s * WG_STAGE_B, in1, scale, g, row0, 16, gated);
 #pragma unroll
                     for (int k = 0; k < 8; ++k) colacc[k] += gated[k];
-                    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-                    c_mbar_arrive(&full[s]);
+                    tfy_fence_proxy_async();
+                    tfy_mbar_arrive(&full[s]);
                 }
                 it.next(); it.next(); it.next(); it.next();
             }
@@ -819,7 +761,7 @@ tfy_conv3x3_c1_wgrad_tc_kernel(const __grid_constant__ CUtensorMap map_dz, const
                                int n_pix, int n_chunks) {
     extern __shared__ uint8_t smem_raw[];
     C_TIMELINE_BEGIN();
-    uint8_t* stages = c_align1024(smem_raw);        // [4] { X~ [128 pix][128 B] sw128 ; dz [128 pix][64 B] sw64 }
+    uint8_t* stages = tfy_align1024(smem_raw);        // [4] { X~ [128 pix][128 B] sw128 ; dz [128 pix][64 B] sw64 }
     uint64_t* full_a = reinterpret_cast<uint64_t*>(stages + (size_t)C1_STAGES * C1_STAGE_B);
     uint64_t* full_b = full_a + C1_STAGES;
     uint64_t* empty = full_b + C1_STAGES;
@@ -827,11 +769,11 @@ tfy_conv3x3_c1_wgrad_tc_kernel(const __grid_constant__ CUtensorMap map_dz, const
 
     const int warp = __shfl_sync(0xffffffffu, (int)threadIdx.x >> 5, 0), lane = threadIdx.x & 31;   // warp-uniform role index
     if (threadIdx.x == 0) {
-        c_prefetch_map(&map_dz);
+        tfy_prefetch_tensormap(&map_dz);
         for (int s = 0; s < C1_STAGES; ++s) {
-            c_mbar_init(&full_a[s], 128);
-            c_mbar_init(&full_b[s], 1);
-            c_mbar_init(&empty[s], 4);
+            tfy_mbar_init(&full_a[s], 128);
+            tfy_mbar_init(&full_b[s], 1);
+            tfy_mbar_init(&empty[s], 4);
         }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
@@ -840,7 +782,7 @@ tfy_conv3x3_c1_wgrad_tc_kernel(const __grid_constant__ CUtensorMap map_dz, const
         const int s = i / (C1_A_B / 16), r = i - s * (C1_A_B / 16);
         *reinterpret_cast<uint4*>(stages + (size_t)s * C1_STAGE_B + (size_t)r * 16) = make_uint4(0, 0, 0, 0);
     }
-    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+    tfy_fence_proxy_async();
     __syncthreads();
     tfy_pdl_sync();                      // upstream grids complete; our dependents may start launching
     if (threadIdx.x == 0) C_MARK(1);
@@ -848,17 +790,13 @@ tfy_conv3x3_c1_wgrad_tc_kernel(const __grid_constant__ CUtensorMap map_dz, const
     const int OH = H - 2, OW = W - 2;
 
     if (warp == 8) {
-        if (c_elect_one()) {
+        if (tfy_elect_one()) {
             for (int i = 0; i < my_chunks; ++i) {
                 const int s = i % C1_STAGES;
-                if (i >= C1_STAGES) c_mbar_wait(&empty[s], ((i / C1_STAGES) - 1) & 1);
+                if (i >= C1_STAGES) tfy_mbar_wait(&empty[s], ((i / C1_STAGES) - 1) & 1);
                 const int chunk = (int)blockIdx.x + i * (int)gridDim.x;
-                c_mbar_expect_tx(&full_b[s], C1_B_B);
-                asm volatile(
-                    "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
-                    ::"r"(c_smem_u32(stages + (size_t)s * C1_STAGE_B + C1_A_B)),
-                    "l"(reinterpret_cast<uint64_t>(&map_dz)), "r"(c_smem_u32(&full_b[s])), "r"(0), "r"(chunk * C1_PIX)
-                    : "memory");
+                tfy_mbar_expect_tx(&full_b[s], C1_B_B);
+                tfy_tma_load_2d(&map_dz, &full_b[s], stages + (size_t)s * C1_STAGE_B + C1_A_B, 0, chunk * C1_PIX);
             }
         }
     } else if (warp >= 4) {
@@ -866,21 +804,21 @@ tfy_conv3x3_c1_wgrad_tc_kernel(const __grid_constant__ CUtensorMap map_dz, const
         tfy_wg_zero<C1_O>(d);
         for (int i = 0; i < my_chunks; ++i) {
             const int s = i % C1_STAGES;
-            c_mbar_wait(&full_a[s], (i / C1_STAGES) & 1);
-            c_mbar_wait(&full_b[s], (i / C1_STAGES) & 1);
+            tfy_mbar_wait(&full_a[s], (i / C1_STAGES) & 1);
+            tfy_mbar_wait(&full_b[s], (i / C1_STAGES) & 1);
             if (i == 0 && threadIdx.x == 128) C_MARK(4);
-            const uint32_t a0 = c_smem_u32(stages + (size_t)s * C1_STAGE_B), b0 = a0 + C1_A_B;
+            const uint32_t a0 = tfy_smem_u32(stages + (size_t)s * C1_STAGE_B), b0 = a0 + C1_A_B;
             tfy_wg_fence();
 #pragma unroll
             for (int j = 0; j < C1_PIX / 16; ++j) {
                 // A = X~^T: M = 64 n inside the 128 B pixel row; B = dz: N = 32 o inside the 64 B pixel row
-                const uint64_t adesc = c_desc(a0 + j * 16 * 128, 8 * 128, SW128);
-                const uint64_t bdesc = c_desc(b0 + j * 16 * 64, 8 * 64, SW64);
+                const uint64_t adesc = tfy_wg_desc(a0 + j * 16 * 128, 16, 8 * 128, SW128);
+                const uint64_t bdesc = tfy_wg_desc(b0 + j * 16 * 64, 16, 8 * 64, SW64);
                 tfy_wgmma_m64n32<1, 1>(d, adesc, bdesc, 1u);
             }
             tfy_wg_commit();
             tfy_wg_wait<0>();
-            if (lane == 0) c_mbar_arrive(&empty[s]);
+            if (lane == 0) tfy_mbar_arrive(&empty[s]);
         }
         if (threadIdx.x == 128) C_MARK(5);
         if (warp == 4) {
@@ -923,12 +861,12 @@ tfy_conv3x3_c1_wgrad_tc_kernel(const __grid_constant__ CUtensorMap map_dz, const
             float c1[8] = {v[8], ok ? 1.f : 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
             const uint4 q0 = TfyPack<__nv_bfloat16>::pack(v), q1 = TfyPack<__nv_bfloat16>::pack(c1);
             if (i + 1 < my_chunks) ok = gather((int)blockIdx.x + (i + 1) * (int)gridDim.x, v);
-            if (i >= C1_STAGES) c_mbar_wait(&empty[s], ((i / C1_STAGES) - 1) & 1);
+            if (i >= C1_STAGES) tfy_mbar_wait(&empty[s], ((i / C1_STAGES) - 1) & 1);
             uint8_t* rowp = stages + (size_t)s * C1_STAGE_B + (size_t)r * 128;
             *reinterpret_cast<uint4*>(rowp + ((0u ^ sw) << 4)) = q0;    // 128B swizzle: chunk ^= row & 7
             *reinterpret_cast<uint4*>(rowp + ((1u ^ sw) << 4)) = q1;
-            asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-            c_mbar_arrive(&full_a[s]);
+            tfy_fence_proxy_async();
+            tfy_mbar_arrive(&full_a[s]);
             if (threadIdx.x == 0) { if (i == 0) C_MARK(2); if (i == my_chunks - 1) C_MARK(3); }
         }
     }
@@ -990,10 +928,6 @@ constexpr int F1_W_B = 2 * C1_O * 16;                                     // 1 K
 constexpr int F1_THREADS = 8 * 32;
 constexpr size_t F1_SMEM = (size_t)F1_STAGES * F1_A_B + F1_W_B + 128 + 256;
 
-__device__ __forceinline__ uint64_t c_desc_nosw(uint32_t smem_addr, uint32_t lbo, uint32_t sbo) {
-    return tfy_wg_desc(smem_addr, lbo, sbo, TFY_WG_NOSWIZZLE);
-}
-
 template <typename XT>
 __global__ void __launch_bounds__(F1_THREADS, 2)
 tfy_conv3x3_c1_fwd_tc_kernel(const XT* __restrict__ x, const __nv_bfloat16* __restrict__ w,
@@ -1007,7 +941,7 @@ tfy_conv3x3_c1_fwd_tc_kernel(const XT* __restrict__ x, const __nv_bfloat16* __re
 
     const int warp = __shfl_sync(0xffffffffu, (int)threadIdx.x >> 5, 0), lane = threadIdx.x & 31;   // warp-uniform role index
     if (threadIdx.x == 0) {
-        for (int s = 0; s < F1_STAGES; ++s) { c_mbar_init(&full[s], 128); c_mbar_init(&empty[s], 4); }
+        for (int s = 0; s < F1_STAGES; ++s) { tfy_mbar_init(&full[s], 128); tfy_mbar_init(&empty[s], 4); }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
     tfy_pdl_sync();                      // (the weights below are produced by the previous step's optimizer kernel)
@@ -1022,28 +956,28 @@ tfy_conv3x3_c1_fwd_tc_kernel(const XT* __restrict__ x, const __nv_bfloat16* __re
         *reinterpret_cast<uint4*>(w_tile + o * 16) = TfyPack<__nv_bfloat16>::pack(k0);
         *reinterpret_cast<uint4*>(w_tile + C1_O * 16 + o * 16) = TfyPack<__nv_bfloat16>::pack(k1);
     }
-    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+    tfy_fence_proxy_async();
     __syncthreads();
     const int my_chunks = ((int)blockIdx.x < n_chunks) ? (n_chunks - 1 - (int)blockIdx.x) / (int)gridDim.x + 1 : 0;
     const int OH = H - 2, OW = W - 2;
 
     if (warp >= 4) {
-        const uint64_t bdesc = c_desc_nosw(c_smem_u32(w_tile), C1_O * 16, 128);
+        const uint64_t bdesc = tfy_wg_desc(tfy_smem_u32(w_tile), C1_O * 16, 128, TFY_WG_NOSWIZZLE);
         const int w = warp & 3;
         for (int i = 0; i < my_chunks; ++i) {
             const int s = i % F1_STAGES;
             const int chunk = (int)blockIdx.x + i * (int)gridDim.x;
-            c_mbar_wait(&full[s], (i / F1_STAGES) & 1);
-            asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+            tfy_mbar_wait(&full[s], (i / F1_STAGES) & 1);
+            tfy_fence_proxy_async();
             float acc[2][C1_O / 2];
             tfy_wg_fence();
 #pragma unroll
             for (int h = 0; h < 2; ++h)       // pixels [64 h, 64 h + 64): 8 core-matrix rows of 128 B further
-                tfy_wgmma_m64n32<0, 0>(acc[h], c_desc_nosw(c_smem_u32(stages + (size_t)s * F1_A_B + h * 64 * 16),
-                                                           F1_PIX * 16, 128), bdesc, 0u);
+                tfy_wgmma_m64n32<0, 0>(acc[h], tfy_wg_desc(tfy_smem_u32(stages + (size_t)s * F1_A_B + h * 64 * 16),
+                                                           F1_PIX * 16, 128, TFY_WG_NOSWIZZLE), bdesc, 0u);
             tfy_wg_commit();
             tfy_wg_wait<0>();
-            if (lane == 0) c_mbar_arrive(&empty[s]);
+            if (lane == 0) tfy_mbar_arrive(&empty[s]);
             // value i of this thread: pixel row 64 h + 16 w + lane / 4 + 8 ((i / 2) % 2), channel 8 (i / 4) + 2 (lane % 4)
 #pragma unroll
             for (int h = 0; h < 2; ++h) {
@@ -1084,32 +1018,21 @@ tfy_conv3x3_c1_fwd_tc_kernel(const XT* __restrict__ x, const __nv_bfloat16* __re
             float c1[8] = {v[8], ok ? 1.f : 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
             const uint4 q0 = TfyPack<__nv_bfloat16>::pack(v), q1 = TfyPack<__nv_bfloat16>::pack(c1);
             if (i + 1 < my_chunks) ok = gather((int)blockIdx.x + (i + 1) * (int)gridDim.x, v);
-            if (i >= F1_STAGES) c_mbar_wait(&empty[s], ((i / F1_STAGES) - 1) & 1);
+            if (i >= F1_STAGES) tfy_mbar_wait(&empty[s], ((i / F1_STAGES) - 1) & 1);
             uint8_t* st = stages + (size_t)s * F1_A_B;
             *reinterpret_cast<uint4*>(st + r * 16) = q0;
             *reinterpret_cast<uint4*>(st + F1_PIX * 16 + r * 16) = q1;
-            asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-            c_mbar_arrive(&full[s]);
+            tfy_fence_proxy_async();
+            tfy_mbar_arrive(&full[s]);
         }
     }
 }
 
 namespace {
-using CEncodeFn = CUresult (*)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
-                               const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
-                               CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-CEncodeFn c_encode = nullptr;
 bool c_attr_set = false;
 int c_sms = 0;
 bool c_init() {
-    if (!c_encode) {
-        void* fn = nullptr;
-        cudaDriverEntryPointQueryResult st;
-        if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &fn, cudaEnableDefault, &st) != cudaSuccess ||
-            st != cudaDriverEntryPointSuccess || !fn)
-            return false;
-        c_encode = reinterpret_cast<CEncodeFn>(fn);
-    }
+    if (!tfy_tensor_map_encoder()) return false;
     if (!c_attr_set) {
         if (cudaFuncSetAttribute(tfy_conv3x3_fprop_pool_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                  (int)FP_SMEM) != cudaSuccess ||
@@ -1141,20 +1064,17 @@ bool c_map_nhwc(CUtensorMap* m, const void* p, int B, int H, int W, int C, int b
     cuuint64_t dims[4] = {(cuuint64_t)C, (cuuint64_t)W, (cuuint64_t)B, (cuuint64_t)H};
     cuuint64_t strides[3] = {(cuuint64_t)C * 2, (cuuint64_t)H * W * C * 2, (cuuint64_t)W * C * 2};
     cuuint32_t box[4] = {(cuuint32_t)C, (cuuint32_t)bw, 2, (cuuint32_t)bh};
-    cuuint32_t estr[4] = {1, 1, 1, 1};
-    return c_encode(m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, const_cast<void*>(p), dims, strides, box, estr,
-                    CU_TENSOR_MAP_INTERLEAVE_NONE, C == 64 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B,
-                    CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
+    return tfy_tensor_map_bf16(m, p, 4, dims, strides, box,
+                               C == 64 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B,
+                               CU_TENSOR_MAP_L2_PROMOTION_L2_128B);
 }
 // weights [O][9][C] bf16 seen as {C, O, 9}; one box = everything, stored [tap][o][32 c] with 64-byte rows
 bool c_map_w(CUtensorMap* m, const void* p) {
     cuuint64_t dims[3] = {(cuuint64_t)CIN, (cuuint64_t)COUT, (cuuint64_t)TAPS};
     cuuint64_t strides[2] = {(cuuint64_t)TAPS * CIN * 2, (cuuint64_t)CIN * 2};
     cuuint32_t box[3] = {(cuuint32_t)CIN, (cuuint32_t)COUT, (cuuint32_t)TAPS};
-    cuuint32_t estr[3] = {1, 1, 1};
-    return c_encode(m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 3, const_cast<void*>(p), dims, strides, box, estr,
-                    CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_64B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
-                    CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
+    return tfy_tensor_map_bf16(m, p, 3, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_64B,
+                               CU_TENSOR_MAP_L2_PROMOTION_L2_128B);
 }
 }  // namespace
 
@@ -1311,10 +1231,8 @@ int tfy_conv3x3_c1_wgrad_tc(const void* x, int x_is_f32, const void* dz, float* 
         cuuint64_t dims[2] = {(cuuint64_t)C1_O, (cuuint64_t)n_pix};
         cuuint64_t strides[1] = {(cuuint64_t)C1_O * 2};
         cuuint32_t box[2] = {(cuuint32_t)C1_O, (cuuint32_t)C1_PIX};
-        cuuint32_t estr[2] = {1, 1};
-        if (c_encode(&mz, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(dz), dims, strides, box, estr,
-                     CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_64B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
-                     CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) != CUDA_SUCCESS)
+        if (!tfy_tensor_map_bf16(&mz, dz, 2, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_64B,
+                                 CU_TENSOR_MAP_L2_PROMOTION_L2_128B))
             return -6;
     }
     const int grid = c_grid(n_chunks);

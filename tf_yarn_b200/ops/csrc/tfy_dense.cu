@@ -16,9 +16,8 @@
 // gloo_allred_task.py:54 running TensorFlow's MatMul gradients).
 //
 // warps 0-3: dW wgmma + epilogue   warps 4-7: dx wgmma + epilogue   warp 8: TMA loads
-#include <cuda.h>
-
 #include "tfy_common.cuh"
+#include "tfy_tma.cuh"
 #include "tfy_wgmma.cuh"
 
 namespace {
@@ -33,47 +32,9 @@ constexpr int ACC_LD = DB_N + 4;                  // fp32 row pitch of a staged 
 constexpr int ACC_BYTES = DB_M * ACC_LD * 4;
 constexpr size_t DB_SMEM = 1024 + DH_BYTES + 2 * TILE_BYTES /*x, w*/ + 2 * TILE_BYTES /*staging*/ + 2 * ACC_BYTES + 256;
 
-__device__ __forceinline__ uint32_t d_smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ void d_mbar_init(uint64_t* bar, uint32_t count) {
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(d_smem_u32(bar)), "r"(count) : "memory");
-}
-__device__ __forceinline__ void d_mbar_arrive(uint64_t* bar) {
-    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(d_smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void d_mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
-    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(d_smem_u32(bar)), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void d_mbar_wait(uint64_t* bar, uint32_t parity) {
-    asm volatile(
-        "{\n\t"
-        ".reg .pred P1;\n\t"
-        "DWAIT_LOOP:\n\t"
-        "mbarrier.try_wait.parity.shared::cta.b64 P1, [%0], %1;\n\t"
-        "@P1 bra DDONE;\n\t"
-        "bra DWAIT_LOOP;\n\t"
-        "DDONE:\n\t"
-        "}" ::"r"(d_smem_u32(bar)), "r"(parity) : "memory");
-}
-__device__ __forceinline__ void d_tma_load_2d(const CUtensorMap* map, uint64_t* bar, void* dst, int c0, int c1) {
-    asm volatile(
-        "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
-        ::"r"(d_smem_u32(dst)), "l"(reinterpret_cast<uint64_t>(map)), "r"(d_smem_u32(bar)), "r"(c0), "r"(c1)
-        : "memory");
-}
-__device__ __forceinline__ void d_tma_store_2d(const CUtensorMap* map, const void* src, int c0, int c1) {
-    asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];"
-                 ::"l"(reinterpret_cast<uint64_t>(map)), "r"(d_smem_u32(src)), "r"(c0), "r"(c1)
-                 : "memory");
-}
-__device__ __forceinline__ bool d_elect_one() {
-    uint32_t pred;
-    asm volatile("{\n\t.reg .pred P;\n\telect.sync _|P, 0xffffffff;\n\tselp.b32 %0, 1, 0, P;\n\t}" : "=r"(pred));
-    return pred != 0;
-}
-// 128-byte swizzled operand views, sbo = 8 rows of 128 B.  K-major: rows = M/N index (64 K-elements each).
-// MN-major: rows = K index (64 M/N-elements each); one M64 / N64 operand is exactly one atom, so lbo is unused.
-__device__ __forceinline__ uint64_t d_desc(uint32_t smem_addr) { return tfy_wg_desc(smem_addr, 16, 1024, TFY_WG_SW128); }
-
+// Operands are 128-byte swizzled views (tfy_wg_desc_sw128), sbo = 8 rows of 128 B.  K-major: rows = M/N index (64
+// K-elements each).  MN-major: rows = K index (64 M/N-elements each); one M64 / N64 operand is exactly one atom, so
+// lbo is unused.
 // dW = dh^T . x (A = dh MN-major: M = units, 64-unit halves TILE_BYTES apart; K = batch rows, 16 rows = 2048 B per
 // MMA; B = x / W tile MN-major: N = 64 in-features in one atom)   -- TA = 1
 // dx = dh . W   (A = dh K-major: M = batch rows, 64-row halves 8 KB apart; K = units: 4 x 32 B inside each 64-unit
@@ -82,11 +43,11 @@ template <int TA>
 __device__ __forceinline__ void d_mma_chunk(float (&acc)[2][DB_N / 2], uint32_t dh0, uint32_t t0, bool first) {
 #pragma unroll
     for (int k = 0; k < DB_K / 16; ++k) {
-        const uint64_t bdesc = d_desc(t0 + k * 2048);
+        const uint64_t bdesc = tfy_wg_desc_sw128(t0 + k * 2048);
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
             const uint32_t a = TA ? dh0 + h * TILE_BYTES + k * 2048 : dh0 + (k >> 2) * TILE_BYTES + (k & 3) * 32 + h * 8192;
-            tfy_wgmma_m64n64<TA, 1>(acc[h], d_desc(a), bdesc, (first && k == 0) ? 0u : 1u);
+            tfy_wgmma_m64n64<TA, 1>(acc[h], tfy_wg_desc_sw128(a), bdesc, (first && k == 0) ? 0u : 1u);
         }
     }
 }
@@ -109,10 +70,10 @@ __device__ __forceinline__ void d_epilogue(float (&acc)[2][DB_N / 2], float* acc
         // 128-byte swizzle of the TMA store map: 16-byte chunk index XOR (row mod 8)
         *reinterpret_cast<uint4*>(dst + ((ch ^ (row & 7)) << 4)) = TfyPack<__nv_bfloat16>::pack(v);
     }
-    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");     // generic-proxy writes -> async proxy
+    tfy_fence_proxy_async();     // generic-proxy writes -> async proxy
     asm volatile("bar.sync %0, 128;" ::"r"(bar) : "memory");
-    if (row < 32 && d_elect_one()) {
-        d_tma_store_2d(map, stage, c0, c1);
+    if (row < 32 && tfy_elect_one()) {
+        tfy_tma_store_2d(map, stage, c0, c1);
         asm volatile("cp.async.bulk.commit_group;" ::: "memory");
         asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");  // smem must outlive the read
     }
@@ -125,7 +86,7 @@ tfy_dense_bwd_kernel(const __grid_constant__ CUtensorMap map_dh, const __grid_co
                      const __grid_constant__ CUtensorMap map_w, const __grid_constant__ CUtensorMap map_dw,
                      const __grid_constant__ CUtensorMap map_dx, int want_dx) {
     extern __shared__ uint8_t smem_raw[];
-    uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
+    uint8_t* smem = tfy_align1024(smem_raw);
     uint8_t* s_dh = smem;                            // [2 boxes][128 rows (batch)][128 B (64 units)]  sw128
     uint8_t* s_x = s_dh + DH_BYTES;                  // [128 rows (batch)][128 B (64 in-features)]     sw128
     uint8_t* s_w = s_x + TILE_BYTES;                 // [128 rows (units)][128 B (64 in-features)]     sw128
@@ -136,35 +97,35 @@ tfy_dense_bwd_kernel(const __grid_constant__ CUtensorMap map_dh, const __grid_co
     const int warp = __shfl_sync(0xffffffffu, (int)threadIdx.x >> 5, 0);   // warp-uniform role index
     const int n0 = blockIdx.x * DB_N;
     if (threadIdx.x == 0) {
-        asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&map_dh)) : "memory");
-        asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&map_x)) : "memory");
-        asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&map_w)) : "memory");
-        asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&map_dw)) : "memory");
-        asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&map_dx)) : "memory");
-        d_mbar_init(full, 1);
+        tfy_prefetch_tensormap(&map_dh);
+        tfy_prefetch_tensormap(&map_x);
+        tfy_prefetch_tensormap(&map_w);
+        tfy_prefetch_tensormap(&map_dw);
+        tfy_prefetch_tensormap(&map_dx);
+        tfy_mbar_init(full, 1);
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
     __syncthreads();
     tfy_pdl_sync();
 
     if (warp == 8) {
-        if (d_elect_one()) {
-            d_mbar_expect_tx(full, DH_BYTES + TILE_BYTES + (want_dx ? TILE_BYTES : 0));
-            d_tma_load_2d(&map_dh, full, s_dh, 0, 0);
-            d_tma_load_2d(&map_dh, full, s_dh + TILE_BYTES, 64, 0);
-            d_tma_load_2d(&map_x, full, s_x, n0, 0);
-            if (want_dx) d_tma_load_2d(&map_w, full, s_w, n0, 0);
+        if (tfy_elect_one()) {
+            tfy_mbar_expect_tx(full, DH_BYTES + TILE_BYTES + (want_dx ? TILE_BYTES : 0));
+            tfy_tma_load_2d(&map_dh, full, s_dh, 0, 0);
+            tfy_tma_load_2d(&map_dh, full, s_dh + TILE_BYTES, 64, 0);
+            tfy_tma_load_2d(&map_x, full, s_x, n0, 0);
+            if (want_dx) tfy_tma_load_2d(&map_w, full, s_w, n0, 0);
         }
         return;
     }
     const int which = warp >> 2;                     // 0 -> dW (warps 0-3), 1 -> dx (warps 4-7)
     if (which == 1 && !want_dx) return;
-    d_mbar_wait(full, 0);
-    const uint32_t dh0 = d_smem_u32(s_dh);
+    tfy_mbar_wait(full, 0);
+    const uint32_t dh0 = tfy_smem_u32(s_dh);
     float acc[2][DB_N / 2];
     tfy_wg_fence();
-    if (which == 0) d_mma_chunk<1>(acc, dh0, d_smem_u32(s_x), true);
-    else d_mma_chunk<0>(acc, dh0, d_smem_u32(s_w), true);
+    if (which == 0) d_mma_chunk<1>(acc, dh0, tfy_smem_u32(s_x), true);
+    else d_mma_chunk<0>(acc, dh0, tfy_smem_u32(s_w), true);
     tfy_wg_commit();
     tfy_wg_wait<0>();
     d_epilogue(acc, s_acc + which * (ACC_BYTES / 4), s_out + which * TILE_BYTES, 1 + which,
@@ -188,7 +149,7 @@ tfy_dense_bwd_tiled_kernel(const __grid_constant__ CUtensorMap map_dh, const __g
                            const __grid_constant__ CUtensorMap map_w, const __grid_constant__ CUtensorMap map_dw,
                            const __grid_constant__ CUtensorMap map_dx, int n_u_tiles, int n_b_tiles, int want_dx) {
     extern __shared__ uint8_t smem_raw[];
-    uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
+    uint8_t* smem = tfy_align1024(smem_raw);
     uint8_t* ring = smem;                                            // [3] { dh box0, dh box1, tile }
     uint8_t* s_out = ring + (size_t)DT_STAGES * DT_STAGE_BYTES;      // staging for the TMA store
     float* s_acc = reinterpret_cast<float*>(s_out + TILE_BYTES);     // [128][ACC_LD] fp32
@@ -203,30 +164,30 @@ tfy_dense_bwd_tiled_kernel(const __grid_constant__ CUtensorMap map_dh, const __g
     const int n_chunks = is_dw ? n_b_tiles : n_u_tiles;              // K loop: batch chunks (dW) / unit chunks (dx)
     if (!is_dw && !want_dx) return;
     if (threadIdx.x == 0) {
-        asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&map_dh)) : "memory");
-        asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(is_dw ? &map_x : &map_w)) : "memory");
-        for (int st = 0; st < DT_STAGES; ++st) { d_mbar_init(&full[st], 1); d_mbar_init(&empty[st], 4); }
+        tfy_prefetch_tensormap(&map_dh);
+        tfy_prefetch_tensormap(is_dw ? &map_x : &map_w);
+        for (int st = 0; st < DT_STAGES; ++st) { tfy_mbar_init(&full[st], 1); tfy_mbar_init(&empty[st], 4); }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
     __syncthreads();
     tfy_pdl_sync();
 
     if (warp == 4) {
-        if (d_elect_one()) {
+        if (tfy_elect_one()) {
             for (int i = 0; i < n_chunks; ++i) {
                 const int st = i % DT_STAGES;
-                if (i >= DT_STAGES) d_mbar_wait(&empty[st], ((i / DT_STAGES) - 1) & 1);
+                if (i >= DT_STAGES) tfy_mbar_wait(&empty[st], ((i / DT_STAGES) - 1) & 1);
                 uint8_t* dst = ring + (size_t)st * DT_STAGE_BYTES;
-                d_mbar_expect_tx(&full[st], DT_STAGE_BYTES);
+                tfy_mbar_expect_tx(&full[st], DT_STAGE_BYTES);
                 const int k0 = i * DB_K;
                 if (is_dw) {           // dh rows = batch chunk, columns = this tile's units; x rows = batch chunk
-                    d_tma_load_2d(&map_dh, &full[st], dst, m0, k0);
-                    d_tma_load_2d(&map_dh, &full[st], dst + TILE_BYTES, m0 + 64, k0);
-                    d_tma_load_2d(&map_x, &full[st], dst + DH_BYTES, n0, k0);
+                    tfy_tma_load_2d(&map_dh, &full[st], dst, m0, k0);
+                    tfy_tma_load_2d(&map_dh, &full[st], dst + TILE_BYTES, m0 + 64, k0);
+                    tfy_tma_load_2d(&map_x, &full[st], dst + DH_BYTES, n0, k0);
                 } else {               // dh rows = this tile's batch rows, columns = unit chunk; W rows = unit chunk
-                    d_tma_load_2d(&map_dh, &full[st], dst, k0, m0);
-                    d_tma_load_2d(&map_dh, &full[st], dst + TILE_BYTES, k0 + 64, m0);
-                    d_tma_load_2d(&map_w, &full[st], dst + DH_BYTES, n0, k0);
+                    tfy_tma_load_2d(&map_dh, &full[st], dst, k0, m0);
+                    tfy_tma_load_2d(&map_dh, &full[st], dst + TILE_BYTES, k0 + 64, m0);
+                    tfy_tma_load_2d(&map_w, &full[st], dst + DH_BYTES, n0, k0);
                 }
             }
         }
@@ -237,49 +198,20 @@ tfy_dense_bwd_tiled_kernel(const __grid_constant__ CUtensorMap map_dh, const __g
     tfy_wg_zero<DB_N>(acc[1]);
     for (int i = 0; i < n_chunks; ++i) {
         const int st = i % DT_STAGES;
-        d_mbar_wait(&full[st], (i / DT_STAGES) & 1);
+        tfy_mbar_wait(&full[st], (i / DT_STAGES) & 1);
         tfy_wg_fence();
-        const uint32_t dh0 = d_smem_u32(ring + (size_t)st * DT_STAGE_BYTES), t0 = dh0 + DH_BYTES;
+        const uint32_t dh0 = tfy_smem_u32(ring + (size_t)st * DT_STAGE_BYTES), t0 = dh0 + DH_BYTES;
         if (is_dw) d_mma_chunk<1>(acc, dh0, t0, false);
         else d_mma_chunk<0>(acc, dh0, t0, false);
         tfy_wg_commit();
         tfy_wg_wait<0>();
-        if (lane == 0) d_mbar_arrive(&empty[st]);
+        if (lane == 0) tfy_mbar_arrive(&empty[st]);
     }
     d_epilogue(acc, s_acc, s_out, 1, is_dw ? &map_dw : &map_dx, n0, m0);
 }
 
 namespace {
-
-using DEncodeFn = CUresult (*)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
-                               const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
-                               CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-DEncodeFn d_encode = nullptr;
 bool d_attr_set = false, d_attr_set_tiled = false;
-
-bool d_load_encode() {
-    if (d_encode) return true;
-    void* fn = nullptr;
-    cudaDriverEntryPointQueryResult st;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &fn, cudaEnableDefault, &st) != cudaSuccess ||
-        st != cudaDriverEntryPointSuccess || !fn)
-        return false;
-    d_encode = reinterpret_cast<DEncodeFn>(fn);
-    return true;
-}
-
-// row-major [rows, cols] bf16 matrix (leading dimension ld elements); box = 64 columns x 128 rows, 128 B swizzle;
-// rows / columns beyond the extent read as zeros and are not written by stores
-bool d_make_map(CUtensorMap* map, const void* ptr, uint64_t rows, uint64_t cols, uint64_t ld) {
-    cuuint64_t dims[2] = {cols, rows};
-    cuuint64_t strides[1] = {ld * 2};
-    cuuint32_t box[2] = {64, 128};
-    cuuint32_t estr[2] = {1, 1};
-    return d_encode(map, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(ptr), dims, strides, box, estr,
-                    CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                    CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
-}
-
 }  // namespace
 
 extern "C" {
@@ -293,7 +225,7 @@ int tfy_dense_bwd(const void* dh, const void* x, const void* w, void* dw, void* 
     if (B < 1 || U < 8 || (U & 7) || (I & 7) || I < 8) return -2;
     if (B > DB_M || U > DB_M) {
         if (((uintptr_t)dh | (uintptr_t)x | (uintptr_t)w | (uintptr_t)dw | (uintptr_t)dx) & 15) return -3;
-        if (!d_load_encode()) return -4;
+        if (!tfy_tensor_map_encoder()) return -4;
         if (!d_attr_set_tiled) {
             if (cudaFuncSetAttribute(tfy_dense_bwd_tiled_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                      (int)DT_SMEM) != cudaSuccess)
@@ -301,8 +233,9 @@ int tfy_dense_bwd(const void* dh, const void* x, const void* w, void* dw, void* 
             d_attr_set_tiled = true;
         }
         CUtensorMap mdh, mx, mw, mdw, mdx;
-        if (!d_make_map(&mdh, dh, B, U, U) || !d_make_map(&mx, x, B, I, I) || !d_make_map(&mw, w, U, I, I) ||
-            !d_make_map(&mdw, dw, U, I, I) || !d_make_map(&mdx, dx ? dx : dw, dx ? B : U, I, I))
+        if (!tfy_tensor_map_bf16_2d(&mdh, dh, B, U, U) || !tfy_tensor_map_bf16_2d(&mx, x, B, I, I) ||
+            !tfy_tensor_map_bf16_2d(&mw, w, U, I, I) || !tfy_tensor_map_bf16_2d(&mdw, dw, U, I, I) ||
+            !tfy_tensor_map_bf16_2d(&mdx, dx ? dx : dw, dx ? B : U, I, I))
             return -6;
         const int n_u = (U + DB_M - 1) / DB_M, n_b = (B + DB_M - 1) / DB_M;
         dim3 grid((I + DB_N - 1) / DB_N, n_u + (dx ? n_b : 0));
@@ -311,7 +244,7 @@ int tfy_dense_bwd(const void* dh, const void* x, const void* w, void* dw, void* 
         return (int)cudaGetLastError();
     }
     if (((uintptr_t)dh | (uintptr_t)x | (uintptr_t)w | (uintptr_t)dw | (uintptr_t)dx) & 15) return -3;
-    if (!d_load_encode()) return -4;
+    if (!tfy_tensor_map_encoder()) return -4;
     if (!d_attr_set) {
         if (cudaFuncSetAttribute(tfy_dense_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)DB_SMEM) !=
             cudaSuccess)
@@ -319,8 +252,9 @@ int tfy_dense_bwd(const void* dh, const void* x, const void* w, void* dw, void* 
         d_attr_set = true;
     }
     CUtensorMap mdh, mx, mw, mdw, mdx;
-    if (!d_make_map(&mdh, dh, B, U, U) || !d_make_map(&mx, x, B, I, I) || !d_make_map(&mw, w, U, I, I) ||
-        !d_make_map(&mdw, dw, U, I, I) || !d_make_map(&mdx, dx ? dx : dw, dx ? B : U, I, I))
+    if (!tfy_tensor_map_bf16_2d(&mdh, dh, B, U, U) || !tfy_tensor_map_bf16_2d(&mx, x, B, I, I) ||
+        !tfy_tensor_map_bf16_2d(&mw, w, U, I, I) || !tfy_tensor_map_bf16_2d(&mdw, dw, U, I, I) ||
+        !tfy_tensor_map_bf16_2d(&mdx, dx ? dx : dw, dx ? B : U, I, I))
         return -6;
     const int grid = (I + DB_N - 1) / DB_N;
     tfy_launch_pdl((tfy_dense_bwd_kernel), dim3(grid), dim3(DB_THREADS), DB_SMEM, s, mdh, mx, mw, mdw, mdx,

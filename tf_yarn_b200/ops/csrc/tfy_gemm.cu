@@ -15,9 +15,8 @@
 //   warp 4   : TMA producer  -- cp.async.bulk.tensor.2d of a 128x64 A box and a 128x64 B box per
 //              stage (128-byte swizzle), completion on an mbarrier (complete_tx)
 // Pipeline: STAGES-deep ring of {A,B} tiles guarded by full/empty mbarriers.
-#include <cuda.h>
-
 #include "tfy_common.cuh"
+#include "tfy_tma.cuh"
 #include "tfy_wgmma.cuh"
 
 namespace {
@@ -28,47 +27,6 @@ constexpr int GEMM_THREADS = 160;
 constexpr int ACC_LD = BN + 4;        // fp32 row pitch of the staged accumulator (conflict-free row reads)
 constexpr size_t SMEM_BYTES = (size_t)STAGES * STAGE_BYTES + (size_t)BM * ACC_LD * 4 + 1024 /*align slack*/ +
                               256 /*barriers*/;
-
-__device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-
-__device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count) : "memory");
-}
-__device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
-    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
-    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
-    asm volatile(
-        "{\n\t"
-        ".reg .pred P1;\n\t"
-        "WAIT_LOOP:\n\t"
-        "mbarrier.try_wait.parity.shared::cta.b64 P1, [%0], %1;\n\t"
-        "@P1 bra DONE;\n\t"
-        "bra WAIT_LOOP;\n\t"
-        "DONE:\n\t"
-        "}" ::"r"(smem_u32(bar)), "r"(parity) : "memory");
-}
-__device__ __forceinline__ void tma_load_2d(const CUtensorMap* map, uint64_t* bar, void* dst, int c0, int c1) {
-    asm volatile(
-        "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
-        ::"r"(smem_u32(dst)), "l"(reinterpret_cast<uint64_t>(map)), "r"(smem_u32(bar)), "r"(c0), "r"(c1)
-        : "memory");
-}
-
-// One lane of a converged warp: the compiler keeps the TMA operands in uniform registers.
-__device__ __forceinline__ bool tc_elect_one() {
-    uint32_t pred;
-    asm volatile("{\n\t.reg .pred P;\n\telect.sync _|P, 0xffffffff;\n\tselp.b32 %0, 1, 0, P;\n\t}" : "=r"(pred));
-    return pred != 0;
-}
-
-// K-major, 128-byte swizzled operand tile: rows of 64 bf16 (128 B); 8-row core groups 1024 B apart.
-__device__ __forceinline__ uint64_t make_kmajor_sw128_desc(uint32_t smem_addr) {
-    return tfy_wg_desc(smem_addr, 16, 1024, TFY_WG_SW128);
-}
 
 }  // namespace
 
@@ -96,7 +54,7 @@ tfy_gemm_bf16_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_con
                      __nv_bfloat16* __restrict__ C, float* __restrict__ C32, const __nv_bfloat16* __restrict__ bias,
                      int M, int N, int K, int ldc, int relu, int out_mode, int k_tiles_per_split, TfySplitKEpilogue ep) {
     extern __shared__ uint8_t smem_raw[];
-    uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
+    uint8_t* smem = tfy_align1024(smem_raw);
     uint8_t* tiles = smem;
     float* acc_s = reinterpret_cast<float*>(smem + (size_t)STAGES * STAGE_BYTES);     // [BM][ACC_LD]
     uint64_t* full = reinterpret_cast<uint64_t*>(acc_s + (size_t)BM * ACC_LD);
@@ -111,11 +69,11 @@ tfy_gemm_bf16_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_con
     const int n_kt = kt1 - kt0;
 
     if (threadIdx.x == 0) {
-        asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&map_a)) : "memory");
-        asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&map_b)) : "memory");
+        tfy_prefetch_tensormap(&map_a);
+        tfy_prefetch_tensormap(&map_b);
         for (int s = 0; s < STAGES; ++s) {
-            mbar_init(&full[s], 1);
-            mbar_init(&empty[s], 4);           // one arrival per MMA warp
+            tfy_mbar_init(&full[s], 1);
+            tfy_mbar_init(&empty[s], 4);           // one arrival per MMA warp
         }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
@@ -123,17 +81,17 @@ tfy_gemm_bf16_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_con
     tfy_pdl_sync();                      // upstream grids complete; our dependents may start launching
 
     if (warp == 4) {
-        if (tc_elect_one()) {
+        if (tfy_elect_one()) {
             for (int i = 0; i < n_kt; ++i) {
                 const int s = i % STAGES;
                 const uint32_t ph = (i / STAGES) & 1;
-                mbar_wait(&empty[s], ph ^ 1);
+                tfy_mbar_wait(&empty[s], ph ^ 1);
                 uint8_t* a_dst = tiles + (size_t)s * STAGE_BYTES;
                 uint8_t* b_dst = a_dst + A_BYTES;
-                mbar_expect_tx(&full[s], STAGE_BYTES);
+                tfy_mbar_expect_tx(&full[s], STAGE_BYTES);
                 const int k0 = (kt0 + i) * BK;
-                tma_load_2d(&map_a, &full[s], a_dst, k0, m0);
-                tma_load_2d(&map_b, &full[s], b_dst, k0, n0);
+                tfy_tma_load_2d(&map_a, &full[s], a_dst, k0, m0);
+                tfy_tma_load_2d(&map_b, &full[s], b_dst, k0, n0);
             }
         }
         return;
@@ -146,21 +104,21 @@ tfy_gemm_bf16_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_con
         tfy_wg_zero<BN>(acc[1]);
         for (int i = 0; i < n_kt; ++i) {
             const int s = i % STAGES;
-            mbar_wait(&full[s], (i / STAGES) & 1);
+            tfy_mbar_wait(&full[s], (i / STAGES) & 1);
             tfy_wg_fence();
-            const uint32_t a_addr = smem_u32(tiles + (size_t)s * STAGE_BYTES);
-            const uint64_t bdesc = make_kmajor_sw128_desc(a_addr + A_BYTES);
+            const uint32_t a_addr = tfy_smem_u32(tiles + (size_t)s * STAGE_BYTES);
+            const uint64_t bdesc = tfy_wg_desc_sw128(a_addr + A_BYTES);
 #pragma unroll
             for (int k = 0; k < BK / UMMA_K; ++k) {
                 // advance 16 bf16 = 32 B along K inside the 128 B swizzle atom: +2 in 16-byte units
 #pragma unroll
                 for (int h = 0; h < 2; ++h)
-                    tfy_wgmma_m64n128<0, 0>(acc[h], make_kmajor_sw128_desc(a_addr + h * 64 * 128) + (uint64_t)(2 * k),
+                    tfy_wgmma_m64n128<0, 0>(acc[h], tfy_wg_desc_sw128(a_addr + h * 64 * 128) + (uint64_t)(2 * k),
                                             bdesc + (uint64_t)(2 * k), 1u);
             }
             tfy_wg_commit();
             tfy_wg_wait<1>();
-            if (i > 0 && lane == 0) mbar_arrive(&empty[(i - 1) % STAGES]);
+            if (i > 0 && lane == 0) tfy_mbar_arrive(&empty[(i - 1) % STAGES]);
         }
         tfy_wg_wait<0>();
         tfy_wg_store_rows<BN>(acc_s, ACC_LD, acc[0], 0);
@@ -287,36 +245,9 @@ tfy_gemm_bf16_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_con
 // host side
 // ---------------------------------------------------------------------------------------------
 namespace {
-
-using EncodeFn = CUresult (*)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
-                              const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
-                              CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-EncodeFn g_encode = nullptr;
+// the operand maps are tfy_tensor_map_bf16_2d: one box is BK columns x BM (= BN) rows
+static_assert(BK == 64 && BM == 128 && BN == 128, "tile shape must match the tensor-map box");
 bool g_attr_set = false;
-
-bool load_encode() {
-    if (g_encode) return true;
-    void* fn = nullptr;
-    cudaDriverEntryPointQueryResult st;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &fn, cudaEnableDefault, &st) != cudaSuccess ||
-        st != cudaDriverEntryPointSuccess || !fn)
-        return false;
-    g_encode = reinterpret_cast<EncodeFn>(fn);
-    return true;
-}
-
-// row-major [rows, K] bf16 matrix with leading dimension ld (elements); box = 64 (K) x 128 (rows)
-bool make_map(CUtensorMap* map, const void* ptr, uint64_t rows, uint64_t K, uint64_t ld) {
-    cuuint64_t dims[2] = {K, rows};
-    cuuint64_t strides[1] = {ld * 2};
-    cuuint32_t box[2] = {(cuuint32_t)BK, (cuuint32_t)BM};
-    cuuint32_t estr[2] = {1, 1};
-    CUresult r = g_encode(map, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(ptr), dims, strides, box, estr,
-                          CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                          CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    return r == CUDA_SUCCESS;
-}
-
 }  // namespace
 
 __global__ void __launch_bounds__(256) tfy_splitk_sum_f32_kernel(const float* __restrict__ slabs, float* __restrict__ out,
@@ -365,7 +296,7 @@ int tfy_gemm_bf16(const void* A, const void* B, void* C, float* C32, const void*
                   int ldb, int ldc, int relu, int split_k, cudaStream_t s) {
     if ((K & 7) || (lda & 7) || (ldb & 7)) return -2;
     if (((uintptr_t)A & 15) || ((uintptr_t)B & 15)) return -3;
-    if (!load_encode()) return -4;
+    if (!tfy_tensor_map_encoder()) return -4;
     if (!g_attr_set) {
         if (cudaFuncSetAttribute(tfy_gemm_bf16_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMEM_BYTES) !=
             cudaSuccess)
@@ -373,7 +304,7 @@ int tfy_gemm_bf16(const void* A, const void* B, void* C, float* C32, const void*
         g_attr_set = true;
     }
     CUtensorMap ma, mb;
-    if (!make_map(&ma, A, M, K, lda) || !make_map(&mb, B, N, K, ldb)) return -6;
+    if (!tfy_tensor_map_bf16_2d(&ma, A, M, K, lda) || !tfy_tensor_map_bf16_2d(&mb, B, N, K, ldb)) return -6;
     const int k_tiles = (K + BK - 1) / BK;
     if (split_k < 1) split_k = 1;
     if (split_k > k_tiles) split_k = k_tiles;
@@ -397,7 +328,7 @@ int tfy_gemm_bf16_splitk_fused(const void* A, const void* B, float* acc32, uint3
                                const TfyOptHyper* hp, int split_k, cudaStream_t s) {
     if ((K & 7) || (lda & 7) || (ldb & 7) || (N & 7)) return -2;
     if (((uintptr_t)A & 15) || ((uintptr_t)B & 15) || ((uintptr_t)y & 15)) return -3;
-    if (!load_encode()) return -4;
+    if (!tfy_tensor_map_encoder()) return -4;
     if (!g_attr_set) {
         if (cudaFuncSetAttribute(tfy_gemm_bf16_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMEM_BYTES) !=
             cudaSuccess)
@@ -405,7 +336,7 @@ int tfy_gemm_bf16_splitk_fused(const void* A, const void* B, float* acc32, uint3
         g_attr_set = true;
     }
     CUtensorMap ma, mb;
-    if (!make_map(&ma, A, M, K, lda) || !make_map(&mb, B, N, K, ldb)) return -6;
+    if (!tfy_tensor_map_bf16_2d(&ma, A, M, K, lda) || !tfy_tensor_map_bf16_2d(&mb, B, N, K, ldb)) return -6;
     const int k_tiles = (K + BK - 1) / BK;
     if (split_k < 1) split_k = 1;
     if (split_k > k_tiles) split_k = k_tiles;

@@ -9,9 +9,8 @@
 //   * epilogue straight from the accumulator registers: bias / ReLU -> bf16 pairs -> global.
 // Roles: warps 0-3 and 4-7 the two consumer warpgroups, warp 8 the TMA producer.
 // The B operand may be a peer (NVLink) address, as in tfy_gemm.cu.
-#include <cuda.h>
-
 #include "tfy_common.cuh"
+#include "tfy_tma.cuh"
 #include "tfy_wgmma.cuh"
 
 namespace {
@@ -23,42 +22,6 @@ constexpr int G2_STAGE_BYTES = G2_A_BYTES + G2_B_BYTES;                // 48 KB 
 constexpr int G2_THREADS = 288;
 constexpr size_t G2_SMEM = 1024 + (size_t)G2_STAGES * G2_STAGE_BYTES + 512;
 
-__device__ __forceinline__ uint32_t g2_smem(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ void g2_mbar_init(uint64_t* bar, uint32_t count) {
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(g2_smem(bar)), "r"(count) : "memory");
-}
-__device__ __forceinline__ void g2_mbar_arrive(uint64_t* bar) {
-    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(g2_smem(bar)) : "memory");
-}
-__device__ __forceinline__ void g2_mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
-    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(g2_smem(bar)), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void g2_mbar_wait(uint64_t* bar, uint32_t parity) {
-    asm volatile(
-        "{\n\t"
-        ".reg .pred P1;\n\t"
-        "G2WAIT_LOOP:\n\t"
-        "mbarrier.try_wait.parity.shared::cta.b64 P1, [%0], %1;\n\t"
-        "@P1 bra G2DONE;\n\t"
-        "bra G2WAIT_LOOP;\n\t"
-        "G2DONE:\n\t"
-        "}" ::"r"(g2_smem(bar)), "r"(parity) : "memory");
-}
-__device__ __forceinline__ void g2_tma_load(const CUtensorMap* map, uint64_t* bar, void* dst, int c0, int c1) {
-    asm volatile(
-        "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
-        ::"r"(g2_smem(dst)), "l"(reinterpret_cast<uint64_t>(map)), "r"(g2_smem(bar)), "r"(c0), "r"(c1)
-        : "memory");
-}
-__device__ __forceinline__ bool g2_elect() {
-    uint32_t pred;
-    asm volatile("{\n\t.reg .pred P;\n\telect.sync _|P, 0xffffffff;\n\tselp.b32 %0, 1, 0, P;\n\t}" : "=r"(pred));
-    return pred != 0;
-}
-__device__ __forceinline__ uint64_t g2_desc(uint32_t smem_addr) {     // K-major, SWIZZLE_128B, 8-row groups 1024 B apart
-    return tfy_wg_desc(smem_addr, 16, 1024, TFY_WG_SW128);
-}
-
 }  // namespace
 
 __global__ void __launch_bounds__(G2_THREADS, 1)
@@ -66,7 +29,7 @@ tfy_gemm2_bf16_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_co
                       __nv_bfloat16* __restrict__ C, const __nv_bfloat16* __restrict__ bias, int M, int N, int K,
                       int ldc, int relu) {
     extern __shared__ uint8_t smem_raw[];
-    uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
+    uint8_t* smem = tfy_align1024(smem_raw);
     uint8_t* ring = smem;
     uint64_t* full = reinterpret_cast<uint64_t*>(ring + (size_t)G2_STAGES * G2_STAGE_BYTES);
     uint64_t* empty = full + G2_STAGES;
@@ -77,11 +40,11 @@ tfy_gemm2_bf16_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_co
     const int k_blocks = (K + G2_BK - 1) / G2_BK;
 
     if (threadIdx.x == 0) {
-        asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&map_a)) : "memory");
-        asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&map_b)) : "memory");
+        tfy_prefetch_tensormap(&map_a);
+        tfy_prefetch_tensormap(&map_b);
         for (int s = 0; s < G2_STAGES; ++s) {
-            g2_mbar_init(&full[s], 1);         // the producer's expect_tx + the TMA bytes
-            g2_mbar_init(&empty[s], 8);        // one arrival per consumer warp
+            tfy_mbar_init(&full[s], 1);         // the producer's expect_tx + the TMA bytes
+            tfy_mbar_init(&empty[s], 8);        // one arrival per consumer warp
         }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
@@ -90,18 +53,18 @@ tfy_gemm2_bf16_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_co
 
     if (warp == 8) {
         // ===== TMA producer: 128 rows of A and 256 rows of B (two 128-row boxes) per stage =====
-        if (g2_elect()) {
+        if (tfy_elect_one()) {
             uint32_t it = 0;
             for (int t = blockIdx.x; t < n_tiles; t += gridDim.x) {
                 const int m0 = (t % tiles_m) * G2_BM, n0 = (t / tiles_m) * G2_BN;
                 for (int kb = 0; kb < k_blocks; ++kb, ++it) {
                     const int s = it % G2_STAGES;
-                    if (it >= G2_STAGES) g2_mbar_wait(&empty[s], ((it / G2_STAGES) - 1) & 1);
+                    if (it >= G2_STAGES) tfy_mbar_wait(&empty[s], ((it / G2_STAGES) - 1) & 1);
                     uint8_t* a_dst = ring + (size_t)s * G2_STAGE_BYTES;
-                    g2_mbar_expect_tx(&full[s], G2_STAGE_BYTES);
-                    g2_tma_load(&map_a, &full[s], a_dst, kb * G2_BK, m0);
-                    g2_tma_load(&map_b, &full[s], a_dst + G2_A_BYTES, kb * G2_BK, n0);
-                    g2_tma_load(&map_b, &full[s], a_dst + G2_A_BYTES + G2_B_BYTES / 2, kb * G2_BK, n0 + 128);
+                    tfy_mbar_expect_tx(&full[s], G2_STAGE_BYTES);
+                    tfy_tma_load_2d(&map_a, &full[s], a_dst, kb * G2_BK, m0);
+                    tfy_tma_load_2d(&map_b, &full[s], a_dst + G2_A_BYTES, kb * G2_BK, n0);
+                    tfy_tma_load_2d(&map_b, &full[s], a_dst + G2_A_BYTES + G2_B_BYTES / 2, kb * G2_BK, n0 + 128);
                 }
             }
         }
@@ -116,19 +79,20 @@ tfy_gemm2_bf16_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_co
         tfy_wg_zero<G2_BN>(acc);
         for (int kb = 0; kb < k_blocks; ++kb, ++it) {
             const int s = it % G2_STAGES;
-            g2_mbar_wait(&full[s], (it / G2_STAGES) & 1);
+            tfy_mbar_wait(&full[s], (it / G2_STAGES) & 1);
             tfy_wg_fence();
-            const uint32_t a_addr = g2_smem(ring + (size_t)s * G2_STAGE_BYTES);
-            const uint64_t adesc = g2_desc(a_addr + h * 64 * 128), bdesc = g2_desc(a_addr + G2_A_BYTES);
+            const uint32_t a_addr = tfy_smem_u32(ring + (size_t)s * G2_STAGE_BYTES);
+            const uint64_t adesc = tfy_wg_desc_sw128(a_addr + h * 64 * 128);
+            const uint64_t bdesc = tfy_wg_desc_sw128(a_addr + G2_A_BYTES);
 #pragma unroll
             for (int k = 0; k < G2_BK / 16; ++k)
                 tfy_wgmma_m64n256<0, 0>(acc, adesc + (uint64_t)(2 * k), bdesc + (uint64_t)(2 * k), 1u);
             tfy_wg_commit();
             tfy_wg_wait<1>();                            // the previous stage's wgmmas have retired
-            if (kb > 0 && lane == 0) g2_mbar_arrive(&empty[(it - 1) % G2_STAGES]);
+            if (kb > 0 && lane == 0) tfy_mbar_arrive(&empty[(it - 1) % G2_STAGES]);
         }
         tfy_wg_wait<0>();
-        if (k_blocks > 0 && lane == 0) g2_mbar_arrive(&empty[(it - 1) % G2_STAGES]);
+        if (k_blocks > 0 && lane == 0) tfy_mbar_arrive(&empty[(it - 1) % G2_STAGES]);
         // fragment layout: value i of this thread is row 16 w + lane / 4 + 8 ((i / 2) % 2), column 8 (i / 4) + 2 (lane % 4)
         const int r0 = m0 + h * 64 + 16 * w + (lane >> 2);
 #pragma unroll
@@ -150,22 +114,8 @@ tfy_gemm2_bf16_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_co
 
 namespace {
 
-using G2EncodeFn = CUresult (*)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
-                                const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
-                                CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-G2EncodeFn g2_encode = nullptr;
 bool g2_attr_set = false;
 int g2_sms = 0;
-
-bool g2_map(CUtensorMap* map, const void* ptr, uint64_t rows, uint64_t cols, uint64_t ld) {
-    cuuint64_t dims[2] = {cols, rows};
-    cuuint64_t strides[1] = {ld * 2};
-    cuuint32_t box[2] = {64, 128};
-    cuuint32_t estr[2] = {1, 1};
-    return g2_encode(map, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(ptr), dims, strides, box, estr,
-                     CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                     CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
-}
 
 }  // namespace
 
@@ -177,14 +127,7 @@ int tfy_gemm2_bf16(const void* A, const void* B, void* C, const void* bias, int 
                    int ldc, int relu, cudaStream_t s) {
     if ((K & 7) || (lda & 7) || (ldb & 7) || (ldc & 7)) return -2;
     if (((uintptr_t)A | (uintptr_t)B | (uintptr_t)C) & 15) return -3;
-    if (!g2_encode) {
-        void* fn = nullptr;
-        cudaDriverEntryPointQueryResult st;
-        if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &fn, cudaEnableDefault, &st) != cudaSuccess ||
-            st != cudaDriverEntryPointSuccess || !fn)
-            return -4;
-        g2_encode = reinterpret_cast<G2EncodeFn>(fn);
-    }
+    if (!tfy_tensor_map_encoder()) return -4;
     if (!g2_attr_set) {
         if (cudaFuncSetAttribute(tfy_gemm2_bf16_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)G2_SMEM) !=
             cudaSuccess)
@@ -195,7 +138,7 @@ int tfy_gemm2_bf16(const void* A, const void* B, void* C, const void* bias, int 
         g2_attr_set = true;
     }
     CUtensorMap ma, mb;
-    if (!g2_map(&ma, A, M, K, lda) || !g2_map(&mb, B, N, K, ldb)) return -6;
+    if (!tfy_tensor_map_bf16_2d(&ma, A, M, K, lda) || !tfy_tensor_map_bf16_2d(&mb, B, N, K, ldb)) return -6;
     const int n_tiles = ((M + G2_BM - 1) / G2_BM) * ((N + G2_BN - 1) / G2_BN);
     const int grid = n_tiles < g2_sms ? n_tiles : g2_sms;
     tfy_launch_pdl((tfy_gemm2_bf16_kernel), dim3(grid), dim3(G2_THREADS), G2_SMEM, s, ma, mb, (__nv_bfloat16*)C,

@@ -64,14 +64,6 @@ struct TfyPsHyper {
 
 namespace {
 
-__device__ __forceinline__ float4 ld_peer_f32x4(const void* p) {
-    float4 v;
-    asm volatile("ld.global.relaxed.sys.L1::no_allocate.v4.f32 {%0,%1,%2,%3}, [%4];"
-                 : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w)
-                 : "l"(p)
-                 : "memory");
-    return v;
-}
 __device__ __forceinline__ void red_add_f32x4(void* p, float4 v) {
     asm volatile("red.relaxed.sys.global.add.v4.f32 [%0], {%1,%2,%3,%4};" ::"l"(p), "f"(v.x), "f"(v.y), "f"(v.z),
                  "f"(v.w)
@@ -143,7 +135,7 @@ __global__ void __launch_bounds__(256) tfy_ps_pull_kernel(const TfyPsSeg* __rest
     LT* dst = reinterpret_cast<LT*>(sg.local);
     const size_t n4 = sg.n / 4;
     for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n4; i += (size_t)gridDim.x * blockDim.x)
-        st_local4<LT>(dst + i * 4, ld_peer_f32x4(src + i * 4));
+        st_local4<LT>(dst + i * 4, tfy_ld_peer_f32x4(src + i * 4));
     if (blockIdx.x == 0)   // scalar tail (n % 4 elements)
         for (size_t i = n4 * 4 + threadIdx.x; i < sg.n; i += blockDim.x) dst[i] = (LT)src[i];
 }
@@ -171,7 +163,7 @@ __device__ __forceinline__ void ps_apply4(int opt, float* w, float* s1, float* s
         const float4 g2 = make_float4(gv.x * gv.x, gv.y * gv.y, gv.z * gv.z, gv.w * gv.w);
         const float4 n_old = atom_add_f32x4(s1, g2);
         const float4 n_new = make_float4(n_old.x + g2.x, n_old.y + g2.y, n_old.z + g2.z, n_old.w + g2.w);
-        const float4 wv = ld_peer_f32x4(w);
+        const float4 wv = tfy_ld_peer_f32x4(w);
         const float inv_lr = 1.f / lr;
         const float4 dz = make_float4(gv.x - (sqrtf(n_new.x) - sqrtf(n_old.x)) * inv_lr * wv.x,
                                       gv.y - (sqrtf(n_new.y) - sqrtf(n_old.y)) * inv_lr * wv.y,
@@ -192,7 +184,7 @@ __device__ __forceinline__ void ps_apply4(int opt, float* w, float* s1, float* s
         delta.z = -lr * gv.z / (sqrtf(old.z + g2.z) + eps);
         delta.w = -lr * gv.w / (sqrtf(old.w + g2.w) + eps);
     } else if (opt == TFY_OPT_ADAM) {
-        float4 m = ld_peer_f32x4(s1), v = ld_peer_f32x4(s2);
+        float4 m = tfy_ld_peer_f32x4(s1), v = tfy_ld_peer_f32x4(s2);
         m = make_float4(p1 * m.x + (1.f - p1) * gv.x, p1 * m.y + (1.f - p1) * gv.y, p1 * m.z + (1.f - p1) * gv.z,
                         p1 * m.w + (1.f - p1) * gv.w);
         v = make_float4(p2 * v.x + (1.f - p2) * gv.x * gv.x, p2 * v.y + (1.f - p2) * gv.y * gv.y,
@@ -266,7 +258,7 @@ tfy_ps_push_kernel(const TfyPsSeg* __restrict__ segs, float grad_scale, const fl
     for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n4; i += (size_t)gridDim.x * blockDim.x) {
         float4 gv = f4_mul(ld_local4<GT>(g + i * 4), grad_scale);
         if (wd != 0.f) {
-            const float4 wv = ld_peer_f32x4(w + i * 4);
+            const float4 wv = tfy_ld_peer_f32x4(w + i * 4);
             gv.x += wd * wv.x; gv.y += wd * wv.y; gv.z += wd * wv.z; gv.w += wd * wv.w;
         }
         float4 neww;
@@ -298,7 +290,7 @@ tfy_ps_embedding_bag_kernel(const float* __restrict__ table, const long long* __
         for (int j = 0; j < L; ++j) {
             long long id = ids[(size_t)b * L + j];
             if (id < 0 || id >= V) continue;
-            const float4 v = ld_peer_f32x4(table + (size_t)id * D + d);
+            const float4 v = tfy_ld_peer_f32x4(table + (size_t)id * D + d);
             acc.x += v.x; acc.y += v.y; acc.z += v.z; acc.w += v.w;
         }
         acc.x *= scale; acc.y *= scale; acc.z *= scale; acc.w *= scale;
@@ -704,7 +696,7 @@ namespace {
 template <int VEC>
 __device__ __forceinline__ float4 ld_row(const float* p) {
     if constexpr (VEC == 4) {
-        return ld_peer_f32x4(p);
+        return tfy_ld_peer_f32x4(p);
     } else {
         float v;
         asm volatile("ld.global.relaxed.sys.L1::no_allocate.f32 %0, [%1];" : "=f"(v) : "l"(p) : "memory");
@@ -767,7 +759,7 @@ __global__ void __launch_bounds__(256) tfy_ps_refresh_shadow_kernel(const TfyPsS
     __nv_bfloat16* sh = reinterpret_cast<__nv_bfloat16*>(sg.remote_shadow);
     const size_t n4 = sg.n / 4;
     for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n4; i += (size_t)gridDim.x * blockDim.x)
-        st_shadow4(sh, i * 4, ld_peer_f32x4(w + i * 4), sg.cols, sg.shadow_ld);
+        st_shadow4(sh, i * 4, tfy_ld_peer_f32x4(w + i * 4), sg.cols, sg.shadow_ld);
     if (blockIdx.x == 0)
         for (size_t i = n4 * 4 + threadIdx.x; i < sg.n; i += blockDim.x)
             sh[shadow_index(i, sg.cols, sg.shadow_ld)] = __float2bfloat16(w[i]);

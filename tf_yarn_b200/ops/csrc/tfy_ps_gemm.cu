@@ -20,9 +20,8 @@
 // warps 0-15: A-tile producers (4 threads per row, 3 chunks in flight each: a gather is a dependent id -> row round
 // trip to (remote) HBM per chunk, so the K loop is only as fast as the number of rows in flight)
 // warps 16-19: wgmma + epilogue   warp 20: TMA (B tiles)
-#include <cuda.h>
-
 #include "tfy_common.cuh"
+#include "tfy_tma.cuh"
 #include "tfy_wgmma.cuh"
 
 namespace {
@@ -36,50 +35,6 @@ constexpr int PG_THREADS = (PG_PROD_WARPS + 5) * 32;                         // 
 constexpr int PG_ACC_BYTES = PG_BM * PG_BN * 4;                              // [8 pieces][32 values][128 threads]
 constexpr size_t PG_SMEM = 1024 + (size_t)PG_STAGES * PG_STAGE_BYTES + PG_ACC_BYTES + 512;
 
-__device__ __forceinline__ uint32_t pg_smem(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ void pg_mbar_init(uint64_t* bar, uint32_t count) {
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(pg_smem(bar)), "r"(count) : "memory");
-}
-__device__ __forceinline__ void pg_mbar_arrive(uint64_t* bar) {
-    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(pg_smem(bar)) : "memory");
-}
-__device__ __forceinline__ void pg_mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
-    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(pg_smem(bar)), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void pg_mbar_wait(uint64_t* bar, uint32_t parity) {
-    asm volatile(
-        "{\n\t"
-        ".reg .pred P1;\n\t"
-        "PGWAIT_LOOP:\n\t"
-        "mbarrier.try_wait.parity.shared::cta.b64 P1, [%0], %1;\n\t"
-        "@P1 bra PGDONE;\n\t"
-        "bra PGWAIT_LOOP;\n\t"
-        "PGDONE:\n\t"
-        "}" ::"r"(pg_smem(bar)), "r"(parity) : "memory");
-}
-__device__ __forceinline__ void pg_tma_load(const CUtensorMap* map, uint64_t* bar, void* dst, int c0, int c1) {
-    asm volatile(
-        "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
-        ::"r"(pg_smem(dst)), "l"(reinterpret_cast<uint64_t>(map)), "r"(pg_smem(bar)), "r"(c0), "r"(c1)
-        : "memory");
-}
-__device__ __forceinline__ bool pg_elect() {
-    uint32_t pred;
-    asm volatile("{\n\t.reg .pred P;\n\telect.sync _|P, 0xffffffff;\n\tselp.b32 %0, 1, 0, P;\n\t}" : "=r"(pred));
-    return pred != 0;
-}
-__device__ __forceinline__ uint64_t pg_desc(uint32_t smem_addr) {      // K-major, SWIZZLE_128B
-    return tfy_wg_desc(smem_addr, 16, 1024, TFY_WG_SW128);
-}
-__device__ __forceinline__ float4 pg_ld_peer(const float* p) {
-    float4 v;
-    asm volatile("ld.global.relaxed.sys.L1::no_allocate.v4.f32 {%0,%1,%2,%3}, [%4];"
-                 : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w)
-                 : "l"(p)
-                 : "memory");
-    return v;
-}
-
 }  // namespace
 
 // tables: device array of T peer pointers to fp32 [V, 64] embedding tables; ids: int64 [T, B]; numeric: fp32 [B, n_num]
@@ -91,7 +46,7 @@ tfy_ps_gather_gemm_kernel(const __grid_constant__ CUtensorMap map_w, const uint6
                           const __nv_bfloat16* __restrict__ bias, __nv_bfloat16* __restrict__ xbuf,
                           __nv_bfloat16* __restrict__ y, int B, int N, int T, int n_num, int Kp, long long V) {
     extern __shared__ uint8_t smem_raw[];
-    uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
+    uint8_t* smem = tfy_align1024(smem_raw);
     uint8_t* ring = smem;
     float* acc_s = reinterpret_cast<float*>(ring + (size_t)PG_STAGES * PG_STAGE_BYTES);
     uint64_t* full_a = reinterpret_cast<uint64_t*>(reinterpret_cast<uint8_t*>(acc_s) + PG_ACC_BYTES);
@@ -102,11 +57,11 @@ tfy_ps_gather_gemm_kernel(const __grid_constant__ CUtensorMap map_w, const uint6
     const int b0 = blockIdx.x * PG_BM, n0 = blockIdx.y * PG_BN;
     const int n_chunks = T + (n_num > 0 ? 1 : 0);
     if (threadIdx.x == 0) {
-        asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&map_w)) : "memory");
+        tfy_prefetch_tensormap(&map_w);
         for (int s = 0; s < PG_STAGES; ++s) {
-            pg_mbar_init(&full_a[s], PG_PROD_THREADS);
-            pg_mbar_init(&full_b[s], 1);
-            pg_mbar_init(&empty[s], 4);        // one arrival per MMA warp
+            tfy_mbar_init(&full_a[s], PG_PROD_THREADS);
+            tfy_mbar_init(&full_b[s], 1);
+            tfy_mbar_init(&empty[s], 4);        // one arrival per MMA warp
         }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
@@ -115,14 +70,14 @@ tfy_ps_gather_gemm_kernel(const __grid_constant__ CUtensorMap map_w, const uint6
 
     if (warp == PG_TMA_WARP) {
         // ===== weights: the ps rank's bf16 shadow, two 128-row boxes per 64-column chunk =====
-        if (pg_elect()) {
+        if (tfy_elect_one()) {
             for (int c = 0; c < n_chunks; ++c) {
                 const int s = c % PG_STAGES;
-                if (c >= PG_STAGES) pg_mbar_wait(&empty[s], ((c / PG_STAGES) - 1) & 1);
+                if (c >= PG_STAGES) tfy_mbar_wait(&empty[s], ((c / PG_STAGES) - 1) & 1);
                 uint8_t* b_dst = ring + (size_t)s * PG_STAGE_BYTES + PG_A_BYTES;
-                pg_mbar_expect_tx(&full_b[s], PG_B_BYTES);
-                pg_tma_load(&map_w, &full_b[s], b_dst, c * PG_BK, n0);
-                pg_tma_load(&map_w, &full_b[s], b_dst + PG_B_BYTES / 2, c * PG_BK, n0 + 128);
+                tfy_mbar_expect_tx(&full_b[s], PG_B_BYTES);
+                tfy_tma_load_2d(&map_w, &full_b[s], b_dst, c * PG_BK, n0);
+                tfy_tma_load_2d(&map_w, &full_b[s], b_dst + PG_B_BYTES / 2, c * PG_BK, n0 + 128);
             }
         }
     } else if (warp >= PG_MMA_WARP) {
@@ -134,14 +89,14 @@ tfy_ps_gather_gemm_kernel(const __grid_constant__ CUtensorMap map_w, const uint6
         for (int c = 0; c < n_chunks; ++c) {
             const int s = c % PG_STAGES;
             const uint32_t ph = (c / PG_STAGES) & 1;
-            pg_mbar_wait(&full_a[s], ph);
-            pg_mbar_wait(&full_b[s], ph);
-            const uint32_t a_addr = pg_smem(ring + (size_t)s * PG_STAGE_BYTES), b_addr = a_addr + PG_A_BYTES;
+            tfy_mbar_wait(&full_a[s], ph);
+            tfy_mbar_wait(&full_b[s], ph);
+            const uint32_t a_addr = tfy_smem_u32(ring + (size_t)s * PG_STAGE_BYTES), b_addr = a_addr + PG_A_BYTES;
 #pragma unroll 1
             for (int q = 0; q < 8; ++q) {
                 float d[32];
-                const uint64_t adesc = pg_desc(a_addr + (q >> 2) * 64 * 128);
-                const uint64_t bdesc = pg_desc(b_addr + (q & 3) * 64 * 128);
+                const uint64_t adesc = tfy_wg_desc_sw128(a_addr + (q >> 2) * 64 * 128);
+                const uint64_t bdesc = tfy_wg_desc_sw128(b_addr + (q & 3) * 64 * 128);
                 tfy_wg_fence();
 #pragma unroll
                 for (int k = 0; k < PG_BK / 16; ++k)
@@ -152,7 +107,7 @@ tfy_ps_gather_gemm_kernel(const __grid_constant__ CUtensorMap map_w, const uint6
 #pragma unroll
                 for (int i = 0; i < 32; ++i) acc_q[i * 128] += d[i];
             }
-            if (lane == 0) pg_mbar_arrive(&empty[s]);
+            if (lane == 0) tfy_mbar_arrive(&empty[s]);
         }
         // ===== epilogue: bias, bf16 pairs (fragment layout: row 16 w + l / 4 (+8), column 8 j + 2 (l % 4)) =====
         const int w = t >> 5;
@@ -185,7 +140,7 @@ tfy_ps_gather_gemm_kernel(const __grid_constant__ CUtensorMap map_w, const uint6
                 if (id >= 0 && id < V) row = reinterpret_cast<const float*>(tables[c]) + (size_t)id * 64 + p * 16;
             }
 #pragma unroll
-            for (int q = 0; q < 4; ++q) dst[q] = row ? pg_ld_peer(row + q * 4) : make_float4(0.f, 0.f, 0.f, 0.f);
+            for (int q = 0; q < 4; ++q) dst[q] = row ? tfy_ld_peer_f32x4(row + q * 4) : make_float4(0.f, 0.f, 0.f, 0.f);
         };
         float4 buf[PG_DEPTH][4];
 #pragma unroll
@@ -213,13 +168,13 @@ tfy_ps_gather_gemm_kernel(const __grid_constant__ CUtensorMap map_w, const uint6
                         pk[0] = TfyPack<__nv_bfloat16>::pack(f);
                         pk[1] = TfyPack<__nv_bfloat16>::pack(f + 8);
                     }
-                    if (c >= PG_STAGES) pg_mbar_wait(&empty[s], ((c / PG_STAGES) - 1) & 1);
+                    if (c >= PG_STAGES) tfy_mbar_wait(&empty[s], ((c / PG_STAGES) - 1) & 1);
                     uint8_t* a_row = ring + (size_t)s * PG_STAGE_BYTES + r * 128;
 #pragma unroll
                     for (int h = 0; h < 2; ++h)
                         *reinterpret_cast<uint4*>(a_row + (((2 * p + h) ^ (r & 7)) << 4)) = pk[h];
-                    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-                    pg_mbar_arrive(&full_a[s]);
+                    tfy_fence_proxy_async();
+                    tfy_mbar_arrive(&full_a[s]);
                     if (live) {                          // keep the activations for the backward (dW = dy^T x)
                         __nv_bfloat16* xr = xbuf + (size_t)b * Kp + c * 64 + p * 16;
 #pragma unroll
@@ -234,10 +189,6 @@ tfy_ps_gather_gemm_kernel(const __grid_constant__ CUtensorMap map_w, const uint6
 }
 
 namespace {
-using PGEncodeFn = CUresult (*)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
-                                const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
-                                CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-PGEncodeFn pg_encode = nullptr;
 bool pg_attr_set = false;
 }  // namespace
 
@@ -250,14 +201,7 @@ int tfy_ps_gather_gemm(const void* w_shadow, const uint64_t* tables, const void*
                        cudaStream_t s) {
     if (B < 1 || N < 8 || (N & 7) || (Kp & 7) || n_num < 0 || n_num > 64 || T < 0 || Kp < 64 * T + n_num) return -2;
     if (((uintptr_t)w_shadow | (uintptr_t)xbuf | (uintptr_t)y) & 15) return -3;
-    if (!pg_encode) {
-        void* fn = nullptr;
-        cudaDriverEntryPointQueryResult st;
-        if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &fn, cudaEnableDefault, &st) != cudaSuccess ||
-            st != cudaDriverEntryPointSuccess || !fn)
-            return -4;
-        pg_encode = reinterpret_cast<PGEncodeFn>(fn);
-    }
+    if (!tfy_tensor_map_encoder()) return -4;
     if (!pg_attr_set) {
         if (cudaFuncSetAttribute(tfy_ps_gather_gemm_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)PG_SMEM) !=
             cudaSuccess)
@@ -265,14 +209,7 @@ int tfy_ps_gather_gemm(const void* w_shadow, const uint64_t* tables, const void*
         pg_attr_set = true;
     }
     CUtensorMap mw;
-    cuuint64_t dims[2] = {(cuuint64_t)Kp, (cuuint64_t)N};
-    cuuint64_t strides[1] = {(cuuint64_t)Kp * 2};
-    cuuint32_t box[2] = {64, 128};
-    cuuint32_t estr[2] = {1, 1};
-    if (pg_encode(&mw, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(w_shadow), dims, strides, box, estr,
-                  CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                  CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) != CUDA_SUCCESS)
-        return -6;
+    if (!tfy_tensor_map_bf16_2d(&mw, w_shadow, N, Kp, Kp)) return -6;
     dim3 grid((B + PG_BM - 1) / PG_BM, (N + PG_BN - 1) / PG_BN);
     tfy_launch_pdl((tfy_ps_gather_gemm_kernel), grid, dim3(PG_THREADS), PG_SMEM, s, mw, tables, (const long long*)ids,
                    (const float*)numeric, (const __nv_bfloat16*)bias, (__nv_bfloat16*)xbuf, (__nv_bfloat16*)y, B, N, T,

@@ -22,6 +22,10 @@ __device__ __forceinline__ uint64_t tfy_wg_desc(uint32_t smem_addr, uint32_t lbo
     d |= (uint64_t)layout << 62;
     return d;
 }
+// 128-byte swizzled operand as TMA writes it with a 64-element bf16 box: rows of 128 B, 8-row groups 1024 B apart.
+__device__ __forceinline__ uint64_t tfy_wg_desc_sw128(uint32_t smem_addr) {
+    return tfy_wg_desc(smem_addr, 16, 1024, TFY_WG_SW128);
+}
 
 // before the first wgmma that reads / writes accumulator registers other instructions touched
 __device__ __forceinline__ void tfy_wg_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
