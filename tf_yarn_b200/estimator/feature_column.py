@@ -53,7 +53,59 @@ class WeightedCategoricalColumn(NamedTuple):
         return self.categorical_column.hashed
 
 
-Categorical = Union[CategoricalColumn, WeightedCategoricalColumn]
+class BucketizedColumn(NamedTuple):
+    """``tf.feature_column.bucketized_column``: element j of a numeric column of shape (k,) falls in bucket c = the
+    number of boundaries <= x (TF's ``Bucketize``, ``std::upper_bound``), and its id is ``c + j * (len(boundaries) +
+    1)``.  So an example has k ids, all present, and ``num_buckets = k * (len(boundaries) + 1)``.  x and the boundaries
+    are compared in float32 on every path; NaN goes to the last bucket, as ``upper_bound`` puts it."""
+    source_column: NumericColumn
+    boundaries: Tuple[float, ...]
+
+    @property
+    def key(self) -> str:
+        return f"{self.source_column.key}_bucketized"
+
+    @property
+    def num_buckets(self) -> int:
+        return self.source_column.dim * (len(self.boundaries) + 1)
+
+
+CROSS_HASH_KEY = 0xDECAFCAFFE
+MAX_CROSS_BUCKETS = 2 ** 62         # the int64 statement of the unsigned modulo (_umod) holds below it
+_U64 = 2 ** 64
+
+
+class CrossedColumn(NamedTuple):
+    """``tf.feature_column.crossed_column``: the Cartesian product of its leaf keys' ids, hashed into
+    ``hash_bucket_size`` buckets.
+
+    A leaf key is a raw integer feature (a string: its values are used as they are), an identity categorical column
+    (its bucket ids) or a bucketized column.  Example b has, for leaf key k, L_k component values, a negative one
+    being missing.  The cross has ``L = prod L_k`` slots in row-major order (the first key varies slowest).  A slot
+    is present iff all its components are; its id is ``h % hash_bucket_size`` in uint64 arithmetic, with
+    ``h = hash_key`` and then ``h = FingerprintCat64(h, (uint64) v)`` for each component value v in key order::
+
+        FingerprintCat64(a, b): M = 0xc6a4a7935bd1e995
+            r = a ^ M;  r ^= ShiftMix(b * M) * M;  r *= M;  r = ShiftMix(r) * M;  r = ShiftMix(r)
+        ShiftMix(x) = x ^ (x >> 47)                (mod 2^64, logical shift)
+
+    An absent slot is -1.  The formula follows TF's ``SparseCrossHashed``; that the ids are TF's own has not been
+    checked against TF."""
+    keys: Tuple[Union[str, CategoricalColumn, BucketizedColumn], ...]     # the leaf keys, nested crosses flattened
+    hash_bucket_size: int
+    hash_key: int = CROSS_HASH_KEY
+
+    @property
+    def key(self) -> str:
+        return "_X_".join(sorted(k if isinstance(k, str) else k.key for k in self.keys))
+
+    @property
+    def num_buckets(self) -> int:
+        return self.hash_bucket_size
+
+
+Categorical = Union[CategoricalColumn, WeightedCategoricalColumn, BucketizedColumn, CrossedColumn]
+DERIVED = (BucketizedColumn, CrossedColumn)         # columns whose ids are computed from other features
 
 
 class EmbeddingColumn(NamedTuple):
@@ -87,6 +139,41 @@ def weighted_categorical_column(categorical_column: CategoricalColumn, weight_fe
     return WeightedCategoricalColumn(categorical_column, weight_feature_key, dtype)
 
 
+def bucketized_column(source_column: NumericColumn, boundaries: Sequence[float]) -> BucketizedColumn:
+    """Buckets of a numeric column of shape (k,) split at strictly increasing ``boundaries`` (see BucketizedColumn)."""
+    if not isinstance(source_column, NumericColumn) or len(source_column.shape) != 1:
+        raise ValueError(f"bucketized_column needs a numeric column of a 1-D shape, got {source_column!r}")
+    bounds = tuple(float(b) for b in boundaries) if isinstance(boundaries, (list, tuple)) else ()
+    if not bounds or any(a >= b for a, b in zip(bounds, bounds[1:])):
+        raise ValueError(f"bucketized_column: boundaries must be a non-empty, strictly increasing list, "
+                         f"got {boundaries!r}")
+    return BucketizedColumn(source_column, bounds)
+
+
+def crossed_column(keys: Sequence, hash_bucket_size: int, hash_key: Optional[int] = None) -> CrossedColumn:
+    """The hashed cross of ``keys`` (strings, identity categorical, bucketized or crossed columns; see
+    CrossedColumn)."""
+    leaves: List = []
+    for k in keys:
+        if isinstance(k, CrossedColumn):
+            leaves.extend(k.keys)
+        elif isinstance(k, WeightedCategoricalColumn):
+            raise ValueError(f"crossed_column does not support weight_tensor, got {k!r}")
+        elif isinstance(k, CategoricalColumn) and k.hashed:
+            raise ValueError(f"crossed_column does not support a hashed categorical column, got {k!r}; cross its "
+                             f"raw feature {k.key!r} instead")
+        elif isinstance(k, (str, CategoricalColumn, BucketizedColumn)):
+            leaves.append(k)
+        else:
+            raise ValueError(f"crossed_column keys must be feature names, identity categorical, bucketized or "
+                             f"crossed columns, got {k!r}")
+    if len(leaves) < 2:
+        raise ValueError(f"crossed_column needs at least two keys, got {keys!r}")
+    if not 1 <= int(hash_bucket_size) < MAX_CROSS_BUCKETS:
+        raise ValueError(f"crossed_column: hash_bucket_size must be >= 1 and < 2^62, got {hash_bucket_size}")
+    return CrossedColumn(tuple(leaves), int(hash_bucket_size), CROSS_HASH_KEY if hash_key is None else int(hash_key))
+
+
 def _check_combiner(combiner: str) -> str:
     if combiner not in COMBINERS:
         raise ValueError(f"combiner must be one of {COMBINERS}, got {combiner!r}")
@@ -105,7 +192,7 @@ def indicator_column(categorical_column: Categorical) -> IndicatorColumn:
 def _categorical(c) -> Optional[Categorical]:
     """The categorical column a wide-tower column is looked up by (None for a numeric column)."""
     c = c.categorical_column if isinstance(c, (EmbeddingColumn, IndicatorColumn)) else c
-    return c if isinstance(c, (CategoricalColumn, WeightedCategoricalColumn)) else None
+    return c if isinstance(c, (CategoricalColumn, WeightedCategoricalColumn) + DERIVED) else None
 
 
 def _ids(col: Categorical, t: torch.Tensor) -> torch.Tensor:
@@ -118,8 +205,97 @@ def _ids(col: Categorical, t: torch.Tensor) -> torch.Tensor:
     return torch.where(raw < 0, -1, ids % col.num_buckets)
 
 
+def _check_source_width(col: BucketizedColumn, width: int) -> None:
+    """A bucketized column's feature must have the k values per example of its shape: its ids are < k * (n + 1)."""
+    if width != col.source_column.dim:
+        raise ValueError(f"bucketized_column {col.key!r}: feature {col.source_column.key!r} has {width} values "
+                         f"per example, the column's shape {col.source_column.shape}")
+
+
+def _bucketize(col: BucketizedColumn, features: Dict[str, torch.Tensor]) -> torch.Tensor:
+    """[B, k] ids of a bucketized column: bucket c + j * (len(boundaries) + 1), compared in float32, NaN last."""
+    x = features[col.source_column.key]
+    x = x.reshape(x.shape[0], -1).float().contiguous()
+    k, n = col.source_column.dim, len(col.boundaries)
+    _check_source_width(col, x.shape[1])
+    bounds = torch.tensor(col.boundaries, dtype=torch.float32, device=x.device)
+    c = torch.searchsorted(bounds, x, right=True)
+    c = torch.where(torch.isnan(x), n, c)
+    return c + torch.arange(k, device=x.device) * (n + 1)
+
+
+def _shift_mix(x: torch.Tensor) -> torch.Tensor:
+    return x ^ ((x >> 47) & ((1 << 17) - 1))          # logical shift of the uint64 held in an int64
+
+
+def _as_i64(u: int) -> int:
+    """The int64 with the bits of the uint64 u mod 2^64."""
+    return (u % _U64 ^ 2 ** 63) - 2 ** 63
+
+
+_M = _as_i64(0xc6a4a7935bd1e995)
+
+
+def _fingerprint_cat64(a: torch.Tensor, b: torch.Tensor) -> torch.Tensor:
+    """FingerprintCat64 on uint64 values held in int64 tensors (multiplication wraps mod 2^64 either way)."""
+    r = a ^ _M
+    r = r ^ (_shift_mix(b * _M) * _M)
+    r = r * _M
+    r = _shift_mix(r) * _M
+    return _shift_mix(r)
+
+
+def _umod(h: torch.Tensor, n: int) -> torch.Tensor:
+    """(uint64) h % n for the int64 h with the same bits (n < 2^62)."""
+    return torch.where(h < 0, (h % n + _U64 % n) % n, h % n)
+
+
+def _leaf_values(k, features: Dict[str, torch.Tensor]) -> torch.Tensor:
+    """[B, L_k] int64 component values of a cross's leaf key (negative = missing)."""
+    if isinstance(k, str):
+        t = features[k]
+        return t.reshape(t.shape[0], -1).long()
+    if isinstance(k, BucketizedColumn):
+        return _bucketize(k, features)
+    t = features[k.key]
+    return _ids(k, t).reshape(t.shape[0], -1)
+
+
+def _cross(col: CrossedColumn, features: Dict[str, torch.Tensor]) -> torch.Tensor:
+    """[B, prod L_k] ids of a crossed column, -1 where a component is missing."""
+    h = present = None
+    for k in col.keys:
+        v = _leaf_values(k, features)
+        if h is None:
+            h = torch.full(v.shape[:1] + (1,), _as_i64(col.hash_key), dtype=torch.int64, device=v.device)
+            present = torch.ones_like(h, dtype=torch.bool)
+        B = v.shape[0]
+        h = _fingerprint_cat64(h[:, :, None], v[:, None, :]).reshape(B, -1)
+        present = (present[:, :, None] & (v >= 0)[:, None, :]).reshape(B, -1)
+    return torch.where(present, _umod(h, col.hash_bucket_size), -1)
+
+
+def _width(col, features: Dict[str, torch.Tensor]) -> int:
+    """L of a column's (or a cross's leaf key's) [B, L] ids, from the features' shapes alone."""
+    if isinstance(col, str):
+        return features[col][0].numel()
+    if isinstance(col, BucketizedColumn):
+        return col.source_column.dim
+    if isinstance(col, CrossedColumn):
+        n = 1
+        for k in col.keys:
+            n *= _width(k, features)
+        return n
+    return features[col.key][0].numel()
+
+
 def _ids_and_weights(col: Categorical, features: Dict[str, torch.Tensor]):
-    """[B, L] bucket ids (-1 = missing) and, for a weighted column, the [B, L] float weights (else None)."""
+    """[B, L] bucket ids (-1 = missing) and, for a weighted column, the [B, L] float weights (else None).  A bucketized
+    or crossed column computes its ids from the features it is built on."""
+    if isinstance(col, BucketizedColumn):
+        return _bucketize(col, features), None
+    if isinstance(col, CrossedColumn):
+        return _cross(col, features), None
     t = features[col.key]
     ids = _ids(col, t).reshape(t.shape[0], -1)
     if not isinstance(col, WeightedCategoricalColumn):
@@ -167,7 +343,7 @@ class CombinedBag(nn.EmbeddingBag):
 class DenseFeatures(nn.Module):
     """Concatenate numeric / indicator / embedding columns into one dense [batch, width] tensor."""
 
-    def __init__(self, columns: Sequence[Union[NumericColumn, EmbeddingColumn, IndicatorColumn]]):
+    def __init__(self, columns: Sequence[Union[NumericColumn, EmbeddingColumn, IndicatorColumn, BucketizedColumn]]):
         super().__init__()
         self.columns = list(columns)
         self.embeddings = nn.ModuleDict()
@@ -182,6 +358,8 @@ class DenseFeatures(nn.Module):
                 width += c.dimension
             elif isinstance(c, IndicatorColumn):
                 width += c.categorical_column.num_buckets
+            elif isinstance(c, BucketizedColumn):       # TF's dense form: the one-hot of its k ids
+                width += c.num_buckets
             else:
                 raise TypeError(f"{c!r} cannot feed a dense layer; wrap it in embedding_column/indicator_column")
         self.width = width
@@ -198,10 +376,11 @@ class DenseFeatures(nn.Module):
                 parts.append(self.embeddings[c.categorical_column.key](ids, w))
             else:
                 # the count of every bucket in the example, or the sum of its weights for a weighted column
-                ids, w = _ids_and_weights(c.categorical_column, features)
+                cat = c if isinstance(c, BucketizedColumn) else c.categorical_column
+                ids, w = _ids_and_weights(cat, features)
                 present = ids >= 0
                 w = present.float() if w is None else torch.where(present, w.float(), 0.0)
-                parts.append(torch.zeros(ids.shape[0], c.categorical_column.num_buckets, device=ids.device)
+                parts.append(torch.zeros(ids.shape[0], cat.num_buckets, device=ids.device)
                              .scatter_add_(1, ids.clamp(min=0), w))
         dtype = next((p.dtype for p in parts if p.is_floating_point()), torch.float32)
         return torch.cat([p.to(dtype) for p in parts], dim=1)

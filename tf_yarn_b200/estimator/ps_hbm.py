@@ -31,7 +31,9 @@ import torch.nn as nn
 import torch.nn.functional as F
 
 from tf_yarn_b200 import _task_commons
+from tf_yarn_b200.estimator import feature_column as fc
 from tf_yarn_b200.estimator import ps as ps_cpu
+from tf_yarn_b200.ops import features as feature_ids
 from tf_yarn_b200.ops import native
 from tf_yarn_b200.parallel.symm import _RawCudaMemory
 
@@ -468,8 +470,14 @@ class _TableGroup:
         ns = lay.var_slots[first]
         self.s1 = torch.tensor([conn.master_ptr(i, 1) for i in tables_idx], dtype=torch.int64, device=dev) if ns >= 1 else None
         self.s2 = torch.tensor([conn.master_ptr(i, 2) for i in tables_idx], dtype=torch.int64, device=dev) if ns >= 2 else None
-        self.V = cat_cols[0].num_buckets
-        self.same_v = all(c.num_buckets == self.V and c.hashed == cat_cols[0].hashed for c in cat_cols)
+        # a group with a bucketized or crossed column takes every column's ids from tfy_feature_ids (torch on a CPU
+        # tensor), which bounds each column's ids by its own V: its tables may differ in V, and the bag and push
+        # kernels are given the largest
+        self.derived = any(isinstance(c, fc.DERIVED) for c in cat_cols)
+        self.feature_ids = feature_ids.FeatureIds(cat_cols, conn.device) if self.derived else None
+        self.V = max(c.num_buckets for c in cat_cols) if self.derived else cat_cols[0].num_buckets
+        self.same_v = not self.derived and all(c.num_buckets == self.V and c.hashed == cat_cols[0].hashed
+                                               for c in cat_cols)
         h = lay.hypers[first]
         self.h = h
         self.opt = conn.var_opt[first]
@@ -490,14 +498,29 @@ class _TableGroup:
     def one_hot(self, features) -> bool:
         """True when the batch has one id per example in every column ([B] or [B, 1]) and no column is weighted: the
         one-id kernels (K5, tfy_ps_multi_bag) serve it.  Decided from shapes, without a device synchronisation."""
+        if self.derived:                # a cross has prod L_k ids per example, a bucketized column k
+            return not self.weighted and all(fc._width(c, features) == 1 for c in self.cols)
         return not self.weighted and all(features[c.key].reshape(features[c.key].shape[0], -1).shape[1] == 1
                                          for c in self.cols)
 
     def ids_of(self, features) -> torch.Tensor:
         """int64 [T, B] bucket ids of the batch (-1 = missing): ONE hash over the stacked columns (26 separate
         3-kernel hashes were 40 % of the step's device time in the first profile)."""
+        if self.derived:
+            ids = self._derived_ids(features)
+            return ids.reshape(ids.shape[0], -1)
         raw = torch.stack([features[c.key].reshape(-1) for c in self.cols]).long()
         return self._bucket(raw)
+
+    def _derived_ids(self, features) -> torch.Tensor:
+        """int64 [T, B, L] ids of a group with bucketized or crossed columns, padded with -1: one tfy_feature_ids launch
+        (per kFeatMaxCols columns) on CUDA tensors, the columns' torch statement on CPU tensors."""
+        if self.conn.device.type == "cuda":
+            self.conn.account(launches=self.feature_ids.launches)
+            return self.feature_ids(features, self.conn.lib)
+        ids = [fc._ids_and_weights(c, features)[0] for c in self.cols]
+        L = max(i.shape[1] for i in ids)
+        return torch.stack([F.pad(i, (0, L - i.shape[1]), value=-1) for i in ids]).contiguous()
 
     def _bucket(self, raw: torch.Tensor) -> torch.Tensor:
         """feature_column._ids of the stacked columns (the CPU plane's mapping, -1 = missing): one call when the
@@ -511,19 +534,24 @@ class _TableGroup:
         """int64 [T, B, L] bucket ids (-1 = missing), every column padded on the device to the group's largest L with
         -1, and the
         fp32 [T, B, L] weights (1 for an unweighted column) or None when no column is weighted."""
-        from tf_yarn_b200.estimator import feature_column as fc
-        raws = [features[c.key] for c in self.cols]
-        raws = [r.reshape(r.shape[0], -1).long() for r in raws]
-        L = max(r.shape[1] for r in raws)
-        ids = self._bucket(torch.stack([F.pad(r, (0, L - r.shape[1]), value=-1) for r in raws]))
+        if self.derived:
+            ids = self._derived_ids(features)
+            shapes = [(ids.shape[1], fc._width(c, features)) for c in self.cols]
+        else:
+            raws = [features[c.key] for c in self.cols]
+            raws = [r.reshape(r.shape[0], -1).long() for r in raws]
+            L = max(r.shape[1] for r in raws)
+            ids = self._bucket(torch.stack([F.pad(r, (0, L - r.shape[1]), value=-1) for r in raws]))
+            shapes = [r.shape for r in raws]
         if not self.weighted:
             return ids, None
+        L = ids.shape[2]
         ws = []
-        for c, r in zip(self.cols, raws):
+        for c, shape in zip(self.cols, shapes):
             if isinstance(c, fc.WeightedCategoricalColumn):
-                w = fc._weights(c, features, r.shape).float()
+                w = fc._weights(c, features, shape).float()
             else:
-                w = torch.ones(r.shape, dtype=torch.float32, device=r.device)
+                w = torch.ones(shape, dtype=torch.float32, device=ids.device)
             ws.append(F.pad(w, (0, L - w.shape[1])))
         return ids, torch.stack(ws).contiguous()
 
@@ -577,7 +605,7 @@ def _try_fuse_wide_tower(conn: HbmConnection, network: nn.Module) -> bool:
             cat_cols.append(cc)
             tables_idx.append(ti)
     group = _TableGroup(conn, tables_idx, cat_cols)
-    if not (group.uniform and group.same_v):
+    if not (group.uniform and (group.same_v or group.derived)):     # mixed V only with the id kernel's bound
         return False
     units = lin.units
     dev = conn.device
