@@ -114,6 +114,21 @@ class EmbeddingColumn(NamedTuple):
     combiner: str = "mean"
 
 
+class SharedEmbeddingColumn(NamedTuple):
+    """One member of ``tf.feature_column.shared_embedding_columns``: a column whose ids look up the table named
+    ``shared_name``, which every member of the collection shares.
+
+    Each member keeps its own ids, weights and position: in ``DenseFeatures`` it adds ``dimension`` columns where it
+    stands, combined by ``combiner`` over its own ids exactly as an ``embedding_column`` would be.  The table is one
+    ``[num_buckets, dimension]`` parameter, ``embeddings[shared_name]``, created once per ``DenseFeatures`` and
+    initialised as an ``embedding_column``'s; its gradient is the sum of the members' gradients.  Two
+    ``DenseFeatures`` built on the same collection each create their own table."""
+    categorical_column: Categorical
+    dimension: int
+    combiner: str
+    shared_name: str
+
+
 class IndicatorColumn(NamedTuple):
     categorical_column: Categorical
 
@@ -183,6 +198,51 @@ def _check_combiner(combiner: str) -> str:
 def embedding_column(categorical_column: Categorical, dimension: int, combiner: str = "mean",
                      **_ignored) -> EmbeddingColumn:
     return EmbeddingColumn(categorical_column, int(dimension), _check_combiner(combiner))
+
+
+def _kind(c) -> Optional[str]:
+    """What a shared collection's members must agree on: the column type (a weighted column counts as its base
+    column; identity and hashed columns differ), or None for a non-categorical column."""
+    c = c.categorical_column if isinstance(c, WeightedCategoricalColumn) else c
+    if isinstance(c, CategoricalColumn):
+        return "hashed" if c.hashed else "identity"
+    return type(c).__name__ if isinstance(c, DERIVED) else None
+
+
+def shared_embedding_columns(categorical_columns: Sequence[Categorical], dimension: int, combiner: str = "mean",
+                             shared_embedding_collection_name: Optional[str] = None,
+                             **_ignored) -> List[SharedEmbeddingColumn]:
+    """``tf.feature_column.shared_embedding_columns``: one SharedEmbeddingColumn per input, in input order, all
+    looking up one table.  The members must be categorical columns of one kind with one ``num_buckets`` and distinct
+    keys.  The default collection name is TF's: the sorted member keys joined by "_", then "_shared_embedding"."""
+    cols = list(categorical_columns)
+    if not cols:
+        raise ValueError("shared_embedding_columns needs at least one categorical column")
+    for c in cols:
+        if _kind(c) is None:
+            raise ValueError(f"shared_embedding_columns: {c!r} is not a categorical column")
+    if len({_kind(c) for c in cols}) > 1:
+        raise ValueError(f"shared_embedding_columns: all columns must be of one kind, got "
+                         f"{sorted({_kind(c) for c in cols})}")
+    if len({c.num_buckets for c in cols}) > 1:
+        raise ValueError(f"shared_embedding_columns: all columns must have the same num_buckets, got "
+                         f"{[c.num_buckets for c in cols]}")
+    keys = [c.key for c in cols]
+    if len(set(keys)) < len(keys):
+        raise ValueError(f"shared_embedding_columns: a column appears twice, keys {keys}")
+    if int(dimension) < 1:
+        raise ValueError(f"shared_embedding_columns: dimension must be >= 1, got {dimension}")
+    _check_combiner(combiner)
+    name = shared_embedding_collection_name or "_".join(sorted(keys)) + "_shared_embedding"
+    return [SharedEmbeddingColumn(c, int(dimension), combiner, name) for c in cols]
+
+
+shared_embeddings = shared_embedding_columns          # the TF2 name
+
+
+def _embedding_key(c) -> str:
+    """The DenseFeatures.embeddings key of an embedding or shared embedding column."""
+    return c.shared_name if isinstance(c, SharedEmbeddingColumn) else c.categorical_column.key
 
 
 def indicator_column(categorical_column: Categorical) -> IndicatorColumn:
@@ -343,18 +403,41 @@ class CombinedBag(nn.EmbeddingBag):
 class DenseFeatures(nn.Module):
     """Concatenate numeric / indicator / embedding columns into one dense [batch, width] tensor."""
 
-    def __init__(self, columns: Sequence[Union[NumericColumn, EmbeddingColumn, IndicatorColumn, BucketizedColumn]]):
+    def __init__(self, columns: Sequence[Union[NumericColumn, EmbeddingColumn, SharedEmbeddingColumn, IndicatorColumn,
+                                               BucketizedColumn]]):
         super().__init__()
         self.columns = list(columns)
         self.embeddings = nn.ModuleDict()
+        # shared name -> positions of its members in self.columns
+        self.shared: Dict[str, List[int]] = {}
         width = 0
-        for c in self.columns:
+        for pos, c in enumerate(self.columns):
             if isinstance(c, NumericColumn):
                 width += c.dim
             elif isinstance(c, EmbeddingColumn):
+                if c.categorical_column.key in self.shared:
+                    raise ValueError(f"embedding column {c.categorical_column.key!r} has the name of a shared "
+                                     f"embedding collection")
                 emb = CombinedBag(c.categorical_column.num_buckets, c.dimension, c.combiner)
                 nn.init.normal_(emb.weight, std=1.0 / c.dimension ** 0.5)
                 self.embeddings[c.categorical_column.key] = emb
+                width += c.dimension
+            elif isinstance(c, SharedEmbeddingColumn):
+                name = c.shared_name
+                if name in self.shared:
+                    first = self.columns[self.shared[name][0]]
+                    if (first.categorical_column.num_buckets, first.dimension, first.combiner) != \
+                            (c.categorical_column.num_buckets, c.dimension, c.combiner):
+                        raise ValueError(f"shared embedding collection {name!r}: members disagree on num_buckets, "
+                                         f"dimension or combiner: {first!r} and {c!r}")
+                    self.shared[name].append(pos)
+                else:
+                    if name in self.embeddings:
+                        raise ValueError(f"shared embedding collection {name!r} has the name of another embedding")
+                    emb = CombinedBag(c.categorical_column.num_buckets, c.dimension, c.combiner)
+                    nn.init.normal_(emb.weight, std=1.0 / c.dimension ** 0.5)
+                    self.embeddings[name] = emb
+                    self.shared[name] = [pos]
                 width += c.dimension
             elif isinstance(c, IndicatorColumn):
                 width += c.categorical_column.num_buckets
@@ -364,13 +447,24 @@ class DenseFeatures(nn.Module):
                 raise TypeError(f"{c!r} cannot feed a dense layer; wrap it in embedding_column/indicator_column")
         self.width = width
 
+    def shared_lookup(self, name: str, features: Dict[str, torch.Tensor]) -> List[torch.Tensor]:
+        """The [B, dimension] values of the members of collection ``name``, in column order.  The HBM parameter server
+        replaces it on the instance with one bag and one push for the whole collection."""
+        emb = self.embeddings[name]
+        return [emb(*_ids_and_weights(self.columns[p].categorical_column, features)) for p in self.shared[name]]
+
     def forward(self, features: Dict[str, torch.Tensor]) -> torch.Tensor:
         parts: List[torch.Tensor] = []
         ref = None
-        for c in self.columns:
+        shared = {}
+        for name, positions in self.shared.items():
+            shared.update(zip(positions, self.shared_lookup(name, features)))
+        for pos, c in enumerate(self.columns):
             if isinstance(c, NumericColumn):
                 t = features[c.key]
                 parts.append(t.reshape(t.shape[0], -1))
+            elif isinstance(c, SharedEmbeddingColumn):
+                parts.append(shared[pos])
             elif isinstance(c, EmbeddingColumn):
                 ids, w = _ids_and_weights(c.categorical_column, features)
                 parts.append(self.embeddings[c.categorical_column.key](ids, w))
@@ -397,6 +491,9 @@ class LinearModel(nn.Module):
         self.columns = list(columns)
         self.units = units
         self.sparse_combiner = _check_combiner(sparse_combiner)
+        for c in self.columns:
+            if isinstance(c, SharedEmbeddingColumn):
+                raise ValueError(f"a linear model does not take shared embedding columns, got {c!r}")
         n_numeric = sum(c.dim for c in self.columns if isinstance(c, NumericColumn))
         self.numeric = nn.Linear(n_numeric, units, bias=False) if n_numeric else None
         if self.numeric is not None:

@@ -56,6 +56,8 @@ native.declare("tfy_ps_multi_bag_weighted", [_vp, _vp, _vp, _i, _i, _i, _i, _i, 
                                              _vp])
 native.declare("tfy_ps_multi_push_rows_weighted", [_vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _ll, _i, _f, _f, _f, _f, _f,
                                                    _f, _vp, _i, _i, _i, _vp, _vp, _i, _vp, _sz, _vp])
+native.declare("tfy_ps_multi_push_rows_shared", [_vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _ll, _i, _f, _f, _f, _f, _f,
+                                                 _f, _vp, _i, _i, _i, _vp, _vp, _i, _i, _vp, _i, _vp, _sz, _vp])
 
 OPT_CODES = {"sgd": native.OPT_SGD, "adagrad": native.OPT_ADAGRAD, "adam": native.OPT_ADAM,
              "ftrl": native.OPT_FTRL}
@@ -71,11 +73,16 @@ class PsSeg(ctypes.Structure):
                 ("cols", ctypes.c_uint32), ("shadow_ld", ctypes.c_uint32)]
 
 
-def push_rows_launches(per_table: int) -> int:
-    """Kernel launches of one sparse push of `per_table` ids per table: a per-table block sort (up to 2048 ids per
+def push_rows_launches(per_table: int, max_members: int = 0) -> int:
+    """Kernel launches of one sparse push of `per_table` ids per column: a per-table block sort (up to 2048 ids per
     table, tfy_ps.cu kPsBlockSortMax) or the key kernel and CUB's device radix sort (histogram, scan and one kernel
-    per 8-bit pass, counted here as one launch), then the short-run and long-run apply kernels."""
-    return 3 if per_table <= 2048 else 4
+    per 8-bit pass, counted here as one launch), then the short-run and long-run apply kernels.  A shared push
+    (tfy_ps_multi_push_rows_shared, max_members > 0 = the most columns any one table has) takes the block sort when
+    max_members * per_table <= 2048, and runs one more kernel: the per-occurrence gradient offsets, which also write
+    a weighted push's factors."""
+    if not max_members:
+        return 3 if per_table <= 2048 else 4
+    return (3 if per_table * max_members <= 2048 else 4) + 1
 
 
 def push_rows_scratch(lib, n: int, device) -> torch.Tensor:
@@ -254,6 +261,8 @@ class HbmConnection:
             mod.forward = _make_linear_forward(conn, idx, mod)
         self.fused_first = _try_fuse_first_layer(conn, network)
         self.fused_wide = _try_fuse_wide_tower(conn, network)
+        self.shared_collections = _serve_shared_collections(
+            conn, network, k5_features=getattr(network, "dense_features", None) if self.fused_first else None)
 
     # ------------------------------------------------------------------ pull / push
     def pull(self, network: nn.Module) -> None:
@@ -458,7 +467,10 @@ def _make_linear_forward(conn: HbmConnection, idx: int, mod: nn.Linear):
 
 
 class _TableGroup:
-    """T embedding tables of one tower served by the multi-table kernels (one launch for the whole group)."""
+    """T embedding columns of one tower served by the multi-table kernels (one launch for the whole group).  Column t
+    looks up the table tables_idx[t]; columns of a shared embedding collection repeat their table.  This is the one
+    place that knows the column -> table map: a group whose columns share tables pushes through
+    tfy_ps_multi_push_rows_shared, so that each distinct (table, row) is folded and applied once per push."""
 
     def __init__(self, conn: HbmConnection, tables_idx: List[int], cat_cols):
         lay = conn.layout
@@ -466,10 +478,25 @@ class _TableGroup:
         first = tables_idx[0]
         self.uniform = all(lay.kinds[i] == lay.kinds[first] and lay.hypers[i] == lay.hypers[first] for i in tables_idx)
         dev = conn.device
-        self.tables = torch.tensor([conn.master_ptr(i) for i in tables_idx], dtype=torch.int64, device=dev)
         ns = lay.var_slots[first]
-        self.s1 = torch.tensor([conn.master_ptr(i, 1) for i in tables_idx], dtype=torch.int64, device=dev) if ns >= 1 else None
-        self.s2 = torch.tensor([conn.master_ptr(i, 2) for i in tables_idx], dtype=torch.int64, device=dev) if ns >= 2 else None
+
+        def ptrs(idx, slot):
+            return torch.tensor([conn.master_ptr(i, slot) for i in idx], dtype=torch.int64, device=dev)
+        # per column: the bags and K5's gather read tables[t]
+        self.tables = ptrs(tables_idx, 0)
+        self.s1 = ptrs(tables_idx, 1) if ns >= 1 else None
+        self.s2 = ptrs(tables_idx, 2) if ns >= 2 else None
+        # per distinct table: the shared push's {w, s1, s2} arrays and table_of[t], the index of column t's table.
+        # Built from the distinct tables in order of first use, the map meets the kernel's preconditions by
+        # construction: every value in [0, n_tables), every table named, none by more than max_members columns.
+        self.distinct = list(dict.fromkeys(tables_idx))
+        if self.shared:
+            table_of = [self.distinct.index(i) for i in tables_idx]
+            self.table_of = torch.tensor(table_of, dtype=torch.int32, device=dev)
+            self.push_tables = ptrs(self.distinct, 0)
+            self.push_s1 = ptrs(self.distinct, 1) if ns >= 1 else None
+            self.push_s2 = ptrs(self.distinct, 2) if ns >= 2 else None
+            self.max_members = max(table_of.count(k) for k in range(len(self.distinct)))
         # a group with a bucketized or crossed column takes every column's ids from tfy_feature_ids (torch on a CPU
         # tensor), which bounds each column's ids by its own V: its tables may differ in V, and the bag and push
         # kernels are given the largest
@@ -483,6 +510,11 @@ class _TableGroup:
         self.opt = conn.var_opt[first]
         self.p3 = float(h["eps"]) if lay.kinds[first] == "ftrl" else 0.0
         self.slots = ns
+
+    @property
+    def shared(self) -> bool:
+        """True when columns share tables: the group then pushes through tfy_ps_multi_push_rows_shared."""
+        return len(set(self.idx)) < len(self.idx)
 
     @classmethod
     def single(cls, conn: HbmConnection, idx: int, V: int) -> "_TableGroup":
@@ -555,9 +587,36 @@ class _TableGroup:
             ws.append(F.pad(w, (0, L - w.shape[1])))
         return ids, torch.stack(ws).contiguous()
 
+    def split(self):
+        """(member columns, group) per distinct table: a mixed-optimizer group pushes table by table."""
+        out = []
+        for ti in self.distinct:
+            members = [t for t, i in enumerate(self.idx) if i == ti]
+            out.append((members, _TableGroup(self.conn, [ti] * len(members), [self.cols[t] for t in members])))
+        return out
+
+    def push_shared(self, ids: torch.Tensor, weights: Optional[torch.Tensor], f: Optional[torch.Tensor], combiner: int,
+                    dout: torch.Tensor, D: int, dout_ld: int, col_stride: int) -> None:
+        """tfy_ps_multi_push_rows_shared: ids / weights [T, B, L] (or ids [T, B]), f [T, B] or None."""
+        conn, h = self.conn, self.h
+        T, B = ids.shape[:2]
+        L = ids.shape[2] if ids.dim() == 3 else 1
+        scratch = push_rows_scratch(conn.lib, T * B * L, dout.device)
+        native.check(conn.lib.tfy_ps_multi_push_rows_shared(
+            self.push_tables.data_ptr(), _ptr(self.push_s1), _ptr(self.push_s2), ids.data_ptr(), dout.data_ptr(),
+            1 if dout.dtype == torch.bfloat16 else 0, B, T, D, self.V, self.opt, float(h["lr"]), float(h["eps"]),
+            float(h["p1"]), float(h["p2"]), self.p3, 1.0, conn.adam_scale.data_ptr(), dout_ld, col_stride, L,
+            _ptr(weights), _ptr(f), combiner, len(self.distinct), self.table_of.data_ptr(), self.max_members,
+            scratch.data_ptr(), scratch.numel(), torch.cuda.current_stream().cuda_stream),
+            "tfy_ps_multi_push_rows_shared")
+        # the rows written are those of the distinct tables; the occurrences read are every column's
+        conn.account(push=T * B * L * D * 4 * (1 + self.slots), launches=push_rows_launches(B * L, self.max_members))
+
     def push_weighted(self, ids: torch.Tensor, weights: Optional[torch.Tensor], f: torch.Tensor, combiner: int,
                       dout: torch.Tensor, D: int, dout_ld: int, col_stride: int) -> None:
         """tfy_ps_multi_push_rows_weighted of a weighted bag's backward: ids / weights [T, B, L], f [T, B]."""
+        if self.shared:
+            return self.push_shared(ids, weights, f, combiner, dout, D, dout_ld, col_stride)
         conn, h = self.conn, self.h
         T, B, L = ids.shape
         scratch = push_rows_scratch(conn.lib, T * B * L, dout.device)
@@ -571,6 +630,8 @@ class _TableGroup:
         conn.account(push=T * B * L * D * 4 * (1 + self.slots), launches=push_rows_launches(B * L) + 1)
 
     def push(self, ids: torch.Tensor, dout: torch.Tensor, D: int, dout_ld: int, col_stride: int) -> None:
+        if self.shared:
+            return self.push_shared(ids, None, None, COMBINER_CODES["sum"], dout, D, dout_ld, col_stride)
         conn, h = self.conn, self.h
         B, T = ids.shape[1], len(self.idx)
         scratch = push_rows_scratch(conn.lib, T * B, dout.device)
@@ -666,6 +727,66 @@ def _try_fuse_wide_tower(conn: HbmConnection, network: nn.Module) -> bool:
     return True
 
 
+def _serve_shared_collections(conn: HbmConnection, network: nn.Module, k5_features=None) -> int:
+    """Shared embedding collections of a DenseFeatures that K5 does not serve: one weighted bag launch for all the
+    members of a collection (T = members, the table repeated, into a [B, C*D] buffer sliced to their positions) and
+    one shared push in its backward, instead of one bag and one push per member.  k5_features is the DenseFeatures
+    whose forward K5 replaced (its collections are pushed by K5's backward).  Returns the collections served."""
+    from tf_yarn_b200.estimator import feature_column as fc
+    by_param = {id(p): i for i, p in enumerate(conn.params)}
+    served = 0
+    for df in network.modules():
+        if not isinstance(df, fc.DenseFeatures) or not df.shared or df is k5_features:
+            continue
+        lookups = {}
+        for name, positions in df.shared.items():
+            emb = df.embeddings[name]
+            ti = by_param.get(id(emb.weight))
+            if ti is None or ti not in conn.sparse or not isinstance(emb, fc.CombinedBag):
+                continue
+            lookups[name] = _shared_lookup(conn, ti, [df.columns[p] for p in positions])
+        if lookups:
+            default = df.shared_lookup
+
+            def shared_lookup(name, features, lookups=lookups, default=default):
+                return lookups[name](features) if name in lookups else default(name, features)
+            df.shared_lookup = shared_lookup
+            served += len(lookups)
+    return served
+
+
+def _shared_lookup(conn: HbmConnection, ti: int, members):
+    """One collection's lookup: the members' [B, D] values from one tfy_ps_multi_bag_weighted launch, and one push of
+    the table for all of them."""
+    C, D = len(members), members[0].dimension
+    code = COMBINER_CODES[members[0].combiner]
+    group = _TableGroup(conn, [ti] * C, [c.categorical_column for c in members])
+    dev = conn.device
+
+    class _SharedBag(torch.autograd.Function):
+        @staticmethod
+        def forward(ctx, ids, weights, anchor):
+            _, B, L = ids.shape
+            out = torch.empty((B, C * D), dtype=torch.float32, device=dev)
+            f = torch.empty((C, B), dtype=torch.float32, device=dev)
+            weighted_bag(conn.lib, group.tables, ids, weights, code, D, group.V, out, C * D, D, f)
+            conn.account(pull=C * B * L * D * 4)
+            ctx.ids, ctx.weights, ctx.f = ids, weights, f
+            return out
+
+        @staticmethod
+        def backward(ctx, dout):
+            group.push_weighted(ctx.ids, ctx.weights, ctx.f, code, dout.contiguous().float(), D, C * D, D)
+            return None, None, None
+
+    anchor = torch.zeros((), device=dev, requires_grad=True)
+
+    def lookup(features):
+        out = _SharedBag.apply(*group.multi_of(features), anchor)
+        return [out[:, D * k:D * k + D] for k in range(C)]
+    return lookup
+
+
 def _try_fuse_first_layer(conn: HbmConnection, network: nn.Module) -> bool:
     """K5: fuse the sparse pull of the embedding rows INTO the first deep GEMM (ops/csrc/tfy_ps_gemm.cu).
 
@@ -688,7 +809,7 @@ def _try_fuse_first_layer(conn: HbmConnection, network: nn.Module) -> bool:
         return False
     emb_cols, num_cols, seen_numeric = [], [], False
     for c in df.columns:
-        if isinstance(c, fc.EmbeddingColumn) and not seen_numeric and c.dimension == 64:
+        if isinstance(c, (fc.EmbeddingColumn, fc.SharedEmbeddingColumn)) and not seen_numeric and c.dimension == 64:
             emb_cols.append(c)
         elif isinstance(c, fc.NumericColumn):
             seen_numeric = True
@@ -700,7 +821,7 @@ def _try_fuse_first_layer(conn: HbmConnection, network: nn.Module) -> bool:
         return False
     tables_idx = []
     for c in emb_cols:
-        emb = df.embeddings[c.categorical_column.key]
+        emb = df.embeddings[fc._embedding_key(c)]
         ti = by_param.get(id(emb.weight))
         if ti is None or ti not in conn.sparse or not isinstance(emb, fc.CombinedBag):
             return False
@@ -719,8 +840,12 @@ def _try_fuse_first_layer(conn: HbmConnection, network: nn.Module) -> bool:
     codes = [COMBINER_CODES[c.combiner] for c in emb_cols]
     one_code = len(set(codes)) == 1
     push_code = COMBINER_CODES["mean"]
-    # tables of mixed optimizers push one by one: {w, s1, s2} pointers of each, for a T = 1 weighted push
-    singles = None if group.uniform else [_TableGroup.single(conn, ti, V) for ti in tables_idx]
+    # tables of mixed optimizers push one by one, each with its own member columns (one, unless the table is shared)
+    per_table = None if group.uniform else group.split()
+
+    def members_dx(dx, members):
+        """The members' 64-column slices of dx side by side, for the push of a shared table."""
+        return torch.cat([dx[:, 64 * t:64 * t + 64] for t in members], dim=1)
 
     def first_backward(xbuf, dy, weight, push):
         """dW and dx in one wgmma kernel against the remote shadow, then push(dx) of the embedding rows."""
@@ -760,7 +885,12 @@ def _try_fuse_first_layer(conn: HbmConnection, network: nn.Module) -> bool:
                     # table t takes columns [64 t, 64 t + 64) of dx: ONE launch for all tables, straight out of dx
                     group.push(ids, dx, 64, Kp, 64)
                     return
-                for t, ti in enumerate(tables_idx):          # (mixed optimizers) table by table
+                for members, sub in per_table:               # (mixed optimizers) table by table
+                    if sub.shared:
+                        sub.push(ids[members].contiguous(), members_dx(dx, members), 64, 64 * len(members), 64)
+                        continue
+                    t = members[0]
+                    ti = tables_idx[t]
                     h = lay.hypers[ti]
                     s1 = conn.master_ptr(ti, 1) if lay.var_slots[ti] >= 1 else None
                     s2 = conn.master_ptr(ti, 2) if lay.var_slots[ti] >= 2 else None
@@ -806,8 +936,14 @@ def _try_fuse_first_layer(conn: HbmConnection, network: nn.Module) -> bool:
                 if group.uniform:
                     group.push_weighted(ids, w, f, push_code, dx, 64, Kp, 64)
                     return
-                for t, one in enumerate(singles):           # (mixed optimizers) table by table
-                    one.push_weighted(ids[t:t + 1], w[t:t + 1] if w is not None else None, f[t:t + 1], push_code,
+                for members, sub in per_table:              # (mixed optimizers) table by table
+                    if sub.shared:
+                        sub.push_weighted(ids[members].contiguous(), w[members].contiguous() if w is not None else None,
+                                          f[members].contiguous(), push_code, members_dx(dx, members), 64,
+                                          64 * len(members), 64)
+                        continue
+                    t = members[0]
+                    sub.push_weighted(ids[t:t + 1], w[t:t + 1] if w is not None else None, f[t:t + 1], push_code,
                                       dx[:, 64 * t:], 64, Kp, 0)
             dw, db = first_backward(xbuf, dy, weight, push)
             return None, None, None, dw, db

@@ -339,6 +339,18 @@ struct TfyPsRows {
     float scale;             // grad_scale (x 1/L for a mean bag), applied to the folded sum
 };
 
+// Column -> table map of a shared push (tfy_ps_multi_push_rows_shared): the rows of column t live in table
+// table_of[t] of n_tables distinct tables, and TfyPsRows' arrays hold those n_tables tables.  The key of an
+// occurrence becomes table_of[t] * V + id, so two columns of one table fold into one run per row; its gradient still
+// comes from its own column.  Preconditions (the caller's map guarantees them): 0 <= table_of[t] < n_tables, every
+// table has at least one column and none has more than max_members.  The unmapped instantiations (M = false) take
+// the map as a trailing argument and ignore it.
+struct TfyPsMap {
+    const int* table_of;
+    int T, n_tables;
+    int max_members;         // the most columns any one table has (1 unmapped): chooses the block sort on the host
+};
+
 namespace {
 __device__ __forceinline__ float* rows_base(const uint64_t* arr, float* one, int t) {
     return arr ? reinterpret_cast<float*>(arr[t]) : one;
@@ -353,16 +365,19 @@ __device__ __forceinline__ float4 ld_grad(const GT* p) {
 // Weighted pushes (W = true) take two more arrays, nullptr meaning "all ones": wts [T, B, L], the weight of every
 // occurrence, and fs [T, B], the bag's per-example factor 1/den.  A zero-weight occurrence is absent: it gets the
 // sentinel key like an out-of-range id, so it touches no row.  The unweighted instantiations ignore both.
-// keys[o] = t * V + id, or T * V (sorts last, never applied) for an absent occurrence; occ[o] = o
-template <bool W>
+// keys[o] = t * V + id, or T * V (sorts last, never applied) for an absent occurrence; occ[o] = o.  Mapped (M):
+// table_of[t] * V + id, sentinel n_tables * V.
+template <bool W, bool M>
 __global__ void __launch_bounds__(256)
 tfy_ps_row_keys_kernel(const long long* __restrict__ ids, int n, int per_table, long long V,
-                       unsigned long long* __restrict__ keys, int* __restrict__ occ, const float* __restrict__ wts) {
-    const unsigned long long sentinel = (unsigned long long)(n / per_table) * (unsigned long long)V;
+                       unsigned long long* __restrict__ keys, int* __restrict__ occ, const float* __restrict__ wts,
+                       TfyPsMap m) {
+    const unsigned long long sentinel = (unsigned long long)(M ? m.n_tables : n / per_table) * (unsigned long long)V;
     for (int o = blockIdx.x * blockDim.x + threadIdx.x; o < n; o += gridDim.x * blockDim.x) {
         const long long id = ids[o];
         keys[o] = (id < 0 || id >= V || (W && wts && wts[o] == 0.f))
-                      ? sentinel : (unsigned long long)(o / per_table) * (unsigned long long)V + id;
+                      ? sentinel
+                      : (unsigned long long)(M ? m.table_of[o / per_table] : o / per_table) * (unsigned long long)V + id;
         occ[o] = o;
     }
 }
@@ -371,35 +386,75 @@ tfy_ps_row_keys_kernel(const long long* __restrict__ ids, int n, int per_table, 
 // segment t in shared memory.  The segments are in table order, so the concatenation is sorted by (table, id) too,
 // except that a segment's out-of-range ids (the sentinel) sit at its end instead of the array's: the apply kernels
 // skip sentinels wherever they are.  One launch instead of a key kernel plus a multi-pass device sort.
+// Mapped (M): block t is table t.  It sorts the concatenation of its columns' segments (in column order, so equal ids
+// stay in (column, b, j) order) and writes it after the segments of the columns of tables < t.
 constexpr int kPsSortThreads = 256, kPsSortItems = 8, kPsBlockSortMax = kPsSortThreads * kPsSortItems;
 
-template <bool W>
+template <bool W, bool M>
 __global__ void __launch_bounds__(kPsSortThreads)
 tfy_ps_segment_sort_kernel(const long long* __restrict__ ids, int per_table, long long V, int local_bits,
-                           unsigned long long* __restrict__ keys, int* __restrict__ occ, const float* __restrict__ wts) {
+                           unsigned long long* __restrict__ keys, int* __restrict__ occ, const float* __restrict__ wts,
+                           TfyPsMap m) {
     using Sort = cub::BlockRadixSort<unsigned int, kPsSortThreads, kPsSortItems, int>;
     __shared__ typename Sort::TempStorage tmp;
     const int t = blockIdx.x;
-    const size_t base = (size_t)t * per_table;
+    size_t base = (size_t)t * per_table;
+    int n_items = per_table;
+    const int* cols = nullptr;
+    if constexpr (M) {
+        __shared__ int s_cols[kPsBlockSortMax];                      // the columns of table t, in column order
+        __shared__ int s_n, s_before;
+        if (threadIdx.x < 32) {
+            const int lane = threadIdx.x;
+            int n = 0, before = 0;
+            for (int c0 = 0; c0 < m.T; c0 += 32) {
+                const int c = c0 + lane;
+                const int tc = c < m.T ? m.table_of[c] : -1;
+                const unsigned mine = __ballot_sync(0xffffffffu, tc == t);
+                const int k = n + __popc(mine & ((1u << lane) - 1u));
+                if (tc == t && k < kPsBlockSortMax) s_cols[k] = c;
+                n += __popc(mine);
+                before += __popc(__ballot_sync(0xffffffffu, tc >= 0 && tc < t));
+            }
+            if (lane == 0) { s_n = n; s_before = before; }
+        }
+        __syncthreads();
+        cols = s_cols;
+        n_items = s_n * per_table;
+        base = (size_t)s_before * per_table;
+        // more columns than max_members promised: leave the table out rather than let the apply kernels read the
+        // scratch's stale keys at the positions the block cannot hold
+        if (n_items > kPsBlockSortMax) {
+            const unsigned long long sentinel = (unsigned long long)gridDim.x * (unsigned long long)V;
+            for (int r = threadIdx.x; r < n_items; r += kPsSortThreads) {
+                keys[base + r] = sentinel;
+                occ[base + r] = (int)base + r;
+            }
+            return;
+        }
+    }
     const unsigned long long sentinel = (unsigned long long)gridDim.x * (unsigned long long)V;
     unsigned int k[kPsSortItems];
     int v[kPsSortItems];
 #pragma unroll
     for (int j = 0; j < kPsSortItems; ++j) {
         const int r = threadIdx.x * kPsSortItems + j;               // blocked arrangement: r keeps the original order
-        if (r < per_table) {
-            const long long id = ids[base + r];
-            k[j] = (id < 0 || id >= V || (W && wts && wts[base + r] == 0.f)) ? (unsigned int)V : (unsigned int)id;
+        // occurrence of item r: base + r, or (mapped) position r % per_table of the (r / per_table)-th column
+        const int o = M ? cols[r < n_items ? r / per_table : 0] * per_table + r % per_table : 0;
+        if (r < n_items) {
+            const long long id = M ? ids[o] : ids[base + r];
+            k[j] = (id < 0 || id >= V || (W && wts && (M ? wts[o] : wts[base + r]) == 0.f)) ? (unsigned int)V
+                                                                                          : (unsigned int)id;
         } else {
             k[j] = 0xffffffffu;                                      // padding: after every real key
         }
-        v[j] = (int)base + r;
+        v[j] = M ? o : (int)base + r;
     }
     Sort(tmp).Sort(k, v, 0, local_bits);
 #pragma unroll
     for (int j = 0; j < kPsSortItems; ++j) {
         const int r = threadIdx.x * kPsSortItems + j;
-        if (r < per_table) {
+        if (r < n_items) {
             keys[base + r] = k[j] == (unsigned int)V ? sentinel : (unsigned long long)t * (unsigned long long)V + k[j];
             occ[base + r] = v[j];
         }
@@ -459,13 +514,16 @@ __device__ __forceinline__ void apply_sum(const TfyPsHyper& h, const RowRef& x, 
 }
 }  // namespace
 
-template <typename GT, int VEC, bool W>
+// Mapped (M): a key's table is table_of[t] of its occurrences' columns t, and each occurrence's gradient is read from
+// its own column t.  occ and cs are then in sorted order, occ[q] being the element offset of the gradient row of the
+// q-th sorted occurrence in dout (tfy_ps_occ_offsets_kernel): no division by B*L in the apply loops.
+template <typename GT, int VEC, bool W, bool M>
 __global__ void __launch_bounds__(256)
 tfy_ps_apply_short_rows_kernel(TfyPsRows r, TfyPsHyper h, const float* __restrict__ adam_scale,
                                const unsigned long long* __restrict__ keys, const int* __restrict__ occ, int n,
-                               const float* __restrict__ cs) {
+                               const float* __restrict__ cs, TfyPsMap m) {
     const int DV = r.D / VEC, BL = r.B * r.L;
-    const unsigned long long sentinel = (unsigned long long)r.T * (unsigned long long)r.V;
+    const unsigned long long sentinel = (unsigned long long)(M ? m.n_tables : r.T) * (unsigned long long)r.V;
     float vs;
     const float lr = ps_adam_lr(h.opt, h.lr, adam_scale, vs);
     const GT* dout = reinterpret_cast<const GT*>(r.dout);
@@ -482,22 +540,26 @@ tfy_ps_apply_short_rows_kernel(TfyPsRows r, TfyPsHyper h, const float* __restric
         float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
         for (int q = p; q < e; ++q) {
             const int o = occ[q], b = (o % BL) / r.L;
-            acc_occ<W>(acc, ld_grad<GT, VEC>(g + (size_t)b * r.dout_ld), cs, o);
+            const GT* go = M ? dout + o + c * VEC : g + (size_t)b * r.dout_ld;
+            acc_occ<W>(acc, ld_grad<GT, VEC>(go), cs, M ? q : o);
         }
         apply_sum<VEC>(h, x, (size_t)c * VEC, acc, r.scale, lr, vs);
     }
 }
 
-template <typename GT, int VEC, bool W>
-__global__ void __launch_bounds__(256)
+// The mapped instantiations carry a minimum-blocks hint of 1 (no constraint at 256 threads).  Without it ptxas held
+// the scalar (VEC = 1) ones to 40 registers and spilled 16 bytes around the optimizer's division calls; with it they
+// take 48 and do not spill.  The unmapped instantiations keep the plain bound and their code.
+template <typename GT, int VEC, bool W, bool M>
+__global__ void __launch_bounds__(256, M ? 1 : 0)
 tfy_ps_apply_long_rows_kernel(TfyPsRows r, TfyPsHyper h, const float* __restrict__ adam_scale,
                               const unsigned long long* __restrict__ keys, const int* __restrict__ occ, int n,
-                              int cl_log2, const float* __restrict__ cs) {
+                              int cl_log2, const float* __restrict__ cs, TfyPsMap m) {
     const int lane = threadIdx.x & 31;
     const int CL = 1 << cl_log2, OL = 32 >> cl_log2;
     const int cl = lane & (CL - 1), ol = lane >> cl_log2;
     const int DV = r.D / VEC, BL = r.B * r.L;
-    const unsigned long long sentinel = (unsigned long long)r.T * (unsigned long long)r.V;
+    const unsigned long long sentinel = (unsigned long long)(M ? m.n_tables : r.T) * (unsigned long long)r.V;
     float vs;
     const float lr = ps_adam_lr(h.opt, h.lr, adam_scale, vs);
     const GT* dout = reinterpret_cast<const GT*>(r.dout);
@@ -532,7 +594,8 @@ tfy_ps_apply_long_rows_kernel(TfyPsRows r, TfyPsHyper h, const float* __restrict
                 if (c < DV)
                     for (int q = p0 + ol; q < e; q += OL) {
                         const int o = occ[q], b = (o % BL) / r.L;
-                        acc_occ<W>(acc, ld_grad<GT, VEC>(g + (size_t)b * r.dout_ld + c * VEC), cs, o);
+                        const GT* go = M ? dout + o : g + (size_t)b * r.dout_ld;
+                        acc_occ<W>(acc, ld_grad<GT, VEC>(go + c * VEC), cs, M ? q : o);
                     }
                 for (int off = 16; off >= CL; off >>= 1) {
                     acc.x += __shfl_xor_sync(0xffffffffu, acc.x, off);
@@ -557,6 +620,21 @@ tfy_ps_occ_factors_kernel(const float* __restrict__ wts, const float* __restrict
         cs[o] = (wts ? wts[o] : 1.f) * (fs ? fs[(o / BL) * B + (o % BL) / L] : 1.f);
 }
 
+// Mapped pushes, in sorted order: for the q-th sorted occurrence o = occ[q] = (t, b, j), goff[q] = t * col_stride +
+// b * dout_ld and (weighted) cs[q] = w_o * f[t, b]
+template <bool W>
+__global__ void __launch_bounds__(256)
+tfy_ps_occ_offsets_kernel(const int* __restrict__ occ, const float* __restrict__ wts, const float* __restrict__ fs,
+                          int n, int B, int L, int dout_ld, int col_stride, int* __restrict__ goff,
+                          float* __restrict__ cs) {
+    const int BL = B * L;
+    for (int q = blockIdx.x * blockDim.x + threadIdx.x; q < n; q += gridDim.x * blockDim.x) {
+        const int o = occ[q], t = o / BL, b = (o % BL) / L;
+        goff[q] = t * col_stride + b * dout_ld;
+        if (W) cs[q] = (wts ? wts[o] : 1.f) * (fs ? fs[t * B + b] : 1.f);
+    }
+}
+
 namespace {
 
 constexpr long long kPsRowsMaxOcc = 1LL << 30;
@@ -575,15 +653,17 @@ size_t rows_sort_temp_bytes(int n, int end_bit) {
 size_t rows_scratch_fixed(int n) { return 2 * align256((size_t)n * 8) + 2 * align256((size_t)n * 4); }
 
 // Fold + apply of one sparse push: key build, stable radix sort, apply of the short and of the long runs.
-// weighted: take the W = true kernels, with occurrence weights wts and per-example factors fs (either may be nullptr).
-int ps_push_rows_launch(const TfyPsRows& r, const TfyPsHyper& h, const float* adam_scale, int grad_is_bf16,
-                        void* scratch, size_t scratch_bytes, cudaStream_t s, bool weighted = false,
-                        const float* wts = nullptr, const float* fs = nullptr) {
+// W: the weighted kernels, with occurrence weights wts and per-example factors fs (either may be nullptr).
+// M: the mapped kernels of a shared push, with the column -> table map m (m.T == r.T).
+template <bool W, bool M>
+int ps_push_rows_fold(const TfyPsRows& r, const TfyPsHyper& h, const float* adam_scale, int grad_is_bf16,
+                      void* scratch, size_t scratch_bytes, cudaStream_t s, const float* wts, const float* fs,
+                      const TfyPsMap& m) {
     const long long n_ll = (long long)r.T * r.B * r.L;
     if (n_ll == 0) return 0;
     if (n_ll < 0 || n_ll > kPsRowsMaxOcc || r.D < 1 || r.V < 1) return -2;
     const int n = (int)n_ll;
-    const unsigned long long sentinel = (unsigned long long)r.T * (unsigned long long)r.V;
+    const unsigned long long sentinel = (unsigned long long)m.n_tables * (unsigned long long)r.V;
     const int end_bit = 64 - __builtin_clzll(sentinel);            // enough bits for every key, the sentinel included
     const size_t temp_bytes = rows_sort_temp_bytes(n, end_bit);
     if (!scratch || temp_bytes == 0 || rows_scratch_fixed(n) + temp_bytes > scratch_bytes) return -5;
@@ -597,29 +677,34 @@ int ps_push_rows_launch(const TfyPsRows& r, const TfyPsHyper& h, const float* ad
     cub::DoubleBuffer<unsigned long long> kb(k0, k1);
     cub::DoubleBuffer<int> vb(v0, v1);
     const int per_table = r.B * r.L;
-    if (per_table <= kPsBlockSortMax && r.V < 0x7fffffffLL) {
+    // the block sort holds one table's occurrences: max_members columns of B*L each at most
+    if ((long long)m.max_members * per_table <= kPsBlockSortMax && r.V < 0x7fffffffLL) {
         const int local_bits = 64 - __builtin_clzll((unsigned long long)r.V);     // ids and the local sentinel V
-        if (weighted)
-            tfy_ps_segment_sort_kernel<true><<<r.T, kPsSortThreads, 0, s>>>(r.ids, per_table, r.V, local_bits, k0, v0,
-                                                                             wts);
-        else
-            tfy_ps_segment_sort_kernel<false><<<r.T, kPsSortThreads, 0, s>>>(r.ids, per_table, r.V, local_bits, k0, v0,
-                                                                              nullptr);
+        tfy_ps_segment_sort_kernel<W, M><<<m.n_tables, kPsSortThreads, 0, s>>>(r.ids, per_table, r.V, local_bits, k0,
+                                                                               v0, W ? wts : nullptr, m);
     } else {
         size_t gk = ((size_t)n + 255) / 256;
         if (gk > TFY_NUM_SMS * 8) gk = TFY_NUM_SMS * 8;
-        if (weighted)
-            tfy_ps_row_keys_kernel<true><<<(unsigned)gk, 256, 0, s>>>(r.ids, n, per_table, r.V, k0, v0, wts);
-        else
-            tfy_ps_row_keys_kernel<false><<<(unsigned)gk, 256, 0, s>>>(r.ids, n, per_table, r.V, k0, v0, nullptr);
+        tfy_ps_row_keys_kernel<W, M><<<(unsigned)gk, 256, 0, s>>>(r.ids, n, per_table, r.V, k0, v0,
+                                                                  W ? wts : nullptr, m);
         size_t tb = temp_bytes;
         cudaError_t err = cub::DeviceRadixSort::SortPairs(temp, tb, kb, vb, n, 0, end_bit, s);
         if (err != cudaSuccess) return (int)err;
     }
 
-    // weighted: the per-occurrence factors go to the sort's alternate key buffer, free once the keys are sorted
+    // weighted: the per-occurrence factors go to the sort's alternate key buffer, free once the keys are sorted;
+    // mapped: the sorted gradient offsets to its alternate value buffer, which the apply kernels then take as occ
     float* cs = nullptr;
-    if (weighted) {
+    const int* occ = vb.Current();
+    if (M) {
+        if (W) cs = reinterpret_cast<float*>(kb.Current() == k0 ? k1 : k0);
+        int* goff = vb.Current() == v0 ? v1 : v0;
+        size_t gf = ((size_t)n + 255) / 256;
+        if (gf > TFY_NUM_SMS * 8) gf = TFY_NUM_SMS * 8;
+        tfy_ps_occ_offsets_kernel<W><<<(unsigned)gf, 256, 0, s>>>(occ, wts, fs, n, r.B, r.L, r.dout_ld, r.col_stride,
+                                                                   goff, cs);
+        occ = goff;
+    } else if (W) {
         cs = reinterpret_cast<float*>(kb.Current() == k0 ? k1 : k0);
         size_t gf = ((size_t)n + 255) / 256;
         if (gf > TFY_NUM_SMS * 8) gf = TFY_NUM_SMS * 8;
@@ -636,22 +721,28 @@ int ps_push_rows_launch(const TfyPsRows& r, const TfyPsHyper& h, const float* ad
     if (gs > TFY_NUM_SMS * 8) gs = TFY_NUM_SMS * 8;
     size_t gl = ((size_t)n + 255) / 256;                                // one warp per 32 sorted positions
     if (gl > TFY_NUM_SMS * 8) gl = TFY_NUM_SMS * 8;
-#define TFY_APPLY_ROWS(GT, VV, WW)                                                                                     \
+#define TFY_APPLY_ROWS(GT, VV)                                                                                         \
     do {                                                                                                               \
-        tfy_ps_apply_short_rows_kernel<GT, VV, WW><<<(unsigned)gs, 256, 0, s>>>(r, h, adam_scale, kb.Current(),       \
-                                                                                 vb.Current(), n, cs);                 \
-        tfy_ps_apply_long_rows_kernel<GT, VV, WW><<<(unsigned)gl, 256, 0, s>>>(r, h, adam_scale, kb.Current(),        \
-                                                                                vb.Current(), n, cl_log2, cs);         \
+        tfy_ps_apply_short_rows_kernel<GT, VV, W, M><<<(unsigned)gs, 256, 0, s>>>(r, h, adam_scale, kb.Current(), occ, \
+                                                                                   n, cs, m);                          \
+        tfy_ps_apply_long_rows_kernel<GT, VV, W, M><<<(unsigned)gl, 256, 0, s>>>(r, h, adam_scale, kb.Current(), occ,  \
+                                                                                  n, cl_log2, cs, m);                  \
     } while (0)
-#define TFY_APPLY_ROWS_W(GT, VV)                                                                                       \
-    do {                                                                                                               \
-        if (weighted) TFY_APPLY_ROWS(GT, VV, true); else TFY_APPLY_ROWS(GT, VV, false);                               \
-    } while (0)
-    if (grad_is_bf16) { if (vec) TFY_APPLY_ROWS_W(__nv_bfloat16, 4); else TFY_APPLY_ROWS_W(__nv_bfloat16, 1); }
-    else { if (vec) TFY_APPLY_ROWS_W(float, 4); else TFY_APPLY_ROWS_W(float, 1); }
-#undef TFY_APPLY_ROWS_W
+    if (grad_is_bf16) { if (vec) TFY_APPLY_ROWS(__nv_bfloat16, 4); else TFY_APPLY_ROWS(__nv_bfloat16, 1); }
+    else { if (vec) TFY_APPLY_ROWS(float, 4); else TFY_APPLY_ROWS(float, 1); }
 #undef TFY_APPLY_ROWS
     return (int)cudaGetLastError();
+}
+
+// The fold of one push, unmapped (every column its own table) unless map is given.
+int ps_push_rows_launch(const TfyPsRows& r, const TfyPsHyper& h, const float* adam_scale, int grad_is_bf16,
+                        void* scratch, size_t scratch_bytes, cudaStream_t s, bool weighted = false,
+                        const float* wts = nullptr, const float* fs = nullptr, const TfyPsMap* map = nullptr) {
+    const TfyPsMap m = map ? *map : TfyPsMap{nullptr, r.T, r.T, 1};
+#define TFY_FOLD(WW, MM) ps_push_rows_fold<WW, MM>(r, h, adam_scale, grad_is_bf16, scratch, scratch_bytes, s, wts, fs, m)
+    if (map) return weighted ? TFY_FOLD(true, true) : TFY_FOLD(false, true);
+    return weighted ? TFY_FOLD(true, false) : TFY_FOLD(false, false);
+#undef TFY_FOLD
 }
 
 }  // namespace
@@ -938,6 +1029,42 @@ int tfy_ps_multi_push_rows_weighted(const uint64_t* tables, const uint64_t* s1s,
     r.B = B; r.L = L; r.T = T; r.D = D; r.V = V; r.dout_ld = dout_ld; r.col_stride = col_stride;
     r.scale = grad_scale;
     return ps_push_rows_launch(r, h, adam_scale, grad_is_bf16, scratch, scratch_bytes, s, true, weights, f);
+}
+
+// The sparse push of columns that share tables (shared embedding columns): the arguments of
+// tfy_ps_multi_push_rows_weighted, except that tables / s1s / s2s hold n_tables DISTINCT tables and the device
+// int32 table_of[T] names the table of every column (0 <= table_of[t] < n_tables, every table named at least once),
+// and max_members is the largest number of columns of any one table: the fold takes the block sort when max_members
+// * B * L <= 2048.  A table with more columns than max_members is then left out of the push.
+// Every distinct (table, row) receives the sum, in (t, b, j) order, of weights[t, b, j] * f[t, b] *
+// dout[b, t * col_stride + d] over the occurrences of all its columns, and its optimizer runs once.  weights and f
+// both nullptr: the unweighted kernels (a one-hot K5 push, combiner 0).
+int tfy_ps_multi_push_rows_shared(const uint64_t* tables, const uint64_t* s1s, const uint64_t* s2s, const void* ids,
+                                  const void* dout, int grad_is_bf16, int B, int T, int D, long long V, int opt,
+                                  float lr, float eps, float p1, float p2, float p3, float grad_scale,
+                                  const float* adam_scale, int dout_ld, int col_stride, int L, const float* weights,
+                                  const float* f, int combiner, int n_tables, const int* table_of, int max_members,
+                                  void* scratch,
+                                  size_t scratch_bytes, cudaStream_t s) {
+    if (L < 1 || B < 0 || T < 0 || combiner < 0 || combiner > 2) return -2;
+    if (n_tables < 1 || n_tables > T || !table_of) return -2;
+    if (max_members < 1 || max_members > T - n_tables + 1) return -2;
+    if (opt != TFY_OPT_SGD && opt != TFY_OPT_ADAGRAD && opt != TFY_OPT_ADAM && opt != TFY_OPT_FTRL) return -3;
+    if (opt != TFY_OPT_SGD && !s1s) return -4;
+    if ((opt == TFY_OPT_ADAM || opt == TFY_OPT_FTRL) && !s2s) return -4;
+    if (!f && combiner != 0) return -4;
+    if (dout_ld <= 0) dout_ld = D;
+    if ((long long)(T - 1) * col_stride + (long long)(B > 0 ? B - 1 : 0) * dout_ld + D > 0x7fffffffLL) return -2;
+    TfyPsHyper h;
+    h.opt = opt; h.lr = lr; h.eps = eps; h.wd = 0.f; h.p1 = p1; h.p2 = p2; h.p3 = p3; h.grad_scale = grad_scale;
+    TfyPsRows r = {};
+    r.tables = tables; r.s1s = s1s; r.s2s = s2s;
+    r.ids = (const long long*)ids; r.dout = dout;
+    r.B = B; r.L = L; r.T = T; r.D = D; r.V = V; r.dout_ld = dout_ld; r.col_stride = col_stride;
+    r.scale = grad_scale;
+    const TfyPsMap map = {table_of, T, n_tables, max_members};
+    return ps_push_rows_launch(r, h, adam_scale, grad_is_bf16, scratch, scratch_bytes, s, weights || f, weights, f,
+                               &map);
 }
 
 }  // extern "C"
