@@ -53,6 +53,9 @@ native.declare("tfy_conv3x3_c1_wgrad_tc", [_vp, _i, _vp, _vp, _vp, _vp, _vp, _i,
 native.declare("tfy_conv3x3_c32_dgrad_unpool", [_vp, _vp, _f, _vp, _vp, _vp, _i, _i, _i, _vp])
 native.declare("tfy_conv3x3_c32_wgrad_unpool", [_vp, _vp, _vp, _f, _vp, _vp, _vp, _vp, _i, _i, _i, _vp])
 native.declare("tfy_conv3x3_c32_wgrad_unpool_ov", [_vp, _vp, _vp, _f, _vp, _vp, _vp, _vp, _i, _i, _i, _vp, _vp])
+native.declare("tfy_conv3x3_c32_wgrad_unpool_deferred", [_vp, _vp, _vp, _f, _vp, _i, _i, _i, _vp, _vp, _vp])
+native.declare("tfy_conv3x3_c32_dgrad_unpool_reduce", [_vp, _vp, _f, _vp, _vp, _vp, _i, _i, _i, _vp, _i, _vp, _vp,
+                                                       _vp])
 native.declare("tfy_conv3x3_c32_wgrad_spare_ctas", [_i, _i, _i])
 native.declare("tfy_dense_bwd", [_vp, _vp, _vp, _vp, _vp, _i, _i, _i, _vp])
 native.declare("tfy_gemm_bf16_splitk_fused", [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _f, _u32, _vp, _i,
@@ -565,16 +568,25 @@ class FastSequentialEngine(GraphTrainEngine):
                 if (st.pool and self._tc_conv(st, B) and grad.is_contiguous()
                         and os.environ.get("TFY_NO_UNPOOL_FUSION") != "1"):
                     # pool/dropout/ReLU backward fused into the operand producers of wgrad and dgrad: the
-                    # 4x larger dz tensor is never written; db comes out of the wgrad kernel
+                    # 4x larger dz tensor is never written; db comes out of the wgrad kernel.  When the dgrad
+                    # launch follows, the wgrad CTAs only store their fp32 partials (no grid barrier) and the
+                    # dgrad kernel reduces them into dW / db behind its main loop: the same bits either way.
                     if "wgrad_scratch" not in self._acc32:
                         self._acc32["wgrad_scratch"] = torch.empty(
                             int(lib.tfy_conv3x3_c32_wgrad_scratch_elems()), dtype=torch.float32, device=grad.device)
+                    part = self._acc32["wgrad_scratch"]
                     ov = self._overlap_desc(li, B, H, W)
-                    self._chk(lib.tfy_conv3x3_c32_wgrad_unpool_ov(
-                        xin.data_ptr(), grad.data_ptr(), aux.data_ptr(), scale,
-                        self._acc32["wgrad_scratch"].data_ptr(), w.grad.data_ptr(), b.grad.data_ptr(),
-                        self._conv_sync.data_ptr(), B, H, W, ctypes.byref(ov) if ov is not None else None, s),
-                        "conv3x3_c32_wgrad_unpool")
+                    ovp = ctypes.byref(ov) if ov is not None else None
+                    n_part = ctypes.c_int(0)
+                    if first:
+                        self._chk(lib.tfy_conv3x3_c32_wgrad_unpool_ov(
+                            xin.data_ptr(), grad.data_ptr(), aux.data_ptr(), scale, part.data_ptr(),
+                            w.grad.data_ptr(), b.grad.data_ptr(), self._conv_sync.data_ptr(), B, H, W, ovp, s),
+                            "conv3x3_c32_wgrad_unpool")
+                    else:
+                        self._chk(lib.tfy_conv3x3_c32_wgrad_unpool_deferred(
+                            xin.data_ptr(), grad.data_ptr(), aux.data_ptr(), scale, part.data_ptr(), B, H, W, ovp,
+                            ctypes.byref(n_part), s), "conv3x3_c32_wgrad_unpool_deferred")
                     dp = grad
                     grad = None
                     if not first:
@@ -582,9 +594,10 @@ class FastSequentialEngine(GraphTrainEngine):
                         fold = (prev.kind == "conv" and prev.relu and not prev.pool and prev.drop == 0
                                 and saved[li - 1][2] is not None and saved[li - 1][2].data_ptr() == xin.data_ptr())
                         grad = torch.empty((B, H, W, Cin), dtype=bf16, device=dp.device)
-                        self._chk(lib.tfy_conv3x3_c32_dgrad_unpool(
+                        self._chk(lib.tfy_conv3x3_c32_dgrad_unpool_reduce(
                             dp.data_ptr(), aux.data_ptr(), scale, w.data_ptr(), xin.data_ptr() if fold else None,
-                            grad.data_ptr(), B, H, W, s), "conv3x3_c32_dgrad_unpool")
+                            grad.data_ptr(), B, H, W, part.data_ptr(), n_part.value, w.grad.data_ptr(),
+                            b.grad.data_ptr(), s), "conv3x3_c32_dgrad_unpool_reduce")
                         pre_gated = fold
                     continue
                 if st.pool:

@@ -51,14 +51,26 @@ constexpr int FP_ACC_LD = COUT + 4, DG_ACC_LD = CIN + 4;
 // 416 threads: the launch bound leaves the MMA warpgroup room for both halves' accumulators (2 x 32 fp32) in flight
 constexpr int FP_STAGES = 3, FP_EPI_WARPS = 8, FP_THREADS = (FP_EPI_WARPS + 4 + 1) * 32;    // 416
 constexpr size_t FP_SMEM = (size_t)FP_STAGES * A_HALO_PAD + W_BYTES + 2 * 128 * FP_ACC_LD * 4 + 1024 + 256;
-constexpr int DG_STAGES = 3, DG_EPI_WARPS = 4, DG_THREADS = (DG_EPI_WARPS + 4 + 1 + 4) * 32;  // 416: +4 un-pool producer warps
-constexpr size_t DG_SMEM = (size_t)DG_STAGES * Z_HALO_B + W_BYTES + 2 * 128 * DG_ACC_LD * 4 + 1024 + 256;
-constexpr int WG_STAGES = 4, WG_STAGE_B = Z_PATCH_B + A_HALO_PAD;                         // 29696
+// 512 threads: + 4 un-pool producer warps, + 3 warps that reduce deferred weight-gradient partials with the TMA warp
+constexpr int DG_STAGES = 3, DG_EPI_WARPS = 4, DG_RED_WARPS = 4;
+constexpr int DG_THREADS = (DG_EPI_WARPS + 4 + 1 + 4 + DG_RED_WARPS - 1) * 32;
+// + the part sums of the deferred weight-gradient reduction (c_wg_reduce): 37 float4 outputs x 16 parts per CTA at
+// batch 128 fit in one chunk
+constexpr int DG_RED_B = 32 * 1024;
+constexpr size_t DG_SMEM =
+    (size_t)DG_STAGES * Z_HALO_B + W_BYTES + 2 * 128 * DG_ACC_LD * 4 + DG_RED_B + 1024 + 256;
+static_assert(DG_SMEM <= 232448, "dgrad shared memory exceeds the sm_90 opt-in limit per block");
+// The ring holds every patch of a CTA at batch 128 (5 of them), so all of them load during the prologue; the MMA
+// warpgroup still takes patches WG_GROUP at a time (one wgmma chain per tap and group), which fixes the fp32
+// summation order of the partial tile whatever the ring depth.
+constexpr int WG_RING = 5, WG_GROUP = 4, WG_STAGE_B = Z_PATCH_B + A_HALO_PAD;              // 29696
 constexpr int WG_WORK_WARPS = 16, WG_THREADS = (WG_WORK_WARPS + 4 + 1) * 32;               // 672
 constexpr int WG_OUT = COUT * TAPS * CIN;                                                 // 18432
 constexpr int WG_PART = WG_OUT + COUT;                 // per-CTA partial: dW tile + db (un-pool variant)
 constexpr int WG_ACC_B = TAPS * 16 * 128 * 4;          // 9 taps x 64 x 32 fp32 in fragment order [tap][16][128 threads]
-constexpr size_t WG_SMEM = (size_t)WG_STAGES * WG_STAGE_B + 1024 + 512 + WG_WORK_WARPS * COUT * 4 + WG_ACC_B;
+constexpr size_t WG_SMEM = (size_t)WG_RING * WG_STAGE_B + 1024 + 512 + WG_WORK_WARPS * COUT * 4 + WG_ACC_B;
+static_assert(WG_SMEM <= 232448, "wgrad shared memory exceeds the sm_90 opt-in limit per block");
+static_assert(2 * WG_RING * 8 <= 512, "wgrad ring barriers overflow their shared-memory slot");
 
 constexpr uint32_t SW128 = TFY_WG_SW128, SW64 = TFY_WG_SW64;
 
@@ -119,6 +131,61 @@ __device__ __forceinline__ void c_unpool_emit(uint8_t* tile, const CUnpoolIn& in
         const int row = row0 + (pos >> 1) * row_dy + (pos & 1);
         *reinterpret_cast<uint4*>(tile + (size_t)row * Z_PIX_B + ((uint32_t)(g ^ (row & 7)) << 4)) =
             TfyPack<__nv_bfloat16>::pack(o);
+    }
+}
+
+// Deferred reduction of the weight gradient's per-CTA partials (DG_RED_WARPS warps, rt = 0 .. 32 DG_RED_WARPS - 1):
+// float4 outputs [f0, f1) of the dW tile + db, each summed over the n_part partials in the order c_wg_slice gives the
+// wgrad CTA that owns it, then converted to bf16.  As in that CTA, part p of an output sums partials p, p + parts, ...
+// (8 loads in flight per thread); the part sums of the outputs are one task each for all reduction threads, so the
+// ~70 KB a CTA reads are in flight at once, and go to buf (DG_RED_B bytes, `stride` per output) to be added in order.
+__device__ __forceinline__ void c_wg_reduce(const float* __restrict__ partials, int n_part, int f0, int f1,
+                                            __nv_bfloat16* __restrict__ dw, __nv_bfloat16* __restrict__ db,
+                                            float4* buf, int rt) {
+    constexpr int TOTAL4 = WG_PART / 4, STRIDE4 = WG_PART / 4, NT = DG_RED_WARPS * 32;
+    if (f0 >= f1) return;                                            // the same for every reduction thread
+    const int per = c_wg_per(TOTAL4, n_part);
+    auto parts_of = [&](int f) { return c_wg_slice(TOTAL4, n_part, f / per, WG_THREADS).parts; };
+    // every owner but the last has the same slice length: the ends of [f0, f1) bound the part sums per output
+    const int stride = max(min(parts_of(f0), n_part), min(parts_of(f1 - 1), n_part));
+    const int chunk = DG_RED_B / (16 * stride);                     // float4 outputs per round
+    const float4* src = reinterpret_cast<const float4*>(partials);
+    for (int c0 = f0; c0 < f1; c0 += chunk) {
+        const int cn = min(chunk, f1 - c0);
+        for (int k = rt; k < cn * stride; k += NT) {
+            const int j = k / stride, p = k - j * stride, parts = parts_of(c0 + j);
+            if (p >= parts || p >= n_part) continue;
+            const float4* col = src + c0 + j;
+            float4 s = make_float4(0.f, 0.f, 0.f, 0.f);
+            for (int q0 = p; q0 < n_part; q0 += 8 * parts) {
+                float4 v[8];
+#pragma unroll
+                for (int u = 0; u < 8; ++u)
+                    if (q0 + u * parts < n_part) v[u] = __ldcg(col + (size_t)(q0 + u * parts) * STRIDE4);
+#pragma unroll
+                for (int u = 0; u < 8; ++u)
+                    if (q0 + u * parts < n_part) { s.x += v[u].x; s.y += v[u].y; s.z += v[u].z; s.w += v[u].w; }
+            }
+            buf[k] = s;
+        }
+        asm volatile("bar.sync 1, %0;" ::"r"(NT) : "memory");
+        for (int j = rt; j < cn; j += NT) {
+            const int parts = parts_of(c0 + j);
+            const float4* ps = buf + j * stride;
+            float4 tot = ps[0];
+            for (int p = 1; p < parts && p < n_part; ++p) {
+                tot.x += ps[p].x; tot.y += ps[p].y; tot.z += ps[p].z; tot.w += ps[p].w;
+            }
+            if (parts > n_part) { tot.x += 0.f; tot.y += 0.f; tot.z += 0.f; tot.w += 0.f; }   // the empty parts
+            __nv_bfloat162 l2 = __floats2bfloat162_rn(tot.x, tot.y), h2 = __floats2bfloat162_rn(tot.z, tot.w);
+            uint2 packed;
+            packed.x = *reinterpret_cast<uint32_t*>(&l2);
+            packed.y = *reinterpret_cast<uint32_t*>(&h2);
+            const int e = (c0 + j) * 4;                              // outputs [0, WG_OUT) = dW, then db
+            if (e < WG_OUT) *reinterpret_cast<uint2*>(dw + e) = packed;
+            else *reinterpret_cast<uint2*>(db + (e - WG_OUT)) = packed;
+        }
+        asm volatile("bar.sync 1, %0;" ::"r"(NT) : "memory");       // buf is reused by the next round
     }
 }
 
@@ -309,19 +376,24 @@ tfy_conv3x3_fprop_pool_kernel(const __grid_constant__ CUtensorMap map_a, const _
 // dz: [B, H-2, W-2, 64]; dx: [B, H, W, 32].  warps 0..3 epilogue, warps 4..7 MMA, warp 8 TMA (zero-fills the halo)
 // ------------------------------------------------------------------------------------------------
 // UNPOOL: the A operand is not loaded from a materialised dz but rebuilt by warps 9..12 from the pooled gradient
-// dp [B, (H-2)/2, (W-2)/2, 64] and the forward kernel's code bytes (c_unpool_task).
+// dp [B, (H-2)/2, (W-2)/2, 64] and the forward kernel's code bytes (c_unpool_task).  With `partials` (UNPOOL only)
+// warp 8, idle once it has issued the weight load, and warps 13..15 reduce a slice of the n_part weight-gradient
+// partials a deferred tfy_conv3x3_wgrad_kernel<true> left behind into bf16 dw / db (c_wg_reduce), behind the main
+// loop.
 template <bool UNPOOL>
 __global__ void __launch_bounds__(DG_THREADS, 1)
 tfy_conv3x3_dgrad_kernel(const __grid_constant__ CUtensorMap map_dz, const __grid_constant__ CUtensorMap map_w,
                          const __nv_bfloat16* __restrict__ gate, __nv_bfloat16* __restrict__ dx, int H, int W,
                          int tiles_x, int tiles_y, int n_patches, const __nv_bfloat16* __restrict__ dp,
-                         const uint8_t* __restrict__ code, float scale) {
+                         const uint8_t* __restrict__ code, float scale, const float* __restrict__ partials,
+                         int n_part, __nv_bfloat16* __restrict__ dw, __nv_bfloat16* __restrict__ db) {
     extern __shared__ uint8_t smem_raw[];
     C_TIMELINE_BEGIN();
     uint8_t* stages = tfy_align1024(smem_raw);                      // [3][10 h][2 n][10 w][128 B], 128B swizzle
     uint8_t* w_tile = stages + (size_t)DG_STAGES * Z_HALO_B;      // [9][64 o][64 B], 64B swizzle
     float* acc_s = reinterpret_cast<float*>(w_tile + W_BYTES);    // [2][128][DG_ACC_LD]
-    uint64_t* full = reinterpret_cast<uint64_t*>(acc_s + 2 * 128 * DG_ACC_LD);
+    float4* red_buf = reinterpret_cast<float4*>(acc_s + 2 * 128 * DG_ACC_LD);   // DG_RED_B: part sums (c_wg_reduce)
+    uint64_t* full = reinterpret_cast<uint64_t*>(reinterpret_cast<uint8_t*>(red_buf) + DG_RED_B);
     uint64_t* empty = full + DG_STAGES;
     uint64_t* tfull = empty + DG_STAGES;
     uint64_t* tempty = tfull + 2;
@@ -356,6 +428,9 @@ tfy_conv3x3_dgrad_kernel(const __grid_constant__ CUtensorMap map_dz, const __gri
                 if (i == 0) C_MARK(2);
             }
         }
+        __syncwarp();
+    } else if (warp > DG_EPI_WARPS + 8) {
+        // reduction warps (below)
     } else if (warp >= DG_EPI_WARPS && warp < DG_EPI_WARPS + 4) {
         // ---------------- MMA warpgroup: both 64-pixel halves of the patch (4 h rows of the halo apart)
         const uint32_t w0 = tfy_smem_u32(w_tile);
@@ -468,6 +543,14 @@ tfy_conv3x3_dgrad_kernel(const __grid_constant__ CUtensorMap map_dz, const __gri
             }
         }
     }
+    if (UNPOOL && partials != nullptr && (warp == DG_EPI_WARPS + 4 || warp > DG_EPI_WARPS + 8)) {
+        const int rt = warp == DG_EPI_WARPS + 4 ? lane : (warp - (DG_EPI_WARPS + 8)) * 32 + lane;
+        constexpr int TOTAL4 = WG_PART / 4;
+        const int per = (TOTAL4 + (int)gridDim.x - 1) / (int)gridDim.x;
+        const int f0 = min((int)blockIdx.x * per, TOTAL4), f1 = min(f0 + per, TOTAL4);
+        c_wg_reduce(partials, n_part, f0, f1, dw, db, red_buf, rt);
+        if (rt == 0) C_MARK(3);
+    }
     __syncthreads();
     if (threadIdx.x == 0) C_MARK(10);
 }
@@ -480,7 +563,9 @@ tfy_conv3x3_dgrad_kernel(const __grid_constant__ CUtensorMap map_dz, const __gri
 // reduces a slice of the 18432 outputs over all partials in a fixed order (deterministic, no atomics) and writes
 // bf16 dW.
 // warps 0..15 un-pool producers (UNPOOL) + final reduction, warps 16..19 MMA + partial tile, warp 20 TMA.
-// sync: 1024 uint32, zero-initialised once (generation + two levels of arrival counters, see below).
+// sync: 1024 uint32, zero-initialised once (generation + two levels of arrival counters, see below).  sync ==
+// nullptr (UNPOOL only): no grid barrier and no reduction -- the compute CTAs store their partials and exit, and
+// the un-pool dgrad kernel that follows reduces them (tfy_conv3x3_dgrad_kernel<true>, c_wg_reduce).
 // ------------------------------------------------------------------------------------------------
 // UNPOOL: dz tiles are rebuilt by warps 0..3 from the pooled gradient dp and the forward kernel's code bytes
 // (c_unpool_task) and the bias gradient db = sum of the gated dp rides along as 64 more outputs.
@@ -504,31 +589,31 @@ tfy_conv3x3_wgrad_kernel(const __grid_constant__ CUtensorMap map_dz, const __gri
     }
     extern __shared__ uint8_t smem_raw[];
     C_TIMELINE_BEGIN();
-    uint8_t* stages = tfy_align1024(smem_raw);    // [4] { dz [8 h][2 n][8 w][128 B] sw128 ; a [10 h][2 n][10 w][64 B] sw64 }
-    uint64_t* full = reinterpret_cast<uint64_t*>(stages + (size_t)WG_STAGES * WG_STAGE_B);
-    uint64_t* empty = full + WG_STAGES;
-    float* s_db = reinterpret_cast<float*>(empty + WG_STAGES);      // [16 warps][64] bias-gradient partials (UNPOOL)
+    uint8_t* stages = tfy_align1024(smem_raw);    // [5] { dz [8 h][2 n][8 w][128 B] sw128 ; a [10 h][2 n][10 w][64 B] sw64 }
+    uint64_t* full = reinterpret_cast<uint64_t*>(stages + (size_t)WG_RING * WG_STAGE_B);
+    uint64_t* empty = full + WG_RING;
+    float* s_db = reinterpret_cast<float*>(empty + WG_RING);        // [16 warps][64] bias-gradient partials (UNPOOL)
     float* acc_s = s_db + WG_WORK_WARPS * COUT;                      // [9 taps][16][128 threads] fp32
 
     const int warp = __shfl_sync(0xffffffffu, (int)threadIdx.x >> 5, 0), lane = threadIdx.x & 31;   // warp-uniform role index
     if (threadIdx.x == 0) {
         if (!UNPOOL) tfy_prefetch_tensormap(&map_dz);
         tfy_prefetch_tensormap(&map_a);
-        for (int s = 0; s < WG_STAGES; ++s) { tfy_mbar_init(&full[s], UNPOOL ? 257 : 1); tfy_mbar_init(&empty[s], 4); }
+        for (int s = 0; s < WG_RING; ++s) { tfy_mbar_init(&full[s], UNPOOL ? 257 : 1); tfy_mbar_init(&empty[s], 4); }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
     __syncthreads();
     tfy_pdl_sync();                      // upstream grids complete; our dependents may start launching
     if (threadIdx.x == 0) C_MARK(1);
-    const uint32_t gen0 = threadIdx.x == 0 ? *reinterpret_cast<volatile uint32_t*>(sync) : 0u;
+    const uint32_t gen0 = (threadIdx.x == 0 && sync) ? *reinterpret_cast<volatile uint32_t*>(sync) : 0u;
     const int my_patches = ((int)blockIdx.x < n_patches) ? (n_patches - 1 - (int)blockIdx.x) / n_cmp + 1 : 0;
 
     if (warp == WG_WORK_WARPS + 4) {
         if (tfy_elect_one()) {
             CPatchIter it(tiles_x, tiles_y, n_cmp);
             for (int i = 0; i < my_patches; ++i, it.next()) {
-                const int s = i % WG_STAGES;
-                if (i >= WG_STAGES) tfy_mbar_wait(&empty[s], ((i / WG_STAGES) - 1) & 1);
+                const int s = i % WG_RING;
+                if (i >= WG_RING) tfy_mbar_wait(&empty[s], ((i / WG_RING) - 1) & 1);
                 uint8_t* st = stages + (size_t)s * WG_STAGE_B;
                 tfy_mbar_expect_tx(&full[s], (UNPOOL ? 0 : Z_PATCH_B) + A_HALO_B);
                 if (!UNPOOL) tfy_tma_load_4d(&map_dz, &full[s], st, 0, it.tx * 8, it.bz * 2, it.ty * 8);
@@ -537,15 +622,16 @@ tfy_conv3x3_wgrad_kernel(const __grid_constant__ CUtensorMap map_dz, const __gri
             }
         }
     } else if (warp >= WG_WORK_WARPS) {
-        // Patches are taken WG_STAGES at a time; per group and tap, one wgmma chain over the group's pixels in
+        // Patches are taken WG_GROUP at a time; per group and tap, one wgmma chain over the group's pixels in
         // registers, then added into the tap's fp32 tile (fragment order: thread t owns words [tap][i][t]).
+        // Patch i sits in ring stage i % WG_RING.
         const int tid = (int)threadIdx.x - WG_WORK_WARPS * 32;
         float* mine = acc_s + tid;
         for (int i = 0; i < TAPS * 16; ++i) mine[i * 128] = 0.f;
-        const int n_groups = (my_patches + WG_STAGES - 1) / WG_STAGES;
+        const int n_groups = (my_patches + WG_GROUP - 1) / WG_GROUP;
         for (int g = 0; g < n_groups; ++g) {
-            const int cnt = min(WG_STAGES, my_patches - g * WG_STAGES);
-            for (int q = 0; q < cnt; ++q) tfy_mbar_wait(&full[q], g & 1);
+            const int i0 = g * WG_GROUP, cnt = min(WG_GROUP, my_patches - i0);
+            for (int q = 0; q < cnt; ++q) tfy_mbar_wait(&full[(i0 + q) % WG_RING], ((i0 + q) / WG_RING) & 1);
             if (UNPOOL) tfy_fence_proxy_async();
             if (g == 0 && tid == 0) C_MARK(4);
             const uint32_t st0 = tfy_smem_u32(stages);
@@ -556,7 +642,7 @@ tfy_conv3x3_wgrad_kernel(const __grid_constant__ CUtensorMap map_dz, const __gri
                 tfy_wg_fence();
 #pragma unroll 1
                 for (int q = 0; q < cnt; ++q) {
-                    const uint32_t dz0 = st0 + q * WG_STAGE_B, a0 = dz0 + Z_PATCH_B;
+                    const uint32_t dz0 = st0 + ((i0 + q) % WG_RING) * WG_STAGE_B, a0 = dz0 + Z_PATCH_B;
 #pragma unroll
                     for (int j = 0; j < 8; ++j) {      // 16 pixels (one h row of both images) per MMA
                         // A = dz^T: M = 64 o inside the 128 B pixel row; K = pixels, 8-pixel groups 1024 B apart
@@ -573,7 +659,7 @@ tfy_conv3x3_wgrad_kernel(const __grid_constant__ CUtensorMap map_dz, const __gri
                 for (int i = 0; i < 16; ++i) mine[(t * 16 + i) * 128] += d[i];
             }
             if (lane == 0)
-                for (int q = 0; q < cnt; ++q) tfy_mbar_arrive(&empty[q]);     // stages reusable
+                for (int q = 0; q < cnt; ++q) tfy_mbar_arrive(&empty[(i0 + q) % WG_RING]);     // stages reusable
         }
         if (tid == 0) C_MARK(5);
         // partial tile rows o = (o, tap) rows of 128 B: value i of this thread is o = 16 w + lane / 4 + 8 ((i / 2) % 2),
@@ -589,7 +675,8 @@ tfy_conv3x3_wgrad_kernel(const __grid_constant__ CUtensorMap map_dz, const __gri
                        make_float2(mine[(t * 16 + i) * 128], mine[(t * 16 + i + 1) * 128]));
             }
         }
-        __threadfence();
+        if (sync) __threadfence();     // the grid barrier follows (deferred: the kernel boundary orders the stores)
+        if (tid == 0) C_MARK(6);
     } else if (my_patches > 0) {
         if (UNPOOL) {
             // ---------------- un-pool producers (all 16 worker warps): a patch needs 4 x 4 pooled pixels x 2 images
@@ -613,8 +700,8 @@ tfy_conv3x3_wgrad_kernel(const __grid_constant__ CUtensorMap map_dz, const __gri
                 const CUnpoolIn in1 = c_unpool_load(dp, code, two, two ? p1 : p0, g);
                 float gated[8];
                 {
-                    const int s = i % WG_STAGES;
-                    if (i >= WG_STAGES) tfy_mbar_wait(&empty[s], ((i / WG_STAGES) - 1) & 1);
+                    const int s = i % WG_RING;
+                    if (i >= WG_RING) tfy_mbar_wait(&empty[s], ((i / WG_RING) - 1) & 1);
                     c_unpool_emit(stages + (size_t)s * WG_STAGE_B, in0, scale, g, row0, 16, gated);
 #pragma unroll
                     for (int k = 0; k < 8; ++k) colacc[k] += gated[k];
@@ -622,8 +709,8 @@ tfy_conv3x3_wgrad_kernel(const __grid_constant__ CUtensorMap map_dz, const __gri
                     tfy_mbar_arrive(&full[s]);
                 }
                 if (two) {
-                    const int i2 = i + 2, s = i2 % WG_STAGES;
-                    if (i2 >= WG_STAGES) tfy_mbar_wait(&empty[s], ((i2 / WG_STAGES) - 1) & 1);
+                    const int i2 = i + 2, s = i2 % WG_RING;
+                    if (i2 >= WG_RING) tfy_mbar_wait(&empty[s], ((i2 / WG_RING) - 1) & 1);
                     c_unpool_emit(stages + (size_t)s * WG_STAGE_B, in1, scale, g, row0, 16, gated);
 #pragma unroll
                     for (int k = 0; k < 8; ++k) colacc[k] += gated[k];
@@ -653,10 +740,11 @@ tfy_conv3x3_wgrad_kernel(const __grid_constant__ CUtensorMap map_dz, const __gri
                 __stcg(partials + (size_t)blockIdx.x * WG_PART + WG_OUT + threadIdx.x, a);
             }
         }
-        __threadfence();
+        if (sync) __threadfence();
     }
     __syncthreads();
     if (threadIdx.x == 0) C_MARK(7);
+    if (sync == nullptr) return;                                    // deferred: the dgrad kernel reduces
 
     // Grid-wide arrive / release (all CTAs are co-resident: grid <= #SMs, one CTA per SM).  Same-sector atomics
     // serialise at ~20-30 cycles each and every returning atomic in a chain costs an L2 round trip, so: arrivals
@@ -685,11 +773,10 @@ tfy_conv3x3_wgrad_kernel(const __grid_constant__ CUtensorMap map_dz, const __gri
     }
     __syncthreads();
     if (threadIdx.x == 0) C_MARK(8);
-    // slice of the outputs owned by this CTA (float4 units), summed over the partials in a fixed order
+    // slice of the outputs owned by this CTA (float4 units), summed over the partials in a fixed order (c_wg_slice)
     constexpr int TOTAL4 = (UNPOOL ? WG_PART : WG_OUT) / 4, STRIDE4 = WG_PART / 4;
-    const int per = (TOTAL4 + n_cmp - 1) / n_cmp;
-    const int lo = (int)blockIdx.x * per, hi = min(lo + per, TOTAL4);
-    const int len = max(hi - lo, 0);
+    const CWgSlice sl = c_wg_slice(TOTAL4, n_cmp, (int)blockIdx.x, WG_THREADS);
+    const int lo = sl.lo, len = sl.len;
     const int n_part = n_cmp;                                       // every CTA wrote a partial
     const float4* src = reinterpret_cast<const float4*>(partials) + lo;
     auto store = [&](int f, const float4& s4) {
@@ -701,10 +788,10 @@ tfy_conv3x3_wgrad_kernel(const __grid_constant__ CUtensorMap map_dz, const __gri
         if (e < WG_OUT) *reinterpret_cast<uint2*>(dw + e) = packed;
         else *reinterpret_cast<uint2*>(db + (e - WG_OUT)) = packed;
     };
-    if (len > 0 && 2 * len <= WG_THREADS) {
+    if (len > 0 && sl.parts > 1) {
         // few outputs per CTA (the usual case: 32): `parts` thread groups split the list of partials
         float4* red = reinterpret_cast<float4*>(stages);             // the ring is idle now
-        const int parts = WG_THREADS / len;
+        const int parts = sl.parts;
         const int f = (int)threadIdx.x % len, part = (int)threadIdx.x / len;
         float4 s4 = make_float4(0.f, 0.f, 0.f, 0.f);
         if (part < parts) {
@@ -1113,8 +1200,9 @@ int tfy_conv3x3_c32_dgrad(const void* dz, const void* w, const void* gate, void*
     CUtensorMap mz, mw;
     if (!c_map_nhwc(&mz, dz, B, H - 2, W - 2, COUT, HALO, HALO) || !c_map_w(&mw, w)) return -6;
     const int tiles_x = (W + 7) / 8, tiles_y = (H + 7) / 8, n_patches = tiles_x * tiles_y * (B / 2);
-    tfy_launch_pdl((tfy_conv3x3_dgrad_kernel<false>), dim3(c_grid(n_patches)), dim3(DG_THREADS), DG_SMEM, s, 
-        mz, mw, (const __nv_bfloat16*)gate, (__nv_bfloat16*)dx, H, W, tiles_x, tiles_y, n_patches, (const __nv_bfloat16*)nullptr, (const uint8_t*)nullptr, 1.0f);
+    tfy_launch_pdl((tfy_conv3x3_dgrad_kernel<false>), dim3(c_grid(n_patches)), dim3(DG_THREADS), DG_SMEM, s,
+        mz, mw, (const __nv_bfloat16*)gate, (__nv_bfloat16*)dx, H, W, tiles_x, tiles_y, n_patches, (const __nv_bfloat16*)nullptr, (const uint8_t*)nullptr, 1.0f,
+        (const float*)nullptr, 0, (__nv_bfloat16*)nullptr, (__nv_bfloat16*)nullptr);
     return (int)cudaGetLastError();
 }
 
@@ -1136,27 +1224,36 @@ int tfy_conv3x3_c32_wgrad(const void* a, const void* dz, float* partials, void* 
 
 // Fused pool/dropout/ReLU backward variants: instead of a materialised dz they take the pooled gradient
 // dp [B, (H-2)/2, (W-2)/2, 64] bf16, the forward kernel's code bytes (same shape) and the dropout scale.
-int tfy_conv3x3_c32_dgrad_unpool(const void* dp, const void* code, float scale, const void* w, const void* gate,
-                                 void* dx, int B, int H, int W, cudaStream_t s) {
+// With `partials`, the kernel also reduces the n_part weight-gradient partials that
+// tfy_conv3x3_c32_wgrad_unpool_deferred left there into dw [64, 3, 3, 32] and db [64] (bf16): the same bits as
+// tfy_conv3x3_c32_wgrad_unpool gives.  partials == nullptr: no reduction (tfy_conv3x3_c32_dgrad_unpool).
+int tfy_conv3x3_c32_dgrad_unpool_reduce(const void* dp, const void* code, float scale, const void* w,
+                                        const void* gate, void* dx, int B, int H, int W, const float* partials,
+                                        int n_part, void* dw, void* db, cudaStream_t s) {
     if ((B % 2) || ((H - 2) % 8) || ((W - 2) % 8)) return -2;
+    if (partials != nullptr && (n_part <= 0 || n_part > 160 || dw == nullptr || db == nullptr)) return -2;
     if (!c_init()) return -4;
     CUtensorMap mw;
     if (!c_map_w(&mw, w)) return -6;
     const int tiles_x = (W + 7) / 8, tiles_y = (H + 7) / 8, n_patches = tiles_x * tiles_y * (B / 2);
     tfy_launch_pdl((tfy_conv3x3_dgrad_kernel<true>), dim3(c_grid(n_patches)), dim3(DG_THREADS), DG_SMEM, s, mw, mw,
                    (const __nv_bfloat16*)gate, (__nv_bfloat16*)dx, H, W, tiles_x, tiles_y, n_patches,
-                   (const __nv_bfloat16*)dp, (const uint8_t*)code, scale);
+                   (const __nv_bfloat16*)dp, (const uint8_t*)code, scale, partials, n_part, (__nv_bfloat16*)dw,
+                   (__nv_bfloat16*)db);
     return (int)cudaGetLastError();
 }
 
-// also writes db [64] = sum over batch and positions of the gated pooled gradient.
-// ov (optional): a fused gradient-exchange/optimizer step to run on SPARE SMs next to the weight gradient
-// (tfy_overlap_role).  ov->n_cta is clamped to the SMs the compute grid leaves free (576 patches -> 116 compute
-// CTAs of 5 patches on a 132-SM H100 -> up to 16 communication CTAs); tfy_conv3x3_c32_wgrad_spare_ctas() tells
-// the caller how many that is so that it can size the overlapped range.
-int tfy_conv3x3_c32_wgrad_unpool_ov(const void* a, const void* dp, const void* code, float scale, float* partials,
-                                    void* dw, void* db, uint32_t* sync, int B, int H, int W, const TfyOverlapStep* ov,
-                                    cudaStream_t s) {
+int tfy_conv3x3_c32_dgrad_unpool(const void* dp, const void* code, float scale, const void* w, const void* gate,
+                                 void* dx, int B, int H, int W, cudaStream_t s) {
+    return tfy_conv3x3_c32_dgrad_unpool_reduce(dp, code, scale, w, gate, dx, B, H, W, nullptr, 0, nullptr, nullptr, s);
+}
+
+}  // extern "C"
+
+namespace {
+// sync == nullptr: deferred reduction (see tfy_conv3x3_wgrad_kernel); *n_part receives the number of partials
+int c_wgrad_unpool(const void* a, const void* dp, const void* code, float scale, float* partials, void* dw, void* db,
+                   uint32_t* sync, int B, int H, int W, const TfyOverlapStep* ov, int* n_part, cudaStream_t s) {
     const int OH = H - 2, OW = W - 2;
     if ((OH % 8) || (OW % 8) || (B % 2)) return -2;
     if (!c_init() || c_sms > 160) return -4;
@@ -1170,10 +1267,35 @@ int tfy_conv3x3_c32_wgrad_unpool_ov(const void* a, const void* dp, const void* c
         if (o.n_cta > c_sms - n_cmp) return -7;       // the role must not displace a compute CTA
         if (o.slot0 < 0 || o.slot0 + o.n_cta > TFY_MAX_BLOCKS) return -8;
     }
+    if (n_part != nullptr) *n_part = n_cmp;
     tfy_launch_pdl((tfy_conv3x3_wgrad_kernel<true>), dim3(n_cmp + o.n_cta), dim3(WG_THREADS), WG_SMEM, s, ma, ma,
                    partials, (__nv_bfloat16*)dw, sync, tiles_x, tiles_y, n_patches, (const __nv_bfloat16*)dp,
                    (const uint8_t*)code, scale, (__nv_bfloat16*)db, OH / 2, OW / 2, o);
     return (int)cudaGetLastError();
+}
+}  // namespace
+
+extern "C" {
+
+// also writes db [64] = sum over batch and positions of the gated pooled gradient.
+// ov (optional): a fused gradient-exchange/optimizer step to run on SPARE SMs next to the weight gradient
+// (tfy_overlap_role).  ov->n_cta is clamped to the SMs the compute grid leaves free (576 patches -> 116 compute
+// CTAs of 5 patches on a 132-SM H100 -> up to 16 communication CTAs); tfy_conv3x3_c32_wgrad_spare_ctas() tells
+// the caller how many that is so that it can size the overlapped range.
+int tfy_conv3x3_c32_wgrad_unpool_ov(const void* a, const void* dp, const void* code, float scale, float* partials,
+                                    void* dw, void* db, uint32_t* sync, int B, int H, int W, const TfyOverlapStep* ov,
+                                    cudaStream_t s) {
+    return c_wgrad_unpool(a, dp, code, scale, partials, dw, db, sync, B, H, W, ov, nullptr, s);
+}
+
+// Deferred variant: the compute CTAs only store their fp32 partials (dW tile + db) in `partials` -- no grid barrier,
+// no reduction -- and *n_part receives their number.  tfy_conv3x3_c32_dgrad_unpool_reduce, the next launch on the
+// stream, turns them into dw / db.
+int tfy_conv3x3_c32_wgrad_unpool_deferred(const void* a, const void* dp, const void* code, float scale,
+                                          float* partials, int B, int H, int W, const TfyOverlapStep* ov,
+                                          int* n_part, cudaStream_t s) {
+    if (n_part == nullptr) return -2;
+    return c_wgrad_unpool(a, dp, code, scale, partials, nullptr, nullptr, nullptr, B, H, W, ov, n_part, s);
 }
 
 int tfy_conv3x3_c32_wgrad_unpool(const void* a, const void* dp, const void* code, float scale, float* partials,

@@ -1,5 +1,5 @@
-// Patch scheduling of the persistent convolution kernels (included by tfy_conv.cu; kept in its own header so that the
-// index arithmetic can be unit-tested on the host: tests/test_native_device_code.py builds it with g++).
+// Patch scheduling and weight-gradient reduction order of the persistent convolution kernels (included by tfy_conv.cu;
+// kept in its own header so that the index arithmetic can be unit-tested on the host with g++).
 #pragma once
 
 // Walks the patch list of a persistent CTA: p = blockIdx.x + i * gridDim.x decomposed into (image pair,
@@ -23,3 +23,20 @@ struct CPatchIter {
         bz += sb;
     }
 };
+
+// Summation order of the conv2 weight gradient's per-CTA fp32 partials (n_part of them; total4 float4 outputs,
+// dW tile then db).  Output f belongs to the slice of owner f / per; the owner's slice length `len` sets how many
+// thread groups (`parts`, of a threads-wide CTA) split the list of partials: part p sums partials p, p + parts, ...
+// in ascending order starting from 0, and the part sums are added in order p = 0 .. parts - 1 (parts = 1: one
+// serial sum).  The wgrad kernel's own reduction and the deferred reduction in the dgrad kernel both follow it, so
+// dW and db are the same bits whichever kernel reduces.
+struct CWgSlice {
+    int lo, len, parts;
+};
+__host__ __device__ __forceinline__ int c_wg_per(int total4, int n_part) { return (total4 + n_part - 1) / n_part; }
+__host__ __device__ __forceinline__ CWgSlice c_wg_slice(int total4, int n_part, int owner, int threads) {
+    const int per = c_wg_per(total4, n_part);
+    const int lo = owner * per, hi = lo + per < total4 ? lo + per : total4;
+    const int len = hi > lo ? hi - lo : 0;
+    return {lo, len, (len > 0 && 2 * len <= threads) ? threads / len : 1};
+}
