@@ -61,6 +61,7 @@ native.declare("tfy_dense_bwd", [_vp, _vp, _vp, _vp, _vp, _i, _i, _i, _vp])
 native.declare("tfy_gemm_bf16_splitk_fused", [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _f, _u32, _vp, _i,
                                               _vp])
 native.declare("tfy_dense_head_scratch_elems", [_i, _i, _i], restype=ctypes.c_size_t)
+native.declare("tfy_nn_max_partial_blocks", [], restype=ctypes.c_size_t)
 native.declare("tfy_dense_head_fused", [_vp, _vp, _vp, _vp, _vp, _f, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i,
                                         _i, _vp])
 native.declare("tfy_dense_head_fused_weighted", [_vp, _vp, _vp, _vp, _vp, _f, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp,
@@ -174,6 +175,10 @@ class FastSequentialEngine(GraphTrainEngine):
                 width = max(width, st.layer.filters, 9 * st.layer.filters)
             elif st.kind == "dense":
                 width = max(width, st.layer.units)
+        # one row of `width` floats per CTA of the bias / weight-gradient reductions (their launchers refuse a grid
+        # of more than tfy_nn_max_partial_blocks() CTAs)
+        if int(self.lib.tfy_nn_max_partial_blocks()) != PARTIAL_BLOCKS:
+            raise RuntimeError("tfy_nn.cu and fastpath.py disagree on the number of partial rows")
         self._partial = torch.zeros(PARTIAL_BLOCKS * width, dtype=torch.float32, device=dev)
         self._counter = torch.zeros(1, dtype=torch.int32, device=dev)
         self._stats = torch.zeros(4, dtype=torch.float32, device=dev)     # hits, rows (, sum w*hit, sum w: weighted)

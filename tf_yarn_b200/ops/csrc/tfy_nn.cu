@@ -15,6 +15,7 @@
 //   tfy_bias_relu_pool_drop_fwd   z -> bias + ReLU + 2x2 max-pool + dropout (+1 code byte)
 //   tfy_pool_drop_relu_bwd        its backward (+ dbias[C])
 //   tfy_softmax_xent          logits(+bias) -> mean loss, dlogits = (softmax - onehot)/B, dbias, #correct
+//                             (tfy_softmax_xent_weighted: the same with Keras sample / class weights)
 //
 // Dropout randomness is counter based: hash(seed, layer salt, optimizer step, element) with the
 // step read from the device-resident TfyOptHyper, so a replayed CUDA graph draws fresh masks.
@@ -24,56 +25,70 @@ namespace {
 
 __device__ __forceinline__ float bf16_to_f(__nv_bfloat16 v) { return __bfloat162float(v); }
 
-// Cross-CTA column sums without a serial tail: every CTA adds its C block sums (in shared memory)
-// into one of TFY_ACC_GROUPS global fp32 accumulator rows with RED (spreading the CTAs over several rows
-// keeps the same-address contention at the L2 atomic units low); the CTA that arrives last swaps every
-// accumulator with zero (atomicExch) -- which reads the totals AND re-arms the buffer for the next
-// launch / graph replay -- and stores the bf16 result.  `gacc` (>= TFY_ACC_GROUPS*C floats) and
-// `counter` must be zero on entry.
-#define TFY_ACC_GROUPS 16
-__device__ void tfy_colsum_publish(const float* s_sum, int C, float* gacc, __nv_bfloat16* out, uint32_t* counter) {
+// The batch reductions below (bias and first-layer weight gradients) are summed in a fixed order -- threads of a
+// CTA in thread order, CTAs in CTA order, no float atomics -- so that two runs give the same bits.
+//
+// Cross-CTA column sums: every CTA has stored its C column sums into its own row `blockIdx.x` of `partial`
+// (plain stores; `partial` holds gridDim.x * C floats, any content on entry).  The CTA that arrives last on
+// `counter` sums the rows in CTA order, stores the bf16 result and re-arms the counter (zero on entry, left zero).
+// With C < blockDim.x, P = blockDim.x / C thread groups each sum every P-th row (loads in flight together) and the
+// P part sums are added in order; s_tmp: >= blockDim.x floats of shared scratch.
+__device__ void tfy_rows_publish(int C, const float* partial, __nv_bfloat16* out, uint32_t* counter, float* s_tmp) {
     __shared__ bool is_last;
-    float* row = gacc + (size_t)(blockIdx.x % TFY_ACC_GROUPS) * C;
-    for (int c = threadIdx.x; c < C; c += blockDim.x) atomicAdd(&row[c], s_sum[c]);
     __threadfence();
     __syncthreads();
-    if (threadIdx.x == 0) {
-        const uint32_t prev = atomicAdd(counter, 1u);
-        is_last = (prev == gridDim.x - 1);
-    }
+    if (threadIdx.x == 0) is_last = (atomicAdd(counter, 1u) == gridDim.x - 1);
     __syncthreads();
     if (!is_last) return;
     __threadfence();
-    for (int c = threadIdx.x; c < C; c += blockDim.x) {
-        float t = 0.f;
-#pragma unroll
-        for (int g = 0; g < TFY_ACC_GROUPS; ++g) t += atomicExch(&gacc[(size_t)g * C + c], 0.f);
-        out[c] = __float2bfloat16(t);
+    const int rows = (int)gridDim.x;
+    const int P = C < (int)blockDim.x ? (int)blockDim.x / C : 1;
+    if (P > 1) {
+        const int c = (int)threadIdx.x % C, part = (int)threadIdx.x / C;
+        if (part < P) {
+            float a = 0.f;
+#pragma unroll 8
+            for (int r = part; r < rows; r += P) a += __ldcg(partial + (size_t)r * C + c);
+            s_tmp[part * C + c] = a;
+        }
+        __syncthreads();
+        if ((int)threadIdx.x < C) {
+            float a = s_tmp[threadIdx.x];
+            for (int q = 1; q < P; ++q) a += s_tmp[q * C + threadIdx.x];
+            out[threadIdx.x] = __float2bfloat16(a);
+        }
+    } else {
+        for (int c = threadIdx.x; c < C; c += blockDim.x) {
+            float a = 0.f;
+#pragma unroll 8
+            for (int r = 0; r < rows; ++r) a += __ldcg(partial + (size_t)r * C + c);
+            out[c] = __float2bfloat16(a);
+        }
     }
     if (threadIdx.x == 0) *counter = 0;
 }
 
-// Per-CTA column sums of values held 8-per-thread (column group g of G = C/8): reduce the lanes of a
-// warp that share a group with shuffles, combine the warps through shared memory (s_sum: [C] floats,
-// zeroed by the caller before use), then publish this CTA's row of `partial`.
-__device__ __forceinline__ void tfy_block_colsum(float (&colacc)[8], int g, int G, bool active, float* s_sum) {
-    if (G < 32 && (32 % G) == 0 && (blockDim.x % 32) == 0) {
-        // lanes l and l + k*G of a warp hold the same column group (the grid stride keeps g = tid % G)
+// Column sums of values held 8-per-thread (column group g = (global thread index) % G of G = C/8, fixed by a grid
+// stride that is a multiple of G; threads at or beyond `stride` hold nothing): every thread parks its 8 sums in
+// s_thr ([blockDim.x][8] floats), column c of this CTA is the sum over the threads of group c/8 in thread order,
+// stored into row blockIdx.x of `partial`; then tfy_rows_publish.
+__device__ __forceinline__ void tfy_block_colsum_publish(const float (&colacc)[8], int C, size_t stride, float* s_thr,
+                                                         float* partial, __nv_bfloat16* out, uint32_t* counter) {
+    const int G = C / 8;
 #pragma unroll
-        for (int k = 0; k < 8; ++k) {
-            float v = active ? colacc[k] : 0.f;
-            for (int off = G; off < 32; off <<= 1) v += __shfl_xor_sync(0xffffffffu, v, off);
-            colacc[k] = v;
-        }
-        if ((threadIdx.x & 31) < G) {
-#pragma unroll
-            for (int k = 0; k < 8; ++k) atomicAdd(&s_sum[g * 8 + k], colacc[k]);
-        }
-    } else if (active) {
-#pragma unroll
-        for (int k = 0; k < 8; ++k) atomicAdd(&s_sum[g * 8 + k], colacc[k]);
-    }
+    for (int k = 0; k < 8; ++k) s_thr[threadIdx.x * 8 + k] = colacc[k];
     __syncthreads();
+    const size_t base = (size_t)blockIdx.x * blockDim.x;
+    const int live = stride > base ? (int)min((size_t)blockDim.x, stride - base) : 0;     // threads holding sums
+    const int g0 = (int)(base % G);                                                          // group of thread 0
+    float* row = partial + (size_t)blockIdx.x * C;
+    for (int c = threadIdx.x; c < C; c += blockDim.x) {
+        const int g = c >> 3, k = c & 7;
+        float a = 0.f;
+        for (int t = (g - g0 + G) % G; t < live; t += G) a += s_thr[t * 8 + k];
+        __stcg(row + c, a);
+    }
+    tfy_rows_publish(C, partial, out, counter, s_thr);
 }
 
 }  // namespace
@@ -131,17 +146,17 @@ tfy_conv3x3_c1_fwd_kernel(const XT* __restrict__ x, const __nv_bfloat16* __restr
 // lane <-> output channel (blocks of 32 channels).  A warp owns whole output rows (b, oh): it loads the
 // three input rows it needs ONCE (coalesced, lane = column; W <= 32 fast path) and walks ow with the
 // window values coming from warp shuffles -- per pixel one 64-byte dz load, 9 shuffles, 9 FMAs and no
-// integer division.  Warps are combined in shared memory, CTAs through tfy_colsum_publish.
+// integer division.  Warps are combined in warp order through one shared row per warp, CTAs through
+// tfy_rows_publish.
 template <typename XT>
 __global__ void __launch_bounds__(256)
 tfy_conv3x3_c1_wgrad_kernel(const XT* __restrict__ x, const __nv_bfloat16* __restrict__ dz,
                             float* __restrict__ partial, __nv_bfloat16* __restrict__ dw, uint32_t* counter, int B,
                             int H, int W, int O) {
-    extern __shared__ float s_acc[];   // [9*O] CTA accumulator
+    extern __shared__ float s_acc[];   // [9*O] CTA sums | [warps][9][32] this channel block's per-warp sums
     const int OH = H - 2, OW = W - 2;
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nwarps = blockDim.x >> 5;
-    for (int i = threadIdx.x; i < 9 * O; i += blockDim.x) s_acc[i] = 0.f;
-    __syncthreads();
+    float* s_warp = s_acc + 9 * O;
     const int nrows = B * OH;
     const int gw = blockIdx.x * nwarps + warp, tw = gridDim.x * nwarps;
     for (int o0 = 0; o0 < O; o0 += 32) {
@@ -177,13 +192,20 @@ tfy_conv3x3_c1_wgrad_kernel(const XT* __restrict__ x, const __nv_bfloat16* __res
                 }
             }
         }
-        if (o_ok) {
 #pragma unroll
-            for (int t = 0; t < 9; ++t) atomicAdd(&s_acc[o * 9 + t], acc[t]);
+        for (int t = 0; t < 9; ++t) s_warp[(warp * 9 + t) * 32 + lane] = acc[t];
+        __syncthreads();
+        for (int i = threadIdx.x; i < 9 * 32; i += blockDim.x) {       // i = t * 32 + lane of channel o0 + lane
+            const int t = i >> 5, o = o0 + (i & 31);
+            float a = 0.f;
+            for (int w = 0; w < nwarps; ++w) a += s_warp[w * 9 * 32 + i];
+            if (o < O) s_acc[o * 9 + t] = a;
         }
+        __syncthreads();
     }
-    __syncthreads();
-    tfy_colsum_publish(s_acc, 9 * O, partial, dw, counter);
+    float* row = partial + (size_t)blockIdx.x * 9 * O;
+    for (int i = threadIdx.x; i < 9 * O; i += blockDim.x) __stcg(row + i, s_acc[i]);
+    tfy_rows_publish(9 * O, partial, dw, counter, s_warp);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -247,9 +269,7 @@ tfy_act_drop_bwd_bias_kernel(const __nv_bfloat16* dy, const uint8_t* __restrict_
                              const __nv_bfloat16* __restrict__ y, __nv_bfloat16* dz, float scale, size_t rows, int C,
                              float* __restrict__ partial, __nv_bfloat16* __restrict__ dbias, uint32_t* counter) {
     tfy_pdl_sync();
-    extern __shared__ float s_sum[];  // [C]
-    for (int c = threadIdx.x; c < C; c += blockDim.x) s_sum[c] = 0.f;
-    __syncthreads();
+    extern __shared__ float s_thr[];  // [blockDim.x][8] per-thread column sums
     const int G = C / 8;
     const size_t total = rows * G;
     // each thread keeps a fixed column group: stride must be a multiple of G
@@ -257,7 +277,6 @@ tfy_act_drop_bwd_bias_kernel(const __nv_bfloat16* dy, const uint8_t* __restrict_
     float colacc[8] = {0, 0, 0, 0, 0, 0, 0, 0};
     const size_t start = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
     const bool active = start < stride;
-    const int g = (int)(start % G);
     if (active) {
         for (size_t idx = start; idx < total; idx += stride) {
             float v[8];
@@ -280,10 +299,7 @@ tfy_act_drop_bwd_bias_kernel(const __nv_bfloat16* dy, const uint8_t* __restrict_
             for (int k = 0; k < 8; ++k) colacc[k] += v[k];
         }
     }
-    if (dbias) {
-        tfy_block_colsum(colacc, g, G, active, s_sum);
-        tfy_colsum_publish(s_sum, C, partial, dbias, counter);
-    }
+    if (dbias) tfy_block_colsum_publish(colacc, C, stride, s_thr, partial, dbias, counter);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -350,9 +366,7 @@ tfy_pool_drop_relu_bwd_kernel(const __nv_bfloat16* __restrict__ dp, const uint8_
                               __nv_bfloat16* __restrict__ dz, float scale, int B, int H, int W, int C,
                               float* __restrict__ partial, __nv_bfloat16* __restrict__ dbias, uint32_t* counter) {
     tfy_pdl_sync();
-    extern __shared__ float s_sum[];
-    for (int c = threadIdx.x; c < C; c += blockDim.x) s_sum[c] = 0.f;
-    __syncthreads();
+    extern __shared__ float s_thr[];  // [blockDim.x][8] per-thread column sums
     const int PH = H / 2, PW = W / 2, G = C / 8;
     const size_t total = (size_t)B * PH * PW * G;
     const size_t stride = ((size_t)gridDim.x * blockDim.x / G) * G;
@@ -388,98 +402,23 @@ tfy_pool_drop_relu_bwd_kernel(const __nv_bfloat16* __restrict__ dp, const uint8_
             }
         }
     }
-    if (dbias) {
-        tfy_block_colsum(colacc, g, G, active, s_sum);
-        tfy_colsum_publish(s_sum, C, partial, dbias, counter);
-    }
+    if (dbias) tfy_block_colsum_publish(colacc, C, stride, s_thr, partial, dbias, counter);
 }
 
 // ---------------------------------------------------------------------------------------------
-// softmax cross-entropy head.  logits [B,C] bf16 (+ optional bias[C]), labels int64.
-// Single CTA (B rows strided over the threads): loss = mean CE (fp32), dlogits = (softmax-onehot)/B
-// (bf16), dbias[C] = column sums of dlogits (bf16), stats[0] += #correct, stats[1] += B.
+// softmax cross-entropy head.  logits [B,C] bf16 (+ optional bias[C]), labels int64.  Single CTA (B rows strided
+// over the threads).  Row r weighs w_r = sample_w[r] * class_w[label_r] (Keras sample_weight / class_weight; a null
+// pointer, or a label outside [0, C), counts as 1): loss = sum_r w_r l_r / B (fp32), dlogits = w_r (softmax - onehot)
+// / B (bf16), dbias = column sums of dlogits (bf16), stats[0..n_stats) += [hits, B, sum w*hit, sum w] (n_stats 2 or
+// 4).  Every block-level sum is taken in a fixed order (warp shuffles, then warps in index order; dbias from one
+// partial row per warp), so the result is the same bit for bit on every run.
 // ---------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(1024)
-tfy_softmax_xent_kernel(const __nv_bfloat16* __restrict__ logits, const __nv_bfloat16* __restrict__ bias,
-                        const long long* __restrict__ labels, float* __restrict__ loss,
-                        __nv_bfloat16* __restrict__ dlogits, __nv_bfloat16* __restrict__ dbias,
-                        float* __restrict__ stats, int B, int C) {
-    extern __shared__ float sm[];  // [C] bias | [C] dbias accumulators | [2] loss, correct
-    float* s_bias = sm;
-    float* s_db = sm + C;
-    float* s_red = sm + 2 * C;
-    for (int c = threadIdx.x; c < C; c += blockDim.x) {
-        s_bias[c] = bias ? bf16_to_f(bias[c]) : 0.f;
-        s_db[c] = 0.f;
-    }
-    if (threadIdx.x < 2) s_red[threadIdx.x] = 0.f;
-    __syncthreads();
-    const float invB = 1.f / (float)B;
-    const int lane = threadIdx.x & 31;
-    float my_loss = 0.f, my_correct = 0.f;
-    // every warp iterates the same number of times so that the shuffles below stay convergent
-    const int rounds = (B + blockDim.x - 1) / blockDim.x;
-    for (int it = 0; it < rounds; ++it) {
-        const int r = it * blockDim.x + threadIdx.x;
-        const bool ok = r < B;
-        const __nv_bfloat16* row = logits + (size_t)(ok ? r : 0) * C;
-        float mx = -3.0e38f;
-        int amax = 0;
-        for (int c = 0; c < C; ++c) {
-            const float v = bf16_to_f(row[c]) + s_bias[c];
-            if (v > mx) { mx = v; amax = c; }
-        }
-        float se = 0.f;
-        for (int c = 0; c < C; ++c) se += __expf(bf16_to_f(row[c]) + s_bias[c] - mx);
-        const float lse = mx + __logf(se);
-        const int lab = ok ? (int)labels[r] : 0;
-        const float inv_se = 1.f / se;
-        for (int c = 0; c < C; ++c) {
-            const float v = bf16_to_f(row[c]) + s_bias[c];
-            float d = (__expf(v - mx) * inv_se - (c == lab ? 1.f : 0.f)) * invB;
-            if (!ok) d = 0.f;
-            if (ok) {
-                if (c == lab) my_loss += lse - v;
-                dlogits[(size_t)r * C + c] = __float2bfloat16(d);
-            }
-            if (dbias) {
-                float t = d;
-#pragma unroll
-                for (int off = 16; off > 0; off >>= 1) t += __shfl_xor_sync(0xffffffffu, t, off);
-                if (lane == 0) atomicAdd(&s_db[c], t);
-            }
-        }
-        if (ok) my_correct += (amax == lab) ? 1.f : 0.f;
-    }
-#pragma unroll
-    for (int off = 16; off > 0; off >>= 1) {
-        my_loss += __shfl_xor_sync(0xffffffffu, my_loss, off);
-        my_correct += __shfl_xor_sync(0xffffffffu, my_correct, off);
-    }
-    if (lane == 0) {
-        atomicAdd(&s_red[0], my_loss);
-        atomicAdd(&s_red[1], my_correct);
-    }
-    __syncthreads();
-    if (threadIdx.x == 0) {
-        *loss = s_red[0] * invB;
-        if (stats) { stats[0] += s_red[1]; stats[1] += (float)B; }
-    }
-    if (dbias)
-        for (int c = threadIdx.x; c < C; c += blockDim.x) dbias[c] = __float2bfloat16(s_db[c]);
-}
-
-// Weighted form of the head above (Keras sample_weight / class_weight): row r weighs
-// w_r = sample_w[r] * class_w[label_r] (a null pointer, or a label outside [0, C), counts as 1).
-// loss = sum_r w_r l_r / B, dlogits = w_r (softmax - onehot) / B, dbias = column sums of dlogits,
-// stats[0..3] += [hits, B, sum w*hit, sum w].  Every block-level sum is taken in a fixed order (warp shuffles,
-// then warps in index order; dbias from one partial row per warp), so the result is the same bit for bit on every run.
 __global__ void __launch_bounds__(1024)
 tfy_softmax_xent_weighted_kernel(const __nv_bfloat16* __restrict__ logits, const __nv_bfloat16* __restrict__ bias,
                                  const long long* __restrict__ labels, const float* __restrict__ sample_w,
                                  const float* __restrict__ class_w, float* __restrict__ loss,
                                  __nv_bfloat16* __restrict__ dlogits, __nv_bfloat16* __restrict__ dbias,
-                                 float* __restrict__ stats, int B, int C) {
+                                 float* __restrict__ stats, int n_stats, int B, int C) {
     tfy_pdl_sync();
     extern __shared__ float sm[];  // [C] bias | [warps][C] dbias partials | [warps][4] loss, hits, w*hits, w
     const int warps = blockDim.x >> 5, warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -545,7 +484,11 @@ tfy_softmax_xent_weighted_kernel(const __nv_bfloat16* __restrict__ logits, const
         for (int w = 0; w < warps; ++w)
             for (int k = 0; k < 4; ++k) t[k] += s_red[w * 4 + k];
         *loss = t[0] * invB;
-        if (stats) { stats[0] += t[1]; stats[1] += (float)B; stats[2] += t[2]; stats[3] += t[3]; }
+        if (stats) {
+            stats[0] += t[1];
+            stats[1] += (float)B;
+            if (n_stats > 2) { stats[2] += t[2]; stats[3] += t[3]; }
+        }
     }
     if (dbias)
         for (int c = threadIdx.x; c < C; c += blockDim.x) {
@@ -935,8 +878,12 @@ static inline int tfy_grid_for(size_t items, int block, int cap) {
 
 extern "C" {
 
-// scratch: fp32 workspace of at least tfy_nn_scratch_floats(...) floats; counter: zero-initialised u32
-size_t tfy_nn_max_partial_blocks() { return 592; }
+// The kernels with a bias / weight-gradient reduction (tfy_conv3x3_c1_wgrad, tfy_act_drop_bwd_bias,
+// tfy_pool_drop_relu_bwd) take `partial`: one row of their reduction width per CTA, for at most
+// TFY_PARTIAL_BLOCKS CTAs (the launchers refuse a larger grid with -3), and `counter`: one zero-initialised u32,
+// left zero.
+#define TFY_PARTIAL_BLOCKS 592
+size_t tfy_nn_max_partial_blocks() { return TFY_PARTIAL_BLOCKS; }
 
 int tfy_conv3x3_c1_fwd(const void* x, int x_is_f32, const void* w, const void* bias, void* y, int B, int H, int W,
                        int O, cudaStream_t s) {
@@ -956,13 +903,16 @@ int tfy_conv3x3_c1_fwd(const void* x, int x_is_f32, const void* w, const void* b
 
 int tfy_conv3x3_c1_wgrad(const void* x, int x_is_f32, const void* dz, float* partial, void* dw, uint32_t* counter,
                          int B, int H, int W, int O, cudaStream_t s) {
-    const int grid = 296;
-    const size_t smem = (size_t)(9 * O > 256 ? 9 * O : 256) * sizeof(float);
+    if (O < 1 || B < 1 || H < 3 || W < 3) return -2;
+    const int grid = 296, block = 256;
+    static_assert(296 <= TFY_PARTIAL_BLOCKS, "one partial row per CTA");
+    const size_t smem = ((size_t)9 * O + (size_t)(block / 32) * 9 * 32) * sizeof(float);
+    if (smem > 48 * 1024) return -2;
     if (x_is_f32)
-        tfy_conv3x3_c1_wgrad_kernel<float><<<grid, 256, smem, s>>>((const float*)x, (const __nv_bfloat16*)dz, partial,
+        tfy_conv3x3_c1_wgrad_kernel<float><<<grid, block, smem, s>>>((const float*)x, (const __nv_bfloat16*)dz, partial,
                                                                     (__nv_bfloat16*)dw, counter, B, H, W, O);
     else
-        tfy_conv3x3_c1_wgrad_kernel<__nv_bfloat16><<<grid, 256, smem, s>>>(
+        tfy_conv3x3_c1_wgrad_kernel<__nv_bfloat16><<<grid, block, smem, s>>>(
             (const __nv_bfloat16*)x, (const __nv_bfloat16*)dz, partial, (__nv_bfloat16*)dw, counter, B, H, W, O);
     return (int)cudaGetLastError();
 }
@@ -992,10 +942,11 @@ int tfy_bias_act_drop_fwd_f32(void* z32, const void* bias, void* y, void* mask, 
 int tfy_act_drop_bwd_bias(const void* dy, const void* mask, const void* y, void* dz, float scale, size_t rows, int C,
                           float* partial, void* dbias, uint32_t* counter, cudaStream_t s) {
     if (C % 8) return -2;
-    int grid = tfy_grid_for(rows * (C / 8), 256, 592);
+    int grid = tfy_grid_for(rows * (C / 8), 256, TFY_PARTIAL_BLOCKS);
     // the kernel needs gridDim*blockDim >= C/8 so that every column group has a thread
     if ((size_t)grid * 256 < (size_t)(C / 8)) grid = (C / 8 + 255) / 256;
-    tfy_launch_pdl((tfy_act_drop_bwd_bias_kernel), dim3(grid), dim3(256), (C > 256 ? C : 256) * sizeof(float), s, 
+    if (dbias && grid > TFY_PARTIAL_BLOCKS) return -3;
+    tfy_launch_pdl((tfy_act_drop_bwd_bias_kernel), dim3(grid), dim3(256), 256 * 8 * sizeof(float), s, 
         (const __nv_bfloat16*)dy, (const uint8_t*)mask, (const __nv_bfloat16*)y, (__nv_bfloat16*)dz, scale, rows, C,
         partial, (__nv_bfloat16*)dbias, counter);
     return (int)cudaGetLastError();
@@ -1016,39 +967,43 @@ int tfy_pool_drop_relu_bwd(const void* dp, const void* code, void* dz, float sca
                            float* partial, void* dbias, uint32_t* counter, cudaStream_t s) {
     if (C % 8 || H % 2 || W % 2) return -2;
     const size_t total = (size_t)B * (H / 2) * (W / 2) * (C / 8);
-    int grid = tfy_grid_for(total, 256, 592);
-    tfy_launch_pdl((tfy_pool_drop_relu_bwd_kernel), dim3(grid), dim3(256), (C > 256 ? C : 256) * sizeof(float), s, 
+    const int grid = tfy_grid_for(total, 256, TFY_PARTIAL_BLOCKS);
+    if ((size_t)grid * 256 < (size_t)(C / 8)) return -3;      // every column group needs a thread
+    tfy_launch_pdl((tfy_pool_drop_relu_bwd_kernel), dim3(grid), dim3(256), 256 * 8 * sizeof(float), s, 
         (const __nv_bfloat16*)dp, (const uint8_t*)code, (__nv_bfloat16*)dz, scale, B, H, W, C, partial,
         (__nv_bfloat16*)dbias, counter);
     return (int)cudaGetLastError();
 }
 
-int tfy_softmax_xent(const void* logits, const void* bias, const void* labels, float* loss, void* dlogits,
-                     void* dbias, float* stats, int B, int C, cudaStream_t s) {
-    int block = B < 1024 ? ((B + 31) / 32) * 32 : 1024;
-    if (block < 32) block = 32;
-    tfy_softmax_xent_kernel<<<1, block, (2 * C + 2) * sizeof(float), s>>>(
-        (const __nv_bfloat16*)logits, (const __nv_bfloat16*)bias, (const long long*)labels, loss,
-        (__nv_bfloat16*)dlogits, (__nv_bfloat16*)dbias, stats, B, C);
-    return (int)cudaGetLastError();
-}
-
-// weighted variant: sample_w [B] and class_w [C] fp32 (either may be null), stats null or 4 floats
-// [hits, B, sum w*hit, sum w]; returns -2 when C is too wide for one partial row of dbias per warp
-int tfy_softmax_xent_weighted(const void* logits, const void* bias, const void* labels, const float* sample_w,
-                              const float* class_w, float* loss, void* dlogits, void* dbias, float* stats, int B, int C,
-                              cudaStream_t s) {
+static int tfy_softmax_xent_launch(const void* logits, const void* bias, const void* labels, const float* sample_w,
+                                   const float* class_w, float* loss, void* dlogits, void* dbias, float* stats,
+                                   int n_stats, int B, int C, cudaStream_t s) {
     if (B < 1 || C < 1) return -2;
     const int max_warps = (int)((48 * 1024 / sizeof(float) - (size_t)C) / ((size_t)C + 4));
-    if (max_warps < 1) return -2;
+    if ((size_t)C >= 48 * 1024 / sizeof(float) || max_warps < 1) return -2;
     int warps = (B + 31) / 32;
     if (warps > 32) warps = 32;
     if (warps > max_warps) warps = max_warps;
     const size_t smem = ((size_t)C + (size_t)warps * (C + 4)) * sizeof(float);
     tfy_launch_pdl((tfy_softmax_xent_weighted_kernel), dim3(1), dim3(warps * 32), smem, s,
                    (const __nv_bfloat16*)logits, (const __nv_bfloat16*)bias, (const long long*)labels, sample_w,
-                   class_w, loss, (__nv_bfloat16*)dlogits, (__nv_bfloat16*)dbias, stats, B, C);
+                   class_w, loss, (__nv_bfloat16*)dlogits, (__nv_bfloat16*)dbias, stats, n_stats, B, C);
     return (int)cudaGetLastError();
+}
+
+// unweighted head (every weight 1), stats null or 2 floats [hits, B]; returns -2 when C is too wide for one partial
+// row of dbias per warp (C > 9000 or so)
+int tfy_softmax_xent(const void* logits, const void* bias, const void* labels, float* loss, void* dlogits,
+                     void* dbias, float* stats, int B, int C, cudaStream_t s) {
+    return tfy_softmax_xent_launch(logits, bias, labels, nullptr, nullptr, loss, dlogits, dbias, stats, 2, B, C, s);
+}
+
+// weighted variant: sample_w [B] and class_w [C] fp32 (either may be null), stats null or 4 floats
+// [hits, B, sum w*hit, sum w]; same return codes
+int tfy_softmax_xent_weighted(const void* logits, const void* bias, const void* labels, const float* sample_w,
+                              const float* class_w, float* loss, void* dlogits, void* dbias, float* stats, int B, int C,
+                              cudaStream_t s) {
+    return tfy_softmax_xent_launch(logits, bias, labels, sample_w, class_w, loss, dlogits, dbias, stats, 4, B, C, s);
 }
 
 // thin cudaMemcpyAsync wrapper: the input pipeline issues its per-step copies through ctypes (about 1 us per call
