@@ -6,8 +6,11 @@ BASELINE config (categorical + embedding columns).
 """
 from __future__ import annotations
 
+import hashlib
+import re
 from typing import Dict, List, NamedTuple, Optional, Sequence, Tuple, Union
 
+import numpy as np
 import torch
 import torch.nn as nn
 import torch.nn.functional as F
@@ -50,7 +53,8 @@ class WeightedCategoricalColumn(NamedTuple):
 
     @property
     def hashed(self) -> bool:
-        return self.categorical_column.hashed
+        """Whether the ids are hashed (a vocabulary column's never are)."""
+        return isinstance(self.categorical_column, CategoricalColumn) and self.categorical_column.hashed
 
 
 class BucketizedColumn(NamedTuple):
@@ -90,8 +94,8 @@ class CrossedColumn(NamedTuple):
         ShiftMix(x) = x ^ (x >> 47)                (mod 2^64, logical shift)
 
     An absent slot is -1.  The formula follows TF's ``SparseCrossHashed``; that the ids are TF's own has not been
-    checked against TF."""
-    keys: Tuple[Union[str, CategoricalColumn, BucketizedColumn], ...]     # the leaf keys, nested crosses flattened
+    checked against TF.  A vocabulary column's OOV buckets are not TF's either (see VocabularyColumn)."""
+    keys: Tuple[Union[str, CategoricalColumn, BucketizedColumn, "VocabularyColumn"], ...]   # nested crosses flattened
     hash_bucket_size: int
     hash_key: int = CROSS_HASH_KEY
 
@@ -104,7 +108,128 @@ class CrossedColumn(NamedTuple):
         return self.hash_bucket_size
 
 
-Categorical = Union[CategoricalColumn, WeightedCategoricalColumn, BucketizedColumn, CrossedColumn]
+MAX_VOCABULARY = 2 ** 31 - 1            # entries of one vocabulary: its ids are int32 on the device
+HASH_MULT = 2654435761                  # categorical_column_with_hash_bucket's multiplicative hash
+
+
+class Vocabulary:
+    """The entries of a vocabulary column, in list (or file) order, as a read-only int64 array: entry i has id i.
+
+    Immutable.  Equality and hashing go through a SHA-256 digest of the entries computed once, so a column holding a
+    million entries is as cheap a dict key as any other; it pickles its entries only.  ``tables(device)`` gives the
+    keys sorted ascending with the id of each, built once per device and shared by every user of the vocabulary there
+    (the torch statement and the HBM plane's id kernels), so a lookup never re-sorts or re-uploads."""
+
+    __slots__ = ("_keys", "_digest", "_sorted", "_tables")
+
+    def __init__(self, entries):
+        keys = _vocabulary_entries(entries)
+        keys.setflags(write=False)
+        self._keys = keys
+        self._digest = hashlib.sha256(keys.tobytes()).digest()
+        order = np.argsort(keys, kind="stable")
+        skeys = keys[order]
+        if skeys.size > 1 and bool(np.any(skeys[1:] == skeys[:-1])):
+            dup = skeys[1:][skeys[1:] == skeys[:-1]][0]
+            raise ValueError(f"vocabulary has duplicate entries, e.g. {int(dup)}")
+        skeys.setflags(write=False)
+        ids = order.astype(np.int32)
+        ids.setflags(write=False)
+        self._sorted = (skeys, ids)
+        self._tables: Dict[torch.device, Tuple[torch.Tensor, torch.Tensor]] = {}
+
+    @property
+    def keys(self) -> np.ndarray:
+        """int64 [n] entries in id order (read-only)."""
+        return self._keys
+
+    @property
+    def sorted(self) -> Tuple[np.ndarray, np.ndarray]:
+        """(int64 keys sorted ascending, int32 id of each), read-only host arrays."""
+        return self._sorted
+
+    def tables(self, device) -> Tuple[torch.Tensor, torch.Tensor]:
+        """The sorted keys (int64) and their ids (int32) on ``device``, uploaded on first use.  Read-only: every user
+        of the vocabulary on that device shares them."""
+        device = torch.device(device)
+        if device.type == "cuda" and device.index is None:
+            device = torch.device("cuda", torch.cuda.current_device())
+        t = self._tables.get(device)
+        if t is None:
+            skeys, ids = self._sorted
+            t = (torch.from_numpy(skeys.copy()).to(device), torch.from_numpy(ids.copy()).to(device))
+            self._tables[device] = t
+        return t
+
+    def __len__(self) -> int:
+        return int(self._keys.size)
+
+    def __eq__(self, other) -> bool:
+        return isinstance(other, Vocabulary) and self._digest == other._digest
+
+    def __hash__(self) -> int:
+        return hash(self._digest)
+
+    def __reduce__(self):
+        return Vocabulary, (self._keys,)
+
+    def __repr__(self) -> str:
+        head = ", ".join(str(int(k)) for k in self._keys[:4])
+        return f"Vocabulary(n={len(self)}, [{head}{', ...' if len(self) > 4 else ''}], sha256={self._digest[:6].hex()})"
+
+
+def _vocabulary_entries(entries) -> np.ndarray:
+    """int64 [n] array of a vocabulary's entries, each an integer in [0, 2^63); ValueError otherwise."""
+    if isinstance(entries, np.ndarray):
+        if entries.ndim != 1 or entries.dtype.kind not in "iu":
+            raise ValueError(f"vocabulary entries must be a 1-D array of integers in [0, 2^63), got an array of "
+                             f"shape {entries.shape} and dtype {entries.dtype}")
+        n = entries.size
+    else:
+        if isinstance(entries, (str, bytes)):
+            raise ValueError(f"vocabulary must be a list of integers, got {entries!r}")
+        n = len(entries)
+    if n == 0:
+        raise ValueError("vocabulary is empty")
+    if n > MAX_VOCABULARY:
+        raise ValueError(f"vocabulary has {n} entries; at most 2^31 - 1 are supported")
+    if isinstance(entries, np.ndarray):
+        if entries.min() < 0 or (entries.dtype.kind == "u" and int(entries.max()) >= 2 ** 63):
+            raise ValueError("vocabulary entries must be integers in [0, 2^63)")
+        return np.array(entries, dtype=np.int64, copy=True)       # a private copy: the caller's array stays its own
+    for v in entries:
+        if isinstance(v, (bool, np.bool_)) or not isinstance(v, (int, np.integer)) or not 0 <= int(v) < 2 ** 63:
+            raise ValueError(f"vocabulary entries must be integers in [0, 2^63), got {v!r}; no column here takes "
+                             f"string features")
+    return np.array([int(v) for v in entries], dtype=np.int64)
+
+
+class VocabularyColumn(NamedTuple):
+    """``tf.feature_column.categorical_column_with_vocabulary_list`` / ``_file`` over integer features.
+
+    Entry i of ``vocabulary`` (its position in the list, its line in the file) has id i; n = len(vocabulary) and
+    ``num_buckets = n + num_oov_buckets``.  A raw value v maps to:
+
+    * -1 (missing) if v < 0, the convention of every column here (TF treats only -1 as missing for integers);
+    * its id if v is in the vocabulary;
+    * else, with ``num_oov_buckets > 0``: ``n + ((uint64) v * 2654435761 mod 2^32) % num_oov_buckets``, the hash of
+      ``categorical_column_with_hash_bucket``.  These OOV ids are not TF's, which hashes the decimal string with
+      Fingerprint64;
+    * else ``default_value`` (-1, the default, is absent).
+
+    The ids are the same on every path: the torch statement (``_vocabulary_ids``, a searchsorted over the sorted keys)
+    and the HBM parameter server's ``tfy_vocab_ids`` kernel, a binary search over the same keys."""
+    key: str
+    vocabulary: Vocabulary
+    num_oov_buckets: int = 0
+    default_value: int = -1
+
+    @property
+    def num_buckets(self) -> int:
+        return len(self.vocabulary) + self.num_oov_buckets
+
+
+Categorical = Union[CategoricalColumn, WeightedCategoricalColumn, BucketizedColumn, CrossedColumn, VocabularyColumn]
 DERIVED = (BucketizedColumn, CrossedColumn)         # columns whose ids are computed from other features
 
 
@@ -145,9 +270,83 @@ def categorical_column_with_hash_bucket(key: str, hash_bucket_size: int, **_igno
     return CategoricalColumn(key, int(hash_bucket_size), True)
 
 
-def weighted_categorical_column(categorical_column: CategoricalColumn, weight_feature_key: str,
+_INT_DTYPES = (None, torch.int32, torch.int64, "int32", "int64")
+
+
+def _integer(fn: str, name: str, v) -> int:
+    """v as an int; ValueError for anything but an integer (a float is not truncated, a bool is not a count)."""
+    if isinstance(v, (bool, np.bool_)) or not isinstance(v, (int, np.integer)):
+        raise ValueError(f"{fn}: {name} must be an integer, got {v!r}")
+    return int(v)
+
+
+def _vocabulary_column(fn: str, key: str, vocabulary: Vocabulary, num_oov_buckets, default_value, dtype):
+    if not any(dtype is d or (isinstance(dtype, str) and dtype == d) for d in _INT_DTYPES):
+        raise ValueError(f"{fn}: dtype must be None, torch.int32/torch.int64 or 'int32'/'int64', got {dtype!r}; no "
+                         f"column here takes string features")
+    n, oov, dflt = len(vocabulary), _integer(fn, "num_oov_buckets", num_oov_buckets), \
+        _integer(fn, "default_value", default_value)
+    if not 0 <= oov <= MAX_VOCABULARY:
+        raise ValueError(f"{fn}: num_oov_buckets must be in [0, 2^31), got {num_oov_buckets}")
+    if oov > 0 and dflt != -1:
+        raise ValueError(f"{fn}: set either num_oov_buckets ({oov}) or default_value ({dflt}), not both")
+    if not -1 <= dflt < n:
+        raise ValueError(f"{fn}: default_value must be -1 or an id in [0, {n}), got {default_value}")
+    return VocabularyColumn(key, vocabulary, oov, dflt)
+
+
+def categorical_column_with_vocabulary_list(key: str, vocabulary_list, dtype=None, default_value: int = -1,
+                                            num_oov_buckets: int = 0) -> VocabularyColumn:
+    """Ids of an integer feature by its position in ``vocabulary_list`` (see VocabularyColumn).  The entries must be
+    distinct integers in [0, 2^63)."""
+    return _vocabulary_column("categorical_column_with_vocabulary_list", key, Vocabulary(vocabulary_list),
+                              num_oov_buckets, default_value, dtype)
+
+
+_DECIMAL = re.compile(r"[+-]?[0-9]+")
+
+
+def _read_vocabulary_file(path: str, vocabulary_size: Optional[int]) -> List[int]:
+    """The entries of a vocabulary file: one base-10 integer per line, surrounding whitespace stripped, a single
+    trailing newline allowed; the first ``vocabulary_size`` lines if given."""
+    with open(path, "r") as fh:
+        text = fh.read()
+    lines = text.split("\n")
+    if lines and lines[-1] == "":
+        lines.pop()
+    if vocabulary_size is not None:
+        vocabulary_size = _integer("categorical_column_with_vocabulary_file", "vocabulary_size", vocabulary_size)
+        if not 1 <= vocabulary_size <= len(lines):
+            raise ValueError(f"vocabulary file {path!r}: vocabulary_size must be in [1, {len(lines)}] (its number of "
+                             f"lines), got {vocabulary_size}")
+        lines = lines[:vocabulary_size]
+    out = []
+    for i, line in enumerate(lines):
+        s = line.strip()
+        if not _DECIMAL.fullmatch(s):
+            raise ValueError(f"vocabulary file {path!r}, line {i + 1}: expected one base-10 integer, got {line!r}")
+        out.append(int(s))
+    return out
+
+
+def categorical_column_with_vocabulary_file(key: str, vocabulary_file: str, vocabulary_size: Optional[int] = None,
+                                            num_oov_buckets: int = 0, default_value: Optional[int] = None,
+                                            dtype=None) -> VocabularyColumn:
+    """Ids of an integer feature by its line in ``vocabulary_file`` (see VocabularyColumn), read once, here."""
+    fn = "categorical_column_with_vocabulary_file"
+    if default_value is None:
+        default_value = -1
+    elif _integer(fn, "num_oov_buckets", num_oov_buckets) > 0:
+        raise ValueError(f"categorical_column_with_vocabulary_file: set either num_oov_buckets ({num_oov_buckets}) "
+                         f"or default_value ({default_value}), not both")
+    return _vocabulary_column("categorical_column_with_vocabulary_file", key,
+                              Vocabulary(_read_vocabulary_file(vocabulary_file, vocabulary_size)), num_oov_buckets,
+                              default_value, dtype)
+
+
+def weighted_categorical_column(categorical_column: Union[CategoricalColumn, VocabularyColumn], weight_feature_key: str,
                                 dtype: torch.dtype = torch.float32) -> WeightedCategoricalColumn:
-    if not isinstance(categorical_column, CategoricalColumn):
+    if not isinstance(categorical_column, (CategoricalColumn, VocabularyColumn)):
         raise ValueError(f"weighted_categorical_column wraps a categorical column, got {categorical_column!r}")
     if not dtype.is_floating_point:
         raise ValueError(f"weighted_categorical_column: dtype must be a float type, got {dtype}")
@@ -177,11 +376,11 @@ def crossed_column(keys: Sequence, hash_bucket_size: int, hash_key: Optional[int
         elif isinstance(k, CategoricalColumn) and k.hashed:
             raise ValueError(f"crossed_column does not support a hashed categorical column, got {k!r}; cross its "
                              f"raw feature {k.key!r} instead")
-        elif isinstance(k, (str, CategoricalColumn, BucketizedColumn)):
+        elif isinstance(k, (str, CategoricalColumn, BucketizedColumn, VocabularyColumn)):
             leaves.append(k)
         else:
-            raise ValueError(f"crossed_column keys must be feature names, identity categorical, bucketized or "
-                             f"crossed columns, got {k!r}")
+            raise ValueError(f"crossed_column keys must be feature names, identity categorical, vocabulary, "
+                             f"bucketized or crossed columns, got {k!r}")
     if len(leaves) < 2:
         raise ValueError(f"crossed_column needs at least two keys, got {keys!r}")
     if not 1 <= int(hash_bucket_size) < MAX_CROSS_BUCKETS:
@@ -206,6 +405,8 @@ def _kind(c) -> Optional[str]:
     c = c.categorical_column if isinstance(c, WeightedCategoricalColumn) else c
     if isinstance(c, CategoricalColumn):
         return "hashed" if c.hashed else "identity"
+    if isinstance(c, VocabularyColumn):
+        return "vocabulary"
     return type(c).__name__ if isinstance(c, DERIVED) else None
 
 
@@ -252,7 +453,29 @@ def indicator_column(categorical_column: Categorical) -> IndicatorColumn:
 def _categorical(c) -> Optional[Categorical]:
     """The categorical column a wide-tower column is looked up by (None for a numeric column)."""
     c = c.categorical_column if isinstance(c, (EmbeddingColumn, IndicatorColumn)) else c
-    return c if isinstance(c, (CategoricalColumn, WeightedCategoricalColumn) + DERIVED) else None
+    return c if isinstance(c, (CategoricalColumn, WeightedCategoricalColumn, VocabularyColumn) + DERIVED) else None
+
+
+def _device_ids(c) -> bool:
+    """True for a column whose ids the HBM parameter server builds on the device (ops/features.py FeatureIds):
+    bucketized, crossed and vocabulary columns, the last also inside a weighted column."""
+    c = c.categorical_column if isinstance(c, WeightedCategoricalColumn) else c
+    return isinstance(c, DERIVED + (VocabularyColumn,))
+
+
+def _vocabulary_ids(col: VocabularyColumn, t: torch.Tensor) -> torch.Tensor:
+    """Ids of a vocabulary column's raw values, same shape (see VocabularyColumn): a lower-bound search over the
+    vocabulary's sorted keys, cached on the values' device."""
+    raw = t.long().contiguous()
+    keys, ids = col.vocabulary.tables(raw.device)
+    n = keys.numel()
+    pos = torch.searchsorted(keys, raw).clamp_(max=n - 1)
+    hit = keys[pos] == raw
+    if col.num_oov_buckets > 0:
+        miss = n + (raw * HASH_MULT) % (2 ** 32) % col.num_oov_buckets     # the low 32 bits of the wrapped product
+    else:
+        miss = torch.full_like(raw, col.default_value)
+    return torch.where(raw < 0, -1, torch.where(hit, ids[pos].long(), miss))
 
 
 def _ids(col: Categorical, t: torch.Tensor) -> torch.Tensor:
@@ -318,6 +541,8 @@ def _leaf_values(k, features: Dict[str, torch.Tensor]) -> torch.Tensor:
     if isinstance(k, BucketizedColumn):
         return _bucketize(k, features)
     t = features[k.key]
+    if isinstance(k, VocabularyColumn):              # a cross hashes the vocabulary ids, as TF's does
+        return _vocabulary_ids(k, t).reshape(t.shape[0], -1)
     return _ids(k, t).reshape(t.shape[0], -1)
 
 
@@ -351,13 +576,17 @@ def _width(col, features: Dict[str, torch.Tensor]) -> int:
 
 def _ids_and_weights(col: Categorical, features: Dict[str, torch.Tensor]):
     """[B, L] bucket ids (-1 = missing) and, for a weighted column, the [B, L] float weights (else None).  A bucketized
-    or crossed column computes its ids from the features it is built on."""
+    or crossed column computes its ids from the features it is built on, a vocabulary column looks its values up."""
     if isinstance(col, BucketizedColumn):
         return _bucketize(col, features), None
     if isinstance(col, CrossedColumn):
         return _cross(col, features), None
     t = features[col.key]
-    ids = _ids(col, t).reshape(t.shape[0], -1)
+    base = col.categorical_column if isinstance(col, WeightedCategoricalColumn) else col
+    if isinstance(base, VocabularyColumn):
+        ids = _vocabulary_ids(base, t).reshape(t.shape[0], -1)
+    else:
+        ids = _ids(col, t).reshape(t.shape[0], -1)
     if not isinstance(col, WeightedCategoricalColumn):
         return ids, None
     return ids, _weights(col, features, ids.shape)

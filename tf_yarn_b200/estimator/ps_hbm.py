@@ -497,10 +497,10 @@ class _TableGroup:
             self.push_s1 = ptrs(self.distinct, 1) if ns >= 1 else None
             self.push_s2 = ptrs(self.distinct, 2) if ns >= 2 else None
             self.max_members = max(table_of.count(k) for k in range(len(self.distinct)))
-        # a group with a bucketized or crossed column takes every column's ids from tfy_feature_ids (torch on a CPU
-        # tensor), which bounds each column's ids by its own V: its tables may differ in V, and the bag and push
-        # kernels are given the largest
-        self.derived = any(isinstance(c, fc.DERIVED) for c in cat_cols)
+        # a group with a bucketized, crossed or vocabulary column (also weighted or as a cross's leaf) takes every
+        # column's ids from tfy_vocab_ids + tfy_feature_ids (torch on a CPU tensor), which bound each column's ids by
+        # its own V: its tables may differ in V, and the bag and push kernels are given the largest
+        self.derived = any(fc._device_ids(c) for c in cat_cols)
         self.feature_ids = feature_ids.FeatureIds(cat_cols, conn.device) if self.derived else None
         self.V = max(c.num_buckets for c in cat_cols) if self.derived else cat_cols[0].num_buckets
         self.same_v = not self.derived and all(c.num_buckets == self.V and c.hashed == cat_cols[0].hashed
@@ -545,8 +545,9 @@ class _TableGroup:
         return self._bucket(raw)
 
     def _derived_ids(self, features) -> torch.Tensor:
-        """int64 [T, B, L] ids of a group with bucketized or crossed columns, padded with -1: one tfy_feature_ids launch
-        (per kFeatMaxCols columns) on CUDA tensors, the columns' torch statement on CPU tensors."""
+        """int64 [T, B, L] ids of a group with bucketized, crossed or vocabulary columns, padded with -1: one
+        tfy_vocab_ids launch per kVocabMaxSrcs vocabulary sources, then one tfy_feature_ids launch per kFeatMaxCols
+        columns, on CUDA tensors; the columns' torch statement on CPU tensors."""
         if self.conn.device.type == "cuda":
             self.conn.account(launches=self.feature_ids.launches)
             return self.feature_ids(features, self.conn.lib)

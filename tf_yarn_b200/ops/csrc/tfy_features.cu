@@ -3,6 +3,8 @@
 // value in the launch's __grid_constant__ parameter, so a captured CUDA graph replays the launch with the pointers it
 // was captured with, like every other kernel of the parameter-server step.  Integer work only: the ids are bit-equal
 // to the torch statement of the columns (feature_column._ids_and_weights).  The per-element math is tfy_features.cuh.
+// A group with vocabulary columns first runs tfy_vocab_ids, which translates their raw values into vocabulary ids
+// that tfy_feature_ids then reads as identity components.
 #include <cuda_runtime.h>
 #include <stdint.h>
 
@@ -21,6 +23,15 @@ __global__ void __launch_bounds__(kThreads) tfy_feature_ids_kernel(const __grid_
         const int b = (int)(i / p.L_max);
         out[i] = tfy_feat_id(p, t, b, (int)(i - (long long)b * p.L_max));
     }
+}
+
+// blockIdx.y = source: its B * width values, grid-stride
+__global__ void __launch_bounds__(kThreads) tfy_vocab_ids_kernel(const __grid_constant__ TfyVocabParams p) {
+    const TfyVocabSrc& s = p.srcs[blockIdx.y];
+    const long long n = (long long)p.B * s.width;
+    long long* out = reinterpret_cast<long long*>(s.out);
+    for (long long i = (long long)blockIdx.x * kThreads + threadIdx.x; i < n; i += (long long)gridDim.x * kThreads)
+        out[i] = tfy_vocab_elem(s, i);
 }
 
 }  // namespace
@@ -58,6 +69,32 @@ int tfy_feature_ids(const TfyFeatureParams* p, cudaStream_t s) {
     const long long cap = (kMaxBlocksX + p->T - 1) / p->T;
     if (gx > cap) gx = cap;
     tfy_feature_ids_kernel<<<dim3((unsigned)gx, (unsigned)p->T), kThreads, 0, s>>>(*p);
+    return (int)cudaGetLastError();
+}
+
+// p: host copy of the descriptors of S <= kVocabMaxSrcs vocabulary sources.  Returns 0, -1 for a descriptor out of
+// range, -2 for B * width beyond int32, -3 for a null pointer, or the launch's CUDA error.
+int tfy_vocab_ids(const TfyVocabParams* p, cudaStream_t s) {
+    if (p == nullptr) return -3;
+    if (p->S < 1 || p->S > kVocabMaxSrcs || p->B < 0) return -1;
+    long long n_max = 0;
+    for (int k = 0; k < p->S; ++k) {
+        const TfyVocabSrc& v = p->srcs[k];
+        if (v.n < 1 || v.n_oov < 0 || v.width < 1 || v.dflt < -1 || v.dflt >= v.n ||
+            (v.n_oov > 0 && v.dflt != -1) || (v.dtype != TFY_FEAT_I32 && v.dtype != TFY_FEAT_I64))
+            return -1;
+        if (v.src == 0 || v.keys == 0 || v.ids == 0) return -3;
+        const long long n = (long long)p->B * v.width;
+        if (n > n_max) n_max = n;
+    }
+    if (p->B == 0) return 0;
+    if (n_max > 0x7fffffffLL) return -2;
+    for (int k = 0; k < p->S; ++k)
+        if (p->srcs[k].out == 0) return -3;
+    long long gx = (n_max + kThreads - 1) / kThreads;
+    const long long cap = (kMaxBlocksX + p->S - 1) / p->S;
+    if (gx > cap) gx = cap;
+    tfy_vocab_ids_kernel<<<dim3((unsigned)gx, (unsigned)p->S), kThreads, 0, s>>>(*p);
     return (int)cudaGetLastError();
 }
 

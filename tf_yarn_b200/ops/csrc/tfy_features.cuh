@@ -14,8 +14,9 @@
 #define TFY_FEAT_HD static inline
 #endif
 
-// Per-launch caps: the parameter struct travels by value in the launch (under the 4 KB kernel-parameter limit).  A
-// tower with more columns or components is split over several launches by the caller (ops/features.py).
+// Per-launch caps: the parameter structs travel by value in the launch (under the 4 KB kernel-parameter limit).  A
+// tower with more columns, components or vocabulary sources is split over several launches by the caller
+// (ops/features.py).
 constexpr int kFeatMaxCols = 32;
 constexpr int kFeatMaxComps = 64;
 
@@ -123,4 +124,78 @@ TFY_FEAT_HD long long tfy_feat_id(const TfyFeatureParams& p, int t, int b, int j
         h = tfy_fingerprint_cat64(h, (uint64_t)v);
     }
     return (long long)(h % (uint64_t)col.V);
+}
+
+// ---- Vocabulary lookup (tfy_vocab_ids): raw integer values -> vocabulary ids, before tfy_feature_ids
+//
+// A source is one (feature, vocabulary column) pair: its [B, width] raw values are translated into an int64 [B, width]
+// buffer that tfy_feature_ids then reads as an identity component of modulus num_buckets.  A source's vocabulary is an
+// int64 array of its n keys sorted ascending and an int32 array of each key's id: the vocabulary's own device copy
+// (feature_column.Vocabulary.tables), shared by every group and column that uses it.  A value v maps to -1 if v < 0;
+// to its id if it is a key; else to n + ((uint64) v * 2654435761 mod 2^32) % n_oov when n_oov > 0; else to dflt
+// (feature_column.VocabularyColumn).  n is at most 2^31 - 1.
+
+constexpr int kVocabMaxSrcs = 32;
+
+struct TfyVocabSrc {
+    uint64_t src;             // [B, width] raw values, row-major, int32 or int64
+    uint64_t out;             // int64 [B, width] ids
+    uint64_t keys;            // int64 [n] sorted keys
+    uint64_t ids;             // int32 [n] id of each key
+    int32_t n;                // vocabulary length, in [1, 2^31 - 1]
+    int32_t n_oov;            // OOV buckets (0: misses take dflt)
+    int32_t dflt;             // id of a miss without OOV buckets, in [-1, n)
+    int32_t dtype;            // TFY_FEAT_I32 / TFY_FEAT_I64
+    int32_t width;            // values per example
+    int32_t pad;
+};
+
+struct TfyVocabParams {
+    int32_t B, S;             // examples, sources
+    TfyVocabSrc srcs[kVocabMaxSrcs];
+};
+
+// The number of the n keys key(0) <= ... <= key(n - 1) that are < x (std::lower_bound), for any n up to 2^31 - 1:
+// the midpoint lo + (hi - lo) / 2 never leaves [lo, hi), where (lo + hi) / 2 would wrap past 2^31 - 1.  `key` is a
+// functor, so that the host test can search a fake key sequence of 2^31 - 1 entries without storing it.
+template <class Key>
+TFY_FEAT_HD int tfy_vocab_lower_bound_by(long long x, int n, const Key& key) {
+    int lo = 0, hi = n;
+    while (lo < hi) {
+        const int mid = lo + ((hi - lo) >> 1);
+        if (key(mid) < x) lo = mid + 1;
+        else hi = mid;
+    }
+    return lo;
+}
+
+struct TfyVocabKeys {
+    const long long* keys;
+#if defined(__CUDACC__)
+    __host__ __device__ __forceinline__
+#endif
+    long long operator()(int i) const { return keys[i]; }
+};
+
+TFY_FEAT_HD int tfy_vocab_lower_bound(long long x, const long long* keys, int n) {
+    return tfy_vocab_lower_bound_by(x, n, TfyVocabKeys{keys});
+}
+
+// Id of one raw value of a source (-1 = missing or absent)
+TFY_FEAT_HD long long tfy_vocab_id(const TfyVocabSrc& s, long long raw) {
+    if (raw < 0) return -1;
+    const long long* keys = reinterpret_cast<const long long*>(s.keys);
+    const int pos = tfy_vocab_lower_bound(raw, keys, s.n);
+    if (pos < s.n && keys[pos] == raw) return (long long)reinterpret_cast<const int32_t*>(s.ids)[pos];
+    if (s.n_oov > 0)
+        return (long long)s.n +
+               (long long)((((unsigned long long)raw * 2654435761ull) & 0xffffffffull) % (unsigned long long)s.n_oov);
+    return (long long)s.dflt;
+}
+
+// Element i of source s's [B, width] values
+TFY_FEAT_HD long long tfy_vocab_elem(const TfyVocabSrc& s, long long i) {
+    const long long raw = s.dtype == TFY_FEAT_I32 ? (long long)reinterpret_cast<const int32_t*>(s.src)[i]
+                                                  : reinterpret_cast<const long long*>(s.src)[i];
+    return tfy_vocab_id(s, raw);
 }
