@@ -47,6 +47,21 @@ extern "C" void tfy_host_patch_walk(int tiles_x, int tiles_y, int n_cta, int blo
     }
 }
 
+// the conv2 forward's raw 32-bit dropout hash of element groups idx0 .. idx0 + n - 1 (tfy_drop_salt / TFY_DROP_HASH):
+// pooled element e is kept iff byte e & 3 of the hash of group e >> 2 is >= c_drop_thr(rate)
+extern "C" void tfy_host_hash_u32(uint32_t seed, uint32_t step, uint64_t idx0, uint32_t* out, int n) {
+    const uint32_t salt = tfy_drop_salt(seed, step);
+    for (int i = 0; i < n; ++i) out[i] = TFY_DROP_HASH(salt, idx0 + (uint64_t)i);
+}
+
+// the conv2 forward's dropout threshold and keep scale at each rate (c_drop_thr, c_keep_scale)
+extern "C" void tfy_host_keep_scale(const float* rate, uint32_t* thr, float* scale, int n) {
+    for (int i = 0; i < n; ++i) {
+        thr[i] = c_drop_thr(rate[i]);
+        scale[i] = c_keep_scale(thr[i]);
+    }
+}
+
 // layout of the structs shared with Python (ctypes mirrors in tf_yarn_b200/ops/native.py)
 #include <stddef.h>
 extern "C" int tfy_host_struct_layout(int which, int* out, int cap) {

@@ -57,6 +57,7 @@ native.declare("tfy_conv3x3_c32_wgrad_unpool_deferred", [_vp, _vp, _vp, _f, _vp,
 native.declare("tfy_conv3x3_c32_dgrad_unpool_reduce", [_vp, _vp, _f, _vp, _vp, _vp, _i, _i, _i, _vp, _i, _vp, _vp,
                                                        _vp])
 native.declare("tfy_conv3x3_c32_wgrad_spare_ctas", [_i, _i, _i])
+native.declare("tfy_conv3x3_c32_keep_scale", [_f, ctypes.POINTER(ctypes.c_float)])
 native.declare("tfy_dense_bwd", [_vp, _vp, _vp, _vp, _vp, _i, _i, _i, _vp])
 native.declare("tfy_gemm_bf16_splitk_fused", [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _f, _u32, _vp, _i,
                                               _vp])
@@ -68,6 +69,15 @@ native.declare("tfy_dense_head_fused_weighted", [_vp, _vp, _vp, _vp, _vp, _f, _v
                                                  _vp, _i, _i, _i, _vp, _vp, _vp])
 
 PARTIAL_BLOCKS = 592
+
+
+def keep_scale(lib, rate: float) -> float:
+    """Scale of the kept elements of tfy_conv3x3_c32_pool_fwd's dropout at ``rate`` (the fp32 value it applies)."""
+    out = ctypes.c_float(0.0)
+    rc = lib.tfy_conv3x3_c32_keep_scale(float(rate), ctypes.byref(out))
+    if rc != 0:
+        raise RuntimeError(f"tfy_conv3x3_c32_keep_scale failed: {rc}")
+    return out.value
 
 
 class _Stage:
@@ -233,6 +243,14 @@ class FastSequentialEngine(GraphTrainEngine):
         H, W, Cin = ly.input_shape_
         return (Cin == 32 and ly.filters == 64 and st.pool and st.relu and (H - 2) % 8 == 0 and (W - 2) % 8 == 0
                 and B % 2 == 0)
+
+    def _conv_drop_scale(self, st, tc: bool) -> float:
+        """Scale of the kept gradients in the backward of conv stage ``st``'s dropout: the one its forward applied.
+        The wgmma forward (``tc``) quantises the rate to 1/256 and scales by 256 / (256 - thr)
+        (tfy_conv3x3_c32_keep_scale); the general pool kernel scales by 1 / (1 - rate)."""
+        if tc:
+            return keep_scale(self.lib, st.drop)
+        return 1.0 / (1.0 - st.drop) if st.drop > 0 else 1.0
 
     def _warn_once(self, key: str, msg: str) -> None:
         if key not in self._warned:
@@ -558,7 +576,7 @@ class FastSequentialEngine(GraphTrainEngine):
                 H, W, Cin = ly.input_shape_
                 O = ly.filters
                 OH, OW = H - 2, W - 2
-                scale = 1.0 / (1.0 - st.drop) if st.drop > 0 else 1.0
+                scale = self._conv_drop_scale(st, st.pool and self._tc_conv(st, B))
                 gated, pre_gated = pre_gated, False
                 if (Cin == 1 and O == 32 and gated and not st.pool and aux is None and first
                         and os.environ.get("TFY_NO_TC_CONV") != "1"):

@@ -248,6 +248,13 @@ __device__ __forceinline__ float tfy_uniform(uint32_t seed, uint32_t step, uint6
                             tfy_hash32((uint32_t)idx * 0xC2B2AE35U + (uint32_t)(idx >> 32) + 0x27d4eb2fU));
     return (float)(h >> 8) * (1.0f / 16777216.0f);
 }
+// The conv2 forward's draws (tfy_conv3x3_fprop_pool_kernel): a per-step salt, then one raw hash per group of 4 pooled
+// elements, one byte per element.  For group indices below 2^32 the raw hash is the one tfy_uniform keeps the top 24
+// bits of.  (A macro: as an inline function it changes the forward kernel's instruction schedule.)
+__device__ __forceinline__ uint32_t tfy_drop_salt(uint32_t seed, uint32_t step) {
+    return seed ^ tfy_hash32(step * 0x9E3779B9U + 0x85ebca6bU);
+}
+#define TFY_DROP_HASH(salt, group) tfy_hash32((salt) ^ tfy_hash32((uint32_t)(group) * 0xC2B2AE35U + 0x27d4eb2fU))
 
 template <typename T>
 struct TfyPack;  // 16-byte pack of T

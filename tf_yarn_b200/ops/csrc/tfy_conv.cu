@@ -194,6 +194,8 @@ __device__ __forceinline__ void c_wg_reduce(const float* __restrict__ partials, 
 // ------------------------------------------------------------------------------------------------
 // forward: pooled = dropout(maxpool2x2(relu(conv(a, W) + bias))), code byte per pooled element
 // (bits 0-1 = argmax position dy*2+dx inside the 2x2 window, bit 2 = gradient flows).
+// Dropout draws one byte per element, so drop_rate is quantised to thr / 256 (thr = drop_rate * 256 rounded to
+// nearest) and kept values are scaled by 256 / (256 - thr): tfy_conv3x3_c32_keep_scale gives the backward that scale.
 // warps 0..7 epilogue (row quadrant = warp & 3, 16-column slices warp >> 2 and (warp >> 2) + 2), warps 8..11 MMA,
 // warp 12 TMA
 // ------------------------------------------------------------------------------------------------
@@ -292,10 +294,11 @@ tfy_conv3x3_fprop_pool_kernel(const __grid_constant__ CUtensorMap map_a, const _
         const uint32_t tag = (uint32_t)(dy * 2 + dx);
         const int OH = H - 2, OW = W - 2, PH = OH / 2, PW = OW / 2;
         const uint32_t step = hp ? (uint32_t)hp->step : 0u;
-        // dropout decisions come 4 to a hash (one byte each): the rate is quantised to 1/256
-        const uint32_t thr = drop_rate > 0.f ? (uint32_t)(drop_rate * 256.f + 0.5f) : 0u;
-        const float keep_scale = 256.f / (256.f - (float)thr);
-        const uint32_t salt = seed ^ tfy_hash32(step * 0x9E3779B9U + 0x85ebca6bU);
+        // dropout decisions come 4 to a hash (one byte each): the rate is quantised to 1/256 and kept values are
+        // scaled by 256 / (256 - thr), not 1 / (1 - rate) (c_drop_thr, tfy_conv_index.cuh)
+        const uint32_t thr = c_drop_thr(drop_rate);
+        const float keep_scale = c_keep_scale(thr);
+        const uint32_t salt = tfy_drop_salt(seed, step);
         // after the two exchanges below lane (dy, dx) owns columns [8 dx + 4 dy, +4) of each of the warp's slices
         float bv[2][4];
 #pragma unroll
@@ -343,8 +346,7 @@ tfy_conv3x3_fprop_pool_kernel(const __grid_constant__ CUtensorMap map_a, const _
                     const float keep = dy ? m8[4 + j] : m8[j];
                     m4[j] = fmaxf(keep, __shfl_xor_sync(0xffffffffu, send, 16));
                 }
-                const uint32_t rnd =
-                    thr ? tfy_hash32(salt ^ tfy_hash32((prow >> 2) * 0xC2B2AE35U + 0x27d4eb2fU)) : 0xffffffffu;
+                const uint32_t rnd = thr ? TFY_DROP_HASH(salt, prow >> 2) : 0xffffffffu;
                 float o[4];
                 uint32_t codes = 0;
 #pragma unroll
@@ -1175,8 +1177,18 @@ int tfy_conv_set_timeline(long long* buf) {
 // number of fp32 elements of the `partials` scratch buffer tfy_conv3x3_c32_wgrad needs
 size_t tfy_conv3x3_c32_wgrad_scratch_elems() { return (size_t)160 * WG_PART; }
 
+// *scale = the scale the backward of tfy_conv3x3_c32_pool_fwd's dropout at `rate` must apply to kept gradients:
+// 256 / (256 - thr) with the rate quantised to thr / 256 (c_drop_thr), the scale the forward applied.
+int tfy_conv3x3_c32_keep_scale(float rate, float* scale) {
+    if (scale == nullptr) return -2;
+    *scale = c_keep_scale(c_drop_thr(rate));
+    return 0;
+}
+
 // a: [B, H, W, 32] bf16 (NHWC), w: [64, 3, 3, 32] bf16, bias: [64] bf16
 // pooled / code: [B, (H-2)/2, (W-2)/2, 64].  Requires (H-2) % 8 == 0, (W-2) % 8 == 0, B % 2 == 0.
+// Dropout: pooled element e is kept iff byte e & 3 of the hash of e >> 2 is >= thr = round(drop_rate * 256), and
+// kept values are scaled by tfy_conv3x3_c32_keep_scale(drop_rate).
 int tfy_conv3x3_c32_pool_fwd(const void* a, const void* w, const void* bias, void* pooled, void* code, int B, int H,
                              int W, float drop_rate, uint32_t seed, const TfyOptHyper* hp, cudaStream_t s) {
     const int OH = H - 2, OW = W - 2;

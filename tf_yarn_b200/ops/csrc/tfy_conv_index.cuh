@@ -1,6 +1,7 @@
 // Patch scheduling and weight-gradient reduction order of the persistent convolution kernels (included by tfy_conv.cu;
 // kept in its own header so that the index arithmetic can be unit-tested on the host with g++).
 #pragma once
+#include <stdint.h>
 
 // Walks the patch list of a persistent CTA: p = blockIdx.x + i * gridDim.x decomposed into (image pair,
 // tile row, tile column) incrementally -- no integer division per patch in the hot loops.
@@ -23,6 +24,17 @@ struct CPatchIter {
         bz += sb;
     }
 };
+
+// Dropout of the conv2 forward (tfy_conv3x3_fprop_pool_kernel).  Its decisions come 4 to a 32-bit hash, one byte each,
+// so the rate is quantised to 1/256: thr = rate * 256 rounded to nearest in fp32 (0 when rate <= 0), pooled element e
+// is kept iff byte e & 3 of TFY_DROP_HASH(salt, e >> 2) (tfy_common.cuh) is >= thr, and kept values are scaled by
+// 256 / (256 - thr), the inverse of the kept fraction.  That keep scale, not 1 / (1 - rate), is what the backward must
+// apply (tfy_conv3x3_c32_keep_scale).  A rate of 255.5 / 256 or more drops every element (thr = 256, scale inf).
+// (stdint.h only: the host builds of this header include nothing else.)
+__host__ __device__ __forceinline__ uint32_t c_drop_thr(float rate) {
+    return rate > 0.f ? (uint32_t)(rate * 256.f + 0.5f) : 0u;
+}
+__host__ __device__ __forceinline__ float c_keep_scale(uint32_t thr) { return 256.f / (256.f - (float)thr); }
 
 // Summation order of the conv2 weight gradient's per-CTA fp32 partials (n_part of them; total4 float4 outputs,
 // dW tile then db).  Output f belongs to the slice of owner f / per; the owner's slice length `len` sets how many
