@@ -3,11 +3,13 @@
 Covers what the reference's task programs and examples touch (SURVEY.md appendix A):
 Estimator / RunConfig / TrainSpec / EvalSpec / EstimatorSpec / ModeKeys / train_and_evaluate /
 session-run hooks / checkpoint index / exporters / canned LinearClassifier, DNNClassifier,
-DNNLinearCombinedClassifier / feature columns / model_to_estimator.
+DNNLinearCombinedClassifier, LinearRegressor, DNNRegressor, DNNLinearCombinedRegressor / feature columns /
+model_to_estimator.
 """
 from tf_yarn_b200.estimator import feature_column  # noqa: F401
-from tf_yarn_b200.estimator.canned import (DNNClassifier, DNNLinearCombinedClassifier, LinearClassifier,  # noqa: F401
-                                           model_to_estimator)
+from tf_yarn_b200.estimator.canned import (SUM_OVER_BATCH_SIZE, DNNClassifier,  # noqa: F401
+                                           DNNLinearCombinedClassifier, DNNLinearCombinedRegressor, DNNRegressor,
+                                           LinearClassifier, LinearRegressor, model_to_estimator)
 from tf_yarn_b200.estimator.checkpoint import get_checkpoint_state, latest_checkpoint  # noqa: F401
 from tf_yarn_b200.estimator.config import ClusterInfo, ConfigProto, RunConfig, SessionConfig  # noqa: F401
 from tf_yarn_b200.estimator.estimator import Estimator  # noqa: F401

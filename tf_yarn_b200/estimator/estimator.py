@@ -313,7 +313,7 @@ class Estimator:
         finally:
             wd.close()
         loss = self._last_loss_t
-        self.last_loss = float(loss) if self._global_step > start_step else self.last_loss
+        self.last_loss = self._read_loss(loss) if self._global_step > start_step else self.last_loss
         if writes_files and (cfg.save_checkpoints_steps or cfg.save_checkpoints_secs) and \
                 self._global_step > start_step:
             st = ckpt.get_checkpoint_state(self._model_dir)
@@ -355,11 +355,11 @@ class Estimator:
             gs = self._global_step
             if writer is not None and cfg.save_summary_steps and \
                     gs // cfg.save_summary_steps > (gs - 1 if self._ps is None else prev_gs) // cfg.save_summary_steps:
-                self.last_loss = float(loss)
+                self.last_loss = self._read_loss(loss)
                 writer.add_scalar("loss", self.last_loss, gs)
             if cfg.log_step_count_steps and gs - last_log_step >= cfg.log_step_count_steps:
                 now = time.time()
-                self.last_loss = float(loss)
+                self.last_loss = self._read_loss(loss)
                 sps = (gs - last_log_step) / max(now - last_log_time, 1e-9)
                 logger.info("global_step/sec: %.4g  loss = %.6g, step = %d", sps, self.last_loss, gs)
                 if writer is not None:
@@ -379,12 +379,27 @@ class Estimator:
             item = next(it, None)
         return item
 
+    def _read_loss(self, loss) -> float:
+        """The loss on the host; then the loss's own ``check()`` (a canned head raises on invalid labels it flagged
+        on the device), which costs no extra wait: the device has just been synchronised by the read."""
+        value = float(loss)
+        check = getattr(self._spec.loss, "check", None) if self._spec is not None else None
+        if check is not None:
+            check()
+        return value
+
+    @staticmethod
+    def _loss(spec: EstimatorSpec, features, labels, outputs) -> torch.Tensor:
+        if spec.weights is None:
+            return spec.loss(labels, outputs)
+        return spec.loss(labels, outputs, spec.weights(features))
+
     def _ps_step_body(self, features, labels) -> torch.Tensor:
         """pull -> forward -> backward -> push against the parameter servers (kernels only: capturable)."""
         self._ps.pull(self._network)
         self._optimizer.zero_grad(set_to_none=False)
         outputs = self._network(features)
-        loss = self._spec.loss(labels, outputs)
+        loss = self._loss(self._spec, features, labels, outputs)
         loss.backward()
         self._ps.push(self._network)
         return loss.detach()
@@ -447,7 +462,7 @@ class Estimator:
             self._ps.pull(self._network)
         self._optimizer.zero_grad(set_to_none=False)
         outputs = self._network(features)
-        loss = spec.loss(labels, outputs)
+        loss = self._loss(spec, features, labels, outputs)
         loss.backward()
         if self._ps is not None:
             self._ps.push(self._network)
@@ -509,13 +524,18 @@ class Estimator:
                 features = _to_device(features, self._device or torch.device("cpu"))
                 labels = _to_device(labels, self._device or torch.device("cpu"))
                 outputs = self._network(features) if self._network is not None else features
+                w = spec.weights(features) if spec.weights is not None else None
                 if spec.loss is not None:
-                    loss_sum += float(spec.loss(labels, outputs))
+                    loss_sum += float(spec.loss(labels, outputs) if w is None else spec.loss(labels, outputs, w))
                 for k, fn in metric_fns.items():
                     if k in stateful:
-                        fn.update_state(labels, outputs)        # device-side state: no host read per batch
+                        # device-side state: no host read per batch
+                        if w is None:
+                            fn.update_state(labels, outputs)
+                        else:
+                            fn.update_state(labels, outputs, sample_weight=w)
                         continue
-                    a, b = fn(labels, outputs)
+                    a, b = fn(labels, outputs) if w is None else fn(labels, outputs, w)
                     num[k] += float(a)
                     den[k] += float(b)
                 n_batches += 1
@@ -529,6 +549,9 @@ class Estimator:
                 h.end(None)
             except TypeError:
                 h.end()
+        check = getattr(spec.loss, "check", None)
+        if check is not None:
+            check()
         results: Dict[str, Any] = {"loss": loss_sum / max(n_batches, 1)}
         for k, fn in metric_fns.items():
             results[k] = fn.result() if k in stateful else num[k] / max(den[k], 1.0)

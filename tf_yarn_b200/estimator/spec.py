@@ -22,7 +22,8 @@ class EstimatorSpec(NamedTuple):
 
     network         ``torch.nn.Module`` mapping the features batch to outputs (logits / predictions).
                     ``None`` makes a parameter-free estimator (the step only advances global_step).
-    loss            callable ``(labels, outputs) -> scalar tensor`` (TRAIN / EVAL).
+    loss            callable ``(labels, outputs) -> scalar tensor`` (TRAIN / EVAL); ``(labels, outputs, weights)``
+                    when ``weights`` is set.
     optimizer       mini-Keras optimizer descriptor, its name, or a zero-arg factory (TRAIN).
     optimizers      optional ``{parameter-name prefix: optimizer}``: a different optimizer per part of the
                     network (longest matching prefix wins, ``optimizer`` is the default) -- TF's wide-and-deep
@@ -31,6 +32,11 @@ class EstimatorSpec(NamedTuple):
                     ``{name: keras.metrics.Metric}`` (``reset_state`` / ``update_state(labels, outputs)`` /
                     ``result``, as TF2 Estimators take them).
     predictions     callable ``outputs -> dict`` (PREDICT), default identity.
+    weights         optional callable ``features -> [B] float tensor``: per-example weights (a canned estimator's
+                    ``weight_column``).  When set, the estimator calls ``loss(labels, outputs, w)``,
+                    ``update_state(labels, outputs, sample_weight=w)`` on Metric ops and ``(num, den)`` ops as
+                    ``fn(labels, outputs, w)``, in training and in evaluation; when ``None`` every call is made
+                    without it.
     train_op / export_outputs are accepted for signature parity and ignored.
     """
     mode: str
@@ -42,6 +48,7 @@ class EstimatorSpec(NamedTuple):
     train_op: Any = None
     export_outputs: Any = None
     optimizers: Optional[Dict[str, Any]] = None
+    weights: Optional[Callable] = None
 
 
 class TrainSpec(NamedTuple):
