@@ -1,4 +1,5 @@
-"""Canned estimators: the Linear / DNN / DNNLinearCombined classifiers and regressors, model_to_estimator.
+"""Canned estimators: the Linear / DNN / DNNLinearCombined classifiers, regressors and head-taking estimators,
+model_to_estimator.
 
 The reference's examples use ``tf.estimator.LinearClassifier(feature_columns, model_dir,
 n_classes[, optimizer][, config])`` (reference: tf_yarn/examples/linear_classifier_example.py:49-52,
@@ -9,7 +10,7 @@ estimator is the BASELINE config that exercises the parameter-server path.
 from __future__ import annotations
 
 import math
-from typing import Any, Callable, Dict, Optional, Sequence
+from typing import Any, Optional, Sequence
 
 import torch
 import torch.nn as nn
@@ -18,179 +19,11 @@ import torch.nn.functional as F
 from tf_yarn_b200.estimator import feature_column as fc
 from tf_yarn_b200.estimator.config import RunConfig
 from tf_yarn_b200.estimator.estimator import Estimator
+from tf_yarn_b200.estimator.head import (SUM_OVER_BATCH_SIZE, BinaryClassHead, MultiClassHead,  # noqa: F401
+                                         RegressionHead, _classification_head, _classification_metrics, _Head,
+                                         _regression_metrics)
 from tf_yarn_b200.estimator.spec import EstimatorSpec
-from tf_yarn_b200.keras import metrics as kmetrics
 from tf_yarn_b200.keras import optimizers as kopt
-from tf_yarn_b200.ops import head as canned_head
-
-
-SUM_OVER_BATCH_SIZE = "sum_over_batch_size"      # tf.keras.losses.Reduction.SUM_OVER_BATCH_SIZE, TF2's default
-
-
-def _weights_fn(weight_column) -> Optional[Callable]:
-    """``features -> [B] float32`` weights of ``weight_column`` (a feature key or a ``NumericColumn``), or ``None``.
-
-    Weights are used as given (no sign check), as TF does."""
-    if weight_column is None:
-        return None
-    key = weight_column.key if isinstance(weight_column, fc.NumericColumn) else weight_column
-    if not isinstance(key, str):
-        raise TypeError(f"weight_column must be a feature key or a numeric_column, got {weight_column!r}")
-
-    def weights(features):
-        if key not in features:
-            raise KeyError(f"weight_column {key!r} is not among the features {sorted(features)}")
-        w = features[key]
-        w = w if torch.is_tensor(w) else torch.as_tensor(w)
-        if not (w.dim() == 1 or (w.dim() == 2 and w.shape[1] == 1)):
-            raise ValueError(f"weight_column {key!r} must have shape [B] or [B, 1], got {list(w.shape)}")
-        return w.reshape(-1).float()
-    return weights
-
-
-class _BatchRatio(kmetrics.Metric):
-    """``sum of the per-batch numerators / sum of the per-batch denominators``, 0 when the denominators sum to 0.
-
-    ``fn(labels, logits, weights) -> (numerator, denominator)`` gives one batch's fp32 sums (``weights`` is ``None``
-    without a weight column).  They are added as fp64 on the device, in batch order, with no host read per batch."""
-
-    def __init__(self, name: str, fn: Callable):
-        super().__init__(name)
-        self._fn = fn
-        self._sum: Optional[torch.Tensor] = None         # float64 [2]: numerator, denominator
-
-    def update_state(self, y_true, y_pred, sample_weight=None) -> None:
-        num, den = self._fn(y_true, y_pred, sample_weight)
-        if self._sum is None:
-            self._sum = torch.zeros(2, dtype=torch.float64, device=y_pred.device)
-        self._sum[0] += num
-        self._sum[1] += den
-
-    def result(self) -> float:
-        if self._sum is None:
-            return 0.0
-        s, n = self._sum.tolist()
-        return s / n if n != 0 else 0.0
-
-    def reset_state(self) -> None:
-        if self._sum is not None:
-            self._sum.zero_()
-
-    def fresh(self) -> "_BatchRatio":
-        return _BatchRatio(self.name, self._fn)
-
-
-def _classification_head(n_classes: int) -> canned_head.CannedHead:
-    if n_classes == 2:
-        return canned_head.CannedHead(canned_head.BINARY, 1)
-    return canned_head.CannedHead(canned_head.MULTI_CLASS, n_classes)
-
-
-def _classification_metrics(n_classes: int) -> Dict[str, Any]:
-    head = canned_head.BINARY if n_classes == 2 else canned_head.MULTI_CLASS
-
-    def class_ids(labels):
-        # a label outside [0, n_classes) is reported by the head (CannedHead.check); clamping keeps the metrics from
-        # indexing with it, and changes nothing for valid labels
-        y = labels.long().reshape(-1)
-        return y if n_classes == 2 else y.clamp(0, n_classes - 1)
-
-    def accuracy(labels, logits, w):
-        if n_classes == 2:
-            pred = (logits.reshape(-1) > 0).long()
-        else:
-            pred = logits.argmax(dim=-1)
-        labels = labels.long().reshape(-1)
-        if w is None:
-            return (pred == labels).sum().float(), float(labels.numel())
-        return (w * (pred == labels).float()).sum(), w.sum()
-
-    def average_loss(labels, logits, w):
-        if w is None:
-            n = labels.reshape(-1).shape[0]
-            return canned_head.torch_head(head, logits, class_ids(labels), None) * n, float(n)
-        return (canned_head.torch_row_losses(head, logits, class_ids(labels)) * w).sum(), w.sum()
-    ops: Dict[str, Any] = {"accuracy": _BatchRatio("accuracy", accuracy),
-                           "average_loss": _BatchRatio("average_loss", average_loss)}
-    if n_classes == 2:
-        # the rest of TF's binary head: tensorflow_estimator head/binary_class_head.py
-        def label_mean(labels, logits, w):
-            y = labels.float().reshape(-1)
-            return (y.sum(), float(y.numel())) if w is None else ((y * w).sum(), w.sum())
-
-        def prediction_mean(labels, logits, w):
-            p = torch.sigmoid(logits.float().reshape(-1))
-            return (p.sum(), float(p.numel())) if w is None else ((p * w).sum(), w.sum())
-
-        ops.update({"auc": kmetrics.AUC(from_logits=True, name="auc"),
-                    "auc_precision_recall": kmetrics.AUC(curve="PR", from_logits=True, name="auc_precision_recall"),
-                    "precision": kmetrics.Precision(from_logits=True), "recall": kmetrics.Recall(from_logits=True),
-                    "label/mean": _BatchRatio("label/mean", label_mean),
-                    "prediction/mean": _BatchRatio("prediction/mean", prediction_mean),
-                    "accuracy_baseline": _AccuracyBaseline()})
-    return ops
-
-
-def _regression_metrics(label_dimension: int) -> Dict[str, Any]:
-    """TF's regression head (tensorflow_estimator head/regression_head.py): each weighted and averaged over all d
-    outputs, ``sum_i w_i sum_j v_ij / (d sum_i w_i)``."""
-    d = label_dimension
-
-    def ratio(values):
-        def fn(labels, logits, w):
-            v = values(labels.float().reshape(logits.shape), logits.float())
-            if w is None:
-                return v.sum(), float(v.numel())
-            return (v.sum(dim=1) * w).sum(), d * w.sum()
-        return fn
-    return {"average_loss": _BatchRatio("average_loss", ratio(lambda y, z: (z - y) ** 2)),
-            "label/mean": _BatchRatio("label/mean", ratio(lambda y, z: y)),
-            "prediction/mean": _BatchRatio("prediction/mean", ratio(lambda y, z: z))}
-
-
-class _AccuracyBaseline(kmetrics.Metric):
-    """``max(m, 1 - m)`` for the (weighted) label mean ``m``: the accuracy of always predicting the majority class."""
-
-    def __init__(self, name: str = "accuracy_baseline"):
-        super().__init__(name)
-        self._sum: Optional[torch.Tensor] = None         # float64 [2]: sum of the (weighted) labels, of the weights
-
-    def update_state(self, y_true, y_pred, sample_weight=None) -> None:
-        y = y_true.detach().reshape(-1).double()
-        if self._sum is None:
-            self._sum = torch.zeros(2, dtype=torch.float64, device=y.device)
-        if sample_weight is None:
-            self._sum[0] += y.sum()
-            self._sum[1] += y.numel()
-        else:
-            w = sample_weight.detach().reshape(-1).double()
-            self._sum[0] += (y * w).sum()
-            self._sum[1] += w.sum()
-
-    def result(self) -> float:
-        if self._sum is None:
-            return 0.0
-        s, n = self._sum.tolist()
-        m = s / n if n else 0.0
-        return max(m, 1.0 - m)
-
-    def reset_state(self) -> None:
-        if self._sum is not None:
-            self._sum.zero_()
-
-
-def _classification_predictions(n_classes: int) -> Callable:
-    def predictions(logits):
-        logits = logits.float()
-        if n_classes == 2:
-            p1 = torch.sigmoid(logits.reshape(-1, 1))
-            probs = torch.cat([1 - p1, p1], dim=1)
-            ids = (p1 > 0.5).long()
-        else:
-            probs = F.softmax(logits, dim=-1)
-            ids = probs.argmax(dim=-1, keepdim=True)
-        return {"logits": logits, "probabilities": probs, "class_ids": ids}
-    return predictions
 
 
 class _WideDeepNet(nn.Module):
@@ -246,22 +79,15 @@ def _tf_default(opt, tower: str, n_columns: int, combined: bool):
     return opt
 
 
-def _regression_predictions(logits):
-    return {"predictions": logits.float()}
-
-
-def _canned_model_fn(linear_columns, dnn_columns, hidden_units, optimizer, dropout=None, linear_optimizer=None,
-                     sparse_combiner="sum", n_classes=2, label_dimension=None, weight_column=None):
-    """The model_fn of every canned estimator: a classifier head for ``n_classes``, or a regression head of
-    ``label_dimension`` outputs when that is given."""
-    if label_dimension is not None:
-        head = canned_head.CannedHead(canned_head.REGRESSION, label_dimension)
-        metrics, predictions = (lambda: _regression_metrics(label_dimension)), _regression_predictions
-    else:
-        head = _classification_head(n_classes)
-        metrics, predictions = (lambda: _classification_metrics(n_classes)), _classification_predictions(n_classes)
-    weights = _weights_fn(weight_column)
-    n_out = head.n_out
+def _canned_model_fn(linear_columns, dnn_columns, hidden_units, optimizer, head: _Head, dropout=None,
+                     linear_optimizer=None, sparse_combiner="sum"):
+    """The model_fn of every canned estimator: the wide and/or deep towers under ``head``."""
+    if not isinstance(head, _Head):
+        raise TypeError(f"head must be one of the heads of tf_yarn_b200.estimator (BinaryClassHead, ...), got "
+                        f"{head!r}")
+    # one CannedHead per model_fn: its device buffers outlive any CUDA graph a train step captured with it
+    loss = head.canned_head()
+    n_out = head.logits_dimension
     combined = bool(linear_columns) and bool(dnn_columns)
     if dnn_columns:
         optimizer = _tf_default(optimizer, "dnn", len(dnn_columns), combined)
@@ -274,19 +100,24 @@ def _canned_model_fn(linear_columns, dnn_columns, hidden_units, optimizer, dropo
                            sparse_combiner=sparse_combiner)
         # the wide tower's parameters live under "linear."; everything else belongs to the deep tower
         per_tower = {"linear.": linear_optimizer} if (linear_optimizer is not None and linear_columns) else None
-        # one head per model_fn: its device buffers outlive any CUDA graph a train step captured with it
-        return EstimatorSpec(mode=mode, network=net, loss=head, optimizer=optimizer, eval_metric_ops=metrics(),
-                             predictions=predictions, optimizers=per_tower, weights=weights)
+        return EstimatorSpec(mode=mode, network=net, loss=loss, optimizer=optimizer, eval_metric_ops=head.metrics(),
+                             predictions=head.predictions, optimizers=per_tower, weights=head.weights)
     return model_fn
 
 
-def _check_regression_args(label_dimension, loss_reduction) -> int:
-    if isinstance(label_dimension, bool) or not isinstance(label_dimension, int) or label_dimension < 1:
-        raise ValueError(f"label_dimension must be an integer >= 1, got {label_dimension!r}")
-    if loss_reduction != SUM_OVER_BATCH_SIZE:
-        raise ValueError(f"loss_reduction must be {SUM_OVER_BATCH_SIZE!r} (SUM_OVER_BATCH_SIZE), got "
-                         f"{loss_reduction!r}")
-    return label_dimension
+def _classifier_head(n_classes, weight_column) -> _Head:
+    if n_classes == 2:
+        return BinaryClassHead(weight_column)
+    return MultiClassHead(n_classes, weight_column)
+
+
+def _check_estimator_args(activation_fn=F.relu, batch_norm=False, warm_start_from=None, name="activation_fn"):
+    if activation_fn not in (F.relu, torch.relu, "relu"):
+        raise ValueError(f"{name} must be relu (the only activation supported), got {activation_fn!r}")
+    if batch_norm:
+        raise ValueError("batch_norm=True is not supported")
+    if warm_start_from is not None:
+        raise ValueError(f"warm_start_from is not supported (got {warm_start_from!r})")
 
 
 class LinearClassifier(Estimator):
@@ -295,16 +126,17 @@ class LinearClassifier(Estimator):
                  **_ignored):
         # FTRL is TF's default for linear models (tf.estimator.LinearClassifier)
         fc._check_combiner(sparse_combiner)
-        super().__init__(_canned_model_fn(list(feature_columns), [], [], optimizer, sparse_combiner=sparse_combiner,
-                                          n_classes=n_classes, weight_column=weight_column), model_dir, config)
+        super().__init__(_canned_model_fn(list(feature_columns), [], [], optimizer,
+                                          _classifier_head(n_classes, weight_column),
+                                          sparse_combiner=sparse_combiner), model_dir, config)
 
 
 class DNNClassifier(Estimator):
     def __init__(self, hidden_units: Sequence[int], feature_columns, model_dir: Optional[str] = None,
                  n_classes: int = 2, weight_column=None, optimizer: Any = "adagrad", dropout: Optional[float] = None,
                  config: Optional[RunConfig] = None, **_ignored):
-        super().__init__(_canned_model_fn([], list(feature_columns), list(hidden_units), optimizer, dropout,
-                                          n_classes=n_classes, weight_column=weight_column), model_dir, config)
+        super().__init__(_canned_model_fn([], list(feature_columns), list(hidden_units), optimizer,
+                                          _classifier_head(n_classes, weight_column), dropout), model_dir, config)
 
 
 class DNNLinearCombinedClassifier(Estimator):
@@ -316,9 +148,9 @@ class DNNLinearCombinedClassifier(Estimator):
                  config: Optional[RunConfig] = None, linear_sparse_combiner: str = "sum", **_ignored):
         fc._check_combiner(linear_sparse_combiner)
         super().__init__(_canned_model_fn(list(linear_feature_columns or []), list(dnn_feature_columns or []),
-                                          list(dnn_hidden_units), dnn_optimizer, dnn_dropout,
-                                          linear_optimizer=linear_optimizer, sparse_combiner=linear_sparse_combiner,
-                                          n_classes=n_classes, weight_column=weight_column),
+                                          list(dnn_hidden_units), dnn_optimizer,
+                                          _classifier_head(n_classes, weight_column), dnn_dropout,
+                                          linear_optimizer=linear_optimizer, sparse_combiner=linear_sparse_combiner),
                          model_dir, config)
 
 
@@ -328,10 +160,10 @@ class LinearRegressor(Estimator):
     def __init__(self, feature_columns, model_dir: Optional[str] = None, label_dimension: int = 1,
                  weight_column=None, optimizer: Any = "ftrl", config: Optional[RunConfig] = None,
                  sparse_combiner: str = "sum", loss_reduction: str = SUM_OVER_BATCH_SIZE):
-        d = _check_regression_args(label_dimension, loss_reduction)
+        head = RegressionHead(label_dimension, weight_column, loss_reduction)
         fc._check_combiner(sparse_combiner)
-        super().__init__(_canned_model_fn(list(feature_columns), [], [], optimizer, sparse_combiner=sparse_combiner,
-                                          label_dimension=d, weight_column=weight_column), model_dir, config)
+        super().__init__(_canned_model_fn(list(feature_columns), [], [], optimizer, head,
+                                          sparse_combiner=sparse_combiner), model_dir, config)
 
 
 class DNNRegressor(Estimator):
@@ -341,9 +173,9 @@ class DNNRegressor(Estimator):
                  label_dimension: int = 1, weight_column=None, optimizer: Any = "adagrad",
                  dropout: Optional[float] = None, config: Optional[RunConfig] = None,
                  loss_reduction: str = SUM_OVER_BATCH_SIZE):
-        d = _check_regression_args(label_dimension, loss_reduction)
-        super().__init__(_canned_model_fn([], list(feature_columns), list(hidden_units), optimizer, dropout,
-                                          label_dimension=d, weight_column=weight_column), model_dir, config)
+        head = RegressionHead(label_dimension, weight_column, loss_reduction)
+        super().__init__(_canned_model_fn([], list(feature_columns), list(hidden_units), optimizer, head, dropout),
+                         model_dir, config)
 
 
 class DNNLinearCombinedRegressor(Estimator):
@@ -355,12 +187,50 @@ class DNNLinearCombinedRegressor(Estimator):
                  dnn_dropout: Optional[float] = None, label_dimension: int = 1, weight_column=None,
                  config: Optional[RunConfig] = None, linear_sparse_combiner: str = "sum",
                  loss_reduction: str = SUM_OVER_BATCH_SIZE):
-        d = _check_regression_args(label_dimension, loss_reduction)
+        head = RegressionHead(label_dimension, weight_column, loss_reduction)
         fc._check_combiner(linear_sparse_combiner)
         super().__init__(_canned_model_fn(list(linear_feature_columns or []), list(dnn_feature_columns or []),
-                                          list(dnn_hidden_units), dnn_optimizer, dnn_dropout,
-                                          linear_optimizer=linear_optimizer, sparse_combiner=linear_sparse_combiner,
-                                          label_dimension=d, weight_column=weight_column),
+                                          list(dnn_hidden_units), dnn_optimizer, head, dnn_dropout,
+                                          linear_optimizer=linear_optimizer, sparse_combiner=linear_sparse_combiner),
+                         model_dir, config)
+
+
+class LinearEstimator(Estimator):
+    """tf.estimator.LinearEstimator: a linear model under any head (FTRL by default, as TF)."""
+
+    def __init__(self, head, feature_columns, model_dir: Optional[str] = None, optimizer: Any = "ftrl",
+                 config: Optional[RunConfig] = None, sparse_combiner: str = "sum", warm_start_from=None):
+        _check_estimator_args(warm_start_from=warm_start_from)
+        fc._check_combiner(sparse_combiner)
+        super().__init__(_canned_model_fn(list(feature_columns), [], [], optimizer, head,
+                                          sparse_combiner=sparse_combiner), model_dir, config)
+
+
+class DNNEstimator(Estimator):
+    """tf.estimator.DNNEstimator: a ReLU network under any head (Adagrad by default, as TF)."""
+
+    def __init__(self, head, hidden_units: Sequence[int], feature_columns, model_dir: Optional[str] = None,
+                 optimizer: Any = "adagrad", activation_fn=F.relu, dropout: Optional[float] = None,
+                 config: Optional[RunConfig] = None, warm_start_from=None, batch_norm: bool = False):
+        _check_estimator_args(activation_fn, batch_norm, warm_start_from)
+        super().__init__(_canned_model_fn([], list(feature_columns), list(hidden_units), optimizer, head, dropout),
+                         model_dir, config)
+
+
+class DNNLinearCombinedEstimator(Estimator):
+    """tf.estimator.DNNLinearCombinedEstimator: wide & deep under any head, with TF's defaults: FTRL for the linear
+    (wide) tower, Adagrad for the DNN (deep) tower."""
+
+    def __init__(self, head, model_dir: Optional[str] = None, linear_feature_columns=None,
+                 linear_optimizer: Any = "ftrl", dnn_feature_columns=None, dnn_optimizer: Any = "adagrad",
+                 dnn_hidden_units: Sequence[int] = (), dnn_activation_fn=F.relu, dnn_dropout: Optional[float] = None,
+                 config: Optional[RunConfig] = None, batch_norm: bool = False, linear_sparse_combiner: str = "sum",
+                 warm_start_from=None):
+        _check_estimator_args(dnn_activation_fn, batch_norm, warm_start_from, name="dnn_activation_fn")
+        fc._check_combiner(linear_sparse_combiner)
+        super().__init__(_canned_model_fn(list(linear_feature_columns or []), list(dnn_feature_columns or []),
+                                          list(dnn_hidden_units or ()), dnn_optimizer, head, dnn_dropout,
+                                          linear_optimizer=linear_optimizer, sparse_combiner=linear_sparse_combiner),
                          model_dir, config)
 
 

@@ -1,8 +1,10 @@
 // The canned estimators' head (estimator/canned.py, ops/head.py): the weighted loss of a batch and its logit gradient
-// in one launch, for the binary, multi-class and regression heads.  The per-element math and the loss contract are
-// in tfy_head.cuh.
+// in one launch, for the binary, multi-class, regression, multi-label, Poisson and logistic heads.  The per-element
+// math and the loss contract are in tfy_head.cuh.
 //
-//   binary, regression: one thread per logit; CTA c owns one contiguous chunk of the B*C logits.
+//   binary, regression, multi-label: one thread per logit; CTA c owns one contiguous chunk of the B*C logits.
+//     Multi-label is the binary kernel itself at C >= 2 (the same element function, weight i / C, mean over B*C).
+//   Poisson, logistic:  the same, in a kernel of its own that also checks each label (tfy_head_label_ok).
 //   multi-class:        one warp per row, looping over C in steps of 32 (any C >= 2); CTA c owns a chunk of rows.
 //
 // Deterministic by construction -- no floating-point atomics, so two runs, and eager vs graph replay, give the same
@@ -13,7 +15,9 @@
 //   * the last CTA to finish (ticket counter) sums the slabs in CTA order, writes (float)(S / (B c)) and re-arms the
 //     counter.
 // A multi-class label outside [0, C) makes its row contribute nothing (zero loss, zero gradient; the row still counts
-// in B) and sets bit 0 of the caller's flag word: bad user data is reported on the host, never a device fault.
+// in B) and sets bit 0 of the caller's flag word: bad user data is reported on the host, never a device fault.  A
+// Poisson label < 0 or a logistic label outside [0, 1] (NaN included) does the same for its element, which still
+// counts in B*C.
 #include <cuda_runtime.h>
 #include <math.h>
 #include <stdint.h>
@@ -104,6 +108,56 @@ tfy_head_elementwise_kernel(const float* __restrict__ z, const void* __restrict_
     finish(cta, slabs, ticket, loss, (double)n);
 }
 
+template <int kHead>
+__device__ __forceinline__ float checked_loss(float z, float y) {
+    if (kHead == TFY_HEAD_POISSON) return tfy_head_poisson_loss(z, y);
+    if (kHead == TFY_HEAD_POISSON_FULL) return tfy_head_poisson_full_loss(z, y);
+    return tfy_head_binary_loss(z, y);
+}
+
+template <int kHead>
+__device__ __forceinline__ float checked_grad(float z, float y) {
+    return kHead == TFY_HEAD_LOGISTIC ? tfy_head_binary_grad(z, y) : tfy_head_poisson_grad(z, y);
+}
+
+// Poisson and logistic: tfy_head_elementwise_kernel plus the label check and the flag word (a kernel of its own, so
+// the binary and regression instantiations keep their parameters and their code).
+template <int kHead, int kLabel>
+__global__ void __launch_bounds__(kThreads)
+tfy_head_checked_kernel(const float* __restrict__ z, const void* __restrict__ labels,
+                        const float* __restrict__ weights, int64_t B, int C, float scale, float* __restrict__ loss,
+                        float* __restrict__ dz, uint32_t* __restrict__ flags, double* __restrict__ slabs,
+                        uint32_t* __restrict__ ticket) {
+    __shared__ double warp_part[kWarps];
+    const int64_t n = B * (int64_t)C;
+    const int64_t chunk = (n + gridDim.x - 1) / gridDim.x;
+    const int64_t begin = (int64_t)blockIdx.x * chunk;
+    const int64_t end = begin + chunk < n ? begin + chunk : n;
+    double acc = 0.0;
+    bool bad = false;
+    for (int64_t i = begin + threadIdx.x; i < end; i += kThreads) {
+        const float zi = z[i];
+        const float yi = label_value<kLabel>(labels, i);
+        float g = 0.f;
+        if (tfy_head_label_ok(kHead, yi)) {
+            const float wi = weights != nullptr ? weights[C == 1 ? i : i / C] : 1.f;
+            acc += (double)wi * (double)checked_loss<kHead>(zi, yi);
+            g = checked_grad<kHead>(zi, yi) * (wi * scale);
+        } else {
+            bad = true;
+        }
+        if (dz != nullptr) dz[i] = g;
+    }
+    if (__any_sync(0xffffffffu, bad) && (threadIdx.x & 31) == 0) atomicOr(flags, kBadLabel);
+    acc = warp_sum(acc);
+    if ((threadIdx.x & 31) == 0) warp_part[threadIdx.x >> 5] = acc;
+    __syncthreads();
+    double cta = 0.0;
+    if (threadIdx.x == 0)
+        for (int v = 0; v < kWarps; ++v) cta += warp_part[v];
+    finish(cta, slabs, ticket, loss, (double)n);
+}
+
 template <int kLabel>
 __global__ void __launch_bounds__(kThreads)
 tfy_head_multi_kernel(const float* __restrict__ z, const void* __restrict__ labels, const float* __restrict__ weights,
@@ -162,19 +216,26 @@ size_t tfy_canned_head_scratch_bytes(int64_t B, int C, int head) {
     return kTicketBytes + (size_t)grid * sizeof(double);
 }
 
-// logits: fp32 [B, C] row-major.  labels: B*C values (binary: C = 1; regression: [B, d]) or B class ids
-// (multi-class), read in place as fp32 (label_dtype 0), int32 (1) or int64 (2).  weights: null (every example weighs
-// 1) or fp32 [B].  head: 0 binary (C must be 1), 1 multi-class (C >= 2), 2 regression (C = d >= 1).  loss: one fp32,
-// the batch's weighted loss sum_i w_i sum_j l_ij / (B c).  dlogits: null (loss only) or fp32 [B, C], dL/dlogits.
-// flags: one uint32 (bit 0: a multi-class label outside [0, C)); bits are only ever set.  scratch: at least
-// tfy_canned_head_scratch_bytes(B, C, head) bytes, zero-filled before the first launch.  Returns 0, -1 for a bad
-// head code or a C the head does not allow, -3 for a bad argument, or the CUDA error of the launch.
+// logits: fp32 [B, C] row-major.  labels: B*C values (binary, logistic: C = 1; regression, Poisson: [B, d];
+// multi-label: [B, C]) or B class ids (multi-class), read in place as fp32 (label_dtype 0), int32 (1) or int64 (2).
+// weights: null (every example weighs 1) or fp32 [B].  head: 0 binary (C must be 1), 1 multi-class (C >= 2),
+// 2 regression (C = d >= 1), 3 multi-label (C >= 2), 4 Poisson and 5 Poisson with the full loss (C = d >= 1),
+// 6 logistic (C = 1).  loss: one fp32, the batch's weighted loss sum_i w_i sum_j l_ij / (B c).  dlogits: null (loss
+// only) or fp32 [B, C], dL/dlogits.  flags: one uint32 (bit 0: a multi-class label outside [0, C), a Poisson label
+// < 0 or a logistic label outside [0, 1]); bits are only ever set; it may be null for heads 0, 2 and 3.  scratch: at
+// least tfy_canned_head_scratch_bytes(B, C, head) bytes, zero-filled before the first launch.  Returns 0, -1 for a
+// bad head code or a C the head does not allow, -3 for a bad argument, or the CUDA error of the launch.
 int tfy_canned_head(const float* logits, const void* labels, int label_dtype, const float* weights, int64_t B, int C,
                     int head, float* loss, float* dlogits, uint32_t* flags, void* scratch, cudaStream_t s) {
-    if (head == TFY_HEAD_BINARY ? C != 1 : head == TFY_HEAD_MULTI ? C < 2 : head == TFY_HEAD_REGRESSION ? C < 1 : true)
+    const bool checked = head == TFY_HEAD_POISSON || head == TFY_HEAD_POISSON_FULL || head == TFY_HEAD_LOGISTIC;
+    if (head == TFY_HEAD_BINARY || head == TFY_HEAD_LOGISTIC ? C != 1
+        : head == TFY_HEAD_MULTI || head == TFY_HEAD_MULTI_LABEL ? C < 2
+        : head == TFY_HEAD_REGRESSION || head == TFY_HEAD_POISSON || head == TFY_HEAD_POISSON_FULL ? C < 1
+        : true)
         return -1;
     if (B <= 0 || logits == nullptr || labels == nullptr || loss == nullptr || scratch == nullptr) return -3;
-    if (label_dtype < kLabelF32 || label_dtype > kLabelI64 || (head == TFY_HEAD_MULTI && flags == nullptr)) return -3;
+    if (label_dtype < kLabelF32 || label_dtype > kLabelI64 || ((head == TFY_HEAD_MULTI || checked) && flags == nullptr))
+        return -3;
     const int grid = head_grid(B, C, head);
     const int64_t per_loss = head == TFY_HEAD_MULTI ? B : B * (int64_t)C;      // B c
     const float scale = (float)(1.0 / (double)per_loss);
@@ -184,16 +245,31 @@ int tfy_canned_head(const float* logits, const void* labels, int label_dtype, co
         kernel<<<grid, kThreads, 0, s>>>(logits, labels, weights, B, C, scale, loss, dlogits, slabs, ticket);
         return (int)cudaGetLastError();
     };
-    auto multi = [&](auto kernel) -> int {
+    auto flagged = [&](auto kernel) -> int {
         kernel<<<grid, kThreads, 0, s>>>(logits, labels, weights, B, C, scale, loss, dlogits, flags, slabs, ticket);
         return (int)cudaGetLastError();
     };
     if (head == TFY_HEAD_MULTI) {
-        if (label_dtype == kLabelI64) return multi(tfy_head_multi_kernel<kLabelI64>);
-        if (label_dtype == kLabelI32) return multi(tfy_head_multi_kernel<kLabelI32>);
-        return multi(tfy_head_multi_kernel<kLabelF32>);
+        if (label_dtype == kLabelI64) return flagged(tfy_head_multi_kernel<kLabelI64>);
+        if (label_dtype == kLabelI32) return flagged(tfy_head_multi_kernel<kLabelI32>);
+        return flagged(tfy_head_multi_kernel<kLabelF32>);
     }
-    if (head == TFY_HEAD_BINARY) {
+    if (head == TFY_HEAD_POISSON) {
+        if (label_dtype == kLabelI64) return flagged(tfy_head_checked_kernel<TFY_HEAD_POISSON, kLabelI64>);
+        if (label_dtype == kLabelI32) return flagged(tfy_head_checked_kernel<TFY_HEAD_POISSON, kLabelI32>);
+        return flagged(tfy_head_checked_kernel<TFY_HEAD_POISSON, kLabelF32>);
+    }
+    if (head == TFY_HEAD_POISSON_FULL) {
+        if (label_dtype == kLabelI64) return flagged(tfy_head_checked_kernel<TFY_HEAD_POISSON_FULL, kLabelI64>);
+        if (label_dtype == kLabelI32) return flagged(tfy_head_checked_kernel<TFY_HEAD_POISSON_FULL, kLabelI32>);
+        return flagged(tfy_head_checked_kernel<TFY_HEAD_POISSON_FULL, kLabelF32>);
+    }
+    if (head == TFY_HEAD_LOGISTIC) {
+        if (label_dtype == kLabelI64) return flagged(tfy_head_checked_kernel<TFY_HEAD_LOGISTIC, kLabelI64>);
+        if (label_dtype == kLabelI32) return flagged(tfy_head_checked_kernel<TFY_HEAD_LOGISTIC, kLabelI32>);
+        return flagged(tfy_head_checked_kernel<TFY_HEAD_LOGISTIC, kLabelF32>);
+    }
+    if (head == TFY_HEAD_BINARY || head == TFY_HEAD_MULTI_LABEL) {
         if (label_dtype == kLabelI64) return elementwise(tfy_head_elementwise_kernel<TFY_HEAD_BINARY, kLabelI64>);
         if (label_dtype == kLabelI32) return elementwise(tfy_head_elementwise_kernel<TFY_HEAD_BINARY, kLabelI32>);
         return elementwise(tfy_head_elementwise_kernel<TFY_HEAD_BINARY, kLabelF32>);
