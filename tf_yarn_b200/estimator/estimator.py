@@ -122,6 +122,7 @@ class Estimator:
         self._spec: Optional[EstimatorSpec] = None
         self._optimizer = None
         self._opt_desc: Optional[kopt.Optimizer] = None
+        self._scheduled = []
         self._opt_by_name: Dict[str, kopt.Optimizer] = {}
         self._global_step = 0
         self._device: Optional[torch.device] = None
@@ -192,13 +193,14 @@ class Estimator:
             d = next((gd for pref, gd in groups if n.startswith(pref)), desc)
             self._opt_by_name[n] = d
             buckets.setdefault(id(d), (d, []))[1].append(p)
+        # (torch optimizer, schedule) of every bucket whose learning rate follows a LearningRateSchedule
+        self._scheduled = []
         if not named:
             self._optimizer = None
-        elif len(buckets) == 1:
-            d, ps = next(iter(buckets.values()))
-            self._optimizer = d.to_torch(ps)
         else:
-            self._optimizer = _MultiOptimizer([d.to_torch(ps) for d, ps in buckets.values()])
+            opts = [(d, d.to_torch(ps)) for d, ps in buckets.values()]
+            self._optimizer = opts[0][1] if len(opts) == 1 else _MultiOptimizer([o for _, o in opts])
+            self._scheduled = [(o, d.schedule) for d, o in opts if getattr(d, "schedule", None) is not None]
 
     def _variables(self) -> List[torch.Tensor]:
         if self._network is None:
@@ -471,6 +473,10 @@ class Estimator:
             from tf_yarn_b200 import hvd
             grads = [p.grad for p in self._network.parameters() if p.grad is not None]
             hvd.grouped_allreduce_(grads, average=True)
+        for opt, schedule in self._scheduled:          # the rate of this update: the schedule at the global step
+            lr = float(schedule(self._global_step))
+            for g in opt.param_groups:
+                g["lr"] = lr
         self._optimizer.step()
         return loss.detach()
 

@@ -152,8 +152,10 @@ def _hyper_of(desc) -> Dict[str, float]:
 class WorkerConnection:
     """What a chief / worker holds: the mapped shards and the variable -> region table."""
 
-    def __init__(self, layout: Layout, shards: List[ShmShard], names: List[str]):
+    def __init__(self, layout: Layout, shards: List[ShmShard], names: List[str], schedules=None):
         self.layout, self.shards, self.names = layout, shards, names
+        # per variable: the LearningRateSchedule of its optimizer (None: the layout's constant lr)
+        self.schedules = list(schedules) if schedules else [None] * len(names)
         self._t = 0
 
     def _region(self, i: int, slot: int = 0) -> torch.Tensor:
@@ -174,6 +176,8 @@ class WorkerConnection:
         lay = self.layout
         params = dict(network.named_parameters())
         self._t += 1
+        # one global step for the whole push (another worker may advance it meanwhile): the pushes applied so far
+        step = max(self.global_step(), 0) if any(s is not None for s in self.schedules) else 0
         with torch.no_grad():
             for i, name in enumerate(self.names):
                 g = params[name].grad
@@ -181,6 +185,8 @@ class WorkerConnection:
                     continue
                 h = lay.hypers[i]
                 lr, p1, p2, eps, wd = h["lr"], h["p1"], h["p2"], h["eps"], h["wd"]
+                if self.schedules[i] is not None:
+                    lr = float(self.schedules[i](step))
                 g = g.detach().reshape(-1).float().cpu()
                 w = self._region(i)
                 if wd:
@@ -269,7 +275,8 @@ def connect_worker(network: nn.Module, opt_desc, cluster, is_chief: bool, global
     for i in range(n_ps):
         path = kv.wait(f"ps:{i}/shard").decode()
         shards.append(ShmShard(path, layout.shard_elems[i], create=False))
-    conn = WorkerConnection(layout, shards, names)
+    conn = WorkerConnection(layout, shards, names,
+                            [getattr((opt_by_name or {}).get(n, opt_desc), "schedule", None) for n in names])
     if is_chief:
         with torch.no_grad():
             for i, (_, p) in enumerate(named):

@@ -989,6 +989,10 @@ def _try_fuse_first_layer(conn: HbmConnection, network: nn.Module) -> bool:
 # ---------------------------------------------------------------------------------------------
 def connect_worker(network: nn.Module, opt_desc, cluster, is_chief: bool, global_step: int,
                    opt_by_name=None) -> HbmConnection:
+    if any(getattr(d, "schedule", None) is not None for d in [opt_desc, *(opt_by_name or {}).values()]):
+        raise ValueError("the HBM parameter server bakes the learning rate into its push kernels and does not run "
+                         "a LearningRateSchedule; use the shared-memory parameter server (TFY_PS_PLANE=shm) or a "
+                         "constant learning rate")
     client = _task_commons.TaskClient.from_current()
     kv = client.kv
     n_ps = len(cluster.spec["ps"])

@@ -109,6 +109,9 @@ class LearningRateScheduler(Callback):
         self.schedule, self.verbose = schedule, verbose
 
     def on_epoch_begin(self, epoch, logs=None):
+        if getattr(getattr(self.model, "optimizer", None), "schedule", None) is not None:
+            raise TypeError("LearningRateScheduler cannot drive an optimizer whose learning_rate is a "
+                            "LearningRateSchedule: the schedule already sets the rate of every step")
         lr = self.model.get_learning_rate()
         try:
             new = self.schedule(epoch, lr)

@@ -55,6 +55,8 @@ class EagerTrainEngine:
         self.distributed = distributed
         self.opt_desc = optimizer
         self.opt = optimizer.to_torch([p for p in net.parameters() if p.requires_grad])
+        self._schedule = getattr(optimizer, "schedule", None)
+        self.iterations = 0                 # updates applied (Keras optimizer.iterations): a schedule's step
         self.kernel_launches = 0
         self._cw = None                     # class-weight table [C] on the device (None: no class_weight)
         self._wacc = [[0.0, 0.0] for _ in self.weighted_metric_fns]     # epoch sums (sum w*m, sum w)
@@ -97,7 +99,12 @@ class EagerTrainEngine:
             for g in grads:
                 g.copy_(flat[o:o + g.numel()].view_as(g))
                 o += g.numel()
+        if self._schedule is not None:
+            lr = float(self._schedule(self.iterations))
+            for g in self.opt.param_groups:
+                g["lr"] = lr
         self.opt.step()
+        self.iterations += 1
         logs = {"loss": loss.detach()}
         with torch.no_grad():
             for name, fn in self.metric_fns:
@@ -131,21 +138,26 @@ class EagerTrainEngine:
         return out
 
     def set_learning_rate(self, lr: float) -> None:
+        if self._schedule is not None:
+            raise TypeError("the learning rate of this optimizer follows a LearningRateSchedule; it cannot be set")
         for g in self.opt.param_groups:
             g["lr"] = lr
 
     def get_learning_rate(self) -> float:
+        if self._schedule is not None:
+            return float(self._schedule(self.iterations))
         return self.opt.param_groups[0]["lr"]
 
     def sync_params_to_module(self) -> None:
         pass
 
     def state_dict(self) -> dict:
-        return {"kind": "eager", "optimizer": self.opt.state_dict()}
+        return {"kind": "eager", "optimizer": self.opt.state_dict(), "iterations": self.iterations}
 
     def load_state_dict(self, state: dict) -> None:
         if state.get("kind") == "eager":
             self.opt.load_state_dict(state["optimizer"])
+            self.iterations = int(state.get("iterations", 0))
 
     # fit() drives the eager engine synchronously
     pipelined = False
@@ -471,7 +483,7 @@ class GraphTrainEngine:
             self.fused.set_lr(lr)
 
     def get_learning_rate(self) -> float:
-        return float(self.fused._hyper_host.lr)
+        return self.fused.current_lr()
 
     def state_dict(self) -> dict:
         st = self.fused.gather_state()

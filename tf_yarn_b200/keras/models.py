@@ -693,7 +693,9 @@ class Model:
             self._pending_broadcast_root = root
 
     def get_learning_rate(self) -> float:
-        return self._engine.get_learning_rate() if self._engine is not None else self.optimizer.learning_rate
+        if self._engine is not None:
+            return self._engine.get_learning_rate()
+        return self.optimizer.current_learning_rate()
 
     def set_learning_rate(self, lr: float) -> None:
         self.optimizer.learning_rate = lr

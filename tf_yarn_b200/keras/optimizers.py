@@ -7,29 +7,59 @@ tests/test_optimizer_math.py).
 """
 from __future__ import annotations
 
-from typing import Iterable
+from typing import Iterable, Optional
 
 import torch
 
+from tf_yarn_b200.keras import schedules
 from tf_yarn_b200.parallel.optspec import OptimizerSpec
 
 
 class Optimizer:
+    """``learning_rate`` is a float or a :class:`~tf_yarn_b200.keras.schedules.LearningRateSchedule`.  A schedule is
+    evaluated at ``optimizer.iterations`` -- the updates already applied -- before every update: on the GPU by the
+    fused step itself, which writes the next step's rate where it advances its device step counter; on the CPU by
+    the engine.  As in Keras 3, the learning rate of a schedule-driven optimizer cannot be set."""
     kind = "sgd"
 
-    def __init__(self, learning_rate: float, **extra):
-        self.learning_rate = float(learning_rate)
+    def __init__(self, learning_rate, **extra):
+        self._learning_rate = learning_rate if schedules.is_schedule(learning_rate) else float(learning_rate)
         self.distributed = False        # set by hvd.DistributedOptimizer
         self.extra = extra
 
+    @property
+    def learning_rate(self):
+        """The float learning rate, or the schedule."""
+        return self._learning_rate
+
+    @learning_rate.setter
+    def learning_rate(self, v) -> None:
+        if self.schedule is not None:
+            raise TypeError(f"{type(self).__name__} was created with a LearningRateSchedule as its learning_rate "
+                            "argument, hence its learning rate is not settable")
+        self._learning_rate = v if schedules.is_schedule(v) else float(v)
+
     # lr alias used by Keras 2 code
     @property
-    def lr(self) -> float:
+    def lr(self):
         return self.learning_rate
 
     @lr.setter
-    def lr(self, v: float) -> None:
-        self.learning_rate = float(v)
+    def lr(self, v) -> None:
+        self.learning_rate = v
+
+    @property
+    def schedule(self) -> Optional[schedules.LearningRateSchedule]:
+        return self._learning_rate if schedules.is_schedule(self._learning_rate) else None
+
+    def current_learning_rate(self, step: int = 0) -> float:
+        """The learning rate of the update after ``step`` updates."""
+        return float(self.schedule(step)) if self.schedule is not None else self._learning_rate
+
+    @property
+    def _lr0(self) -> float:
+        """The float learning rate of the ``torch.optim`` rendition (the schedule's first; engines advance it)."""
+        return self.current_learning_rate(0)
 
     def to_spec(self) -> OptimizerSpec:
         raise NotImplementedError
@@ -38,7 +68,8 @@ class Optimizer:
         raise NotImplementedError
 
     def get_config(self):
-        return {"class_name": type(self).__name__, "learning_rate": self.learning_rate, **self.extra}
+        lr = schedules.serialize(self.schedule) if self.schedule is not None else self._learning_rate
+        return {"class_name": type(self).__name__, "learning_rate": lr, **self.extra}
 
 
 class SGD(Optimizer):
@@ -52,7 +83,7 @@ class SGD(Optimizer):
         return OptimizerSpec.sgd(self.learning_rate, self.momentum, 0.0, self.nesterov, self.weight_decay)
 
     def to_torch(self, params):
-        return torch.optim.SGD(params, lr=self.learning_rate, momentum=self.momentum, nesterov=self.nesterov,
+        return torch.optim.SGD(params, lr=self._lr0, momentum=self.momentum, nesterov=self.nesterov,
                                weight_decay=self.weight_decay)
 
 
@@ -67,7 +98,7 @@ class Adadelta(Optimizer):
         return OptimizerSpec.adadelta(self.learning_rate, self.rho, self.epsilon, self.weight_decay)
 
     def to_torch(self, params):
-        return torch.optim.Adadelta(params, lr=self.learning_rate, rho=self.rho, eps=self.epsilon,
+        return torch.optim.Adadelta(params, lr=self._lr0, rho=self.rho, eps=self.epsilon,
                                     weight_decay=self.weight_decay)
 
 
@@ -86,12 +117,13 @@ class Adam(Optimizer):
 
     def to_torch(self, params):
         cls = torch.optim.AdamW if self.decoupled else torch.optim.Adam
-        return cls(params, lr=self.learning_rate, betas=(self.beta_1, self.beta_2), eps=self.epsilon,
+        return cls(params, lr=self._lr0, betas=(self.beta_1, self.beta_2), eps=self.epsilon,
                    weight_decay=self.weight_decay)
 
 
 class AdamW(Adam):
     def __init__(self, learning_rate: float = 0.001, weight_decay: float = 0.004, **kw):
+        kw.pop("decoupled_weight_decay", None)       # in get_config() of an AdamW: always True
         super().__init__(learning_rate, weight_decay=weight_decay, decoupled_weight_decay=True, **kw)
 
 
@@ -109,7 +141,7 @@ class Adagrad(Optimizer):
                                      self.initial_accumulator_value)
 
     def to_torch(self, params):
-        return torch.optim.Adagrad(params, lr=self.learning_rate, eps=self.epsilon,
+        return torch.optim.Adagrad(params, lr=self._lr0, eps=self.epsilon,
                                    weight_decay=self.weight_decay,
                                    initial_accumulator_value=self.initial_accumulator_value)
 
@@ -135,7 +167,7 @@ class Ftrl(Optimizer):
         return OptimizerSpec.ftrl(self.learning_rate, self.l1, self.l2, self.beta, self.initial_accumulator_value)
 
     def to_torch(self, params):
-        return TorchFtrl(params, lr=self.learning_rate, l1=self.l1, l2=self.l2, beta=self.beta,
+        return TorchFtrl(params, lr=self._lr0, l1=self.l1, l2=self.l2, beta=self.beta,
                          initial_accumulator_value=self.initial_accumulator_value)
 
 
@@ -191,7 +223,7 @@ class RMSprop(Optimizer):
                                      self.weight_decay)
 
     def to_torch(self, params):
-        return TorchRMSprop(params, lr=self.learning_rate, rho=self.rho, momentum=self.momentum, eps=self.epsilon,
+        return TorchRMSprop(params, lr=self._lr0, rho=self.rho, momentum=self.momentum, eps=self.epsilon,
                             centered=self.centered, weight_decay=self.weight_decay)
 
 
@@ -256,4 +288,6 @@ def get(identifier) -> Optimizer:
 def from_config(cfg) -> Optimizer:
     cfg = dict(cfg)
     cls = _BY_NAME[cfg.pop("class_name").lower()]
+    if isinstance(cfg.get("learning_rate"), dict):
+        cfg["learning_rate"] = schedules.deserialize(cfg["learning_rate"])
     return cls(**cfg)

@@ -157,8 +157,19 @@ __global__ void tfy_barrier_kernel(TfyCommCtx c) { tfy_block_barrier(c); }
 // launch).  Splitting a step into ranges lets the engine run the update of gradients that are final early (the
 // big Dense kernel) inside the convolution-backward kernel (tfy_overlap_role) while this launch only handles the
 // rest; `advance` is set on the last launch of a step only, so every range of the step sees the same step counter.
-template <typename GT, typename PT, int OPT, int MODE, int U>
-__global__ void __launch_bounds__(256)
+// Minimum resident CTAs per SM of an instantiation (__launch_bounds__): 0 (none) for the constant-rate kernels, whose
+// code is as before.  The scheduled ones are held to the occupancy of their constant-rate twins, which the schedule's
+// tail would otherwise lower: 3 CTAs of 128 threads (at most 80 registers) in LOCAL mode, and in the multi-GPU modes
+// 2 CTAs of 256 threads (at most 128 registers, which every optimizer but RMSprop fits) -- the grid of a multi-GPU
+// step (up to 2 CTAs per SM) must be resident, since with zero_grads every CTA waits at the exit barrier.
+constexpr int tfy_k4_min_blocks(int opt, int mode, bool sched) {
+    return !sched ? 0 : mode == TFY_MODE_LOCAL ? 3 : opt == TFY_OPT_RMSPROP ? 1 : 2;
+}
+
+// SCHED (launched with TFY_OPT_LR_SCHEDULE): hp heads a TfyHyperBlock, and advancing the step also writes the
+// scheduled learning rate of the next one.
+template <typename GT, typename PT, int OPT, int MODE, int U, bool SCHED = false>
+__global__ void __launch_bounds__(256, tfy_k4_min_blocks(OPT, MODE, SCHED))
 tfy_fused_step_kernel(TfyCommCtx c, uint64_t grad_off, uint64_t param_off, size_t shard_n,
                       float* __restrict__ master, float* __restrict__ s1, float* __restrict__ s2,
                       TfyOptHyper* __restrict__ hp, int zero_grads, size_t g_lo, size_t g_hi, int advance) {
@@ -214,9 +225,12 @@ tfy_fused_step_kernel(TfyCommCtx c, uint64_t grad_off, uint64_t param_off, size_
         }
     }
 
-    // advance the device-side step counter exactly once per launch
+    // advance the device-side step counter (and a scheduled learning rate) exactly once per launch
     if (MODE != TFY_MODE_LOCAL) {
-        if (tfy_grid_finish(c, ep) && threadIdx.x == 0 && advance) hp->step = step + 1;
+        if (tfy_grid_finish(c, ep) && threadIdx.x == 0 && advance) {
+            if constexpr (SCHED) tfy_advance_scheduled_step(hp, step);
+            else hp->step = step + 1;
+        }
     } else {
         __syncthreads();
         if (threadIdx.x == 0) {
@@ -224,10 +238,20 @@ tfy_fused_step_kernel(TfyCommCtx c, uint64_t grad_off, uint64_t param_off, size_
             const uint32_t prev = atomicAdd(&hp->done, 1u);
             if (prev == gridDim.x - 1) {
                 hp->done = 0;
-                if (advance) hp->step = step + 1;
+                if (advance) {
+                    if constexpr (SCHED) tfy_advance_scheduled_step(hp, step);
+                    else hp->step = step + 1;
+                }
             }
         }
     }
+}
+
+// hp->lr = schedule(hp->step) of a TfyHyperBlock: the rate of the next step when the step counter is installed or
+// restored, by the same device function the scheduled fused step evaluates
+__global__ void tfy_lr_schedule_sync_kernel(TfyOptHyper* hp) {
+    if (threadIdx.x == 0 && blockIdx.x == 0)
+        hp->lr = tfy_lr_schedule_eval(reinterpret_cast<const TfyHyperBlock*>(hp)->sched, (int64_t)hp->step);
 }
 
 // ---------------------------------------------------------------------------
@@ -241,6 +265,11 @@ static inline int tfy_pick_grid(size_t work_items, int block, int max_grid) {
 }
 
 extern "C" {
+
+int tfy_lr_schedule_sync(TfyOptHyper* hp, cudaStream_t s) {
+    tfy_lr_schedule_sync_kernel<<<1, 32, 0, s>>>(hp);
+    return (int)cudaGetLastError();
+}
 
 int tfy_barrier(const TfyCommCtx* c, int grid, cudaStream_t s) {
     if (grid < 1) grid = 1;
@@ -307,15 +336,22 @@ static int tfy_fused_step_groups(const TfyCommCtx* c, int grad_dtype, int param_
                                  float* s2, TfyOptHyper* hp, int zero_grads, int grid, int block, size_t g_lo,
                                  size_t g_hi, size_t span_groups, int advance, cudaStream_t s) {
     if (mode == TFY_MODE_NVLS && c->mc_base == 0) return -5;
+    const bool sched = (opt & TFY_OPT_LR_SCHEDULE) != 0;
+    opt &= ~TFY_OPT_LR_SCHEDULE;
     if (block <= 0) block = (mode == TFY_MODE_LOCAL) ? 128 : 256;
     // single GPU: nothing to synchronise with, so oversubscribe the SMs for memory-level parallelism;
     // multi GPU: the cross-GPU barriers are grid-level (one signal per rank pair), 2 groups in flight per thread
     if (grid <= 0) grid = tfy_pick_grid(span_groups + 1, block * (mode == TFY_MODE_LOCAL ? 1 : 2),
                                         mode == TFY_MODE_LOCAL ? TFY_NUM_SMS * 6 : TFY_NUM_SMS * 2);
     if (grid > TFY_MAX_BLOCKS) grid = TFY_MAX_BLOCKS;
-#define TFY_FS4(GT, PT, O, M, U)                                                                                 \
-    tfy_launch_pdl_if(tfy_pdl_enabled() || tfy_pdl_k4_enabled(), (tfy_fused_step_kernel<GT, PT, O, M, U>), dim3(grid), dim3(block), 0, s, *c, grad_off, param_off, \
+#define TFY_FS5(GT, PT, O, M, U, S)                                                                              \
+    tfy_launch_pdl_if(tfy_pdl_enabled() || tfy_pdl_k4_enabled(), (tfy_fused_step_kernel<GT, PT, O, M, U, S>), dim3(grid), dim3(block), 0, s, *c, grad_off, param_off, \
                    shard_n, master, s1, s2, hp, zero_grads, g_lo, g_hi, advance)
+#define TFY_FS4(GT, PT, O, M, U)                          \
+    do {                                                  \
+        if (sched) TFY_FS5(GT, PT, O, M, U, true);        \
+        else TFY_FS5(GT, PT, O, M, U, false);             \
+    } while (0)
 #define TFY_FS3(GT, PT, O)                                                  \
     do {                                                                    \
         if (mode == TFY_MODE_LOCAL) TFY_FS4(GT, PT, O, TFY_MODE_LOCAL, 1);  \
@@ -338,6 +374,7 @@ static int tfy_fused_step_groups(const TfyCommCtx* c, int grad_dtype, int param_
 #undef TFY_FS2
 #undef TFY_FS3
 #undef TFY_FS4
+#undef TFY_FS5
     return (int)cudaGetLastError();
 }
 

@@ -10,6 +10,8 @@
 #include <stdlib.h>
 #include <string.h>
 
+#include "tfy_lr_schedule.cuh"
+
 #define TFY_NUM_SMS 132               // H100 SXM: sizes the grid caps of the streaming kernels
 #define TFY_MAX_RANKS 16
 #define TFY_MAX_BLOCKS 1024            // barrier slots (one per CTA index)
@@ -42,10 +44,27 @@ struct TfyOptHyper {
     uint32_t pad;
 };
 
+// The hyper block of a fused step launched with TFY_OPT_LR_SCHEDULE: the schedule follows the hyper-parameters, and
+// the step stores hp.lr = schedule(hp.step) whenever it advances hp.step (tfy_lr_schedule.cuh).
+struct TfyHyperBlock {
+    TfyOptHyper hp;
+    TfyLrSchedule sched;
+};
+
+// Called by the one thread that advances the step counter of a scheduled step, after every CTA of the step has read
+// hp->lr.
+__device__ __forceinline__ void tfy_advance_scheduled_step(TfyOptHyper* hp, int step) {
+    hp->step = step + 1;
+    hp->lr = tfy_lr_schedule_eval(reinterpret_cast<const TfyHyperBlock*>(hp)->sched, (int64_t)step + 1);
+}
+
 enum TfyDtype { TFY_BF16 = 0, TFY_F32 = 1 };
 enum TfyAlgo { TFY_ALGO_ONESHOT = 0, TFY_ALGO_TWOSHOT = 1, TFY_ALGO_NVLS = 2 };
 enum TfyOpt { TFY_OPT_SGD = 0, TFY_OPT_ADADELTA = 1, TFY_OPT_ADAM = 2, TFY_OPT_ADAGRAD = 3, TFY_OPT_FTRL = 4,
                TFY_OPT_RMSPROP = 5 };
+// Or-ed into the `opt` code of a fused-step launch: `hp` heads a TfyHyperBlock and the step evaluates its schedule.
+// The bit selects separate instantiations, so the kernels of a constant learning rate carry no schedule code.
+#define TFY_OPT_LR_SCHEDULE 0x100
 enum TfyMode { TFY_MODE_LOCAL = 0, TFY_MODE_P2P = 1, TFY_MODE_NVLS = 2 };
 
 // ---------------------------------------------------------------------------

@@ -48,6 +48,43 @@ class OptHyper(ctypes.Structure):
     ]
 
 
+LR_MAX_BOUNDARIES = 16
+OPT_LR_SCHEDULE = 0x100          # or-ed into a fused step's opt code: hp heads a HyperBlock whose schedule it evaluates
+LR_CONSTANT, LR_EXPONENTIAL, LR_PIECEWISE, LR_POLYNOMIAL, LR_INVERSE_TIME, LR_COSINE, LR_COSINE_RESTARTS = range(7)
+
+
+class LrSchedule(ctypes.Structure):
+    """Mirror of TfyLrSchedule (ops/csrc/tfy_lr_schedule.cuh)."""
+    _fields_ = [
+        ("kind", ctypes.c_int32),
+        ("flags", ctypes.c_int32),
+        ("n_boundaries", ctypes.c_int32),
+        ("pad", ctypes.c_int32),
+        ("initial_lr", ctypes.c_double),
+        ("decay_steps", ctypes.c_double),
+        ("decay_rate", ctypes.c_double),
+        ("end_lr", ctypes.c_double),
+        ("power", ctypes.c_double),
+        ("alpha", ctypes.c_double),
+        ("warmup_target", ctypes.c_double),
+        ("warmup_steps", ctypes.c_double),
+        ("t_mul", ctypes.c_double),
+        ("m_mul", ctypes.c_double),
+        ("boundaries", ctypes.c_double * LR_MAX_BOUNDARIES),
+        ("values", ctypes.c_float * (LR_MAX_BOUNDARIES + 1)),
+        ("pad2", ctypes.c_int32),
+    ]
+
+
+class HyperBlock(ctypes.Structure):
+    """Mirror of TfyHyperBlock (ops/csrc/tfy_common.cuh): the device-resident hyper-parameters of a fused optimizer,
+    followed by its learning-rate schedule (read only by a step launched with ``OPT_LR_SCHEDULE``)."""
+    _fields_ = [
+        ("hp", OptHyper),
+        ("sched", LrSchedule),
+    ]
+
+
 class OverlapStep(ctypes.Structure):
     """Mirror of TfyOverlapStep (ops/csrc/tfy_fused_step.cuh): a fused gradient-exchange / optimizer step that the
     communication CTAs of a persistent compute kernel run next to the compute."""
@@ -93,6 +130,8 @@ def _declare(lib: ctypes.CDLL) -> None:
     lib.tfy_symm_close.restype = None
 
     lib.tfy_barrier.argtypes = [ctxp, i, vp]
+    if hasattr(lib, "tfy_lr_schedule_sync"):
+        lib.tfy_lr_schedule_sync.argtypes = [vp, vp]
     lib.tfy_allreduce.argtypes = [ctxp, i, i, u64, sz, f, vp, i, i, vp]
     lib.tfy_broadcast.argtypes = [ctxp, u64, sz, i, i, i, i, vp]
     lib.tfy_allgather.argtypes = [ctxp, u64, sz, i, i, vp]

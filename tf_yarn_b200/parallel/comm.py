@@ -263,6 +263,30 @@ class Communicator:
 # ---------------------------------------------------------------------------
 # K4: fused reduce-scatter -> optimizer -> all-gather over flat buffers
 # ---------------------------------------------------------------------------
+def hyper_block(spec: OptimizerSpec, step: int = 0) -> "native.HyperBlock":
+    """The device hyper block of ``spec`` at ``step`` completed updates.  With a learning-rate schedule, ``hp.lr`` is
+    the rate of the next update and the fused step writes each later one where it advances the step counter."""
+    blk = native.HyperBlock()
+    blk.hp = native.OptHyper(spec.lr, spec.p1, spec.p2, spec.eps, spec.weight_decay, 1.0, step, spec.flags, 0, 0)
+    if spec.schedule is not None:
+        fields = dict(spec.schedule._device_fields())
+        bounds, values = fields.pop("boundaries", ()), fields.pop("values", ())
+        for k, v in fields.items():
+            setattr(blk.sched, k, v)
+        for i, b in enumerate(bounds):
+            blk.sched.boundaries[i] = b
+        for i, v in enumerate(values):
+            blk.sched.values[i] = v
+        blk.hp.lr = float(spec.schedule(step))
+    return blk
+
+
+def launch_code(spec: OptimizerSpec) -> int:
+    """The ``opt`` code of a fused-step launch: the optimizer, plus ``OPT_LR_SCHEDULE`` when a schedule drives the
+    learning rate (its instantiations advance the rate with the step counter; the others carry no schedule code)."""
+    return spec.code | (native.OPT_LR_SCHEDULE if spec.schedule is not None else 0)
+
+
 class FusedShardedOptimizer:
     """Flat parameter / gradient buffers + the fused K4 step.
 
@@ -311,10 +335,12 @@ class FusedShardedOptimizer:
         self.master = torch.zeros(self.shard_n, dtype=torch.float32, device=dev)
         self.s1 = torch.full((self.shard_n,), spec.init_s1, dtype=torch.float32, device=dev)
         self.s2 = torch.zeros(spec.s2_numel(self.shard_n), dtype=torch.float32, device=dev)
-        self._hyper_host = native.OptHyper(spec.lr, spec.p1, spec.p2, spec.eps, spec.weight_decay, 1.0, 0,
-                                           spec.flags, 0, 0)
-        self.hyper = torch.zeros(ctypes.sizeof(native.OptHyper), dtype=torch.uint8, device=dev)
+        self._block = hyper_block(spec)
+        self._code = launch_code(spec)
+        self._hyper_host = self._block.hp
+        self.hyper = torch.zeros(ctypes.sizeof(native.HyperBlock), dtype=torch.uint8, device=dev)
         self._push_hyper()
+        self._sync_scheduled_lr()
         self.param_views = [self.flat_params[o:o + n].view(shp) for o, n, shp in
                             zip(self.offsets, self.numels, self.shapes)]
         self.grad_views = [self.flat_grads[o:o + n].view(shp) for o, n, shp in
@@ -324,12 +350,22 @@ class FusedShardedOptimizer:
 
     # -- hyper-parameters (device resident so CUDA graphs see updates) --------
     def _push_hyper(self) -> None:
-        raw = bytes(self._hyper_host)
+        raw = bytes(self._block)
         host = torch.frombuffer(bytearray(raw), dtype=torch.uint8)
         self.hyper.copy_(host)
 
+    def _sync_scheduled_lr(self, stream=None) -> None:
+        """With a schedule: ``hp.lr = schedule(hp.step)`` written on the device by the function the fused step
+        evaluates, so the rate of an installed or restored step has the bits an uninterrupted run would read."""
+        if self.spec.schedule is not None:
+            native.check(self.comm.lib.tfy_lr_schedule_sync(self.hyper.data_ptr(), _stream_ptr(stream)),
+                         "tfy_lr_schedule_sync")
+
     def set_lr(self, lr: float) -> None:
         """Update lr on the device (4-byte async copy; safe between graph replays)."""
+        if self.spec.schedule is not None:
+            raise TypeError("the learning rate of this optimizer follows a LearningRateSchedule, which the fused "
+                            "step evaluates on the device; it cannot be set")
         self._hyper_host.lr = float(lr)
         t = torch.tensor([lr], dtype=torch.float32).view(torch.uint8)
         self.hyper[0:4].copy_(t, non_blocking=True)
@@ -344,7 +380,15 @@ class FusedShardedOptimizer:
         return int(self.hyper[24:28].view(torch.int32).item())
 
     def set_step_count(self, n: int) -> None:
+        """Set the device step counter; with a schedule, also the rate of the next step (``schedule(n)``)."""
         self.hyper[24:28].copy_(torch.tensor([n], dtype=torch.int32).view(torch.uint8))
+        self._sync_scheduled_lr()
+
+    def current_lr(self) -> float:
+        """The learning rate of the next step (with a schedule, the one the device holds: a 4-byte read)."""
+        if self.spec.schedule is not None:
+            return float(self.hyper[0:4].view(torch.float32).item())
+        return float(self._hyper_host.lr)
 
     # -- initialisation ------------------------------------------------------
     def init_from(self, tensors: Sequence[torch.Tensor], broadcast_root: Optional[int] = 0) -> None:
@@ -379,13 +423,13 @@ class FusedShardedOptimizer:
                 raise ValueError("ranged steps do not clear gradients: construct with zero_grads=False")
             g0, g1 = shard_groups
             rc = c.lib.tfy_fused_step_shard_range(
-                c.arena.ctx_ref, _DT[self.grad_dtype], _DT[self.param_dtype], self.spec.code, c.mode,
+                c.arena.ctx_ref, _DT[self.grad_dtype], _DT[self.param_dtype], self._code, c.mode,
                 self.grad_off, self.param_off, self.shard_n,
                 self.master.data_ptr(), self.s1.data_ptr(), self.s2.data_ptr(), self.hyper.data_ptr(),
                 0, 0, int(block), int(g0), int(g1), int(advance), _stream_ptr(stream))
         elif elem_range is None and advance:
             rc = c.lib.tfy_fused_step(
-                c.arena.ctx_ref, _DT[self.grad_dtype], _DT[self.param_dtype], self.spec.code, c.mode,
+                c.arena.ctx_ref, _DT[self.grad_dtype], _DT[self.param_dtype], self._code, c.mode,
                 self.grad_off, self.param_off, self.shard_n,
                 self.master.data_ptr(), self.s1.data_ptr(), self.s2.data_ptr(), self.hyper.data_ptr(),
                 int(self.zero_grads), self.grid, self.block, _stream_ptr(stream))
@@ -396,7 +440,7 @@ class FusedShardedOptimizer:
             if e0 % 8 or e1 % 8 or not 0 <= e0 <= e1 <= self.n:
                 raise ValueError(f"bad element range {elem_range} for a buffer of {self.n}")
             rc = c.lib.tfy_fused_step_range(
-                c.arena.ctx_ref, _DT[self.grad_dtype], _DT[self.param_dtype], self.spec.code, c.mode,
+                c.arena.ctx_ref, _DT[self.grad_dtype], _DT[self.param_dtype], self._code, c.mode,
                 self.grad_off, self.param_off, self.shard_n,
                 self.master.data_ptr(), self.s1.data_ptr(), self.s2.data_ptr(), self.hyper.data_ptr(),
                 0, 0, int(block), e0, e1, int(advance), _stream_ptr(stream))

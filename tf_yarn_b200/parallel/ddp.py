@@ -32,7 +32,7 @@ import torch
 import torch.nn as nn
 
 from tf_yarn_b200.ops import native
-from tf_yarn_b200.parallel.comm import _DT, Communicator
+from tf_yarn_b200.parallel.comm import _DT, Communicator, _stream_ptr, hyper_block, launch_code
 from tf_yarn_b200.parallel.optspec import OptimizerSpec
 
 _vp, _i, _u64, _sz = ctypes.c_void_p, ctypes.c_int, ctypes.c_uint64, ctypes.c_size_t
@@ -197,11 +197,12 @@ class DistributedDataParallel(nn.Module):
             b.master = b.pflat[r * b.shard_n:(r + 1) * b.shard_n].float().clone()
             b.s1 = torch.full((b.shard_n,), spec.init_s1, dtype=torch.float32, device=dev)
             b.s2 = torch.zeros(spec.s2_numel(b.shard_n), dtype=torch.float32, device=dev)
-            host = native.OptHyper(spec.lr, spec.p1, spec.p2, spec.eps, spec.weight_decay, 1.0, 0, spec.flags, 0, 0)
-            b.hyper = torch.frombuffer(bytearray(bytes(host)), dtype=torch.uint8).to(dev)
+            b.hyper = torch.frombuffer(bytearray(bytes(hyper_block(spec))), dtype=torch.uint8).to(dev)
+            if spec.schedule is not None:
+                native.check(comm.lib.tfy_lr_schedule_sync(b.hyper.data_ptr(), _stream_ptr()), "tfy_lr_schedule_sync")
             native.check(comm.lib.tfy_reducer_set_fused(
                 self._reducer, bi, _DT[b.dtype], b.poff, b.master.data_ptr(), b.s1.data_ptr(), b.s2.data_ptr(),
-                b.shard_n, spec.code, comm.mode, b.hyper.data_ptr()), "tfy_reducer_set_fused")
+                b.shard_n, launch_code(spec), comm.mode, b.hyper.data_ptr()), "tfy_reducer_set_fused")
         torch.cuda.current_stream().synchronize()
         if world > 1:
             comm.barrier()
@@ -341,14 +342,55 @@ class DistributedDataParallel(nn.Module):
     # (tf_yarn/pytorch/model_ckpt.py saves ``model.module.state_dict()`` when it sees a wrapper).
 
 
+class _ScheduledParamGroup(dict):
+    """``param_groups[0]`` of a fused optimizer whose rate follows a LearningRateSchedule: ``["lr"]`` reads the rate
+    the fused step will use next from the device (a 4-byte read), and setting it -- e.g. by a torch LR scheduler --
+    raises at once, since the fused step writes every rate itself."""
+
+    def __init__(self, opt: "_FusedOptimizer", params):
+        super().__init__(params=params)
+        self._opt = opt
+
+    def __getitem__(self, key):
+        if key == "lr":
+            return self._opt.current_lr()
+        return super().__getitem__(key)
+
+    def __setitem__(self, key, value):
+        if key in ("lr", "initial_lr"):
+            raise TypeError("the learning rate of this optimizer follows a LearningRateSchedule, which the fused "
+                            "step evaluates on the device; it cannot be set")
+        super().__setitem__(key, value)
+
+    def setdefault(self, key, default=None):
+        if key not in self:
+            self[key] = default
+        return self[key]
+
+    def __contains__(self, key):
+        return key == "lr" or super().__contains__(key)
+
+
 class _FusedOptimizer:
     """Optimizer-shaped handle of :meth:`DistributedDataParallel.fuse_optimizer`."""
 
     def __init__(self, ddp: "DistributedDataParallel", spec: OptimizerSpec):
         self._ddp, self.spec = ddp, spec
-        self.param_groups = [{"lr": spec.lr, "params": [p for b in ddp._buckets for p in b.params]}]
+        params = [p for b in ddp._buckets for p in b.params]
+        if spec.schedule is not None:
+            self.param_groups = [_ScheduledParamGroup(self, params)]
+        else:
+            self.param_groups = [{"lr": spec.lr, "params": params}]
+
+    def current_lr(self) -> float:
+        """The learning rate of the next step (with a schedule, the one the device holds)."""
+        if self.spec.schedule is None:
+            return float(self.param_groups[0]["lr"])
+        return float(self._ddp._buckets[0].hyper[0:4].view(torch.float32).item())
 
     def step(self, closure=None):
+        if self.spec.schedule is not None:          # the fused step writes every rate itself
+            return None
         lr = float(self.param_groups[0]["lr"])
         if lr != self.spec.lr:                       # an LR scheduler changed it: 4-byte copies, graph/stream safe
             self.set_lr(lr)
@@ -358,6 +400,9 @@ class _FusedOptimizer:
         return None
 
     def set_lr(self, lr: float) -> None:
+        if self.spec.schedule is not None:
+            raise TypeError("the learning rate of this optimizer follows a LearningRateSchedule, which the fused "
+                            "step evaluates on the device; it cannot be set")
         self.spec.lr = float(lr)
         t = torch.tensor([lr], dtype=torch.float32).view(torch.uint8)
         for b in self._ddp._buckets:
@@ -390,6 +435,9 @@ class _FusedOptimizer:
                 b.s1.fill_(self.spec.init_s1)
                 b.s2.zero_()
             b.hyper[24:28].copy_(torch.tensor([st["step"]], dtype=torch.int32).view(torch.uint8))
+            if self.spec.schedule is not None:      # the rate of the restored step, written by the device function
+                native.check(self._ddp.comm.lib.tfy_lr_schedule_sync(b.hyper.data_ptr(), _stream_ptr()),
+                             "tfy_lr_schedule_sync")
         if foreign:
             import logging
             logging.getLogger(__name__).warning(

@@ -15,6 +15,11 @@ class OptimizerSpec:
         kind = kind.lower()
         if kind not in self.KINDS:
             raise ValueError(f"unknown fused optimizer {kind!r}")
+        # a learning-rate schedule (keras.optimizers.schedules): `lr` is its rate at step 0, the fused step writes the
+        # rate of every later step on the device
+        self.schedule = lr if callable(lr) and hasattr(lr, "get_config") else None
+        if self.schedule is not None:
+            lr = self.schedule(0)
         self.kind, self.lr, self.p1, self.p2, self.eps = kind, float(lr), float(p1), float(p2), float(eps)
         self.weight_decay, self.flags, self.init_s1 = float(weight_decay), int(flags), float(init_s1)
         if kind == "adamw":
