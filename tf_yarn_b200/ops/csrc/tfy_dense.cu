@@ -7,9 +7,10 @@
 // batch <= 128, units <= 128, in-features = 9216).  The two GEMMs share the dh operand, have the same
 // output width and a tiny K, so ONE CTA per 64-column slice of the in-features does both: dh (32 KB) and the
 // slice's x and W tiles (16 KB each) arrive by TMA, one warpgroup per product issues wgmma M64 N64 K16 on both
-// 64-row halves of its 128-row accumulator, and converts it to bf16 in shared memory for a TMA store (dW straight
-// into the flat gradient buffer the fused optimizer/collective step consumes).  No operand is transposed in
-// memory: the SAME shared-memory bytes of dh serve as the K-major A operand of dx and, through the transpose flag
+// 64-row halves of its 128-row accumulator, and packs it to bf16 from registers into the B-operand tile it has
+// finished reading, for a TMA store (dW straight into the flat gradient buffer the fused optimizer/collective step
+// consumes).  At 65 KB of shared memory two CTAs fit per SM, so the 144 CTAs of the 9216-wide layer run in one
+// wave.  No operand is transposed in memory: the SAME shared-memory bytes of dh serve as the K-major A operand of dx and, through the transpose flag
 // of the wgmma, as the MN-major A operand of dW; x and W tiles are MN-major B operands as they sit in memory
 // (in-features contiguous).  This replaces two cuBLAS GEMM launches of the round-1 step
 // (reference path being replaced: the Dense backward of the Keras/Horovod worker, tf_yarn/tensorflow/tasks/
@@ -28,9 +29,7 @@ constexpr int DB_K = 128;             // batch (dW) / units (dx)
 constexpr int DB_THREADS = 288;
 constexpr int DH_BYTES = DB_M * 128 * 2;          // two 64-column boxes of 128 rows x 128 B
 constexpr int TILE_BYTES = 128 * 128;             // 128 rows x 64 bf16
-constexpr int ACC_LD = DB_N + 4;                  // fp32 row pitch of a staged accumulator
-constexpr int ACC_BYTES = DB_M * ACC_LD * 4;
-constexpr size_t DB_SMEM = 1024 + DH_BYTES + 2 * TILE_BYTES /*x, w*/ + 2 * TILE_BYTES /*staging*/ + 2 * ACC_BYTES + 256;
+constexpr size_t DB_SMEM = 1024 + DH_BYTES + 2 * TILE_BYTES /*x, w*/ + 256;
 
 // Operands are 128-byte swizzled views (tfy_wg_desc_sw128), sbo = 8 rows of 128 B.  K-major: rows = M/N index (64
 // K-elements each).  MN-major: rows = K index (64 M/N-elements each); one M64 / N64 operand is exactly one atom, so
@@ -52,27 +51,28 @@ __device__ __forceinline__ void d_mma_chunk(float (&acc)[2][DB_N / 2], uint32_t 
     }
 }
 
-// Warpgroup epilogue: accumulator -> fp32 rows (acc_s) -> bf16, 128-byte-swizzled [128 rows][128 B] tile (stage)
-// -> one TMA store.  `bar` is the named barrier of the warpgroup.
-__device__ __forceinline__ void d_epilogue(float (&acc)[2][DB_N / 2], float* acc_s, uint8_t* stage, int bar,
-                                           const CUtensorMap* map, int c0, int c1) {
-    tfy_wg_store_rows<DB_N>(acc_s, ACC_LD, acc[0], 0);
-    tfy_wg_store_rows<DB_N>(acc_s, ACC_LD, acc[1], 64);
-    asm volatile("bar.sync %0, 128;" ::"r"(bar) : "memory");
-    const int row = threadIdx.x & 127;
-    const float* src = acc_s + row * ACC_LD;
-    uint8_t* dst = stage + row * 128;
+// Warpgroup epilogue: accumulator -> bf16, 128-byte-swizzled [128 rows][128 B] tile (stage) -> one TMA store.  Each
+// thread packs its fragment's column pairs straight from registers (the rounding TfyPack<bf16> applies), so `stage`
+// may be the B-operand tile the warpgroup's wgmma has just read.  `bar` is the named barrier of the warpgroup.
+__device__ __forceinline__ void d_epilogue(float (&acc)[2][DB_N / 2], uint8_t* stage, int bar, const CUtensorMap* map,
+                                           int c0, int c1) {
+    const int w = (threadIdx.x >> 5) & 3, l = threadIdx.x & 31;
+    asm volatile("bar.sync %0, 128;" ::"r"(bar) : "memory");     // every warp's wgmma is done reading `stage`
 #pragma unroll
-    for (int ch = 0; ch < 8; ++ch) {                  // 8 chunks of 16 B (8 bf16) per 128-byte row
-        float v[8];
-        *reinterpret_cast<float4*>(v) = *reinterpret_cast<const float4*>(src + ch * 8);
-        *reinterpret_cast<float4*>(v + 4) = *reinterpret_cast<const float4*>(src + ch * 8 + 4);
-        // 128-byte swizzle of the TMA store map: 16-byte chunk index XOR (row mod 8)
-        *reinterpret_cast<uint4*>(dst + ((ch ^ (row & 7)) << 4)) = TfyPack<__nv_bfloat16>::pack(v);
+    for (int h = 0; h < 2; ++h) {
+        // fragment rows 16 w + l / 4 and 8 below it; columns 8 j + 2 (l % 4) + {0, 1} = bytes 4 (l % 4) of 16-byte
+        // chunk j, stored at chunk j XOR (row mod 8) (the 128-byte swizzle of the TMA store map; row mod 8 = l / 4)
+        uint8_t* r0 = stage + (h * 64 + 16 * w + (l >> 2)) * 128 + 4 * (l & 3);
+#pragma unroll
+        for (int j = 0; j < DB_N / 8; ++j) {
+            const int sw = (j ^ (l >> 2)) << 4;
+            *reinterpret_cast<uint32_t*>(r0 + sw) = tfy_pack_bf16x2(acc[h][4 * j], acc[h][4 * j + 1]);
+            *reinterpret_cast<uint32_t*>(r0 + 8 * 128 + sw) = tfy_pack_bf16x2(acc[h][4 * j + 2], acc[h][4 * j + 3]);
+        }
     }
     tfy_fence_proxy_async();     // generic-proxy writes -> async proxy
     asm volatile("bar.sync %0, 128;" ::"r"(bar) : "memory");
-    if (row < 32 && tfy_elect_one()) {
+    if ((threadIdx.x & 127) < 32 && tfy_elect_one()) {
         tfy_tma_store_2d(map, stage, c0, c1);
         asm volatile("cp.async.bulk.commit_group;" ::: "memory");
         asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");  // smem must outlive the read
@@ -81,7 +81,7 @@ __device__ __forceinline__ void d_epilogue(float (&acc)[2][DB_N / 2], float* acc
 
 }  // namespace
 
-__global__ void __launch_bounds__(DB_THREADS, 1)
+__global__ void __launch_bounds__(DB_THREADS, 2)
 tfy_dense_bwd_kernel(const __grid_constant__ CUtensorMap map_dh, const __grid_constant__ CUtensorMap map_x,
                      const __grid_constant__ CUtensorMap map_w, const __grid_constant__ CUtensorMap map_dw,
                      const __grid_constant__ CUtensorMap map_dx, int want_dx) {
@@ -90,9 +90,7 @@ tfy_dense_bwd_kernel(const __grid_constant__ CUtensorMap map_dh, const __grid_co
     uint8_t* s_dh = smem;                            // [2 boxes][128 rows (batch)][128 B (64 units)]  sw128
     uint8_t* s_x = s_dh + DH_BYTES;                  // [128 rows (batch)][128 B (64 in-features)]     sw128
     uint8_t* s_w = s_x + TILE_BYTES;                 // [128 rows (units)][128 B (64 in-features)]     sw128
-    uint8_t* s_out = s_w + TILE_BYTES;               // [2][128 rows][128 B] staging for the TMA stores, sw128
-    float* s_acc = reinterpret_cast<float*>(s_out + 2 * TILE_BYTES);    // [2][128][ACC_LD] fp32
-    uint64_t* full = reinterpret_cast<uint64_t*>(reinterpret_cast<uint8_t*>(s_acc) + 2 * ACC_BYTES);
+    uint64_t* full = reinterpret_cast<uint64_t*>(s_w + TILE_BYTES);
 
     const int warp = __shfl_sync(0xffffffffu, (int)threadIdx.x >> 5, 0);   // warp-uniform role index
     const int n0 = blockIdx.x * DB_N;
@@ -128,8 +126,8 @@ tfy_dense_bwd_kernel(const __grid_constant__ CUtensorMap map_dh, const __grid_co
     else d_mma_chunk<0>(acc, dh0, tfy_smem_u32(s_w), true);
     tfy_wg_commit();
     tfy_wg_wait<0>();
-    d_epilogue(acc, s_acc + which * (ACC_BYTES / 4), s_out + which * TILE_BYTES, 1 + which,
-               which == 0 ? &map_dw : &map_dx, n0, 0);
+    // dW is staged in the x tile, dx in the W tile: each is read by its own warpgroup's wgmma only
+    d_epilogue(acc, which == 0 ? s_x : s_w, 1 + which, which == 0 ? &map_dw : &map_dx, n0, 0);
 }
 
 // ---------------------------------------------------------------------------------------------------------
@@ -141,7 +139,7 @@ tfy_dense_bwd_kernel(const __grid_constant__ CUtensorMap map_dh, const __grid_co
 // ---------------------------------------------------------------------------------------------------------
 namespace {
 constexpr int DT_STAGES = 3, DT_STAGE_BYTES = DH_BYTES + TILE_BYTES, DT_THREADS = 160;
-constexpr size_t DT_SMEM = 1024 + (size_t)DT_STAGES * DT_STAGE_BYTES + TILE_BYTES + ACC_BYTES + 256;
+constexpr size_t DT_SMEM = 1024 + (size_t)DT_STAGES * DT_STAGE_BYTES + TILE_BYTES + 256;
 }  // namespace
 
 __global__ void __launch_bounds__(DT_THREADS, 1)
@@ -152,8 +150,7 @@ tfy_dense_bwd_tiled_kernel(const __grid_constant__ CUtensorMap map_dh, const __g
     uint8_t* smem = tfy_align1024(smem_raw);
     uint8_t* ring = smem;                                            // [3] { dh box0, dh box1, tile }
     uint8_t* s_out = ring + (size_t)DT_STAGES * DT_STAGE_BYTES;      // staging for the TMA store
-    float* s_acc = reinterpret_cast<float*>(s_out + TILE_BYTES);     // [128][ACC_LD] fp32
-    uint64_t* full = reinterpret_cast<uint64_t*>(reinterpret_cast<uint8_t*>(s_acc) + ACC_BYTES);
+    uint64_t* full = reinterpret_cast<uint64_t*>(s_out + TILE_BYTES);
     uint64_t* empty = full + DT_STAGES;
 
     const int warp = __shfl_sync(0xffffffffu, (int)threadIdx.x >> 5, 0), lane = threadIdx.x & 31;   // warp-uniform role index
@@ -207,7 +204,7 @@ tfy_dense_bwd_tiled_kernel(const __grid_constant__ CUtensorMap map_dh, const __g
         tfy_wg_wait<0>();
         if (lane == 0) tfy_mbar_arrive(&empty[st]);
     }
-    d_epilogue(acc, s_acc, s_out, 1, is_dw ? &map_dw : &map_dx, n0, m0);
+    d_epilogue(acc, s_out, 1, is_dw ? &map_dw : &map_dx, n0, m0);
 }
 
 namespace {

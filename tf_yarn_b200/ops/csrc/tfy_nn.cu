@@ -212,13 +212,11 @@ tfy_conv3x3_c1_wgrad_kernel(const XT* __restrict__ x, const __nv_bfloat16* __res
 // y = dropout(act(z + bias[c])) over a [rows, C] bf16 matrix (C % 8 == 0); y may alias z.
 // mask (optional, 1 byte per element): 1 = gradient flows (act'(.) != 0 and kept).
 // ---------------------------------------------------------------------------------------------
-// ZT = __nv_bfloat16: z is a bf16 matrix.  ZT = float: z holds the `splits` fp32 partial-product slabs
-// ([splits][rows][C]) of the split-K GEMM; they are summed here in slab order (the same result on every run).
 template <typename ZT>
 __global__ void __launch_bounds__(256)
 tfy_bias_act_drop_fwd_kernel(ZT* z, const __nv_bfloat16* __restrict__ bias, __nv_bfloat16* y,
                              uint8_t* __restrict__ mask, size_t rows, int C, int relu, float drop_rate, uint32_t seed,
-                             const TfyOptHyper* __restrict__ hp, int splits) {
+                             const TfyOptHyper* __restrict__ hp) {
     tfy_pdl_sync();
     const int G = C / 8;
     const size_t total = rows * G;
@@ -228,18 +226,7 @@ tfy_bias_act_drop_fwd_kernel(ZT* z, const __nv_bfloat16* __restrict__ bias, __nv
          idx += (size_t)gridDim.x * blockDim.x) {
         const int g = idx % G;
         float v[8], bv[8];
-        if (sizeof(ZT) == 4) {
-#pragma unroll
-            for (int k = 0; k < 8; ++k) v[k] = 0.f;
-#pragma unroll 8
-            for (int sl = 0; sl < splits; ++sl) {              // unrolled: eight slabs' loads in flight at once
-                const float4* zp = reinterpret_cast<const float4*>(z) + (size_t)sl * total * 2 + idx * 2;
-                const float4 a = __ldcg(zp), b = __ldcg(zp + 1);
-                v[0] += a.x; v[1] += a.y; v[2] += a.z; v[3] += a.w; v[4] += b.x; v[5] += b.y; v[6] += b.z; v[7] += b.w;
-            }
-        } else {
-            TfyPack<__nv_bfloat16>::unpack(tfy_ld16(reinterpret_cast<const __nv_bfloat16*>(z) + idx * 8), v);
-        }
+        TfyPack<__nv_bfloat16>::unpack(tfy_ld16(reinterpret_cast<const __nv_bfloat16*>(z) + idx * 8), v);
         if (bias) {
             TfyPack<__nv_bfloat16>::unpack(tfy_ld16(bias + g * 8), bv);
 #pragma unroll
@@ -260,6 +247,51 @@ tfy_bias_act_drop_fwd_kernel(ZT* z, const __nv_bfloat16* __restrict__ bias, __nv
         }
         tfy_st16(y + idx * 8, TfyPack<__nv_bfloat16>::pack(v));
         if (mask) *reinterpret_cast<uint2*>(mask + idx * 8) = make_uint2(m_lo, m_hi);
+    }
+}
+
+// Same, from the `splits` fp32 partial-product slabs z32 ([splits][rows][C]) of the split-K GEMM, summed in slab
+// order (the same result on every run).  It sits between the GEMM and the head on the step's critical path and moves
+// little data, so its time is L2 latency: one thread per 4 elements (one float4 per slab) and every slab's load in
+// flight at once.  Element e draws tfy_uniform(seed, step, e), as in the bf16 kernel above.
+__global__ void __launch_bounds__(32)
+tfy_bias_act_drop_fwd_kernel_slabs(const float* __restrict__ z32, const __nv_bfloat16* __restrict__ bias,
+                                   __nv_bfloat16* __restrict__ y, uint8_t* __restrict__ mask, size_t n4, int C,
+                                   int relu, float drop_rate, uint32_t seed, const TfyOptHyper* __restrict__ hp,
+                                   int splits) {
+    tfy_pdl_sync();
+    const uint32_t step = hp ? (uint32_t)hp->step : 0u;
+    const float keep_scale = drop_rate > 0.f ? 1.f / (1.f - drop_rate) : 1.f;
+    for (size_t q = (size_t)blockIdx.x * blockDim.x + threadIdx.x; q < n4; q += (size_t)gridDim.x * blockDim.x) {
+        const size_t e0 = q * 4;
+        float v[4] = {0.f, 0.f, 0.f, 0.f};
+        for (int s0 = 0; s0 < splits; s0 += 24) {          // up to 24 loads issued before the first add
+            float4 a[24];
+#pragma unroll
+            for (int j = 0; j < 24; ++j)
+                if (s0 + j < splits) a[j] = __ldcg(reinterpret_cast<const float4*>(z32) + (size_t)(s0 + j) * n4 + q);
+#pragma unroll
+            for (int j = 0; j < 24; ++j)
+                if (s0 + j < splits) { v[0] += a[j].x; v[1] += a[j].y; v[2] += a[j].z; v[3] += a[j].w; }
+        }
+        if (bias) {
+            const uint2 b = *reinterpret_cast<const uint2*>(bias + e0 % C);
+            v[0] += tfy_bf16lo(b.x); v[1] += tfy_bf16hi(b.x); v[2] += tfy_bf16lo(b.y); v[3] += tfy_bf16hi(b.y);
+        }
+        uint32_t m = 0;
+#pragma unroll
+        for (int k = 0; k < 4; ++k) {
+            bool on = true;
+            if (relu) { on = v[k] > 0.f; v[k] = on ? v[k] : 0.f; }
+            if (drop_rate > 0.f) {
+                const bool keep = tfy_uniform(seed, step, e0 + k) >= drop_rate;
+                v[k] = keep ? v[k] * keep_scale : 0.f;
+                on = on && keep;
+            }
+            m |= (on ? 1u : 0u) << (8 * k);
+        }
+        *reinterpret_cast<uint2*>(y + e0) = make_uint2(tfy_pack_bf16x2(v[0], v[1]), tfy_pack_bf16x2(v[2], v[3]));
+        if (mask) *reinterpret_cast<uint32_t*>(mask + e0) = m;
     }
 }
 
@@ -923,7 +955,7 @@ int tfy_bias_act_drop_fwd(const void* z, const void* bias, void* y, void* mask, 
     const int grid = tfy_grid_for(rows * (C / 8), 256, TFY_NUM_SMS * 8);
     tfy_launch_pdl((tfy_bias_act_drop_fwd_kernel<__nv_bfloat16>), dim3(grid), dim3(256), 0, s, (__nv_bfloat16*)z, (const __nv_bfloat16*)bias,
                                                                      (__nv_bfloat16*)y, (uint8_t*)mask, rows, C, relu,
-                                                                     drop_rate, seed, hp, 1);
+                                                                     drop_rate, seed, hp);
     return (int)cudaGetLastError();
 }
 
@@ -932,10 +964,11 @@ int tfy_bias_act_drop_fwd_f32(void* z32, const void* bias, void* y, void* mask, 
                               float drop_rate, uint32_t seed, const TfyOptHyper* hp, int splits, cudaStream_t s) {
     if (C % 8 || splits < 1) return -2;
     // one warp per block: every thread reads `splits` slabs, so the reads are spread over as many SMs as possible
-    const int grid = tfy_grid_for(rows * (C / 8), 32, TFY_NUM_SMS * 16);
-    tfy_launch_pdl((tfy_bias_act_drop_fwd_kernel<float>), dim3(grid), dim3(32), 0, s, (float*)z32, (const __nv_bfloat16*)bias,
-                                                             (__nv_bfloat16*)y, (uint8_t*)mask, rows, C, relu,
-                                                             drop_rate, seed, hp, splits);
+    const size_t n4 = rows * (size_t)(C / 4);
+    const int grid = tfy_grid_for(n4, 32, TFY_NUM_SMS * 16);
+    tfy_launch_pdl(tfy_bias_act_drop_fwd_kernel_slabs, dim3(grid), dim3(32), 0, s, (const float*)z32,
+                   (const __nv_bfloat16*)bias, (__nv_bfloat16*)y, (uint8_t*)mask, n4, C, relu, drop_rate, seed, hp,
+                   splits);
     return (int)cudaGetLastError();
 }
 
