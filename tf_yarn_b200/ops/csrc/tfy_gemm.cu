@@ -291,7 +291,8 @@ int tfy_splitk_sum_f32(const float* slabs, float* out, int splits, size_t slab, 
 // split_k > 1 (or C == nullptr): C32 is a workspace of tfy_gemm_bf16_splitk_slabs(K, split_k) x M x ldc floats; slab z
 // (C32 + z * M * ldc) receives the partial product of K-slice z, to be summed in slab order (tfy_splitk_sum_f32,
 // tfy_bias_act_drop_fwd_f32).
-// Requirements: K % 8 == 0, lda % 8 == 0, ldb % 8 == 0, 16-byte aligned base pointers.
+// Requirements: K % 8 == 0, lda % 8 == 0, ldb % 8 == 0 (-2), 16-byte aligned A, B, and C (when ldc % 8 == 0) or C32
+// (when ldc % 4 == 0) as soon as N >= 16 (-3).
 int tfy_gemm_bf16(const void* A, const void* B, void* C, float* C32, const void* bias, int M, int N, int K, int lda,
                   int ldb, int ldc, int relu, int split_k, cudaStream_t s) {
     if ((K & 7) || (lda & 7) || (ldb & 7)) return -2;
@@ -312,6 +313,9 @@ int tfy_gemm_bf16(const void* A, const void* B, void* C, float* C32, const void*
     split_k = (k_tiles + per - 1) / per;
     const int out_mode = (split_k > 1 || (C == nullptr && C32 != nullptr)) ? 1 : 0;
     if (out_mode == 1 && C32 == nullptr) return -7;
+    // the epilogue stores 16 bytes at a time (8 bf16 / 4 floats) whenever the row pitch allows it and a row has 16 columns
+    if (N >= 16 && (out_mode == 0 ? ((ldc & 7) == 0 && ((uintptr_t)C & 15)) : ((ldc & 3) == 0 && ((uintptr_t)C32 & 15))))
+        return -3;
     dim3 grid((M + BM - 1) / BM, (N + BN - 1) / BN, split_k);
     tfy_launch_pdl((tfy_gemm_bf16_kernel), dim3(grid), dim3(GEMM_THREADS), SMEM_BYTES, s, ma, mb, (__nv_bfloat16*)C, C32,
                                                                 (const __nv_bfloat16*)bias, M, N, K, ldc, relu,
@@ -321,13 +325,16 @@ int tfy_gemm_bf16(const void* A, const void* B, void* C, float* C32, const void*
 
 // Split-K GEMM with the fused epilogue: y[M,N] (bf16) = dropout(act(A . B^T + bias)), mask[M,N] (optional bytes).
 // acc32: fp32 scratch of tfy_gemm_bf16_splitk_slabs(K, split_k) x M x N floats (slabs of row pitch N); counters: two uint32 per
-// 128x128 output tile, zero on entry, left zero.  N % 8 == 0.  The K-slice CTAs of a tile meet on a counter, so the
+// 128x128 output tile, zero on entry, left zero.  N % 8 == 0 (-2); A, B, y, acc32 and bias 16-byte aligned, mask 8-byte
+// aligned (-3).  The K-slice CTAs of a tile meet on a counter, so the
 // whole grid must be co-resident: returns -8 when tiles x split_k exceeds the SM count (use the two-launch path).
 int tfy_gemm_bf16_splitk_fused(const void* A, const void* B, float* acc32, uint32_t* counters, const void* bias, void* y,
                                void* mask, int M, int N, int K, int lda, int ldb, int relu, float drop_rate, uint32_t seed,
                                const TfyOptHyper* hp, int split_k, cudaStream_t s) {
     if ((K & 7) || (lda & 7) || (ldb & 7) || (N & 7)) return -2;
     if (((uintptr_t)A & 15) || ((uintptr_t)B & 15) || ((uintptr_t)y & 15)) return -3;
+    // the epilogue reads acc32 and bias 16 bytes at a time and writes the mask 8 bytes at a time
+    if (((uintptr_t)acc32 & 15) || ((uintptr_t)bias & 15) || ((uintptr_t)mask & 7)) return -3;
     if (!tfy_tensor_map_encoder()) return -4;
     if (!g_attr_set) {
         if (cudaFuncSetAttribute(tfy_gemm_bf16_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMEM_BYTES) !=

@@ -1047,7 +1047,8 @@ int tfy_memcpy_async(void* dst, const void* src, size_t bytes, cudaStream_t s) {
 
 int tfy_nn_set_timeline(long long* buf) { return (int)cudaMemcpyToSymbol(n_timeline, &buf, sizeof(buf)); }
 
-// fused classifier head (forward + backward); returns -2 when the shape is outside the kernel's envelope.
+// fused classifier head (forward + backward); returns -2 when the shape is outside the kernel's envelope, -3 when h,
+// w2 or scratch is not 16-byte aligned or dw2 not 8-byte aligned.
 // scratch: tfy_dense_head_scratch_elems(K, C, B) floats and counter: one uint32, zero on entry (left zero).
 // loss_host: optional second destination of the loss, e.g. a pinned host scalar (device-accessible under UVA).
 size_t tfy_dense_head_scratch_elems(int K, int C, int B) {
@@ -1062,6 +1063,8 @@ static int tfy_dense_head_launch(const void* h, const void* w2, const void* b2, 
                                  void* dh, void* db1, float* scratch, uint32_t* counter, int B, int K, int C,
                                  const float* sample_w, const float* class_w, cudaStream_t s) {
     if (!(K == 128 || K == 256 || K == 512) || C < 1 || C > HEAD_CMAX || B < 1) return -2;
+    // h, W2 and the scratch slabs are read 16 bytes at a time, dW2 written 8 bytes at a time
+    if ((((uintptr_t)h | (uintptr_t)w2 | (uintptr_t)scratch) & 15) || ((uintptr_t)dw2 & 7)) return -3;
     constexpr int NRED = WEIGHTED ? 4 : 2;
     const size_t smem = (size_t)HEAD_ROWS * (K + 8) * 2 +
                         ((size_t)HEAD_CMAX * K + HEAD_ROWS * HEAD_CMAX + HEAD_CMAX + NRED * HEAD_WARPS + (K > 256 ? K : 256)) * 4;
