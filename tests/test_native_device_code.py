@@ -1,8 +1,11 @@
 """The update formulas of the fused K4 kernel (ops/csrc/tfy_fused_step.cuh: tfy_step_consts + tfy_opt_update_rt), built
 for the host and checked against torch.optim on the CPU -- through the framework's own chain: mini-Keras optimizer
--> OptimizerSpec (hyper-parameter packing) -> TfyOptHyper (device struct) -> per-element update.  The GPU tests cover
-SGD / Adadelta / Adam / Adagrad in LOCAL mode on a H100; this also covers FTRL, AdamW, Nesterov momentum, weight decay
-and the 1/world gradient scaling, on every box."""
+-> OptimizerSpec (hyper-parameter packing) -> TfyOptHyper (device struct) -> per-element update, with exact
+sqrt / rsqrt / division in place of the SFU approximations.  It covers every optimizer, AdamW, Nesterov momentum,
+weight decay and the 1/world gradient scaling, on every box.  On an H100, test_gpu_fused_step.py runs the kernel itself
+for all six optimizers, every (gradient, parameter) dtype pair, ranged and split launches, the MNIST-CNN's size, the
+U=2 multi-GPU instantiations at world 1 and the overlap role, against the float64 reference of
+fused_step_reference.py."""
 import ctypes
 import os
 import shutil

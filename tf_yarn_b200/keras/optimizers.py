@@ -2,8 +2,9 @@
 
 A descriptor only carries hyper-parameters.  On H100 the train engine maps it to
 the fused K4 kernel (``OptimizerSpec``); on CPU it is instantiated as the
-equivalent ``torch.optim`` optimizer (same update formulas, see
-tests/test_optimizer_math.py).
+equivalent ``torch.optim`` optimizer (same update formulas: tests/test_native_device_code.py checks the kernel's
+update against them on the CPU, tests/fused_step_reference.py states them in float64, and
+tests/test_gpu_fused_step.py holds the kernel to that reference on the GPU).
 """
 from __future__ import annotations
 

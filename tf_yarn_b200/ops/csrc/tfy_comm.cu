@@ -264,6 +264,20 @@ static inline int tfy_pick_grid(size_t work_items, int block, int max_grid) {
     return (int)g;
 }
 
+// Largest grid of `kernel` whose CTAs are all resident at once.  A multi-GPU fused step needs that: with zero_grads
+// every CTA waits at the exit barrier for the last one to arrive, so a CTA that has to wait for a free SM never
+// starts.  The RMSprop instantiations take more than 128 registers and fit one 256-thread CTA per SM, not two.
+template <typename K>
+static int tfy_resident_grid(K kernel, int grid, int block) {
+    int dev = 0, sms = 0, per_sm = 0;
+    if (cudaGetDevice(&dev) != cudaSuccess ||
+        cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess ||
+        cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, block, 0) != cudaSuccess)
+        return grid;
+    const int cap = per_sm * sms;
+    return cap > 0 && grid > cap ? cap : grid;
+}
+
 extern "C" {
 
 int tfy_lr_schedule_sync(TfyOptHyper* hp, cudaStream_t s) {
@@ -345,8 +359,11 @@ static int tfy_fused_step_groups(const TfyCommCtx* c, int grad_dtype, int param_
                                         mode == TFY_MODE_LOCAL ? TFY_NUM_SMS * 6 : TFY_NUM_SMS * 2);
     if (grid > TFY_MAX_BLOCKS) grid = TFY_MAX_BLOCKS;
 #define TFY_FS5(GT, PT, O, M, U, S)                                                                              \
-    tfy_launch_pdl_if(tfy_pdl_enabled() || tfy_pdl_k4_enabled(), (tfy_fused_step_kernel<GT, PT, O, M, U, S>), dim3(grid), dim3(block), 0, s, *c, grad_off, param_off, \
-                   shard_n, master, s1, s2, hp, zero_grads, g_lo, g_hi, advance)
+    do {                                                                                                         \
+        if (M != TFY_MODE_LOCAL) grid = tfy_resident_grid(tfy_fused_step_kernel<GT, PT, O, M, U, S>, grid, block); \
+        tfy_launch_pdl_if(tfy_pdl_enabled() || tfy_pdl_k4_enabled(), (tfy_fused_step_kernel<GT, PT, O, M, U, S>), dim3(grid), dim3(block), 0, s, *c, grad_off, param_off, \
+                       shard_n, master, s1, s2, hp, zero_grads, g_lo, g_hi, advance);                          \
+    } while (0)
 #define TFY_FS4(GT, PT, O, M, U)                          \
     do {                                                  \
         if (sched) TFY_FS5(GT, PT, O, M, U, true);        \
