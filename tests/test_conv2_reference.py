@@ -185,7 +185,7 @@ class _RecLib:
 
 
 @pytest.mark.parametrize("rate", [0.0, 0.1, 0.3, 0.9, 0.99])
-def test_fast_path_backward_scale_of_a_tensor_core_stage_is_the_kernel_rule(rate):
+def test_conv_drop_scale_is_the_keep_scale_rule_for_a_tensor_core_stage(rate):
     from tf_yarn_b200.keras import layers as L
     from tf_yarn_b200.keras.fastpath import FastSequentialEngine
     st = types.SimpleNamespace(kind="conv", layer=L.Conv2D(64, 3, activation="relu"), relu=True, pool=True, drop=rate)
@@ -195,8 +195,5 @@ def test_fast_path_backward_scale_of_a_tensor_core_stage_is_the_kernel_rule(rate
     # a stage whose forward ran the general pool kernel keeps that kernel's 1 / (1 - rate)
     assert FastSequentialEngine._conv_drop_scale(eng, st, False) == (1.0 / (1.0 - rate) if rate > 0 else 1.0)
     assert eng.lib.calls == [rate]
-    # and the backward asks for it with the stage's forward kind
-    import inspect
-    src = inspect.getsource(FastSequentialEngine._forward_backward)
-    assert "scale = self._conv_drop_scale(st, st.pool and self._tc_conv(st, B))" in src
-    assert src.count("1.0 / (1.0 - st.drop)") == 1           # only the Dense stage's own mask kernels
+    # which of the two the step's backward kernels receive is read from the step's launch trace:
+    # test_fastpath_step_trace.py::test_pooled_conv_backward_scale_is_the_one_its_forward_applied

@@ -71,7 +71,7 @@ def test_models_outside_the_grammar_fall_back(layers, loss, metrics):
     assert _plan(layers, loss=loss, metrics=metrics) is None
 
 
-def test_kernel_envelopes_split_k_and_tensor_core_conv(monkeypatch):
+def test_kernel_envelopes_split_k_and_tensor_core_conv_shapes():
     """Which shapes go to the split-K wgmma GEMM and to the wgmma convolution kernels (everything else is served by
     cuBLAS / cuDNN with a one-time warning)."""
     E = fastpath.FastSequentialEngine
@@ -80,7 +80,7 @@ def test_kernel_envelopes_split_k_and_tensor_core_conv(monkeypatch):
     assert E._split_k(128, 128, 9217) == 1             # K not a multiple of 8 (TMA row pitch)
     assert E._split_k(2048, 1024, 9216) == 1           # many output tiles: a plain GEMM fills the machine
     assert 1 < E._split_k(256, 256, 4096) <= 144 // 4  # 4 tiles share the 144 CTAs
-    monkeypatch.delenv("TFY_NO_TC_CONV", raising=False)
+    assert E._split_k(128, 128, 9216, 4) == 36         # TFY_SPLITK_TILES=4: 4 k-tiles per CTA
     m = keras_mnist_cnn()
     m.compile(loss=LOGITS, optimizer="sgd")
     m.build()
@@ -89,5 +89,5 @@ def test_kernel_envelopes_split_k_and_tensor_core_conv(monkeypatch):
     assert E._tc_conv(c2, 128) and E._tc_conv(c2, 2)
     assert not E._tc_conv(c2, 3)                       # odd batch: images are processed in pairs
     assert not E._tc_conv(c1, 128)                     # C_in = 1 has its own first-layer kernels
-    monkeypatch.setenv("TFY_NO_TC_CONV", "1")
-    assert not E._tc_conv(c2, 128)                     # A/B switch
+    # the TFY_NO_TC_CONV switch is applied when the step's kernels are chosen, to these and the C_in = 1 kernels:
+    # test_fastpath_step_trace.py::test_no_tc_conv_switch_turns_every_tensor_core_convolution_kernel_off

@@ -24,6 +24,7 @@ from __future__ import annotations
 
 import ctypes
 import os
+import types
 from typing import List, Optional
 
 import torch
@@ -196,16 +197,9 @@ class FastSequentialEngine(GraphTrainEngine):
         self._hp = self.fused.hyper.data_ptr()
         self._k = 0
         self._acc32 = {}
-        # Gradient-exchange overlap (opt-in, TFY_OVERLAP=1): parameters whose gradients are final before the
-        # convolution weight-gradient kernel starts (every layer AFTER that convolution: for the MNIST-CNN the two
-        # Dense layers, 98 % of the bytes) can be reduce-scattered / updated / all-gathered by COMMUNICATION CTAs
-        # inside that kernel (ops/csrc/tfy_fused_step.cuh: tfy_overlap_role) on the 4 SMs its patch grid leaves
-        # idle, the trailing fused-step launch handling the rest.  Numerically equivalent (GPU test); off by default
-        # because the cost of the trailing launch is the LATENCY chain signal -> in-switch reduce -> store/ack ->
-        # signal, which a smaller range does not shorten.
-        self._overlap = os.environ.get("TFY_OVERLAP", "0") == "1"
-        self._ov_used = False
-        self._ov_gmid = 0
+        self._resolved_b = None          # batch size the plan's kernels were chosen for (_resolve)
+        self._overlap = False
+        self._ov_gmid = 0                # first shard group the weight-gradient kernel updates (0: none)
         self._warned = set()
         self._conv_sync = torch.zeros(1024, dtype=torch.int32, device=dev)     # grid barrier of the wgrad kernel
         self._c1_acc = torch.zeros(160 * 320, dtype=torch.float32, device=dev)   # first-layer dW/db per-CTA partials
@@ -225,20 +219,22 @@ class FastSequentialEngine(GraphTrainEngine):
         return mod.weight, mod.bias
 
     @staticmethod
-    def _split_k(M: int, N: int, K: int) -> int:
-        """Split factor of the wgmma GEMM for skinny-output / long-K dense layers (1 = use cuBLAS)."""
+    def _bf16(t: torch.Tensor) -> torch.Tensor:
+        return t if (t.dtype == torch.bfloat16 and t.is_contiguous()) else t.to(torch.bfloat16).contiguous()
+
+    @staticmethod
+    def _split_k(M: int, N: int, K: int, per_cta: int = 6) -> int:
+        """Split factor of the wgmma GEMM for skinny-output / long-K dense layers (1 = use cuBLAS); ``per_cta``
+        k-tiles per CTA (6 == the TMA ring depth)."""
         tiles = ((M + 127) // 128) * ((N + 127) // 128)
         k_tiles = (K + 63) // 64
         if K % 8 or tiles > 8 or k_tiles < 32:
             return 1
-        per_cta = int(os.environ.get("TFY_SPLITK_TILES", "6"))   # k-tiles per CTA (6 == the TMA ring depth)
         return max(1, min(k_tiles // per_cta, 144 // tiles))
 
     @staticmethod
     def _tc_conv(st, B: int) -> bool:
-        """True when the stage is served by the wgmma implicit-GEMM kernels of ops/csrc/tfy_conv.cu."""
-        if os.environ.get("TFY_NO_TC_CONV") == "1":       # A/B switch: cuDNN + separate pool kernel instead
-            return False
+        """True when the stage's shape is served by the wgmma implicit-GEMM kernels of ops/csrc/tfy_conv.cu."""
         ly = st.layer
         H, W, Cin = ly.input_shape_
         return (Cin == 32 and ly.filters == 64 and st.pool and st.relu and (H - 2) % 8 == 0 and (W - 2) % 8 == 0
@@ -258,7 +254,7 @@ class FastSequentialEngine(GraphTrainEngine):
             import logging
             logging.getLogger(__name__).warning(msg)
 
-    def _overlap_desc(self, li: int, B: int, H: int, W: int):
+    def _overlap_desc(self, li: int, B: int, H: int, W: int, groups_override: Optional[str]):
         """Fused-step descriptor for the communication CTAs of conv stage ``li``'s weight-gradient kernel, or None.
 
         Overlapped: shard-relative groups [g_mid, S/8) of EVERY rank (balanced), where g_mid*8 is at least the
@@ -266,8 +262,7 @@ class FastSequentialEngine(GraphTrainEngine):
         shard starts with the still-pending convolution parameters).  The size of the overlapped part is bounded
         by what ``n_cta`` SMs can move while the weight gradient runs (TFY_OVERLAP_GROUPS overrides)."""
         fused = self.fused
-        if not self._overlap or self._ov_used or fused.zero_grads or fused.param_dtype != torch.bfloat16 \
-                or fused.grad_dtype != torch.bfloat16:
+        if fused.zero_grads or fused.param_dtype != torch.bfloat16 or fused.grad_dtype != torch.bfloat16:
             return None
         if fused.spec.kind == "rmsprop":             # no overlap role for RMSprop: the trailing step updates everything
             return None
@@ -284,13 +279,12 @@ class FastSequentialEngine(GraphTrainEngine):
         g_split = (e_split + 7) // 8
         if g_split >= groups:
             return None                              # rank 0's shard is all pending parameters: nothing balanced to take
-        budget = int(os.environ.get("TFY_OVERLAP_GROUPS", str(2000 * n_cta)))
+        budget = int(groups_override) if groups_override is not None else 2000 * n_cta
         g_mid = max(g_split, groups - budget)
         if groups - g_mid < 64:
             return None
-        ov = fused.overlap_step(g_mid, groups, n_cta)
-        self._ov_used, self._ov_gmid = True, g_mid
-        return ov
+        self._ov_gmid = g_mid
+        return fused.overlap_step(g_mid, groups, n_cta)
 
     def _host_loss_ptr(self):
         """Pinned scalar of the slot being captured: the head kernel stores the loss there directly (UVA), so the
@@ -301,9 +295,10 @@ class FastSequentialEngine(GraphTrainEngine):
         self._loss_in_host[slot] = True
         return self._loss_host[slot].data_ptr()
 
-    def _splitk_acc(self, key, slabs: int, M: int, N: int) -> torch.Tensor:
-        if key not in self._acc32 or tuple(self._acc32[key].shape) != (slabs, M, N):
-            self._acc32[key] = torch.zeros((slabs, M, N), dtype=torch.float32, device=self.device)
+    def _scratch(self, key, numel: int, dtype=torch.float32) -> torch.Tensor:
+        """Engine-owned scratch buffer ``key`` of at least ``numel`` elements, zeroed when (re)allocated."""
+        if key not in self._acc32 or self._acc32[key].numel() < numel:
+            self._acc32[key] = torch.zeros(numel, dtype=dtype, device=self.device)
         return self._acc32[key]
 
     def pop_metrics(self):
@@ -329,355 +324,345 @@ class FastSequentialEngine(GraphTrainEngine):
                 self._s())
 
     def _capture(self, x, y, w=None) -> None:
+        self._resolve(x.shape[0])
         super()._capture(x, y, w)
         with torch.cuda.stream(self.stream):
             self._stats.zero_()          # warm-up steps must not count in the epoch metrics
         self.stream.synchronize()
 
-    # ------------------------------------------------------------------ the step
-    @torch.no_grad()
-    def _forward_backward(self, x, y, sw=None) -> None:
-        lib, s = self.lib, self._s()
-        self._k = 0
-        B = x.shape[0]
-        bf16 = torch.bfloat16
-        saved = []
-        cur = x                    # NHWC for images, [B, F] for vectors
-        cur_is_f32 = cur.dtype == torch.float32
-        # -------- forward
-        for li, st in enumerate(self.plan):
-            seed = (self._seed * 2654435761 + li * 97) & 0x7fffffff
+    # ------------------------------------------------------------------ kernel choice
+    def _resolve(self, B: int) -> None:
+        """Choose every stage's kernels for batch size ``B`` and allocate their scratch buffers.  Runs at capture and
+        whenever a step's batch size differs from the last one resolved; the A/B switches are read here, so a change
+        to one takes effect at the next capture or batch-size change."""
+        env = os.environ.get
+        tc_conv = env("TFY_NO_TC_CONV") != "1"         # off: cuDNN + the general pool kernels instead
+        unpool_fusion = env("TFY_NO_UNPOOL_FUSION") != "1"
+        tc_dense_bwd = env("TFY_NO_TC_DENSE_BWD") != "1"
+        fused_head = env("TFY_NO_FUSED_HEAD") != "1"
+        splitk_fuse = env("TFY_SPLITK_FUSE") == "1"
+        splitk_tiles = int(env("TFY_SPLITK_TILES", "6"))
+        # Gradient-exchange overlap (opt-in, TFY_OVERLAP=1): parameters whose gradients are final before the
+        # convolution weight-gradient kernel starts (every layer AFTER that convolution: for the MNIST-CNN the two
+        # Dense layers, 98 % of the bytes) can be reduce-scattered / updated / all-gathered by COMMUNICATION CTAs
+        # inside that kernel (ops/csrc/tfy_fused_step.cuh: tfy_overlap_role) on the 4 SMs its patch grid leaves
+        # idle, the trailing fused-step launch handling the rest.  Numerically equivalent (GPU test); off by default
+        # because the cost of the trailing launch is the LATENCY chain signal -> in-switch reduce -> store/ack ->
+        # signal, which a smaller range does not shorten.
+        self._overlap = env("TFY_OVERLAP", "0") == "1"
+        overlap_groups = env("TFY_OVERLAP_GROUPS")
+        lib, plan = self.lib, self.plan
+        for li, st in enumerate(plan):
+            prev = plan[li - 1] if li > 0 else None
+            st.li, st.first = li, li == 0
+            st.seed = (self._seed * 2654435761 + li * 97) & 0x7fffffff
+            st.gated = False         # conv: the next stage's data gradient applies this stage's ReLU gate
             if st.kind == "conv":
                 ly = st.layer
-                w, b = self._wb(ly)
                 H, W, Cin = ly.input_shape_
                 O = ly.filters
-                OH, OW = H - 2, W - 2
-                fused_pre = False
-                if self._tc_conv(st, B):
-                    # wgmma implicit GEMM; bias + ReLU + 2x2 max-pool + dropout in the epilogue
-                    xin = cur if (cur.dtype == bf16 and cur.is_contiguous()) else cur.to(bf16).contiguous()
-                    p = torch.empty((B, OH // 2, OW // 2, O), dtype=bf16, device=cur.device)
-                    code = torch.empty((B, OH // 2, OW // 2, O), dtype=torch.uint8, device=cur.device)
-                    self._chk(lib.tfy_conv3x3_c32_pool_fwd(xin.data_ptr(), w.data_ptr(), b.data_ptr(), p.data_ptr(),
-                                                           code.data_ptr(), B, H, W, float(st.drop), seed, self._hp,
-                                                           s), "conv3x3_c32_pool_fwd")
-                    saved.append((xin, False, None, code))
-                    cur = p
-                    cur_is_f32 = False
-                    continue
-                if Cin == 1:
-                    # direct kernel: conv + bias + relu in one launch (relu folded only when requested)
-                    a = torch.empty((B, OH, OW, O), dtype=bf16, device=cur.device)
-                    if st.relu and not st.pool:
-                        if O == 32 and os.environ.get("TFY_NO_TC_CONV") != "1":
-                            self._chk(lib.tfy_conv3x3_c1_fwd_tc(cur.data_ptr(), int(cur_is_f32), w.data_ptr(),
-                                                                b.data_ptr(), a.data_ptr(), B, H, W, s),
-                                      "conv3x3_c1_fwd_tc")
-                        else:
-                            self._chk(lib.tfy_conv3x3_c1_fwd(cur.data_ptr(), int(cur_is_f32), w.data_ptr(),
-                                                             b.data_ptr(), a.data_ptr(), B, H, W, O, s),
-                                      "conv3x3_c1_fwd")
-                        fused_pre = True
-                        z = a
-                    else:
-                        z = None
+                st.tc = tc_conv and self._tc_conv(st, B)
+                if st.tc:
+                    st.fwd = "c32_pool_tc"
+                elif Cin == 1 and st.relu and not st.pool:
+                    st.fwd = "c1_tc" if O == 32 and tc_conv else "c1"
                 else:
-                    z = None
-                if z is None:
+                    st.fwd = "cudnn"
                     self._warn_once(f"conv_fwd:{li}", f"Conv2D layer {li} ({Cin} -> {O} channels, {H}x{W}, batch {B}) is "
                                     "outside the wgmma convolution kernels' envelope (C_in 32 / C_out 64 with ReLU + 2x2 "
                                     "pool, or C_in 1): forward and backward use cuDNN")
-                    xin = cur.to(bf16) if cur.dtype != bf16 else cur
-                    zc = F.conv2d(xin.permute(0, 3, 1, 2), w)       # NCHW logical over NHWC bytes
-                    z = zc.permute(0, 2, 3, 1)
-                    if not z.is_contiguous():
-                        z = z.contiguous()
-                if st.pool:
-                    p = torch.empty((B, OH // 2, OW // 2, O), dtype=bf16, device=cur.device)
-                    code = torch.empty((B, OH // 2, OW // 2, O), dtype=torch.uint8, device=cur.device)
-                    self._chk(lib.tfy_bias_relu_pool_drop_fwd(z.data_ptr(), b.data_ptr(), p.data_ptr(), code.data_ptr(),
-                                                              B, OH, OW, O, float(st.drop), seed, self._hp, s),
-                              "bias_relu_pool_drop_fwd")
-                    saved.append((cur, cur_is_f32, None, code))
-                    cur = p
-                else:
-                    mask = None
-                    if not fused_pre:
-                        if st.drop > 0:
-                            mask = torch.empty((B, OH, OW, O), dtype=torch.uint8, device=cur.device)
-                        self._chk(lib.tfy_bias_act_drop_fwd(z.data_ptr(), b.data_ptr(), z.data_ptr(),
-                                                            mask.data_ptr() if mask is not None else None,
-                                                            B * OH * OW, O, int(st.relu), float(st.drop), seed,
-                                                            self._hp, s), "bias_act_drop_fwd")
-                    elif st.drop > 0:
-                        mask = torch.empty((B, OH, OW, O), dtype=torch.uint8, device=cur.device)
-                        self._chk(lib.tfy_bias_act_drop_fwd(z.data_ptr(), None, z.data_ptr(), mask.data_ptr(),
-                                                            B * OH * OW, O, 1, float(st.drop), seed, self._hp, s),
-                                  "bias_act_drop_fwd")
-                    saved.append((cur, cur_is_f32, z, mask))
-                    cur = z
-                cur_is_f32 = False
-            elif st.kind == "flatten":
-                saved.append(cur.shape)
-                cur = cur.reshape(B, -1)
-            elif st.kind == "dense":
-                ly = st.layer
-                w, b = self._wb(ly)
-                xin = cur.to(bf16) if cur.dtype != bf16 else cur
-                mask = torch.empty((B, ly.units), dtype=torch.uint8, device=cur.device) \
-                    if (st.drop > 0 or st.relu) else None
-                K = xin.shape[1]
-                split = self._split_k(B, ly.units, K)
-                if split > 1:
-                    # skinny GEMM with a long K (e.g. 128 x 128 x 9216): split K over ~48 CTAs of the
-                    # wgmma kernel; each K-slice stores its fp32 partial in its own slab and the epilogue sums the
-                    # slabs in slice order
-                    acc = self._splitk_acc(li, int(lib.tfy_gemm_bf16_splitk_slabs(K, split)), B, ly.units)
-                    z = torch.empty((B, ly.units), dtype=bf16, device=cur.device)
-                    tiles = ((B + 127) // 128) * ((ly.units + 127) // 128)
-                    co_resident = tiles * split <= torch.cuda.get_device_properties(cur.device).multi_processor_count
-                    if co_resident and os.environ.get("TFY_SPLITK_FUSE") == "1":
-                        # ONE launch (opt-in): the K-slice CTAs of a tile meet on a counter, then each applies bias +
-                        # ReLU + dropout to 1/split of the tile (summing the slabs in slice order) and writes the bf16
-                        # activations and the gate mask.  (The slices spin on each other: the grid must be co-resident.)
-                        # Off by default: the fence + counter + spin can cost more than the short second kernel of
-                        # the same CUDA graph it removes.
-                        key = ("splitk_cnt", li)
-                        if key not in self._acc32:
-                            self._acc32[key] = torch.zeros(2 * tiles, dtype=torch.int32, device=cur.device)
-                        self._chk(lib.tfy_gemm_bf16_splitk_fused(
-                            xin.data_ptr(), w.data_ptr(), acc.data_ptr(), self._acc32[key].data_ptr(), b.data_ptr(),
-                            z.data_ptr(), mask.data_ptr() if mask is not None else None, B, ly.units, K,
-                            xin.stride(0), w.stride(0), int(st.relu), float(st.drop), seed, self._hp, split, s),
-                            "gemm_bf16_splitk_fused")
-                    else:
-                        self._chk(lib.tfy_gemm_bf16(xin.data_ptr(), w.data_ptr(), None, acc.data_ptr(), None, B,
-                                                    ly.units, K, xin.stride(0), w.stride(0), ly.units, 0, split, s),
-                                  "gemm_bf16(split-K)")
-                        self._chk(lib.tfy_bias_act_drop_fwd_f32(acc.data_ptr(), b.data_ptr(), z.data_ptr(),
-                                                                mask.data_ptr() if mask is not None else None, B,
-                                                                ly.units, int(st.relu), float(st.drop), seed, self._hp,
-                                                                acc.shape[0], s), "bias_act_drop_fwd_f32")
-                else:
-                    self._warn_once(f"dense_fwd:{li}", f"Dense layer {li} ({K} -> {ly.units}, batch {B}) is outside the "
-                                    "split-K wgmma GEMM's envelope (long K, at most 8 output tiles): forward uses cuBLAS")
-                    z = torch.mm(xin, w.t())
-                    self._chk(lib.tfy_bias_act_drop_fwd(z.data_ptr(), b.data_ptr(), z.data_ptr(),
-                                                        mask.data_ptr() if mask is not None else None, B, ly.units,
-                                                        int(st.relu), float(st.drop), seed, self._hp, s),
-                              "bias_act_drop_fwd")
-                saved.append((xin, mask))
-                cur = z
-                cur_is_f32 = False
-            else:  # head
-                ly = st.layer
-                w, b = self._wb(ly)
-                xin = cur.to(bf16) if cur.dtype != bf16 else cur
-                prev = self.plan[li - 1] if li > 0 else None
-                K, C = xin.shape[1], ly.units
-                if (prev is not None and prev.kind == "dense" and K in (128, 256, 512) and C <= 16
-                        and xin.is_contiguous() and os.environ.get("TFY_NO_FUSED_HEAD") != "1"):
-                    # one launch: logits, loss, dlogits, dW2, db2 and the gradient entering the previous Dense
-                    # layer (its ReLU / dropout gate and bias gradient included)
-                    pmask = saved[li - 1][1]
-                    pscale = 1.0 / (1.0 - prev.drop) if prev.drop > 0 else 1.0
-                    _, pb = self._wb(prev.layer)
-                    need = int(lib.tfy_dense_head_scratch_elems(K, C, B))      # one slab per 16 rows of the batch
-                    if "head_scratch" not in self._acc32 or self._acc32["head_scratch"].numel() < need:
-                        self._acc32["head_scratch"] = torch.zeros(need, dtype=torch.float32, device=cur.device)
-                        self._acc32["head_counter"] = torch.zeros(1, dtype=torch.int32, device=cur.device)
-                    dh = torch.empty((B, K), dtype=bf16, device=cur.device)
-                    if self._wmode == (False, False):
-                        self._chk(lib.tfy_dense_head_fused(
-                            xin.data_ptr(), w.data_ptr(), b.data_ptr(), y.data_ptr(),
-                            pmask.data_ptr() if pmask is not None else None, pscale, self._loss.data_ptr(),
-                                self._host_loss_ptr(), self._stats_ptr(), w.grad.data_ptr(), b.grad.data_ptr(),
-                            dh.data_ptr(), pb.grad.data_ptr(), self._acc32["head_scratch"].data_ptr(),
-                            self._acc32["head_counter"].data_ptr(), B, K, C, s), "dense_head_fused")
-                    else:
-                        # Keras sample / class weights: each row's dlogits scaled by its weight inside the kernel
-                        self._chk(lib.tfy_dense_head_fused_weighted(
-                            xin.data_ptr(), w.data_ptr(), b.data_ptr(), y.data_ptr(),
-                            pmask.data_ptr() if pmask is not None else None, pscale, self._loss.data_ptr(),
-                            self._host_loss_ptr(), self._stats_ptr(), w.grad.data_ptr(), b.grad.data_ptr(),
-                            dh.data_ptr(), pb.grad.data_ptr(), self._acc32["head_scratch"].data_ptr(),
-                            self._acc32["head_counter"].data_ptr(), B, K, C, *self._weight_ptrs(sw)),
-                            "dense_head_fused_weighted")
-                    saved.append(("fused", dh))
-                    continue
-                self._warn_once(f"head:{li}", f"classifier head {li} ({xin.shape[1]} -> {ly.units}, batch {B}) is outside "
-                                "the fused head kernel's envelope (K in 128/256/512, at most 16 classes, Dense "
-                                "predecessor): logits and gradients use cuBLAS")
-                logits = torch.mm(xin, w.t())
-                C = ly.units
-                dlogits = torch.empty((B, C), dtype=bf16, device=cur.device)
-                if self._wmode == (False, False):
-                    self._chk(lib.tfy_softmax_xent(logits.data_ptr(), b.data_ptr(), y.data_ptr(), self._loss.data_ptr(),
-                                                   dlogits.data_ptr(), b.grad.data_ptr(), self._stats_ptr(), B, C, s),
-                              "softmax_xent")
-                else:
-                    sw_ptr, cw_ptr, _ = self._weight_ptrs(sw)
-                    self._chk(lib.tfy_softmax_xent_weighted(logits.data_ptr(), b.data_ptr(), y.data_ptr(), sw_ptr,
-                                                            cw_ptr, self._loss.data_ptr(), dlogits.data_ptr(),
-                                                            b.grad.data_ptr(), self._stats_ptr(), B, C, s),
-                              "softmax_xent_weighted")
-                saved.append((xin, dlogits))
-        # -------- backward
-        grad = None
-        pre_gated = False          # the dgrad kernel of the next layer already applied this layer's ReLU gate
-        dense_gated = False        # the fused head already produced the gated gradient + db of the Dense below
-        for li in range(len(self.plan) - 1, -1, -1):
-            st = self.plan[li]
-            sv = saved[li]
-            first = li == 0
-            if st.kind == "head" and sv[0] == "fused":
-                grad = sv[1]
-                dense_gated = True          # the Dense layer below already has its gated gradient and db
-            elif st.kind == "head":
-                xin, dlogits = sv
-                w, _ = self._wb(st.layer)
-                torch.mm(dlogits.t(), xin, out=w.grad)
-                grad = torch.mm(dlogits, w) if not first else None
-            elif st.kind == "dense":
-                xin, mask = sv
-                ly = st.layer
-                w, b = self._wb(ly)
-                scale = 1.0 / (1.0 - st.drop) if st.drop > 0 else 1.0
-                if dense_gated:
-                    dense_gated = False
-                else:
-                    self._chk(lib.tfy_act_drop_bwd_bias(grad.data_ptr(), mask.data_ptr() if mask is not None else None,
-                                                        None, grad.data_ptr(), scale, B, ly.units,
-                                                        self._partial.data_ptr(), b.grad.data_ptr(),
-                                                        self._counter.data_ptr(), s), "act_drop_bwd_bias")
-                I = xin.shape[1]
-                if (ly.units % 8 == 0 and I % 8 == 0 and grad.is_contiguous()
-                        and xin.is_contiguous() and w.is_contiguous() and w.grad.is_contiguous()
-                        and os.environ.get("TFY_NO_TC_DENSE_BWD") != "1"):
-                    # dW = dh^T x (straight into the flat gradient buffer) and dx = dh W in ONE wgmma kernel
-                    dx = torch.empty((B, I), dtype=bf16, device=grad.device) if not first else None
-                    self._chk(lib.tfy_dense_bwd(grad.data_ptr(), xin.data_ptr(), w.data_ptr(), w.grad.data_ptr(),
-                                                dx.data_ptr() if dx is not None else None, B, ly.units, I, s),
-                              "dense_bwd")
-                    grad = dx
-                else:
-                    self._warn_once(f"dense_bwd:{li}", f"Dense layer {li} ({I} -> {ly.units}, batch {B}) is outside "
-                                    "the wgmma dense-backward kernel's envelope: cuBLAS computes dW / dx")
-                    torch.mm(grad.t(), xin, out=w.grad)
-                    grad = torch.mm(grad, w) if not first else None
-            elif st.kind == "flatten":
-                if grad is not None:
-                    grad = grad.reshape(sv)
-            else:  # conv
-                xin, xin_f32, zout, aux = sv
-                ly = st.layer
-                w, b = self._wb(ly)
-                H, W, Cin = ly.input_shape_
-                O = ly.filters
-                OH, OW = H - 2, W - 2
-                scale = self._conv_drop_scale(st, st.pool and self._tc_conv(st, B))
-                gated, pre_gated = pre_gated, False
-                if (Cin == 1 and O == 32 and gated and not st.pool and aux is None and first
-                        and os.environ.get("TFY_NO_TC_CONV") != "1"):
-                    # first layer: dW and db in ONE tensor-core kernel (im2col built in shared memory)
-                    dz = grad if grad.is_contiguous() else grad.contiguous()
-                    self._chk(lib.tfy_conv3x3_c1_wgrad_tc(xin.data_ptr(), int(xin_f32), dz.data_ptr(),
-                                                          self._c1_acc.data_ptr(), self._c1_cnt.data_ptr(),
-                                                          w.grad.data_ptr(), b.grad.data_ptr(), B, H, W, s),
-                              "conv3x3_c1_wgrad_tc")
-                    grad = None
-                    continue
-                if (st.pool and self._tc_conv(st, B) and grad.is_contiguous()
-                        and os.environ.get("TFY_NO_UNPOOL_FUSION") != "1"):
-                    # pool/dropout/ReLU backward fused into the operand producers of wgrad and dgrad: the
-                    # 4x larger dz tensor is never written; db comes out of the wgrad kernel.  When the dgrad
-                    # launch follows, the wgrad CTAs only store their fp32 partials (no grid barrier) and the
-                    # dgrad kernel reduces them into dW / db behind its main loop: the same bits either way.
-                    if "wgrad_scratch" not in self._acc32:
-                        self._acc32["wgrad_scratch"] = torch.empty(
-                            int(lib.tfy_conv3x3_c32_wgrad_scratch_elems()), dtype=torch.float32, device=grad.device)
-                    part = self._acc32["wgrad_scratch"]
-                    ov = self._overlap_desc(li, B, H, W)
-                    ovp = ctypes.byref(ov) if ov is not None else None
-                    n_part = ctypes.c_int(0)
-                    if first:
-                        self._chk(lib.tfy_conv3x3_c32_wgrad_unpool_ov(
-                            xin.data_ptr(), grad.data_ptr(), aux.data_ptr(), scale, part.data_ptr(),
-                            w.grad.data_ptr(), b.grad.data_ptr(), self._conv_sync.data_ptr(), B, H, W, ovp, s),
-                            "conv3x3_c32_wgrad_unpool")
-                    else:
-                        self._chk(lib.tfy_conv3x3_c32_wgrad_unpool_deferred(
-                            xin.data_ptr(), grad.data_ptr(), aux.data_ptr(), scale, part.data_ptr(), B, H, W, ovp,
-                            ctypes.byref(n_part), s), "conv3x3_c32_wgrad_unpool_deferred")
-                    dp = grad
-                    grad = None
-                    if not first:
-                        prev = self.plan[li - 1]
-                        fold = (prev.kind == "conv" and prev.relu and not prev.pool and prev.drop == 0
-                                and saved[li - 1][2] is not None and saved[li - 1][2].data_ptr() == xin.data_ptr())
-                        grad = torch.empty((B, H, W, Cin), dtype=bf16, device=dp.device)
-                        self._chk(lib.tfy_conv3x3_c32_dgrad_unpool_reduce(
-                            dp.data_ptr(), aux.data_ptr(), scale, w.data_ptr(), xin.data_ptr() if fold else None,
-                            grad.data_ptr(), B, H, W, part.data_ptr(), n_part.value, w.grad.data_ptr(),
-                            b.grad.data_ptr(), s), "conv3x3_c32_dgrad_unpool_reduce")
-                        pre_gated = fold
-                    continue
-                if st.pool:
-                    dz = torch.empty((B, OH, OW, O), dtype=bf16, device=grad.device)
-                    self._chk(lib.tfy_pool_drop_relu_bwd(grad.data_ptr(), aux.data_ptr(), dz.data_ptr(), scale, B, OH,
-                                                         OW, O, self._partial.data_ptr(), b.grad.data_ptr(),
-                                                         self._counter.data_ptr(), s), "pool_drop_relu_bwd")
-                else:
-                    dz = grad if grad.is_contiguous() else grad.contiguous()
-                    use_mask = aux is not None
-                    self._chk(lib.tfy_act_drop_bwd_bias(dz.data_ptr(), aux.data_ptr() if use_mask else None,
-                                                        zout.data_ptr() if (st.relu and not use_mask
-                                                                            and not gated) else None,
-                                                        dz.data_ptr(), scale, B * OH * OW, O,
-                                                        self._partial.data_ptr(), b.grad.data_ptr(),
-                                                        self._counter.data_ptr(), s), "act_drop_bwd_bias")
-                if Cin == 1:
-                    self._chk(lib.tfy_conv3x3_c1_wgrad(xin.data_ptr(), int(xin_f32), dz.data_ptr(),
-                                                       self._partial.data_ptr(), w.grad.data_ptr(),
-                                                       self._counter.data_ptr(), B, H, W, O, s), "conv3x3_c1_wgrad")
-                    grad = None
-                    if not first:
+                st.scale = self._conv_drop_scale(st, st.tc)
+                if st.tc:
+                    st.bwd = "unpool" if unpool_fusion else "tc"
+                elif Cin == 1:
+                    if not st.first:
                         raise RuntimeError("C_in=1 convolution must be the first layer")
-                elif self._tc_conv(st, B):
-                    if "wgrad_scratch" not in self._acc32:       # per-CTA fp32 partial tiles (L2 resident)
-                        self._acc32["wgrad_scratch"] = torch.empty(
-                            int(lib.tfy_conv3x3_c32_wgrad_scratch_elems()), dtype=torch.float32, device=dz.device)
-                    acc = self._acc32["wgrad_scratch"]
-                    self._chk(lib.tfy_conv3x3_c32_wgrad(xin.data_ptr(), dz.data_ptr(), acc.data_ptr(),
-                                                        w.grad.data_ptr(), self._conv_sync.data_ptr(), B, H, W, s),
-                              "conv3x3_c32_wgrad")
-                    grad = None
-                    if not first:
-                        prev = self.plan[li - 1]
-                        # fold the producer's ReLU gate into the dgrad epilogue when its output IS our input
-                        fold = (prev.kind == "conv" and prev.relu and not prev.pool and prev.drop == 0
-                                and saved[li - 1][2] is not None and saved[li - 1][2].data_ptr() == xin.data_ptr())
-                        grad = torch.empty((B, H, W, Cin), dtype=bf16, device=dz.device)
-                        self._chk(lib.tfy_conv3x3_c32_dgrad(dz.data_ptr(), w.data_ptr(),
-                                                            xin.data_ptr() if fold else None, grad.data_ptr(), B, H,
-                                                            W, s), "conv3x3_c32_dgrad")
-                        pre_gated = fold
-                    continue
+                    st.bwd = "c1"
                 else:
-                    xb = xin.to(bf16) if xin.dtype != bf16 else xin
-                    dx, dw, _ = torch.ops.aten.convolution_backward(
-                        dz.permute(0, 3, 1, 2), xb.permute(0, 3, 1, 2), w, None, [1, 1], [0, 0], [1, 1], False,
-                        [0, 0], 1, [not first, True, False])
-                    w.grad.copy_(dw)
-                    grad = None
-                    if not first:
-                        g = dx.permute(0, 2, 3, 1)
-                        grad = g if g.is_contiguous() else g.contiguous()
-        if self._ov_used:
+                    st.bwd = "cudnn"
+                # the tensor-core data gradient applies the producer's ReLU gate when its output IS our input
+                st.fold = (st.tc and prev is not None and prev.kind == "conv" and prev.relu and not prev.pool
+                           and prev.drop == 0)
+                if st.fold:
+                    prev.gated = True
+                    if prev.first and prev.fwd == "c1_tc":
+                        prev.bwd = "c1_tc"      # first layer: dW and db in ONE tensor-core kernel
+                if st.tc:                       # per-CTA fp32 partial tiles (L2 resident)
+                    self._scratch("wgrad_scratch", int(lib.tfy_conv3x3_c32_wgrad_scratch_elems()))
+                st.overlap = None
+            elif st.kind == "dense":
+                ly = st.layer
+                K, N = ly.input_shape_[-1], ly.units
+                w, _ = self._wb(ly)
+                st.scale = 1.0 / (1.0 - st.drop) if st.drop > 0 else 1.0
+                st.split = self._split_k(B, N, K, splitk_tiles)
+                tiles = ((B + 127) // 128) * ((N + 127) // 128)
+                co_resident = tiles * st.split <= torch.cuda.get_device_properties(self.device).multi_processor_count
+                st.splitk_fused = st.split > 1 and co_resident and splitk_fuse
+                if st.split > 1:
+                    st.slabs = int(lib.tfy_gemm_bf16_splitk_slabs(K, st.split))
+                    self._scratch(li, st.slabs * B * N)
+                    if st.splitk_fused:
+                        self._scratch(("splitk_cnt", li), 2 * tiles, torch.int32)
+                else:
+                    self._warn_once(f"dense_fwd:{li}", f"Dense layer {li} ({K} -> {N}, batch {B}) is outside the "
+                                    "split-K wgmma GEMM's envelope (long K, at most 8 output tiles): forward uses cuBLAS")
+                st.tc_bwd = N % 8 == 0 and K % 8 == 0 and w.is_contiguous() and w.grad.is_contiguous() and tc_dense_bwd
+                if not st.tc_bwd:
+                    self._warn_once(f"dense_bwd:{li}", f"Dense layer {li} ({K} -> {N}, batch {B}) is outside "
+                                    "the wgmma dense-backward kernel's envelope: cuBLAS computes dW / dx")
+                st.head_gated = False   # the fused head produces this layer's gated gradient and db
+            elif st.kind == "head":
+                ly = st.layer
+                K, C = ly.input_shape_[-1], ly.units
+                st.fused = (prev is not None and prev.kind == "dense" and K in (128, 256, 512) and C <= 16
+                            and fused_head)
+                if st.fused:
+                    prev.head_gated = True
+                    self._scratch("head_scratch", int(lib.tfy_dense_head_scratch_elems(K, C, B)))   # a slab per 16 rows
+                    self._scratch("head_counter", 1, torch.int32)
+                else:
+                    self._warn_once(f"head:{li}", f"classifier head {li} ({K} -> {C}, batch {B}) is outside "
+                                    "the fused head kernel's envelope (K in 128/256/512, at most 16 classes, Dense "
+                                    "predecessor): logits and gradients use cuBLAS")
+        self._ov_gmid = 0
+        if self._overlap:               # the last un-pool-fused weight gradient the descriptor fits
+            for st in reversed(plan):
+                if st.kind == "conv" and st.bwd == "unpool":
+                    H, W, _ = st.layer.input_shape_
+                    st.overlap = self._overlap_desc(st.li, B, H, W, overlap_groups)
+                    if st.overlap is not None:
+                        break
+        self._resolved_b = B
+
+    # ------------------------------------------------------------------ the step
+    @torch.no_grad()
+    def _forward_backward(self, x, y, sw=None) -> None:
+        if x.shape[0] != self._resolved_b:
+            self._resolve(x.shape[0])
+        self._k = 0
+        saved = []
+        cur = x                    # NHWC for images, [B, F] for vectors
+        for st in self.plan:
+            sv = types.SimpleNamespace()
+            if st.kind == "head":
+                self._head_fwd(st, sv, cur, saved[-1] if saved else None, y, sw)
+            else:
+                cur = getattr(self, f"_{st.kind}_fwd")(st, sv, cur)
+            saved.append(sv)
+        grad = None
+        for st, sv in zip(reversed(self.plan), reversed(saved)):
+            grad = getattr(self, f"_{st.kind}_bwd")(st, sv, grad)
+        if self._ov_gmid:
             # the communication CTAs of the weight-gradient kernel already handled groups [g_mid, end) of every shard
             self.fused.step(shard_groups=(0, self._ov_gmid), advance=True)
-            self._ov_used = False
         else:
             self.fused.step()
         self._launches_per_step = self._k + 1     # our kernels launched per step (library GEMMs excluded)
+
+    def _conv_fwd(self, st, sv, x):
+        lib, s, bf16 = self.lib, self._s(), torch.bfloat16
+        w, b = self._wb(st.layer)
+        B = x.shape[0]
+        H, W, Cin = st.layer.input_shape_
+        O, OH, OW = st.layer.filters, H - 2, W - 2
+        sv.x = self._bf16(x) if st.fwd == "c32_pool_tc" else x
+        if st.fwd == "c32_pool_tc":
+            # wgmma implicit GEMM; bias + ReLU + 2x2 max-pool + dropout in the epilogue
+            p = torch.empty((B, OH // 2, OW // 2, O), dtype=bf16, device=x.device)
+            sv.code = torch.empty((B, OH // 2, OW // 2, O), dtype=torch.uint8, device=x.device)
+            self._chk(lib.tfy_conv3x3_c32_pool_fwd(sv.x.data_ptr(), w.data_ptr(), b.data_ptr(), p.data_ptr(),
+                                                   sv.code.data_ptr(), B, H, W, float(st.drop), st.seed, self._hp, s),
+                      "conv3x3_c32_pool_fwd")
+            return p
+        if st.fwd == "cudnn":
+            z = F.conv2d(self._bf16(x).permute(0, 3, 1, 2), w).permute(0, 2, 3, 1).contiguous()   # NCHW over NHWC
+        else:
+            # direct kernel: conv + bias + relu in one launch
+            z = torch.empty((B, OH, OW, O), dtype=bf16, device=x.device)
+            if st.fwd == "c1_tc":
+                self._chk(lib.tfy_conv3x3_c1_fwd_tc(x.data_ptr(), int(x.dtype == torch.float32), w.data_ptr(),
+                                                    b.data_ptr(), z.data_ptr(), B, H, W, s), "conv3x3_c1_fwd_tc")
+            else:
+                self._chk(lib.tfy_conv3x3_c1_fwd(x.data_ptr(), int(x.dtype == torch.float32), w.data_ptr(),
+                                                 b.data_ptr(), z.data_ptr(), B, H, W, O, s), "conv3x3_c1_fwd")
+        if st.pool:
+            p = torch.empty((B, OH // 2, OW // 2, O), dtype=bf16, device=x.device)
+            sv.code = torch.empty((B, OH // 2, OW // 2, O), dtype=torch.uint8, device=x.device)
+            self._chk(lib.tfy_bias_relu_pool_drop_fwd(z.data_ptr(), b.data_ptr(), p.data_ptr(), sv.code.data_ptr(),
+                                                      B, OH, OW, O, float(st.drop), st.seed, self._hp, s),
+                      "bias_relu_pool_drop_fwd")
+            return p
+        sv.z = z
+        sv.mask = torch.empty((B, OH, OW, O), dtype=torch.uint8, device=x.device) if st.drop > 0 else None
+        if st.fwd == "cudnn" or sv.mask is not None:     # (the direct kernels applied bias + ReLU already)
+            self._chk(lib.tfy_bias_act_drop_fwd(z.data_ptr(), b.data_ptr() if st.fwd == "cudnn" else None, z.data_ptr(),
+                                                sv.mask.data_ptr() if sv.mask is not None else None, B * OH * OW, O,
+                                                int(st.relu), float(st.drop), st.seed, self._hp, s), "bias_act_drop_fwd")
+        return z
+
+    def _conv_bwd(self, st, sv, grad):
+        lib, s = self.lib, self._s()
+        w, b = self._wb(st.layer)
+        B = grad.shape[0]
+        H, W, Cin = st.layer.input_shape_
+        O, OH, OW = st.layer.filters, H - 2, W - 2
+        x_f32 = int(sv.x.dtype == torch.float32)
+        gate = sv.x.data_ptr() if st.fold else None      # the producer's ReLU gate, applied by the tensor-core dgrad
+        if st.bwd == "c1_tc":
+            self._chk(lib.tfy_conv3x3_c1_wgrad_tc(sv.x.data_ptr(), x_f32, grad.data_ptr(), self._c1_acc.data_ptr(),
+                                                  self._c1_cnt.data_ptr(), w.grad.data_ptr(), b.grad.data_ptr(), B, H,
+                                                  W, s), "conv3x3_c1_wgrad_tc")
+            return None
+        if st.bwd == "unpool":
+            # pool/dropout/ReLU backward fused into the operand producers of wgrad and dgrad: the 4x larger dz tensor
+            # is never written; db comes out of the wgrad kernel.  When the dgrad launch follows, the wgrad CTAs only
+            # store their fp32 partials (no grid barrier) and the dgrad kernel reduces them into dW / db behind its
+            # main loop: the same bits either way.
+            part = self._acc32["wgrad_scratch"]
+            ovp = ctypes.byref(st.overlap) if st.overlap is not None else None
+            if st.first:
+                self._chk(lib.tfy_conv3x3_c32_wgrad_unpool_ov(
+                    sv.x.data_ptr(), grad.data_ptr(), sv.code.data_ptr(), st.scale, part.data_ptr(), w.grad.data_ptr(),
+                    b.grad.data_ptr(), self._conv_sync.data_ptr(), B, H, W, ovp, s), "conv3x3_c32_wgrad_unpool")
+                return None
+            n_part = ctypes.c_int(0)
+            dx = torch.empty((B, H, W, Cin), dtype=torch.bfloat16, device=grad.device)
+            self._chk(lib.tfy_conv3x3_c32_wgrad_unpool_deferred(
+                sv.x.data_ptr(), grad.data_ptr(), sv.code.data_ptr(), st.scale, part.data_ptr(), B, H, W, ovp,
+                ctypes.byref(n_part), s), "conv3x3_c32_wgrad_unpool_deferred")
+            self._chk(lib.tfy_conv3x3_c32_dgrad_unpool_reduce(
+                grad.data_ptr(), sv.code.data_ptr(), st.scale, w.data_ptr(), gate, dx.data_ptr(), B, H, W,
+                part.data_ptr(), n_part.value, w.grad.data_ptr(), b.grad.data_ptr(), s),
+                "conv3x3_c32_dgrad_unpool_reduce")
+            return dx
+        if st.pool:
+            dz = torch.empty((B, OH, OW, O), dtype=torch.bfloat16, device=grad.device)
+            self._chk(lib.tfy_pool_drop_relu_bwd(grad.data_ptr(), sv.code.data_ptr(), dz.data_ptr(), st.scale, B, OH,
+                                                 OW, O, self._partial.data_ptr(), b.grad.data_ptr(),
+                                                 self._counter.data_ptr(), s), "pool_drop_relu_bwd")
+        else:
+            dz = grad
+            relu_gate = sv.z.data_ptr() if (st.relu and sv.mask is None and not st.gated) else None
+            self._chk(lib.tfy_act_drop_bwd_bias(dz.data_ptr(), sv.mask.data_ptr() if sv.mask is not None else None,
+                                                relu_gate, dz.data_ptr(), st.scale, B * OH * OW, O,
+                                                self._partial.data_ptr(), b.grad.data_ptr(), self._counter.data_ptr(),
+                                                s), "act_drop_bwd_bias")
+        if st.bwd == "c1":
+            self._chk(lib.tfy_conv3x3_c1_wgrad(sv.x.data_ptr(), x_f32, dz.data_ptr(), self._partial.data_ptr(),
+                                               w.grad.data_ptr(), self._counter.data_ptr(), B, H, W, O, s),
+                      "conv3x3_c1_wgrad")
+            return None
+        if st.bwd == "tc":
+            self._chk(lib.tfy_conv3x3_c32_wgrad(sv.x.data_ptr(), dz.data_ptr(), self._acc32["wgrad_scratch"].data_ptr(),
+                                                w.grad.data_ptr(), self._conv_sync.data_ptr(), B, H, W, s),
+                      "conv3x3_c32_wgrad")
+            if st.first:
+                return None
+            dx = torch.empty((B, H, W, Cin), dtype=torch.bfloat16, device=grad.device)
+            self._chk(lib.tfy_conv3x3_c32_dgrad(dz.data_ptr(), w.data_ptr(), gate, dx.data_ptr(), B, H, W, s),
+                      "conv3x3_c32_dgrad")
+            return dx
+        gx, dw, _ = torch.ops.aten.convolution_backward(
+            dz.permute(0, 3, 1, 2), self._bf16(sv.x).permute(0, 3, 1, 2), w, None, [1, 1], [0, 0], [1, 1], False,
+            [0, 0], 1, [not st.first, True, False])
+        w.grad.copy_(dw)
+        return None if st.first else gx.permute(0, 2, 3, 1).contiguous()
+
+    def _flatten_fwd(self, st, sv, x):
+        sv.shape = x.shape
+        return x.reshape(x.shape[0], -1)
+
+    def _flatten_bwd(self, st, sv, grad):
+        return grad.reshape(sv.shape) if grad is not None else None
+
+    def _dense_fwd(self, st, sv, x):
+        lib, s, ly = self.lib, self._s(), st.layer
+        w, b = self._wb(ly)
+        sv.x = xin = self._bf16(x)
+        (B, K), N = xin.shape, ly.units
+        sv.mask = torch.empty((B, N), dtype=torch.uint8, device=x.device) if (st.drop > 0 or st.relu) else None
+        mask = sv.mask.data_ptr() if sv.mask is not None else None
+        if st.split == 1:
+            z = torch.mm(xin, w.t())
+            self._chk(lib.tfy_bias_act_drop_fwd(z.data_ptr(), b.data_ptr(), z.data_ptr(), mask, B, N, int(st.relu),
+                                                float(st.drop), st.seed, self._hp, s), "bias_act_drop_fwd")
+            return z
+        # skinny GEMM with a long K (e.g. 128 x 128 x 9216): split K over ~48 CTAs of the wgmma kernel; each K-slice
+        # stores its fp32 partial in its own slab and the epilogue sums the slabs in slice order
+        acc = self._acc32[st.li]
+        z = torch.empty((B, N), dtype=torch.bfloat16, device=x.device)
+        if st.splitk_fused:
+            # ONE launch (opt-in): the K-slice CTAs of a tile meet on a counter, then each applies bias + ReLU +
+            # dropout to 1/split of the tile (summing the slabs in slice order) and writes the bf16 activations and
+            # the gate mask.  (The slices spin on each other: the grid must be co-resident.)  Off by default: the
+            # fence + counter + spin can cost more than the short second kernel of the same CUDA graph it removes.
+            self._chk(lib.tfy_gemm_bf16_splitk_fused(
+                xin.data_ptr(), w.data_ptr(), acc.data_ptr(), self._acc32[("splitk_cnt", st.li)].data_ptr(),
+                b.data_ptr(), z.data_ptr(), mask, B, N, K, xin.stride(0), w.stride(0), int(st.relu), float(st.drop),
+                st.seed, self._hp, st.split, s), "gemm_bf16_splitk_fused")
+        else:
+            self._chk(lib.tfy_gemm_bf16(xin.data_ptr(), w.data_ptr(), None, acc.data_ptr(), None, B, N, K,
+                                        xin.stride(0), w.stride(0), N, 0, st.split, s), "gemm_bf16(split-K)")
+            self._chk(lib.tfy_bias_act_drop_fwd_f32(acc.data_ptr(), b.data_ptr(), z.data_ptr(), mask, B, N,
+                                                    int(st.relu), float(st.drop), st.seed, self._hp, st.slabs, s),
+                      "bias_act_drop_fwd_f32")
+        return z
+
+    def _dense_bwd(self, st, sv, grad):
+        lib, s = self.lib, self._s()
+        w, b = self._wb(st.layer)
+        (B, I), N = sv.x.shape, st.layer.units
+        if not st.head_gated:
+            self._chk(lib.tfy_act_drop_bwd_bias(grad.data_ptr(), sv.mask.data_ptr() if sv.mask is not None else None,
+                                                None, grad.data_ptr(), st.scale, B, N, self._partial.data_ptr(),
+                                                b.grad.data_ptr(), self._counter.data_ptr(), s), "act_drop_bwd_bias")
+        if not st.tc_bwd:
+            torch.mm(grad.t(), sv.x, out=w.grad)
+            return None if st.first else torch.mm(grad, w)
+        # dW = dh^T x (straight into the flat gradient buffer) and dx = dh W in ONE wgmma kernel
+        dx = None if st.first else torch.empty((B, I), dtype=torch.bfloat16, device=grad.device)
+        self._chk(lib.tfy_dense_bwd(grad.data_ptr(), sv.x.data_ptr(), w.data_ptr(), w.grad.data_ptr(),
+                                    dx.data_ptr() if dx is not None else None, B, N, I, s), "dense_bwd")
+        return dx
+
+    def _head_fwd(self, st, sv, x, below, y, sw):
+        lib, s = self.lib, self._s()
+        w, b = self._wb(st.layer)
+        xin = self._bf16(x)
+        (B, K), C = xin.shape, st.layer.units
+        if st.fused:
+            # one launch: logits, loss, dlogits, dW2, db2 and the gradient entering the previous Dense layer (its
+            # ReLU / dropout gate and bias gradient included)
+            prev = self.plan[st.li - 1]
+            _, pb = self._wb(prev.layer)
+            sv.dh = torch.empty((B, K), dtype=torch.bfloat16, device=x.device)
+            args = (xin.data_ptr(), w.data_ptr(), b.data_ptr(), y.data_ptr(),
+                    below.mask.data_ptr() if below.mask is not None else None, prev.scale, self._loss.data_ptr(),
+                    self._host_loss_ptr(), self._stats_ptr(), w.grad.data_ptr(), b.grad.data_ptr(), sv.dh.data_ptr(),
+                    pb.grad.data_ptr(), self._acc32["head_scratch"].data_ptr(), self._acc32["head_counter"].data_ptr(),
+                    B, K, C)
+            if self._wmode == (False, False):
+                self._chk(lib.tfy_dense_head_fused(*args, s), "dense_head_fused")
+            else:
+                # Keras sample / class weights: each row's dlogits scaled by its weight inside the kernel
+                self._chk(lib.tfy_dense_head_fused_weighted(*args, *self._weight_ptrs(sw)), "dense_head_fused_weighted")
+            return
+        logits = torch.mm(xin, w.t())
+        sv.x, sv.dlogits = xin, torch.empty((B, C), dtype=torch.bfloat16, device=x.device)
+        if self._wmode == (False, False):
+            self._chk(lib.tfy_softmax_xent(logits.data_ptr(), b.data_ptr(), y.data_ptr(), self._loss.data_ptr(),
+                                           sv.dlogits.data_ptr(), b.grad.data_ptr(), self._stats_ptr(), B, C, s),
+                      "softmax_xent")
+        else:
+            sw_ptr, cw_ptr, _ = self._weight_ptrs(sw)
+            self._chk(lib.tfy_softmax_xent_weighted(logits.data_ptr(), b.data_ptr(), y.data_ptr(), sw_ptr, cw_ptr,
+                                                    self._loss.data_ptr(), sv.dlogits.data_ptr(), b.grad.data_ptr(),
+                                                    self._stats_ptr(), B, C, s), "softmax_xent_weighted")
+
+    def _head_bwd(self, st, sv, grad):
+        if st.fused:
+            return sv.dh          # the fused head already produced the Dense layer's gated gradient and db
+        w, _ = self._wb(st.layer)
+        torch.mm(sv.dlogits.t(), sv.x, out=w.grad)
+        return None if st.first else torch.mm(sv.dlogits, w)
