@@ -29,6 +29,7 @@ from tf_yarn_b200 import keras  # noqa: E402
 from tf_yarn_b200.estimator import canned, ps, ps_hbm  # noqa: E402
 from tf_yarn_b200.estimator import feature_column as fc  # noqa: E402
 from tf_yarn_b200.models import wide_deep as wdm  # noqa: E402
+from tf_yarn_b200.ops import features as feature_ids  # noqa: E402
 from tf_yarn_b200.ops import native  # noqa: E402
 
 B, V, N_CAT, N_NUM, HIDDEN = 512, 100_000, 26, 13, [1024, 512, 256]
@@ -90,13 +91,8 @@ def main(out_dir):
 
     # ---- id preparation alone
     cat_cols = [fc._categorical(c) for c in wide if fc._categorical(c) is not None]
-    net0 = canned._WideDeepNet(wide, [], [], 1)
-    named0 = ps._named_trainables(net0)
-    lay0 = ps.make_layout(named0, 1, keras.optimizers.Ftrl(0.05))
-    fake = types.SimpleNamespace(layout=lay0, lib=lib, device=torch.device("cuda"), var_opt=[native.OPT_FTRL] * 99,
-                                 master_ptr=lambda i, s=0: 0, account=lambda **k: None)
-    group = ps_hbm._TableGroup(fake, list(range(len(cat_cols))), cat_cols)
-    kernel_ids = group.feature_ids(feats, lib)
+    builder = feature_ids.FeatureIds(cat_cols, torch.device("cuda"))
+    kernel_ids = builder(feats, lib)
     torch_ids = torch.stack([torch.nn.functional.pad(i, (0, kernel_ids.shape[2] - i.shape[1]), value=-1)
                              for i in (fc._ids_and_weights(c, feats)[0] for c in cat_cols)])
     torch.cuda.synchronize()
@@ -104,13 +100,13 @@ def main(out_dir):
     T, _, L = kernel_ids.shape
     src_bytes = sum(v.numel() * v.element_size() for k, v in feats.items())
     out_bytes = T * B * L * 8
-    ids = {"T": T, "L_max": L, "launches": group.feature_ids.launches,
-           "kernel_us": _time(lambda: group.feature_ids(feats, lib), 2000),
+    ids = {"T": T, "L_max": L, "launches": builder.launches,
+           "kernel_us": _time(lambda: builder(feats, lib), 2000),
            "torch_us": _time(lambda: [fc._ids_and_weights(c, feats) for c in cat_cols], 200),
            "bytes": src_bytes + out_bytes, "hbm_floor_us": (src_bytes + out_bytes) / HBM_BYTES_PER_S * 1e6}
     with torch.profiler.profile(activities=[torch.profiler.ProfilerActivity.CUDA]) as prof:
         for _ in range(20):
-            group.feature_ids(feats, lib)
+            builder(feats, lib)
         torch.cuda.synchronize()
     dev_us = [e.device_time_total for e in prof.events()
               if e.device_type == torch.autograd.DeviceType.CUDA and "tfy_feature_ids" in e.name]

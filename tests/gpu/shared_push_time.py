@@ -72,13 +72,13 @@ def _deep_push(net, conn, feats):
     by_param = {id(p): i for i, p in enumerate(conn.params)}
     emb = [c for c in df.columns if isinstance(c, (fc.EmbeddingColumn, fc.SharedEmbeddingColumn))]
     idx = [by_param[id(df.embeddings[fc._embedding_key(c)].weight)] for c in emb]
-    group = ps_hbm._TableGroup(conn, idx, [c.categorical_column for c in emb])
+    group = ps_hbm._TableGroup(conn, idx, [c.categorical_column for c in emb], 64, 64)
     ids = group.ids_of(feats)
     Kp = conn.shadow_ld(by_param[id(lin.weight)])
     dx = (torch.randn(B, Kp, device="cuda") * 1e-3).to(torch.bfloat16)
 
     def push():
-        group.push(ids, dx, 64, Kp, 64)
+        group.push(ids, dx, dout_ld=Kp)
     out = {"entry_point": "tfy_ps_multi_push_rows_shared" if group.shared else "tfy_ps_multi_push_rows",
            "tables": len(group.distinct), "max_members": group.max_members if group.shared else 1,
            "events_us_per_push": _time(push, 2000)}

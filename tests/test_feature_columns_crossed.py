@@ -15,6 +15,7 @@ import torch
 
 import crossed_reference as ref
 import multihot_reference as mh
+from hbm_fake import hbm_connection
 from tf_yarn_b200 import TaskSpec, data, keras
 from tf_yarn_b200 import estimator as est
 from tf_yarn_b200.ops import features as feature_ids
@@ -295,35 +296,13 @@ def test_a_bucketized_feature_wider_than_its_column_never_leaves_the_column(host
 
 
 # ---------------------------------------------------------------------------------------------- HBM routing
-def _hbm_connection(network, n_ps=2):
-    """An HbmConnection over fake base addresses (no GPU): enough for the structural decisions it takes."""
-    from tf_yarn_b200.estimator import ps, ps_hbm
-    named = ps._named_trainables(network)
-    layout = ps.make_layout(named, n_ps, keras.optimizers.Ftrl(0.05))
-    conn = ps_hbm.HbmConnection.__new__(ps_hbm.HbmConnection)
-    conn.layout, conn.names = layout, [n for n, _ in named]
-    conn.lib = None
-    conn.var_opt = [ps_hbm.OPT_CODES[k] for k in layout.kinds]
-    conn.ps_base = [1 << 40, 2 << 40][:n_ps]
-    conn.device = torch.device("cpu")
-    params = dict(network.named_parameters())
-    conn.params = [params[n] for n in conn.names]
-    conn.sparse, conn.gemm = {}, {}
-    conn._classify(network)
-    conn.dense_idx = [i for i in range(len(conn.names)) if i not in conn.sparse]
-    conn.pull_idx = [i for i in conn.dense_idx if i not in conn.gemm]
-    conn.adam_scale = torch.ones(2)
-    conn._acct = {"pull_bytes": 0, "push_bytes": 0, "launches_per_step": 0}
-    return conn
-
-
 def test_hbm_wide_tower_with_crosses_of_mixed_v_is_fused_and_padded():
     from tf_yarn_b200.estimator import canned, ps_hbm
     cols = _columns()
     hashed = [fc.categorical_column_with_hash_bucket("edu", 1000), fc.categorical_column_with_identity("occ", 7)]
     wide = hashed + [cols["bucketized"], cols["raw_x_identity"], cols["raw_x_bucketized"]]
     net = canned._WideDeepNet(wide, [], [], 1)
-    conn = _hbm_connection(net)
+    conn = hbm_connection(net, "ftrl")
     assert ps_hbm._try_fuse_wide_tower(conn, net) is True
     f = _special_batch(B=9)
     idx = [conn.names.index(f"linear.tables.{c.key}.weight") for c in wide]
@@ -347,7 +326,7 @@ def test_hbm_wide_tower_with_crosses_of_mixed_v_is_fused_and_padded():
     # one id per example (k = 1 bucketized, crosses of one-hot keys): the one-id kernels' [T, B] ids
     one = [cols["bucketized_k1"], fc.crossed_column(["one", fc.categorical_column_with_identity("occ", 7)], 100),
            hashed[0]]
-    g1 = ps_hbm._TableGroup(_hbm_connection(canned._WideDeepNet(one, [], [], 1)), [0, 1, 2], one)
+    g1 = ps_hbm._TableGroup(hbm_connection(canned._WideDeepNet(one, [], [], 1), "ftrl"), [0, 1, 2], one)
     f1 = dict(f, occ=f["occ"][:, :1], edu=f["edu"][:, :1])
     assert g1.one_hot(f1) and g1.ids_of(f1).shape == (3, 9)
     assert torch.equal(g1.ids_of(f1)[1], _ids(one[1], f1)[:, 0])
@@ -357,7 +336,7 @@ def test_hbm_wide_tower_of_mixed_v_without_new_columns_is_still_refused():
     from tf_yarn_b200.estimator import canned, ps_hbm
     wide = [fc.categorical_column_with_hash_bucket("a", 1000), fc.categorical_column_with_hash_bucket("b", 500)]
     net = canned._WideDeepNet(wide, [], [], 1)
-    conn = _hbm_connection(net)
+    conn = hbm_connection(net, "ftrl")
     assert ps_hbm._try_fuse_wide_tower(conn, net) is False
     group = ps_hbm._TableGroup(conn, [0, 1], wide)
     assert not group.derived and group.feature_ids is None and group.V == 1000 and not group.same_v
@@ -371,7 +350,7 @@ def test_hbm_deep_tower_with_new_columns():
     x = fc.crossed_column(["edu", "one"], 18)
     net = canned._WideDeepNet([], [fc.embedding_column(b, 64), fc.embedding_column(x, 64), fc.numeric_column("one")],
                               [64], 1)
-    conn = _hbm_connection(net)
+    conn = hbm_connection(net, "ftrl")
     assert ps_hbm._try_fuse_first_layer(conn, net) is True
     f = _special_batch(B=9)
     d = net.dense_features(f)
@@ -379,7 +358,7 @@ def test_hbm_deep_tower_with_new_columns():
     assert torch.equal(d.ids[0], _ids(b, f)) and torch.equal(d.ids[1, :, :2], _ids(x, f))
     for extra in (b, fc.indicator_column(x)):
         net = canned._WideDeepNet([], [fc.embedding_column(x, 64), extra], [64], 1)
-        assert ps_hbm._try_fuse_first_layer(_hbm_connection(net), net) is False
+        assert ps_hbm._try_fuse_first_layer(hbm_connection(net, "ftrl"), net) is False
 
 
 # ---------------------------------------------------------------------------------------------- training

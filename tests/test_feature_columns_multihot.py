@@ -10,6 +10,7 @@ import pytest
 import torch
 
 import multihot_reference as mh
+from hbm_fake import hbm_connection
 from tf_yarn_b200 import TaskSpec, data, keras
 from tf_yarn_b200 import estimator as est
 
@@ -279,29 +280,6 @@ def test_shared_memory_parameter_server_trains_the_weighted_multihot_task(tmp_pa
 
 
 # ---------------------------------------------------------------------------------------------- HBM routing
-def _hbm_connection(network, opt="adagrad", n_ps=2):
-    """An HbmConnection over fake base addresses (no GPU): enough for the structural decisions it takes."""
-    from tf_yarn_b200.estimator import ps, ps_hbm
-    named = ps._named_trainables(network)
-    desc = {"adagrad": keras.optimizers.Adagrad(0.05), "sgd": keras.optimizers.SGD(0.1)}[opt]
-    layout = ps.make_layout(named, n_ps, desc)
-    conn = ps_hbm.HbmConnection.__new__(ps_hbm.HbmConnection)
-    conn.layout, conn.names = layout, [n for n, _ in named]
-    conn.lib = None
-    conn.var_opt = [ps_hbm.OPT_CODES[k] for k in layout.kinds]
-    conn.ps_base = [1 << 40, 2 << 40][:n_ps] + [3 << 40] * max(0, n_ps - 2)
-    conn.device = torch.device("cpu")
-    params = dict(network.named_parameters())
-    conn.params = [params[n] for n in conn.names]
-    conn.sparse, conn.gemm = {}, {}
-    conn._classify(network)
-    conn.dense_idx = [i for i in range(len(conn.names)) if i not in conn.sparse]
-    conn.pull_idx = [i for i in conn.dense_idx if i not in conn.gemm]
-    conn.adam_scale = torch.ones(2)
-    conn._acct = {"pull_bytes": 0, "push_bytes": 0, "launches_per_step": 0}
-    return conn
-
-
 def test_hbm_plane_routes_one_hot_to_k5_and_multihot_or_weighted_to_the_weighted_bag():
     from tf_yarn_b200.estimator import canned, ps_hbm
     V = 1000
@@ -316,7 +294,7 @@ def test_hbm_plane_routes_one_hot_to_k5_and_multihot_or_weighted_to_the_weighted
     for columns, combiner in ((cats, "sqrtn"), (wcats, "mean")):
         net = canned._WideDeepNet(columns, [fc.embedding_column(c, 64, combiner) for c in columns] + [num], [256, 64],
                                   1, sparse_combiner="sum")
-        conn = _hbm_connection(net)
+        conn = hbm_connection(net)
         assert ps_hbm._try_fuse_first_layer(conn, net) is True
         assert ps_hbm._try_fuse_wide_tower(conn, net) is True
         weighted = columns is wcats
@@ -340,10 +318,10 @@ def test_hbm_plane_routes_one_hot_to_k5_and_multihot_or_weighted_to_the_weighted
             assert torch.equal(d.ids.reshape(3, B, -1)[:, :, 0][ok], want[ok])   # ids >= 0 mapped as before
     # the wide tower's one-id kernels serve a one-hot unweighted batch only under the sum combiner
     net = canned._WideDeepNet(cats, [], [], 1, sparse_combiner="mean")
-    assert ps_hbm._try_fuse_wide_tower(_hbm_connection(net), net) is True
-    group = ps_hbm._TableGroup(_hbm_connection(net), [0, 1, 2], cats)
+    assert ps_hbm._try_fuse_wide_tower(hbm_connection(net), net) is True
+    group = ps_hbm._TableGroup(hbm_connection(net), [0, 1, 2], cats)
     assert group.one_hot(one_hot) and not group.one_hot(multi)
-    assert not ps_hbm._TableGroup(_hbm_connection(net), [0, 1, 2], wcats).one_hot(one_hot)
+    assert not ps_hbm._TableGroup(hbm_connection(net), [0, 1, 2], wcats).one_hot(one_hot)
 
 
 @pytest.mark.parametrize("hashed", [False, True], ids=["identity", "hashed"])
@@ -355,7 +333,7 @@ def test_hbm_bucketing_matches_the_feature_columns_for_large_ids(hashed):
     V, B = 100_000, 64
     cats = [_col(f"c{i}", V, hashed, i == 1) for i in range(3)]
     net = canned._WideDeepNet(cats, [], [], 1)
-    group = ps_hbm._TableGroup(_hbm_connection(net), [0, 1, 2], cats)
+    group = ps_hbm._TableGroup(hbm_connection(net), [0, 1, 2], cats)
     g = torch.Generator().manual_seed(0)
     special = torch.tensor([0, 1, V - 1, V, 3_470_000_000, 3_600_000_000, 4_000_000_000, 2 ** 32 - 1, 2 ** 32,
                             2 ** 40 + 7, -1, -2, -V, -(2 ** 32), -(2 ** 40)])

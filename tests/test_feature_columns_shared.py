@@ -5,7 +5,7 @@ import pytest
 import torch
 
 import shared_embedding_reference as sref
-from test_feature_columns_crossed import _hbm_connection
+from hbm_fake import hbm_connection
 from tf_yarn_b200 import keras
 from tf_yarn_b200.estimator import feature_column as fc
 
@@ -122,7 +122,7 @@ def test_hbm_k5_takes_shared_columns_with_a_column_to_table_map():
     s2 = fc.shared_embedding_columns([cats[1], cats[3]], 64)
     net = _net([s1[0], s2[0], s1[1], s2[1], fc.embedding_column(fc.categorical_column_with_hash_bucket("e", 50), 64),
                 fc.numeric_column("n")])
-    conn = _hbm_connection(net)
+    conn = hbm_connection(net, "ftrl")
     assert ps_hbm._try_fuse_first_layer(conn, net) is True
     name = {c: conn.names.index(f"dense_features.embeddings.{c}.weight") for c in
             (s1[0].shared_name, s2[0].shared_name, "e")}
@@ -155,7 +155,7 @@ def test_hbm_thirteen_shared_pairs_push_with_the_block_sort():
     cats = [fc.categorical_column_with_hash_bucket(f"c{i}", 50) for i in range(26)]
     pairs = [fc.shared_embedding_columns([cats[i], cats[i + 13]], 64) for i in range(13)]
     net = _net([p[0] for p in pairs] + [p[1] for p in pairs])
-    conn = _hbm_connection(net)
+    conn = hbm_connection(net, "ftrl")
     assert ps_hbm._try_fuse_first_layer(conn, net) is True
     idx = [conn.names.index(f"dense_features.embeddings.{c.shared_name}.weight") for c in net.dense_features.columns]
     group = ps_hbm._TableGroup(conn, idx, [c.categorical_column for c in net.dense_features.columns])
@@ -163,20 +163,20 @@ def test_hbm_thirteen_shared_pairs_push_with_the_block_sort():
     assert ps_hbm.push_rows_launches(512, group.max_members) == 4
 
 
-def test_hbm_unfused_tower_serves_each_collection_with_one_bag_and_one_push(monkeypatch):
+def test_hbm_unfused_tower_serves_each_collection_with_one_bag_and_one_group_push(monkeypatch):
     """Without K5 (a 32-wide collection), each collection's members are looked up by one weighted bag (T = members,
     the table repeated, col_stride D) and pushed by one shared push; the lookup returns the members' slices."""
     from tf_yarn_b200.estimator import ps_hbm
     cats = [fc.categorical_column_with_identity(f"c{i}", 30) for i in range(3)]
     sh = fc.shared_embedding_columns(cats, 32, "sqrtn")
     net = _net([sh[2], fc.numeric_column("n"), sh[0], sh[1]])
-    conn = _hbm_connection(net)
+    conn = hbm_connection(net, "ftrl")
     assert ps_hbm._try_fuse_first_layer(conn, net) is False
     bags, pushes = [], []
-    monkeypatch.setattr(ps_hbm, "weighted_bag", lambda lib, tables, ids, weights, code, D, V, out, out_ld, cs, f:
+    monkeypatch.setattr(ps_hbm, "weighted_bag", lambda lib, tables, ids, weights, code, D, V, out, out_ld, cs, f, num:
                         bags.append((tables.tolist(), tuple(ids.shape), code, D, V, out_ld, cs)) or out.zero_())
-    monkeypatch.setattr(ps_hbm._TableGroup, "push_shared",
-                        lambda self, ids, w, f, code, dout, D, ld, cs: pushes.append((self.table_of.tolist(), D, ld, cs)))
+    monkeypatch.setattr(ps_hbm._TableGroup, "push", lambda self, ids, dout, w, f, code, ld=None: pushes.append(
+        (self.table_of.tolist(), self.D, self.out_ld if ld is None else ld, self.col_stride)))
     assert ps_hbm._serve_shared_collections(conn, net) == 1
     df = net.dense_features
     B = 5

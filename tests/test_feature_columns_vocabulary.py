@@ -18,7 +18,7 @@ import torch
 import multihot_reference as mh
 import shared_embedding_reference as sref
 import vocabulary_reference as ref
-from test_feature_columns_crossed import _hbm_connection
+from hbm_fake import hbm_connection
 from tf_yarn_b200 import TaskSpec, data, keras
 from tf_yarn_b200 import estimator as est
 from tf_yarn_b200.ops import features as feature_ids
@@ -419,7 +419,7 @@ def test_hbm_wide_tower_of_vocabulary_columns_is_derived_and_fused():
     va, vb = lst("a", ENTRIES, num_oov_buckets=3), lst("b", ENTRIES[:4])
     wide = [va, vb, fc.categorical_column_with_hash_bucket("a", 1000)]
     net = canned._WideDeepNet(wide, [], [], 1)
-    conn = _hbm_connection(net)
+    conn = hbm_connection(net, "ftrl")
     assert ps_hbm._try_fuse_wide_tower(conn, net) is True
     group = ps_hbm._TableGroup(conn, [0, 1, 2], wide)
     assert group.derived and group.V == 1000 and group.feature_ids.launches == 2     # one vocabulary + one id launch
@@ -446,7 +446,7 @@ def test_hbm_weighted_vocabulary_column_multi_of():
     wa = fc.weighted_categorical_column(lst("a", ENTRIES, num_oov_buckets=2), "aw")
     vb = lst("b", ENTRIES[:5], default_value=1)
     net = canned._WideDeepNet([wa, vb], [], [], 1)
-    conn = _hbm_connection(net)
+    conn = hbm_connection(net, "ftrl")
     assert ps_hbm._try_fuse_wide_tower(conn, net) is True
     f = _model_batch(B=11)
     group = ps_hbm._TableGroup(conn, [0, 1], [wa, vb])
@@ -463,7 +463,7 @@ def test_hbm_deep_tower_with_vocabulary_columns():
     va, vb = lst("a", ENTRIES, num_oov_buckets=2), lst("b", ENTRIES[:6], num_oov_buckets=6)       # V = 12 both
     net = canned._WideDeepNet([], [fc.embedding_column(va, 64), fc.embedding_column(vb, 64),
                                    fc.numeric_column("n", (2,))], [64], 1)
-    conn = _hbm_connection(net)
+    conn = hbm_connection(net, "ftrl")
     assert ps_hbm._try_fuse_first_layer(conn, net) is True
     f = _model_batch(B=9)
     f["a"] = f["a"][:, :1]
@@ -471,7 +471,7 @@ def test_hbm_deep_tower_with_vocabulary_columns():
     assert d.one_hot and d.ids.shape == (2, 9)
     assert torch.equal(d.ids[0], _ids(va, f)[:, 0]) and torch.equal(d.ids[1], _ids(vb, f)[:, 0])
     net = canned._WideDeepNet([], [fc.embedding_column(va, 64), fc.embedding_column(lst("b", [1, 2]), 64)], [64], 1)
-    assert ps_hbm._try_fuse_first_layer(_hbm_connection(net), net) is False
+    assert ps_hbm._try_fuse_first_layer(hbm_connection(net, "ftrl"), net) is False
 
 
 # ---------------------------------------------------------------------------------------------- training

@@ -508,7 +508,7 @@ def test_push_with_heavy_duplicates_is_reproducible(lib, opt):
         assert torch.equal(a, b)
 
 
-def test_wide_tower_push_captured_in_a_cuda_graph_matches_eager(lib):
+def test_wide_tower_group_push_captured_in_a_cuda_graph_matches_eager(lib):
     """_TableGroup.push (the wide tower's FTRL push) captured with torch.cuda.graph and replayed from a restored state
     gives the eager result bit for bit: the duplicate fold needs no host synchronisation."""
     from tf_yarn_b200.estimator import ps_hbm
@@ -518,22 +518,24 @@ def test_wide_tower_push_captured_in_a_cuda_graph_matches_eager(lib):
     conn = types.SimpleNamespace(lib=lib, adam_scale=torch.ones(2, device="cuda"), account=lambda **k: None)
     group = ps_hbm._TableGroup.__new__(ps_hbm._TableGroup)
     group.conn, group.idx, group.tables, group.s1, group.s2 = conn, list(range(T)), tb.ptrs[0], tb.s1, tb.s2
-    group.V, group.h, group.opt, group.p3, group.slots = V, dict(HP[ref.FTRL]), ref.FTRL, HP[ref.FTRL]["p3"], 2
+    h = HP[ref.FTRL]
+    group.V, group.hp, group.slots = V, (ref.FTRL, h["lr"], h["eps"], h["p1"], h["p2"], h["p3"]), 2
+    group.D, group.col_stride, group.out_ld, group.one_table, group.parts = 1, 0, 1, False, None
     ids = torch.from_numpy(_ids(rng, (T, B), V, oor=False)).cuda()
     dout = torch.from_numpy(rng.standard_normal((B, 1)) * 0.5).float().cuda()
     snap = tb.snapshot()
     s = torch.cuda.Stream()
     s.wait_stream(torch.cuda.current_stream())
     with torch.cuda.stream(s):                              # warm-up off the capture stream, as torch recommends
-        group.push(ids, dout, 1, 1, 0)
+        group.push(ids, dout)
     torch.cuda.current_stream().wait_stream(s)
     tb.restore(snap)
-    group.push(ids, dout, 1, 1, 0)
+    group.push(ids, dout)
     torch.cuda.synchronize()
     eager = [b.t.clone() for bb in tb.bufs for b in bb]
     graph = torch.cuda.CUDAGraph()
     with torch.cuda.graph(graph):
-        group.push(ids, dout, 1, 1, 0)
+        group.push(ids, dout)
     for _ in range(2):
         tb.restore(snap)
         graph.replay()

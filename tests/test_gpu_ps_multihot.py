@@ -274,25 +274,28 @@ def test_weighted_push_error_codes(lib):
         assert torch.equal(a, b)                                            # nothing was applied
 
 
-def _group(lib, tb, T, V, opt):
+def _group(lib, tb, T, V, D, opt):
     from tf_yarn_b200.estimator import ps_hbm
     conn = types.SimpleNamespace(lib=lib, adam_scale=torch.ones(2, device="cuda"), account=lambda **k: None)
     group = ps_hbm._TableGroup.__new__(ps_hbm._TableGroup)
     group.conn, group.idx, group.tables, group.s1, group.s2 = conn, list(range(T)), tb.ptrs[0], tb.s1, tb.s2
-    group.V, group.h, group.opt, group.p3, group.slots = V, dict(HP[opt]), opt, HP[opt]["p3"], 2
+    h = HP[opt]
+    group.V, group.hp, group.slots = V, (opt, h["lr"], h["eps"], h["p1"], h["p2"], h["p3"]), 2
+    group.D, group.col_stride, group.one_table, group.parts = D, D, False, None
+    group.out_ld = D * T
     return group
 
 
 @pytest.mark.parametrize("opt", [ref.ADAM, ref.FTRL], ids=["adam", "ftrl"])
-def test_weighted_push_is_reproducible_and_captures_in_a_cuda_graph(lib, opt):
-    """_TableGroup.push_weighted twice from the same state gives bit-identical tables and slots, and the same push
-    captured with torch.cuda.graph and replayed matches it bit for bit: no host synchronisation in the fold, on
+def test_weighted_group_push_is_reproducible_and_captures_in_a_cuda_graph(lib, opt):
+    """_TableGroup.push of a weighted bag's batch twice from the same state gives bit-identical tables and slots, and
+    the same push captured with torch.cuda.graph and replayed matches it bit for bit: no host synchronisation in the fold, on
     both sort paths (B*L = 1536 and 2560)."""
     rng = np.random.default_rng(21 + opt)
     T, V, B, D = 4, 200, 512, 64
     for L in (3, 5):
         tb = _Tables(opt, T, V, D, rng)
-        group = _group(lib, tb, T, V, opt)
+        group = _group(lib, tb, T, V, D, opt)
         ids = torch.from_numpy(_ids(rng, (T, B, L), V)).cuda()
         w = torch.from_numpy(_weights(rng, (T, B, L))).float().cuda()
         f = torch.from_numpy(mh.factors(ids.cpu().numpy(), w.cpu().numpy(), V, "sqrtn")).float().cuda()
@@ -300,7 +303,7 @@ def test_weighted_push_is_reproducible_and_captures_in_a_cuda_graph(lib, opt):
         snap = tb.snapshot()
 
         def push():
-            group.push_weighted(ids, w, f, CODES["sqrtn"], dout, D, D * T, D)
+            group.push(ids, dout, w, f, CODES["sqrtn"])
         s = torch.cuda.Stream()
         s.wait_stream(torch.cuda.current_stream())
         with torch.cuda.stream(s):                          # warm-up off the capture stream, as torch recommends

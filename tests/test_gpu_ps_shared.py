@@ -130,9 +130,9 @@ def test_identity_map_is_bit_equal_to_the_unshared_push(lib, L, weighted):
 
 
 @pytest.mark.parametrize("L", [1, 3])
-def test_shared_push_is_reproducible_and_captures_in_a_cuda_graph(lib, L):
-    """_TableGroup.push_weighted of a group whose columns share tables ([0, 1, 0, 2, 1]): twice from the same state
-    bit-identical, and a captured CUDA graph's replay equal to eager, on both sort paths."""
+def test_shared_group_push_is_reproducible_and_captures_in_a_cuda_graph(lib, L):
+    """_TableGroup.push of a weighted bag's batch in a group whose columns share tables ([0, 1, 0, 2, 1]): twice from
+    the same state bit-identical, and a captured CUDA graph's replay equal to eager, on both sort paths."""
     from tf_yarn_b200.estimator import ps_hbm
     import types
     rng = np.random.default_rng(40 + L)
@@ -141,8 +141,9 @@ def test_shared_push_is_reproducible_and_captures_in_a_cuda_graph(lib, L):
     tb = _Tables(ref.FTRL, n, V, D, rng)
     conn = types.SimpleNamespace(lib=lib, adam_scale=torch.ones(2, device="cuda"), account=lambda **k: None)
     group = ps_hbm._TableGroup.__new__(ps_hbm._TableGroup)
-    group.conn, group.h, group.opt, group.p3, group.slots, group.V = conn, dict(HP[ref.FTRL]), ref.FTRL, \
-        HP[ref.FTRL]["p3"], 2, V
+    h = HP[ref.FTRL]
+    group.conn, group.hp, group.slots, group.V = conn, (ref.FTRL, h["lr"], h["eps"], h["p1"], h["p2"], h["p3"]), 2, V
+    group.D, group.col_stride, group.out_ld, group.one_table, group.parts = D, D, D * T, False, None
     group.idx, group.distinct, group.max_members = table_of, list(range(n)), _max_members(table_of)
     group.push_tables, group.push_s1, group.push_s2 = tb.ptrs
     group.table_of = torch.tensor(table_of, dtype=torch.int32, device="cuda")
@@ -153,7 +154,7 @@ def test_shared_push_is_reproducible_and_captures_in_a_cuda_graph(lib, L):
     snap = tb.snapshot()
 
     def push():
-        group.push_weighted(ids, w, f, CODES["sqrtn"], dout, D, D * T, D)
+        group.push(ids, dout, w, f, CODES["sqrtn"])
     s = torch.cuda.Stream()
     s.wait_stream(torch.cuda.current_stream())
     with torch.cuda.stream(s):

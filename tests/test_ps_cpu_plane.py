@@ -5,6 +5,7 @@ tf_yarn/tensorflow/tasks/tf_task_common.py:46-50)."""
 import pytest
 import torch
 
+from hbm_fake import hbm_connection
 from tf_yarn_b200 import keras
 from tf_yarn_b200.estimator import ps
 
@@ -116,29 +117,6 @@ def test_hbm_shard_sizing_covers_master_slots_and_row_padded_shadows():
                 assert regions[-1][1] <= reserved, (trial, regions[-1], reserved)
 
 
-def _hbm_connection(network, opt="adagrad", n_ps=2):
-    """An HbmConnection over fake base addresses (no GPU): enough for the structural decisions it takes."""
-    from tf_yarn_b200.estimator import ps_hbm
-    named = ps._named_trainables(network)
-    desc = {"adagrad": keras.optimizers.Adagrad(0.05), "sgd": keras.optimizers.SGD(0.1)}[opt]
-    layout = ps.make_layout(named, n_ps, desc)
-    conn = ps_hbm.HbmConnection.__new__(ps_hbm.HbmConnection)
-    conn.layout, conn.names = layout, [n for n, _ in named]
-    conn.lib = None
-    conn.var_opt = [ps_hbm.OPT_CODES[k] for k in layout.kinds]
-    conn.ps_base = [1 << 40, 2 << 40][:n_ps] + [3 << 40] * max(0, n_ps - 2)
-    conn.device = torch.device("cpu")
-    params = dict(network.named_parameters())
-    conn.params = [params[n] for n in conn.names]
-    conn.sparse, conn.gemm = {}, {}
-    conn._classify(network)
-    conn.dense_idx = [i for i in range(len(conn.names)) if i not in conn.sparse]
-    conn.pull_idx = [i for i in conn.dense_idx if i not in conn.gemm]
-    conn.adam_scale = torch.ones(2)
-    conn._acct = {"pull_bytes": 0, "push_bytes": 0, "launches_per_step": 0}
-    return conn
-
-
 def test_hbm_plane_classifies_variables_and_decides_the_fusions():
     """Which variables are served sparsely / streamed by the remote-weight GEMM / pulled, and when the embedding gather
     is fused into the first deep GEMM (K5) and the wide tower into the multi-table kernels -- decided from the network
@@ -149,7 +127,7 @@ def test_hbm_plane_classifies_variables_and_decides_the_fusions():
 
     wide, deep = wdm.feature_columns(vocab=1000, emb_dim=64, n_cat=3, n_num=13)
     net = canned._WideDeepNet(wide, deep, [256, 64], 1)
-    conn = _hbm_connection(net)
+    conn = hbm_connection(net)
     names = conn.names
     sparse = sorted(names[i] for i in conn.sparse)
     gemm = sorted(names[i] for i in conn.gemm)
@@ -162,17 +140,17 @@ def test_hbm_plane_classifies_variables_and_decides_the_fusions():
 
     # numeric columns BEFORE the embeddings: every embedding no longer starts at a multiple of 64 columns
     net2 = canned._WideDeepNet(wide, [deep[-1]] + deep[:-1], [256, 64], 1)
-    assert ps_hbm._try_fuse_first_layer(_hbm_connection(net2), net2) is False
+    assert ps_hbm._try_fuse_first_layer(hbm_connection(net2), net2) is False
     # embedding dimension 16: outside the fused kernel's row format
     wide3, deep3 = wdm.feature_columns(vocab=1000, emb_dim=16, n_cat=3, n_num=13)
     net3 = canned._WideDeepNet(wide3, deep3, [256, 64], 1)
-    assert ps_hbm._try_fuse_first_layer(_hbm_connection(net3), net3) is False
+    assert ps_hbm._try_fuse_first_layer(hbm_connection(net3), net3) is False
     # first hidden width not a multiple of 8: the layer is not served by the remote-weight GEMM at all
     net4 = canned._WideDeepNet(wide, deep, [100, 64], 1)
-    conn4 = _hbm_connection(net4)
+    conn4 = hbm_connection(net4)
     assert "hidden.0.weight" not in [conn4.names[i] for i in conn4.gemm]
     assert ps_hbm._try_fuse_first_layer(conn4, net4) is False
     # tables of different vocabulary sizes cannot share one multi-table launch
     cols = [fc.categorical_column_with_hash_bucket("a", 100), fc.categorical_column_with_hash_bucket("b", 200)]
     net5 = canned._WideDeepNet(cols, [], [], 1)
-    assert ps_hbm._try_fuse_wide_tower(_hbm_connection(net5), net5) is False
+    assert ps_hbm._try_fuse_wide_tower(hbm_connection(net5), net5) is False

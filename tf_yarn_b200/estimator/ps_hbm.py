@@ -62,6 +62,7 @@ native.declare("tfy_ps_multi_push_rows_shared", [_vp, _vp, _vp, _vp, _vp, _i, _i
 OPT_CODES = {"sgd": native.OPT_SGD, "adagrad": native.OPT_ADAGRAD, "adam": native.OPT_ADAM,
              "ftrl": native.OPT_FTRL}
 COMBINER_CODES = {"sum": 0, "mean": 1, "sqrtn": 2}      # tfy_ps_multi_bag_weighted / tfy_ps_multi_push_rows_weighted
+SUM, MEAN = COMBINER_CODES["sum"], COMBINER_CODES["mean"]
 
 
 class PsSeg(ctypes.Structure):
@@ -143,7 +144,7 @@ class HbmConnection:
 
     def __init__(self, layout: ps_cpu.Layout, comm, ranks: Dict[str, int], region_off: int, names: List[str],
                  header: ps_cpu.ShmShard, network: nn.Module):
-        self.layout, self.comm, self.names, self.header = layout, comm, names, header
+        self.layout, self.names, self.header = layout, names, header
         self.lib = native.load()
         bad = sorted({k for k in layout.kinds if k not in OPT_CODES})
         if bad:
@@ -151,7 +152,6 @@ class HbmConnection:
         self.var_opt = [OPT_CODES[k] for k in layout.kinds]
         arena = comm.arena
         self.ps_base = [arena.peer_base[ranks[f"ps:{i}"]] + region_off for i in range(layout.n_ps)]
-        self.region_bytes = shard_bytes(layout)
         dev = torch.device(f"cuda:{comm.device}")
         self.device = dev
         params = dict(network.named_parameters())
@@ -167,8 +167,6 @@ class HbmConnection:
         self._push_segs = None
         self._push_ptrs = None
         self._max_n = max([self._n4(i) for i in self.dense_idx] + [4])
-        self.pull_stream = torch.cuda.Stream(device=dev)
-        self._pull_done: Optional[torch.cuda.Event] = None
         # Adam bias correction {1/(1-b1^t), 1/sqrt(1-b2^t)}: device scalars the push kernels read, refreshed from the
         # global step before every push (so a captured CUDA graph sees them advance)
         self._adam = [i for i, k in enumerate(layout.kinds) if k == "adam"]
@@ -240,16 +238,20 @@ class HbmConnection:
             segs[k].remote_shadow = self.shadow_ptr(i) if i in self.gemm else 0
             segs[k].local = (p.grad.data_ptr() if for_push else p.data_ptr())
             segs[k].n = self.layout.numel[i]
-            segs[k].opt = self.var_opt[i]
-            segs[k].lr, segs[k].eps, segs[k].wd = float(h["lr"]), float(h["eps"]), float(h["wd"])
-            # FTRL: l1, l2, beta (OptimizerSpec.ftrl keeps beta in eps) | Adam: beta1, beta2
-            segs[k].p1, segs[k].p2 = float(h["p1"]), float(h["p2"])
-            segs[k].p3 = float(h["eps"]) if self.layout.kinds[i] == "ftrl" else 0.0
+            segs[k].opt, segs[k].lr, segs[k].eps, segs[k].p1, segs[k].p2, segs[k].p3 = self.push_hypers(i)
+            segs[k].wd = float(h["wd"])
             ld = self.shadow_ld(i) if i in self.gemm else 0
             segs[k].cols = int(self.layout.variables[i][1][1]) if ld else 0
             segs[k].shadow_ld = ld
         dev_segs = torch.frombuffer(bytearray(bytes(segs)), dtype=torch.uint8).to(self.device)
         return dev_segs
+
+    def push_hypers(self, i: int) -> tuple:
+        """(opt, lr, eps, p1, p2, p3) of variable i as every push kernel takes them.  FTRL: l1, l2, beta in p1, p2,
+        p3 (OptimizerSpec.ftrl keeps beta in eps) | Adam: beta1, beta2 in p1, p2."""
+        h = self.layout.hypers[i]
+        p3 = float(h["eps"]) if self.layout.kinds[i] == "ftrl" else 0.0
+        return self.var_opt[i], float(h["lr"]), float(h["eps"]), float(h["p1"]), float(h["p2"]), p3
 
     # ------------------------------------------------------------------ install the fused ops
     def install(self, network: nn.Module) -> None:
@@ -335,67 +337,9 @@ class HbmConnection:
 
 
 def _make_bag_forward(conn: HbmConnection, idx: int, mod: nn.EmbeddingBag):
-    lib = conn.lib
-    V, D = mod.num_embeddings, mod.embedding_dim
-    mean = 1 if mod.mode == "mean" else 0
-
-    class _Bag(torch.autograd.Function):
-        @staticmethod
-        def forward(ctx, ids, anchor):
-            ids = ids.contiguous().long()
-            B, L = ids.shape
-            out = torch.empty((B, D), dtype=torch.float32, device=ids.device)
-            native.check(lib.tfy_ps_embedding_bag(conn.master_ptr(idx), ids.data_ptr(), out.data_ptr(), 0, B, L, D, V,
-                                                  mean, torch.cuda.current_stream().cuda_stream),
-                         "tfy_ps_embedding_bag")
-            conn.account(pull=B * L * D * 4)
-            ctx.ids = ids
-            return out
-
-        @staticmethod
-        def backward(ctx, dout):
-            ids = ctx.ids
-            B, L = ids.shape
-            dout = dout.contiguous().float()
-            lay = conn.layout
-            h = lay.hypers[idx]
-            s1 = conn.master_ptr(idx, 1) if lay.var_slots[idx] >= 1 else None
-            s2 = conn.master_ptr(idx, 2) if lay.var_slots[idx] >= 2 else None
-            p3 = float(h["eps"]) if lay.kinds[idx] == "ftrl" else 0.0
-            scratch = push_rows_scratch(lib, B * L, dout.device)
-            native.check(lib.tfy_ps_push_rows(conn.master_ptr(idx), s1, s2, ids.data_ptr(), dout.data_ptr(), 0, B, L, D,
-                                              V, mean, conn.var_opt[idx], float(h["lr"]), float(h["eps"]),
-                                              float(h["p1"]), float(h["p2"]), p3, 1.0, conn.adam_scale.data_ptr(), 0,
-                                              scratch.data_ptr(), scratch.numel(),
-                                              torch.cuda.current_stream().cuda_stream), "tfy_ps_push_rows")
-            conn.account(push=B * L * D * 4 * (1 + lay.var_slots[idx]), launches=push_rows_launches(B * L))
-            return None, None
-
-    # multi-hot, weighted or sqrtn input: the weighted bag and push with T = 1
     combiner = getattr(mod, "combiner", mod.mode)
-    code = COMBINER_CODES[combiner]
-    group = _TableGroup.single(conn, idx, V)
-    tables = group.tables
-
-    class _WBag(torch.autograd.Function):
-        @staticmethod
-        def forward(ctx, ids, weights, anchor):
-            B, L = ids.shape
-            out = torch.empty((B, D), dtype=torch.float32, device=ids.device)
-            f = torch.empty((1, B), dtype=torch.float32, device=ids.device)
-            weighted_bag(lib, tables, ids[None], weights[None] if weights is not None else None, code, D, V, out, D, 0,
-                         f)
-            conn.account(pull=B * L * D * 4)
-            ctx.ids, ctx.weights, ctx.f = ids, weights, f
-            return out
-
-        @staticmethod
-        def backward(ctx, dout):
-            ids = ctx.ids
-            w = ctx.weights[None] if ctx.weights is not None else None
-            group.push_weighted(ids[None], w, ctx.f, code, dout.contiguous().float(), D, D, 0)
-            return None, None, None
-
+    group = _TableGroup(conn, [idx], [fc.CategoricalColumn("", mod.num_embeddings)], mod.embedding_dim,
+                        combiners=[COMBINER_CODES[combiner]], one_table=True)
     anchor = torch.zeros((), device=conn.device, requires_grad=True)
 
     def run(ids, weights):
@@ -403,14 +347,14 @@ def _make_bag_forward(conn: HbmConnection, idx: int, mod: nn.EmbeddingBag):
         if ids.dim() == 1:
             ids = ids[:, None]
         if weights is None and ids.shape[1] == 1 and combiner in ("sum", "mean"):
-            return _Bag.apply(ids, anchor)          # one id per example: the one-table kernels
+            return _Lookup.apply(group, ids.reshape(1, -1), None, anchor)     # one id per example: the one-table kernels
         if weights is not None:
             weights = weights.contiguous().float().reshape(ids.shape[0], -1)
             if weights.shape != ids.shape:
                 raise ValueError(f"weights {tuple(weights.shape)} do not match ids {tuple(ids.shape)}")
-        return _WBag.apply(ids, weights, anchor)
+            weights = weights[None]
+        return _Lookup.apply(group, ids[None], weights, anchor)     # multi-hot, weighted or sqrtn: the weighted bag
 
-    from tf_yarn_b200.estimator import feature_column as fc
     if isinstance(mod, fc.CombinedBag):
         def forward(ids, weights=None):
             return run(ids, weights)
@@ -466,15 +410,37 @@ def _make_linear_forward(conn: HbmConnection, idx: int, mod: nn.Linear):
     return forward
 
 
-class _TableGroup:
-    """T embedding columns of one tower served by the multi-table kernels (one launch for the whole group).  Column t
-    looks up the table tables_idx[t]; columns of a shared embedding collection repeat their table.  This is the one
-    place that knows the column -> table map: a group whose columns share tables pushes through
-    tfy_ps_multi_push_rows_shared, so that each distinct (table, row) is folded and applied once per push."""
+def _rows(x: Optional[torch.Tensor], rows) -> Optional[torch.Tensor]:
+    """x[rows] (a slice: a view; a list of rows: a contiguous copy), or None."""
+    if x is None:
+        return None
+    return x[rows] if isinstance(rows, slice) else x[rows].contiguous()
 
-    def __init__(self, conn: HbmConnection, tables_idx: List[int], cat_cols):
+
+class _TableGroup:
+    """T embedding columns of one consumer, looked up by one bag and pushed by one push; the only code that launches
+    a sparse bag or push.  Column t looks up the table tables_idx[t]; columns of a shared embedding collection repeat
+    their table.  The consumer's output holds column t's D values at columns [t * col_stride, t * col_stride + D) of
+    each row, or all columns summed into [0, D) when col_stride is 0; combiners[t] is column t's bag combiner.
+
+    A batch comes as ids int64 [T, B] when every column has one id per example and none is weighted (the one-id
+    kernels), else as ids / weights [T, B, L] (the weighted bag).  The kernel serving it:
+
+    * one-id bag: tfy_ps_embedding_bag for a one_table group (an unfused EmbeddingBag), else tfy_ps_multi_bag;
+    * weighted bag: tfy_ps_multi_bag_weighted, once per column when the columns' combiners differ;
+    * push: tables of mixed optimizers one by one (below); columns sharing tables tfy_ps_multi_push_rows_shared, so
+      that each distinct (table, row) is folded and applied once; a weighted bag's push
+      tfy_ps_multi_push_rows_weighted; one-id batches tfy_ps_push_rows for a one_table group, else
+      tfy_ps_multi_push_rows.
+    """
+
+    def __init__(self, conn: HbmConnection, tables_idx: List[int], cat_cols, D: int = 0, col_stride: int = 0,
+                 combiners: Optional[List[int]] = None, one_table: bool = False):
         lay = conn.layout
         self.conn, self.idx, self.cols = conn, tables_idx, cat_cols
+        self.D, self.col_stride, self.one_table = D, col_stride, one_table
+        self.combiners = combiners or [SUM] * len(tables_idx)
+        self.out_ld = col_stride * len(tables_idx) if col_stride else D
         first = tables_idx[0]
         self.uniform = all(lay.kinds[i] == lay.kinds[first] and lay.hypers[i] == lay.hypers[first] for i in tables_idx)
         dev = conn.device
@@ -505,26 +471,17 @@ class _TableGroup:
         self.V = max(c.num_buckets for c in cat_cols) if self.derived else cat_cols[0].num_buckets
         self.same_v = not self.derived and all(c.num_buckets == self.V and c.hashed == cat_cols[0].hashed
                                                for c in cat_cols)
-        h = lay.hypers[first]
-        self.h = h
-        self.opt = conn.var_opt[first]
-        self.p3 = float(h["eps"]) if lay.kinds[first] == "ftrl" else 0.0
+        self.hp = conn.push_hypers(first)
         self.slots = ns
+        self.parts = None if self.uniform else self.split()
 
     @property
     def shared(self) -> bool:
         """True when columns share tables: the group then pushes through tfy_ps_multi_push_rows_shared."""
         return len(set(self.idx)) < len(self.idx)
 
-    @classmethod
-    def single(cls, conn: HbmConnection, idx: int, V: int) -> "_TableGroup":
-        """The one table of an unfused bag (push_weighted only)."""
-        from tf_yarn_b200.estimator import feature_column as fc
-        return cls(conn, [idx], [fc.CategoricalColumn("", V)])
-
     @property
     def weighted(self) -> bool:
-        from tf_yarn_b200.estimator import feature_column as fc
         return any(isinstance(c, fc.WeightedCategoricalColumn) for c in self.cols)
 
     def one_hot(self, features) -> bool:
@@ -558,7 +515,6 @@ class _TableGroup:
     def _bucket(self, raw: torch.Tensor) -> torch.Tensor:
         """feature_column._ids of the stacked columns (the CPU plane's mapping, -1 = missing): one call when the
         columns share V and hashing, else column by column."""
-        from tf_yarn_b200.estimator import feature_column as fc
         if self.same_v:
             return fc._ids(self.cols[0], raw).contiguous()
         return torch.stack([fc._ids(c, r) for c, r in zip(self.cols, raw)]).contiguous()
@@ -593,63 +549,116 @@ class _TableGroup:
         out = []
         for ti in self.distinct:
             members = [t for t, i in enumerate(self.idx) if i == ti]
-            out.append((members, _TableGroup(self.conn, [ti] * len(members), [self.cols[t] for t in members])))
+            shared = len(members) > 1
+            out.append((members, _TableGroup(self.conn, [ti] * len(members), [self.cols[t] for t in members], self.D,
+                                             self.D if shared else 0, one_table=not shared)))
         return out
 
-    def push_shared(self, ids: torch.Tensor, weights: Optional[torch.Tensor], f: Optional[torch.Tensor], combiner: int,
-                    dout: torch.Tensor, D: int, dout_ld: int, col_stride: int) -> None:
-        """tfy_ps_multi_push_rows_shared: ids / weights [T, B, L] (or ids [T, B]), f [T, B] or None."""
-        conn, h = self.conn, self.h
+    def bag(self, ids: torch.Tensor, weights: Optional[torch.Tensor] = None, out: Optional[torch.Tensor] = None,
+            out_ld: Optional[int] = None, numeric: Optional[torch.Tensor] = None):
+        """Look up a batch into out (fp32 [B, out_ld] allocated when None; the weighted bag writes the numeric
+        columns after the embeddings).  Returns out and, for the weighted bag, f fp32 [T, B]: each row's 1/den,
+        which its push takes."""
+        conn, lib, D, V = self.conn, self.conn.lib, self.D, self.V
         T, B = ids.shape[:2]
         L = ids.shape[2] if ids.dim() == 3 else 1
-        scratch = push_rows_scratch(conn.lib, T * B * L, dout.device)
-        native.check(conn.lib.tfy_ps_multi_push_rows_shared(
-            self.push_tables.data_ptr(), _ptr(self.push_s1), _ptr(self.push_s2), ids.data_ptr(), dout.data_ptr(),
-            1 if dout.dtype == torch.bfloat16 else 0, B, T, D, self.V, self.opt, float(h["lr"]), float(h["eps"]),
-            float(h["p1"]), float(h["p2"]), self.p3, 1.0, conn.adam_scale.data_ptr(), dout_ld, col_stride, L,
-            _ptr(weights), _ptr(f), combiner, len(self.distinct), self.table_of.data_ptr(), self.max_members,
-            scratch.data_ptr(), scratch.numel(), torch.cuda.current_stream().cuda_stream),
-            "tfy_ps_multi_push_rows_shared")
-        # the rows written are those of the distinct tables; the occurrences read are every column's
-        conn.account(push=T * B * L * D * 4 * (1 + self.slots), launches=push_rows_launches(B * L, self.max_members))
+        out_ld = self.out_ld if out_ld is None else out_ld
+        if out is None:
+            out = torch.empty((B, out_ld), dtype=torch.float32, device=ids.device)
+        f, launches = None, 1
+        if ids.dim() == 2 and self.one_table:
+            native.check(lib.tfy_ps_embedding_bag(conn.master_ptr(self.idx[0]), ids.data_ptr(), out.data_ptr(), 0, B, L,
+                                                  D, V, int(self.combiners[0] == MEAN),
+                                                  torch.cuda.current_stream().cuda_stream), "tfy_ps_embedding_bag")
+        elif ids.dim() == 2:
+            native.check(lib.tfy_ps_multi_bag(self.tables.data_ptr(), ids.data_ptr(), out.data_ptr(), 0, B, T, D, V,
+                                              torch.cuda.current_stream().cuda_stream), "tfy_ps_multi_bag")
+        else:
+            f = torch.empty((T, B), dtype=torch.float32, device=ids.device)
+            if len(set(self.combiners)) == 1:
+                weighted_bag(lib, self.tables, ids, weights, self.combiners[0], D, V, out, out_ld, self.col_stride, f,
+                             numeric)
+            else:       # the bag takes one combiner per launch: column by column, numeric after the last
+                launches = T
+                for t in range(T):
+                    weighted_bag(lib, self.tables[t:t + 1], ids[t:t + 1], _rows(weights, slice(t, t + 1)),
+                                 self.combiners[t], D, V, out[:, self.col_stride * t:], out_ld, self.col_stride,
+                                 f[t:t + 1], numeric if t == T - 1 else None)
+        conn.account(pull=T * B * L * D * 4, launches=launches)
+        return out, f
 
-    def push_weighted(self, ids: torch.Tensor, weights: Optional[torch.Tensor], f: torch.Tensor, combiner: int,
-                      dout: torch.Tensor, D: int, dout_ld: int, col_stride: int) -> None:
-        """tfy_ps_multi_push_rows_weighted of a weighted bag's backward: ids / weights [T, B, L], f [T, B]."""
+    def push(self, ids: torch.Tensor, dout: torch.Tensor, weights: Optional[torch.Tensor] = None,
+             f: Optional[torch.Tensor] = None, combiner: int = SUM, dout_ld: Optional[int] = None) -> None:
+        """Apply the row gradients of a bag's batch (ids, weights and the bag's f) with each table's optimizer.  dout
+        [B, *] is laid out as the bag's output, with row pitch dout_ld (None: the bag's own out_ld).  combiner goes to
+        the kernels that take one; with f given it only says that f is."""
+        if self.parts is not None:              # mixed optimizers: table by table, each with its member columns
+            for members, sub in self.parts:
+                if sub.shared:
+                    cols = [dout[:, self.col_stride * t:self.col_stride * t + self.D] for t in members]
+                    sub.push(_rows(ids, members), torch.cat(cols, dim=1), _rows(weights, members), _rows(f, members),
+                             combiner)
+                else:
+                    t = slice(members[0], members[0] + 1)
+                    sub.push(ids[t], dout[:, self.col_stride * members[0]:], _rows(weights, t), _rows(f, t), combiner,
+                             self.out_ld if dout_ld is None else dout_ld)
+            return
+        conn, lib, D, V = self.conn, self.conn.lib, self.D, self.V
+        T, B = ids.shape[:2]
+        L = ids.shape[2] if ids.dim() == 3 else 1
+        ld = self.out_ld if dout_ld is None else dout_ld
+        scratch = push_rows_scratch(lib, T * B * L, dout.device)
+        hyper = (*self.hp, 1.0, conn.adam_scale.data_ptr())
+        tail = (scratch.data_ptr(), scratch.numel(), torch.cuda.current_stream().cuda_stream)
+        args = (ids.data_ptr(), dout.data_ptr(), int(dout.dtype == torch.bfloat16), B)
         if self.shared:
-            return self.push_shared(ids, weights, f, combiner, dout, D, dout_ld, col_stride)
-        conn, h = self.conn, self.h
-        T, B, L = ids.shape
-        scratch = push_rows_scratch(conn.lib, T * B * L, dout.device)
-        native.check(conn.lib.tfy_ps_multi_push_rows_weighted(
-            self.tables.data_ptr(), _ptr(self.s1), _ptr(self.s2), ids.data_ptr(), dout.data_ptr(),
-            1 if dout.dtype == torch.bfloat16 else 0, B, T, D, self.V, self.opt, float(h["lr"]), float(h["eps"]),
-            float(h["p1"]), float(h["p2"]), self.p3, 1.0, conn.adam_scale.data_ptr(), dout_ld, col_stride, L,
-            _ptr(weights), f.data_ptr(), combiner, scratch.data_ptr(), scratch.numel(),
-            torch.cuda.current_stream().cuda_stream), "tfy_ps_multi_push_rows_weighted")
-        # one launch more than an unweighted push: the per-occurrence factors w * f
-        conn.account(push=T * B * L * D * 4 * (1 + self.slots), launches=push_rows_launches(B * L) + 1)
+            name = "tfy_ps_multi_push_rows_shared"
+            rc = lib.tfy_ps_multi_push_rows_shared(
+                self.push_tables.data_ptr(), _ptr(self.push_s1), _ptr(self.push_s2), *args, T, D, V, *hyper, ld,
+                self.col_stride, L, _ptr(weights), _ptr(f), combiner, len(self.distinct), self.table_of.data_ptr(),
+                self.max_members, *tail)
+        elif f is not None:
+            name = "tfy_ps_multi_push_rows_weighted"
+            rc = lib.tfy_ps_multi_push_rows_weighted(self.tables.data_ptr(), _ptr(self.s1), _ptr(self.s2), *args, T, D,
+                                                     V, *hyper, ld, self.col_stride, L, _ptr(weights), f.data_ptr(),
+                                                     combiner, *tail)
+        elif self.one_table:                    # dout_ld 0: rows of D
+            name = "tfy_ps_push_rows"
+            i = self.idx[0]
+            slot = [conn.master_ptr(i, s) if s <= self.slots else None for s in range(3)]
+            rc = lib.tfy_ps_push_rows(*slot, *args, L, D, V, int(combiner == MEAN), *hyper, dout_ld or 0, *tail)
+        else:
+            name = "tfy_ps_multi_push_rows"
+            rc = lib.tfy_ps_multi_push_rows(self.tables.data_ptr(), _ptr(self.s1), _ptr(self.s2), *args, T, D, V,
+                                            *hyper, ld, self.col_stride, *tail)
+        native.check(rc, name)
+        # the rows written are those of the distinct tables; the occurrences read are every column's.  A weighted
+        # push runs one kernel more than an unweighted one: the per-occurrence factors w * f (the shared push's
+        # offsets kernel writes them)
+        launches = push_rows_launches(B * L, self.max_members if self.shared else 0)
+        conn.account(push=T * B * L * D * 4 * (1 + self.slots), launches=launches + int(f is not None and not self.shared))
 
-    def push(self, ids: torch.Tensor, dout: torch.Tensor, D: int, dout_ld: int, col_stride: int) -> None:
-        if self.shared:
-            return self.push_shared(ids, None, None, COMBINER_CODES["sum"], dout, D, dout_ld, col_stride)
-        conn, h = self.conn, self.h
-        B, T = ids.shape[1], len(self.idx)
-        scratch = push_rows_scratch(conn.lib, T * B, dout.device)
-        native.check(conn.lib.tfy_ps_multi_push_rows(
-            self.tables.data_ptr(), self.s1.data_ptr() if self.s1 is not None else None,
-            self.s2.data_ptr() if self.s2 is not None else None, ids.data_ptr(), dout.data_ptr(),
-            1 if dout.dtype == torch.bfloat16 else 0, B, T, D, self.V, self.opt, float(h["lr"]), float(h["eps"]),
-            float(h["p1"]), float(h["p2"]), self.p3, 1.0, conn.adam_scale.data_ptr(), dout_ld, col_stride,
-            scratch.data_ptr(), scratch.numel(), torch.cuda.current_stream().cuda_stream), "tfy_ps_multi_push_rows")
-        conn.account(push=T * B * D * 4 * (1 + self.slots), launches=push_rows_launches(B))
+
+class _Lookup(torch.autograd.Function):
+    """An embedding lookup over a table group: group.bag forward, group.push backward.  anchor is a leaf that
+    requires grad, so that the backward runs although no input does."""
+
+    @staticmethod
+    def forward(ctx, group, ids, weights, anchor):
+        out, ctx.f = group.bag(ids, weights)
+        ctx.group, ctx.ids, ctx.weights = group, ids, weights
+        return out
+
+    @staticmethod
+    def backward(ctx, dout):
+        ctx.group.push(ctx.ids, dout.contiguous().float(), ctx.weights, ctx.f, ctx.group.combiners[0])
+        return None, None, None, None
 
 
 def _try_fuse_wide_tower(conn: HbmConnection, network: nn.Module) -> bool:
     """The wide tower (fc.LinearModel): T per-bucket weight tables [V, units] looked up once per example and summed.
     One multi-table gather kernel forward, one multi-table push (FTRL / ... fused) backward, instead of T launches
     each plus T adds."""
-    from tf_yarn_b200.estimator import feature_column as fc
     if os.environ.get("TFY_PS_FUSE_WIDE", "1") == "0":
         return False
     lin = getattr(network, "linear", None)
@@ -666,57 +675,20 @@ def _try_fuse_wide_tower(conn: HbmConnection, network: nn.Module) -> bool:
                 return False
             cat_cols.append(cc)
             tables_idx.append(ti)
-    group = _TableGroup(conn, tables_idx, cat_cols)
+    combiner = lin.sparse_combiner
+    # every table gets the same gradient (col_stride 0)
+    group = _TableGroup(conn, tables_idx, cat_cols, lin.units,
+                        combiners=[COMBINER_CODES[combiner]] * len(tables_idx))
     if not (group.uniform and (group.same_v or group.derived)):     # mixed V only with the id kernel's bound
         return False
-    units = lin.units
-    dev = conn.device
-    combiner = lin.sparse_combiner
-    code = COMBINER_CODES[combiner]
-
-    class _MultiBag(torch.autograd.Function):
-        @staticmethod
-        def forward(ctx, ids, anchor):
-            B = ids.shape[1]
-            out = torch.empty((B, units), dtype=torch.float32, device=dev)
-            native.check(conn.lib.tfy_ps_multi_bag(group.tables.data_ptr(), ids.data_ptr(), out.data_ptr(), 0, B,
-                                                   len(tables_idx), units, group.V,
-                                                   torch.cuda.current_stream().cuda_stream), "tfy_ps_multi_bag")
-            conn.account(pull=B * len(tables_idx) * units * 4)
-            ctx.ids = ids
-            return out
-
-        @staticmethod
-        def backward(ctx, dout):
-            group.push(ctx.ids, dout.contiguous().float(), units, units, 0)     # every table gets the same gradient
-            return None, None
-
-    class _WMultiBag(torch.autograd.Function):
-        """Multi-hot, weighted or non-sum wide tower: every column combined by the sparse combiner, then summed."""
-
-        @staticmethod
-        def forward(ctx, ids, weights, anchor):
-            T, B, L = ids.shape
-            out = torch.empty((B, units), dtype=torch.float32, device=dev)
-            f = torch.empty((T, B), dtype=torch.float32, device=dev)
-            weighted_bag(conn.lib, group.tables, ids, weights, code, units, group.V, out, units, 0, f)
-            conn.account(pull=T * B * L * units * 4)
-            ctx.ids, ctx.weights, ctx.f = ids, weights, f
-            return out
-
-        @staticmethod
-        def backward(ctx, dout):
-            group.push_weighted(ctx.ids, ctx.weights, ctx.f, code, dout.contiguous().float(), units, units, 0)
-            return None, None, None
-
-    anchor = torch.zeros((), device=dev, requires_grad=True)
+    anchor = torch.zeros((), device=conn.device, requires_grad=True)
     num_cols = [c for c in lin.columns if isinstance(c, fc.NumericColumn)]
 
     def forward(features):
         if combiner == "sum" and group.one_hot(features):
-            out = _MultiBag.apply(group.ids_of(features), anchor)
-        else:
-            out = _WMultiBag.apply(*group.multi_of(features), anchor)
+            out = _Lookup.apply(group, group.ids_of(features), None, anchor)
+        else:       # multi-hot, weighted or non-sum: every column combined by the sparse combiner, then summed
+            out = _Lookup.apply(group, *group.multi_of(features), anchor)
         if lin.numeric is not None and num_cols:
             nums = [features[c.key].reshape(features[c.key].shape[0], -1).float() for c in num_cols]
             x = nums[0] if len(nums) == 1 else torch.cat(nums, dim=1)
@@ -733,7 +705,6 @@ def _serve_shared_collections(conn: HbmConnection, network: nn.Module, k5_featur
     members of a collection (T = members, the table repeated, into a [B, C*D] buffer sliced to their positions) and
     one shared push in its backward, instead of one bag and one push per member.  k5_features is the DenseFeatures
     whose forward K5 replaced (its collections are pushed by K5's backward).  Returns the collections served."""
-    from tf_yarn_b200.estimator import feature_column as fc
     by_param = {id(p): i for i, p in enumerate(conn.params)}
     served = 0
     for df in network.modules():
@@ -760,30 +731,12 @@ def _shared_lookup(conn: HbmConnection, ti: int, members):
     """One collection's lookup: the members' [B, D] values from one tfy_ps_multi_bag_weighted launch, and one push of
     the table for all of them."""
     C, D = len(members), members[0].dimension
-    code = COMBINER_CODES[members[0].combiner]
-    group = _TableGroup(conn, [ti] * C, [c.categorical_column for c in members])
-    dev = conn.device
-
-    class _SharedBag(torch.autograd.Function):
-        @staticmethod
-        def forward(ctx, ids, weights, anchor):
-            _, B, L = ids.shape
-            out = torch.empty((B, C * D), dtype=torch.float32, device=dev)
-            f = torch.empty((C, B), dtype=torch.float32, device=dev)
-            weighted_bag(conn.lib, group.tables, ids, weights, code, D, group.V, out, C * D, D, f)
-            conn.account(pull=C * B * L * D * 4)
-            ctx.ids, ctx.weights, ctx.f = ids, weights, f
-            return out
-
-        @staticmethod
-        def backward(ctx, dout):
-            group.push_weighted(ctx.ids, ctx.weights, ctx.f, code, dout.contiguous().float(), D, C * D, D)
-            return None, None, None
-
-    anchor = torch.zeros((), device=dev, requires_grad=True)
+    group = _TableGroup(conn, [ti] * C, [c.categorical_column for c in members], D, D,
+                        combiners=[COMBINER_CODES[members[0].combiner]] * C)
+    anchor = torch.zeros((), device=conn.device, requires_grad=True)
 
     def lookup(features):
-        out = _SharedBag.apply(*group.multi_of(features), anchor)
+        out = _Lookup.apply(group, *group.multi_of(features), anchor)
         return [out[:, D * k:D * k + D] for k in range(C)]
     return lookup
 
@@ -796,7 +749,6 @@ def _try_fuse_first_layer(conn: HbmConnection, network: nn.Module) -> bool:
     ``network.hidden[0]`` is a Linear served by the remote-weight GEMM.  The gather of the rows from the ps ranks'
     HBM becomes the A-operand producer of that GEMM; the backward (dW, dx) is one wgmma kernel against the same
     remote shadow, and the row gradients are pushed straight out of its dx.  TFY_PS_FUSE_FIRST=0 disables it."""
-    from tf_yarn_b200.estimator import feature_column as fc
     from tf_yarn_b200.ops.gemm import gemm_bf16
     if os.environ.get("TFY_PS_FUSE_FIRST", "1") == "0":
         return False
@@ -833,121 +785,58 @@ def _try_fuse_first_layer(conn: HbmConnection, network: nn.Module) -> bool:
     dev = conn.device
     N, K, Kp = lin.out_features, lin.in_features, conn.shadow_ld(widx)
     shadow = conn.shadow_ptr(widx)
-    group = _TableGroup(conn, tables_idx, [c.categorical_column for c in emb_cols])
-    table_ptrs = group.tables
-    lib, lay = conn.lib, conn.layout
-    # the bag takes one combiner per launch: a group whose columns differ is gathered table by table.  The push takes
-    # the per-table 1/den in f, so one push serves any mix (its combiner argument only says that f is given).
-    codes = [COMBINER_CODES[c.combiner] for c in emb_cols]
-    one_code = len(set(codes)) == 1
-    push_code = COMBINER_CODES["mean"]
-    # tables of mixed optimizers push one by one, each with its own member columns (one, unless the table is shared)
-    per_table = None if group.uniform else group.split()
-
-    def members_dx(dx, members):
-        """The members' 64-column slices of dx side by side, for the push of a shared table."""
-        return torch.cat([dx[:, 64 * t:64 * t + 64] for t in members], dim=1)
-
-    def first_backward(xbuf, dy, weight, push):
-        """dW and dx in one wgmma kernel against the remote shadow, then push(dx) of the embedding rows."""
-        B = xbuf.shape[0]
-        dyb = dy.to(torch.bfloat16).contiguous()
-        dw = torch.empty((N, Kp), dtype=torch.bfloat16, device=dev)
-        dx = torch.empty((B, Kp), dtype=torch.bfloat16, device=dev)
-        native.check(lib.tfy_dense_bwd(dyb.data_ptr(), xbuf.data_ptr(), shadow, dw.data_ptr(), dx.data_ptr(), B, N,
-                                       Kp, torch.cuda.current_stream().cuda_stream), "tfy_dense_bwd")
-        conn.account(pull=N * Kp * 2)
-        push(dx)
-        return dw[:, :K].to(weight.dtype), dy.float().sum(0).to(weight.dtype)
+    # table t takes columns [64 t, 64 t + 64) of the activation buffer and of dx.  The bag takes one combiner per
+    # launch (a group whose columns differ is gathered table by table); the push takes each column's 1/den in f, so
+    # it is told "mean" whatever the mix
+    group = _TableGroup(conn, tables_idx, [c.categorical_column for c in emb_cols], 64, 64,
+                        combiners=[COMBINER_CODES[c.combiner] for c in emb_cols])
 
     class _FusedFirst(torch.autograd.Function):
+        """One id per example: the gather is the A-operand producer of the GEMM (tfy_ps_gather_gemm)."""
+
         @staticmethod
-        def forward(ctx, ids, numeric, weight, bias):
+        def forward(ctx, ids, weights, numeric, weight, bias):
             B = ids.shape[1]
             xbuf = torch.zeros((B, Kp), dtype=torch.bfloat16, device=dev)
             y = torch.empty((B, N), dtype=torch.bfloat16, device=dev)
             bb = bias.to(torch.bfloat16)
-            native.check(lib.tfy_ps_gather_gemm(shadow, table_ptrs.data_ptr(), ids.data_ptr(),
-                                                numeric.data_ptr() if numeric is not None else None, bb.data_ptr(),
-                                                xbuf.data_ptr(), y.data_ptr(), B, N, T, n_num, Kp, V,
-                                                torch.cuda.current_stream().cuda_stream), "tfy_ps_gather_gemm")
+            native.check(conn.lib.tfy_ps_gather_gemm(shadow, group.tables.data_ptr(), ids.data_ptr(),
+                                                     numeric.data_ptr() if numeric is not None else None,
+                                                     bb.data_ptr(), xbuf.data_ptr(), y.data_ptr(), B, N, T, n_num, Kp,
+                                                     V, torch.cuda.current_stream().cuda_stream), "tfy_ps_gather_gemm")
             conn.account(pull=B * T * 64 * 4 + N * Kp * 2)
             ctx.save_for_backward(xbuf, ids, weight)
+            ctx.weights, ctx.f = None, None
             return y.to(weight.dtype)
 
         @staticmethod
         def backward(ctx, dy):
+            """dW and dx in one wgmma kernel against the remote shadow, then the push of the embedding rows straight
+            out of dx."""
             xbuf, ids, weight = ctx.saved_tensors
             B = xbuf.shape[0]
-            s = torch.cuda.current_stream().cuda_stream
+            dyb = dy.to(torch.bfloat16).contiguous()
+            dw = torch.empty((N, Kp), dtype=torch.bfloat16, device=dev)
+            dx = torch.empty((B, Kp), dtype=torch.bfloat16, device=dev)
+            native.check(conn.lib.tfy_dense_bwd(dyb.data_ptr(), xbuf.data_ptr(), shadow, dw.data_ptr(), dx.data_ptr(),
+                                                B, N, Kp, torch.cuda.current_stream().cuda_stream), "tfy_dense_bwd")
+            conn.account(pull=N * Kp * 2)
+            group.push(ids, dx, ctx.weights, ctx.f, SUM if ctx.f is None else MEAN, Kp)
+            return None, None, None, dw[:, :K].to(weight.dtype), dy.float().sum(0).to(weight.dtype)
 
-            def push(dx):
-                if group.uniform:
-                    # table t takes columns [64 t, 64 t + 64) of dx: ONE launch for all tables, straight out of dx
-                    group.push(ids, dx, 64, Kp, 64)
-                    return
-                for members, sub in per_table:               # (mixed optimizers) table by table
-                    if sub.shared:
-                        sub.push(ids[members].contiguous(), members_dx(dx, members), 64, 64 * len(members), 64)
-                        continue
-                    t = members[0]
-                    ti = tables_idx[t]
-                    h = lay.hypers[ti]
-                    s1 = conn.master_ptr(ti, 1) if lay.var_slots[ti] >= 1 else None
-                    s2 = conn.master_ptr(ti, 2) if lay.var_slots[ti] >= 2 else None
-                    p3 = float(h["eps"]) if lay.kinds[ti] == "ftrl" else 0.0
-                    scratch = push_rows_scratch(lib, B, dev)
-                    native.check(lib.tfy_ps_push_rows(
-                        conn.master_ptr(ti), s1, s2, ids[t].data_ptr(), dx.data_ptr() + 2 * 64 * t, 1, B, 1, 64, V, 0,
-                        conn.var_opt[ti], float(h["lr"]), float(h["eps"]), float(h["p1"]), float(h["p2"]), p3, 1.0,
-                        conn.adam_scale.data_ptr(), Kp, scratch.data_ptr(), scratch.numel(), s), "tfy_ps_push_rows")
-                    conn.account(push=B * 64 * 4 * (1 + lay.var_slots[ti]), launches=push_rows_launches(B))
-            dw, db = first_backward(xbuf, dy, weight, push)
-            return None, None, dw, db
-
-    class _BagFirst(torch.autograd.Function):
+    class _BagFirst(_FusedFirst):
         """Multi-hot or weighted batches: the weighted bag writes the activation buffer K5 would (embeddings, then
         the numeric columns), then the remote-weight GEMM; the backward is K5's, with the weighted push."""
 
         @staticmethod
         def forward(ctx, ids, weights, numeric, weight, bias):
-            _, B, L = ids.shape
-            xbuf = torch.zeros((B, Kp), dtype=torch.bfloat16, device=dev)
-            f = torch.empty((T, B), dtype=torch.float32, device=dev)
-            if one_code:
-                weighted_bag(lib, table_ptrs, ids, weights, codes[0], 64, V, xbuf, Kp, 64, f, numeric)
-            else:                                           # table t into columns [64 t, 64 t + 64); numeric last
-                for t in range(T):
-                    weighted_bag(lib, table_ptrs[t:t + 1], ids[t:t + 1],
-                                 weights[t:t + 1] if weights is not None else None, codes[t], 64, V, xbuf[:, 64 * t:],
-                                 Kp, 64, f[t:t + 1], numeric if t == T - 1 else None)
+            xbuf = torch.zeros((ids.shape[1], Kp), dtype=torch.bfloat16, device=dev)
+            _, f = group.bag(ids, weights, xbuf, Kp, numeric)
             y = gemm_bf16(xbuf, None, bias=bias.to(torch.bfloat16), b_ptr=shadow, b_rows=N, b_ld=Kp, impl="1cta")
-            conn.account(pull=T * B * L * 64 * 4, launches=1 if one_code else T)
             conn.account(pull=N * Kp * 2)
             ctx.save_for_backward(xbuf, ids, weight)
             ctx.weights, ctx.f = weights, f
             return y.to(weight.dtype)
-
-        @staticmethod
-        def backward(ctx, dy):
-            xbuf, ids, weight = ctx.saved_tensors
-            w, f = ctx.weights, ctx.f
-
-            def push(dx):
-                if group.uniform:
-                    group.push_weighted(ids, w, f, push_code, dx, 64, Kp, 64)
-                    return
-                for members, sub in per_table:              # (mixed optimizers) table by table
-                    if sub.shared:
-                        sub.push_weighted(ids[members].contiguous(), w[members].contiguous() if w is not None else None,
-                                          f[members].contiguous(), push_code, members_dx(dx, members), 64,
-                                          64 * len(members), 64)
-                        continue
-                    t = members[0]
-                    sub.push_weighted(ids[t:t + 1], w[t:t + 1] if w is not None else None, f[t:t + 1], push_code,
-                                      dx[:, 64 * t:], 64, Kp, 0)
-            dw, db = first_backward(xbuf, dy, weight, push)
-            return None, None, None, dw, db
 
     class _Deferred:
         """What the patched DenseFeatures returns: the raw inputs of the fused first layer (weights is None and ids
@@ -973,9 +862,8 @@ def _try_fuse_first_layer(conn: HbmConnection, network: nn.Module) -> bool:
 
     def lin_forward(x):
         if isinstance(x, _Deferred):
-            if x.one_hot:
-                return _FusedFirst.apply(x.ids, x.numeric, lin.weight, lin.bias)
-            return _BagFirst.apply(x.ids, x.weights, x.numeric, lin.weight, lin.bias)
+            fn = _FusedFirst if x.one_hot else _BagFirst
+            return fn.apply(x.ids, x.weights, x.numeric, lin.weight, lin.bias)
         return _make_linear_forward(conn, widx, lin)(x)
 
     df.forward = df_forward
