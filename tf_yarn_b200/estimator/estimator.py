@@ -128,6 +128,7 @@ class Estimator:
         self._device: Optional[torch.device] = None
         self._ps = None
         self._ps_graph = None
+        self._ps_state: Optional[Dict[str, dict]] = None
         self._last_loss_t = None
         self._pending_broadcast: Optional[int] = None
         self.last_loss: Optional[float] = None
@@ -224,7 +225,9 @@ class Estimator:
                    "network": self._network.state_dict() if self._network is not None else None,
                    "optimizer": self._optimizer.state_dict() if self._optimizer is not None else None}
         if self._ps is not None:
+            # the ps holds the weights and their optimizer slots: the local torch optimizer is never stepped
             payload["network"] = self._ps.state_dict_from_ps(self._network)
+            payload["ps_state"] = self._ps.optimizer_state()
         path = ckpt.save_checkpoint(self._model_dir, self._global_step, payload, self._config.keep_checkpoint_max)
         logger.info("Saved checkpoint for step %d: %s", self._global_step, path)
         return path
@@ -241,6 +244,8 @@ class Estimator:
                 self._optimizer.load_state_dict(payload["optimizer"])
             except (ValueError, KeyError):
                 logger.warning("optimizer state in %s does not match; starting it fresh", path)
+        # the parameter servers' optimizer slots, for the connect_worker call in train (None: fresh slots)
+        self._ps_state = payload.get("ps_state") if with_optimizer and self._ps is None else None
         self._global_step = int(payload.get("global_step", 0))
         logger.info("Restored from %s (global step %d)", path, self._global_step)
         return True
@@ -277,10 +282,13 @@ class Estimator:
             if self._device.type == "cuda" and os.environ.get("TFY_PS_PLANE", "auto") != "shm":
                 from tf_yarn_b200.estimator import ps_hbm
                 self._ps = ps_hbm.connect_worker(self._network, self._opt_desc, cluster, is_chief,
-                                                 self._global_step, opt_by_name=self._opt_by_name)
+                                                 self._global_step, opt_by_name=self._opt_by_name,
+                                                 ps_state=self._ps_state)
             else:
                 self._ps = ps_mod.connect_worker(self._network, self._opt_desc, cluster, is_chief,
-                                                 self._global_step, opt_by_name=self._opt_by_name)
+                                                 self._global_step, opt_by_name=self._opt_by_name,
+                                                 ps_state=self._ps_state)
+            self._ps_state = None
             if not is_chief:
                 self._global_step = self._ps.global_step()
         if self._pending_broadcast is not None:

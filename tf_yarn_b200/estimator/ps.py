@@ -42,16 +42,21 @@ logger = logging.getLogger(__name__)
 KV_LAYOUT = "ps/layout"
 KV_READY = "ps/ready"
 
-# optimizer slots per variable (besides the value itself)
-_SLOTS = {"sgd": 0, "adagrad": 1, "adadelta": 2, "adam": 2, "adamw": 2, "ftrl": 2}
+# optimizer slots per variable (besides the value itself), in their order in the shard
+_SLOT_NAMES = {"sgd": (), "adagrad": ("accumulator",), "adadelta": ("accum_grad", "accum_update"), "adam": ("m", "v"),
+               "adamw": ("m", "v"), "ftrl": ("n", "z")}
+
+
+def slot_names(kind: str, hyper: Dict[str, float]) -> Tuple[str, ...]:
+    """Slots of one variable, in shard order.  RMSprop's depend on its hyper-parameters: mean square, then the
+    momentum buffer (p2 = momentum > 0), then the mean gradient (flags bit 0 = centered)."""
+    if kind == "rmsprop":
+        return ("ms",) + (("momentum",) if hyper["p2"] > 0 else ()) + (("mg",) if int(hyper["flags"]) & 1 else ())
+    return _SLOT_NAMES[kind]
 
 
 def _var_slots(kind: str, hyper: Dict[str, float]) -> int:
-    """Slots of one variable.  RMSprop's depend on its hyper-parameters: mean square, then the momentum buffer
-    (p2 = momentum > 0), then the mean gradient (flags bit 0 = centered)."""
-    if kind == "rmsprop":
-        return 1 + (hyper["p2"] > 0) + (int(hyper["flags"]) & 1)
-    return _SLOTS[kind]
+    return len(slot_names(kind, hyper))
 
 
 def _job_tag() -> str:
@@ -246,6 +251,10 @@ class WorkerConnection:
         self.pull(network)
         return network.state_dict()
 
+    def optimizer_state(self) -> Dict[str, dict]:
+        """Every variable's optimizer slots, read from the ps shards (`export_slots`)."""
+        return export_slots(self.layout, self._region)
+
 
 def _named_trainables(network: nn.Module) -> List[Tuple[str, nn.Parameter]]:
     return [(n, p) for n, p in network.named_parameters() if p.requires_grad]
@@ -258,9 +267,61 @@ def make_layout(named, n_ps: int, opt_desc, opt_by_name=None) -> Layout:
                   [d.to_spec().kind for d in descs], [_hyper_of(d) for d in descs])
 
 
+# ---- optimizer slots in checkpoints (both data planes) ----------------------------------------------
+def export_slots(layout: Layout, region) -> Dict[str, dict]:
+    """A checkpoint's ``ps_state``: per variable name its optimizer kind, shape, slot names and slots (fp32 CPU
+    copies, in shard order).  region(i, s) is slot s of variable i in the shards (slot 0: the value, not saved here).
+    """
+    out = {}
+    for i, (name, shape) in enumerate(layout.variables):
+        names = slot_names(layout.kinds[i], layout.hypers[i])
+        out[name] = {"kind": layout.kinds[i], "shape": list(shape), "slot_names": list(names),
+                     "slots": [region(i, s).detach().to(device="cpu", dtype=torch.float32, copy=True)
+                               for s in range(1, 1 + len(names))]}
+    return out
+
+
+def match_slots(ps_state: Dict[str, dict], layout: Layout) -> List[Optional[List[torch.Tensor]]]:
+    """Per variable of `layout`: the saved slots of `ps_state` to install, or None for fresh ones.  Variables are
+    matched by name, so the number of ps tasks may change.  A variable's slots are restored when its optimizer kind,
+    its slots and its element count all match the saved ones; hyper-parameters such as the learning rate may differ,
+    as in TF.  One warning names every variable that starts fresh."""
+    out: List[Optional[List[torch.Tensor]]] = []
+    fresh = []
+    for i, (name, _) in enumerate(layout.variables):
+        e = ps_state.get(name)
+        want = list(slot_names(layout.kinds[i], layout.hypers[i]))
+        n = layout.numel[i]
+        if e is not None and e["kind"] == layout.kinds[i] and list(e.get("slot_names", ())) == want and \
+                int(np.prod(e["shape"])) == n and len(e["slots"]) == len(want) and \
+                all(t.numel() == n for t in e["slots"]):
+            out.append(list(e["slots"]))
+        else:
+            out.append(None)
+            fresh.append(name)
+    if fresh:
+        logger.warning("parameter-server optimizer state of %s does not match the checkpoint; starting it fresh",
+                       ", ".join(fresh))
+    return out
+
+
+def init_slots(layout: Layout, region, ps_state: Optional[Dict[str, dict]] = None) -> None:
+    """The chief's initialisation of every variable's optimizer slots in zeroed shards: the slots of a checkpoint's
+    `ps_state` where `match_slots` restores them, else the optimizer's initial values (Adagrad's and FTRL's first
+    slot at init_s1, every other slot 0).  region(i, s) as for `export_slots`."""
+    saved = match_slots(ps_state, layout) if ps_state is not None else [None] * len(layout.variables)
+    for i, slots in enumerate(saved):
+        if slots is not None:
+            for s, t in enumerate(slots, 1):
+                region(i, s).copy_(t.reshape(-1))
+        elif layout.kinds[i] in ("adagrad", "ftrl"):
+            region(i, 1).fill_(layout.hypers[i]["init_s1"])
+
+
 def connect_worker(network: nn.Module, opt_desc, cluster, is_chief: bool, global_step: int,
-                   opt_by_name=None) -> WorkerConnection:
-    """Chief: publish the layout, wait for the shards, initialise them.  Worker: wait until ready."""
+                   opt_by_name=None, ps_state: Optional[Dict[str, dict]] = None) -> WorkerConnection:
+    """Chief: publish the layout, wait for the shards, initialise them (the optimizer slots from `ps_state`, a
+    checkpoint's, where they match: `init_slots`).  Worker: wait until ready."""
     client = _task_commons.TaskClient.from_current()
     kv = client.kv
     n_ps = len(cluster.spec["ps"])
@@ -281,8 +342,7 @@ def connect_worker(network: nn.Module, opt_desc, cluster, is_chief: bool, global
         with torch.no_grad():
             for i, (_, p) in enumerate(named):
                 conn._region(i).copy_(p.detach().reshape(-1).float().cpu())
-                if layout.kinds[i] in ("adagrad", "ftrl"):
-                    conn._region(i, 1).fill_(layout.hypers[i]["init_s1"])
+            init_slots(layout, conn._region, ps_state)
         shards[0].set_global_step(global_step)
         kv[KV_READY] = b"1"
         logger.info("parameter servers initialised: %d variables on %d ps", len(names), n_ps)

@@ -335,6 +335,12 @@ class HbmConnection:
                 p.copy_(self.remote_tensor(i).view(p.shape))
         return network.state_dict()
 
+    def optimizer_state(self) -> Dict[str, dict]:
+        """Every variable's optimizer slots, read from the ps ranks (ps.export_slots).  The bf16 shadows are derived
+        from the masters and are not part of it."""
+        torch.cuda.synchronize()
+        return ps_cpu.export_slots(self.layout, self.remote_tensor)
+
 
 def _make_bag_forward(conn: HbmConnection, idx: int, mod: nn.EmbeddingBag):
     combiner = getattr(mod, "combiner", mod.mode)
@@ -876,7 +882,9 @@ def _try_fuse_first_layer(conn: HbmConnection, network: nn.Module) -> bool:
 # connection set-up (collective over the cluster)
 # ---------------------------------------------------------------------------------------------
 def connect_worker(network: nn.Module, opt_desc, cluster, is_chief: bool, global_step: int,
-                   opt_by_name=None) -> HbmConnection:
+                   opt_by_name=None, ps_state: Optional[Dict[str, dict]] = None) -> HbmConnection:
+    """Chief: publish the layout, initialise the shards (the optimizer slots from `ps_state`, a checkpoint's, where
+    they match: ps.init_slots) and their bf16 shadows.  Worker: wait until ready.  Both then install the kernels."""
     if any(getattr(d, "schedule", None) is not None for d in [opt_desc, *(opt_by_name or {}).values()]):
         raise ValueError("the HBM parameter server bakes the learning rate into its push kernels and does not run "
                          "a LearningRateSchedule; use the shared-memory parameter server (TFY_PS_PLANE=shm) or a "
@@ -900,8 +908,7 @@ def connect_worker(network: nn.Module, opt_desc, cluster, is_chief: bool, global
         with torch.no_grad():
             for i, (_, p) in enumerate(named):
                 conn.remote_tensor(i).copy_(p.detach().reshape(-1).float())
-                if layout.kinds[i] in ("adagrad", "ftrl"):
-                    conn.remote_tensor(i, 1).fill_(layout.hypers[i]["init_s1"])
+            ps_cpu.init_slots(layout, conn.remote_tensor, ps_state)
         conn.refresh_shadows()
         header.set_global_step(global_step)
         torch.cuda.synchronize()
