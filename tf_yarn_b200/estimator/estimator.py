@@ -182,12 +182,16 @@ class Estimator:
 
     def _make_optimizer(self, spec: EstimatorSpec):
         desc = self._resolve_opt(spec.optimizer)
-        self._opt_desc = desc
-        named = [(n, p) for n, p in self._network.named_parameters() if p.requires_grad] \
-            if self._network is not None else []
         # per-prefix optimizers (longest prefix wins); self._opt_by_name maps every parameter to its descriptor
         groups = [(pref, self._resolve_opt(o)) for pref, o in (spec.optimizers or {}).items()]
         groups.sort(key=lambda g: -len(g[0]))
+        # refused before any optimizer state is set, so every later train() call refuses it again
+        if any(getattr(d, "gradient_accumulation_steps", None) is not None for d in [desc, *(g for _, g in groups)]):
+            raise ValueError("Estimator does not support gradient_accumulation_steps (neither the local and "
+                             "all-reduce paths nor the parameter servers accumulate gradients): use Model.fit")
+        self._opt_desc = desc
+        named = [(n, p) for n, p in self._network.named_parameters() if p.requires_grad] \
+            if self._network is not None else []
         self._opt_by_name = {}
         buckets = {}
         for n, p in named:

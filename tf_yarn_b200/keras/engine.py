@@ -17,6 +17,10 @@ configuration:
 
 ``EagerTrainEngine`` (CPU plumbing configuration) — plain torch ops, gloo
 all-reduce of the gradients, ``torch.optim`` with the same update formulas.
+
+With ``gradient_accumulation_steps=N`` (Keras 3) the engines count batches, not updates: batch ``s`` adds its
+gradients to an fp32 sum, and batch ``s`` with ``(s + 1) % N == 0`` applies ``sum * fl32(1/N)`` (averaged over the
+ranks) with the learning rate ``schedule(s)`` and Adam's bias correction at ``t = s + 1``, then clears the sum.
 """
 from __future__ import annotations
 
@@ -25,6 +29,7 @@ import ctypes
 import logging
 from typing import Callable, Dict, List, Optional, Sequence, Tuple
 
+import numpy as np
 import torch
 import torch.nn as nn
 
@@ -56,7 +61,13 @@ class EagerTrainEngine:
         self.opt_desc = optimizer
         self.opt = optimizer.to_torch([p for p in net.parameters() if p.requires_grad])
         self._schedule = getattr(optimizer, "schedule", None)
-        self.iterations = 0                 # updates applied (Keras optimizer.iterations): a schedule's step
+        self.accum_steps = getattr(optimizer, "gradient_accumulation_steps", None)
+        if self.accum_steps is not None:
+            # .grad is the accumulator and lives on the module's parameters: a previous fit (whose last gradients
+            # stay there) must not leak into the first update.  load_state_dict puts a saved pending sum back.
+            for p in net.parameters():
+                p.grad = None
+        self.iterations = 0                 # batches trained (Keras optimizer.iterations): a schedule's step
         self.kernel_launches = 0
         self._cw = None                     # class-weight table [C] on the device (None: no class_weight)
         self._wacc = [[0.0, 0.0] for _ in self.weighted_metric_fns]     # epoch sums (sum w*m, sum w)
@@ -77,10 +88,10 @@ class EagerTrainEngine:
                 dist.broadcast(t.data, src=root)
 
     def train_step(self, x, y, w=None) -> Dict[str, torch.Tensor]:
-        import torch.distributed as dist
         self.net.train()
         x, y = _to_device_batch(x, self.device), _to_device_batch(y, self.device)
-        self.opt.zero_grad(set_to_none=False)
+        if self.accum_steps is None:
+            self.opt.zero_grad(set_to_none=False)
         out = self.net(x)
         sw = None
         if w is None and self._cw is None:
@@ -88,22 +99,9 @@ class EagerTrainEngine:
         else:
             sw = weighting.sample_weights(y, w.to(self.device) if w is not None else None, self._cw)
             loss = weighting.weighted_loss(loss_mod.per_sample(self.loss_fn), y, out, sw)
-        loss.backward()
-        world = self._world()
-        if world > 1:
-            grads = [p.grad for p in self.net.parameters() if p.grad is not None]
-            flat = torch.cat([g.reshape(-1) for g in grads])
-            dist.all_reduce(flat)
-            flat /= world
-            o = 0
-            for g in grads:
-                g.copy_(flat[o:o + g.numel()].view_as(g))
-                o += g.numel()
-        if self._schedule is not None:
-            lr = float(self._schedule(self.iterations))
-            for g in self.opt.param_groups:
-                g["lr"] = lr
-        self.opt.step()
+        loss.backward()              # with accumulation: .grad += this batch's gradients (fp32, in batch order)
+        if self.accum_steps is None or (self.iterations + 1) % self.accum_steps == 0:
+            self._apply_gradients()
         self.iterations += 1
         logs = {"loss": loss.detach()}
         with torch.no_grad():
@@ -121,6 +119,51 @@ class EagerTrainEngine:
                 acc[0] += float(num)
                 acc[1] += float(den)
         return logs
+
+    def _apply_gradients(self) -> None:
+        """The update of batch ``self.iterations``: the gradients averaged over the ranks (and, accumulating, the sum
+        of the last N batches scaled by fl32(1/N)), the learning rate at ``iterations``; then, accumulating, the sum
+        is cleared."""
+        import torch.distributed as dist
+        world = self._world()
+        if world > 1:
+            grads = [p.grad for p in self.net.parameters() if p.grad is not None]
+            flat = torch.cat([g.reshape(-1) for g in grads])
+            dist.all_reduce(flat)
+            flat /= world
+            o = 0
+            for g in grads:
+                g.copy_(flat[o:o + g.numel()].view_as(g))
+                o += g.numel()
+        if self._schedule is not None:
+            lr = float(self._schedule(self.iterations))
+            for g in self.opt.param_groups:
+                g["lr"] = lr
+        if self.accum_steps is not None:
+            scale = float(np.float32(1.0 / self.accum_steps))
+            for p in self.net.parameters():
+                if p.grad is not None:
+                    p.grad.mul_(scale)
+            self._align_adam_step()
+        self.opt.step()
+        if self.accum_steps is not None:
+            self.opt.zero_grad(set_to_none=False)
+
+    def _align_adam_step(self) -> None:
+        """Keras 3 applies the update of batch ``s`` with Adam's bias correction at ``t = s + 1`` (``iterations``
+        counts batches); ``torch.optim.Adam`` counts its own steps, so its counter is set to ``s`` before it adds 1."""
+        if not isinstance(self.opt, (torch.optim.Adam, torch.optim.AdamW)):
+            return
+        from torch.optim.optimizer import _get_scalar_dtype
+        for grp in self.opt.param_groups:
+            for p in grp["params"]:
+                st = self.opt.state[p]
+                if not st:                  # the lazy initialisation of torch.optim.Adam, with the step set
+                    st["exp_avg"] = torch.zeros_like(p, memory_format=torch.preserve_format)
+                    st["exp_avg_sq"] = torch.zeros_like(p, memory_format=torch.preserve_format)
+                    if grp.get("amsgrad"):
+                        st["max_exp_avg_sq"] = torch.zeros_like(p, memory_format=torch.preserve_format)
+                st["step"] = torch.tensor(float(self.iterations), dtype=_get_scalar_dtype())
 
     @property
     def stateful_metrics(self) -> List[Metric]:
@@ -151,13 +194,35 @@ class EagerTrainEngine:
     def sync_params_to_module(self) -> None:
         pass
 
+    def _pending_accumulation(self) -> bool:
+        return self.accum_steps is not None and self.iterations % self.accum_steps != 0
+
     def state_dict(self) -> dict:
-        return {"kind": "eager", "optimizer": self.opt.state_dict(), "iterations": self.iterations}
+        """With batches accumulated since the last update, the state carries their sum (``grad_accum``).  A
+        checkpoint is written by one rank alone, without a collective, so over several ranks it holds that rank's part
+        of the sum only.  A resume puts it back on rank 0 and zeros on the others, so the first update after it lacks
+        the other ranks' pending batches while still dividing by ``world * N`` (a warning says so at save time;
+        docs/Migration.md states it).  The GPU engines gather every rank's part and have no such gap."""
+        st = {"kind": "eager", "optimizer": self.opt.state_dict(), "iterations": self.iterations}
+        if self._pending_accumulation():
+            if self._world() > 1:
+                logger.warning("checkpoint in the middle of a gradient accumulation over %d ranks: only this rank's "
+                               "pending gradients are saved, so the first update after resuming from it leaves out "
+                               "the other ranks' pending batches", self._world())
+            st["grad_accum"] = [p.grad.detach().clone() if p.grad is not None else None
+                                for p in self.net.parameters() if p.requires_grad]
+        return st
 
     def load_state_dict(self, state: dict) -> None:
         if state.get("kind") == "eager":
             self.opt.load_state_dict(state["optimizer"])
             self.iterations = int(state.get("iterations", 0))
+            if self.accum_steps is not None:
+                pending = state.get("grad_accum")
+                first = self._world() == 1 or _rank() == 0
+                for i, p in enumerate(p for p in self.net.parameters() if p.requires_grad):
+                    g = pending[i] if (pending is not None and first) else None
+                    p.grad = g.to(p.device).clone() if g is not None else torch.zeros_like(p)
 
     # fit() drives the eager engine synchronously
     pipelined = False
@@ -167,6 +232,7 @@ class GraphTrainEngine:
     """CUDA-graph train step with the fused reduce-scatter/optimizer/all-gather kernel."""
 
     pipelined = True
+    accum_steps: Optional[int] = None        # the optimizer's gradient_accumulation_steps
 
     def __init__(self, net: nn.Module, loss_fn: Callable, optimizer, metric_fns: Sequence[Tuple[str, Callable]],
                  device: torch.device, distributed: bool, example_x, example_y,
@@ -195,8 +261,14 @@ class GraphTrainEngine:
         # (O, kh, kw, I) so that the parameter seen by cuDNN is a channels_last view of its slice
         init = [p.detach().float().permute(0, 2, 3, 1).contiguous() if p.dim() == 4 else p.detach().float()
                 for p in self.params]
+        # gradient_accumulation_steps: two captured graphs per input slot, an accumulation batch (forward, backward,
+        # accumulate + advance the step counter) and an update batch (forward, backward, accumulate, fused step over
+        # the accumulator); the host picks one from its batch counter
+        self.accum_steps = getattr(optimizer, "gradient_accumulation_steps", None)
+        self._batch = 0                      # batches launched (the device step counter, which counts batches)
         self.fused = FusedShardedOptimizer(comm, [tuple(t.shape) for t in init], optimizer.to_spec(),
-                                           param_dtype=compute_dtype, grad_dtype=compute_dtype, zero_grads=True)
+                                           param_dtype=compute_dtype, grad_dtype=compute_dtype, zero_grads=True,
+                                           accumulation_steps=self.accum_steps)
         self.fused.init_from(init, broadcast_root=None)
         net.to(compute_dtype)
         # re-point the module's parameters / grads at the flat symmetric buffers
@@ -218,7 +290,10 @@ class GraphTrainEngine:
                                        dtype=torch.float32, device=device)
         self._example = (example_x, example_y)
         self.kernel_launches = 0
-        self._launches_per_step = 1          # the fused K4 kernel
+        self._launches_per_step = 1          # the fused K4 kernel (accumulating: + the accumulate kernel)
+        self._launches_per_accum_step = 1    # accumulating: the accumulate kernel of an accumulation batch
+        if self.accum_steps is not None:
+            self._launches_per_step = 2
         self._captured = False
         # Keras sample weighting.  The weighting mode -- (class_weight, sample_weight) -- is part of the captured
         # graphs: a step in another mode captures them again.  The class-weight table is an engine-owned device
@@ -267,7 +342,21 @@ class GraphTrainEngine:
         pass  # module parameters ARE the flat buffer
 
     # ------------------------------------------------------------------ step body
-    def _forward_backward(self, x, y, w=None) -> None:
+    def _apply_gradients(self, update: bool) -> int:
+        """The end of a step: the fused optimizer step, or -- accumulating -- the accumulate kernel, followed on an
+        update batch by the fused step over the accumulator.  Returns the launches made."""
+        if self.accum_steps is None:
+            self.fused.step()
+            return 1
+        self.fused.accumulate(advance=not update)
+        if update:
+            self.fused.step_accumulated()
+        return 2 if update else 1
+
+    def _next_is_update(self) -> bool:
+        return self.accum_steps is None or (self._batch + 1) % self.accum_steps == 0
+
+    def _forward_backward(self, x, y, w=None, update: bool = True) -> None:
         xin = x
         if torch.is_tensor(xin) and torch.is_floating_point(xin):
             xin = xin.to(self.compute_dtype)
@@ -298,7 +387,7 @@ class GraphTrainEngine:
                     num, den = fn(y, out, sample_weight=sw)
                     self._metric_acc[i, 0] += num
                     self._metric_acc[i, 1] += den
-        self.fused.step()
+        self._apply_gradients(update)
 
     def _capture(self, x, y, w=None) -> None:
         self.net.train()
@@ -321,15 +410,18 @@ class GraphTrainEngine:
         self._fast_copy = hasattr(self._lib, "tfy_memcpy_async")
         fused = self.fused
         snap = (fused.master.clone(), fused.s1.clone(), fused.s2.clone(), fused.flat_params.clone(),
-                fused.hyper.clone(), self._metric_acc.clone())
+                fused.hyper.clone(), self._metric_acc.clone(),
+                fused.flat_acc.clone() if fused.flat_acc is not None else None)
         # stateful metrics allocate their device state on their first update (a warm-up step): empty until then
         metric_snap = [[t.clone() for t in m.state_tensors()] for m in self.stateful_metrics]
         self.stream.wait_stream(torch.cuda.current_stream())
         with torch.cuda.stream(self.stream):
-            for _ in range(3):
-                self._forward_backward(self._static_x, self._static_y, self._staging_w[0])
+            for i in range(3):          # accumulating: an accumulation, an update and an accumulation batch
+                self._forward_backward(self._static_x, self._static_y, self._staging_w[0],
+                                       update=self.accum_steps is None or i == 1)
         self.stream.synchronize()
         self.graphs = [None, None]
+        self._acc_graphs = [None, None]
         if self.use_graph:
             # a CUDAGraph of an older engine being garbage-collected while this stream captures would
             # invalidate the capture (cudaGraphExecDestroy is not allowed then): collect now, pause GC
@@ -339,18 +431,19 @@ class GraphTrainEngine:
             gc.disable()
             try:
                 for slot in range(2):
-                    g = torch.cuda.CUDAGraph()
-                    sx, sy = self._staging[slot]
-                    sw = self._staging_w[slot]
-                    # the graphs never run concurrently (same stream), so they share one memory pool
-                    pool = self.graphs[0].pool() if slot else None
-                    self._capture_slot = slot
-                    with torch.cuda.graph(g, stream=self.stream, pool=pool):
-                        self._forward_backward(sx, sy, sw)
-                        if not self._loss_in_host[slot]:      # (the fast path's head kernel writes it itself)
-                            self._loss_host[slot].copy_(self._loss, non_blocking=True)     # D2H node of the graph
-                    self._capture_slot = None
-                    self.graphs[slot] = g
+                    for update in ((True,) if self.accum_steps is None else (True, False)):
+                        g = torch.cuda.CUDAGraph()
+                        sx, sy = self._staging[slot]
+                        sw = self._staging_w[slot]
+                        # the graphs never run concurrently (same stream), so they share one memory pool
+                        pool = self.graphs[0].pool() if self.graphs[0] is not None else None
+                        self._capture_slot = slot
+                        with torch.cuda.graph(g, stream=self.stream, pool=pool):
+                            self._forward_backward(sx, sy, sw, update)
+                            if not self._loss_in_host[slot]:      # (the fast path's head kernel writes it itself)
+                                self._loss_host[slot].copy_(self._loss, non_blocking=True)  # D2H node of the graph
+                        self._capture_slot = None
+                        (self.graphs if update else self._acc_graphs)[slot] = g
                 self.graph = self.graphs[0]
             finally:
                 if was_enabled:
@@ -359,6 +452,8 @@ class GraphTrainEngine:
         with torch.cuda.stream(self.stream):
             fused.master.copy_(snap[0]); fused.s1.copy_(snap[1]); fused.s2.copy_(snap[2])
             fused.flat_params.copy_(snap[3]); fused.hyper.copy_(snap[4]); self._metric_acc.copy_(snap[5])
+            if snap[6] is not None:
+                fused.flat_acc.copy_(snap[6])
             fused.flat_grads.zero_()
             for m, saved in zip(self.stateful_metrics, metric_snap):
                 if saved:
@@ -423,23 +518,25 @@ class GraphTrainEngine:
         slot, ready = ticket
         st = self.stream
         st.wait_event(ready)
+        update = self._next_is_update()
         if torch.cuda.current_stream() == st:
-            self._launch_on_current(slot)
+            self._launch_on_current(slot, update)
         else:
             with torch.cuda.stream(st):
-                self._launch_on_current(slot)
+                self._launch_on_current(slot, update)
         done = self._done_ev[slot]
         done.record(st)
         self._slot_free[slot] = done          # the slot may be refilled once this step has run
-        self.kernel_launches += self._launches_per_step
+        self._batch += 1
+        self.kernel_launches += self._launches_per_step if update else self._launches_per_accum_step
         return done
 
-    def _launch_on_current(self, slot: int) -> None:
+    def _launch_on_current(self, slot: int, update: bool = True) -> None:
         if self.graph is not None:
-            self.graphs[slot].replay()
+            (self.graphs if update else self._acc_graphs)[slot].replay()
         else:
             sx, sy = self._staging[slot]
-            self._forward_backward(sx, sy, self._staging_w[slot])
+            self._forward_backward(sx, sy, self._staging_w[slot], update)
             self._loss_host[slot].copy_(self._loss, non_blocking=True)
 
     def loss_host(self, slot: int) -> torch.Tensor:
@@ -494,6 +591,12 @@ class GraphTrainEngine:
             dev = self.fused.master.device
             self.fused.load_state({k: (v.to(dev) if torch.is_tensor(v) else v) for k, v in state.items()
                                    if k != "kind"})
+            self._batch = int(state.get("step", 0))
+
+
+def _rank() -> int:
+    import torch.distributed as dist
+    return dist.get_rank() if dist.is_initialized() else 0
 
 
 _solo = {}

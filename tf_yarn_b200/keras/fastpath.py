@@ -264,6 +264,8 @@ class FastSequentialEngine(GraphTrainEngine):
         fused = self.fused
         if fused.zero_grads or fused.param_dtype != torch.bfloat16 or fused.grad_dtype != torch.bfloat16:
             return None
+        if self.accum_steps is not None:             # the overlap role reads the bf16 gradients, not the accumulator
+            return None
         if fused.spec.kind == "rmsprop":             # no overlap role for RMSprop: the trailing step updates everything
             return None
         n_cta = int(self.lib.tfy_conv3x3_c32_wgrad_spare_ctas(B, H, W))
@@ -437,7 +439,7 @@ class FastSequentialEngine(GraphTrainEngine):
 
     # ------------------------------------------------------------------ the step
     @torch.no_grad()
-    def _forward_backward(self, x, y, sw=None) -> None:
+    def _forward_backward(self, x, y, sw=None, update: bool = True) -> None:
         if x.shape[0] != self._resolved_b:
             self._resolve(x.shape[0])
         self._k = 0
@@ -456,9 +458,14 @@ class FastSequentialEngine(GraphTrainEngine):
         if self._ov_gmid:
             # the communication CTAs of the weight-gradient kernel already handled groups [g_mid, end) of every shard
             self.fused.step(shard_groups=(0, self._ov_gmid), advance=True)
+            n_step = 1
         else:
-            self.fused.step()
-        self._launches_per_step = self._k + 1     # our kernels launched per step (library GEMMs excluded)
+            n_step = self._apply_gradients(update)
+        # our kernels launched per step (library GEMMs excluded)
+        if update:
+            self._launches_per_step = self._k + n_step
+        else:
+            self._launches_per_accum_step = self._k + n_step
 
     def _conv_fwd(self, st, sv, x):
         lib, s, bf16 = self.lib, self._s(), torch.bfloat16

@@ -8,6 +8,7 @@ tests/test_gpu_fused_step.py holds the kernel to that reference on the GPU).
 """
 from __future__ import annotations
 
+import numbers
 from typing import Iterable, Optional
 
 import torch
@@ -18,13 +19,26 @@ from tf_yarn_b200.parallel.optspec import OptimizerSpec
 
 class Optimizer:
     """``learning_rate`` is a float or a :class:`~tf_yarn_b200.keras.schedules.LearningRateSchedule`.  A schedule is
-    evaluated at ``optimizer.iterations`` -- the updates already applied -- before every update: on the GPU by the
+    evaluated at ``optimizer.iterations`` -- the batches already trained -- before every update: on the GPU by the
     fused step itself, which writes the next step's rate where it advances its device step counter; on the CPU by
-    the engine.  As in Keras 3, the learning rate of a schedule-driven optimizer cannot be set."""
+    the engine.  As in Keras 3, the learning rate of a schedule-driven optimizer cannot be set.
+
+    ``gradient_accumulation_steps`` (Keras 3) is ``None`` (off) or an integer ``N >= 2``.  ``iterations`` then still
+    counts batches, and for batch ``s = 0, 1, ...`` with gradient ``g_s`` (the batch mean, sample and class weights
+    included):
+
+    * ``acc += g_s``, summed in fp32 in batch order;
+    * if ``(s + 1) % N == 0``, the update applies ``g = acc * fl32(1/N)`` (averaged over the ranks when
+      distributed) with the learning rate ``schedule(s)`` and Adam's bias correction at ``t = s + 1``, then
+      ``acc = 0``;
+    * the weights do not change on the other batches.  A sum not yet applied stays pending across epochs and the
+      end of ``fit``, and a checkpoint carries it.
+    """
     kind = "sgd"
 
-    def __init__(self, learning_rate, **extra):
+    def __init__(self, learning_rate, gradient_accumulation_steps=None, **extra):
         self._learning_rate = learning_rate if schedules.is_schedule(learning_rate) else float(learning_rate)
+        self.gradient_accumulation_steps = _check_accumulation_steps(gradient_accumulation_steps)
         self.distributed = False        # set by hvd.DistributedOptimizer
         self.extra = extra
 
@@ -70,13 +84,26 @@ class Optimizer:
 
     def get_config(self):
         lr = schedules.serialize(self.schedule) if self.schedule is not None else self._learning_rate
-        return {"class_name": type(self).__name__, "learning_rate": lr, **self.extra}
+        cfg = {"class_name": type(self).__name__, "learning_rate": lr, **self.extra}
+        if self.gradient_accumulation_steps is not None:
+            cfg["gradient_accumulation_steps"] = self.gradient_accumulation_steps
+        return cfg
+
+
+def _check_accumulation_steps(n):
+    """``None`` or an integer ``>= 2`` (bools, floats and smaller values are refused, as by Keras 3)."""
+    if n is None:
+        return None
+    if isinstance(n, bool) or not isinstance(n, numbers.Integral) or n < 2:
+        raise ValueError(f"gradient_accumulation_steps must be None or an integer >= 2, got {n!r}")
+    return int(n)
 
 
 class SGD(Optimizer):
     def __init__(self, learning_rate: float = 0.01, momentum: float = 0.0, nesterov: bool = False,
-                 weight_decay: float = 0.0, lr: float = None):
-        super().__init__(lr if lr is not None else learning_rate, momentum=momentum, nesterov=nesterov,
+                 weight_decay: float = 0.0, lr: float = None, gradient_accumulation_steps: int = None):
+        super().__init__(lr if lr is not None else learning_rate, gradient_accumulation_steps, momentum=momentum,
+                         nesterov=nesterov,
                          weight_decay=weight_decay)
         self.momentum, self.nesterov, self.weight_decay = momentum, nesterov, weight_decay
 
@@ -90,8 +117,8 @@ class SGD(Optimizer):
 
 class Adadelta(Optimizer):
     def __init__(self, learning_rate: float = 0.001, rho: float = 0.95, epsilon: float = 1e-7,
-                 weight_decay: float = 0.0, lr: float = None):
-        super().__init__(lr if lr is not None else learning_rate, rho=rho, epsilon=epsilon,
+                 weight_decay: float = 0.0, lr: float = None, gradient_accumulation_steps: int = None):
+        super().__init__(lr if lr is not None else learning_rate, gradient_accumulation_steps, rho=rho, epsilon=epsilon,
                          weight_decay=weight_decay)
         self.rho, self.epsilon, self.weight_decay = rho, epsilon, weight_decay
 
@@ -106,8 +133,9 @@ class Adadelta(Optimizer):
 class Adam(Optimizer):
     def __init__(self, learning_rate: float = 0.001, beta_1: float = 0.9, beta_2: float = 0.999,
                  epsilon: float = 1e-7, weight_decay: float = 0.0, decoupled_weight_decay: bool = False,
-                 lr: float = None):
-        super().__init__(lr if lr is not None else learning_rate, beta_1=beta_1, beta_2=beta_2, epsilon=epsilon,
+                 lr: float = None, gradient_accumulation_steps: int = None):
+        super().__init__(lr if lr is not None else learning_rate, gradient_accumulation_steps, beta_1=beta_1,
+                         beta_2=beta_2, epsilon=epsilon,
                          weight_decay=weight_decay, decoupled_weight_decay=decoupled_weight_decay)
         self.beta_1, self.beta_2, self.epsilon = beta_1, beta_2, epsilon
         self.weight_decay, self.decoupled = weight_decay, decoupled_weight_decay
@@ -130,8 +158,9 @@ class AdamW(Adam):
 
 class Adagrad(Optimizer):
     def __init__(self, learning_rate: float = 0.001, initial_accumulator_value: float = 0.1,
-                 epsilon: float = 1e-7, weight_decay: float = 0.0, lr: float = None):
-        super().__init__(lr if lr is not None else learning_rate,
+                 epsilon: float = 1e-7, weight_decay: float = 0.0, lr: float = None,
+                 gradient_accumulation_steps: int = None):
+        super().__init__(lr if lr is not None else learning_rate, gradient_accumulation_steps,
                          initial_accumulator_value=initial_accumulator_value, epsilon=epsilon,
                          weight_decay=weight_decay)
         self.initial_accumulator_value, self.epsilon, self.weight_decay = \
@@ -154,10 +183,12 @@ class Ftrl(Optimizer):
 
     def __init__(self, learning_rate: float = 0.001, learning_rate_power: float = -0.5,
                  initial_accumulator_value: float = 0.1, l1_regularization_strength: float = 0.0,
-                 l2_regularization_strength: float = 0.0, beta: float = 0.0, lr: float = None):
+                 l2_regularization_strength: float = 0.0, beta: float = 0.0, lr: float = None,
+                 gradient_accumulation_steps: int = None):
         if learning_rate_power != -0.5:
             raise ValueError("Ftrl: only learning_rate_power=-0.5 is implemented")
-        super().__init__(lr if lr is not None else learning_rate, learning_rate_power=learning_rate_power,
+        super().__init__(lr if lr is not None else learning_rate, gradient_accumulation_steps,
+                         learning_rate_power=learning_rate_power,
                          initial_accumulator_value=initial_accumulator_value,
                          l1_regularization_strength=l1_regularization_strength,
                          l2_regularization_strength=l2_regularization_strength, beta=beta)
@@ -211,10 +242,12 @@ class RMSprop(Optimizer):
     kind = "rmsprop"
 
     def __init__(self, learning_rate: float = 0.001, rho: float = 0.9, momentum: float = 0.0, epsilon: float = 1e-7,
-                 centered: bool = False, weight_decay: float = 0.0, lr: float = None):
+                 centered: bool = False, weight_decay: float = 0.0, lr: float = None,
+                 gradient_accumulation_steps: int = None):
         if momentum < 0:
             raise ValueError(f"RMSprop momentum must be >= 0, got {momentum}")
-        super().__init__(lr if lr is not None else learning_rate, rho=rho, momentum=momentum, epsilon=epsilon,
+        super().__init__(lr if lr is not None else learning_rate, gradient_accumulation_steps, rho=rho,
+                         momentum=momentum, epsilon=epsilon,
                          centered=centered, weight_decay=weight_decay)
         self.rho, self.momentum, self.epsilon = rho, momentum, epsilon
         self.centered, self.weight_decay = bool(centered), weight_decay

@@ -1,7 +1,8 @@
 """Keras learning-rate schedules (``keras.optimizers.schedules``).
 
-A schedule maps ``step`` -- the number of updates already applied, Keras's ``optimizer.iterations`` -- to the learning
-rate of the next update.  The formulas are tf.keras 2.13+ / Keras 3's:
+A schedule maps ``step`` -- Keras's ``optimizer.iterations``, the number of batches already trained (the number of
+updates already applied unless the optimizer sets ``gradient_accumulation_steps``) -- to the learning rate of an
+update made at that step.  The formulas are tf.keras 2.13+ / Keras 3's:
 
 * ``ExponentialDecay``: ``initial_learning_rate * decay_rate ** p`` with ``p = step / decay_steps``
   (``floor``-ed when ``staircase``).

@@ -11,8 +11,10 @@
 // The arithmetic is float64, rounded to float once at the end, so the host build of this header and the device agree
 // with a float64 reference to float32 rounding.  Every rate the fused step reads is written by this device function:
 // the one of the first step and of a restored step too (tfy_lr_schedule_sync), so an interrupted run and an
-// uninterrupted one read the same bits whatever the host's libm or FMA contraction would give.  The formulas are tf.keras 2.13+ / Keras 3's, `step` being the
-// number of updates already applied (the module docstring of tf_yarn_b200/keras/schedules.py states each of them).
+// uninterrupted one read the same bits whatever the host's libm or FMA contraction would give.  The formulas are
+// tf.keras 2.13+ / Keras 3's, `step` being Keras's `iterations`: the batches already trained, which are the updates
+// already applied unless gradients are accumulated (the module docstring of tf_yarn_b200/keras/schedules.py states
+// each of them).
 #pragma once
 #include <math.h>
 #include <stdint.h>

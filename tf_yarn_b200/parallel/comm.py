@@ -20,6 +20,9 @@ from tf_yarn_b200.parallel.symm import Rendezvous, SymmArena
 
 _DT = {torch.bfloat16: native.BF16, torch.float32: native.F32}
 
+_vp, _i, _sz = ctypes.c_void_p, ctypes.c_int, ctypes.c_size_t
+native.declare("tfy_grad_accumulate", [_vp, _vp, _i, _sz, _i, _vp, _i, _i, _vp])
+
 # below this many bytes the latency-optimal one-shot kernel wins (one barrier
 # pair + every rank reads everything); above it the 2-phase kernels move 1/N of
 # the data per rank.
@@ -301,12 +304,18 @@ class FusedShardedOptimizer:
     shard (``multimem.ld_reduce``), bf16->fp32 cast and 1/world scaling, the
     optimizer update on the fp32 master shard, and the multicast store of the
     new parameters into every rank's replica (``multimem.st``).
+
+    ``accumulation_steps=N`` (Keras ``gradient_accumulation_steps``) adds ``flat_acc``, an fp32 accumulator of the
+    gradient buffer's layout in the symmetric arena (the same offset on every rank, where the step reads the peers'
+    copies): :meth:`accumulate` adds a batch's gradients into it, and :meth:`step_accumulated` applies
+    ``flat_acc * fl32(1/N)`` (``grad_scale``), averaged over the ranks, and clears it.
     """
 
     def __init__(self, comm: Communicator, shapes: Sequence[Sequence[int]], spec: OptimizerSpec,
                  param_dtype: torch.dtype = torch.bfloat16, grad_dtype: Optional[torch.dtype] = None,
-                 zero_grads: bool = True):
+                 zero_grads: bool = True, accumulation_steps: Optional[int] = None):
         self.comm, self.spec = comm, spec
+        self.accum_steps = accumulation_steps
         self.param_dtype = param_dtype
         self.grad_dtype = grad_dtype or param_dtype
         self.zero_grads = zero_grads
@@ -338,6 +347,11 @@ class FusedShardedOptimizer:
         self._block = hyper_block(spec)
         self._code = launch_code(spec)
         self._hyper_host = self._block.hp
+        self.acc_off, self.flat_acc = None, None
+        if accumulation_steps is not None:
+            self.acc_off, self.flat_acc = arena.empty((self.n,), torch.float32, align=4096)
+            self.flat_acc.zero_()
+            self._hyper_host.grad_scale = 1.0 / accumulation_steps      # rounded to fp32 by the ctypes field
         self.hyper = torch.zeros(ctypes.sizeof(native.HyperBlock), dtype=torch.uint8, device=dev)
         self._push_hyper()
         self._sync_scheduled_lr()
@@ -447,6 +461,35 @@ class FusedShardedOptimizer:
         native.check(rc, "tfy_fused_step")
         c.launches += 1
 
+    def accumulate(self, advance: bool, stream=None) -> None:
+        """``flat_acc += flat_grads`` in fp32 (one launch), clearing the gradients behind it when the optimizer was
+        built with ``zero_grads``.  ``advance``: this batch is not an update, so this launch advances the step counter
+        (and a scheduled learning rate) instead of the fused step."""
+        if self.flat_acc is None:
+            raise ValueError("accumulate() needs an optimizer constructed with accumulation_steps")
+        c = self.comm
+        native.check(c.lib.tfy_grad_accumulate(
+            self.flat_acc.data_ptr(), self.flat_grads.data_ptr(), _DT[self.grad_dtype], self.n, int(self.zero_grads),
+            self.hyper.data_ptr(), int(self.spec.schedule is not None), int(advance), _stream_ptr(stream)),
+            "tfy_grad_accumulate")
+        c.launches += 1
+
+    def step_accumulated(self, stream=None) -> None:
+        """The update of an accumulation: the fused step over ``flat_acc`` (fp32 gradients, scaled by ``grad_scale``
+        = fl32(1/N)), which clears the accumulator behind itself and advances the step counter."""
+        if self.flat_acc is None:
+            raise ValueError("step_accumulated() needs an optimizer constructed with accumulation_steps")
+        c = self.comm
+        native.check(c.lib.tfy_fused_step(
+            c.arena.ctx_ref, native.F32, _DT[self.param_dtype], self._code, c.mode, self.acc_off, self.param_off,
+            self.shard_n, self.master.data_ptr(), self.s1.data_ptr(), self.s2.data_ptr(), self.hyper.data_ptr(),
+            1, self.grid, self.block, _stream_ptr(stream)), "tfy_fused_step")
+        c.launches += 1
+
+    def pending_accumulation(self) -> bool:
+        """True when batches have been accumulated since the last update."""
+        return self.accum_steps is not None and self.step_count % self.accum_steps != 0
+
     def overlap_step(self, g0: int, g1: int, n_cta: int, slot0: int = 960):
         """Descriptor of the fused step of shard-relative groups ``[g0, g1)`` for the communication CTAs of a
         persistent compute kernel (``tfy_conv3x3_c32_wgrad_unpool_ov``): they reduce-scatter, update and
@@ -481,6 +524,14 @@ class FusedShardedOptimizer:
         """Materialise full (unsharded) fp32 master / state tensors on every rank."""
         out = {name: self._gather_full(t) for name, t in self._states()}
         out["step"] = self.step_count
+        if self.pending_accumulation():
+            # the sum of the batches since the last update; over several ranks, the sum of every rank's (a
+            # collective, as the gathers above): a resume puts it on rank 0, so the next update sees the same total
+            # up to the order of the fp32 sums
+            acc = self.flat_acc.clone()
+            if self.comm.world > 1:
+                self.comm.all_reduce([acc], average=False)
+            out["grad_accum"] = acc
         return out
 
     def _gather_full(self, shard: torch.Tensor) -> torch.Tensor:
@@ -502,6 +553,11 @@ class FusedShardedOptimizer:
             if name in ("master", "s1") or name in state:
                 t.copy_(state[name][sl])
         self.flat_params.copy_(state["master"].to(self.flat_params.device).to(self.param_dtype))
+        if self.flat_acc is not None:
+            if "grad_accum" in state and r == 0:
+                self.flat_acc.copy_(state["grad_accum"])
+            else:
+                self.flat_acc.zero_()
         self.set_step_count(int(state.get("step", 0)))
 
     def unflatten(self, full: torch.Tensor) -> List[torch.Tensor]:
