@@ -380,19 +380,31 @@ static inline cudaError_t tfy_launch_pdl_if(bool enable, void (*kernel)(KArgs...
     return cudaLaunchKernelEx(&cfg, kernel, static_cast<KArgs>(args)...);
 }
 
+// The same launch for a kernel whose CTAs run in clusters of cluster.x x cluster.y x cluster.z (the grid a multiple of
+// it); a 1 x 1 x 1 cluster launches without the cluster attribute.
 template <typename... KArgs, typename... Args>
-static inline cudaError_t tfy_launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t s,
-                                         Args... args) {
+static inline cudaError_t tfy_launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 cluster, dim3 block, size_t smem,
+                                         cudaStream_t s, Args... args) {
     cudaLaunchConfig_t cfg;
     memset(&cfg, 0, sizeof(cfg));
     cfg.gridDim = grid;
     cfg.blockDim = block;
     cfg.dynamicSmemBytes = smem;
     cfg.stream = s;
-    cudaLaunchAttribute attr[1];
+    cudaLaunchAttribute attr[2];
     attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
     attr[0].val.programmaticStreamSerializationAllowed = tfy_pdl_enabled() ? 1 : 0;
+    attr[1].id = cudaLaunchAttributeClusterDimension;
+    attr[1].val.clusterDim.x = cluster.x;
+    attr[1].val.clusterDim.y = cluster.y;
+    attr[1].val.clusterDim.z = cluster.z;
     cfg.attrs = attr;
-    cfg.numAttrs = 1;
+    cfg.numAttrs = (cluster.x * cluster.y * cluster.z > 1) ? 2 : 1;
     return cudaLaunchKernelEx(&cfg, kernel, static_cast<KArgs>(args)...);
+}
+
+template <typename... KArgs, typename... Args>
+static inline cudaError_t tfy_launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t s,
+                                         Args... args) {
+    return tfy_launch_pdl(kernel, grid, dim3(1, 1, 1), block, smem, s, args...);
 }

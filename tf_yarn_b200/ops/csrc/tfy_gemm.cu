@@ -15,18 +15,47 @@
 //   warp 4   : TMA producer  -- cp.async.bulk.tensor.2d of a 128x64 A box and a 128x64 B box per
 //              stage (128-byte swizzle), completion on an mbarrier (complete_tx)
 // Pipeline: STAGES-deep ring of {A,B} tiles guarded by full/empty mbarriers.
+//
+// Sub-tiled split-K (slab output only): when tiles x K-slices leave most SMs idle, the FM x FN CTAs of a cluster share
+// one tile -- CTA (cx, cy) owns rows [64 cx, 64 cx + 64) of it when FM = 2 and columns [64 cy, 64 cy + 64) when FN = 2.
+// Each runs, for its rows and columns, the k16 chain the one-tile CTA runs (same wgmma shape along M, same K order,
+// one accumulator from zero), so the slabs are the same bits.  The A rows a CTA needs are shared with the FN CTAs of
+// its cluster row and the B rows with the FM CTAs of its column: each CTA loads 1/FN of its A box and 1/FM of its B
+// box and multicasts them, and a stage is refilled only after the consumers of every CTA of the cluster released it.
 #include "tfy_common.cuh"
 #include "tfy_tma.cuh"
 #include "tfy_wgmma.cuh"
 
 namespace {
 
-constexpr int BM = 128, BN = 128, BK = 64, UMMA_K = 16, STAGES = 4;
-constexpr int A_BYTES = BM * BK * 2, B_BYTES = BN * BK * 2, STAGE_BYTES = A_BYTES + B_BYTES;
+constexpr int BM = 128, BN = 128, BK = 64, UMMA_K = 16;
 constexpr int GEMM_THREADS = 160;
-constexpr int ACC_LD = BN + 4;        // fp32 row pitch of the staged accumulator (conflict-free row reads)
-constexpr size_t SMEM_BYTES = (size_t)STAGES * STAGE_BYTES + (size_t)BM * ACC_LD * 4 + 1024 /*align slack*/ +
-                              256 /*barriers*/;
+constexpr int RING_BYTES = 4 * (BM + BN) * BK * 2;   // four stages of the one-tile CTA
+
+// The shape of one CTA's work when FM x FN CTAs share a 128 x 128 tile.
+template <int FM, int FN>
+struct GemmGeom {
+    static constexpr int CLUSTER = FM * FN;
+    static constexpr int SM = BM / FM, SN = BN / FN;                   // rows of A and of B this CTA multiplies
+    static constexpr int A_BYTES = SM * BK * 2, B_BYTES = SN * BK * 2, STAGE_BYTES = A_BYTES + B_BYTES;
+    static constexpr int STAGES = RING_BYTES / STAGE_BYTES;            // 4 (one tile), 5 (2 x 1), 8 (2 x 2)
+    static constexpr int BOX_ROWS = 128 / CLUSTER;                     // rows of the A and B boxes one CTA loads
+    static constexpr int ACC_LD = SN + 4;     // fp32 row pitch of the staged accumulator (conflict-free row reads)
+    static constexpr size_t SMEM = (size_t)STAGES * STAGE_BYTES + (size_t)SM * ACC_LD * 4 + 1024 /*align slack*/ +
+                                   256 /*barriers*/;
+    static_assert(2 * STAGES * 8 <= 256, "ring barriers overflow their shared-memory slot");
+    static_assert(A_BYTES % 1024 == 0 && (SM / FN) * 128 % 1024 == 0 && (SN / FM) * 128 % 1024 == 0,
+                  "boxes must land on 128-byte-swizzle atoms");
+};
+
+// Optional per-CTA event timeline (tests/gpu/gemm_timeline.py): 16 slots per CTA, slot 0 the CTA's start on the
+// global timer (ns), the others SM-clock deltas from it.  CTA index: x + gridDim.x * (y + gridDim.y * z).
+__device__ long long* g_timeline = nullptr;
+#define G_MARK(k)                                                                                         \
+    do {                                                                                                  \
+        if (g_tl) g_tl[(size_t)(blockIdx.x + gridDim.x * (blockIdx.y + gridDim.y * blockIdx.z)) * 16 + (k)] = \
+            clock64() - g_t0;                                                                             \
+    } while (0)
 
 }  // namespace
 
@@ -48,20 +77,33 @@ struct TfySplitKEpilogue {
 };
 
 // out_mode 0: C (bf16) = act(acc + bias)      out_mode 1: slab blockIdx.z of C32 (fp32) = acc   (split-K partials)
-// out_mode 2: as 1, then the K-slice CTAs of every tile run the fused epilogue above
+// out_mode 2: as 1, then the K-slice CTAs of every tile run the fused epilogue above (one CTA per tile only)
+// FM x FN > 1: a cluster of FM x FN CTAs shares each tile (out_mode 1 only); the grid is (tiles_m FM, tiles_n FN, splits).
+template <int FM, int FN>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
 tfy_gemm_bf16_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b,
                      __nv_bfloat16* __restrict__ C, float* __restrict__ C32, const __nv_bfloat16* __restrict__ bias,
                      int M, int N, int K, int ldc, int relu, int out_mode, int k_tiles_per_split, TfySplitKEpilogue ep) {
+    using Geom = GemmGeom<FM, FN>;
+    constexpr int STAGES = Geom::STAGES, A_BYTES = Geom::A_BYTES, STAGE_BYTES = Geom::STAGE_BYTES, ACC_LD = Geom::ACC_LD;
     extern __shared__ uint8_t smem_raw[];
+    long long* const g_tl = g_timeline;
+    const long long g_t0 = clock64();
+    if (g_tl && threadIdx.x == 0) {
+        unsigned long long ns;
+        asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(ns));
+        g_tl[(size_t)(blockIdx.x + gridDim.x * (blockIdx.y + gridDim.y * blockIdx.z)) * 16] = (long long)ns;
+    }
     uint8_t* smem = tfy_align1024(smem_raw);
     uint8_t* tiles = smem;
-    float* acc_s = reinterpret_cast<float*>(smem + (size_t)STAGES * STAGE_BYTES);     // [BM][ACC_LD]
-    uint64_t* full = reinterpret_cast<uint64_t*>(acc_s + (size_t)BM * ACC_LD);
+    float* acc_s = reinterpret_cast<float*>(smem + (size_t)STAGES * STAGE_BYTES);     // [Geom::SM][ACC_LD]
+    uint64_t* full = reinterpret_cast<uint64_t*>(acc_s + (size_t)Geom::SM * ACC_LD);
     uint64_t* empty = full + STAGES;
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int m0 = blockIdx.x * BM, n0 = blockIdx.y * BN;
+    // this CTA's coordinates in its cluster (cluster rank cx + FM cy) and the first row of A and of B it multiplies
+    const int cx = (int)blockIdx.x % FM, cy = (int)blockIdx.y % FN;
+    const int m0 = (int)blockIdx.x * Geom::SM, n0 = (int)blockIdx.y * Geom::SN;
     const int total_k_tiles = (K + BK - 1) / BK;
     const int kt0 = blockIdx.z * k_tiles_per_split;
     int kt1 = kt0 + k_tiles_per_split;
@@ -73,12 +115,16 @@ tfy_gemm_bf16_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_con
         tfy_prefetch_tensormap(&map_b);
         for (int s = 0; s < STAGES; ++s) {
             tfy_mbar_init(&full[s], 1);
-            tfy_mbar_init(&empty[s], 4);           // one arrival per MMA warp
+            tfy_mbar_init(&empty[s], 4 * Geom::CLUSTER);   // one arrival per MMA warp of every CTA the stage feeds
         }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
-    __syncthreads();
+    if constexpr (Geom::CLUSTER > 1)
+        tfy_cluster_sync<true>();        // the peers' barriers are initialised before anything lands on them
+    else
+        __syncthreads();
     tfy_pdl_sync();                      // upstream grids complete; our dependents may start launching
+    if (threadIdx.x == 0) G_MARK(1);
 
     if (warp == 4) {
         if (tfy_elect_one()) {
@@ -88,23 +134,42 @@ tfy_gemm_bf16_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_con
                 tfy_mbar_wait(&empty[s], ph ^ 1);
                 uint8_t* a_dst = tiles + (size_t)s * STAGE_BYTES;
                 uint8_t* b_dst = a_dst + A_BYTES;
-                tfy_mbar_expect_tx(&full[s], STAGE_BYTES);
+                tfy_mbar_expect_tx(&full[s], STAGE_BYTES);   // including the boxes the peers multicast to us
                 const int k0 = (kt0 + i) * BK;
-                tfy_tma_load_2d(&map_a, &full[s], a_dst, k0, m0);
-                tfy_tma_load_2d(&map_b, &full[s], b_dst, k0, n0);
+                if constexpr (FN == 1) {
+                    tfy_tma_load_2d(&map_a, &full[s], a_dst, k0, m0);
+                } else {                 // our share of the A rows, to every CTA of our cluster row
+                    constexpr int rows = Geom::SM / FN;
+                    uint16_t mask = 0;
+                    for (int y = 0; y < FN; ++y) mask |= (uint16_t)(1u << (cx + FM * y));
+                    tfy_tma_load_2d_multicast(&map_a, &full[s], a_dst + cy * rows * 128, k0, m0 + cy * rows, mask);
+                }
+                if constexpr (FM == 1) {
+                    tfy_tma_load_2d(&map_b, &full[s], b_dst, k0, n0);
+                } else {                 // our share of the B rows, to every CTA of our cluster column
+                    constexpr int rows = Geom::SN / FM;
+                    const uint16_t mask = (uint16_t)(((1u << FM) - 1u) << (FM * cy));
+                    tfy_tma_load_2d_multicast(&map_b, &full[s], b_dst + cx * rows * 128, k0, n0 + cx * rows, mask);
+                }
             }
+        }
+        if constexpr (Geom::CLUSTER > 1) {
+            __syncwarp();
+            tfy_cluster_sync();          // the peers stop arriving on our barriers before this CTA exits
         }
         return;
     }
     {
-        // ---- MMA: the warpgroup accumulates both 64-row halves; a stage is released once the wgmmas of the
+        // ---- MMA: the warpgroup accumulates its 64-row halves; a stage is released once the wgmmas of the
         // NEXT stage are issued and the older group has retired (one group in flight behind the TMA ring)
-        float acc[2][BN / 2];
-        tfy_wg_zero<BN>(acc[0]);
-        tfy_wg_zero<BN>(acc[1]);
+        constexpr int HALVES = Geom::SM / 64;
+        float acc[HALVES][Geom::SN / 2];
+#pragma unroll
+        for (int h = 0; h < HALVES; ++h) tfy_wg_zero<Geom::SN>(acc[h]);
         for (int i = 0; i < n_kt; ++i) {
             const int s = i % STAGES;
             tfy_mbar_wait(&full[s], (i / STAGES) & 1);
+            if (i == 0 && threadIdx.x == 0) G_MARK(2);
             tfy_wg_fence();
             const uint32_t a_addr = tfy_smem_u32(tiles + (size_t)s * STAGE_BYTES);
             const uint64_t bdesc = tfy_wg_desc_sw128(a_addr + A_BYTES);
@@ -112,33 +177,44 @@ tfy_gemm_bf16_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_con
             for (int k = 0; k < BK / UMMA_K; ++k) {
                 // advance 16 bf16 = 32 B along K inside the 128 B swizzle atom: +2 in 16-byte units
 #pragma unroll
-                for (int h = 0; h < 2; ++h)
-                    tfy_wgmma_m64n128<0, 0>(acc[h], tfy_wg_desc_sw128(a_addr + h * 64 * 128) + (uint64_t)(2 * k),
-                                            bdesc + (uint64_t)(2 * k), 1u);
+                for (int h = 0; h < HALVES; ++h) {
+                    const uint64_t adesc = tfy_wg_desc_sw128(a_addr + h * 64 * 128) + (uint64_t)(2 * k);
+                    if constexpr (Geom::SN == 128)
+                        tfy_wgmma_m64n128<0, 0>(acc[h], adesc, bdesc + (uint64_t)(2 * k), 1u);
+                    else
+                        tfy_wgmma_m64n64<0, 0>(acc[h], adesc, bdesc + (uint64_t)(2 * k), 1u);
+                }
             }
             tfy_wg_commit();
             tfy_wg_wait<1>();
-            if (i > 0 && lane == 0) tfy_mbar_arrive(&empty[(i - 1) % STAGES]);
+            if constexpr (Geom::CLUSTER > 1) {   // lane r releases the stage to cluster CTA r
+                if (i > 0 && lane < Geom::CLUSTER) tfy_mbar_arrive_cluster(&empty[(i - 1) % STAGES], lane);
+            } else {
+                if (i > 0 && lane == 0) tfy_mbar_arrive(&empty[(i - 1) % STAGES]);
+            }
         }
         tfy_wg_wait<0>();
-        tfy_wg_store_rows<BN>(acc_s, ACC_LD, acc[0], 0);
-        tfy_wg_store_rows<BN>(acc_s, ACC_LD, acc[1], 64);
+        if (threadIdx.x == 0) G_MARK(3);
+#pragma unroll
+        for (int h = 0; h < HALVES; ++h) tfy_wg_store_rows<Geom::SN>(acc_s, ACC_LD, acc[h], 64 * h);
         asm volatile("bar.sync 1, 128;" ::: "memory");
     }
     {
-        // epilogue: warp q owns rows [32 q, 32 q + 32) of the tile, one row per thread
-        const int quad = warp & 3;
-        const int row = m0 + quad * 32 + lane;
+        // epilogue: FM threads per row of the CTA's tile (one when it is the whole 128-row tile), each storing
+        // Geom::SN / FM consecutive columns
+        constexpr int COLS = Geom::SN / FM;
+        const int r = threadIdx.x / FM, c0 = (threadIdx.x % FM) * COLS;
+        const int row = m0 + r;
         const bool row_ok = row < M;
-        const float* acc_row = acc_s + (size_t)(quad * 32 + lane) * ACC_LD;
+        const float* acc_row = acc_s + (size_t)r * ACC_LD;
 #pragma unroll 1
-        for (int c = 0; c < BN; c += 16) {
+        for (int c = c0; c < c0 + COLS; c += 16) {
             const int n = n0 + c;
             if (!row_ok || n >= N || n_kt <= 0) continue;
             float v[16];
 #pragma unroll
             for (int j = 0; j < 16; j += 4) *reinterpret_cast<float4*>(v + j) = *reinterpret_cast<const float4*>(acc_row + c + j);
-            if (out_mode >= 1) {
+            if (Geom::CLUSTER > 1 || out_mode >= 1) {
                 float* dst = C32 + (size_t)blockIdx.z * M * ldc + (size_t)row * ldc + n;
                 if (n + 16 <= N && (ldc & 3) == 0 && (n & 3) == 0) {
 #pragma unroll
@@ -169,8 +245,13 @@ tfy_gemm_bf16_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_con
                 }
             }
         }
+        if (g_tl) {                                  // every thread of the tile has issued its stores
+            asm volatile("bar.sync 1, 128;" ::: "memory");
+            if (threadIdx.x == 0) G_MARK(4);
+        }
     }
-    if (out_mode == 2) {
+    if constexpr (Geom::CLUSTER > 1) tfy_cluster_sync();
+    if (Geom::CLUSTER == 1 && out_mode == 2) {
         // ---- fused split-K epilogue, spread over ALL K-slice CTAs of the tile ----
         // Every CTA arrives on the tile's counter after its slab stores, waits until all gridDim.z slices have arrived
         // (they are co-resident: the host only selects this mode when the whole grid fits the SMs) and then finishes
@@ -245,9 +326,42 @@ tfy_gemm_bf16_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_con
 // host side
 // ---------------------------------------------------------------------------------------------
 namespace {
-// the operand maps are tfy_tensor_map_bf16_2d: one box is BK columns x BM (= BN) rows
+// the operand maps are tfy_tensor_map_bf16_2d: one box is BK columns x GemmGeom::BOX_ROWS rows
 static_assert(BK == 64 && BM == 128 && BN == 128, "tile shape must match the tensor-map box");
-bool g_attr_set = false;
+
+int sm_count() {
+    static int sms = 0;
+    if (!sms) {
+        int dev = 0;
+        cudaGetDevice(&dev);
+        cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+    }
+    return sms;
+}
+
+// Launches tfy_gemm_bf16_kernel<FM, FN> on (tiles_m, tiles_n, splits) tiles; the tensor maps are built here because
+// their box depends on the split of the tile.
+template <int FM, int FN>
+int launch_gemm(const void* A, const void* B, __nv_bfloat16* C, float* C32, const __nv_bfloat16* bias, int M, int N,
+                int K, int lda, int ldb, int ldc, int relu, int out_mode, int per, int splits, TfySplitKEpilogue ep,
+                cudaStream_t s) {
+    using Geom = GemmGeom<FM, FN>;
+    static bool attr_set = false;
+    if (!attr_set) {
+        if (cudaFuncSetAttribute(tfy_gemm_bf16_kernel<FM, FN>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                 (int)Geom::SMEM) != cudaSuccess)
+            return -5;
+        attr_set = true;
+    }
+    CUtensorMap ma, mb;
+    if (!tfy_tensor_map_bf16_2d(&ma, A, M, K, lda, Geom::BOX_ROWS) ||
+        !tfy_tensor_map_bf16_2d(&mb, B, N, K, ldb, Geom::BOX_ROWS))
+        return -6;
+    const dim3 grid(((M + BM - 1) / BM) * FM, ((N + BN - 1) / BN) * FN, splits);
+    tfy_launch_pdl((tfy_gemm_bf16_kernel<FM, FN>), grid, dim3(FM, FN, 1), dim3(GEMM_THREADS), Geom::SMEM, s, ma, mb, C,
+                   C32, bias, M, N, K, ldc, relu, out_mode, per, ep);
+    return (int)cudaGetLastError();
+}
 }  // namespace
 
 __global__ void __launch_bounds__(256) tfy_splitk_sum_f32_kernel(const float* __restrict__ slabs, float* __restrict__ out,
@@ -265,6 +379,9 @@ __global__ void __launch_bounds__(256) tfy_splitk_sum_f32_kernel(const float* __
 }
 
 extern "C" {
+
+// debug: device buffer of 16 x int64 per CTA receiving the event timeline of the next launches (nullptr = off)
+int tfy_gemm_set_timeline(long long* buf) { return (int)cudaMemcpyToSymbol(g_timeline, &buf, sizeof(buf)); }
 
 // Number of K-slices (= workspace slabs) tfy_gemm_bf16 / tfy_gemm_bf16_splitk_fused run for a requested split_k.
 int tfy_gemm_bf16_splitk_slabs(int K, int split_k) {
@@ -298,14 +415,6 @@ int tfy_gemm_bf16(const void* A, const void* B, void* C, float* C32, const void*
     if ((K & 7) || (lda & 7) || (ldb & 7)) return -2;
     if (((uintptr_t)A & 15) || ((uintptr_t)B & 15)) return -3;
     if (!tfy_tensor_map_encoder()) return -4;
-    if (!g_attr_set) {
-        if (cudaFuncSetAttribute(tfy_gemm_bf16_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMEM_BYTES) !=
-            cudaSuccess)
-            return -5;
-        g_attr_set = true;
-    }
-    CUtensorMap ma, mb;
-    if (!tfy_tensor_map_bf16_2d(&ma, A, M, K, lda) || !tfy_tensor_map_bf16_2d(&mb, B, N, K, ldb)) return -6;
     const int k_tiles = (K + BK - 1) / BK;
     if (split_k < 1) split_k = 1;
     if (split_k > k_tiles) split_k = k_tiles;
@@ -316,11 +425,16 @@ int tfy_gemm_bf16(const void* A, const void* B, void* C, float* C32, const void*
     // the epilogue stores 16 bytes at a time (8 bf16 / 4 floats) whenever the row pitch allows it and a row has 16 columns
     if (N >= 16 && (out_mode == 0 ? ((ldc & 7) == 0 && ((uintptr_t)C & 15)) : ((ldc & 3) == 0 && ((uintptr_t)C32 & 15))))
         return -3;
-    dim3 grid((M + BM - 1) / BM, (N + BN - 1) / BN, split_k);
-    tfy_launch_pdl((tfy_gemm_bf16_kernel), dim3(grid), dim3(GEMM_THREADS), SMEM_BYTES, s, ma, mb, (__nv_bfloat16*)C, C32,
-                                                                (const __nv_bfloat16*)bias, M, N, K, ldc, relu,
-                                                                out_mode, per, TfySplitKEpilogue{});
-    return (int)cudaGetLastError();
+    // slabs of a grid that leaves SMs idle: share each tile among the CTAs of a cluster, as many as still fit one wave
+    const int ctas = ((M + BM - 1) / BM) * ((N + BN - 1) / BN) * split_k;
+    const int sub = out_mode == 1 ? (4 * ctas <= sm_count() ? 4 : 2 * ctas <= sm_count() ? 2 : 1) : 1;
+    const TfySplitKEpilogue ep{};
+    if (sub == 4)
+        return launch_gemm<2, 2>(A, B, nullptr, C32, nullptr, M, N, K, lda, ldb, ldc, 0, 1, per, split_k, ep, s);
+    if (sub == 2)
+        return launch_gemm<2, 1>(A, B, nullptr, C32, nullptr, M, N, K, lda, ldb, ldc, 0, 1, per, split_k, ep, s);
+    return launch_gemm<1, 1>(A, B, (__nv_bfloat16*)C, C32, (const __nv_bfloat16*)bias, M, N, K, lda, ldb, ldc, relu,
+                             out_mode, per, split_k, ep, s);
 }
 
 // Split-K GEMM with the fused epilogue: y[M,N] (bf16) = dropout(act(A . B^T + bias)), mask[M,N] (optional bytes).
@@ -336,14 +450,6 @@ int tfy_gemm_bf16_splitk_fused(const void* A, const void* B, float* acc32, uint3
     // the epilogue reads acc32 and bias 16 bytes at a time and writes the mask 8 bytes at a time
     if (((uintptr_t)acc32 & 15) || ((uintptr_t)bias & 15) || ((uintptr_t)mask & 7)) return -3;
     if (!tfy_tensor_map_encoder()) return -4;
-    if (!g_attr_set) {
-        if (cudaFuncSetAttribute(tfy_gemm_bf16_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMEM_BYTES) !=
-            cudaSuccess)
-            return -5;
-        g_attr_set = true;
-    }
-    CUtensorMap ma, mb;
-    if (!tfy_tensor_map_bf16_2d(&ma, A, M, K, lda) || !tfy_tensor_map_bf16_2d(&mb, B, N, K, ldb)) return -6;
     const int k_tiles = (K + BK - 1) / BK;
     if (split_k < 1) split_k = 1;
     if (split_k > k_tiles) split_k = k_tiles;
@@ -352,19 +458,9 @@ int tfy_gemm_bf16_splitk_fused(const void* A, const void* B, float* acc32, uint3
     TfySplitKEpilogue ep;
     ep.counters = counters; ep.y = (__nv_bfloat16*)y; ep.mask = (uint8_t*)mask; ep.hp = hp;
     ep.drop_rate = drop_rate; ep.seed = seed; ep.ldy = N;
-    dim3 grid((M + BM - 1) / BM, (N + BN - 1) / BN, split_k);
-    {
-        static int sms = 0;
-        if (!sms) {
-            int dev = 0;
-            cudaGetDevice(&dev);
-            cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-        }
-        if ((int)(grid.x * grid.y * grid.z) > sms) return -8;
-    }
-    tfy_launch_pdl((tfy_gemm_bf16_kernel), dim3(grid), dim3(GEMM_THREADS), SMEM_BYTES, s, ma, mb, (__nv_bfloat16*)nullptr,
-                   acc32, (const __nv_bfloat16*)bias, M, N, K, N, relu, 2, per, ep);
-    return (int)cudaGetLastError();
+    if (((M + BM - 1) / BM) * ((N + BN - 1) / BN) * split_k > sm_count()) return -8;
+    return launch_gemm<1, 1>(A, B, nullptr, acc32, (const __nv_bfloat16*)bias, M, N, K, lda, ldb, N, relu, 2, per,
+                             split_k, ep, s);
 }
 
 }  // extern "C"

@@ -23,6 +23,26 @@ __device__ __forceinline__ void tfy_mbar_init(uint64_t* bar, uint32_t count) {
 __device__ __forceinline__ void tfy_mbar_arrive(uint64_t* bar) {
     asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(tfy_smem_u32(bar)) : "memory");
 }
+// Arrival on the mbarrier at bar's offset in the shared memory of cluster CTA `rank` (this CTA's own included).  It
+// releases at CTA scope only: it signals that this thread's async-proxy reads of a stage (wgmma) have retired, and a
+// cluster-scope release would wait for every earlier store of the thread to become visible to the cluster.
+__device__ __forceinline__ void tfy_mbar_arrive_cluster(uint64_t* bar, uint32_t rank) {
+    asm volatile(
+        "{\n\t.reg .b32 ra;\n\t"
+        "mapa.shared::cluster.u32 ra, %0, %1;\n\t"
+        "mbarrier.arrive.shared::cluster.b64 _, [ra];\n\t}"
+        ::"r"(tfy_smem_u32(bar)), "r"(rank)
+        : "memory");
+}
+// Every thread of every CTA of the cluster.  RELAXED: the arrival orders none of the thread's earlier accesses (enough
+// after fence.mbarrier_init, which releases the barrier initialisation itself); otherwise it releases them.
+template <bool RELAXED = false>
+__device__ __forceinline__ void tfy_cluster_sync() {
+    if constexpr (RELAXED)
+        asm volatile("barrier.cluster.arrive.relaxed;\n\tbarrier.cluster.wait.acquire;" ::: "memory");
+    else
+        asm volatile("barrier.cluster.arrive.release;\n\tbarrier.cluster.wait.acquire;" ::: "memory");
+}
 __device__ __forceinline__ void tfy_mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
     asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(tfy_smem_u32(bar)), "r"(bytes)
                  : "memory");
@@ -45,6 +65,17 @@ __device__ __forceinline__ void tfy_tma_load_2d(const CUtensorMap* map, uint64_t
     asm volatile(
         "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
         ::"r"(tfy_smem_u32(dst)), "l"(reinterpret_cast<uint64_t>(map)), "r"(tfy_smem_u32(bar)), "r"(c0), "r"(c1)
+        : "memory");
+}
+// The same box written at dst's offset in the shared memory of every CTA of the cluster whose rank is set in cta_mask,
+// completion counted on the mbarrier at bar's offset in each of them.
+__device__ __forceinline__ void tfy_tma_load_2d_multicast(const CUtensorMap* map, uint64_t* bar, void* dst, int c0,
+                                                          int c1, uint16_t cta_mask) {
+    asm volatile(
+        "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster"
+        " [%0], [%1, {%4, %5}], [%2], %3;"
+        ::"r"(tfy_smem_u32(dst)), "l"(reinterpret_cast<uint64_t>(map)), "r"(tfy_smem_u32(bar)), "h"(cta_mask),
+          "r"(c0), "r"(c1)
         : "memory");
 }
 __device__ __forceinline__ void tfy_tma_load_3d(const CUtensorMap* map, uint64_t* bar, void* dst, int c0, int c1,
@@ -120,11 +151,12 @@ inline bool tfy_tensor_map_bf16(CUtensorMap* map, const void* ptr, cuuint32_t ra
 }
 
 // Row-major [rows, cols] bf16 matrix with leading dimension ld (elements): the K-major GEMM operand map.  One box is
-// 64 columns (one 128-byte swizzle atom) x 128 rows.
-inline bool tfy_tensor_map_bf16_2d(CUtensorMap* map, const void* ptr, uint64_t rows, uint64_t cols, uint64_t ld) {
+// 64 columns (one 128-byte swizzle atom) x box_rows rows.
+inline bool tfy_tensor_map_bf16_2d(CUtensorMap* map, const void* ptr, uint64_t rows, uint64_t cols, uint64_t ld,
+                                   uint32_t box_rows = 128) {
     const cuuint64_t dims[2] = {cols, rows};
     const cuuint64_t strides[1] = {ld * 2};
-    const cuuint32_t box[2] = {64, 128};
+    const cuuint32_t box[2] = {64, box_rows};
     return tfy_tensor_map_bf16(map, ptr, 2, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_128B,
                                CU_TENSOR_MAP_L2_PROMOTION_L2_256B);
 }
