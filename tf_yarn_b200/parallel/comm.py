@@ -115,8 +115,11 @@ class Communicator:
         for t in tensors:
             by_dtype.setdefault(t.dtype, []).append(t)
         for dtype, group in by_dtype.items():
+            if dtype not in _DT and dtype != torch.float16:
+                self._all_reduce_exact(group, average, stream)
+                continue
             if dtype not in _DT:
-                # exotic dtypes go through fp32
+                # fp16 goes through fp32: one rounding of the fp32 sum
                 tmp = [g.float() for g in group]
                 self.all_reduce(tmp, average, stream)
                 for g, x in zip(group, tmp):
@@ -145,6 +148,27 @@ class Communicator:
                 batch.append(t)
                 used += n
             self._flush(batch, dtype, average, stream)
+
+    def _all_reduce_exact(self, group: Sequence[torch.Tensor], average: bool, stream) -> None:
+        """float64 and integer tensors, which fp32 would round (int64 above 2^24, say): every rank's bytes are
+        all-gathered and summed in rank order in the tensor's own dtype, as the CPU plane's gloo sum is.  An average
+        divides by the world size (integers: truncated toward zero)."""
+        div = torch.full((), self.world, dtype=group[0].dtype, device=group[0].device)
+        for t in group:
+            src = t.reshape(-1) if t.is_contiguous() else t.contiguous().view(-1)
+            chunk = max(1, (self.fusion_bytes // self.world) // 16 * 16 // t.element_size())
+            for s in range(0, src.numel(), chunk):
+                piece = src[s:s + chunk]
+                parts = self.all_gather(piece, stream).view(self.world, -1)
+                acc = parts[0].clone()
+                for r in range(1, self.world):
+                    acc += parts[r]
+                if average:
+                    # a device tensor divisor: a true division, not a multiplication by a rounded reciprocal
+                    acc = acc / div if acc.is_floating_point() else torch.div(acc, div, rounding_mode="trunc")
+                piece.copy_(acc)
+            if not t.is_contiguous():
+                t.copy_(src.view_as(t))
 
     def _flush(self, batch: List[torch.Tensor], dtype, average: bool, stream) -> None:
         if not batch:
