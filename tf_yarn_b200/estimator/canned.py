@@ -70,12 +70,12 @@ def _tf_default(opt, tower: str, n_columns: int, combined: bool):
         return opt
     name = opt.lower()
     per_columns = 1.0 / math.sqrt(max(n_columns, 1))
-    if tower == "dnn" and name in ("adagrad", "rmsprop"):
-        cls = kopt.Adagrad if name == "adagrad" else kopt.RMSprop
-        return cls(0.001 if combined else 0.05)
-    if tower == "linear" and name in ("ftrl", "rmsprop"):
-        cls = kopt.Ftrl if name == "ftrl" else kopt.RMSprop
-        return cls(min(0.005 if combined else 0.2, per_columns))
+    by_name = {"adagrad": kopt.Adagrad, "ftrl": kopt.Ftrl, "rmsprop": kopt.RMSprop, "adamax": kopt.Adamax,
+               "nadam": kopt.Nadam}
+    if tower == "dnn" and name in ("adagrad", "rmsprop", "adamax", "nadam"):
+        return by_name[name](0.001 if combined else 0.05)
+    if tower == "linear" and name in ("ftrl", "rmsprop", "adamax", "nadam"):
+        return by_name[name](min(0.005 if combined else 0.2, per_columns))
     return opt
 
 

@@ -44,7 +44,7 @@ KV_READY = "ps/ready"
 
 # optimizer slots per variable (besides the value itself), in their order in the shard
 _SLOT_NAMES = {"sgd": (), "adagrad": ("accumulator",), "adadelta": ("accum_grad", "accum_update"), "adam": ("m", "v"),
-               "adamw": ("m", "v"), "ftrl": ("n", "z")}
+               "adamw": ("m", "v"), "ftrl": ("n", "z"), "adamax": ("m", "u")}
 
 
 def slot_names(kind: str, hyper: Dict[str, float]) -> Tuple[str, ...]:
@@ -192,7 +192,7 @@ class WorkerConnection:
                 lr, p1, p2, eps, wd = h["lr"], h["p1"], h["p2"], h["eps"], h["wd"]
                 if self.schedules[i] is not None:
                     lr = float(self.schedules[i](step))
-                g = g.detach().reshape(-1).float().cpu()
+                g = g0 = g.detach().reshape(-1).float().cpu()
                 w = self._region(i)
                 if wd:
                     g = g + wd * w
@@ -225,6 +225,15 @@ class WorkerConnection:
                         w.sub_(m)
                     else:
                         w.sub_(inc)
+                elif kind == "adamax":         # lazy: rows whose gradient is all zero keep their value and slots
+                    rows = params[name].shape[0] if params[name].dim() > 0 else 1
+                    hit = (g0.view(rows, -1) != 0).any(dim=1)
+                    m, u = self._region(i, 1).view(rows, -1), self._region(i, 2).view(rows, -1)
+                    gr, wr = g.view(rows, -1)[hit], w.view(rows, -1)
+                    t = max(self.global_step(), 0) + 1     # the step being applied, as for Adam
+                    m[hit] = p1 * m[hit] + (1 - p1) * gr
+                    u[hit] = torch.maximum(p2 * u[hit], gr.abs())
+                    wr[hit] = wr[hit] - lr / (1 - p1 ** t) * m[hit] / (u[hit] + eps)
                 elif kind == "adadelta":
                     sq, dx = self._region(i, 1), self._region(i, 2)
                     sq.mul_(p1).addcmul_(g, g, value=1 - p1)
@@ -318,14 +327,25 @@ def init_slots(layout: Layout, region, ps_state: Optional[Dict[str, dict]] = Non
             region(i, 1).fill_(layout.hypers[i]["init_s1"])
 
 
+def refuse_nadam(named, opt_desc, opt_by_name=None) -> None:
+    """Both parameter-server planes refuse Nadam: the running product of its momentum schedule belongs to one
+    optimizer, which asynchronous workers do not share."""
+    for name, _ in named:
+        if (opt_by_name or {}).get(name, opt_desc).to_spec().kind == "nadam":
+            raise ValueError(f"the parameter server does not run Nadam (variable {name!r}): the running product of "
+                             "its momentum schedule belongs to one optimizer, which asynchronous workers do not "
+                             "share; use Adam")
+
+
 def connect_worker(network: nn.Module, opt_desc, cluster, is_chief: bool, global_step: int,
                    opt_by_name=None, ps_state: Optional[Dict[str, dict]] = None) -> WorkerConnection:
     """Chief: publish the layout, wait for the shards, initialise them (the optimizer slots from `ps_state`, a
     checkpoint's, where they match: `init_slots`).  Worker: wait until ready."""
+    named = _named_trainables(network)
+    refuse_nadam(named, opt_desc, opt_by_name)
     client = _task_commons.TaskClient.from_current()
     kv = client.kv
     n_ps = len(cluster.spec["ps"])
-    named = _named_trainables(network)
     names = [n for n, _ in named]
     if is_chief:
         layout = make_layout(named, n_ps, opt_desc, opt_by_name)

@@ -885,6 +885,7 @@ def connect_worker(network: nn.Module, opt_desc, cluster, is_chief: bool, global
                    opt_by_name=None, ps_state: Optional[Dict[str, dict]] = None) -> HbmConnection:
     """Chief: publish the layout, initialise the shards (the optimizer slots from `ps_state`, a checkpoint's, where
     they match: ps.init_slots) and their bf16 shadows.  Worker: wait until ready.  Both then install the kernels."""
+    ps_cpu.refuse_nadam(ps_cpu._named_trainables(network), opt_desc, opt_by_name)
     if any(getattr(d, "schedule", None) is not None for d in [opt_desc, *(opt_by_name or {}).values()]):
         raise ValueError("the HBM parameter server bakes the learning rate into its push kernels and does not run "
                          "a LearningRateSchedule; use the shared-memory parameter server (TFY_PS_PLANE=shm) or a "

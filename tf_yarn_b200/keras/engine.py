@@ -151,18 +151,25 @@ class EagerTrainEngine:
 
     def _align_adam_step(self) -> None:
         """Keras 3 applies the update of batch ``s`` with Adam's bias correction at ``t = s + 1`` (``iterations``
-        counts batches); ``torch.optim.Adam`` counts its own steps, so its counter is set to ``s`` before it adds 1."""
-        if not isinstance(self.opt, (torch.optim.Adam, torch.optim.AdamW)):
+        counts batches); ``torch.optim.Adam`` counts its own steps, so its counter is set to ``s`` before it adds 1.
+        The same holds for Adamax's bias correction and Nadam's momentum schedule."""
+        from tf_yarn_b200.keras.optimizers import TorchAdamax
+        if not isinstance(self.opt, (torch.optim.Adam, torch.optim.AdamW, torch.optim.NAdam, TorchAdamax)):
             return
         from torch.optim.optimizer import _get_scalar_dtype
         for grp in self.opt.param_groups:
             for p in grp["params"]:
                 st = self.opt.state[p]
-                if not st:                  # the lazy initialisation of torch.optim.Adam, with the step set
+                if not st:                  # the lazy initialisation of the optimizer, with the step set
                     st["exp_avg"] = torch.zeros_like(p, memory_format=torch.preserve_format)
-                    st["exp_avg_sq"] = torch.zeros_like(p, memory_format=torch.preserve_format)
+                    if isinstance(self.opt, TorchAdamax):
+                        st["exp_inf"] = torch.zeros_like(p, memory_format=torch.preserve_format)
+                    else:
+                        st["exp_avg_sq"] = torch.zeros_like(p, memory_format=torch.preserve_format)
                     if grp.get("amsgrad"):
                         st["max_exp_avg_sq"] = torch.zeros_like(p, memory_format=torch.preserve_format)
+                    if isinstance(self.opt, torch.optim.NAdam):     # Nadam's product advances on updates only
+                        st["mu_product"] = torch.ones((), dtype=_get_scalar_dtype())
                 st["step"] = torch.tensor(float(self.iterations), dtype=_get_scalar_dtype())
 
     @property

@@ -266,7 +266,7 @@ class FastSequentialEngine(GraphTrainEngine):
             return None
         if self.accum_steps is not None:             # the overlap role reads the bf16 gradients, not the accumulator
             return None
-        if fused.spec.kind == "rmsprop":             # no overlap role for RMSprop: the trailing step updates everything
+        if fused.spec.kind in ("rmsprop", "adamax", "nadam"):   # no overlap role: the trailing step updates everything
             return None
         n_cta = int(self.lib.tfy_conv3x3_c32_wgrad_spare_ctas(B, H, W))
         later = [st for st in self.plan[li + 1:] if st.kind in ("conv", "dense", "head")]

@@ -299,8 +299,91 @@ class TorchRMSprop(torch.optim.Optimizer):
                     p.sub_(inc)
 
 
+class Adamax(Optimizer):
+    """Adamax as ``tf.keras.optimizers.Adamax`` defines it, per element, at update ``t = iterations + 1``::
+
+        m = beta_1 * m + (1 - beta_1) * g
+        u = max(beta_2 * u, |g|)
+        p -= lr / (1 - beta_1^t) * m / (u + epsilon)
+
+    ``torch.optim.Adamax`` puts epsilon inside the max (``max(beta_2 u, |g| + epsilon)``), so the torch rendition is
+    :class:`TorchAdamax`.  ``weight_decay`` is coupled: ``g += weight_decay * p`` before the update."""
+    kind = "adamax"
+
+    def __init__(self, learning_rate: float = 0.001, beta_1: float = 0.9, beta_2: float = 0.999,
+                 epsilon: float = 1e-7, weight_decay: float = 0.0, lr: float = None,
+                 gradient_accumulation_steps: int = None):
+        super().__init__(lr if lr is not None else learning_rate, gradient_accumulation_steps, beta_1=beta_1,
+                         beta_2=beta_2, epsilon=epsilon, weight_decay=weight_decay)
+        self.beta_1, self.beta_2, self.epsilon, self.weight_decay = beta_1, beta_2, epsilon, weight_decay
+
+    def to_spec(self):
+        return OptimizerSpec.adamax(self.learning_rate, self.beta_1, self.beta_2, self.epsilon, self.weight_decay)
+
+    def to_torch(self, params):
+        return TorchAdamax(params, lr=self._lr0, betas=(self.beta_1, self.beta_2), eps=self.epsilon,
+                           weight_decay=self.weight_decay)
+
+
+class TorchAdamax(torch.optim.Optimizer):
+    """torch.optim rendition of the Keras Adamax (epsilon outside the max; see :class:`Adamax`).  Its state has the
+    names of ``torch.optim.Adamax``'s: ``step``, ``exp_avg`` (m) and ``exp_inf`` (u)."""
+
+    def __init__(self, params, lr=1e-3, betas=(0.9, 0.999), eps=1e-7, weight_decay=0.0):
+        super().__init__(params, dict(lr=lr, betas=tuple(betas), eps=eps, weight_decay=weight_decay))
+
+    @torch.no_grad()
+    def step(self, closure=None):
+        for grp in self.param_groups:
+            lr, (b1, b2), eps, wd = grp["lr"], grp["betas"], grp["eps"], grp["weight_decay"]
+            for p in grp["params"]:
+                if p.grad is None:
+                    continue
+                st = self.state[p]
+                if not st:
+                    st["step"] = torch.tensor(0.0)
+                    st["exp_avg"] = torch.zeros_like(p)
+                    st["exp_inf"] = torch.zeros_like(p)
+                st["step"] += 1
+                t = float(st["step"])
+                g = p.grad + wd * p if wd else p.grad
+                m, u = st["exp_avg"], st["exp_inf"]
+                m.mul_(b1).add_(g, alpha=1 - b1)
+                torch.maximum(u * b2, g.abs(), out=u)
+                p.addcdiv_(m, u + eps, value=-lr / (1 - b1 ** t))
+
+
+class Nadam(Optimizer):
+    """Nadam as ``torch.optim.NAdam`` with ``momentum_decay=0.004`` (tf.keras 2's ``schedule_decay``) defines it, per
+    element, at update ``t = iterations + 1``::
+
+        mu_t = beta_1 * (1 - 0.5 * 0.96^(0.004 t));  mu_product_t = mu_product_{t-1} * mu_t
+        m = beta_1 * m + (1 - beta_1) * g
+        v = beta_2 * v + (1 - beta_2) * g^2
+        d = sqrt(v / (1 - beta_2^t)) + epsilon
+        p -= lr (1 - mu_t) / (1 - mu_product_t) * g / d + lr mu_{t+1} / (1 - mu_product_t mu_{t+1}) * m / d
+
+    ``mu_product`` depends on the history of the step counter, so the fused step keeps it in float64 on the device and
+    checkpoints carry it.  ``weight_decay`` is coupled: ``g += weight_decay * p`` before the update."""
+    kind = "nadam"
+
+    def __init__(self, learning_rate: float = 0.001, beta_1: float = 0.9, beta_2: float = 0.999,
+                 epsilon: float = 1e-7, weight_decay: float = 0.0, lr: float = None,
+                 gradient_accumulation_steps: int = None):
+        super().__init__(lr if lr is not None else learning_rate, gradient_accumulation_steps, beta_1=beta_1,
+                         beta_2=beta_2, epsilon=epsilon, weight_decay=weight_decay)
+        self.beta_1, self.beta_2, self.epsilon, self.weight_decay = beta_1, beta_2, epsilon, weight_decay
+
+    def to_spec(self):
+        return OptimizerSpec.nadam(self.learning_rate, self.beta_1, self.beta_2, self.epsilon, self.weight_decay)
+
+    def to_torch(self, params):
+        return torch.optim.NAdam(params, lr=self._lr0, betas=(self.beta_1, self.beta_2), eps=self.epsilon,
+                                 weight_decay=self.weight_decay, momentum_decay=0.004)
+
+
 _BY_NAME = {"sgd": SGD, "adadelta": Adadelta, "adam": Adam, "adamw": AdamW, "adagrad": Adagrad, "ftrl": Ftrl,
-            "rmsprop": RMSprop}
+            "rmsprop": RMSprop, "adamax": Adamax, "nadam": Nadam}
 
 
 def get(identifier) -> Optimizer:

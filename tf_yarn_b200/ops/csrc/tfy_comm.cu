@@ -152,7 +152,7 @@ __global__ void tfy_barrier_kernel(TfyCommCtx c) { tfy_block_barrier(c); }
 // GT: gradient dtype in the symmetric grad buffer, PT: dtype of the replicated
 // compute parameters.  master/s1/s2: local fp32 arrays of shard_n elements
 // (rank r owns elements [r*shard_n, (r+1)*shard_n) of the flat buffers); RMSprop's s2 holds up to two states
-// back to back (tfy_rmsprop_states).
+// back to back (tfy_rmsprop_states).  For Nadam, hp heads a TfyNadamHyperBlock.
 // [g_lo, g_hi): shard-relative groups of 8 elements this launch handles (the whole shard for the classic single
 // launch).  Splitting a step into ranges lets the engine run the update of gradients that are final early (the
 // big Dense kernel) inside the convolution-backward kernel (tfy_overlap_role) while this launch only handles the
@@ -230,6 +230,7 @@ tfy_fused_step_kernel(TfyCommCtx c, uint64_t grad_off, uint64_t param_off, size_
         if (tfy_grid_finish(c, ep) && threadIdx.x == 0 && advance) {
             if constexpr (SCHED) tfy_advance_scheduled_step(hp, step);
             else hp->step = step + 1;
+            if constexpr (OPT == TFY_OPT_NADAM) tfy_nadam_advance(hp, k);
         }
     } else {
         __syncthreads();
@@ -241,6 +242,7 @@ tfy_fused_step_kernel(TfyCommCtx c, uint64_t grad_off, uint64_t param_off, size_
                 if (advance) {
                     if constexpr (SCHED) tfy_advance_scheduled_step(hp, step);
                     else hp->step = step + 1;
+                    if constexpr (OPT == TFY_OPT_NADAM) tfy_nadam_advance(hp, k);
                 }
             }
         }
@@ -382,6 +384,8 @@ static int tfy_fused_step_groups(const TfyCommCtx* c, int grad_dtype, int param_
         else if (opt == TFY_OPT_ADAM) TFY_FS3(GT, PT, TFY_OPT_ADAM); \
         else if (opt == TFY_OPT_FTRL) TFY_FS3(GT, PT, TFY_OPT_FTRL); \
         else if (opt == TFY_OPT_RMSPROP) TFY_FS3(GT, PT, TFY_OPT_RMSPROP); \
+        else if (opt == TFY_OPT_ADAMAX) TFY_FS3(GT, PT, TFY_OPT_ADAMAX); \
+        else if (opt == TFY_OPT_NADAM) TFY_FS3(GT, PT, TFY_OPT_NADAM); \
         else TFY_FS3(GT, PT, TFY_OPT_ADAGRAD);                     \
     } while (0)
     if (grad_dtype == TFY_BF16 && param_dtype == TFY_BF16) TFY_FS2(__nv_bfloat16, __nv_bfloat16);

@@ -6,6 +6,7 @@
 #pragma once
 #include <cuda_runtime.h>
 #include <cuda_bf16.h>
+#include <stddef.h>
 #include <stdint.h>
 #include <stdlib.h>
 #include <string.h>
@@ -33,8 +34,8 @@ struct TfyCommCtx {
 // and the step counter advancing without being re-captured.
 struct TfyOptHyper {
     float lr;
-    float p1;            // Adadelta: rho   | Adam: beta1 | SGD: momentum | Adagrad: initial acc (unused in kernel) | RMSprop: rho
-    float p2;            // Adam: beta2     | SGD: dampening | RMSprop: momentum
+    float p1;            // Adadelta: rho   | Adam, Adamax, Nadam: beta1 | SGD: momentum | Adagrad: initial acc (unused in kernel) | RMSprop: rho
+    float p2;            // Adam, Adamax, Nadam: beta2 | SGD: dampening | RMSprop: momentum
     float eps;
     float weight_decay;
     float grad_scale;    // multiplied into the (already averaged) gradient, e.g. 1/loss_scale
@@ -51,6 +52,19 @@ struct TfyHyperBlock {
     TfyLrSchedule sched;
 };
 
+// Nadam's hyper block: TfyHyperBlock's layout followed by the running product of its momentum schedule,
+// mu_product = mu_1 * ... * mu_t after t updates (1 before the first).  It depends on the history of the step counter
+// and device and host pow differ, so it is kept on the device in float64 rather than rebuilt from t: every CTA of a
+// step reads it with lr, and the thread that advances hp.step writes the next one (tfy_nadam_advance).
+struct TfyNadamHyperBlock {
+    TfyOptHyper hp;
+    TfyLrSchedule sched;
+    double mu_product;
+};
+static_assert(offsetof(TfyNadamHyperBlock, sched) == offsetof(TfyHyperBlock, sched) &&
+                  sizeof(TfyHyperBlock) == offsetof(TfyNadamHyperBlock, mu_product),
+              "a Nadam hyper block starts with a TfyHyperBlock");
+
 // Called by the one thread that advances the step counter of a scheduled step, after every CTA of the step has read
 // hp->lr.
 __device__ __forceinline__ void tfy_advance_scheduled_step(TfyOptHyper* hp, int step) {
@@ -61,7 +75,7 @@ __device__ __forceinline__ void tfy_advance_scheduled_step(TfyOptHyper* hp, int 
 enum TfyDtype { TFY_BF16 = 0, TFY_F32 = 1 };
 enum TfyAlgo { TFY_ALGO_ONESHOT = 0, TFY_ALGO_TWOSHOT = 1, TFY_ALGO_NVLS = 2 };
 enum TfyOpt { TFY_OPT_SGD = 0, TFY_OPT_ADADELTA = 1, TFY_OPT_ADAM = 2, TFY_OPT_ADAGRAD = 3, TFY_OPT_FTRL = 4,
-               TFY_OPT_RMSPROP = 5 };
+               TFY_OPT_RMSPROP = 5, TFY_OPT_ADAMAX = 6, TFY_OPT_NADAM = 7 };
 // Or-ed into the `opt` code of a fused-step launch: `hp` heads a TfyHyperBlock and the step evaluates its schedule.
 // The bit selects separate instantiations, so the kernels of a constant learning rate carry no schedule code.
 #define TFY_OPT_LR_SCHEDULE 0x100

@@ -122,6 +122,12 @@ __device__ __forceinline__ void tfy_opt_update_rt(int opt_rt, float& p, float g,
         s2 += g - (sq_new - tfy_sqrt_approx(s1)) * tfy_div_approx(p, lr);
         s1 = n_new;
         p = fabsf(s2) <= p1 ? 0.f : -tfy_div_approx(s2 - copysignf(p1, s2), tfy_div_approx(eps + sq_new, lr) + 2.f * p2);
+    } else if (opt == TFY_OPT_ADAMAX) {
+        // tf.keras Adamax: s1 = m, s2 = u (exponentially weighted infinity norm), epsilon outside the max
+        g += wd * p;
+        s1 = p1 * s1 + (1.f - p1) * g;
+        s2 = fmaxf(p2 * s2, fabsf(g));
+        p -= lr_bc1 * tfy_div_approx(s1, s2 + eps);
     } else {  // Adagrad
         g += wd * p;
         s1 += g * g;
@@ -171,6 +177,8 @@ struct TfyStepConsts {
     float lr, p1, p2, eps, wd, gscale, lr_bc1, bc2_rsqrt;
     int flags;
     bool first_step;
+    float lr_mu;          // Nadam: lr mu_{t+1} / (1 - mu_product_t mu_{t+1}), the coefficient of m
+    double mu_product;    // Nadam: mu_product_t, which the thread that advances the step stores (tfy_nadam_advance)
 };
 
 __device__ __forceinline__ TfyStepConsts tfy_step_consts(const TfyOptHyper* hp, int world, int opt) {
@@ -184,9 +192,38 @@ __device__ __forceinline__ TfyStepConsts tfy_step_consts(const TfyOptHyper* hp, 
         const float t = (float)(step + 1);
         k.lr_bc1 = k.lr / (1.f - powf(k.p1, t));
         k.bc2_rsqrt = rsqrtf(1.f - powf(k.p2, t));
+    } else if (opt == TFY_OPT_ADAMAX) {
+        const float t = (float)(step + 1);
+        k.lr_bc1 = k.lr / (1.f - powf(k.p1, t));
+    } else if (opt == TFY_OPT_NADAM) {
+        // torch.optim.NAdam with momentum_decay = 0.004: mu_t = beta1 (1 - 0.5 * 0.96^(0.004 t)); lr_bc1 is the
+        // coefficient of g, lr (1 - mu_t) / (1 - mu_product_t), and lr_mu that of m
+        const float t = (float)(step + 1);
+        k.bc2_rsqrt = rsqrtf(1.f - powf(k.p2, t));
+        const double b1 = k.p1, tt = (double)step + 1.0;
+        const double mu = b1 * (1.0 - 0.5 * pow(0.96, 0.004 * tt));
+        const double mu_next = b1 * (1.0 - 0.5 * pow(0.96, 0.004 * (tt + 1.0)));
+        k.mu_product = reinterpret_cast<const TfyNadamHyperBlock*>(hp)->mu_product * mu;
+        k.lr_bc1 = (float)((double)k.lr * (1.0 - mu) / (1.0 - k.mu_product));
+        k.lr_mu = (float)((double)k.lr * mu_next / (1.0 - k.mu_product * mu_next));
     }
     k.first_step = (step == 0);
     return k;
+}
+
+// Nadam (torch.optim.NAdam, momentum_decay = 0.004; tf.keras 2's schedule_decay): s1 = m, s2 = v,
+// d = sqrt(v / (1 - beta2^t)) + eps, p -= (lr_bc1 g + lr_mu m) / d with the coefficients of tfy_step_consts.
+__device__ __forceinline__ void tfy_nadam_update(float& p, float g, float& s1, float& s2, const TfyStepConsts& k) {
+    g += k.wd * p;
+    s1 = k.p1 * s1 + (1.f - k.p1) * g;
+    s2 = k.p2 * s2 + (1.f - k.p2) * g * g;
+    const float d = tfy_sqrt_approx(s2) * k.bc2_rsqrt + k.eps;
+    p -= tfy_div_approx(k.lr_bc1 * g + k.lr_mu * s1, d);
+}
+
+// Called by the thread that advances hp.step of a Nadam step, after every CTA has read the product (tfy_step_consts)
+__device__ __forceinline__ void tfy_nadam_advance(TfyOptHyper* hp, const TfyStepConsts& k) {
+    reinterpret_cast<TfyNadamHyperBlock*>(hp)->mu_product = k.mu_product;
 }
 
 // State of U groups held in registers between the (early) state loads and the update; THREE adds the third state
@@ -206,7 +243,8 @@ __device__ __forceinline__ void tfy_step_load_state(TfyStepRegs<U, THREE>& r, in
                                                     const float* s1, const float* s2, size_t g_first, size_t stride,
                                                     size_t g_hi, const float* s3 = nullptr) {
     const int opt = OPT_T >= 0 ? OPT_T : opt_rt;
-    const bool two = (opt == TFY_OPT_ADADELTA || opt == TFY_OPT_ADAM || opt == TFY_OPT_FTRL) ||
+    const bool two = (opt == TFY_OPT_ADADELTA || opt == TFY_OPT_ADAM || opt == TFY_OPT_FTRL ||
+                      opt == TFY_OPT_ADAMAX || opt == TFY_OPT_NADAM) ||
                      (opt == TFY_OPT_RMSPROP && s2 != nullptr);
 #pragma unroll
     for (int u = 0; u < U; ++u) {
@@ -241,7 +279,8 @@ __device__ __forceinline__ void tfy_step_batch(const TfyCommCtx& c, int opt_rt, 
     constexpr int NG = 8 / GP::N;  // 16-byte packs per 8 gradient elements
     constexpr int NP = 8 / PP::N;
     const int opt = OPT_T >= 0 ? OPT_T : opt_rt;
-    const bool two = (opt == TFY_OPT_ADADELTA || opt == TFY_OPT_ADAM || opt == TFY_OPT_FTRL) ||
+    const bool two = (opt == TFY_OPT_ADADELTA || opt == TFY_OPT_ADAM || opt == TFY_OPT_FTRL ||
+                      opt == TFY_OPT_ADAMAX || opt == TFY_OPT_NADAM) ||
                      (opt == TFY_OPT_RMSPROP && s2 != nullptr);
     float g[U][8];
 #pragma unroll
@@ -289,6 +328,9 @@ __device__ __forceinline__ void tfy_step_batch(const TfyCommCtx& c, int opt_rt, 
                 zp[0] = make_float4(z[0], z[1], z[2], z[3]);
                 zp[1] = make_float4(z[4], z[5], z[6], z[7]);
             }
+        } else if constexpr (OPT_T == TFY_OPT_NADAM) {
+#pragma unroll
+            for (int q = 0; q < 8; ++q) tfy_nadam_update(p[q], g[u][q] * k.gscale, a[q], b[q], k);
         } else {
 #pragma unroll
             for (int q = 0; q < 8; ++q)
@@ -319,8 +361,9 @@ __device__ __forceinline__ void tfy_step_batch(const TfyCommCtx& c, int opt_rt, 
 // while the compute CTAs run the convolution weight gradient.  Co-residency with the compute CTAs is guaranteed
 // by construction (one CTA per SM, grid <= #SMs), which a second kernel on a side stream cannot promise.
 // bf16 gradients and parameters; optimizer and transport are runtime values (the role is latency-bound).
-// RMSprop has no role instantiation (its third state is not part of TfyOverlapStep): the host never builds a
-// descriptor for it (FusedShardedOptimizer.overlap_step raises) and the trailing launch updates every group.
+// RMSprop, Adamax and Nadam have no role instantiation (RMSprop's third state and Nadam's running product are not
+// part of TfyOverlapStep): the host never builds a descriptor for them (FusedShardedOptimizer.overlap_step raises)
+// and the trailing launch updates every group.
 // Cross-GPU protocol: ONE barrier (slots `slot0 + i`) before the reduction; the all-gathered parameters are
 // published by the exit barrier of the trailing tfy_fused_step launch of the same step (stream order).
 // ---------------------------------------------------------------------------------------------------------

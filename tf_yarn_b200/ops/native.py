@@ -19,7 +19,7 @@ FLAGS_BYTES = MAX_BLOCKS * MAX_RANKS * 4
 
 BF16, F32 = 0, 1
 ALGO_ONESHOT, ALGO_TWOSHOT, ALGO_NVLS = 0, 1, 2
-OPT_SGD, OPT_ADADELTA, OPT_ADAM, OPT_ADAGRAD, OPT_FTRL, OPT_RMSPROP = 0, 1, 2, 3, 4, 5
+OPT_SGD, OPT_ADADELTA, OPT_ADAM, OPT_ADAGRAD, OPT_FTRL, OPT_RMSPROP, OPT_ADAMAX, OPT_NADAM = range(8)
 MODE_LOCAL, MODE_P2P, MODE_NVLS = 0, 1, 2
 
 
@@ -82,6 +82,16 @@ class HyperBlock(ctypes.Structure):
     _fields_ = [
         ("hp", OptHyper),
         ("sched", LrSchedule),
+    ]
+
+
+class NadamHyperBlock(ctypes.Structure):
+    """Mirror of TfyNadamHyperBlock (ops/csrc/tfy_common.cuh): a HyperBlock followed by Nadam's running product
+    ``mu_product`` of its momentum schedule (float64, 1 before the first update), which the fused step advances."""
+    _fields_ = [
+        ("hp", OptHyper),
+        ("sched", LrSchedule),
+        ("mu_product", ctypes.c_double),
     ]
 
 

@@ -290,10 +290,12 @@ class Communicator:
 # ---------------------------------------------------------------------------
 # K4: fused reduce-scatter -> optimizer -> all-gather over flat buffers
 # ---------------------------------------------------------------------------
-def hyper_block(spec: OptimizerSpec, step: int = 0) -> "native.HyperBlock":
+def hyper_block(spec: OptimizerSpec, step: int = 0):
     """The device hyper block of ``spec`` at ``step`` completed updates.  With a learning-rate schedule, ``hp.lr`` is
-    the rate of the next update and the fused step writes each later one where it advances the step counter."""
-    blk = native.HyperBlock()
+    the rate of the next update and the fused step writes each later one where it advances the step counter.  Nadam's
+    block (``native.NadamHyperBlock``) adds the running product of its momentum schedule, 1 before any update: a
+    block for a later step gets it from a checkpoint (``FusedShardedOptimizer.load_state``)."""
+    blk = native.NadamHyperBlock(mu_product=1.0) if spec.kind == "nadam" else native.HyperBlock()
     blk.hp = native.OptHyper(spec.lr, spec.p1, spec.p2, spec.eps, spec.weight_decay, 1.0, step, spec.flags, 0, 0)
     if spec.schedule is not None:
         fields = dict(spec.schedule._device_fields())
@@ -376,7 +378,7 @@ class FusedShardedOptimizer:
             self.acc_off, self.flat_acc = arena.empty((self.n,), torch.float32, align=4096)
             self.flat_acc.zero_()
             self._hyper_host.grad_scale = 1.0 / accumulation_steps      # rounded to fp32 by the ctypes field
-        self.hyper = torch.zeros(ctypes.sizeof(native.HyperBlock), dtype=torch.uint8, device=dev)
+        self.hyper = torch.zeros(ctypes.sizeof(self._block), dtype=torch.uint8, device=dev)
         self._push_hyper()
         self._sync_scheduled_lr()
         self.param_views = [self.flat_params[o:o + n].view(shp) for o, n, shp in
@@ -525,6 +527,9 @@ class FusedShardedOptimizer:
         if self.spec.kind == "rmsprop":
             raise ValueError("overlap_step does not run RMSprop: its states do not fit the descriptor; "
                              "update every group with step()")
+        if self.spec.kind in ("adamax", "nadam"):
+            raise ValueError(f"overlap_step does not run {self.spec.kind.capitalize()}: the communication role has no "
+                             "instantiation for it; update every group with step()")
         c = self.comm
         ov = native.OverlapStep()
         ov.c = c.arena.ctx
@@ -548,6 +553,8 @@ class FusedShardedOptimizer:
         """Materialise full (unsharded) fp32 master / state tensors on every rank."""
         out = {name: self._gather_full(t) for name, t in self._states()}
         out["step"] = self.step_count
+        if self.spec.kind == "nadam":
+            out["mu_product"] = self.mu_product
         if self.pending_accumulation():
             # the sum of the batches since the last update; over several ranks, the sum of every rank's (a
             # collective, as the gathers above): a resume puts it on rank 0, so the next update sees the same total
@@ -583,6 +590,19 @@ class FusedShardedOptimizer:
             else:
                 self.flat_acc.zero_()
         self.set_step_count(int(state.get("step", 0)))
+        if self.spec.kind == "nadam":
+            self._mu_product_bytes().copy_(torch.tensor([float(state.get("mu_product", 1.0))],
+                                                        dtype=torch.float64).view(torch.uint8))
+
+    def _mu_product_bytes(self) -> torch.Tensor:
+        off = native.NadamHyperBlock.mu_product.offset
+        return self.hyper[off:off + 8]
+
+    @property
+    def mu_product(self) -> float:
+        """Nadam: the running product of the momentum schedule after the completed updates (float64, on the
+        device)."""
+        return float(self._mu_product_bytes().view(torch.float64).item())
 
     def unflatten(self, full: torch.Tensor) -> List[torch.Tensor]:
         return [full[o:o + n].view(shp) for o, n, shp in zip(self.offsets, self.numels, self.shapes)]

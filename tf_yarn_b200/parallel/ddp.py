@@ -162,21 +162,24 @@ class DistributedDataParallel(nn.Module):
     def fuse_optimizer(self, kind: str = "sgd", **hyper):
         """Move the optimizer INTO the gradient exchange: every bucket runs the fused reduce-scatter -> update
         -> all-gather kernel (K4: ``multimem.ld_reduce`` of the owned 1/world shard, SGD-momentum / Adam / Adagrad /
-        Adadelta / RMSprop on fp32 master + sharded state, ``multimem.st`` of the new parameters) on the communication
-        stream as soon as its gradients are complete, so the whole optimizer step overlaps backward.  Parameters are
+        Adadelta / RMSprop / Adamax / Nadam on fp32 master + sharded state, ``multimem.st`` of the new parameters) on
+        the communication stream as soon as its gradients are complete, so the whole optimizer step overlaps backward.  Parameters are
         re-pointed at flat symmetric buffers.  Returns an optimizer-shaped object (``step`` / ``zero_grad`` are
         no-ops: by the time backward returns, the update is queued behind it).  Gradient clipping between
         ``backward()`` and ``step()`` is not available in this mode.
 
         ``hyper`` are the keyword arguments of the matching ``OptimizerSpec`` constructor, e.g.
         ``fuse_optimizer("rmsprop", lr=1e-3, rho=0.9, momentum=0.9, eps=1e-7, centered=True)`` for the Keras
-        RMSprop (epsilon inside the square root, lr inside the momentum buffer)."""
+        RMSprop (epsilon inside the square root, lr inside the momentum buffer), or
+        ``fuse_optimizer("adamax" | "nadam", lr=1e-3, beta1=0.9, beta2=0.999, eps=1e-7)`` for the Keras Adamax and
+        Nadam.  Every bucket of a Nadam step keeps its own running product of the momentum schedule."""
         if not self._reducer:
             raise RuntimeError("fuse_optimizer needs the native reducer (CUDA)")
         if self._fused is not None:
             return self._fused
         kinds = {"sgd": OptimizerSpec.sgd, "adam": OptimizerSpec.adam, "adagrad": OptimizerSpec.adagrad,
-                 "adadelta": OptimizerSpec.adadelta, "rmsprop": OptimizerSpec.rmsprop}
+                 "adadelta": OptimizerSpec.adadelta, "rmsprop": OptimizerSpec.rmsprop,
+                 "adamax": OptimizerSpec.adamax, "nadam": OptimizerSpec.nadam}
         if kind not in kinds:
             raise ValueError(f"unknown fused optimizer {kind!r}")
         spec = kinds[kind](**hyper)
@@ -414,6 +417,8 @@ class _FusedOptimizer:
         for b in self._ddp._buckets:
             out["buckets"].append({"master": b.master.cpu(), "s1": b.s1.cpu(), "s2": b.s2.cpu(),
                                    "step": int(b.hyper[24:28].view(torch.int32).item()), "rank": comm.rank})
+            if self.spec.kind == "nadam":
+                out["buckets"][-1]["mu_product"] = float(b.hyper[_MU_OFF:_MU_OFF + 8].view(torch.float64).item())
         return out
 
     def load_state_dict(self, state: dict) -> None:
@@ -435,6 +440,9 @@ class _FusedOptimizer:
                 b.s1.fill_(self.spec.init_s1)
                 b.s2.zero_()
             b.hyper[24:28].copy_(torch.tensor([st["step"]], dtype=torch.int32).view(torch.uint8))
+            if self.spec.kind == "nadam":
+                b.hyper[_MU_OFF:_MU_OFF + 8].copy_(
+                    torch.tensor([float(st.get("mu_product", 1.0))], dtype=torch.float64).view(torch.uint8))
             if self.spec.schedule is not None:      # the rate of the restored step, written by the device function
                 native.check(self._ddp.comm.lib.tfy_lr_schedule_sync(b.hyper.data_ptr(), _stream_ptr()),
                              "tfy_lr_schedule_sync")
@@ -443,6 +451,9 @@ class _FusedOptimizer:
             logging.getLogger(__name__).warning(
                 "rank %d: the optimizer checkpoint holds another rank's shard; fp32 master rebuilt from the restored "
                 "parameters, moments restart on this rank", me)
+
+
+_MU_OFF = native.NadamHyperBlock.mu_product.offset     # Nadam's running product in a bucket's hyper block
 
 
 def wrap_model(model: nn.Module, device, ddp_kwargs: Optional[dict] = None, comm: Optional[Communicator] = None):

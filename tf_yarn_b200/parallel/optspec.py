@@ -1,14 +1,15 @@
 """Fused-optimizer hyper-parameter description (no CUDA dependency)."""
 from __future__ import annotations
 
-OPT_SGD, OPT_ADADELTA, OPT_ADAM, OPT_ADAGRAD, OPT_FTRL, OPT_RMSPROP = 0, 1, 2, 3, 4, 5
+OPT_SGD, OPT_ADADELTA, OPT_ADAM, OPT_ADAGRAD, OPT_FTRL, OPT_RMSPROP, OPT_ADAMAX, OPT_NADAM = range(8)
 
 
 class OptimizerSpec:
     """Hyper-parameters of a fused optimizer (device-independent description)."""
 
     KINDS = {"sgd": OPT_SGD, "adadelta": OPT_ADADELTA, "adam": OPT_ADAM,
-             "adamw": OPT_ADAM, "adagrad": OPT_ADAGRAD, "ftrl": OPT_FTRL, "rmsprop": OPT_RMSPROP}
+             "adamw": OPT_ADAM, "adagrad": OPT_ADAGRAD, "ftrl": OPT_FTRL, "rmsprop": OPT_RMSPROP,
+             "adamax": OPT_ADAMAX, "nadam": OPT_NADAM}
 
     def __init__(self, kind: str, lr: float, p1: float = 0.0, p2: float = 0.0, eps: float = 1e-7,
                  weight_decay: float = 0.0, flags: int = 0, init_s1: float = 0.0):
@@ -33,7 +34,7 @@ class OptimizerSpec:
     def n_states(self) -> int:
         if self.kind == "rmsprop":
             return 1 + (self.p2 > 0) + (self.flags & 1)
-        return 2 if self.kind in ("adadelta", "adam", "adamw", "ftrl") else 1
+        return 2 if self.kind in ("adadelta", "adam", "adamw", "ftrl", "adamax", "nadam") else 1
 
     def s2_numel(self, shard_n: int) -> int:
         """Length of the fp32 ``s2`` buffer of a shard of ``shard_n`` elements: every state after the first, back to
@@ -70,3 +71,16 @@ class OptimizerSpec:
         if momentum < 0:
             raise ValueError(f"RMSprop momentum must be >= 0, got {momentum}")
         return OptimizerSpec("rmsprop", lr, rho, momentum, eps, weight_decay, 1 if centered else 0)
+
+    @staticmethod
+    def adamax(lr=1e-3, beta1=0.9, beta2=0.999, eps=1e-7, weight_decay=0.0):
+        """Adamax as tf.keras defines it: s1 = m, s2 = u = max(beta2 u, |g|), p -= lr / (1 - beta1^t) m / (u + eps)
+        (epsilon outside the max); p1 = beta1, p2 = beta2."""
+        return OptimizerSpec("adamax", lr, beta1, beta2, eps, weight_decay)
+
+    @staticmethod
+    def nadam(lr=1e-3, beta1=0.9, beta2=0.999, eps=1e-7, weight_decay=0.0):
+        """Nadam as torch.optim.NAdam with momentum_decay = 0.004 (tf.keras 2's schedule_decay): s1 = m, s2 = v;
+        p1 = beta1, p2 = beta2.  The running product of its momentum schedule follows the hyper-parameters on the
+        device (TfyNadamHyperBlock)."""
+        return OptimizerSpec("nadam", lr, beta1, beta2, eps, weight_decay)
