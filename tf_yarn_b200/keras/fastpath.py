@@ -1,8 +1,8 @@
 """Fast path of the H100 train engine: explicit forward/backward out of fused kernels.
 
 For ``Sequential`` models made of Conv2D(3x3, valid, stride 1) / MaxPooling2D(2x2) /
-Dropout / Flatten / Dense layers with relu|linear activations and a sparse-categorical
-cross-entropy (from logits) head -- the MNIST-CNN of the headline benchmark, the wine MLP --
+Dropout / Flatten / Dense layers with relu|linear activations and a sparse-categorical or categorical
+(one-hot / soft targets, label smoothing) cross-entropy head -- the MNIST-CNN of the headline benchmark, the wine MLP --
 the step does not go through autograd at all:
 
 * convolutions are wgmma implicit GEMMs (:mod:`ops/csrc/tfy_conv.cu`): conv2 forward with
@@ -46,6 +46,7 @@ native.declare("tfy_bias_relu_pool_drop_fwd", [_vp, _vp, _vp, _vp, _i, _i, _i, _
 native.declare("tfy_pool_drop_relu_bwd", [_vp, _vp, _vp, _f, _i, _i, _i, _i, _vp, _vp, _vp, _vp])
 native.declare("tfy_softmax_xent", [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _vp])
 native.declare("tfy_softmax_xent_weighted", [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _vp])
+native.declare("tfy_softmax_xent_soft", [_vp, _vp, _vp, _f, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _vp])
 native.declare("tfy_conv3x3_c32_pool_fwd", [_vp, _vp, _vp, _vp, _vp, _i, _i, _i, _f, _u32, _vp, _vp])
 native.declare("tfy_conv3x3_c32_dgrad", [_vp, _vp, _vp, _vp, _i, _i, _i, _vp])
 native.declare("tfy_conv3x3_c32_wgrad", [_vp, _vp, _vp, _vp, _vp, _i, _i, _i, _vp])
@@ -68,6 +69,8 @@ native.declare("tfy_dense_head_fused", [_vp, _vp, _vp, _vp, _vp, _f, _vp, _vp, _
                                         _i, _vp])
 native.declare("tfy_dense_head_fused_weighted", [_vp, _vp, _vp, _vp, _vp, _f, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp,
                                                  _vp, _i, _i, _i, _vp, _vp, _vp])
+native.declare("tfy_dense_head_fused_soft", [_vp, _vp, _vp, _vp, _f, _vp, _f, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp,
+                                             _i, _i, _i, _vp, _vp, _vp])
 
 PARTIAL_BLOCKS = 592
 
@@ -89,24 +92,42 @@ class _Stage:
         self.__dict__.update(kw)
 
 
+def head_loss(loss):
+    """``(categorical, label_smoothing, head activation)`` of a loss the fused head computes, or None.  The head computes
+    softmax + cross-entropy from logits: either the loss takes logits and the last layer is linear, or the last layer
+    is a softmax and the loss takes probabilities.  Sparse losses read int64 labels [B], categorical ones fp32 targets
+    [B, C]."""
+    from tf_yarn_b200.keras import losses as kl
+    if isinstance(loss, (kl.SparseCategoricalCrossentropy, kl.CategoricalCrossentropy)):
+        categorical = isinstance(loss, kl.CategoricalCrossentropy)
+        return (categorical, loss.label_smoothing if categorical else 0.0,
+                "linear" if loss.from_logits else "softmax")
+    if isinstance(loss, str) and loss in ("sparse_categorical_crossentropy", "categorical_crossentropy"):
+        return loss == "categorical_crossentropy", 0.0, "softmax"
+    return None
+
+
+def label_dtype(loss) -> Optional[torch.dtype]:
+    """Dtype of the labels the fused head reads for ``loss`` (None: not a fused-head loss)."""
+    head = head_loss(loss)
+    if head is None:
+        return None
+    return torch.float32 if head[0] else torch.int64
+
+
 def build_plan(model) -> Optional[List[_Stage]]:
     """Pattern-match the layer list; None if the model is outside the fast-path grammar."""
-    from tf_yarn_b200.keras import losses as kl
-    loss = model.loss
-    # the fused head computes softmax + cross-entropy from logits: either the loss takes logits and the
-    # last layer is linear, or the last layer is a softmax and the loss takes probabilities
-    if isinstance(loss, kl.SparseCategoricalCrossentropy):
-        want_head_activation = "linear" if loss.from_logits else "softmax"
-    elif loss == "sparse_categorical_crossentropy":
-        want_head_activation = "softmax"
-    else:
+    head = head_loss(model.loss)
+    if head is None:
         return None
+    categorical, _, want_head_activation = head
+    # the head kernel counts the hits of the accuracy that goes with the loss; one weighted accuracy at most
+    accuracies = ("accuracy", "acc", "categorical_accuracy" if categorical else "sparse_categorical_accuracy")
     for m in model._metrics_spec:
-        if m not in ("accuracy", "acc", "sparse_categorical_accuracy"):
+        if m not in accuracies:
             return None
-    # the head kernel counts the (weighted) hits: one weighted accuracy at most
     weighted = getattr(model, "_weighted_metrics_spec", [])
-    if len(weighted) > 1 or any(m not in ("accuracy", "acc", "sparse_categorical_accuracy") for m in weighted):
+    if len(weighted) > 1 or any(m not in accuracies for m in weighted):
         return None
     layers = [ly for ly in model.layers if not isinstance(ly, L.InputLayer)]
     plan: List[_Stage] = []
@@ -204,6 +225,12 @@ class FastSequentialEngine(GraphTrainEngine):
         self._conv_sync = torch.zeros(1024, dtype=torch.int32, device=dev)     # grid barrier of the wgrad kernel
         self._c1_acc = torch.zeros(160 * 320, dtype=torch.float32, device=dev)   # first-layer dW/db per-CTA partials
         self._c1_cnt = torch.zeros(1, dtype=torch.int32, device=dev)
+        # what the head reads: int64 labels [B] (sparse loss), or fp32 targets [B, C] and the label smoothing
+        # (categorical loss: self._ls is not None).  The staging slots hold labels of this dtype, so a batch of another
+        # dtype is converted by the staging copy instead of being misread.
+        categorical, ls, _ = head_loss(model.loss)
+        self._ls = float(ls) if categorical else None
+        self._y_dtype = torch.float32 if categorical else torch.int64
 
     # ------------------------------------------------------------------ helpers
     def _s(self):
@@ -325,9 +352,19 @@ class FastSequentialEngine(GraphTrainEngine):
         return (sw.data_ptr() if sw is not None else None, self._cw.data_ptr() if self._wmode[0] else None,
                 self._s())
 
+    def _head_targets(self, y: torch.Tensor) -> torch.Tensor:
+        """``y`` in the dtype the head reads; a categorical target must be ``[B, C]``."""
+        if self._ls is not None:
+            C = self.plan[-1].layer.units
+            if y.dim() != 2 or y.shape[-1] != C:
+                raise ValueError(f"categorical targets of shape {tuple(y.shape)} do not match the model's output "
+                                 f"(batch, {C}): pass one-hot or soft targets of shape (batch, {C}), or class indices "
+                                 "with SparseCategoricalCrossentropy")
+        return y if y.dtype == self._y_dtype else y.to(self._y_dtype)
+
     def _capture(self, x, y, w=None) -> None:
         self._resolve(x.shape[0])
-        super()._capture(x, y, w)
+        super()._capture(x, self._head_targets(y), w)
         with torch.cuda.stream(self.stream):
             self._stats.zero_()          # warm-up steps must not count in the epoch metrics
         self.stream.synchronize()
@@ -644,12 +681,16 @@ class FastSequentialEngine(GraphTrainEngine):
             prev = self.plan[st.li - 1]
             _, pb = self._wb(prev.layer)
             sv.dh = torch.empty((B, K), dtype=torch.bfloat16, device=x.device)
-            args = (xin.data_ptr(), w.data_ptr(), b.data_ptr(), y.data_ptr(),
-                    below.mask.data_ptr() if below.mask is not None else None, prev.scale, self._loss.data_ptr(),
+            rest = (below.mask.data_ptr() if below.mask is not None else None, prev.scale, self._loss.data_ptr(),
                     self._host_loss_ptr(), self._stats_ptr(), w.grad.data_ptr(), b.grad.data_ptr(), sv.dh.data_ptr(),
                     pb.grad.data_ptr(), self._acc32["head_scratch"].data_ptr(), self._acc32["head_counter"].data_ptr(),
                     B, K, C)
-            if self._wmode == (False, False):
+            args = (xin.data_ptr(), w.data_ptr(), b.data_ptr(), y.data_ptr()) + rest
+            if self._ls is not None:
+                # categorical loss: fp32 targets [B, C] and the label smoothing (null weights: unweighted kernel)
+                self._chk(lib.tfy_dense_head_fused_soft(xin.data_ptr(), w.data_ptr(), b.data_ptr(), y.data_ptr(),
+                                                        self._ls, *rest, *self._weight_ptrs(sw)), "dense_head_fused_soft")
+            elif self._wmode == (False, False):
                 self._chk(lib.tfy_dense_head_fused(*args, s), "dense_head_fused")
             else:
                 # Keras sample / class weights: each row's dlogits scaled by its weight inside the kernel
@@ -657,7 +698,12 @@ class FastSequentialEngine(GraphTrainEngine):
             return
         logits = torch.mm(xin, w.t())
         sv.x, sv.dlogits = xin, torch.empty((B, C), dtype=torch.bfloat16, device=x.device)
-        if self._wmode == (False, False):
+        if self._ls is not None:
+            sw_ptr, cw_ptr, _ = self._weight_ptrs(sw)
+            self._chk(lib.tfy_softmax_xent_soft(logits.data_ptr(), b.data_ptr(), y.data_ptr(), self._ls, sw_ptr, cw_ptr,
+                                                self._loss.data_ptr(), sv.dlogits.data_ptr(), b.grad.data_ptr(),
+                                                self._stats_ptr(), B, C, s), "softmax_xent_soft")
+        elif self._wmode == (False, False):
             self._chk(lib.tfy_softmax_xent(logits.data_ptr(), b.data_ptr(), y.data_ptr(), self._loss.data_ptr(),
                                            sv.dlogits.data_ptr(), b.grad.data_ptr(), self._stats_ptr(), B, C, s),
                       "softmax_xent")

@@ -1,7 +1,11 @@
 """Loss functions (mean over the batch), computed in fp32.
 
 Every built-in loss also has a per-sample form (``per_sample``): one value per sample, shape ``[B]``, the mean over
-the non-batch dimensions.  Keras ``sample_weight`` / ``class_weight`` training reduces it as ``sum(w * l) / B``."""
+the non-batch dimensions.  Keras ``sample_weight`` / ``class_weight`` training reduces it as ``sum(w * l) / B``.
+
+The categorical and binary cross-entropies take Keras' ``label_smoothing`` ``ls`` in [0, 1]: the targets become
+``y (1 - ls) + ls / C`` (C classes) and ``y (1 - ls) + ls / 2`` respectively.  With ``ls = 0`` the targets are used
+as they are."""
 from __future__ import annotations
 
 from typing import Callable, Union
@@ -19,15 +23,35 @@ def sparse_categorical_crossentropy(y_true, y_pred, from_logits: bool = False):
     return F.nll_loss(torch.log(y_pred.clamp_min(1e-7)), y_true)
 
 
-def categorical_crossentropy(y_true, y_pred, from_logits: bool = False):
+def _smoothing(label_smoothing) -> float:
+    ls = float(label_smoothing)
+    if not 0.0 <= ls <= 1.0:
+        raise ValueError(f"label_smoothing must be in [0, 1], got {label_smoothing!r}")
+    return ls
+
+
+def _categorical_targets(y_true, y_pred, label_smoothing):
+    y = y_true.float()
+    ls = _smoothing(label_smoothing)
+    return y * (1.0 - ls) + ls / y_pred.shape[-1] if ls else y
+
+
+def _binary_targets(y_true, label_smoothing):
+    y = y_true.float().reshape(-1)
+    ls = _smoothing(label_smoothing)
+    return y * (1.0 - ls) + 0.5 * ls if ls else y
+
+
+def categorical_crossentropy(y_true, y_pred, from_logits: bool = False, label_smoothing: float = 0.0):
     y_pred = y_pred.float()
+    y_true = _categorical_targets(y_true, y_pred, label_smoothing)
     logp = F.log_softmax(y_pred, dim=-1) if from_logits else torch.log(y_pred.clamp_min(1e-7))
-    return -(y_true.float() * logp).sum(dim=-1).mean()
+    return -(y_true * logp).sum(dim=-1).mean()
 
 
-def binary_crossentropy(y_true, y_pred, from_logits: bool = False):
+def binary_crossentropy(y_true, y_pred, from_logits: bool = False, label_smoothing: float = 0.0):
     y_pred = y_pred.float().reshape(-1)
-    y_true = y_true.float().reshape(-1)
+    y_true = _binary_targets(y_true, label_smoothing)
     if from_logits:
         return F.binary_cross_entropy_with_logits(y_pred, y_true)
     return F.binary_cross_entropy(y_pred.clamp(1e-7, 1 - 1e-7), y_true)
@@ -55,16 +79,17 @@ def sparse_categorical_crossentropy_per_sample(y_true, y_pred, from_logits: bool
     return _per_row(F.nll_loss(torch.log(y_pred.clamp_min(1e-7)), y_true, reduction="none"), batch)
 
 
-def categorical_crossentropy_per_sample(y_true, y_pred, from_logits: bool = False):
+def categorical_crossentropy_per_sample(y_true, y_pred, from_logits: bool = False, label_smoothing: float = 0.0):
     y_pred = y_pred.float()
+    y_true = _categorical_targets(y_true, y_pred, label_smoothing)
     logp = F.log_softmax(y_pred, dim=-1) if from_logits else torch.log(y_pred.clamp_min(1e-7))
-    return _per_row(-(y_true.float() * logp).sum(dim=-1), y_pred.shape[0])
+    return _per_row(-(y_true * logp).sum(dim=-1), y_pred.shape[0])
 
 
-def binary_crossentropy_per_sample(y_true, y_pred, from_logits: bool = False):
+def binary_crossentropy_per_sample(y_true, y_pred, from_logits: bool = False, label_smoothing: float = 0.0):
     batch = y_pred.shape[0]
     y_pred = y_pred.float().reshape(-1)
-    y_true = y_true.float().reshape(-1)
+    y_true = _binary_targets(y_true, label_smoothing)
     if from_logits:
         return _per_row(F.binary_cross_entropy_with_logits(y_pred, y_true, reduction="none"), batch)
     return _per_row(F.binary_cross_entropy(y_pred.clamp(1e-7, 1 - 1e-7), y_true, reduction="none"), batch)
@@ -90,21 +115,27 @@ class SparseCategoricalCrossentropy:
 
 
 class CategoricalCrossentropy:
-    def __init__(self, from_logits: bool = False):
+    """Keras ``CategoricalCrossentropy``: one-hot or soft targets ``[B, C]``, classes on the last axis only."""
+
+    def __init__(self, from_logits: bool = False, label_smoothing: float = 0.0, axis: int = -1):
+        if axis != -1:
+            raise ValueError(f"CategoricalCrossentropy supports axis=-1 only, got axis={axis!r}")
         self.from_logits = from_logits
+        self.label_smoothing = _smoothing(label_smoothing)
         self.__name__ = "categorical_crossentropy"
 
     def __call__(self, y_true, y_pred):
-        return categorical_crossentropy(y_true, y_pred, self.from_logits)
+        return categorical_crossentropy(y_true, y_pred, self.from_logits, self.label_smoothing)
 
 
 class BinaryCrossentropy:
-    def __init__(self, from_logits: bool = False):
+    def __init__(self, from_logits: bool = False, label_smoothing: float = 0.0):
         self.from_logits = from_logits
+        self.label_smoothing = _smoothing(label_smoothing)
         self.__name__ = "binary_crossentropy"
 
     def __call__(self, y_true, y_pred):
-        return binary_crossentropy(y_true, y_pred, self.from_logits)
+        return binary_crossentropy(y_true, y_pred, self.from_logits, self.label_smoothing)
 
 
 _BY_NAME = {
@@ -131,7 +162,10 @@ def per_sample(identifier: Union[str, Callable]) -> Callable:
     fn = get(identifier)
     if isinstance(fn, (SparseCategoricalCrossentropy, CategoricalCrossentropy, BinaryCrossentropy)):
         base, from_logits = _PER_SAMPLE[_BY_NAME[fn.__name__]], fn.from_logits
-        return lambda y_true, y_pred: base(y_true, y_pred, from_logits)
+        if isinstance(fn, SparseCategoricalCrossentropy):
+            return lambda y_true, y_pred: base(y_true, y_pred, from_logits)
+        ls = fn.label_smoothing
+        return lambda y_true, y_pred: base(y_true, y_pred, from_logits, ls)
     for builtin, form in _PER_SAMPLE.items():
         if fn is builtin:
             return form
@@ -164,7 +198,10 @@ def serialize(identifier):
     if isinstance(identifier, str):
         return {"name": identifier}
     if isinstance(identifier, (SparseCategoricalCrossentropy, CategoricalCrossentropy, BinaryCrossentropy)):
-        return {"name": identifier.__name__, "from_logits": identifier.from_logits}
+        cfg = {"name": identifier.__name__, "from_logits": identifier.from_logits}
+        if getattr(identifier, "label_smoothing", 0.0):      # (absent at 0: configs written without it stay as they are)
+            cfg["label_smoothing"] = identifier.label_smoothing
+        return cfg
     return None
 
 
@@ -175,5 +212,7 @@ def deserialize(cfg):
         cls = {"sparse_categorical_crossentropy": SparseCategoricalCrossentropy,
                "categorical_crossentropy": CategoricalCrossentropy,
                "binary_crossentropy": BinaryCrossentropy}[cfg["name"]]
+        if "label_smoothing" in cfg:
+            return cls(from_logits=cfg["from_logits"], label_smoothing=cfg["label_smoothing"])
         return cls(from_logits=cfg["from_logits"])
     return cfg["name"]

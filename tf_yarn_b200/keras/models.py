@@ -79,13 +79,17 @@ _NO_WATCHDOG = _NoWatchdog()
 
 class _ArrayBatches:
     """Batches out of in-memory arrays; pinned host memory when feeding a GPU.  With sample weights ``w`` the
-    batches are ``(x, y, w)`` triples (``w`` fp32 ``[B]``), gathered with the same permutation as x and y."""
+    batches are ``(x, y, w)`` triples (``w`` fp32 ``[B]``), gathered with the same permutation as x and y.  ``y_dtype``:
+    the labels are cast to it once, here (the dtype the train step reads)."""
 
-    def __init__(self, x, y, batch_size: int, shuffle: bool, pin: bool, drop_remainder: bool, w=None):
+    def __init__(self, x, y, batch_size: int, shuffle: bool, pin: bool, drop_remainder: bool, w=None,
+                 y_dtype: Optional[torch.dtype] = None):
         self.x, self.y = _as_tensor(x), (_as_tensor(y) if y is not None else None)
         self.w = _as_tensor(w).reshape(-1).float().contiguous() if w is not None else None
         if self.x.dtype == torch.float64:
             self.x = self.x.float()
+        if self.y is not None and y_dtype is not None and self.y.dtype != y_dtype:
+            self.y = self.y.to(y_dtype)
         self.n = self.x.shape[0]
         if self.w is not None and self.w.shape[0] != self.n:
             raise ValueError(f"sample_weight has {self.w.shape[0]} entries for {self.n} samples")
@@ -410,8 +414,14 @@ class Model:
         self._class_weight_pending = True
         if hasattr(x, "shape") and not hasattr(x, "__next__"):
             on_gpu = (self._device or default_device()).type == "cuda"
+            y_dtype = None
+            if on_gpu:
+                # the fused classifier head reads int64 labels or fp32 targets: narrower integer labels (uint8 from
+                # the Keras MNIST loader, int32) and float64 one-hot targets are cast once, not per step
+                from tf_yarn_b200.keras import fastpath
+                y_dtype = fastpath.label_dtype(self.loss)
             batches = _ArrayBatches(x, y, batch_size or 32, shuffle, pin=on_gpu, drop_remainder=on_gpu,
-                                    w=sample_weight)
+                                    w=sample_weight, y_dtype=y_dtype)
             make_iter = lambda: iter(batches)   # noqa: E731
             if steps_per_epoch is None:
                 steps_per_epoch = len(batches)

@@ -16,6 +16,7 @@
 //   tfy_pool_drop_relu_bwd        its backward (+ dbias[C])
 //   tfy_softmax_xent          logits(+bias) -> mean loss, dlogits = (softmax - onehot)/B, dbias, #correct
 //                             (tfy_softmax_xent_weighted: the same with Keras sample / class weights)
+//                             (tfy_softmax_xent_soft: fp32 one-hot / soft targets with Keras label smoothing)
 //
 // Dropout randomness is counter based: hash(seed, layer salt, optimizer step, element) with the
 // step read from the device-resident TfyOptHyper, so a replayed CUDA graph draws fresh masks.
@@ -444,14 +445,22 @@ tfy_pool_drop_relu_bwd_kernel(const __nv_bfloat16* __restrict__ dp, const uint8_
 // / B (bf16), dbias = column sums of dlogits (bf16), stats[0..n_stats) += [hits, B, sum w*hit, sum w] (n_stats 2 or
 // 4).  Every block-level sum is taken in a fixed order (warp shuffles, then warps in index order; dbias from one
 // partial row per warp), so the result is the same bit for bit on every run.
+//
+// Target modes of the classifier-head kernels.  SPARSE: int64 class labels.  DENSE (Keras CategoricalCrossentropy):
+// fp32 targets y [B, C], one-hot or soft, smoothed as t_c = y_c (1 - ls) + ls / C; with S = sum_c t_c, a row's loss
+// is sum_c t_c (lse - v_c) and its dlogits (p_c S - t_c) w_r / B; its class (hit test, class weight) is argmax_c y_c,
+// ties to the lowest index.  A one-hot row with ls = 0 has t = onehot and S = 1 exactly, and every expression keeps
+// the SPARSE mode's order of operations, so the two modes give the same bits.
 // ---------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(1024)
-tfy_softmax_xent_weighted_kernel(const __nv_bfloat16* __restrict__ logits, const __nv_bfloat16* __restrict__ bias,
-                                 const long long* __restrict__ labels, const float* __restrict__ sample_w,
-                                 const float* __restrict__ class_w, float* __restrict__ loss,
-                                 __nv_bfloat16* __restrict__ dlogits, __nv_bfloat16* __restrict__ dbias,
-                                 float* __restrict__ stats, int n_stats, int B, int C) {
-    tfy_pdl_sync();
+enum : int { TFY_HEAD_SPARSE = 0, TFY_HEAD_DENSE = 1 };
+
+template <int TARGET>
+__device__ __forceinline__ void
+tfy_softmax_xent_body(const __nv_bfloat16* __restrict__ logits, const __nv_bfloat16* __restrict__ bias,
+                      const long long* __restrict__ labels, const float* __restrict__ targets, float ls,
+                      const float* __restrict__ sample_w, const float* __restrict__ class_w, float* __restrict__ loss,
+                      __nv_bfloat16* __restrict__ dlogits, __nv_bfloat16* __restrict__ dbias,
+                      float* __restrict__ stats, int n_stats, int B, int C) {
     extern __shared__ float sm[];  // [C] bias | [warps][C] dbias partials | [warps][4] loss, hits, w*hits, w
     const int warps = blockDim.x >> 5, warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     float* s_bias = sm;
@@ -463,11 +472,26 @@ tfy_softmax_xent_weighted_kernel(const __nv_bfloat16* __restrict__ logits, const
     const float invB = 1.f / (float)B;
     float acc[4] = {0.f, 0.f, 0.f, 0.f};        // loss, hits, w*hits, w
     const int rounds = (B + blockDim.x - 1) / blockDim.x;      // same trip count on every warp: shuffles converge
+    const float keep = 1.f - ls, add = ls / (float)C;            // DENSE: t = y * keep + add
     for (int it = 0; it < rounds; ++it) {
         const int r = it * blockDim.x + threadIdx.x;
         const bool ok = r < B;
         const __nv_bfloat16* row = logits + (size_t)(ok ? r : 0) * C;
-        const int lab = ok ? (int)labels[r] : -1;
+        const float* trow = nullptr;
+        int lab = -1;
+        float S = 0.f;                                           // DENSE: sum of this row's smoothed targets
+        if constexpr (TARGET == TFY_HEAD_SPARSE) {
+            lab = ok ? (int)labels[r] : -1;
+        } else if (ok) {
+            trow = targets + (size_t)r * C;
+            float ym = -INFINITY;
+            lab = 0;
+            for (int c = 0; c < C; ++c) {
+                const float y = trow[c];
+                if (y > ym) { ym = y; lab = c; }
+                S += fmaf(y, keep, add);
+            }
+        }
         float wr = 0.f;
         if (ok) {
             wr = sample_w ? sample_w[r] : 1.f;
@@ -483,12 +507,23 @@ tfy_softmax_xent_weighted_kernel(const __nv_bfloat16* __restrict__ logits, const
         for (int c = 0; c < C; ++c) se += __expf(bf16_to_f(row[c]) + s_bias[c] - mx);
         const float lse = mx + __logf(se);
         const float inv_se = 1.f / se;
+        float lrow = 0.f;                                        // DENSE: sum_c t_c (lse - v_c)
         for (int c = 0; c < C; ++c) {
             const float v = bf16_to_f(row[c]) + s_bias[c];
-            float d = (__expf(v - mx) * inv_se - (c == lab ? 1.f : 0.f)) * invB * wr;
+            float d;
+            if constexpr (TARGET == TFY_HEAD_SPARSE) {
+                d = (__expf(v - mx) * inv_se - (c == lab ? 1.f : 0.f)) * invB * wr;
+            } else {
+                // p S - t as one fma of (e, inv_se S): the SPARSE mode's fma(e, inv_se, -onehot) when S = 1
+                const float t = ok ? fmaf(trow[c], keep, add) : 0.f;
+                d = fmaf(__expf(v - mx), inv_se * S, -t) * invB * wr;
+                lrow = fmaf(t, lse - v, lrow);
+            }
             if (!ok) d = 0.f;
             if (ok) {
-                if (c == lab) acc[0] += wr * (lse - v);
+                if constexpr (TARGET == TFY_HEAD_SPARSE) {
+                    if (c == lab) acc[0] += wr * (lse - v);
+                }
                 dlogits[(size_t)r * C + c] = __float2bfloat16(d);
             }
             if (dbias) {
@@ -497,6 +532,9 @@ tfy_softmax_xent_weighted_kernel(const __nv_bfloat16* __restrict__ logits, const
                 for (int off = 16; off > 0; off >>= 1) t += __shfl_xor_sync(0xffffffffu, t, off);
                 if (lane == 0) s_db[(size_t)warp * C + c] += t;        // one writer per (warp, class)
             }
+        }
+        if constexpr (TARGET == TFY_HEAD_DENSE) {
+            if (ok) acc[0] += wr * lrow;
         }
         if (ok && amax == lab) { acc[1] += 1.f; acc[2] += wr; }
         acc[3] += wr;
@@ -530,6 +568,29 @@ tfy_softmax_xent_weighted_kernel(const __nv_bfloat16* __restrict__ logits, const
         }
 }
 
+__global__ void __launch_bounds__(1024)
+tfy_softmax_xent_weighted_kernel(const __nv_bfloat16* __restrict__ logits, const __nv_bfloat16* __restrict__ bias,
+                                 const long long* __restrict__ labels, const float* __restrict__ sample_w,
+                                 const float* __restrict__ class_w, float* __restrict__ loss,
+                                 __nv_bfloat16* __restrict__ dlogits, __nv_bfloat16* __restrict__ dbias,
+                                 float* __restrict__ stats, int n_stats, int B, int C) {
+    tfy_pdl_sync();
+    tfy_softmax_xent_body<TFY_HEAD_SPARSE>(logits, bias, labels, nullptr, 0.f, sample_w, class_w, loss, dlogits, dbias,
+                                           stats, n_stats, B, C);
+}
+
+// DENSE target mode: targets [B, C] fp32, label smoothing ls
+__global__ void __launch_bounds__(1024)
+tfy_softmax_xent_soft_kernel(const __nv_bfloat16* __restrict__ logits, const __nv_bfloat16* __restrict__ bias,
+                             const float* __restrict__ targets, float ls, const float* __restrict__ sample_w,
+                             const float* __restrict__ class_w, float* __restrict__ loss,
+                             __nv_bfloat16* __restrict__ dlogits, __nv_bfloat16* __restrict__ dbias,
+                             float* __restrict__ stats, int n_stats, int B, int C) {
+    tfy_pdl_sync();
+    tfy_softmax_xent_body<TFY_HEAD_DENSE>(logits, bias, nullptr, targets, ls, sample_w, class_w, loss, dlogits, dbias,
+                                          stats, n_stats, B, C);
+}
+
 
 // ---------------------------------------------------------------------------------------------
 // Classifier head, forward AND backward, in one launch (the whole problem is ~0.5 MFLOP):
@@ -549,6 +610,9 @@ tfy_softmax_xent_weighted_kernel(const __nv_bfloat16* __restrict__ logits, const
 // label outside [0, C), counts as 1).  Its dlogits row is scaled by w_r, so dW2, db2, dh and db1 follow; the loss is
 // sum_r w_r l_r / B, and stats holds 4 floats [hits, B, sum w*hit, sum w].  The two extra sums use the spare floats
 // of each CTA's reduction slab and are summed in CTA order like the others.
+// TARGET (TFY_HEAD_SPARSE / TFY_HEAD_DENSE, see tfy_softmax_xent_body): the DENSE mode reads targets [B, C] fp32 and
+// the label smoothing ls; lane c of a row's 16 loads y_rc, and two more 16-lane shuffle reductions give the row's
+// class (argmax_c y_rc) and S.  Only the s_dl tile and the per-row loss / hit differ: everything after them is shared.
 // ---------------------------------------------------------------------------------------------
 // debug: per-CTA event timeline of the head kernel (16 slots of SM-clock deltas per CTA), see tfy_nn_set_timeline
 __device__ long long* n_timeline = nullptr;
@@ -558,6 +622,7 @@ __device__ long long* n_timeline = nullptr;
     } while (0)
 
 constexpr int HEAD_THREADS = 256, HEAD_CMAX = 16, HEAD_ROWS = 16, HEAD_WARPS = HEAD_THREADS / 32;
+
 
 template <int K, bool WEIGHTED>
 __global__ void __launch_bounds__(HEAD_THREADS)
@@ -575,327 +640,28 @@ tfy_dense_head_fused_kernel(const __nv_bfloat16* __restrict__ h, const __nv_bflo
     // fully unrolled, so its loads are issued back to back (the first version had ~18 serialised L2 round
     // trips in five-iteration loops: 15 us for 0.5 MFLOP).
     tfy_pdl_sync();
-    long long* const n_tl = n_timeline;
-    const long long n_t0 = clock64();
-    extern __shared__ __align__(16) uint8_t head_smem[];
-    constexpr int KP = K + 8;                                       // padded row (bank spread)
-    constexpr int NRED = WEIGHTED ? 4 : 2;                          // per-warp sums: loss, correct (, w*correct, w)
-    __nv_bfloat16* s_h = reinterpret_cast<__nv_bfloat16*>(head_smem);                 // [16][KP]
-    float* s_w = reinterpret_cast<float*>(head_smem + (size_t)HEAD_ROWS * KP * 2);    // [16][K], rows >= C are zero
-    float* s_dl = s_w + (size_t)HEAD_CMAX * K;                                                // [16][HEAD_CMAX]
-    float* s_b = s_dl + HEAD_ROWS * HEAD_CMAX;                                        // [HEAD_CMAX]
-    float* s_red = s_b + HEAD_CMAX;                                                   // [warp][NRED]
-    float* s_col = s_red + NRED * HEAD_WARPS;                                         // [max(K, 256)], 16-byte aligned
-    __shared__ uint32_t s_last;
-    const int tid = threadIdx.x;
-    const int row0 = blockIdx.x * HEAD_ROWS;
-    const int rows = min(HEAD_ROWS, B - row0);
-    const size_t slab = (size_t)C * K + HEAD_CMAX + K + 4;          // this CTA's partial sums
-    float* g_dw = scratch + blockIdx.x * slab;
-    float* g_db2 = g_dw + (size_t)C * K;
-    float* g_db1 = g_db2 + HEAD_CMAX;
-    float* g_red = g_db1 + K;
+    constexpr int TARGET = TFY_HEAD_SPARSE;
+    [[maybe_unused]] const float* const targets = nullptr;
+    [[maybe_unused]] const float ls = 0.f;
+#include "tfy_dense_head_body.cuh"
+}
 
-    // ---- A: stage this CTA's rows of h (bf16), W2 and b2 (fp32)
-    const int kv = K / 8;
-    for (int i = tid; i < HEAD_ROWS * kv; i += HEAD_THREADS) {
-        const int r = i / kv, g = i - r * kv;
-        *reinterpret_cast<uint4*>(s_h + (size_t)r * KP + g * 8) =
-            r < rows ? tfy_ld16(h + (size_t)(row0 + r) * K + g * 8) : make_uint4(0, 0, 0, 0);
-    }
-    {
-        constexpr int WV = HEAD_CMAX * K / 8 / HEAD_THREADS;        // 16-byte packs of W2 per thread (upper bound)
-        uint4 wv[WV];
-#pragma unroll
-        for (int q = 0; q < WV; ++q) {
-            const int i = tid + q * HEAD_THREADS;
-            wv[q] = i < C * K / 8 ? tfy_ld16(w2 + (size_t)i * 8) : make_uint4(0, 0, 0, 0);
-        }
-#pragma unroll
-        for (int q = 0; q < WV; ++q) {                          // packs beyond C*K/8 were loaded as zeros
-            const int i = tid + q * HEAD_THREADS;
-            TfyPack<__nv_bfloat16>::unpack(wv[q], s_w + (size_t)i * 8);
-        }
-    }
-    if (tid < HEAD_CMAX) s_b[tid] = (tid < C && b2) ? bf16_to_f(b2[tid]) : 0.f;
-    for (int i = tid; i < HEAD_ROWS * HEAD_CMAX; i += HEAD_THREADS) s_dl[i] = 0.f;
-    __syncthreads();
-
-    N_MARK(1);
-    // ---- B/C: logits (16 threads per row), softmax, loss, dlogits
-    const float invB = 1.f / (float)B;
-    {
-        // Classes are padded to 16 with zero weights (no per-class branches) and taken 4 at a time in a ROLLED
-        // loop: this code runs once per launch on 8 warps, so it is instruction-fetch bound -- the fully
-        // unrolled version (2400 instructions) spent 7k cycles here, mostly waiting for the I-cache.
-        const int r = tid >> 4, part = tid & 15;
-        constexpr int kq = K / 16;
-        const int lab = r < rows ? (int)labels[row0 + r] : -1;     // issued early: used after the GEMV
-        float wr = 0.f;                                             // this row's weight (WEIGHTED only)
-        if constexpr (WEIGHTED) {
-            if (r < rows) {
-                wr = sample_w ? sample_w[row0 + r] : 1.f;
-                if (class_w && lab >= 0 && lab < C) wr *= class_w[lab];
-            }
-        }
-        const __nv_bfloat16* hr = s_h + (size_t)r * KP + part * kq;
-        float* s_logit = s_col;                                     // [16][16] scratch (s_col is used later)
-#pragma unroll 1
-        for (int cb = 0; cb < HEAD_CMAX; cb += 4) {
-            float acc[4] = {0.f, 0.f, 0.f, 0.f};
-#pragma unroll 1
-            for (int k = 0; k < kq; k += 8) {
-                float hv[8];
-                TfyPack<__nv_bfloat16>::unpack(*reinterpret_cast<const uint4*>(hr + k), hv);
-#pragma unroll
-                for (int c = 0; c < 4; ++c) {
-                    const float* wp = s_w + (size_t)(cb + c) * K + part * kq + k;
-                    const float4 w0 = *reinterpret_cast<const float4*>(wp);
-                    const float4 w1 = *reinterpret_cast<const float4*>(wp + 4);
-                    acc[c] = fmaf(hv[0], w0.x, acc[c]); acc[c] = fmaf(hv[1], w0.y, acc[c]);
-                    acc[c] = fmaf(hv[2], w0.z, acc[c]); acc[c] = fmaf(hv[3], w0.w, acc[c]);
-                    acc[c] = fmaf(hv[4], w1.x, acc[c]); acc[c] = fmaf(hv[5], w1.y, acc[c]);
-                    acc[c] = fmaf(hv[6], w1.z, acc[c]); acc[c] = fmaf(hv[7], w1.w, acc[c]);
-                }
-            }
-#pragma unroll
-            for (int off = 1; off < 16; off <<= 1) {
-#pragma unroll
-                for (int c = 0; c < 4; ++c) acc[c] += __shfl_xor_sync(0xffffffffu, acc[c], off);
-            }
-            if (part == 0) *reinterpret_cast<float4*>(s_logit + r * HEAD_CMAX + cb) = make_float4(acc[0], acc[1], acc[2], acc[3]);
-        }
-        __syncwarp();
-        // softmax / cross-entropy with one lane per class (the 16 lanes of a row group): a handful of shuffle
-        // steps instead of three serial 10-iteration loops on one lane per row
-        {
-            const int c = part;
-            const bool live = c < C && r < rows;
-            const float v = live ? s_logit[r * HEAD_CMAX + c] + s_b[c] : -3.0e38f;
-            float mx = v;
-            int amax = c;
-#pragma unroll
-            for (int off = 1; off < 16; off <<= 1) {
-                const float ov = __shfl_xor_sync(0xffffffffu, mx, off);
-                const int oa = __shfl_xor_sync(0xffffffffu, amax, off);
-                if (ov > mx || (ov == mx && oa < amax)) { mx = ov; amax = oa; }
-            }
-            const float e = live ? __expf(v - mx) : 0.f;
-            float se = e;
-#pragma unroll
-            for (int off = 1; off < 16; off <<= 1) se += __shfl_xor_sync(0xffffffffu, se, off);
-            const bool hit = live && c == lab;
-            if constexpr (WEIGHTED) {
-                if (live) s_dl[r * HEAD_CMAX + c] = (e / se - (hit ? 1.f : 0.f)) * invB * wr;
-            } else {
-                if (live) s_dl[r * HEAD_CMAX + c] = (e / se - (hit ? 1.f : 0.f)) * invB;
-            }
-            float my_loss = hit ? (mx + __logf(se)) - v : 0.f;
-            float my_correct = (hit && amax == lab) ? 1.f : 0.f;
-            float my_wcorrect = 0.f, my_w = 0.f;
-            if constexpr (WEIGHTED) {
-                my_loss *= wr;
-                my_wcorrect = my_correct * wr;
-                my_w = (c == 0 && r < rows) ? wr : 0.f;             // once per row
-            }
-#pragma unroll
-            for (int off = 16; off > 0; off >>= 1) {
-                my_loss += __shfl_xor_sync(0xffffffffu, my_loss, off);
-                my_correct += __shfl_xor_sync(0xffffffffu, my_correct, off);
-                if constexpr (WEIGHTED) {
-                    my_wcorrect += __shfl_xor_sync(0xffffffffu, my_wcorrect, off);
-                    my_w += __shfl_xor_sync(0xffffffffu, my_w, off);
-                }
-            }
-            if ((tid & 31) == 0) {
-                s_red[NRED * (tid >> 5)] = my_loss;
-                s_red[NRED * (tid >> 5) + 1] = my_correct;
-                if constexpr (WEIGHTED) {
-                    s_red[NRED * (tid >> 5) + 2] = my_wcorrect;
-                    s_red[NRED * (tid >> 5) + 3] = my_w;
-                }
-            }
-        }
-    }
-    __syncthreads();
-    for (int i = tid; i < K; i += HEAD_THREADS) s_col[i] = 0.f;     // s_logit scratch -> column sums
-    __syncthreads();
-    if (tid == 0) {
-        float l = 0.f, c = 0.f;
-        for (int w = 0; w < HEAD_WARPS; ++w) { l += s_red[NRED * w]; c += s_red[NRED * w + 1]; }
-        __stcg(g_red, l);
-        __stcg(g_red + 1, c);
-        if constexpr (WEIGHTED) {
-            float wc = 0.f, ws = 0.f;
-            for (int w = 0; w < HEAD_WARPS; ++w) { wc += s_red[NRED * w + 2]; ws += s_red[NRED * w + 3]; }
-            __stcg(g_red + 2, wc);
-            __stcg(g_red + 3, ws);
-        }
-    }
-
-    N_MARK(2);
-    // ---- D: partial dW2[c][k] = sum_r dl[r][c] h[r][k]; db2[c] = sum_r dl[r][c]
-    {
-        // a thread keeps one column k of h (16 values) in registers and runs over the classes it owns
-        constexpr int KREP = K >= HEAD_THREADS ? K / HEAD_THREADS : 1;
-        constexpr int CSTEP = K >= HEAD_THREADS ? 1 : HEAD_THREADS / K;
-#pragma unroll
-        for (int kr = 0; kr < KREP; ++kr) {
-            const int k = (K >= HEAD_THREADS) ? tid + kr * HEAD_THREADS : tid % K;
-            float hc[HEAD_ROWS];
-#pragma unroll
-            for (int r = 0; r < HEAD_ROWS; ++r) hc[r] = bf16_to_f(s_h[(size_t)r * KP + k]);
-#pragma unroll 1
-            for (int cc = 0; cc < HEAD_CMAX / CSTEP; ++cc) {
-                const int c = cc * CSTEP + ((K >= HEAD_THREADS) ? 0 : tid / K);
-                if (c >= C) break;
-                float a = 0.f;
-#pragma unroll
-                for (int r = 0; r < HEAD_ROWS; ++r) a = fmaf(s_dl[r * HEAD_CMAX + c], hc[r], a);
-                if (c < C) __stcg(g_dw + (size_t)c * K + k, a);
-            }
-        }
-    }
-    if (tid < C) {
-        float a = 0.f;
-#pragma unroll
-        for (int r = 0; r < HEAD_ROWS; ++r) a += s_dl[r * HEAD_CMAX + tid];
-        __stcg(g_db2 + tid, a);
-    }
-
-    N_MARK(3);
-    // ---- E: dh[r][k] = (sum_c dl[r][c] W2[c][k]) * gate * scale; db1[k] = sum_r dh[r][k]
-    if (dh) {
-        // a thread keeps one column k of W2 (16 classes) in registers and runs over the rows it owns
-        constexpr int KREP = K >= HEAD_THREADS ? K / HEAD_THREADS : 1;
-        constexpr int RSTEP = K >= HEAD_THREADS ? 1 : HEAD_THREADS / K;
-#pragma unroll
-        for (int kr = 0; kr < KREP; ++kr) {
-            const int k = (K >= HEAD_THREADS) ? tid + kr * HEAD_THREADS : tid % K;
-            const int rbase = (K >= HEAD_THREADS) ? 0 : tid / K;
-            float wk[HEAD_CMAX];
-#pragma unroll
-            for (int c = 0; c < HEAD_CMAX; ++c) wk[c] = s_w[(size_t)c * K + k];
-            uint32_t mkbits = 0;                                    // gate bits of the rows this thread owns
-#pragma unroll
-            for (int j = 0; j < HEAD_ROWS / RSTEP; ++j) {
-                const int r = rbase + j * RSTEP;
-                const uint32_t bit = (mask1 && r < rows) ? (uint32_t)(mask1[(size_t)(row0 + r) * K + k] & 1) : 1u;
-                mkbits |= bit << j;
-            }
-            float col = 0.f;
-#pragma unroll 2
-            for (int j = 0; j < HEAD_ROWS / RSTEP; ++j) {
-                const int r = rbase + j * RSTEP;
-                float v = 0.f;
-#pragma unroll
-                for (int c4 = 0; c4 < HEAD_CMAX; c4 += 4) {
-                    const float4 d = *reinterpret_cast<const float4*>(s_dl + r * HEAD_CMAX + c4);
-                    v = fmaf(d.x, wk[c4], v); v = fmaf(d.y, wk[c4 + 1], v);
-                    v = fmaf(d.z, wk[c4 + 2], v); v = fmaf(d.w, wk[c4 + 3], v);
-                }
-                if (mask1) v = ((mkbits >> j) & 1u) ? v * scale1 : 0.f;
-                if (r < rows) {
-                    dh[(size_t)(row0 + r) * K + k] = __float2bfloat16(v);
-                    col += v;
-                }
-            }
-            if (db1) atomicAdd(&s_col[k], col);     // at most two addends per column: order-independent
-        }
-        if (db1) {
-            __syncthreads();
-            for (int k = tid; k < K; k += HEAD_THREADS) __stcg(g_db1 + k, s_col[k]);
-        }
-    }
-
-    N_MARK(4);
-    // ---- the last CTA converts the batch sums and clears the scratch buffer
-    __threadfence();
-    __syncthreads();
-    N_MARK(5);
-    if (tid == 0) s_last = (atomicAdd(counter, 1u) == gridDim.x - 1) ? 1u : 0u;
-    __syncthreads();
-    N_MARK(6);
-    if (s_last) {
-        __threadfence();
-        const int G = (int)gridDim.x;
-        {
-            constexpr int FV = HEAD_CMAX * K / 4 / HEAD_THREADS;    // float4 packs per thread (upper bound)
-            float4 fv[FV];
-#pragma unroll
-            for (int q = 0; q < FV; ++q) fv[q] = make_float4(0.f, 0.f, 0.f, 0.f);
-#pragma unroll 8
-            for (int g = 0; g < G; ++g) {                           // CTA order; unrolled: loads in flight together
-                float4* src = reinterpret_cast<float4*>(scratch + (size_t)g * slab);
-#pragma unroll
-                for (int q = 0; q < FV; ++q) {
-                    const int i = tid + q * HEAD_THREADS;
-                    if (i < C * K / 4) {
-                        const float4 v = __ldcg(src + i);
-                        fv[q].x += v.x; fv[q].y += v.y; fv[q].z += v.z; fv[q].w += v.w;
-                        __stcg(src + i, make_float4(0.f, 0.f, 0.f, 0.f));
-                    }
-                }
-            }
-#pragma unroll
-            for (int q = 0; q < FV; ++q) {
-                const int i = tid + q * HEAD_THREADS;
-                if (i < C * K / 4) {
-                    __nv_bfloat162 lo = __floats2bfloat162_rn(fv[q].x, fv[q].y), hi = __floats2bfloat162_rn(fv[q].z, fv[q].w);
-                    uint2 packed;
-                    packed.x = *reinterpret_cast<uint32_t*>(&lo);
-                    packed.y = *reinterpret_cast<uint32_t*>(&hi);
-                    *reinterpret_cast<uint2*>(dw2 + (size_t)i * 4) = packed;
-                }
-            }
-        }
-        const size_t o_db2 = (size_t)C * K, o_db1 = o_db2 + HEAD_CMAX, o_red = o_db1 + K;
-        if (tid < HEAD_CMAX) {
-            float a = 0.f;
-#pragma unroll 8
-            for (int g = 0; g < G; ++g) {
-                a += __ldcg(scratch + g * slab + o_db2 + tid);
-                __stcg(scratch + g * slab + o_db2 + tid, 0.f);
-            }
-            if (tid < C && db2) db2[tid] = __float2bfloat16(a);
-        }
-        for (int k = tid; k < K; k += HEAD_THREADS) {
-            float a = 0.f;
-#pragma unroll 8
-            for (int g = 0; g < G; ++g) {
-                a += __ldcg(scratch + g * slab + o_db1 + k);
-                __stcg(scratch + g * slab + o_db1 + k, 0.f);
-            }
-            if (db1) db1[k] = __float2bfloat16(a);
-        }
-        if (tid == 0) {
-            float l = 0.f, c = 0.f;
-#pragma unroll 8
-            for (int g = 0; g < G; ++g) {
-                l += __ldcg(scratch + g * slab + o_red);
-                c += __ldcg(scratch + g * slab + o_red + 1);
-                __stcg(scratch + g * slab + o_red, 0.f);
-                __stcg(scratch + g * slab + o_red + 1, 0.f);
-            }
-            const float mean_loss = l * invB;
-            *loss = mean_loss;
-            if (loss_host) *loss_host = mean_loss;      // pinned host scalar (UVA): no D2H copy node per step
-            if (stats) { stats[0] += c; stats[1] += (float)B; }
-            if constexpr (WEIGHTED) {
-                float wc = 0.f, ws = 0.f;
-#pragma unroll 8
-                for (int g = 0; g < G; ++g) {
-                    wc += __ldcg(scratch + g * slab + o_red + 2);
-                    ws += __ldcg(scratch + g * slab + o_red + 3);
-                    __stcg(scratch + g * slab + o_red + 2, 0.f);
-                    __stcg(scratch + g * slab + o_red + 3, 0.f);
-                }
-                if (stats) { stats[2] += wc; stats[3] += ws; }
-            }
-            *counter = 0u;
-        }
-    }
-    N_MARK(7);
+// DENSE target mode: targets [B, C] fp32, label smoothing ls
+template <int K, bool WEIGHTED>
+__global__ void __launch_bounds__(HEAD_THREADS)
+tfy_dense_head_fused_soft_kernel(const __nv_bfloat16* __restrict__ h, const __nv_bfloat16* __restrict__ w2,
+                                 const __nv_bfloat16* __restrict__ b2, const float* __restrict__ targets, float ls,
+                                 const uint8_t* __restrict__ mask1, float scale1, float* __restrict__ loss,
+                                 float* __restrict__ loss_host, float* __restrict__ stats,
+                                 __nv_bfloat16* __restrict__ dw2,
+                                 __nv_bfloat16* __restrict__ db2, __nv_bfloat16* __restrict__ dh,
+                                 __nv_bfloat16* __restrict__ db1, float* __restrict__ scratch,
+                                 uint32_t* __restrict__ counter, int B, int C,
+                                 const float* __restrict__ sample_w, const float* __restrict__ class_w) {
+    tfy_pdl_sync();
+    constexpr int TARGET = TFY_HEAD_DENSE;
+    [[maybe_unused]] const long long* const labels = nullptr;
+#include "tfy_dense_head_body.cuh"
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -1008,9 +774,10 @@ int tfy_pool_drop_relu_bwd(const void* dp, const void* code, void* dz, float sca
     return (int)cudaGetLastError();
 }
 
-static int tfy_softmax_xent_launch(const void* logits, const void* bias, const void* labels, const float* sample_w,
-                                   const float* class_w, float* loss, void* dlogits, void* dbias, float* stats,
-                                   int n_stats, int B, int C, cudaStream_t s) {
+// labels (int64, SPARSE mode) or targets (fp32 [B, C], DENSE mode with label smoothing ls): exactly one is non-null
+static int tfy_softmax_xent_launch(const void* logits, const void* bias, const void* labels, const float* targets,
+                                   float ls, const float* sample_w, const float* class_w, float* loss, void* dlogits,
+                                   void* dbias, float* stats, int n_stats, int B, int C, cudaStream_t s) {
     if (B < 1 || C < 1) return -2;
     const int max_warps = (int)((48 * 1024 / sizeof(float) - (size_t)C) / ((size_t)C + 4));
     if ((size_t)C >= 48 * 1024 / sizeof(float) || max_warps < 1) return -2;
@@ -1018,17 +785,26 @@ static int tfy_softmax_xent_launch(const void* logits, const void* bias, const v
     if (warps > 32) warps = 32;
     if (warps > max_warps) warps = max_warps;
     const size_t smem = ((size_t)C + (size_t)warps * (C + 4)) * sizeof(float);
-    tfy_launch_pdl((tfy_softmax_xent_weighted_kernel), dim3(1), dim3(warps * 32), smem, s,
-                   (const __nv_bfloat16*)logits, (const __nv_bfloat16*)bias, (const long long*)labels, sample_w,
-                   class_w, loss, (__nv_bfloat16*)dlogits, (__nv_bfloat16*)dbias, stats, n_stats, B, C);
+    if (targets)
+        tfy_launch_pdl((tfy_softmax_xent_soft_kernel), dim3(1), dim3(warps * 32), smem, s,
+                       (const __nv_bfloat16*)logits, (const __nv_bfloat16*)bias, targets, ls, sample_w, class_w, loss,
+                       (__nv_bfloat16*)dlogits, (__nv_bfloat16*)dbias, stats, n_stats, B, C);
+    else
+        tfy_launch_pdl((tfy_softmax_xent_weighted_kernel), dim3(1), dim3(warps * 32), smem, s,
+                       (const __nv_bfloat16*)logits, (const __nv_bfloat16*)bias, (const long long*)labels, sample_w,
+                       class_w, loss, (__nv_bfloat16*)dlogits, (__nv_bfloat16*)dbias, stats, n_stats, B, C);
     return (int)cudaGetLastError();
 }
+
+// Keras label smoothing: a finite ls in [0, 1]
+static inline bool tfy_valid_smoothing(float ls) { return ls >= 0.f && ls <= 1.f; }
 
 // unweighted head (every weight 1), stats null or 2 floats [hits, B]; returns -2 when C is too wide for one partial
 // row of dbias per warp (C > 9000 or so)
 int tfy_softmax_xent(const void* logits, const void* bias, const void* labels, float* loss, void* dlogits,
                      void* dbias, float* stats, int B, int C, cudaStream_t s) {
-    return tfy_softmax_xent_launch(logits, bias, labels, nullptr, nullptr, loss, dlogits, dbias, stats, 2, B, C, s);
+    return tfy_softmax_xent_launch(logits, bias, labels, nullptr, 0.f, nullptr, nullptr, loss, dlogits, dbias, stats, 2,
+                                   B, C, s);
 }
 
 // weighted variant: sample_w [B] and class_w [C] fp32 (either may be null), stats null or 4 floats
@@ -1036,7 +812,20 @@ int tfy_softmax_xent(const void* logits, const void* bias, const void* labels, f
 int tfy_softmax_xent_weighted(const void* logits, const void* bias, const void* labels, const float* sample_w,
                               const float* class_w, float* loss, void* dlogits, void* dbias, float* stats, int B, int C,
                               cudaStream_t s) {
-    return tfy_softmax_xent_launch(logits, bias, labels, sample_w, class_w, loss, dlogits, dbias, stats, 4, B, C, s);
+    return tfy_softmax_xent_launch(logits, bias, labels, nullptr, 0.f, sample_w, class_w, loss, dlogits, dbias, stats, 4,
+                                   B, C, s);
+}
+
+// dense-target variant (Keras CategoricalCrossentropy): targets [B, C] fp32, one-hot or soft, label smoothing ls in
+// [0, 1]; sample_w and class_w as above (either may be null; the class of a row is argmax_c targets[r][c]).  stats
+// null, or 2 floats [hits, B] when both weight pointers are null, else 4.  -2 also when ls is outside [0, 1] or
+// B * C exceeds INT_MAX.
+int tfy_softmax_xent_soft(const void* logits, const void* bias, const float* targets, float ls, const float* sample_w,
+                          const float* class_w, float* loss, void* dlogits, void* dbias, float* stats, int B, int C,
+                          cudaStream_t s) {
+    if (!targets || !tfy_valid_smoothing(ls) || (long long)B * C > INT_MAX) return -2;
+    return tfy_softmax_xent_launch(logits, bias, nullptr, targets, ls, sample_w, class_w, loss, dlogits, dbias, stats,
+                                   (sample_w || class_w) ? 4 : 2, B, C, s);
 }
 
 // thin cudaMemcpyAsync wrapper: the input pipeline issues its per-step copies through ctypes (about 1 us per call
@@ -1057,8 +846,10 @@ size_t tfy_dense_head_scratch_elems(int K, int C, int B) {
 
 }  // extern "C"
 
-template <bool WEIGHTED>
-static int tfy_dense_head_launch(const void* h, const void* w2, const void* b2, const void* labels, const void* mask1,
+// TARGET: TFY_HEAD_SPARSE reads `labels` (int64), TFY_HEAD_DENSE reads `targets` (fp32 [B, C]) and `ls`
+template <bool WEIGHTED, int TARGET>
+static int tfy_dense_head_launch(const void* h, const void* w2, const void* b2, const void* labels,
+                                 const float* targets, float ls, const void* mask1,
                                  float scale1, float* loss, float* loss_host, float* stats, void* dw2, void* db2,
                                  void* dh, void* db1, float* scratch, uint32_t* counter, int B, int K, int C,
                                  const float* sample_w, const float* class_w, cudaStream_t s) {
@@ -1069,26 +860,38 @@ static int tfy_dense_head_launch(const void* h, const void* w2, const void* b2, 
     const size_t smem = (size_t)HEAD_ROWS * (K + 8) * 2 +
                         ((size_t)HEAD_CMAX * K + HEAD_ROWS * HEAD_CMAX + HEAD_CMAX + NRED * HEAD_WARPS + (K > 256 ? K : 256)) * 4;
     const int grid = (B + HEAD_ROWS - 1) / HEAD_ROWS;
-#define TFY_HEAD(KK)                                                                                                   \
+#define TFY_HEAD_SMEM(KERNEL)                                                                                          \
     do {                                                                                                               \
         static bool configured = false;                                                                                \
         if (smem > 48 * 1024 && !configured) {                                                                         \
-            if (cudaFuncSetAttribute(tfy_dense_head_fused_kernel<KK, WEIGHTED>,                                        \
-                                     cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024) != cudaSuccess)           \
+            if (cudaFuncSetAttribute(KERNEL, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024) != cudaSuccess)   \
                 return -5;                                                                                             \
             configured = true;                                                                                         \
         }                                                                                                              \
-        tfy_launch_pdl((tfy_dense_head_fused_kernel<KK, WEIGHTED>), dim3(grid), dim3(HEAD_THREADS), smem, s,           \
-                       (const __nv_bfloat16*)h, (const __nv_bfloat16*)w2, (const __nv_bfloat16*)b2,                    \
-                       (const long long*)labels, (const uint8_t*)mask1, scale1, loss, loss_host, stats,              \
-                       (__nv_bfloat16*)dw2,                                                                            \
-                       (__nv_bfloat16*)db2, (__nv_bfloat16*)dh, (__nv_bfloat16*)db1, scratch, counter, B, C,           \
-                       sample_w, class_w);                                                                             \
+    } while (0)
+#define TFY_HEAD(KK)                                                                                                   \
+    do {                                                                                                               \
+        if constexpr (TARGET == TFY_HEAD_SPARSE) {                                                                     \
+            TFY_HEAD_SMEM((tfy_dense_head_fused_kernel<KK, WEIGHTED>));                                                \
+            tfy_launch_pdl((tfy_dense_head_fused_kernel<KK, WEIGHTED>), dim3(grid), dim3(HEAD_THREADS), smem, s,       \
+                           (const __nv_bfloat16*)h, (const __nv_bfloat16*)w2, (const __nv_bfloat16*)b2,                \
+                           (const long long*)labels, (const uint8_t*)mask1, scale1, loss, loss_host, stats,            \
+                           (__nv_bfloat16*)dw2, (__nv_bfloat16*)db2, (__nv_bfloat16*)dh, (__nv_bfloat16*)db1, scratch, \
+                           counter, B, C, sample_w, class_w);                                                          \
+        } else {                                                                                                       \
+            TFY_HEAD_SMEM((tfy_dense_head_fused_soft_kernel<KK, WEIGHTED>));                                           \
+            tfy_launch_pdl((tfy_dense_head_fused_soft_kernel<KK, WEIGHTED>), dim3(grid), dim3(HEAD_THREADS), smem, s,  \
+                           (const __nv_bfloat16*)h, (const __nv_bfloat16*)w2, (const __nv_bfloat16*)b2, targets, ls,   \
+                           (const uint8_t*)mask1, scale1, loss, loss_host, stats, (__nv_bfloat16*)dw2,                 \
+                           (__nv_bfloat16*)db2, (__nv_bfloat16*)dh, (__nv_bfloat16*)db1, scratch, counter, B, C,       \
+                           sample_w, class_w);                                                                         \
+        }                                                                                                              \
     } while (0)
     if (K == 128) TFY_HEAD(128);
     else if (K == 256) TFY_HEAD(256);
     else TFY_HEAD(512);
 #undef TFY_HEAD
+#undef TFY_HEAD_SMEM
     return (int)cudaGetLastError();
 }
 
@@ -1098,8 +901,9 @@ int tfy_dense_head_fused(const void* h, const void* w2, const void* b2, const vo
                          float scale1, float* loss, float* loss_host, float* stats, void* dw2, void* db2, void* dh,
                          void* db1,
                          float* scratch, uint32_t* counter, int B, int K, int C, cudaStream_t s) {
-    return tfy_dense_head_launch<false>(h, w2, b2, labels, mask1, scale1, loss, loss_host, stats, dw2, db2, dh, db1,
-                                        scratch, counter, B, K, C, nullptr, nullptr, s);
+    return tfy_dense_head_launch<false, TFY_HEAD_SPARSE>(h, w2, b2, labels, nullptr, 0.f, mask1, scale1, loss,
+                                                         loss_host, stats, dw2, db2, dh, db1, scratch, counter, B, K,
+                                                         C, nullptr, nullptr, s);
 }
 
 // weighted variant: sample_w [B] and class_w [C] fp32 (either may be null), stats null or 4 floats
@@ -1108,8 +912,28 @@ int tfy_dense_head_fused_weighted(const void* h, const void* w2, const void* b2,
                                   float scale1, float* loss, float* loss_host, float* stats, void* dw2, void* db2,
                                   void* dh, void* db1, float* scratch, uint32_t* counter, int B, int K, int C,
                                   const float* sample_w, const float* class_w, cudaStream_t s) {
-    return tfy_dense_head_launch<true>(h, w2, b2, labels, mask1, scale1, loss, loss_host, stats, dw2, db2, dh, db1,
-                                       scratch, counter, B, K, C, sample_w, class_w, s);
+    return tfy_dense_head_launch<true, TFY_HEAD_SPARSE>(h, w2, b2, labels, nullptr, 0.f, mask1, scale1, loss, loss_host,
+                                                        stats, dw2, db2, dh, db1, scratch, counter, B, K, C, sample_w,
+                                                        class_w, s);
+}
+
+// dense-target variant (Keras CategoricalCrossentropy): targets [B, C] fp32, one-hot or soft, label smoothing ls in
+// [0, 1]; sample_w [B] and class_w [C] fp32, either may be null (the class of a row is argmax_c targets[r][c]).  The
+// unweighted kernel runs when both are null (stats null or 2 floats [hits, B]), the weighted one otherwise (stats
+// null or 4 floats).  Same envelope, scratch size and return codes as tfy_dense_head_fused; -2 also when targets is
+// null, ls is outside [0, 1] or B * C exceeds INT_MAX.
+int tfy_dense_head_fused_soft(const void* h, const void* w2, const void* b2, const float* targets, float ls,
+                              const void* mask1, float scale1, float* loss, float* loss_host, float* stats, void* dw2,
+                              void* db2, void* dh, void* db1, float* scratch, uint32_t* counter, int B, int K, int C,
+                              const float* sample_w, const float* class_w, cudaStream_t s) {
+    if (!targets || !tfy_valid_smoothing(ls) || (long long)B * C > INT_MAX) return -2;
+    if (sample_w || class_w)
+        return tfy_dense_head_launch<true, TFY_HEAD_DENSE>(h, w2, b2, nullptr, targets, ls, mask1, scale1, loss,
+                                                           loss_host, stats, dw2, db2, dh, db1, scratch, counter, B, K,
+                                                           C, sample_w, class_w, s);
+    return tfy_dense_head_launch<false, TFY_HEAD_DENSE>(h, w2, b2, nullptr, targets, ls, mask1, scale1, loss,
+                                                        loss_host, stats, dw2, db2, dh, db1, scratch, counter, B, K, C,
+                                                        nullptr, nullptr, s);
 }
 
 }  // extern "C"
