@@ -2,8 +2,9 @@
 
 For ``Sequential`` models made of Conv2D(3x3, valid, stride 1) / MaxPooling2D(2x2) /
 Dropout / Flatten / Dense layers with relu|linear activations and a sparse-categorical or categorical
-(one-hot / soft targets, label smoothing) cross-entropy head -- the MNIST-CNN of the headline benchmark, the wine MLP --
-the step does not go through autograd at all:
+(one-hot / soft targets, label smoothing) cross-entropy head, or a binary cross-entropy head (binary or multi-label,
+label smoothing) -- the MNIST-CNN of the headline benchmark, the wine MLP -- the step does not go through autograd at
+all:
 
 * convolutions are wgmma implicit GEMMs (:mod:`ops/csrc/tfy_conv.cu`): conv2 forward with
   bias + ReLU + 2x2 max-pool + dropout in the epilogue, conv2 data / weight gradients whose dz
@@ -47,6 +48,7 @@ native.declare("tfy_pool_drop_relu_bwd", [_vp, _vp, _vp, _f, _i, _i, _i, _i, _vp
 native.declare("tfy_softmax_xent", [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _vp])
 native.declare("tfy_softmax_xent_weighted", [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _vp])
 native.declare("tfy_softmax_xent_soft", [_vp, _vp, _vp, _f, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _vp])
+native.declare("tfy_sigmoid_xent", [_vp, _vp, _vp, _f, _i, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _vp])
 native.declare("tfy_conv3x3_c32_pool_fwd", [_vp, _vp, _vp, _vp, _vp, _i, _i, _i, _f, _u32, _vp, _vp])
 native.declare("tfy_conv3x3_c32_dgrad", [_vp, _vp, _vp, _vp, _i, _i, _i, _vp])
 native.declare("tfy_conv3x3_c32_wgrad", [_vp, _vp, _vp, _vp, _vp, _i, _i, _i, _vp])
@@ -71,6 +73,8 @@ native.declare("tfy_dense_head_fused_weighted", [_vp, _vp, _vp, _vp, _vp, _f, _v
                                                  _vp, _i, _i, _i, _vp, _vp, _vp])
 native.declare("tfy_dense_head_fused_soft", [_vp, _vp, _vp, _vp, _f, _vp, _f, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp,
                                              _i, _i, _i, _vp, _vp, _vp])
+native.declare("tfy_dense_head_fused_binary", [_vp, _vp, _vp, _vp, _f, _i, _vp, _f, _vp, _vp, _vp, _vp, _vp, _vp, _vp,
+                                               _vp, _vp, _i, _i, _i, _vp, _vp, _vp])
 
 PARTIAL_BLOCKS = 592
 
@@ -107,8 +111,21 @@ def head_loss(loss):
     return None
 
 
+def binary_head_loss(loss):
+    """``(label_smoothing, head activation)`` of a binary cross-entropy loss the fused head computes, or None.  The head
+    computes sigmoid cross-entropy from logits: either the loss takes logits and the last layer is linear, or the last
+    layer is a sigmoid and the loss takes probabilities.  It reads fp32 targets [B, C] ([B] or [B, 1] when C = 1)."""
+    from tf_yarn_b200.keras import losses as kl
+    if isinstance(loss, kl.BinaryCrossentropy):
+        return loss.label_smoothing, "linear" if loss.from_logits else "sigmoid"
+    if isinstance(loss, str) and loss == "binary_crossentropy":
+        return 0.0, "sigmoid"
+    return None
+
+
 def label_dtype(loss) -> Optional[torch.dtype]:
-    """Dtype of the labels the fused head reads for ``loss`` (None: not a fused-head loss)."""
+    """Dtype ``fit`` casts array labels to once for a softmax head's ``loss`` (None: no cast).  Binary targets are not
+    cast there: whatever their dtype, the staging copy converts them to the fp32 the binary head reads."""
     head = head_loss(loss)
     if head is None:
         return None
@@ -117,12 +134,16 @@ def label_dtype(loss) -> Optional[torch.dtype]:
 
 def build_plan(model) -> Optional[List[_Stage]]:
     """Pattern-match the layer list; None if the model is outside the fast-path grammar."""
-    head = head_loss(model.loss)
-    if head is None:
-        return None
-    categorical, _, want_head_activation = head
+    head, binary = head_loss(model.loss), binary_head_loss(model.loss)
     # the head kernel counts the hits of the accuracy that goes with the loss; one weighted accuracy at most
-    accuracies = ("accuracy", "acc", "categorical_accuracy" if categorical else "sparse_categorical_accuracy")
+    if head is not None:
+        categorical, _, want_head_activation = head
+        accuracies = ("accuracy", "acc", "categorical_accuracy" if categorical else "sparse_categorical_accuracy")
+    elif binary is not None:
+        _, want_head_activation = binary
+        accuracies = ("accuracy", "acc", "binary_accuracy")
+    else:
+        return None
     for m in model._metrics_spec:
         if m not in accuracies:
             return None
@@ -226,11 +247,14 @@ class FastSequentialEngine(GraphTrainEngine):
         self._c1_acc = torch.zeros(160 * 320, dtype=torch.float32, device=dev)   # first-layer dW/db per-CTA partials
         self._c1_cnt = torch.zeros(1, dtype=torch.int32, device=dev)
         # what the head reads: int64 labels [B] (sparse loss), or fp32 targets [B, C] and the label smoothing
-        # (categorical loss: self._ls is not None).  The staging slots hold labels of this dtype, so a batch of another
-        # dtype is converted by the staging copy instead of being misread.
-        categorical, ls, _ = head_loss(model.loss)
+        # (categorical loss: self._ls is not None; binary cross-entropy: self._binary = (label smoothing, whether the
+        # model's output is the sigmoid)).  The staging slots hold labels of this dtype, so a batch of another dtype is
+        # converted by the staging copy instead of being misread.
+        head, binary = head_loss(model.loss), binary_head_loss(model.loss)
+        categorical, ls, _ = head if head is not None else (False, 0.0, None)
         self._ls = float(ls) if categorical else None
-        self._y_dtype = torch.float32 if categorical else torch.int64
+        self._binary = (float(binary[0]), binary[1] == "sigmoid") if binary is not None else None
+        self._y_dtype = torch.float32 if (categorical or binary is not None) else torch.int64
 
     # ------------------------------------------------------------------ helpers
     def _s(self):
@@ -353,9 +377,15 @@ class FastSequentialEngine(GraphTrainEngine):
                 self._s())
 
     def _head_targets(self, y: torch.Tensor) -> torch.Tensor:
-        """``y`` in the dtype the head reads; a categorical target must be ``[B, C]``."""
+        """``y`` in the dtype the head reads; a categorical target must be ``[B, C]``, a binary one ``[B, C]``, or
+        ``[B]`` when C = 1."""
+        C = self.plan[-1].layer.units
+        if self._binary is not None:
+            if not ((y.dim() == 2 and y.shape[-1] == C) or (C == 1 and y.dim() == 1)):
+                want = "(batch,) or (batch, 1)" if C == 1 else f"(batch, {C})"
+                raise ValueError(f"binary targets of shape {tuple(y.shape)} do not match the model's output "
+                                 f"(batch, {C}): pass 0/1 or soft targets of shape {want}")
         if self._ls is not None:
-            C = self.plan[-1].layer.units
             if y.dim() != 2 or y.shape[-1] != C:
                 raise ValueError(f"categorical targets of shape {tuple(y.shape)} do not match the model's output "
                                  f"(batch, {C}): pass one-hot or soft targets of shape (batch, {C}), or class indices "
@@ -686,7 +716,11 @@ class FastSequentialEngine(GraphTrainEngine):
                     pb.grad.data_ptr(), self._acc32["head_scratch"].data_ptr(), self._acc32["head_counter"].data_ptr(),
                     B, K, C)
             args = (xin.data_ptr(), w.data_ptr(), b.data_ptr(), y.data_ptr()) + rest
-            if self._ls is not None:
+            if self._binary is not None:
+                # binary cross-entropy: fp32 targets, the label smoothing and whether the model's output is the sigmoid
+                self._chk(lib.tfy_dense_head_fused_binary(*args[:4], self._binary[0], int(self._binary[1]), *rest,
+                                                          *self._weight_ptrs(sw)), "dense_head_fused_binary")
+            elif self._ls is not None:
                 # categorical loss: fp32 targets [B, C] and the label smoothing (null weights: unweighted kernel)
                 self._chk(lib.tfy_dense_head_fused_soft(xin.data_ptr(), w.data_ptr(), b.data_ptr(), y.data_ptr(),
                                                         self._ls, *rest, *self._weight_ptrs(sw)), "dense_head_fused_soft")
@@ -698,7 +732,13 @@ class FastSequentialEngine(GraphTrainEngine):
             return
         logits = torch.mm(xin, w.t())
         sv.x, sv.dlogits = xin, torch.empty((B, C), dtype=torch.bfloat16, device=x.device)
-        if self._ls is not None:
+        if self._binary is not None:
+            sw_ptr, cw_ptr, _ = self._weight_ptrs(sw)
+            self._chk(lib.tfy_sigmoid_xent(logits.data_ptr(), b.data_ptr(), y.data_ptr(), self._binary[0],
+                                           int(self._binary[1]), sw_ptr, cw_ptr, self._loss.data_ptr(),
+                                           sv.dlogits.data_ptr(), b.grad.data_ptr(), self._stats_ptr(), B, C, s),
+                      "sigmoid_xent")
+        elif self._ls is not None:
             sw_ptr, cw_ptr, _ = self._weight_ptrs(sw)
             self._chk(lib.tfy_softmax_xent_soft(logits.data_ptr(), b.data_ptr(), y.data_ptr(), self._ls, sw_ptr, cw_ptr,
                                                 self._loss.data_ptr(), sv.dlogits.data_ptr(), b.grad.data_ptr(),

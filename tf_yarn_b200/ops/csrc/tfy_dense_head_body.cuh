@@ -1,7 +1,8 @@
-// Body of the fused classifier-head kernels of tfy_nn.cu (tfy_dense_head_fused_kernel and
-// tfy_dense_head_fused_soft_kernel): a statement sequence, included inside each kernel after its tfy_pdl_sync(), in
-// the scope of the kernel's parameters and of the constants TARGET (TFY_HEAD_SPARSE or TFY_HEAD_DENSE), `labels`,
-// `targets` and `ls` (the ones a mode does not read are null / 0).  It is a textual include rather than a shared
+// Body of the fused classifier-head kernels of tfy_nn.cu (tfy_dense_head_fused_kernel,
+// tfy_dense_head_fused_soft_kernel and tfy_dense_head_fused_binary_kernel): a statement sequence, included inside each
+// kernel after its tfy_pdl_sync(), in the scope of the kernel's parameters and of the constants TARGET
+// (TFY_HEAD_SPARSE, TFY_HEAD_DENSE or TFY_HEAD_BINARY), `labels`, `targets`, `ls` and `sigmoid_out` (the ones a mode
+// does not read are null / 0 / false).  It is a textual include rather than a shared
 // __device__ function because inlining such a function compiles the existing sparse instantiations to different
 // (reordered) SASS; included, they stay instruction for instruction what they were.
     long long* const n_tl = n_timeline;
@@ -59,9 +60,10 @@
         // unrolled version (2400 instructions) spent 7k cycles here, mostly waiting for the I-cache.
         const int r = tid >> 4, part = tid & 15;
         constexpr int kq = K / 16;
-        // the row's class, issued early: used after the GEMV (DENSE: argmax_c y_rc, y_rc held by lane c)
+        // the row's class, issued early: used after the GEMV (DENSE: argmax_c y_rc, y_rc held by lane c; BINARY: the
+        // same for C > 1, round(y_r0) half to even for C = 1)
         int lab = -1;
-        [[maybe_unused]] float y = 0.f;                            // DENSE: this lane's target y_rc
+        [[maybe_unused]] float y = 0.f;                            // DENSE, BINARY: this lane's target y_rc
         if constexpr (TARGET == TFY_HEAD_SPARSE) {
             lab = r < rows ? (int)labels[row0 + r] : -1;
         } else {
@@ -76,12 +78,16 @@
                 if (ov > ym || (ov == ym && oa < ya)) { ym = ov; ya = oa; }
             }
             if (r < rows) lab = ya;
+            if constexpr (TARGET == TFY_HEAD_BINARY) {
+                if (r < rows && C == 1) lab = __float2int_rn(ym);      // ym: the row's only target
+            }
         }
         float wr = 0.f;                                             // this row's weight (WEIGHTED only)
         if constexpr (WEIGHTED) {
             if (r < rows) {
                 wr = sample_w ? sample_w[row0 + r] : 1.f;
-                if (class_w && lab >= 0 && lab < C) wr *= class_w[lab];
+                // (a binary head's class table has max(C, 2) entries: classes 0 and 1 when C = 1)
+                if (class_w && lab >= 0 && lab < (TARGET == TFY_HEAD_BINARY ? max(C, 2) : C)) wr *= class_w[lab];
             }
         }
         const __nv_bfloat16* hr = s_h + (size_t)r * KP + part * kq;
@@ -114,7 +120,45 @@
         __syncwarp();
         // softmax / cross-entropy with one lane per class (the 16 lanes of a row group): a handful of shuffle
         // steps instead of three serial 10-iteration loops on one lane per row
-        {
+        if constexpr (TARGET == TFY_HEAD_BINARY) {
+            // sigmoid cross-entropy, one lane per output: every logit is one element of the row's mean
+            const int c = part;
+            const bool live = c < C && r < rows;
+            const float z = live ? s_logit[r * HEAD_CMAX + c] + s_b[c] : 0.f;
+            const float t = fmaf(y, 1.f - ls, 0.5f * ls);
+            const float sg = tfy_head_sigmoid(z);
+            const float invC = 1.f / (float)C;
+            const float out = sigmoid_out ? sg : z;                 // the model's output, as binary_accuracy reads it
+            const bool hit = live && ((out > 0.5f) == (y > 0.5f));
+            float dz = (sg - t) * (invB * invC);
+            if constexpr (WEIGHTED) dz *= wr;
+            if (live) s_dl[r * HEAD_CMAX + c] = dz;
+            float my_loss = live ? tfy_head_binary_loss(z, t) * invC : 0.f;
+            float my_correct = hit ? 1.f : 0.f;
+            float my_wcorrect = 0.f, my_w = 0.f;
+            if constexpr (WEIGHTED) {
+                my_loss *= wr;
+                my_wcorrect = hit ? wr * invC : 0.f;
+                my_w = (c == 0 && r < rows) ? wr : 0.f;             // once per row
+            }
+#pragma unroll
+            for (int off = 16; off > 0; off >>= 1) {
+                my_loss += __shfl_xor_sync(0xffffffffu, my_loss, off);
+                my_correct += __shfl_xor_sync(0xffffffffu, my_correct, off);
+                if constexpr (WEIGHTED) {
+                    my_wcorrect += __shfl_xor_sync(0xffffffffu, my_wcorrect, off);
+                    my_w += __shfl_xor_sync(0xffffffffu, my_w, off);
+                }
+            }
+            if ((tid & 31) == 0) {
+                s_red[NRED * (tid >> 5)] = my_loss;
+                s_red[NRED * (tid >> 5) + 1] = my_correct;
+                if constexpr (WEIGHTED) {
+                    s_red[NRED * (tid >> 5) + 2] = my_wcorrect;
+                    s_red[NRED * (tid >> 5) + 3] = my_w;
+                }
+            }
+        } else {
             const int c = part;
             const bool live = c < C && r < rows;
             const float v = live ? s_logit[r * HEAD_CMAX + c] + s_b[c] : -3.0e38f;
@@ -340,7 +384,11 @@
             const float mean_loss = l * invB;
             *loss = mean_loss;
             if (loss_host) *loss_host = mean_loss;      // pinned host scalar (UVA): no D2H copy node per step
-            if (stats) { stats[0] += c; stats[1] += (float)B; }
+            if constexpr (TARGET == TFY_HEAD_BINARY) {
+                if (stats) { stats[0] += c; stats[1] += (float)B * (float)C; }      // hits over elements
+            } else {
+                if (stats) { stats[0] += c; stats[1] += (float)B; }
+            }
             if constexpr (WEIGHTED) {
                 float wc = 0.f, ws = 0.f;
 #pragma unroll 8

@@ -37,12 +37,14 @@ TFY_HEAD_HD float tfy_head_binary_loss(float z, float y) {
     return fmaxf(z, 0.f) - z * y + log1pf(expf(-fabsf(z)));
 }
 
-// sigmoid(z) - y, with exp of a non-positive argument only (no overflow for any z)
-TFY_HEAD_HD float tfy_head_binary_grad(float z, float y) {
+// sigmoid(z), with exp of a non-positive argument only (no overflow for any z)
+TFY_HEAD_HD float tfy_head_sigmoid(float z) {
     const float e = expf(-fabsf(z));
-    const float s = z >= 0.f ? 1.f / (1.f + e) : e / (1.f + e);
-    return s - y;
+    return z >= 0.f ? 1.f / (1.f + e) : e / (1.f + e);
 }
+
+// sigmoid(z) - y
+TFY_HEAD_HD float tfy_head_binary_grad(float z, float y) { return tfy_head_sigmoid(z) - y; }
 
 TFY_HEAD_HD float tfy_head_regression_loss(float z, float y) {
     const float r = z - y;

@@ -17,10 +17,12 @@
 //   tfy_softmax_xent          logits(+bias) -> mean loss, dlogits = (softmax - onehot)/B, dbias, #correct
 //                             (tfy_softmax_xent_weighted: the same with Keras sample / class weights)
 //                             (tfy_softmax_xent_soft: fp32 one-hot / soft targets with Keras label smoothing)
+//   tfy_sigmoid_xent          its sigmoid twin (Keras BinaryCrossentropy, binary and multi-label)
 //
 // Dropout randomness is counter based: hash(seed, layer salt, optimizer step, element) with the
 // step read from the device-resident TfyOptHyper, so a replayed CUDA graph draws fresh masks.
 #include "tfy_common.cuh"
+#include "tfy_head.cuh"
 
 namespace {
 
@@ -451,8 +453,15 @@ tfy_pool_drop_relu_bwd_kernel(const __nv_bfloat16* __restrict__ dp, const uint8_
 // is sum_c t_c (lse - v_c) and its dlogits (p_c S - t_c) w_r / B; its class (hit test, class weight) is argmax_c y_c,
 // ties to the lowest index.  A one-hot row with ls = 0 has t = onehot and S = 1 exactly, and every expression keeps
 // the SPARSE mode's order of operations, so the two modes give the same bits.
+// BINARY (Keras BinaryCrossentropy; the fused head and tfy_sigmoid_xent): fp32 targets y [B, C], every logit z one
+// element of the row's mean, t = y (1 - ls) + ls / 2, l = max(z, 0) - z t + log1p(exp(-|z|)) (tfy_head.cuh's binary
+// element function), a row's loss (1/C) sum_c l_c and its dlogits w_r (sigmoid(z) - t) / (B C).  Its hits are per
+// element, (out > 0.5) == (y > 0.5) with out the model's output (sigmoid(z), or z after a linear layer), and stats
+// count [hits, B C, sum_r w_r hits_r / C, sum_r w_r]; a row's class (class weight) is round(y) half to even for C = 1,
+// argmax_c y_c otherwise, in a class table of max(C, 2) entries.  The mode shares TfyHead's TFY_HEAD_BINARY (the
+// canned binary head, whose element functions it computes); the softmax modes are numbered after TfyHead's.
 // ---------------------------------------------------------------------------------------------
-enum : int { TFY_HEAD_SPARSE = 0, TFY_HEAD_DENSE = 1 };
+enum : int { TFY_HEAD_SPARSE = TFY_HEAD_LOGISTIC + 1, TFY_HEAD_DENSE };
 
 template <int TARGET>
 __device__ __forceinline__ void
@@ -591,6 +600,102 @@ tfy_softmax_xent_soft_kernel(const __nv_bfloat16* __restrict__ logits, const __n
                                           stats, n_stats, B, C);
 }
 
+// BINARY target mode: targets [B, C] fp32, label smoothing ls, sigmoid_out: the model's output is sigmoid(z) (else z).
+// The block shape, shared-memory layout and reduction order are tfy_softmax_xent_body's.
+__global__ void __launch_bounds__(1024)
+tfy_sigmoid_xent_kernel(const __nv_bfloat16* __restrict__ logits, const __nv_bfloat16* __restrict__ bias,
+                        const float* __restrict__ targets, float ls, int sigmoid_out,
+                        const float* __restrict__ sample_w, const float* __restrict__ class_w, float* __restrict__ loss,
+                        __nv_bfloat16* __restrict__ dlogits, __nv_bfloat16* __restrict__ dbias,
+                        float* __restrict__ stats, int n_stats, int B, int C) {
+    tfy_pdl_sync();
+    extern __shared__ float sm[];  // [C] bias | [warps][C] dbias partials | [warps][4] loss, hits, w*hits/C, w
+    const int warps = blockDim.x >> 5, warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    float* s_bias = sm;
+    float* s_db = sm + C;
+    float* s_red = s_db + (size_t)warps * C;
+    for (int c = threadIdx.x; c < C; c += blockDim.x) s_bias[c] = bias ? bf16_to_f(bias[c]) : 0.f;
+    for (int i = threadIdx.x; i < warps * C; i += blockDim.x) s_db[i] = 0.f;
+    __syncthreads();
+    const float invB = 1.f / (float)B, invC = 1.f / (float)C;
+    const int n_cls = max(C, 2);                                 // class-weight table entries
+    float acc[4] = {0.f, 0.f, 0.f, 0.f};        // loss, hits, w*hits/C, w
+    const int rounds = (B + blockDim.x - 1) / blockDim.x;      // same trip count on every warp: shuffles converge
+    const float keep = 1.f - ls, add = 0.5f * ls;               // t = y * keep + add
+    for (int it = 0; it < rounds; ++it) {
+        const int r = it * blockDim.x + threadIdx.x;
+        const bool ok = r < B;
+        const __nv_bfloat16* row = logits + (size_t)(ok ? r : 0) * C;
+        const float* trow = targets + (size_t)(ok ? r : 0) * C;
+        float wr = 0.f;
+        if (ok) {
+            int lab = 0;
+            if (C == 1) {
+                lab = __float2int_rn(trow[0]);
+            } else {
+                float ym = -INFINITY;
+                for (int c = 0; c < C; ++c)
+                    if (trow[c] > ym) { ym = trow[c]; lab = c; }
+            }
+            wr = sample_w ? sample_w[r] : 1.f;
+            if (class_w && lab >= 0 && lab < n_cls) wr *= class_w[lab];
+        }
+        float lrow = 0.f, hrow = 0.f;                            // sum_c l_c, hits of the row
+        for (int c = 0; c < C; ++c) {
+            float d = 0.f;
+            if (ok) {
+                const float z = bf16_to_f(row[c]) + s_bias[c];
+                const float y = trow[c];
+                const float t = fmaf(y, keep, add);
+                const float sg = tfy_head_sigmoid(z);
+                lrow += tfy_head_binary_loss(z, t);
+                hrow += ((sigmoid_out ? sg : z) > 0.5f) == (y > 0.5f) ? 1.f : 0.f;
+                d = (sg - t) * (invB * invC) * wr;
+                dlogits[(size_t)r * C + c] = __float2bfloat16(d);
+            }
+            if (dbias) {
+                float t = d;
+#pragma unroll
+                for (int off = 16; off > 0; off >>= 1) t += __shfl_xor_sync(0xffffffffu, t, off);
+                if (lane == 0) s_db[(size_t)warp * C + c] += t;        // one writer per (warp, class)
+            }
+        }
+        if (ok) {
+            acc[0] += wr * (lrow * invC);
+            acc[1] += hrow;
+            acc[2] += wr * (hrow * invC);
+            acc[3] += wr;
+        }
+    }
+#pragma unroll
+    for (int off = 16; off > 0; off >>= 1) {
+#pragma unroll
+        for (int k = 0; k < 4; ++k) acc[k] += __shfl_xor_sync(0xffffffffu, acc[k], off);
+    }
+    if (lane == 0) {
+#pragma unroll
+        for (int k = 0; k < 4; ++k) s_red[warp * 4 + k] = acc[k];
+    }
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        float t[4] = {0.f, 0.f, 0.f, 0.f};
+        for (int w = 0; w < warps; ++w)
+            for (int k = 0; k < 4; ++k) t[k] += s_red[w * 4 + k];
+        *loss = t[0] * invB;
+        if (stats) {
+            stats[0] += t[1];
+            stats[1] += (float)B * (float)C;
+            if (n_stats > 2) { stats[2] += t[2]; stats[3] += t[3]; }
+        }
+    }
+    if (dbias)
+        for (int c = threadIdx.x; c < C; c += blockDim.x) {
+            float a = 0.f;
+            for (int w = 0; w < warps; ++w) a += s_db[(size_t)w * C + c];
+            dbias[c] = __float2bfloat16(a);
+        }
+}
+
 
 // ---------------------------------------------------------------------------------------------
 // Classifier head, forward AND backward, in one launch (the whole problem is ~0.5 MFLOP):
@@ -643,6 +748,7 @@ tfy_dense_head_fused_kernel(const __nv_bfloat16* __restrict__ h, const __nv_bflo
     constexpr int TARGET = TFY_HEAD_SPARSE;
     [[maybe_unused]] const float* const targets = nullptr;
     [[maybe_unused]] const float ls = 0.f;
+    [[maybe_unused]] const int sigmoid_out = 0;
 #include "tfy_dense_head_body.cuh"
 }
 
@@ -660,6 +766,25 @@ tfy_dense_head_fused_soft_kernel(const __nv_bfloat16* __restrict__ h, const __nv
                                  const float* __restrict__ sample_w, const float* __restrict__ class_w) {
     tfy_pdl_sync();
     constexpr int TARGET = TFY_HEAD_DENSE;
+    [[maybe_unused]] const long long* const labels = nullptr;
+    [[maybe_unused]] const int sigmoid_out = 0;
+#include "tfy_dense_head_body.cuh"
+}
+
+// BINARY target mode: targets [B, C] fp32, label smoothing ls, sigmoid_out: the model's output is sigmoid(z) (else z)
+template <int K, bool WEIGHTED>
+__global__ void __launch_bounds__(HEAD_THREADS)
+tfy_dense_head_fused_binary_kernel(const __nv_bfloat16* __restrict__ h, const __nv_bfloat16* __restrict__ w2,
+                                   const __nv_bfloat16* __restrict__ b2, const float* __restrict__ targets, float ls,
+                                   int sigmoid_out, const uint8_t* __restrict__ mask1, float scale1,
+                                   float* __restrict__ loss, float* __restrict__ loss_host, float* __restrict__ stats,
+                                   __nv_bfloat16* __restrict__ dw2,
+                                   __nv_bfloat16* __restrict__ db2, __nv_bfloat16* __restrict__ dh,
+                                   __nv_bfloat16* __restrict__ db1, float* __restrict__ scratch,
+                                   uint32_t* __restrict__ counter, int B, int C,
+                                   const float* __restrict__ sample_w, const float* __restrict__ class_w) {
+    tfy_pdl_sync();
+    constexpr int TARGET = TFY_HEAD_BINARY;
     [[maybe_unused]] const long long* const labels = nullptr;
 #include "tfy_dense_head_body.cuh"
 }
@@ -774,17 +899,27 @@ int tfy_pool_drop_relu_bwd(const void* dp, const void* code, void* dz, float sca
     return (int)cudaGetLastError();
 }
 
+// Block of the single-CTA cross-entropy kernels (one row per thread, at most 32 warps) and its shared memory: the
+// bias, one partial row of dbias per warp and 4 sums per warp.  False when C is too wide for that (C > 9000 or so).
+static bool tfy_xent_block(int B, int C, int* warps, size_t* smem) {
+    if (B < 1 || C < 1) return false;
+    const int max_warps = (int)((48 * 1024 / sizeof(float) - (size_t)C) / ((size_t)C + 4));
+    if ((size_t)C >= 48 * 1024 / sizeof(float) || max_warps < 1) return false;
+    int w = (B + 31) / 32;
+    if (w > 32) w = 32;
+    if (w > max_warps) w = max_warps;
+    *warps = w;
+    *smem = ((size_t)C + (size_t)w * (C + 4)) * sizeof(float);
+    return true;
+}
+
 // labels (int64, SPARSE mode) or targets (fp32 [B, C], DENSE mode with label smoothing ls): exactly one is non-null
 static int tfy_softmax_xent_launch(const void* logits, const void* bias, const void* labels, const float* targets,
                                    float ls, const float* sample_w, const float* class_w, float* loss, void* dlogits,
                                    void* dbias, float* stats, int n_stats, int B, int C, cudaStream_t s) {
-    if (B < 1 || C < 1) return -2;
-    const int max_warps = (int)((48 * 1024 / sizeof(float) - (size_t)C) / ((size_t)C + 4));
-    if ((size_t)C >= 48 * 1024 / sizeof(float) || max_warps < 1) return -2;
-    int warps = (B + 31) / 32;
-    if (warps > 32) warps = 32;
-    if (warps > max_warps) warps = max_warps;
-    const size_t smem = ((size_t)C + (size_t)warps * (C + 4)) * sizeof(float);
+    int warps;
+    size_t smem;
+    if (!tfy_xent_block(B, C, &warps, &smem)) return -2;
     if (targets)
         tfy_launch_pdl((tfy_softmax_xent_soft_kernel), dim3(1), dim3(warps * 32), smem, s,
                        (const __nv_bfloat16*)logits, (const __nv_bfloat16*)bias, targets, ls, sample_w, class_w, loss,
@@ -828,6 +963,25 @@ int tfy_softmax_xent_soft(const void* logits, const void* bias, const float* tar
                                    (sample_w || class_w) ? 4 : 2, B, C, s);
 }
 
+// sigmoid twin of tfy_softmax_xent_soft (Keras BinaryCrossentropy, binary C = 1 or multi-label C > 1): targets [B, C]
+// fp32, label smoothing ls in [0, 1], sigmoid_out non-zero when the model's output is sigmoid(z) (a sigmoid layer)
+// rather than z (hit test only); sample_w [B] and class_w [max(C, 2)] fp32, either may be null (the class of a row is
+// round(y) for C = 1, argmax_c y_c otherwise).  loss = sum_r w_r (1/C) sum_c l_rc / B, dlogits [B, C] and dbias [C]
+// bf16, stats null or [hits, B C] (+ [sum w hits / C, sum w] when a weight pointer is non-null).  Same return codes
+// as tfy_softmax_xent_soft.
+int tfy_sigmoid_xent(const void* logits, const void* bias, const float* targets, float ls, int sigmoid_out,
+                     const float* sample_w, const float* class_w, float* loss, void* dlogits, void* dbias,
+                     float* stats, int B, int C, cudaStream_t s) {
+    int warps;
+    size_t smem;
+    if (!targets || !tfy_valid_smoothing(ls) || (long long)B * C > INT_MAX) return -2;
+    if (!tfy_xent_block(B, C, &warps, &smem)) return -2;
+    tfy_launch_pdl((tfy_sigmoid_xent_kernel), dim3(1), dim3(warps * 32), smem, s, (const __nv_bfloat16*)logits,
+                   (const __nv_bfloat16*)bias, targets, ls, sigmoid_out ? 1 : 0, sample_w, class_w, loss,
+                   (__nv_bfloat16*)dlogits, (__nv_bfloat16*)dbias, stats, (sample_w || class_w) ? 4 : 2, B, C);
+    return (int)cudaGetLastError();
+}
+
 // thin cudaMemcpyAsync wrapper: the input pipeline issues its per-step copies through ctypes (about 1 us per call
 // instead of ~10 us for Tensor.copy_ under a stream context manager)
 int tfy_memcpy_async(void* dst, const void* src, size_t bytes, cudaStream_t s) {
@@ -846,10 +1000,11 @@ size_t tfy_dense_head_scratch_elems(int K, int C, int B) {
 
 }  // extern "C"
 
-// TARGET: TFY_HEAD_SPARSE reads `labels` (int64), TFY_HEAD_DENSE reads `targets` (fp32 [B, C]) and `ls`
+// TARGET: TFY_HEAD_SPARSE reads `labels` (int64), TFY_HEAD_DENSE reads `targets` (fp32 [B, C]) and `ls`,
+// TFY_HEAD_BINARY also `sigmoid_out`
 template <bool WEIGHTED, int TARGET>
 static int tfy_dense_head_launch(const void* h, const void* w2, const void* b2, const void* labels,
-                                 const float* targets, float ls, const void* mask1,
+                                 const float* targets, float ls, int sigmoid_out, const void* mask1,
                                  float scale1, float* loss, float* loss_host, float* stats, void* dw2, void* db2,
                                  void* dh, void* db1, float* scratch, uint32_t* counter, int B, int K, int C,
                                  const float* sample_w, const float* class_w, cudaStream_t s) {
@@ -878,6 +1033,13 @@ static int tfy_dense_head_launch(const void* h, const void* w2, const void* b2, 
                            (const long long*)labels, (const uint8_t*)mask1, scale1, loss, loss_host, stats,            \
                            (__nv_bfloat16*)dw2, (__nv_bfloat16*)db2, (__nv_bfloat16*)dh, (__nv_bfloat16*)db1, scratch, \
                            counter, B, C, sample_w, class_w);                                                          \
+        } else if constexpr (TARGET == TFY_HEAD_BINARY) {                                                              \
+            TFY_HEAD_SMEM((tfy_dense_head_fused_binary_kernel<KK, WEIGHTED>));                                         \
+            tfy_launch_pdl((tfy_dense_head_fused_binary_kernel<KK, WEIGHTED>), dim3(grid), dim3(HEAD_THREADS), smem,   \
+                           s, (const __nv_bfloat16*)h, (const __nv_bfloat16*)w2, (const __nv_bfloat16*)b2, targets,    \
+                           ls, sigmoid_out, (const uint8_t*)mask1, scale1, loss, loss_host, stats,                     \
+                           (__nv_bfloat16*)dw2, (__nv_bfloat16*)db2, (__nv_bfloat16*)dh, (__nv_bfloat16*)db1, scratch, \
+                           counter, B, C, sample_w, class_w);                                                          \
         } else {                                                                                                       \
             TFY_HEAD_SMEM((tfy_dense_head_fused_soft_kernel<KK, WEIGHTED>));                                           \
             tfy_launch_pdl((tfy_dense_head_fused_soft_kernel<KK, WEIGHTED>), dim3(grid), dim3(HEAD_THREADS), smem, s,  \
@@ -901,7 +1063,7 @@ int tfy_dense_head_fused(const void* h, const void* w2, const void* b2, const vo
                          float scale1, float* loss, float* loss_host, float* stats, void* dw2, void* db2, void* dh,
                          void* db1,
                          float* scratch, uint32_t* counter, int B, int K, int C, cudaStream_t s) {
-    return tfy_dense_head_launch<false, TFY_HEAD_SPARSE>(h, w2, b2, labels, nullptr, 0.f, mask1, scale1, loss,
+    return tfy_dense_head_launch<false, TFY_HEAD_SPARSE>(h, w2, b2, labels, nullptr, 0.f, 0, mask1, scale1, loss,
                                                          loss_host, stats, dw2, db2, dh, db1, scratch, counter, B, K,
                                                          C, nullptr, nullptr, s);
 }
@@ -912,9 +1074,9 @@ int tfy_dense_head_fused_weighted(const void* h, const void* w2, const void* b2,
                                   float scale1, float* loss, float* loss_host, float* stats, void* dw2, void* db2,
                                   void* dh, void* db1, float* scratch, uint32_t* counter, int B, int K, int C,
                                   const float* sample_w, const float* class_w, cudaStream_t s) {
-    return tfy_dense_head_launch<true, TFY_HEAD_SPARSE>(h, w2, b2, labels, nullptr, 0.f, mask1, scale1, loss, loss_host,
-                                                        stats, dw2, db2, dh, db1, scratch, counter, B, K, C, sample_w,
-                                                        class_w, s);
+    return tfy_dense_head_launch<true, TFY_HEAD_SPARSE>(h, w2, b2, labels, nullptr, 0.f, 0, mask1, scale1, loss,
+                                                        loss_host, stats, dw2, db2, dh, db1, scratch, counter, B, K, C,
+                                                        sample_w, class_w, s);
 }
 
 // dense-target variant (Keras CategoricalCrossentropy): targets [B, C] fp32, one-hot or soft, label smoothing ls in
@@ -928,12 +1090,34 @@ int tfy_dense_head_fused_soft(const void* h, const void* w2, const void* b2, con
                               const float* sample_w, const float* class_w, cudaStream_t s) {
     if (!targets || !tfy_valid_smoothing(ls) || (long long)B * C > INT_MAX) return -2;
     if (sample_w || class_w)
-        return tfy_dense_head_launch<true, TFY_HEAD_DENSE>(h, w2, b2, nullptr, targets, ls, mask1, scale1, loss,
+        return tfy_dense_head_launch<true, TFY_HEAD_DENSE>(h, w2, b2, nullptr, targets, ls, 0, mask1, scale1, loss,
                                                            loss_host, stats, dw2, db2, dh, db1, scratch, counter, B, K,
                                                            C, sample_w, class_w, s);
-    return tfy_dense_head_launch<false, TFY_HEAD_DENSE>(h, w2, b2, nullptr, targets, ls, mask1, scale1, loss,
+    return tfy_dense_head_launch<false, TFY_HEAD_DENSE>(h, w2, b2, nullptr, targets, ls, 0, mask1, scale1, loss,
                                                         loss_host, stats, dw2, db2, dh, db1, scratch, counter, B, K, C,
                                                         nullptr, nullptr, s);
+}
+
+// sigmoid variant (Keras BinaryCrossentropy, binary C = 1 or multi-label C > 1): targets [B, C] fp32, label smoothing
+// ls in [0, 1], sigmoid_out non-zero when the model's output is sigmoid(z) (a sigmoid layer) rather than z (hit test
+// only: the loss is computed from z either way); sample_w [B] and class_w [max(C, 2)] fp32, either may be null (the
+// class of a row is round(y) for C = 1, argmax_c y_c otherwise).  stats null or [hits, B C] (+ [sum w hits / C,
+// sum w] when a weight pointer is non-null).  Same envelope, scratch size and return codes as
+// tfy_dense_head_fused_soft.
+int tfy_dense_head_fused_binary(const void* h, const void* w2, const void* b2, const float* targets, float ls,
+                                int sigmoid_out, const void* mask1, float scale1, float* loss, float* loss_host,
+                                float* stats, void* dw2, void* db2, void* dh, void* db1, float* scratch,
+                                uint32_t* counter, int B, int K, int C, const float* sample_w, const float* class_w,
+                                cudaStream_t s) {
+    if (!targets || !tfy_valid_smoothing(ls) || (long long)B * C > INT_MAX) return -2;
+    sigmoid_out = sigmoid_out ? 1 : 0;
+    if (sample_w || class_w)
+        return tfy_dense_head_launch<true, TFY_HEAD_BINARY>(h, w2, b2, nullptr, targets, ls, sigmoid_out, mask1,
+                                                            scale1, loss, loss_host, stats, dw2, db2, dh, db1, scratch,
+                                                            counter, B, K, C, sample_w, class_w, s);
+    return tfy_dense_head_launch<false, TFY_HEAD_BINARY>(h, w2, b2, nullptr, targets, ls, sigmoid_out, mask1, scale1,
+                                                         loss, loss_host, stats, dw2, db2, dh, db1, scratch, counter, B,
+                                                         K, C, nullptr, nullptr, s);
 }
 
 }  // extern "C"
